@@ -484,6 +484,23 @@ LWSE_API int lwse_resident_tick_wait(lwse_engine* e, lwse_tick* t);
 LWSE_API int lwse_resident_place_outputs(lwse_engine* e, lwse_place_out* out);
 LWSE_API int lwse_resident_occupancy(lwse_engine* e, uint32_t* occupancy_out);
 
+/* How the most recently submitted tick ran (read-only; nothing waits).  A request table grouped by
+ * namespace runs the namespace-parallel form; one that is not (a patch moved a request to another
+ * namespace) runs the same form through a namespace index the device builds, rebuilt by the ticks
+ * whose patches change a request's namespace.  The general form only runs where the namespace form
+ * cannot: too many domains for one CTA's shared memory, or LWSE_PLACE_FORM=general. */
+typedef struct lwse_tick_info {
+  uint32_t place_form;  /* LWSE_TICK_FORM_*                                                   */
+  uint32_t indexed;     /* 1: the namespace form read the requests through the namespace index */
+  uint32_t index_built; /* 1: this tick (re)built that index                                  */
+  uint32_t graph;       /* 1: the tick was replayed as a CUDA graph                           */
+} lwse_tick_info;
+#define LWSE_TICK_FORM_NONE 0u      /* no placement round (no LWSE_TICK_PLACE)               */
+#define LWSE_TICK_FORM_GENERAL 1u   /* the general form (+ a diff kernel)                    */
+#define LWSE_TICK_FORM_NAMESPACE 2u /* namespace-parallel, two-level                         */
+#define LWSE_TICK_FORM_SCAN 3u      /* namespace-parallel, scan (LWSE_SWEEP_PLACE_SCAN)       */
+LWSE_API int lwse_resident_tick_info(lwse_engine* e, lwse_tick_info* info);
+
 /* ------------------------------------------------------------------------- */
 /* Placement (build-defined spec — the reference has no node scoring)        */
 /* ------------------------------------------------------------------------- */

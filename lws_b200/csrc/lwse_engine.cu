@@ -87,13 +87,14 @@ struct PlaceNsExchange {
   uint64_t half_bytes;
   bool lagged;
 };
+enum PlaceNsIndex : uint32_t { kNsIndexNone = 0, kNsIndexReuse = 1, kNsIndexBuild = 2 };
 bool place_ns_supported(uint32_t n_nodes, uint32_t n_domains);
 int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, const uint32_t* d_node_order, uint32_t n_nodes,
                     uint32_t n_usable, uint32_t n_domains, const lwse_place_req* d_reqs, uint32_t n_reqs,
                     const uint32_t* d_occupancy, uint32_t n_parts, uint64_t part_stride_bytes, uint32_t n_namespaces,
                     lwse_place_out* d_out, void* d_scratch, size_t scratch_bytes, bool fresh, uint32_t call_index, bool scan,
                     int sm_count, cudaStream_t s, int* cuda_err, const uint32_t** d_counters_out, bool first_pdl,
-                    const PlaceNsChanges* changes, const PlaceNsExchange* xch);
+                    const PlaceNsChanges* changes, const PlaceNsExchange* xch, PlaceNsIndex index);
 int launch_place_diff(const lwse_place_out* d_cur, lwse_place_out* d_prev, uint32_t n, uint32_t* d_rows,
                       lwse_place_out* d_outs, uint32_t capacity, uint32_t* d_count, cudaStream_t s, int* cuda_err);
 // lwse_ds_kernels.cu
@@ -258,6 +259,9 @@ struct lwse_engine {
   const uint32_t* place_scans_ptr = nullptr;   // device: its (request, round) search counter (grouped form), or null
   bool r_place_grouped = false;      // the resident request table is grouped by namespace
   std::vector<uint32_t> r_req_ns;    // its namespace column (host copy: patches must not regroup it)
+  bool r_ns_index_ok = false;        // the namespace index in place_ns_scratch matches that column
+                                     // (ungrouped tables; any other namespace-form call overwrites ns_first)
+  lwse_tick_info last_tick_info{};   // what the last submitted tick ran (lwse_resident_tick_info)
   const uint32_t* place_counters = nullptr;  // device: counters / phase stamps of the last placement call
   const uint32_t* place_unpinned = nullptr;  // device: its unpinned-request count
   DevBuf ds, ds_roles, ds_revroles, ds_out, ds_role_out, ds_revrole_out;
@@ -880,21 +884,17 @@ static int apply_patches_locked(lwse_engine* e, const lwse_patch_seg* segs, uint
     uint32_t rb;
     resident_table(e, g.table, &base, &rows, &rb);
     *wrote = true;
-    if (g.table == LWSE_TABLE_PLACE_REQS && e->r_place_grouped) {
-      // a request that moves to another namespace breaks the grouping the fast placement kernels rely on
+    if (g.table == LWSE_TABLE_PLACE_REQS) {
+      // a request that moves to another namespace breaks the grouping the fast placement kernels rely on,
+      // and the namespace index of an ungrouped table
       const lwse_place_req* v = static_cast<const lwse_place_req*>(g.values);
       for (uint32_t k = 0; k < g.n; k++) {
         const uint32_t row = (g.flags & LWSE_PATCH_RANGE) ? g.first_row + k : g.rows[k];
         if (row < e->rn_reqs && v[k].ns != e->r_req_ns[row]) {
           e->r_req_ns[row] = v[k].ns;
           e->r_place_grouped = false;
+          e->r_ns_index_ok = false;
         }
-      }
-    } else if (g.table == LWSE_TABLE_PLACE_REQS) {
-      const lwse_place_req* v = static_cast<const lwse_place_req*>(g.values);
-      for (uint32_t k = 0; k < g.n; k++) {
-        const uint32_t row = (g.flags & LWSE_PATCH_RANGE) ? g.first_row + k : g.rows[k];
-        if (row < e->rn_reqs) e->r_req_ns[row] = v[k].ns;
       }
     }
     if (g.flags & LWSE_PATCH_RANGE) {  // one DMA copy straight into the table
@@ -1054,11 +1054,13 @@ static const int g_place_form_env = [] {  // LWSE_PLACE_FORM=general|grouped|sca
 }();
 
 // The namespace-parallel form (request table grouped by namespace): condense kernel + one CTA per
-// namespace.  `first_pdl`: nothing on the stream right before writes the request table.
+// namespace.  `first_pdl`: nothing on the stream right before writes the request table.  `index` other
+// than kNsIndexNone: the resident request table, not grouped — the indexed form.
 static int place_grouped_locked(lwse_engine* e, const lwse_place_req* d_reqs, uint32_t n_reqs, const uint32_t* d_occupancy,
                                 uint32_t n_parts, uint64_t part_stride_bytes, uint32_t n_namespaces, lwse_place_out* d_out,
                                 bool scan, uint32_t* rounds_out, uint32_t* scans_out, cudaStream_t s, bool first_pdl,
-                                const lwse::PlaceNsChanges* changes = nullptr, const lwse::PlaceNsExchange* xch = nullptr) {
+                                const lwse::PlaceNsChanges* changes = nullptr, const lwse::PlaceNsExchange* xch = nullptr,
+                                lwse::PlaceNsIndex index = lwse::kNsIndexNone) {
   const size_t scratch = lwse::place_ns_scratch_bytes(e->n_nodes, e->n_domains, n_reqs, n_namespaces);
   const void* before = e->place_ns_scratch.p;
   LWSE_CUDA(e, e->place_ns_scratch.reserve(scratch));
@@ -1075,8 +1077,9 @@ static int place_grouped_locked(lwse_engine* e, const lwse_place_req* d_reqs, ui
                                        (const uint32_t*)e->node_order.p, e->n_nodes, e->n_usable, e->n_domains, d_reqs, n_reqs,
                                        d_occupancy, n_parts, part_stride_bytes, n_namespaces, d_out, e->place_ns_scratch.p,
                                        scratch, fresh, e->place_ns_calls++, scan, e->sm_count, s, &cuda_err, &counters,
-                                       first_pdl && !fresh, changes, xch);
+                                       first_pdl && !fresh, changes, xch, index);
   if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+  e->r_ns_index_ok = index != lwse::kNsIndexNone;  // (a grouped call writes its own ns_first over the index's)
   e->launches += (uint64_t)launched;
   e->place_rounds_ptr = counters;
   e->place_scans_ptr = counters + 3;
@@ -1097,7 +1100,8 @@ static int place_locked(lwse_engine* e, const lwse_place_req* d_reqs, uint32_t n
                         const uint32_t* d_occupancy, uint32_t n_namespaces, lwse_place_out* d_out,
                         uint32_t* rounds_out, cudaStream_t s, uint32_t n_parts, uint32_t reqs_per_part,
                         uint64_t part_stride_bytes, bool after_push = false, uint32_t form = kFormGeneral,
-                        bool first_pdl = false, const lwse::PlaceNsChanges* changes = nullptr, bool* diffed = nullptr) {
+                        bool first_pdl = false, const lwse::PlaceNsChanges* changes = nullptr, bool* diffed = nullptr,
+                        lwse::PlaceNsIndex index = lwse::kNsIndexNone) {
   if ((n_reqs && (!d_reqs || !d_out)) || n_namespaces == 0) return LWSE_ERR_INVALID_ARG;
   if (e->n_nodes == 0 || e->n_domains == 0) return LWSE_ERR_NOT_READY;
   if (g_place_form_env == 0) form = kFormGeneral;
@@ -1106,7 +1110,7 @@ static int place_locked(lwse_engine* e, const lwse_place_req* d_reqs, uint32_t n
   if (form != kFormGeneral && n_parts <= 1 && lwse::place_ns_supported(e->n_nodes, e->n_domains)) {
     if (diffed) *diffed = changes != nullptr;
     return place_grouped_locked(e, d_reqs, n_reqs, d_occupancy, 1, 0, n_namespaces, d_out, form == kFormScan, rounds_out, nullptr,
-                                s, first_pdl, changes);
+                                s, first_pdl, changes, nullptr, index);
   }
   const size_t scratch = lwse::place_scratch_bytes(e->n_nodes, e->n_domains, n_reqs, n_namespaces);
   const void* before = e->place_scratch.p;
@@ -1326,7 +1330,8 @@ LWSE_API int lwse_reconcile_exchanged_device(lwse_engine* e, const lwse_lws_tabl
 static int shared_occupancy_place_locked(lwse_engine* e, const lwse_place_req* d_reqs, uint32_t n_reqs,
                                          const uint32_t* d_local_occ, uint32_t n_namespaces, lwse_place_out* d_out,
                                          uint32_t form, bool lagged, cudaStream_t ps,
-                                         const lwse::PlaceNsChanges* changes = nullptr) {
+                                         const lwse::PlaceNsChanges* changes = nullptr,
+                                         lwse::PlaceNsIndex index = lwse::kNsIndexNone) {
   // While a tick graph is being captured the step is not a parameter: the push kernel takes it from
   // the device counter every push advances (and the condense kernel the blocks to sum from the same
   // counter), so that the replayed nodes follow the step; the replay itself advances e->xch_step.
@@ -1347,7 +1352,8 @@ static int shared_occupancy_place_locked(lwse_engine* e, const lwse_place_req* d
                                   e->xch_half, lagged};
   if (form != kFormGeneral && lwse::place_ns_supported(e->n_nodes, e->n_domains))
     return place_grouped_locked(e, d_reqs, n_reqs, static_cast<const uint32_t*>(e->xch.p), e->xch_world, e->xch_stride, n_namespaces,
-                                d_out, form == kFormScan, nullptr, nullptr, ps, /*first_pdl=*/true, changes, &xch);  // behind the push kernel
+                                d_out, form == kFormScan, nullptr, nullptr, ps, /*first_pdl=*/true, changes, &xch,
+                                index);  // behind the push kernel
   return LWSE_ERR_UNSUPPORTED;  // the shared-occupancy form needs a request table grouped by namespace
 }
 
@@ -1508,6 +1514,7 @@ LWSE_API int lwse_resident_place_load(lwse_engine* e, const lwse_place_req* reqs
   e->rn_namespaces = n_namespaces;
   e->r_place_loaded = true;
   e->r_place_grouped = grouped_by_namespace(reqs, n_reqs);
+  e->r_ns_index_ok = false;  // an ungrouped table: the first tick builds the namespace index
   e->r_req_ns.resize(n_reqs);
   for (uint32_t i = 0; i < n_reqs; i++) e->r_req_ns[i] = reqs[i].ns;
   return reserve_change_lists(e);
@@ -1562,6 +1569,37 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
   const bool do_place = (flags & LWSE_TICK_PLACE) && e->r_place_loaded && e->rn_reqs > 0;
   const bool do_sweep = !(flags & LWSE_TICK_NO_SWEEP) && (e->rn_lws || e->rn_groups);
   if (n_segs && !segs) return LWSE_ERR_INVALID_ARG;
+  // The round's form, decided before any patch is applied (it is part of a tick graph's key).  A request
+  // table grouped by namespace — and not ungrouped by this tick's patches — runs the namespace kernels as
+  // they are; any other table runs them through the namespace index, rebuilt when the namespace column
+  // changed since the last build.  The general form only where the namespace form cannot run.
+  bool ns_moves = false;
+  for (uint32_t i = 0; do_place && i < n_segs && !ns_moves; i++) {
+    const lwse_patch_seg& g = segs[i];
+    if (g.table != LWSE_TABLE_PLACE_REQS || g.n == 0 || !g.values || (!(g.flags & LWSE_PATCH_RANGE) && !g.rows)) continue;
+    const lwse_place_req* v = static_cast<const lwse_place_req*>(g.values);
+    for (uint32_t k = 0; k < g.n && !ns_moves; k++) {
+      const uint32_t row = (g.flags & LWSE_PATCH_RANGE) ? g.first_row + k : g.rows[k];
+      ns_moves = row < e->rn_reqs && v[k].ns != e->r_req_ns[row];
+    }
+  }
+  const bool ns_form = do_place && g_place_form_env != 0 && lwse::place_ns_supported(e->n_nodes, e->n_domains);
+  const bool indexed = ns_form && !(e->r_place_grouped && !ns_moves);
+  const lwse::PlaceNsIndex ns_index = !indexed                              ? lwse::kNsIndexNone
+                                      : (ns_moves || !e->r_ns_index_ok) ? lwse::kNsIndexBuild
+                                                                          : lwse::kNsIndexReuse;
+  const bool scan_form = (flags & LWSE_SWEEP_PLACE_SCAN) || g_place_form_env == 2;
+  auto record_info = [&](bool graph) {
+    lwse_tick_info& ti = e->last_tick_info;
+    ti.place_form = !do_place ? LWSE_TICK_FORM_NONE
+                    : !ns_form ? LWSE_TICK_FORM_GENERAL
+                    : scan_form ? LWSE_TICK_FORM_SCAN
+                                : LWSE_TICK_FORM_NAMESPACE;
+    ti.indexed = indexed ? 1u : 0u;
+    ti.index_built = ns_index == lwse::kNsIndexBuild ? 1u : 0u;
+    ti.graph = graph ? 1u : 0u;
+    if (indexed) e->r_ns_index_ok = true;  // (also after a replay, which enqueues no call that would say so)
+  };
   // sequence numbers count the ticks that end in a publish kernel (the device counts the same ones)
   uint32_t seq = 0;
   if (do_sweep || do_place) {
@@ -1629,8 +1667,7 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
     // the general placement kernel keeps its counters in two alternating scratch halves (a call resets
     // the half the next one uses): its round may not start before the previous tick's publish kernel
     // has read them.  (The namespace kernels count in the tick slot's own block.)
-    if (do_place && !(e->r_place_grouped && g_place_form_env != 0 && lwse::place_ns_supported(e->n_nodes, e->n_domains)))
-      LWSE_CUDA(e, cudaStreamWaitEvent(ps, e->ev_pub, 0));
+    if (do_place && !ns_form) LWSE_CUDA(e, cudaStreamWaitEvent(ps, e->ev_pub, 0));
   }
   ScatterPlan main_plan;
   auto apply_main = [&](bool defer) -> int {
@@ -1679,7 +1716,7 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
     return LWSE_OK;
   };
   auto enqueue_place = [&]() -> int {
-    const uint32_t form = !e->r_place_grouped ? kFormGeneral : (flags & LWSE_SWEEP_PLACE_SCAN) ? kFormScan : kFormGrouped;
+    const uint32_t form = !ns_form ? kFormGeneral : (flags & LWSE_SWEEP_PLACE_SCAN) ? kFormScan : kFormGrouped;
     // the namespace kernels append the changed rows themselves; the general form gets a diff kernel
     const lwse::PlaceNsChanges changes{(lwse_place_out*)e->r_pout_prev.p, reinterpret_cast<uint32_t*>(chg_v + e->chg_off[4]),
                                        reinterpret_cast<lwse_place_out*>(chg_v + e->chg_off[5]), cnt + 4, e->rn_reqs, (int)slot,
@@ -1689,12 +1726,12 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
       if (!e->xch_connected) return LWSE_ERR_NOT_READY;
       rc = shared_occupancy_place_locked(e, (const lwse_place_req*)e->r_preq.p, e->rn_reqs, (const uint32_t*)e->r_occ.p,
                                          e->rn_namespaces, (lwse_place_out*)e->r_pout.p, form,
-                                         (flags & LWSE_EXCHANGE_LAGGED) != 0, ps, &changes);
+                                         (flags & LWSE_EXCHANGE_LAGGED) != 0, ps, &changes, ns_index);
       diffed = rc == LWSE_OK;
     } else {
       rc = place_locked(e, (const lwse_place_req*)e->r_preq.p, e->rn_reqs, (const uint32_t*)e->r_occ.p, e->rn_namespaces,
                         (lwse_place_out*)e->r_pout.p, nullptr, ps, 1, e->rn_reqs, 0, false, form, place_first_pdl, &changes,
-                        &diffed);
+                        &diffed, ns_index);
     }
     if (rc != LWSE_OK) return rc;
     if (!diffed) {
@@ -1742,14 +1779,15 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
   const bool graph_ok = (e->use_graph >= 2 || (e->use_graph == 1 && in_flight)) && all_in_place && !any_range &&
                         (!shared_occ || (do_place && e->xch_connected)) &&
                         (do_sweep || do_place) && !(has_side && !do_place) &&
-                        (!do_place || (e->r_place_grouped && g_place_form_env != 0 && lwse::place_ns_supported(e->n_nodes, e->n_domains)));
+                        (!do_place || ns_form);
   if (graph_ok) {
     bool has_patches = false;
     for (uint32_t i = 0; i < n_segs; i++)
       if (segs[i].n) has_patches = true;
     const uint32_t key = (has_patches ? 1u : 0u) | (do_sweep ? 8u : 0u) | (do_place ? 16u : 0u) |
                          ((flags & LWSE_SWEEP_GANG) ? 32u : 0u) | ((flags & LWSE_SWEEP_PLACE_SCAN) ? 64u : 0u) | (slot << 8) |
-                         (shared_occ ? 512u : 0u) | ((shared_occ && (flags & LWSE_EXCHANGE_LAGGED)) ? 1024u : 0u);
+                         (shared_occ ? 512u : 0u) | ((shared_occ && (flags & LWSE_EXCHANGE_LAGGED)) ? 1024u : 0u) |
+                         (indexed ? 2048u : 0u) | (ns_index == lwse::kNsIndexBuild ? 4096u : 0u);
     lwse_engine::TickGraph& tg = e->tick_graphs[key];
     bool replay = !tg.failed && tg.seen >= 1;  // the first tick of a shape runs eagerly: every buffer settles
     tg.seen++;
@@ -1759,7 +1797,6 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
       rc = apply_patches_locked(e, segs, n_segs, &w, 0xFFFFFFFFu, s, 0, nullptr, 0, &gp, /*plan_only=*/true);
       if (rc != LWSE_OK) return rc;
       if (gp.eager_only || gp.recount) replay = false;
-      if (do_place && !e->r_place_grouped) replay = false;  // (a patch moved a request to another namespace)
     }
     const size_t desc_bytes = 512;
     if (replay && (lwse::scatter_desc_bytes() > desc_bytes || e->tdesc.reserve(2 * desc_bytes) != cudaSuccess ||
@@ -1867,6 +1904,7 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
       gts.published = true;
       gts.wrote = has_patches;
       e->t_submitted++;
+      record_info(true);
       return LWSE_OK;
     }
   }
@@ -1906,6 +1944,7 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
   ts.published = published;
   ts.wrote = wrote || wrote_side;
   e->t_submitted++;
+  record_info(false);
   return LWSE_OK;
 }
 
@@ -2051,6 +2090,13 @@ LWSE_API int lwse_resident_occupancy(lwse_engine* e, uint32_t* occupancy_out) {
   DeviceGuard guard(e->device);
   LWSE_CUDA(e, cudaStreamSynchronize(e->stream));
   LWSE_CUDA(e, cudaMemcpy(occupancy_out, e->r_occ.p, (size_t)e->n_nodes * 4, cudaMemcpyDeviceToHost));
+  return LWSE_OK;
+}
+
+LWSE_API int lwse_resident_tick_info(lwse_engine* e, lwse_tick_info* info) {
+  if (!e || !info) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  *info = e->last_tick_info;
   return LWSE_OK;
 }
 

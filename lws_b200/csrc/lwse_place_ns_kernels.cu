@@ -33,6 +33,16 @@
 //                           (domain score, lower domain, node score, lower node) — identical rows.
 //   Inside a tick both forms also append the result rows that differ from the previous tick's to
 //   the device change list (PlaceNsArgs::prev …) — no separate diff kernel.
+//
+// Indexed form — a request table NOT grouped by namespace (a patch moved a request to another
+// namespace): the namespace kernel reaches its requests through a namespace index,
+// ns_rows[ns_first[v] .. ns_first[v+1]) = the request rows of namespace v, built on the device by
+//   place_index_count_kernel   requests per namespace
+//   place_index_scan_kernel    exclusive scan -> ns_first, per-namespace cursors
+//   place_index_fill_kernel    ns_rows, by cursor
+// The order inside a namespace is arbitrary and the result does not depend on it: keys carry the
+// request ROW, pinned claims are atomicMin on those keys and the unpinned list is built with atomics
+// anyway.  The index is rebuilt only when the namespace column changed; other calls reuse it.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -43,7 +53,7 @@ namespace lwse {
 
 struct PlaceNsArgs {
   const lwse_node_rec* nodes;
-  const lwse_place_req* reqs;  // grouped by namespace (ns non-decreasing)
+  const lwse_place_req* reqs;  // grouped by namespace (ns non-decreasing), unless ns_rows is set
   const uint32_t* occupancy;   // nullable; n_parts blocks of n_nodes counters, part_stride_bytes apart
   lwse_place_out* out;
   const uint32_t* dom_first;   // static index (lwse_upload_nodes)
@@ -53,6 +63,10 @@ struct PlaceNsArgs {
   uint32_t* g_dom_free;  // n_domains (+ padding)
   uint32_t* ns_first;    // n_namespaces + 1
   uint32_t* unpinned;    // n_reqs: namespace v's live unpinned requests at [ns_first[v], …)
+  // indexed form (null: the table is grouped and a position is a row)
+  uint32_t* ns_rows;     // n_reqs: position -> request row
+  uint32_t* ns_count;    // n_namespaces: requests per namespace (all zero between index builds)
+  uint32_t* ns_cursor;   // n_namespaces: fill cursors
   uint32_t* counters;    // this call's block: [0] max rounds [1] live unpinned [2] order violations [3] (request, round) scans
   uint32_t* next_counters;  // the other block, cleared for the next call
   uint32_t n_nodes, n_usable, n_domains, n_reqs, n_namespaces;
@@ -133,24 +147,27 @@ __global__ void __launch_bounds__(256) place_condense_kernel(const PlaceNsArgs a
     sum = __reduce_add_sync(0xFFFFFFFFu, sum);
     if (lane == 0) a.g_dom_free[d] = sum;
   }
-  // B. the namespace index of the (promised) grouped request table
-  if (a.n_reqs == 0u) {
+  // B. the namespace index of the (promised) grouped request table; the indexed form has its own
+  const bool grouped = a.ns_rows == nullptr;
+  if (grouped && a.n_reqs == 0u) {
     for (uint32_t v = gtid; v <= a.n_namespaces; v += gsize) a.ns_first[v] = 0u;
   }
   for (uint32_t i = gtid; i < a.n_reqs; i += gsize) {
     const uint4 hi = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + i) + 1);
     const uint32_t b = hi.y;
-    uint32_t lo_v;  // namespaces (lo_v, b] start at request i; for i == 0 also namespace lo_v itself
-    if (i == 0u) {
-      for (uint32_t v = 0; v <= min(b, a.n_namespaces); v++) a.ns_first[v] = 0u;
-    } else {
-      const uint32_t prev = ldg_keep_u32(reinterpret_cast<const uint32_t*>(a.reqs + i - 1) + 5);  // .ns
-      if (prev > b) atomicAdd(a.counters + 2, 1u);  // not grouped: the caller broke its promise
-      lo_v = min(prev, a.n_namespaces);
-      for (uint32_t v = lo_v + 1u; v <= min(b, a.n_namespaces); v++) a.ns_first[v] = i;
+    if (grouped) {
+      uint32_t lo_v;  // namespaces (lo_v, b] start at request i; for i == 0 also namespace lo_v itself
+      if (i == 0u) {
+        for (uint32_t v = 0; v <= min(b, a.n_namespaces); v++) a.ns_first[v] = 0u;
+      } else {
+        const uint32_t prev = ldg_keep_u32(reinterpret_cast<const uint32_t*>(a.reqs + i - 1) + 5);  // .ns
+        if (prev > b) atomicAdd(a.counters + 2, 1u);  // not grouped: the caller broke its promise
+        lo_v = min(prev, a.n_namespaces);
+        for (uint32_t v = lo_v + 1u; v <= min(b, a.n_namespaces); v++) a.ns_first[v] = i;
+      }
+      if (i == a.n_reqs - 1u)
+        for (uint32_t v = min(b, a.n_namespaces) + 1u; v <= a.n_namespaces; v++) a.ns_first[v] = a.n_reqs;
     }
-    if (i == a.n_reqs - 1u)
-      for (uint32_t v = min(b, a.n_namespaces) + 1u; v <= a.n_namespaces; v++) a.ns_first[v] = a.n_reqs;
     if (b >= a.n_namespaces) {  // no such namespace: never takes part in a round
       const bool pinned = hi.w != LWSE_NONE;
       const uint4 row = make_uint4(LWSE_NONE, pinned ? hi.w : LWSE_NONE, (pinned ? LWSE_PLACE_PINNED : 0u) | LWSE_PLACE_UNSCHEDULABLE, 0u);
@@ -169,6 +186,87 @@ __global__ void __launch_bounds__(256) place_condense_kernel(const PlaceNsArgs a
     }
   }
   if (gtid < 8u && a.next_counters != nullptr) a.next_counters[gtid] = 0u;
+}
+
+// --------------------------------------------------------------------------
+// the namespace index of an ungrouped request table (indexed form)
+// --------------------------------------------------------------------------
+// A warp looks at 32 consecutive rows and takes one atomic per namespace among them
+// (__match_any_sync): an ungrouped table is still mostly runs of one namespace.  Rows whose
+// namespace does not exist are left out (the condense kernel marks them UNSCHEDULABLE).
+__device__ __forceinline__ uint32_t index_ns_of(const PlaceNsArgs& a, uint32_t i) {
+  if (i >= a.n_reqs) return LWSE_NONE;
+  const uint32_t v = ldg_keep_u32(reinterpret_cast<const uint32_t*>(a.reqs + i) + 5);  // .ns
+  return v < a.n_namespaces ? v : LWSE_NONE;
+}
+
+__global__ void __launch_bounds__(256) place_index_count_kernel(const PlaceNsArgs a) {
+  pdl_launch_dependents();
+  pdl_wait_prior();  // the request table a tick's scatter patched; the previous call's readers of the index
+  const uint32_t lane = threadIdx.x & 31u, stride = gridDim.x * blockDim.x;
+  for (uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; base < a.n_reqs; base += stride) {
+    const uint32_t v = index_ns_of(a, base + lane);
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, v);
+    if (v != LWSE_NONE && lane == (uint32_t)__ffs(peers) - 1u) atomicAdd(a.ns_count + v, (uint32_t)__popc(peers));
+  }
+}
+
+// one CTA: ns_first = exclusive scan of the counts, the cursors start there, the counts go back to zero
+constexpr uint32_t kIndexScanThreads = 1024;
+__global__ void __launch_bounds__(kIndexScanThreads) place_index_scan_kernel(const PlaceNsArgs a) {
+  __shared__ uint32_t s_warp[32], s_carry;
+  pdl_launch_dependents();
+  pdl_wait_prior();
+  const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+  if (tid == 0) s_carry = 0u;
+  __syncthreads();
+  for (uint32_t base = 0; base < a.n_namespaces; base += kIndexScanThreads) {
+    const uint32_t v = base + tid;
+    const uint32_t c = v < a.n_namespaces ? __ldcg(a.ns_count + v) : 0u;
+    uint32_t x = c;  // inclusive scan inside the warp
+#pragma unroll
+    for (uint32_t o = 1; o < 32u; o <<= 1) {
+      const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o);
+      if (lane >= o) x += y;
+    }
+    if (lane == 31u) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+      uint32_t w = s_warp[lane];
+#pragma unroll
+      for (uint32_t o = 1; o < 32u; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, w, o);
+        if (lane >= o) w += y;
+      }
+      s_warp[lane] = w;
+    }
+    __syncthreads();
+    const uint32_t first = s_carry + (warp ? s_warp[warp - 1u] : 0u) + x - c;
+    if (v < a.n_namespaces) {
+      a.ns_first[v] = first;
+      a.ns_cursor[v] = first;
+      a.ns_count[v] = 0u;
+    }
+    __syncthreads();  // everybody has read s_carry and s_warp
+    if (tid == kIndexScanThreads - 1u) s_carry = first + c;
+    __syncthreads();
+  }
+  if (tid == 0) a.ns_first[a.n_namespaces] = s_carry;
+}
+
+__global__ void __launch_bounds__(256) place_index_fill_kernel(const PlaceNsArgs a) {
+  pdl_launch_dependents();
+  pdl_wait_prior();
+  const uint32_t lane = threadIdx.x & 31u, stride = gridDim.x * blockDim.x;
+  for (uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; base < a.n_reqs; base += stride) {
+    const uint32_t i = base + lane, v = index_ns_of(a, i);
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, v);
+    const uint32_t leader = (uint32_t)__ffs(peers) - 1u;
+    uint32_t pos = 0;
+    if (v != LWSE_NONE && lane == leader) pos = atomicAdd(a.ns_cursor + v, (uint32_t)__popc(peers));
+    pos = __shfl_sync(0xFFFFFFFFu, pos, (int)leader);
+    if (v != LWSE_NONE) a.ns_rows[pos + (uint32_t)__popc(peers & ((1u << lane) - 1u))] = i;
+  }
 }
 
 // --------------------------------------------------------------------------
@@ -224,7 +322,9 @@ __device__ __forceinline__ void diff_row(const PlaceNsArgs& a, uint32_t r, const
 #else
 #define LWSE_NS_BOUNDS __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
 #endif
-template <bool kScan>
+// kIndexed: the requests of a namespace are reached through the index (ns_rows); results, keys and the
+// unpinned list carry the request ROW either way.
+template <bool kScan, bool kIndexed>
 __global__ void LWSE_NS_BOUNDS
     place_ns_kernel(const PlaceNsArgs a, const __grid_constant__ CUtensorMap words_map) {
   extern __shared__ uint8_t s_dyn[];
@@ -298,11 +398,17 @@ __global__ void LWSE_NS_BOUNDS
     // ---- phase 1: pinned claims, the list of live unpinned requests ----
     // the first kNsKeep requests of a thread stay in registers until their result is written
     uint4 k_lo[kNsKeep], k_hi[kNsKeep];
-    uint32_t k_dom[kNsKeep];
+    uint32_t k_dom[kNsKeep], k_row[kNsKeep];
+    auto row_of = [&](uint32_t p) -> uint32_t {  // position in the namespace's range -> request row
+      if constexpr (kIndexed) return __ldcg(a.ns_rows + p);
+      return p;
+    };
 #pragma unroll
     for (uint32_t j = 0; j < kNsKeep; j++) {  // all request loads of the thread in flight together
-      const uint32_t r = first + tid + j * blockDim.x;
-      if (r < last) {
+      const uint32_t p = first + tid + j * blockDim.x;
+      if (p < last) {
+        const uint32_t r = row_of(p);
+        if constexpr (kIndexed) k_row[j] = r;
         k_lo[j] = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r));
         k_hi[j] = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r) + 1);
       }
@@ -350,19 +456,22 @@ __global__ void LWSE_NS_BOUNDS
     };
 #pragma unroll
     for (uint32_t j = 0; j < kNsKeep; j++) {
-      const uint32_t r = first + tid + j * blockDim.x;
-      if (r < last) k_dom[j] = claim(r, k_lo[j], k_hi[j]);
+      const uint32_t p = first + tid + j * blockDim.x;
+      if (p < last) k_dom[j] = claim(kIndexed ? k_row[j] : p, k_lo[j], k_hi[j]);
     }
-    for (uint32_t r = first + tid + kNsKeep * blockDim.x; r < last; r += blockDim.x)  // big namespaces: the rest, unkept
+    for (uint32_t p = first + tid + kNsKeep * blockDim.x; p < last; p += blockDim.x) {  // big namespaces: the rest, unkept
+      const uint32_t r = row_of(p);
       claim(r, ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r)), ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r) + 1));
+    }
     __syncthreads();
     // results of the pinned requests: final from here on (pinned keys are below every unpinned key)
 #pragma unroll
     for (uint32_t j = 0; j < kNsKeep; j++) {
-      const uint32_t r = first + tid + j * blockDim.x;
-      if (r < last) result(r, k_lo[j], k_hi[j], k_dom[j]);
+      const uint32_t p = first + tid + j * blockDim.x;
+      if (p < last) result(kIndexed ? k_row[j] : p, k_lo[j], k_hi[j], k_dom[j]);
     }
-    for (uint32_t r = first + tid + kNsKeep * blockDim.x; r < last; r += blockDim.x) {
+    for (uint32_t p = first + tid + kNsKeep * blockDim.x; p < last; p += blockDim.x) {
+      const uint32_t r = row_of(p);
       const uint4 lo = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r)), hi = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r) + 1);
       uint32_t d = LWSE_NONE;
       if (hi.w != LWSE_NONE && hi.w < a.n_nodes) {
@@ -553,8 +662,9 @@ struct PlaceNsExchange {  // multi-rank: d_occupancy is the base of the exchange
 static size_t up256(size_t v) { return (v + 255) / 256 * 256; }
 
 // scratch: [words (rows x 1 KB)] [nodes2 (same)] [dom_free] [ns_first] [unpinned] [counters: 2 blocks of 8 words]
+//          [indexed form: ns_rows] [ns_count] [ns_cursor]
 struct NsLayout {
-  size_t words, nodes2, dom_free, ns_first, unpinned, counters, total;
+  size_t words, nodes2, dom_free, ns_first, unpinned, counters, ns_rows, ns_count, ns_cursor, total;
   uint32_t word_rows;
 };
 static NsLayout ns_layout(uint32_t n_nodes, uint32_t n_domains, uint32_t n_reqs, uint32_t n_namespaces) {
@@ -574,6 +684,12 @@ static NsLayout ns_layout(uint32_t n_nodes, uint32_t n_domains, uint32_t n_reqs,
   off += up256((size_t)n_reqs * 4 + 16);
   l.counters = off;
   off += 256;
+  l.ns_rows = off;
+  off += up256((size_t)n_reqs * 4 + 16);
+  l.ns_count = off;
+  off += up256((size_t)n_namespaces * 4 + 16);
+  l.ns_cursor = off;
+  off += up256((size_t)n_namespaces * 4 + 16);
   l.total = off;
   return l;
 }
@@ -616,13 +732,18 @@ static bool encode_words_map(CUtensorMap* map, void* g_words, uint32_t word_rows
             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// index: kNsIndexNone = the request table is grouped by namespace; otherwise the indexed form, with the
+// index kept in the scratch (kNsIndexReuse: as the last build left it — the caller knows the namespace
+// column has not changed since; kNsIndexBuild: built first).
+enum PlaceNsIndex : uint32_t { kNsIndexNone = 0, kNsIndexReuse = 1, kNsIndexBuild = 2 };
+
 // Returns kernels launched or -1.  `fresh`: the scratch was (re)allocated: zero it first.
 int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, const uint32_t* d_node_order, uint32_t n_nodes,
                     uint32_t n_usable, uint32_t n_domains, const lwse_place_req* d_reqs, uint32_t n_reqs,
                     const uint32_t* d_occupancy, uint32_t n_parts, uint64_t part_stride_bytes, uint32_t n_namespaces,
                     lwse_place_out* d_out, void* d_scratch, size_t scratch_bytes, bool fresh, uint32_t call_index, bool scan,
                     int sm_count, cudaStream_t s, int* cuda_err, const uint32_t** d_counters_out, bool first_pdl,
-                    const PlaceNsChanges* changes, const PlaceNsExchange* xch) {
+                    const PlaceNsChanges* changes, const PlaceNsExchange* xch, PlaceNsIndex index) {
   *cuda_err = 0;
   const NsLayout l = ns_layout(n_nodes, n_domains, n_reqs, n_namespaces);
   if (scratch_bytes < l.total || n_reqs > 0xFFFFFFu) {
@@ -647,6 +768,12 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
   a.g_dom_free = reinterpret_cast<uint32_t*>(base + l.dom_free);
   a.ns_first = reinterpret_cast<uint32_t*>(base + l.ns_first);
   a.unpinned = reinterpret_cast<uint32_t*>(base + l.unpinned);
+  if (index != kNsIndexNone) {
+    if (fresh) index = kNsIndexBuild;  // (the zeroed scratch holds no index)
+    a.ns_rows = reinterpret_cast<uint32_t*>(base + l.ns_rows);
+    a.ns_count = reinterpret_cast<uint32_t*>(base + l.ns_count);
+    a.ns_cursor = reinterpret_cast<uint32_t*>(base + l.ns_cursor);
+  }
   // counters: 256 bytes = 8 blocks of 8 words.  Blocks 0 / 1 alternate between calls (a call clears the
   // block the next one uses); blocks 2 / 3 belong to the tick slots.
   const int tick_slot = (changes && changes->prev) ? changes->tick_slot : -1;
@@ -700,16 +827,29 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
   }();
   a.use_tensor_map = (a.stage_words && map_ok && !no_tensor_map) ? 1u : 0u;
 
+  int launched = 2;
+  // first_pdl: the predecessor on the stream is a kernel — programmatically dependent then (every
+  // kernel here waits at its top, before its first read, so this is safe even behind a tick's scatter
+  // kernel, whose tail the launch latency overlaps); behind a copy / memset / event an ordinary launch
+  bool pdl = first_pdl;
+  if (index == kNsIndexBuild) {  // count -> scan -> fill, a thread per request
+    uint64_t grid = ((uint64_t)n_reqs + 255) / 256;
+    if (grid < 1) grid = 1;
+    if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
+    e = launch_pdl(place_index_count_kernel, dim3((unsigned)grid), dim3(256), 0, s, pdl, a);
+    if (e == cudaSuccess) e = launch_pdl(place_index_scan_kernel, dim3(1), dim3(kIndexScanThreads), 0, s, true, a);
+    if (e == cudaSuccess) e = launch_pdl(place_index_fill_kernel, dim3((unsigned)grid), dim3(256), 0, s, true, a);
+    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    pdl = true;
+    launched += 3;
+  }
   {  // condense: a warp per domain, a thread per request
     uint64_t threads = (uint64_t)n_domains * 32u;
     if (threads < n_reqs) threads = n_reqs;
     uint64_t grid = (threads + 255) / 256;
     if (grid < 1) grid = 1;
     if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
-    // first_pdl: the predecessor on the stream is a kernel — programmatically dependent then (the
-    // kernel waits at its top, before its first read, so this is safe even behind a tick's scatter
-    // kernel, whose tail the launch latency overlaps); behind a copy / memset / event an ordinary launch
-    e = launch_pdl(place_condense_kernel, dim3((unsigned)grid), dim3(256), 0, s, first_pdl, a);
+    e = launch_pdl(place_condense_kernel, dim3((unsigned)grid), dim3(256), 0, s, pdl, a);
     if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
     if (changes && changes->mid_event) {
       e = cudaEventRecord(static_cast<cudaEvent_t>(changes->mid_event), s);
@@ -719,17 +859,20 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
   {
     unsigned grid = n_namespaces < (unsigned)sm_count * 2u ? n_namespaces : (unsigned)sm_count * 2u;
     if (grid < 1u) grid = 1u;
-    auto kern = scan ? place_ns_kernel<true> : place_ns_kernel<false>;
-    static thread_local size_t attr_set[2] = {0, 0};
-    if (smem > attr_set[scan ? 1 : 0]) {
+    const bool indexed = index != kNsIndexNone;
+    auto kern = scan ? (indexed ? place_ns_kernel<true, true> : place_ns_kernel<true, false>)
+                     : (indexed ? place_ns_kernel<false, true> : place_ns_kernel<false, false>);
+    const int variant = (scan ? 1 : 0) | (indexed ? 2 : 0);
+    static thread_local size_t attr_set[4] = {0, 0, 0, 0};
+    if (smem > attr_set[variant]) {
       e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
-      attr_set[scan ? 1 : 0] = smem;
+      attr_set[variant] = smem;
     }
     e = launch_pdl(kern, dim3(grid), dim3(scan ? kNsScanThreads : kNsThreads), smem, s, true, a, map);
     if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
   }
-  return 2;
+  return launched;
 }
 
 cudaError_t set_place_ns_carveout(int pct) {  // see set_sweep_carveout (lwse_lws_kernels.cu)
@@ -739,8 +882,10 @@ cudaError_t set_place_ns_carveout(int pct) {  // see set_sweep_carveout (lwse_lw
     if (r != cudaSuccess) e = r;
   };
   set((const void*)place_condense_kernel);
-  set((const void*)place_ns_kernel<false>);
-  set((const void*)place_ns_kernel<true>);
+  set((const void*)place_ns_kernel<false, false>);
+  set((const void*)place_ns_kernel<true, false>);
+  set((const void*)place_ns_kernel<false, true>);
+  set((const void*)place_ns_kernel<true, true>);
   return e;
 }
 

@@ -41,6 +41,7 @@ SYMBOLS = {
     "lwse_resident_tick_wait": ([C.c_void_p, C.POINTER(R.Tick)], C.c_int),
     "lwse_resident_place_outputs": ([C.c_void_p, C.c_void_p], C.c_int),
     "lwse_resident_occupancy": ([C.c_void_p, C.c_void_p], C.c_int),
+    "lwse_resident_tick_info": ([C.c_void_p, C.c_void_p], C.c_int),
     "lwse_place_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
         C.c_int,
@@ -362,6 +363,16 @@ class Engine:
         occ = np.zeros(max(self.n_nodes, 1), dtype=np.uint32)
         self._check(lib().lwse_resident_occupancy(self._h, R.ptr(occ)))
         return occ[: self.n_nodes]
+
+    TICK_FORMS = {0: "none", 1: "general", 2: "namespace", 3: "scan"}
+
+    def resident_tick_info(self) -> dict:
+        """How the most recently submitted tick ran: ``form`` (none | general | namespace | scan),
+        ``indexed`` (the namespace form went through the namespace index: the request table is not
+        grouped), ``index_built`` (this tick rebuilt that index), ``graph`` (replayed as a CUDA graph)."""
+        w = (C.c_uint32 * 4)()
+        self._check(lib().lwse_resident_tick_info(self._h, w))
+        return {"form": self.TICK_FORMS[w[0]], "indexed": bool(w[1]), "index_built": bool(w[2]), "graph": bool(w[3])}
 
     def resident_patch(self, which: int, rows, values):
         """Overwrite rows of a resident table (rows: uint32 indices, values: packed rows)."""

@@ -5,18 +5,28 @@ The reference reads its world through informer-cache ``List`` calls on every rec
 engine keeps the same world as resident record tables; this module keeps them current from the
 watch stream, so that a reconcile pass is ``lwse_resident_tick(patches)`` instead of a re-encode:
 
-* the tables are laid out in **slots**: every LeaderWorkerSet owns a fixed range of group rows,
-  pod rows and placement-request rows with some slack, so an event never moves another object;
+* the tables are laid out in **slots**: every LeaderWorkerSet owns one LWS row and a fixed range of
+  group rows, pod rows and placement-request rows with some slack, so an event never moves another
+  object.  The tables carry spare rows of every kind (LWS rows included) and spare namespace ids;
 * an event marks its object dirty; ``flush()`` re-encodes just the dirty objects with the very
   function the full encoder uses (``encoder.encode_lws`` on the object's slice of the cache — the
   incremental tables therefore mean exactly what a fresh encode means), compares the fresh rows
   with the resident ones and emits one patch segment per table holding only the rows that differ;
-* an object that outgrows its slots is moved to the spare rows at the end of the tables; when
-  those run out ``needs_reload`` is set and the caller re-encodes everything (``lwse_resident_load``).
+* a LeaderWorkerSet ``ADDED`` takes a vacant LWS row and slot ranges (first fit among the ranges
+  freed by earlier deletions, otherwise from the spare tail); pods and StatefulSets seen before
+  their set (separate informers do not order events between each other) are cached and encoded
+  with it.  ``DELETED`` zeroes the object's LWS, group and pod rows (node occupancy stays exact)
+  and makes its request rows inert; its rows are free again from the next ``flush()``;
+* an object that outgrows its slots moves to free rows; when the spare LWS rows, slot rows or
+  namespace ids run out ``needs_reload`` is set and the caller re-encodes everything
+  (``lwse_resident_load``), which lays objects out in (namespace, name) order again.
 
-Rows that no object references (slack, vacated slots) are never read by the engine: group rows are
+Rows that no object references (slack, vacant rows) are never read for a result: group rows are
 reached through ``lws.group_base/count``, pod rows through ``groups.pod_base/count``; unused
-placement-request rows are inert (unpinned, size 0).
+placement-request rows are inert (unpinned, size 0).  Reused request rows can carry another
+namespace than their neighbours: the request table is then no longer grouped by namespace, and the
+engine's resident tick runs the placement round through a namespace index (DESIGN §3.5).
+``object_of_lws_row`` / ``object_of_group_row`` route a changed result row back to its object.
 """
 from __future__ import annotations
 
@@ -36,7 +46,7 @@ class Slots:
     group_cap: int
     pod_base: int
     pod_cap: int
-    req_base: int  # placement request rows = group rows of exclusive objects (same count as group_cap), or -1
+    req_base: int  # placement request rows = group rows of exclusive objects (same rows as the group range)
 
 
 @dataclass
@@ -61,6 +71,31 @@ def _slack(n: int) -> int:
     return n + max(2, n // 4)
 
 
+def _take(free: list, cap: int) -> Optional[int]:
+    """First fit in a list of free [base, length] ranges: the base of `cap` rows, or None."""
+    for i, (base, n) in enumerate(free):
+        if n >= cap:
+            if n == cap:
+                free.pop(i)
+            else:
+                free[i] = [base + cap, n - cap]
+            return base
+    return None
+
+
+def _give(free: list, base: int, cap: int):
+    """Return a range to a free list, merged with its neighbours."""
+    free.append([base, cap])
+    free.sort()
+    merged = [free[0]]
+    for b, n in free[1:]:
+        if merged[-1][0] + merged[-1][1] == b:
+            merged[-1][1] += n
+        else:
+            merged.append([b, n])
+    free[:] = merged
+
+
 class IncrementalEncoder:
     """Resident tables + the slice of the informer cache they were encoded from."""
 
@@ -72,7 +107,7 @@ class IncrementalEncoder:
         self.node_rec, self.domain_values, self.node_index = self._encoded_nodes
         self.ns_ids = dict(namespaces or {})  # namespace name → dense id (exclusivity scope)
         self.items: dict[tuple, encoder.LwsItem] = {(it.lws.namespace, it.lws.name): it for it in items}
-        self.pods: dict[tuple, dict] = {}  # (ns, set name) → {pod name: Pod}
+        self.pods: dict[tuple, dict] = {}  # (ns, set name) → {pod name: Pod}; also for sets not (yet) known
         self.sts: dict[tuple, dict] = {}   # (ns, set name) → {sts name: StatefulSet}  (the leader sts lives in the item)
         for p in cluster.pods:
             self.pods.setdefault((p.namespace, p.labels.get(api.SetNameLabelKey)), {})[p.name] = p
@@ -80,18 +115,16 @@ class IncrementalEncoder:
             self.sts.setdefault((s.namespace, s.labels.get(api.SetNameLabelKey)), {})[s.name] = s
         self.needs_reload = False
         self.dirty: set = set()
+        self._deleted: set = set()  # objects deleted since the last flush whose rows are still resident
         # ---- first layout: objects in (namespace id, name) order so that the request table is grouped by namespace
         keys = sorted(self.items, key=lambda k: (self._ns_id(k[0]), k))
         fresh = {k: self._encode_object(k) for k in keys}
         self.slots: dict[tuple, Slots] = {}
-        g = p = r = 0
+        g = p = 0
         for i, k in enumerate(keys):
-            t = fresh[k]
-            gcap = _slack(max(len(t.groups), self._wanted_groups(k)))
-            size = max(1, self.items[k].lws.size)
-            pcap = max(_slack(len(t.pod_state)), gcap * (size + 1))
-            self.slots[k] = Slots(i, g, gcap, p, pcap, r)
-            g, p, r = g + gcap, p + pcap, r + gcap
+            gcap, pcap = self._caps(k, len(fresh[k].groups), len(fresh[k].pod_state))
+            self.slots[k] = Slots(i, g, gcap, p, pcap, g)
+            g, p = g + gcap, p + pcap
         self.order = keys
         n_lws = len(keys)
         self.lws = R.aligned_empty(n_lws + max(4, int(n_lws * spare)), R.LWS_REC)
@@ -99,13 +132,21 @@ class IncrementalEncoder:
         self.pod_state = R.aligned_empty(p + max(64, int(p * spare)), R.POD_STATE)
         self.pod_ident = R.aligned_empty(len(self.pod_state), R.POD_IDENT)
         self.reqs = R.aligned_empty(len(self.groups), R.PLACE_REQ)
-        self.n_lws, self.g_end, self.p_end, self.r_end = n_lws, g, p, r
+        self.n_lws, self.g_end, self.p_end, self.r_end = n_lws, g, p, g
+        # free rows below the ends (vacated by deletions and relocations): [base, length] ranges
+        self._free_lws: list = []
+        self._free_groups: list = []
+        self._free_pods: list = []
+        self._freed: list = []  # (free list, base, length) released by this flush: free from the next one
+        self._lws_key: dict[int, tuple] = {}
+        self._group_lws = np.full(len(self.groups), -1, dtype=np.int64)  # group row → owning LWS row, -1 = free
         last_ns = max([self._ns_id(k[0]) for k in keys], default=0)
         self.reqs["leader_node"] = R.NONE  # inert rows: unpinned, size 0 — never claim anything;
         self.reqs["ns"] = last_ns          # the spare tail keeps the table grouped by namespace
         for k in keys:
+            self._own(k)
             self._write_object(k, fresh[k], None)
-        self.n_namespaces = max(1, last_ns + 1, len(self.ns_ids))
+        self.n_namespaces = max(1, last_ns + 1, len(self.ns_ids)) + max(4, int(len(self.ns_ids) * spare))
 
     # ------------------------------------------------------------------ helpers
     def _ns_id(self, namespace: str) -> int:
@@ -120,6 +161,12 @@ class IncrementalEncoder:
         if it.leader_sts is not None:
             want = max(want, it.leader_sts.replicas)
         return max(want, 0)
+
+    def _caps(self, key, ng: int, npod: int) -> tuple:
+        """(group rows, pod rows) of a slot for an object with `ng` groups and `npod` pods."""
+        gcap = _slack(max(ng, self._wanted_groups(key)))
+        size = max(1, self.items[key].lws.size)
+        return gcap, max(_slack(npod), gcap * (size + 1))
 
     def _encode_object(self, key) -> encoder.LwsTables:
         it = self.items[key]
@@ -140,12 +187,32 @@ class IncrementalEncoder:
             out[idx] = rq
         return out
 
+    def _put(self, patches: Optional[Patches], table_id: int, table: np.ndarray, base: int, fresh_rows: np.ndarray):
+        """Write rows [base, base + n) of a table; with `patches`, emit the rows that changed."""
+        n = len(fresh_rows)
+        if n == 0:
+            return
+        cur = table[base: base + n]
+        if patches is None:
+            cur[:] = fresh_rows
+            return
+        a = np.ascontiguousarray(cur).view(np.uint8).reshape(n, -1)
+        b = np.ascontiguousarray(fresh_rows).view(np.uint8).reshape(n, -1)
+        diff = np.flatnonzero((a != b).any(axis=1))
+        if len(diff):
+            vals = R.aligned_empty(len(diff), table.dtype)
+            vals[:] = fresh_rows[diff]
+            cur[diff] = vals
+            patches._pending.setdefault(table_id, ([], []))
+            patches._pending[table_id][0].extend((diff + base).tolist())
+            patches._pending[table_id][1].append(vals)
+
     def _write_object(self, key, t: encoder.LwsTables, patches: Optional[Patches]):
         """Place the object's fresh rows into its slots; with `patches`, emit the rows that changed."""
         sl = self.slots[key]
         ng, npod = len(t.groups), len(t.pod_state)
         if ng > sl.group_cap or npod > sl.pod_cap:
-            if not self._relocate(key, ng, npod):
+            if not self._relocate(key, ng, npod, patches):
                 self.needs_reload = True
                 return
             sl = self.slots[key]
@@ -156,50 +223,85 @@ class IncrementalEncoder:
         grp["pod_base"] = grp["pod_base"].astype(np.int64) + sl.pod_base
         reqs = self._object_requests(key, t, sl)
 
-        def put(table_id, table, base, fresh_rows):
-            n = len(fresh_rows)
-            if n == 0:
-                return
-            cur = table[base: base + n]
-            if patches is None:
-                cur[:] = fresh_rows
-                return
-            a = np.ascontiguousarray(cur).view(np.uint8).reshape(n, -1)
-            b = np.ascontiguousarray(fresh_rows).view(np.uint8).reshape(n, -1)
-            diff = np.flatnonzero((a != b).any(axis=1))
-            if len(diff):
-                vals = R.aligned_empty(len(diff), table.dtype)
-                vals[:] = fresh_rows[diff]
-                cur[diff] = vals
-                patches._pending.setdefault(table_id, ([], []))
-                patches._pending[table_id][0].extend((diff + base).tolist())
-                patches._pending[table_id][1].append(vals)
-
-        put(R.TABLE_LWS, self.lws, sl.lws_row, lws_row)
-        put(R.TABLE_GROUPS, self.groups, sl.group_base, grp)
+        self._put(patches, R.TABLE_LWS, self.lws, sl.lws_row, lws_row)
+        self._put(patches, R.TABLE_GROUPS, self.groups, sl.group_base, grp)
         # the pod columns are written over the WHOLE slot range: rows a shrinking object no longer
         # references go back to zero (the engine counts node occupancy over every identity row)
         pst = R.aligned_empty(sl.pod_cap, R.POD_STATE)
         pst[:npod] = t.pod_state
         pid = R.aligned_empty(sl.pod_cap, R.POD_IDENT)
         pid[:npod] = t.pod_ident
-        put(R.TABLE_POD_STATE, self.pod_state, sl.pod_base, pst)
-        put(R.TABLE_POD_IDENT, self.pod_ident, sl.pod_base, pid)
-        put(R.TABLE_PLACE_REQS, self.reqs, sl.req_base, reqs)
+        self._put(patches, R.TABLE_POD_STATE, self.pod_state, sl.pod_base, pst)
+        self._put(patches, R.TABLE_POD_IDENT, self.pod_ident, sl.pod_base, pid)
+        self._put(patches, R.TABLE_PLACE_REQS, self.reqs, sl.req_base, reqs)
 
-    def _relocate(self, key, ng: int, npod: int) -> bool:
-        """Move an object that outgrew its slots to the spare rows at the end of the tables."""
+    def _alloc(self, gcap: int, pcap: int) -> Optional[tuple]:
+        """(group base, pod base) of free ranges — first fit among freed ranges, else the spare tail — or None."""
+        g = _take(self._free_groups, gcap)
+        if g is None and self.g_end + gcap <= len(self.groups):
+            g, self.g_end = self.g_end, self.g_end + gcap
+            self.r_end = self.g_end
+        if g is None:
+            return None
+        p = _take(self._free_pods, pcap)
+        if p is None and self.p_end + pcap <= len(self.pod_state):
+            p, self.p_end = self.p_end, self.p_end + pcap
+        if p is None:
+            self._freed.append((self._free_groups, g, gcap))
+            return None
+        return g, p
+
+    def _vacate(self, sl: Slots, ns: int, patches: Optional[Patches], whole: bool):
+        """The object's rows stop taking part: pod rows back to zero (occupancy), request rows inert;
+        with `whole` (a deletion) its group rows and LWS row too.  The rows are free from the next flush."""
+        inert = R.aligned_empty(sl.group_cap, R.PLACE_REQ)
+        inert["leader_node"] = R.NONE
+        inert["ns"] = ns
+        self._put(patches, R.TABLE_PLACE_REQS, self.reqs, sl.req_base, inert)
+        self._put(patches, R.TABLE_POD_STATE, self.pod_state, sl.pod_base, R.aligned_empty(sl.pod_cap, R.POD_STATE))
+        self._put(patches, R.TABLE_POD_IDENT, self.pod_ident, sl.pod_base, R.aligned_empty(sl.pod_cap, R.POD_IDENT))
+        if whole:
+            self._put(patches, R.TABLE_GROUPS, self.groups, sl.group_base, R.aligned_empty(sl.group_cap, R.GROUP_REC))
+            self._put(patches, R.TABLE_LWS, self.lws, sl.lws_row, R.aligned_empty(1, R.LWS_REC))
+            self._lws_key.pop(sl.lws_row, None)
+            self._freed.append((self._free_lws, sl.lws_row, 1))
+        self._group_lws[sl.group_base: sl.group_base + sl.group_cap] = -1
+        self._freed.append((self._free_groups, sl.group_base, sl.group_cap))
+        self._freed.append((self._free_pods, sl.pod_base, sl.pod_cap))
+
+    def _own(self, key):
         sl = self.slots[key]
-        gcap = _slack(max(ng, self._wanted_groups(key)))
-        size = max(1, self.items[key].lws.size)
-        pcap = max(_slack(npod), gcap * (size + 1))
-        if self.g_end + gcap > len(self.groups) or self.p_end + pcap > len(self.pod_state) or self.r_end + gcap > len(self.reqs):
+        self._lws_key[sl.lws_row] = key
+        self._group_lws[sl.group_base: sl.group_base + sl.group_cap] = sl.lws_row
+
+    def _relocate(self, key, ng: int, npod: int, patches: Optional[Patches]) -> bool:
+        """Move an object that outgrew its slots to free rows."""
+        sl = self.slots[key]
+        gcap, pcap = self._caps(key, ng, npod)
+        got = self._alloc(gcap, pcap)
+        if got is None:
             return False
-        # the vacated request rows must stop claiming: they are rewritten as inert by the diff below
-        self._vacated_reqs = (sl.req_base, sl.group_cap, self._ns_id(key[0]))
-        self._vacated_pods = (sl.pod_base, sl.pod_cap)  # and the vacated pod rows must stop occupying nodes
-        self.slots[key] = Slots(sl.lws_row, self.g_end, gcap, self.p_end, pcap, self.r_end)
-        self.g_end, self.p_end, self.r_end = self.g_end + gcap, self.p_end + pcap, self.r_end + gcap
+        self._vacate(sl, self._ns_id(key[0]), patches, whole=False)
+        self.slots[key] = Slots(sl.lws_row, got[0], gcap, got[1], pcap, got[0])
+        self._own(key)
+        return True
+
+    def _create(self, key, t: encoder.LwsTables) -> bool:
+        """Slots for a new object: a vacant LWS row and free ranges.  False: nothing left, reload."""
+        if self._ns_id(key[0]) >= self.n_namespaces:
+            return False
+        row = _take(self._free_lws, 1)
+        if row is None and self.n_lws < len(self.lws):
+            row, self.n_lws = self.n_lws, self.n_lws + 1
+        if row is None:
+            return False
+        gcap, pcap = self._caps(key, len(t.groups), len(t.pod_state))
+        got = self._alloc(gcap, pcap)
+        if got is None:
+            self._freed.append((self._free_lws, row, 1))
+            return False
+        self.slots[key] = Slots(row, got[0], gcap, got[1], pcap, got[0])
+        self._own(key)
         return True
 
     # ------------------------------------------------------------------- events
@@ -207,40 +309,49 @@ class IncrementalEncoder:
         return (obj.namespace, obj.labels.get(api.SetNameLabelKey))
 
     def pod_event(self, kind: str, pod: api.Pod):
-        """kind: ADDED | MODIFIED | DELETED (a watch event of the pod informer)."""
+        """kind: ADDED | MODIFIED | DELETED (a watch event of the pod informer).  Pods of a set not
+        known (yet, or any more) are only cached."""
         key = self._set_key(pod)
-        if key not in self.items:
-            return
         bucket = self.pods.setdefault(key, {})
         if kind == "DELETED":
             bucket.pop(pod.name, None)
         else:
             bucket[pod.name] = pod
-        self.dirty.add(key)
+        if key in self.items:
+            self.dirty.add(key)
 
     def statefulset_event(self, kind: str, sts: api.StatefulSet):
         key = self._set_key(sts)
-        if key not in self.items:
-            return
-        it = self.items[key]
-        if sts.name == it.lws.name and api.GroupIndexLabelKey not in sts.labels:  # the leader StatefulSet
+        it = self.items.get(key)
+        if it is not None and sts.name == it.lws.name and api.GroupIndexLabelKey not in sts.labels:  # the leader StatefulSet
             it.leader_sts = None if kind == "DELETED" else sts
-        else:
+        else:  # (a leader StatefulSet seen before its set waits here too)
             bucket = self.sts.setdefault(key, {})
             if kind == "DELETED":
                 bucket.pop(sts.name, None)
             else:
                 bucket[sts.name] = sts
-        self.dirty.add(key)
+        if it is not None:
+            self.dirty.add(key)
 
     def lws_event(self, kind: str, item: encoder.LwsItem):
-        """MODIFIED only: a new or deleted object changes the table shapes → reload."""
+        """ADDED | MODIFIED | DELETED of a LeaderWorkerSet.  A new object takes spare rows at the next
+        ``flush()``; a deleted one gives its rows back there."""
         key = (item.lws.namespace, item.lws.name)
-        if kind != "MODIFIED" or key not in self.items:
-            self.needs_reload = True
+        if kind == "DELETED":
+            if self.items.pop(key, None) is not None:
+                self.dirty.discard(key)
+                if key in self.slots:
+                    self._deleted.add(key)
             return
-        keep = self.items[key]
-        item.leader_sts = item.leader_sts if item.leader_sts is not None else keep.leader_sts
+        keep = self.items.get(key)
+        if keep is not None:
+            item.leader_sts = item.leader_sts if item.leader_sts is not None else keep.leader_sts
+        elif item.leader_sts is None:  # a new object: its leader StatefulSet may already be cached
+            bucket = self.sts.get(key, {})
+            leader = bucket.get(item.lws.name)
+            if leader is not None and api.GroupIndexLabelKey not in leader.labels:
+                item.leader_sts = bucket.pop(item.lws.name)
         self.items[key] = item
         self.dirty.add(key)
 
@@ -248,35 +359,19 @@ class IncrementalEncoder:
         """Re-encode the dirty objects → the patch segments of one ``lwse_resident_tick``."""
         patches = Patches()
         patches._pending = {}
+        for key in sorted(self._deleted):
+            self._vacate(self.slots.pop(key), self._ns_id(key[0]), patches, whole=True)
+        self._deleted.clear()
         for key in sorted(self.dirty):
-            self._vacated_reqs = None
-            self._vacated_pods = None
-            self._write_object(key, self._encode_object(key), patches)
-            if self._vacated_reqs is not None:
-                base, cap, ns = self._vacated_reqs
-                inert = R.aligned_empty(cap, R.PLACE_REQ)
-                inert["leader_node"] = R.NONE
-                inert["ns"] = ns
-                cur = self.reqs[base: base + cap]
-                diff = np.flatnonzero((np.ascontiguousarray(cur).view(np.uint8).reshape(cap, -1)
-                                       != inert.view(np.uint8).reshape(cap, -1)).any(axis=1))
-                if len(diff):
-                    cur[diff] = inert[diff]
-                    patches._pending.setdefault(R.TABLE_PLACE_REQS, ([], []))
-                    patches._pending[R.TABLE_PLACE_REQS][0].extend((diff + base).tolist())
-                    patches._pending[R.TABLE_PLACE_REQS][1].append(inert[diff].copy())
-            if self._vacated_pods is not None:
-                base, cap = self._vacated_pods
-                for table_id, table in ((R.TABLE_POD_STATE, self.pod_state), (R.TABLE_POD_IDENT, self.pod_ident)):
-                    cur = table[base: base + cap]
-                    used = np.flatnonzero(np.ascontiguousarray(cur).view(np.uint8).reshape(cap, -1).any(axis=1))
-                    if len(used):
-                        zeros = R.aligned_empty(len(used), table.dtype)
-                        cur[used] = zeros
-                        patches._pending.setdefault(table_id, ([], []))
-                        patches._pending[table_id][0].extend((used + base).tolist())
-                        patches._pending[table_id][1].append(zeros)
+            t = self._encode_object(key)
+            if key not in self.slots and not self._create(key, t):
+                self.needs_reload = True
+                continue
+            self._write_object(key, t, patches)
         self.dirty.clear()
+        for free, base, n in self._freed:  # rows given back in this flush may be patched in it: reuse from the next
+            _give(free, base, n)
+        self._freed.clear()
         for table_id in (R.TABLE_LWS, R.TABLE_GROUPS, R.TABLE_POD_STATE, R.TABLE_POD_IDENT, R.TABLE_PLACE_REQS):
             if table_id in patches._pending:
                 rows, chunks = patches._pending[table_id]
@@ -291,11 +386,26 @@ class IncrementalEncoder:
                 self.pod_ident[: self.p_end], self.reqs[: self.r_end])
 
     def full_tables(self):
-        """The whole allocation (what ``resident_load`` should take, so that relocations stay in range)."""
-        return self.lws[: self.n_lws], self.groups, self.pod_state, self.pod_ident, self.reqs
+        """The whole allocation, spare rows included (what ``resident_load`` / ``resident_place_load``
+        should take, so that new objects and relocations stay in range)."""
+        return self.lws, self.groups, self.pod_state, self.pod_ident, self.reqs
 
     def group_row(self, namespace: str, name: str, group_index: int) -> int:
         return self.slots[(namespace, name)].group_base + group_index
 
     def lws_row(self, namespace: str, name: str) -> int:
         return self.slots[(namespace, name)].lws_row
+
+    def object_of_lws_row(self, row: int) -> Optional[tuple]:
+        """(namespace, name) of the object an LWS result row belongs to, or None for a vacant row."""
+        return self._lws_key.get(int(row))
+
+    def object_of_group_row(self, row: int) -> Optional[tuple]:
+        """(namespace, name, group index) of a group result row, or None for a vacant or slack row."""
+        row = int(row)
+        lr = int(self._group_lws[row]) if 0 <= row < len(self._group_lws) else -1
+        key = self._lws_key.get(lr)
+        if key is None:
+            return None
+        gi = row - self.slots[key].group_base
+        return (key[0], key[1], gi) if gi < int(self.lws["group_count"][lr]) else None
