@@ -343,7 +343,9 @@ LWSE_API uint64_t lwse_hash64(const void* bytes, size_t len);
 /* ------------------------------------------------------------------------- */
 /* Node table                                                                */
 /* ------------------------------------------------------------------------- */
-/* Copies n node rows to the device; they stay resident across sweeps. */
+/* Copies n node rows to the device; they stay resident across sweeps (and are patched row by row
+ * with LWSE_TABLE_NODES).  After lwse_resident_load, the occupancy counters of the resident pods are
+ * recounted for the new table. */
 LWSE_API int lwse_upload_nodes(lwse_engine* e, const lwse_node_rec* nodes, uint32_t n_nodes,
                                uint32_t n_domains);
 
@@ -370,7 +372,14 @@ typedef enum lwse_table {
   LWSE_TABLE_GROUPS = 1,    /* lwse_group_rec  */
   LWSE_TABLE_POD_STATE = 2, /* lwse_pod_state  */
   LWSE_TABLE_POD_IDENT = 3, /* lwse_pod_ident  */
-  LWSE_TABLE_PLACE_REQS = 4 /* lwse_place_req (lwse_resident_place_load)  */
+  LWSE_TABLE_PLACE_REQS = 4, /* lwse_place_req (lwse_resident_place_load)  */
+  LWSE_TABLE_NODES = 5        /* lwse_node_rec: the table of the last lwse_upload_nodes.  Rows must be
+                                 < its n_nodes: patches never change the table's size, so the caller
+                                 reserves spare rows (flags = 0: no request can use them) at upload.
+                                 A patched row means what an uploaded row means: a node is usable iff
+                                 SCHEDULABLE, HAS_TOPOLOGY and domain_id < n_domains.  Multi-rank
+                                 ticks (LWSE_TICK_SHARED_OCCUPANCY): every rank applies the same node
+                                 patches in the same tick.                                      */
 } lwse_table;
 
 /* Result rows that differ from the previous resident sweep (all rows after a load).
@@ -500,6 +509,19 @@ typedef struct lwse_tick_info {
 #define LWSE_TICK_FORM_NAMESPACE 2u /* namespace-parallel, two-level                         */
 #define LWSE_TICK_FORM_SCAN 3u      /* namespace-parallel, scan (LWSE_SWEEP_PLACE_SCAN)       */
 LWSE_API int lwse_resident_tick_info(lwse_engine* e, lwse_tick_info* info);
+
+/* What the node-row patches (LWSE_TABLE_NODES) of the most recently submitted tick did (read-only).
+ * The placement round reads the usable nodes through a domain-sorted index on the device.  A patch
+ * that only changes a node's capacity keeps the index; one that changes whether a node is usable,
+ * or the domain of a usable node, has the next placement round rebuild it first (three kernels in
+ * front of the round). */
+typedef struct lwse_node_info {
+  uint32_t rows_patched; /* node rows in the tick's segments                                      */
+  uint32_t index_built;  /* 1: this tick rebuilt the node index                                    */
+  uint32_t n_usable;     /* usable nodes after the tick's patches                                  */
+  uint32_t reserved;
+} lwse_node_info;
+LWSE_API int lwse_resident_node_info(lwse_engine* e, lwse_node_info* info);
 
 /* ------------------------------------------------------------------------- */
 /* Placement (build-defined spec — the reference has no node scoring)        */

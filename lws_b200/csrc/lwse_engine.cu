@@ -90,11 +90,15 @@ struct PlaceNsExchange {
 enum PlaceNsIndex : uint32_t { kNsIndexNone = 0, kNsIndexReuse = 1, kNsIndexBuild = 2 };
 bool place_ns_supported(uint32_t n_nodes, uint32_t n_domains);
 int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, const uint32_t* d_node_order, uint32_t n_nodes,
-                    uint32_t n_usable, uint32_t n_domains, const lwse_place_req* d_reqs, uint32_t n_reqs,
+                    uint32_t n_domains, const lwse_place_req* d_reqs, uint32_t n_reqs,
                     const uint32_t* d_occupancy, uint32_t n_parts, uint64_t part_stride_bytes, uint32_t n_namespaces,
                     lwse_place_out* d_out, void* d_scratch, size_t scratch_bytes, bool fresh, uint32_t call_index, bool scan,
                     int sm_count, cudaStream_t s, int* cuda_err, const uint32_t** d_counters_out, bool first_pdl,
                     const PlaceNsChanges* changes, const PlaceNsExchange* xch, PlaceNsIndex index);
+size_t node_index_scratch_bytes(uint32_t n_domains);
+int launch_node_index(const lwse_node_rec* d_nodes, uint32_t n_nodes, uint32_t n_domains, uint32_t* d_dom_first,
+                      uint32_t* d_node_order, uint32_t* d_node_pos, void* d_scratch, int sm_count, cudaStream_t s,
+                      bool pdl, int* cuda_err);
 int launch_place_diff(const lwse_place_out* d_cur, lwse_place_out* d_prev, uint32_t n, uint32_t* d_rows,
                       lwse_place_out* d_outs, uint32_t capacity, uint32_t* d_count, cudaStream_t s, int* cuda_err);
 // lwse_ds_kernels.cu
@@ -189,8 +193,14 @@ struct lwse_engine {
   uint64_t launches = 0;
   // resident node table
   DevBuf nodes;
-  DevBuf dom_first, node_order, node_pos;  // static domain-sorted index of the node table (placement)
+  DevBuf dom_first, node_order, node_pos;  // domain-sorted index of the usable nodes (placement), built on the device
+  DevBuf node_ix;                          // its build's per-domain counters and cursors (zero between builds)
   uint32_t n_nodes = 0, n_domains = 0;
+  std::vector<lwse_node_rec> h_nodes;      // host mirror of the node table: decides whether a patch needs a new index
+  bool node_index_stale = false;           // node patches changed usability / domains since the last build
+  bool main_unforked = false;              // a tick without a round patched tables on the engine's stream, and no
+                                           // round on the side stream has been ordered behind that scatter yet
+  lwse_node_info last_node_info{};         // lwse_resident_node_info
   // staging for the *_host entry points
   DevBuf lws, groups, pod_state, pod_ident, lws_out, group_out, occupancy, scan_scratch;
   DevBuf place_reqs, place_out, place_occ, place_scratch;
@@ -469,7 +479,7 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
       if (e->xch_connected && p != e->xch_rank && e->xch_peer[p]) cudaIpcCloseMemHandle(e->xch_peer[p]);
     e->xch.release();
     e->xch_peers_dev.release();
-    DevBuf* bufs[] = {&e->nodes,      &e->dom_first, &e->node_order, &e->node_pos, &e->lws,         &e->groups,     &e->pod_state,   &e->pod_ident,
+    DevBuf* bufs[] = {&e->nodes,      &e->dom_first, &e->node_order, &e->node_pos, &e->node_ix, &e->lws,  &e->groups,     &e->pod_state,   &e->pod_ident,
                       &e->scan_scratch, &e->lws_out,
                       &e->group_out,  &e->occupancy,   &e->place_reqs, &e->place_out,   &e->place_occ,
                       &e->place_scratch, &e->ds,       &e->ds_roles,   &e->ds_revroles, &e->ds_out,
@@ -503,6 +513,58 @@ LWSE_API int lwse_last_cuda_error(const lwse_engine* e) { return e ? e->last_cud
 LWSE_API void* lwse_stream(const lwse_engine* e) { return e ? (void*)e->stream : nullptr; }
 LWSE_API uint64_t lwse_launch_count(const lwse_engine* e) { return e ? e->launches : 0; }
 
+// A node a placement request can use: schedulable, labelled with the topology key, a domain in range.
+static bool node_usable(const lwse_node_rec& nd, uint32_t n_domains) {
+  return (nd.flags & LWSE_NODE_SCHEDULABLE) && (nd.flags & LWSE_NODE_HAS_TOPOLOGY) && nd.domain_id < n_domains;
+}
+
+// The domain-sorted node index (dom_first / node_order / node_pos), rebuilt on `s` from the device node
+// rows when node patches made it stale.  Called by every placement call in front of its round (in a tick:
+// on the side stream, behind the scatter that patched the rows).  `pdl`: the predecessor on `s` is a kernel.
+static int build_node_index_locked(lwse_engine* e, cudaStream_t s, bool pdl, bool* built = nullptr) {
+  if (built) *built = false;
+  if (!e->node_index_stale) return LWSE_OK;
+  int cuda_err = 0;
+  const int launched = lwse::launch_node_index((const lwse_node_rec*)e->nodes.p, e->n_nodes, e->n_domains, (uint32_t*)e->dom_first.p,
+                                               (uint32_t*)e->node_order.p, (uint32_t*)e->node_pos.p, e->node_ix.p, e->sm_count, s,
+                                               pdl, &cuda_err);
+  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+  e->launches += (uint64_t)launched;
+  e->node_index_stale = false;
+  if (built) *built = true;
+  return LWSE_OK;
+}
+
+// Node-row patches of a tick (or of lwse_resident_patch), before any of them is applied: checks the
+// segments, brings the host mirror up to date and marks the index stale when a row's usability, or the
+// domain of a usable row, changed.  Capacity-only patches keep the index.  Returns the rows patched or < 0.
+static int node_patches_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs) {
+  uint32_t n_rows = 0;
+  for (uint32_t i = 0; i < n_segs; i++) {
+    const lwse_patch_seg& g = segs[i];
+    if (g.table != LWSE_TABLE_NODES || g.n == 0) continue;
+    if (e->n_nodes == 0) return LWSE_ERR_NOT_READY;
+    if (!g.values || (!(g.flags & LWSE_PATCH_RANGE) && !g.rows)) return LWSE_ERR_INVALID_ARG;
+    if ((g.flags & LWSE_PATCH_RANGE) && (uint64_t)g.first_row + g.n > e->n_nodes) return LWSE_ERR_BAD_TABLE;
+  }
+  for (uint32_t i = 0; i < n_segs; i++) {
+    const lwse_patch_seg& g = segs[i];
+    if (g.table != LWSE_TABLE_NODES) continue;
+    const lwse_node_rec* v = static_cast<const lwse_node_rec*>(g.values);
+    for (uint32_t k = 0; k < g.n; k++) {
+      const uint32_t row = (g.flags & LWSE_PATCH_RANGE) ? g.first_row + k : g.rows[k];
+      if (row >= e->n_nodes) continue;  // (the scatter kernel skips it too)
+      lwse_node_rec& old = e->h_nodes[row];
+      const bool was = node_usable(old, e->n_domains), is = node_usable(v[k], e->n_domains);
+      if (was != is || (is && old.domain_id != v[k].domain_id)) e->node_index_stale = true;
+      e->n_usable = e->n_usable - (was ? 1u : 0u) + (is ? 1u : 0u);
+      old = v[k];
+      n_rows++;
+    }
+  }
+  return (int)n_rows;
+}
+
 LWSE_API int lwse_upload_nodes(lwse_engine* e, const lwse_node_rec* nodes, uint32_t n_nodes,
                                uint32_t n_domains) {
   if (!e || (n_nodes && !nodes) || !aligned16(nodes)) return LWSE_ERR_INVALID_ARG;
@@ -514,46 +576,40 @@ LWSE_API int lwse_upload_nodes(lwse_engine* e, const lwse_node_rec* nodes, uint3
     if (drc != LWSE_OK) return drc;
     invalidate_tick_graphs(e);
   }
+  // every placement call orders behind the previous one (which may still read the index rewritten here)
+  if (e->place_pending) LWSE_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_place, 0));
   LWSE_CUDA(e, e->nodes.reserve((size_t)n_nodes * sizeof(lwse_node_rec) + 16));
-  // Static index for the placement round: the usable nodes (schedulable, labelled with a
-  // topology domain) in domain order — a counting sort, done once per node-table upload.
-  // dom_first[d] .. dom_first[d + 1] is the run of domain d in node_order; node_pos is the
-  // inverse (LWSE_NONE for nodes no request can use).
-  std::vector<uint32_t> first((size_t)n_domains + 2, 0u), order, pos(n_nodes ? n_nodes : 1, LWSE_NONE);
-  auto usable = [&](const lwse_node_rec& nd) {
-    return (nd.flags & LWSE_NODE_SCHEDULABLE) && (nd.flags & LWSE_NODE_HAS_TOPOLOGY) && nd.domain_id < n_domains;
-  };
-  for (uint32_t n = 0; n < n_nodes; n++)
-    if (usable(nodes[n])) first[(size_t)nodes[n].domain_id + 1]++;
-  for (uint32_t d = 0; d < n_domains; d++) first[(size_t)d + 1] += first[d];
-  order.resize(first[n_domains] ? first[n_domains] : 1, 0u);
-  {
-    std::vector<uint32_t> cursor(first.begin(), first.end() - 1);
-    for (uint32_t n = 0; n < n_nodes; n++)
-      if (usable(nodes[n])) {
-        const uint32_t p = cursor[nodes[n].domain_id]++;
-        order[p] = n;
-        pos[n] = p;
-      }
-  }
   LWSE_CUDA(e, e->dom_first.reserve(((size_t)n_domains + 1) * 4 + 16));
   // (padded to whole rows of 256 entries: the namespace-parallel placement kernel stages the index
   // into shared memory with one bulk copy of that size)
   const size_t order_padded = ((size_t)(n_nodes + 255u) / 256u + 1u) * 1024u;
   LWSE_CUDA(e, e->node_order.reserve(order_padded + 16));
   LWSE_CUDA(e, cudaMemsetAsync(e->node_order.p, 0, order_padded, e->stream));
-  LWSE_CUDA(e, e->node_pos.reserve(pos.size() * 4 + 16));
+  LWSE_CUDA(e, e->node_pos.reserve((size_t)n_nodes * 4 + 16));
+  LWSE_CUDA(e, e->node_ix.reserve(lwse::node_index_scratch_bytes(n_domains)));
+  LWSE_CUDA(e, cudaMemsetAsync(e->node_ix.p, 0, lwse::node_index_scratch_bytes(n_domains), e->stream));
   if (n_nodes)
     LWSE_CUDA(e, cudaMemcpyAsync(e->nodes.p, nodes, (size_t)n_nodes * sizeof(lwse_node_rec),
                                  cudaMemcpyHostToDevice, e->stream));
-  LWSE_CUDA(e, cudaMemcpyAsync(e->dom_first.p, first.data(), ((size_t)n_domains + 1) * 4, cudaMemcpyHostToDevice,
-                               e->stream));
-  LWSE_CUDA(e, cudaMemcpyAsync(e->node_order.p, order.data(), order.size() * 4, cudaMemcpyHostToDevice, e->stream));
-  LWSE_CUDA(e, cudaMemcpyAsync(e->node_pos.p, pos.data(), pos.size() * 4, cudaMemcpyHostToDevice, e->stream));
-  LWSE_CUDA(e, cudaStreamSynchronize(e->stream));  // the host vectors above go out of scope
   e->n_nodes = n_nodes;
   e->n_domains = n_domains;
-  e->n_usable = (uint32_t)first[n_domains];
+  e->h_nodes.assign(nodes, nodes + n_nodes);
+  e->n_usable = 0;
+  for (const lwse_node_rec& nd : e->h_nodes) e->n_usable += node_usable(nd, n_domains) ? 1u : 0u;
+  e->node_index_stale = true;
+  {
+    const int rc = build_node_index_locked(e, e->stream, false);
+    if (rc != LWSE_OK) return rc;
+  }
+  if (e->r_loaded && n_nodes) {  // the resident pods' occupancy, counted again for the new table
+    LWSE_CUDA(e, e->r_occ.reserve((size_t)n_nodes * 4 + 16));
+    int cuda_err = 0;
+    int launched = lwse::launch_occupancy((const lwse_pod_ident*)e->r_pid.p, e->rn_pods, (uint32_t*)e->r_occ.p, n_nodes,
+                                          e->sm_count, e->stream, &cuda_err);
+    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+    e->launches += (uint64_t)launched;
+  }
+  LWSE_CUDA(e, cudaStreamSynchronize(e->stream));
   e->place_ns_geometry[0] = e->place_ns_geometry[1] = e->place_ns_geometry[2] = e->place_ns_geometry[3] = 0;
   e->place_geometry[0] = e->place_geometry[1] = e->place_geometry[2] = e->place_geometry[3] = 0;  // re-initialise the scratch
   return LWSE_OK;
@@ -794,6 +850,9 @@ static bool resident_table(lwse_engine* e, uint32_t which, void** base, uint64_t
     case LWSE_TABLE_PLACE_REQS:
       if (!e->r_place_loaded) return false;
       *base = e->r_preq.p; *rows = e->rn_reqs; *row_bytes = sizeof(lwse_place_req); return true;
+    case LWSE_TABLE_NODES:
+      if (e->n_nodes == 0) return false;
+      *base = e->nodes.p; *rows = e->n_nodes; *row_bytes = sizeof(lwse_node_rec); return true;
     default: return false;
   }
 }
@@ -1008,7 +1067,8 @@ LWSE_API int lwse_resident_patch(lwse_engine* e, lwse_table which, const uint32_
                                  uint32_t n) {
   if (!e || (n && (!rows || !values))) return LWSE_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(e->mu);
-  if (!e->r_loaded) return LWSE_ERR_NOT_READY;
+  // (node rows only need the node table; the next placement call rebuilds the node index if they ask for it)
+  if (which == LWSE_TABLE_NODES ? e->n_nodes == 0 : !e->r_loaded) return LWSE_ERR_NOT_READY;
   if (n == 0) return LWSE_OK;
   DeviceGuard guard(e->device);
   {
@@ -1020,9 +1080,18 @@ LWSE_API int lwse_resident_patch(lwse_engine* e, lwse_table which, const uint32_
   seg.n = n;
   seg.rows = rows;
   seg.values = values;
+  if (which == LWSE_TABLE_NODES) {
+    // the round of the last placement call may still read the rows (and it reads them on another stream)
+    if (e->place_pending) LWSE_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_place, 0));
+    const int nrc = node_patches_locked(e, &seg, 1);
+    if (nrc < 0) return nrc;
+  }
   bool wrote = false;
   const int rc = apply_patches_locked(e, &seg, 1, &wrote);
-  if (rc != LWSE_OK) return rc;
+  if (rc != LWSE_OK) {
+    if (which == LWSE_TABLE_NODES) e->node_index_stale = true;  // (see tick_submit_locked)
+    return rc;
+  }
   // the caller's buffers (and the staging copy) are free again once the scatter ran
   LWSE_CUDA(e, cudaStreamSynchronize(e->stream));
   return LWSE_OK;
@@ -1071,13 +1140,18 @@ static int place_grouped_locked(lwse_engine* e, const lwse_place_req* d_reqs, ui
   const bool eager = cudaStreamIsCapturing(s, &capturing) == cudaSuccess && capturing == cudaStreamCaptureStatusNone;
   if (fresh && eager) invalidate_tick_graphs(e);  // (their kernel nodes hold the old scratch pointers)
   if (eager && e->place_pending) LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_place, 0));
+  bool built = false;
+  {
+    const int rc = build_node_index_locked(e, s, false, &built);
+    if (rc != LWSE_OK) return rc;
+  }
   int cuda_err = 0;
   const uint32_t* counters = nullptr;
   int launched = lwse::launch_place_ns((const lwse_node_rec*)e->nodes.p, (const uint32_t*)e->dom_first.p,
-                                       (const uint32_t*)e->node_order.p, e->n_nodes, e->n_usable, e->n_domains, d_reqs, n_reqs,
+                                       (const uint32_t*)e->node_order.p, e->n_nodes, e->n_domains, d_reqs, n_reqs,
                                        d_occupancy, n_parts, part_stride_bytes, n_namespaces, d_out, e->place_ns_scratch.p,
                                        scratch, fresh, e->place_ns_calls++, scan, e->sm_count, s, &cuda_err, &counters,
-                                       first_pdl && !fresh, changes, xch, index);
+                                       (first_pdl || built) && !fresh, changes, xch, index);
   if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
   e->r_ns_index_ok = index != lwse::kNsIndexNone;  // (a grouped call writes its own ns_first over the index's)
   e->launches += (uint64_t)launched;
@@ -1125,6 +1199,10 @@ static int place_locked(lwse_engine* e, const lwse_place_req* d_reqs, uint32_t n
   cudaStreamCaptureStatus capturing = cudaStreamCaptureStatusNone;
   const bool eager = cudaStreamIsCapturing(s, &capturing) == cudaSuccess && capturing == cudaStreamCaptureStatusNone;
   if (eager && e->place_pending) LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_place, 0));
+  {
+    const int rc = build_node_index_locked(e, s, false);
+    if (rc != LWSE_OK) return rc;
+  }
   int cuda_err = 0;
   int launched = lwse::launch_place((const lwse_node_rec*)e->nodes.p, (const uint32_t*)e->dom_first.p,
                                     (const uint32_t*)e->node_order.p, (const uint32_t*)e->node_pos.p, e->n_nodes,
@@ -1556,8 +1634,39 @@ static inline uint8_t* d_desc_of(lwse_engine* e, uint32_t slot, size_t desc_byte
   return static_cast<uint8_t*>(e->tdesc_dev.p) + slot * desc_bytes;
 }
 
+// The checks apply_patches_locked makes on a tick's segments, all of them before anything (the node-table
+// mirror included) changes.
+static int check_segments(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs) {
+  if (n_segs == 0) return LWSE_OK;
+  if (!segs || n_segs > LWSE_TICK_MAX_SEGS) return LWSE_ERR_INVALID_ARG;
+  for (uint32_t i = 0; i < n_segs; i++) {
+    const lwse_patch_seg& g = segs[i];
+    void* base;
+    uint64_t rows;
+    uint32_t rb;
+    if (!resident_table(e, g.table, &base, &rows, &rb)) return LWSE_ERR_INVALID_ARG;
+    if (g.n == 0) continue;
+    if (!g.values || (!(g.flags & LWSE_PATCH_RANGE) && !g.rows)) return LWSE_ERR_INVALID_ARG;
+    if ((g.flags & LWSE_PATCH_RANGE) && (uint64_t)g.first_row + g.n > rows) return LWSE_ERR_BAD_TABLE;
+  }
+  return LWSE_OK;
+}
+
+static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, uint32_t flags);
+
 // Enqueue one tick (nothing waits): slot = t_submitted & 1.  At most two ticks are in flight.
 static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, uint32_t flags) {
+  const int rc = tick_submit_body(e, segs, n_segs, flags);
+  if (rc != LWSE_OK && segs) {
+    // A tick that fails once its node rows are in the mirror (a CUDA error, no staging memory) may or may
+    // not have patched them on the device: the next round rebuilds the index from the device rows.
+    for (uint32_t i = 0; i < n_segs && i < LWSE_TICK_MAX_SEGS; i++)
+      if (segs[i].table == LWSE_TABLE_NODES && segs[i].n) e->node_index_stale = true;
+  }
+  return rc;
+}
+
+static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, uint32_t flags) {
   if (e->t_submitted - e->t_waited >= 2) return LWSE_ERR_NOT_READY;  // wait for the oldest tick first
   const bool in_flight = e->t_submitted != e->t_waited;
   const uint32_t slot = (uint32_t)(e->t_submitted & 1u);
@@ -1568,7 +1677,10 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
   uint32_t* cnt = static_cast<uint32_t*>(e->r_counts.p) + slot * 16u;          // and their counters
   const bool do_place = (flags & LWSE_TICK_PLACE) && e->r_place_loaded && e->rn_reqs > 0;
   const bool do_sweep = !(flags & LWSE_TICK_NO_SWEEP) && (e->rn_lws || e->rn_groups);
-  if (n_segs && !segs) return LWSE_ERR_INVALID_ARG;
+  {
+    const int crc = check_segments(e, segs, n_segs);
+    if (crc != LWSE_OK) return crc;
+  }
   // The round's form, decided before any patch is applied (it is part of a tick graph's key).  A request
   // table grouped by namespace — and not ungrouped by this tick's patches — runs the namespace kernels as
   // they are; any other table runs them through the namespace index, rebuilt when the namespace column
@@ -1589,6 +1701,12 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
                                       : (ns_moves || !e->r_ns_index_ok) ? lwse::kNsIndexBuild
                                                                           : lwse::kNsIndexReuse;
   const bool scan_form = (flags & LWSE_SWEEP_PLACE_SCAN) || g_place_form_env == 2;
+  // Node rows: the mirror decides, before anything is enqueued, whether this tick's round rebuilds the node
+  // index (also part of a tick graph's key).  A tick without a round leaves a stale index to the next one.
+  const int node_rows = node_patches_locked(e, segs, n_segs);
+  if (node_rows < 0) return node_rows;
+  const bool node_rebuild = do_place && e->node_index_stale;
+  e->last_node_info = lwse_node_info{(uint32_t)node_rows, node_rebuild ? 1u : 0u, e->n_usable, 0u};
   auto record_info = [&](bool graph) {
     lwse_tick_info& ti = e->last_tick_info;
     ti.place_form = !do_place ? LWSE_TICK_FORM_NONE
@@ -1625,14 +1743,19 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
   // the side stream, everything else by the sweep on the engine's stream — the round then starts
   // behind its own few rows (read in place over PCIe: no copy-engine launch) while the copy engine
   // still moves the pod patches, and is mostly done when the sweep needs the SMs.  Identity-row
-  // patches move occupancy counts, which the round reads: with those in the tick it forks behind
-  // the main scatter.  ONE publish kernel behind the join copies all change lists out.
+  // patches move occupancy counts and node-row patches change the nodes, both of which the round
+  // reads: with either in the tick it forks behind the main scatter.  ONE publish kernel behind the
+  // join copies all change lists out.
   constexpr uint32_t kSideTables = 1u << LWSE_TABLE_PLACE_REQS;
   bool has_ident = false, has_side = false;
   for (uint32_t i = 0; i < n_segs; i++) {
     if (segs[i].n && segs[i].table == LWSE_TABLE_POD_IDENT) has_ident = true;
     if (segs[i].n && segs[i].table == LWSE_TABLE_PLACE_REQS) has_side = true;
   }
+  // (a round also forks behind the engine's stream when an earlier tick without a round patched tables there
+  // that no round has been ordered behind yet: its node rows and occupancy counters may still be in flight)
+  const bool prior_unforked = do_place && e->main_unforked;
+  const bool fork_behind_main = has_ident || node_rows > 0 || prior_unforked;
   bool wrote = false, wrote_side = false;
   size_t stage_used = 0;
   int rc = LWSE_OK;
@@ -1644,7 +1767,8 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
   //                engine works; then the scatter and the sweep behind the copy
   //   1            the round's launches first, then copy + scatter + sweep (segments in the arena only)
   //   2            copy + scatter, the round, the sweep
-  // With identity patches the round forks behind the main scatter (it reads the occupancy counters).
+  // With identity or node patches the round forks behind the main scatter (it reads the occupancy
+  // counters and the node rows).
   bool all_in_place = true;  // no segment needs the staging buffer
   for (uint32_t i = 0; i < n_segs; i++) {
     if (!segs[i].n || (segs[i].flags & LWSE_PATCH_RANGE)) continue;
@@ -1654,7 +1778,7 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
     if (!resident_table(e, segs[i].table, &tb, &trows, &rb)) return LWSE_ERR_INVALID_ARG;
     if (!rows_in_place(e, segs[i]) || !values_in_place(e, segs[i], rb)) all_in_place = false;
   }
-  int order = has_ident ? 2 : e->tick_order;
+  int order = fork_behind_main ? 2 : e->tick_order;
   if (order == 1 && !all_in_place) order = 0;  // (the two calls share the staging buffer: main part first)
   if (in_flight) {
     // a tick is still running.  Its DMA may still read the staging buffer: segments outside the arena
@@ -1674,7 +1798,7 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
     return apply_patches_locked(e, segs, n_segs, &wrote, ~kSideTables, s, 0, &stage_used, 0, defer ? &main_plan : nullptr);
   };
   auto apply_side = [&]() -> int {
-    if (has_ident && wrote && (has_side || do_place)) {
+    if (fork_behind_main && (wrote || prior_unforked) && (has_side || do_place)) {
       LWSE_CUDA(e, cudaEventRecord(e->ev_fork, s));
       LWSE_CUDA(e, cudaStreamWaitEvent(ps, e->ev_fork, 0));
     }
@@ -1787,7 +1911,8 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
     const uint32_t key = (has_patches ? 1u : 0u) | (do_sweep ? 8u : 0u) | (do_place ? 16u : 0u) |
                          ((flags & LWSE_SWEEP_GANG) ? 32u : 0u) | ((flags & LWSE_SWEEP_PLACE_SCAN) ? 64u : 0u) | (slot << 8) |
                          (shared_occ ? 512u : 0u) | ((shared_occ && (flags & LWSE_EXCHANGE_LAGGED)) ? 1024u : 0u) |
-                         (indexed ? 2048u : 0u) | (ns_index == lwse::kNsIndexBuild ? 4096u : 0u);
+                         (indexed ? 2048u : 0u) | (ns_index == lwse::kNsIndexBuild ? 4096u : 0u) |
+                         (node_rows > 0 ? 8192u : 0u) | (node_rebuild ? 16384u : 0u);
     lwse_engine::TickGraph& tg = e->tick_graphs[key];
     bool replay = !tg.failed && tg.seen >= 1;  // the first tick of a shape runs eagerly: every buffer settles
     tg.seen++;
@@ -1862,6 +1987,7 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
           tg.failed = true;
           replay = false;
           pl[0] = pl[1] = pl[2] = lwse::PublishListHost{};
+          e->node_index_stale = e->node_index_stale || node_rebuild;  // (the eager run below builds it)
         } else {
           tg.place_ns = e->tick_place_ns;
           tg.rounds_ptr = e->place_rounds_ptr;
@@ -1880,6 +2006,7 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
       }
       LWSE_CUDA(e, cudaGraphLaunch(tg.exec, s));
       e->launches += tg.kernels;
+      if (node_rebuild) e->node_index_stale = false;  // (the graph's round built it)
       e->graph_ticks++;
       if (shared_occ) e->xch_step++;  // (the replayed push kernel advanced the device counter by one)
       if (!pl[0].count && do_sweep) {  // (replayed without capturing: the lists the graph's kernels append to)
@@ -1904,6 +2031,7 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
       gts.published = true;
       gts.wrote = has_patches;
       e->t_submitted++;
+      e->main_unforked = !do_place && (e->main_unforked || has_patches);
       record_info(true);
       return LWSE_OK;
     }
@@ -1944,6 +2072,7 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
   ts.published = published;
   ts.wrote = wrote || wrote_side;
   e->t_submitted++;
+  e->main_unforked = !do_place && (e->main_unforked || wrote);
   record_info(false);
   return LWSE_OK;
 }
@@ -2097,6 +2226,13 @@ LWSE_API int lwse_resident_tick_info(lwse_engine* e, lwse_tick_info* info) {
   if (!e || !info) return LWSE_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(e->mu);
   *info = e->last_tick_info;
+  return LWSE_OK;
+}
+
+LWSE_API int lwse_resident_node_info(lwse_engine* e, lwse_node_info* info) {
+  if (!e || !info) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  *info = e->last_node_info;
   return LWSE_OK;
 }
 

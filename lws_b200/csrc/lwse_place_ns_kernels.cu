@@ -8,7 +8,7 @@
 // that fit the shared memory of ONE CTA:
 //
 //   place_condense_kernel   node rows + occupancy -> sorted node words + per-domain capacity
-//                           (a warp per domain over its run of the static domain-sorted index:
+//                           (a warp per domain over its run of the domain-sorted node index:
 //                           no atomics), and the namespace index of the request table
 //                           (ns_first[v] = first request of namespace v; order violations counted).
 //   place_ns_kernel         one CTA per namespace.  The capacities and the domain index are staged
@@ -56,7 +56,7 @@ struct PlaceNsArgs {
   const lwse_place_req* reqs;  // grouped by namespace (ns non-decreasing), unless ns_rows is set
   const uint32_t* occupancy;   // nullable; n_parts blocks of n_nodes counters, part_stride_bytes apart
   lwse_place_out* out;
-  const uint32_t* dom_first;   // static index (lwse_upload_nodes)
+  const uint32_t* dom_first;   // the node index (node_index_*_kernel); dom_first[n_domains] = usable nodes
   const uint32_t* node_order;
   uint32_t* g_words;     // condensed node words in domain-sorted position, padded with zeros to whole rows of 256
   uint32_t* g_nodes2;    // the same positions: free slots (4 bits) | node index — the two-level form's level 2
@@ -69,7 +69,7 @@ struct PlaceNsArgs {
   uint32_t* ns_cursor;   // n_namespaces: fill cursors
   uint32_t* counters;    // this call's block: [0] max rounds [1] live unpinned [2] order violations [3] (request, round) scans
   uint32_t* next_counters;  // the other block, cleared for the next call
-  uint32_t n_nodes, n_usable, n_domains, n_reqs, n_namespaces;
+  uint32_t n_nodes, n_domains, n_reqs, n_namespaces;
   uint32_t n_parts;
   uint64_t part_stride_bytes;
   uint32_t word_rows;   // rows of 256 words of g_words
@@ -211,18 +211,25 @@ __global__ void __launch_bounds__(256) place_index_count_kernel(const PlaceNsArg
   }
 }
 
-// one CTA: ns_first = exclusive scan of the counts, the cursors start there, the counts go back to zero
+// one CTA: first = exclusive scan of the counts (first[n] = the total), the cursors start there, the
+// counts go back to zero.  Shared by the namespace index (per namespace) and the node index (per domain).
+struct IndexScanArgs {
+  uint32_t* count;
+  uint32_t* first;
+  uint32_t* cursor;
+  uint32_t n;
+};
 constexpr uint32_t kIndexScanThreads = 1024;
-__global__ void __launch_bounds__(kIndexScanThreads) place_index_scan_kernel(const PlaceNsArgs a) {
+__global__ void __launch_bounds__(kIndexScanThreads) place_index_scan_kernel(const IndexScanArgs a) {
   __shared__ uint32_t s_warp[32], s_carry;
   pdl_launch_dependents();
   pdl_wait_prior();
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   if (tid == 0) s_carry = 0u;
   __syncthreads();
-  for (uint32_t base = 0; base < a.n_namespaces; base += kIndexScanThreads) {
+  for (uint32_t base = 0; base < a.n; base += kIndexScanThreads) {
     const uint32_t v = base + tid;
-    const uint32_t c = v < a.n_namespaces ? __ldcg(a.ns_count + v) : 0u;
+    const uint32_t c = v < a.n ? __ldcg(a.count + v) : 0u;
     uint32_t x = c;  // inclusive scan inside the warp
 #pragma unroll
     for (uint32_t o = 1; o < 32u; o <<= 1) {
@@ -242,16 +249,16 @@ __global__ void __launch_bounds__(kIndexScanThreads) place_index_scan_kernel(con
     }
     __syncthreads();
     const uint32_t first = s_carry + (warp ? s_warp[warp - 1u] : 0u) + x - c;
-    if (v < a.n_namespaces) {
-      a.ns_first[v] = first;
-      a.ns_cursor[v] = first;
-      a.ns_count[v] = 0u;
+    if (v < a.n) {
+      a.first[v] = first;
+      a.cursor[v] = first;
+      a.count[v] = 0u;
     }
     __syncthreads();  // everybody has read s_carry and s_warp
     if (tid == kIndexScanThreads - 1u) s_carry = first + c;
     __syncthreads();
   }
-  if (tid == 0) a.ns_first[a.n_namespaces] = s_carry;
+  if (tid == 0) a.first[a.n] = s_carry;
 }
 
 __global__ void __launch_bounds__(256) place_index_fill_kernel(const PlaceNsArgs a) {
@@ -267,6 +274,97 @@ __global__ void __launch_bounds__(256) place_index_fill_kernel(const PlaceNsArgs
     pos = __shfl_sync(0xFFFFFFFFu, pos, (int)leader);
     if (v != LWSE_NONE) a.ns_rows[pos + (uint32_t)__popc(peers & ((1u << lane) - 1u))] = i;
   }
+}
+
+// --------------------------------------------------------------------------
+// the domain-sorted node index every placement form reads (lwse_upload_nodes, node-row patches)
+// --------------------------------------------------------------------------
+// dom_first[d] .. dom_first[d + 1] is the run of domain d in node_order, dom_first[n_domains] the
+// number of usable nodes (schedulable, labelled, domain_id < n_domains); node_pos is the inverse of
+// node_order, LWSE_NONE for a node no request can use.  The same count / scan / fill as the
+// namespace index: the order inside a run is arbitrary, and every form breaks node ties by row.
+struct NodeIndexArgs {
+  const lwse_node_rec* nodes;
+  uint32_t* dom_count;   // n_domains: nodes per domain (all zero between builds)
+  uint32_t* dom_cursor;  // n_domains: fill cursors
+  uint32_t* dom_first;   // n_domains + 1
+  uint32_t* node_order;
+  uint32_t* node_pos;
+  uint32_t n_nodes, n_domains;
+};
+
+__device__ __forceinline__ uint32_t index_domain_of(const NodeIndexArgs& a, uint32_t n) {
+  if (n >= a.n_nodes) return LWSE_NONE;
+  const uint4 nr = __ldcg(reinterpret_cast<const uint4*>(a.nodes + n));  // (rows a tick's scatter just patched)
+  const uint32_t flags = nr.w >> 16;
+  const bool usable = (flags & LWSE_NODE_SCHEDULABLE) && (flags & LWSE_NODE_HAS_TOPOLOGY) && nr.z < a.n_domains;
+  return usable ? nr.z : LWSE_NONE;
+}
+
+__global__ void __launch_bounds__(256) node_index_count_kernel(const NodeIndexArgs a) {
+  pdl_launch_dependents();
+  pdl_wait_prior();  // the node rows a tick's scatter patched; the previous round's readers of the index
+  const uint32_t lane = threadIdx.x & 31u, stride = gridDim.x * blockDim.x;
+  for (uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; base < a.n_nodes; base += stride) {
+    const uint32_t d = index_domain_of(a, base + lane);
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, d);
+    if (d != LWSE_NONE && lane == (uint32_t)__ffs(peers) - 1u) atomicAdd(a.dom_count + d, (uint32_t)__popc(peers));
+  }
+}
+
+__global__ void __launch_bounds__(256) node_index_fill_kernel(const NodeIndexArgs a) {
+  pdl_launch_dependents();
+  pdl_wait_prior();
+  const uint32_t lane = threadIdx.x & 31u, stride = gridDim.x * blockDim.x;
+  for (uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; base < a.n_nodes; base += stride) {
+    const uint32_t n = base + lane, d = index_domain_of(a, n);
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, d);
+    const uint32_t leader = (uint32_t)__ffs(peers) - 1u;
+    uint32_t pos = 0;
+    if (d != LWSE_NONE && lane == leader) pos = atomicAdd(a.dom_cursor + d, (uint32_t)__popc(peers));
+    pos = __shfl_sync(0xFFFFFFFFu, pos, (int)leader);
+    if (n < a.n_nodes) {
+      if (d != LWSE_NONE) {
+        pos += (uint32_t)__popc(peers & ((1u << lane) - 1u));
+        a.node_order[pos] = n;
+        a.node_pos[n] = pos;
+      } else {
+        a.node_pos[n] = LWSE_NONE;
+      }
+    }
+  }
+}
+
+size_t node_index_scratch_bytes(uint32_t n_domains) { return (size_t)n_domains * 8u + 16u; }
+
+// count -> scan -> fill on `s`.  `scratch` (node_index_scratch_bytes) must be zero before the first build;
+// every build leaves it zero again.  `pdl`: the predecessor on `s` is a kernel.  Returns kernels launched or -1.
+int launch_node_index(const lwse_node_rec* d_nodes, uint32_t n_nodes, uint32_t n_domains, uint32_t* d_dom_first,
+                      uint32_t* d_node_order, uint32_t* d_node_pos, void* d_scratch, int sm_count, cudaStream_t s,
+                      bool pdl, int* cuda_err) {
+  *cuda_err = 0;
+  NodeIndexArgs a{};
+  a.nodes = d_nodes;
+  a.dom_count = static_cast<uint32_t*>(d_scratch);
+  a.dom_cursor = a.dom_count + n_domains;
+  a.dom_first = d_dom_first;
+  a.node_order = d_node_order;
+  a.node_pos = d_node_pos;
+  a.n_nodes = n_nodes;
+  a.n_domains = n_domains;
+  uint64_t grid = ((uint64_t)n_nodes + 255) / 256;
+  if (grid < 1) grid = 1;
+  if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
+  cudaError_t e = launch_pdl(node_index_count_kernel, dim3((unsigned)grid), dim3(256), 0, s, pdl, a);
+  if (e == cudaSuccess)
+    e = launch_pdl(place_index_scan_kernel, dim3(1), dim3(kIndexScanThreads), 0, s, true,
+                   IndexScanArgs{a.dom_count, a.dom_first, a.dom_cursor, n_domains});
+  if (e == cudaSuccess) e = launch_pdl(node_index_fill_kernel, dim3((unsigned)grid), dim3(256), 0, s, true, a);
+  if (e != cudaSuccess) {
+    *cuda_err = (int)e;
+    return -1;
+  }
+  return 3;
 }
 
 // --------------------------------------------------------------------------
@@ -580,8 +678,11 @@ __global__ void LWSE_NS_BOUNDS
         } else {
           // Brute force: every (request, node) pair of the staged table.  Lexicographic arg-max of
           // (domain score, lower domain, node score, lower node) — the two-level result.
+          // (the usable-node count from the staged index, not a launch parameter: a replayed tick graph
+          // keeps its parameters while node-row patches change the count)
           uint32_t my_hi = 0, my_d = LWSE_NONE, my_lo = 0, my_n = LWSE_NONE;
-          for (uint32_t i = lane; i < a.n_usable; i += 32u) {
+          const uint32_t n_usable = s_first[a.n_domains];
+          for (uint32_t i = lane; i < n_usable; i += 32u) {
             const uint32_t w = words[i], d = w & 0x0FFFFFFFu;
             if ((w >> 28) == 0u || s_free[d] < size || s_hold[d] < key) continue;
             const uint32_t h = mix32n(key_lo ^ (d * 0x9E3779B1u)) | 1u;
@@ -739,7 +840,7 @@ enum PlaceNsIndex : uint32_t { kNsIndexNone = 0, kNsIndexReuse = 1, kNsIndexBuil
 
 // Returns kernels launched or -1.  `fresh`: the scratch was (re)allocated: zero it first.
 int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, const uint32_t* d_node_order, uint32_t n_nodes,
-                    uint32_t n_usable, uint32_t n_domains, const lwse_place_req* d_reqs, uint32_t n_reqs,
+                    uint32_t n_domains, const lwse_place_req* d_reqs, uint32_t n_reqs,
                     const uint32_t* d_occupancy, uint32_t n_parts, uint64_t part_stride_bytes, uint32_t n_namespaces,
                     lwse_place_out* d_out, void* d_scratch, size_t scratch_bytes, bool fresh, uint32_t call_index, bool scan,
                     int sm_count, cudaStream_t s, int* cuda_err, const uint32_t** d_counters_out, bool first_pdl,
@@ -785,7 +886,6 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
     a.next_counters = reinterpret_cast<uint32_t*>(base + l.counters) + ((call_index + 1u) & 1u) * 8u;
   }
   a.n_nodes = n_nodes;
-  a.n_usable = n_usable;
   a.n_domains = n_domains;
   a.n_reqs = n_reqs;
   a.n_namespaces = n_namespaces;
@@ -837,7 +937,9 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
     if (grid < 1) grid = 1;
     if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
     e = launch_pdl(place_index_count_kernel, dim3((unsigned)grid), dim3(256), 0, s, pdl, a);
-    if (e == cudaSuccess) e = launch_pdl(place_index_scan_kernel, dim3(1), dim3(kIndexScanThreads), 0, s, true, a);
+    if (e == cudaSuccess)
+      e = launch_pdl(place_index_scan_kernel, dim3(1), dim3(kIndexScanThreads), 0, s, true,
+                     IndexScanArgs{a.ns_count, a.ns_first, a.ns_cursor, n_namespaces});
     if (e == cudaSuccess) e = launch_pdl(place_index_fill_kernel, dim3((unsigned)grid), dim3(256), 0, s, true, a);
     if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
     pdl = true;

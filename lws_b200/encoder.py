@@ -109,20 +109,25 @@ def _state_column(pod_rows) -> np.ndarray:
     return col
 
 
+def encode_node(n: api.Node, topology_key: Optional[str], domains: dict) -> tuple:
+    """One node row.  ``domains``: label value → dense domain id; a new value takes the next id."""
+    flags = R.NODE_SCHEDULABLE if n.schedulable else 0
+    dom = R.NONE
+    h = 0
+    if topology_key is not None and topology_key in n.labels:
+        val = n.labels[topology_key]
+        flags |= R.NODE_HAS_TOPOLOGY
+        dom = domains.setdefault(val, len(domains))
+        h = R.hash64(val)
+    return (h, dom, min(n.capacity, 0xFFFF), flags)
+
+
 def encode_nodes(nodes: Iterable[api.Node], topology_key: Optional[str]):
     nodes = list(nodes)
     rec = R.aligned_empty(len(nodes), R.NODE_REC)
     domains: dict[str, int] = {}
     for i, n in enumerate(nodes):
-        flags = R.NODE_SCHEDULABLE if n.schedulable else 0
-        dom = R.NONE
-        h = 0
-        if topology_key is not None and topology_key in n.labels:
-            val = n.labels[topology_key]
-            flags |= R.NODE_HAS_TOPOLOGY
-            dom = domains.setdefault(val, len(domains))
-            h = R.hash64(val)
-        rec[i] = (h, dom, min(n.capacity, 0xFFFF), flags)
+        rec[i] = encode_node(n, topology_key, domains)
     values = [None] * len(domains)
     for v, d in domains.items():
         values[d] = v

@@ -42,6 +42,7 @@ SYMBOLS = {
     "lwse_resident_place_outputs": ([C.c_void_p, C.c_void_p], C.c_int),
     "lwse_resident_occupancy": ([C.c_void_p, C.c_void_p], C.c_int),
     "lwse_resident_tick_info": ([C.c_void_p, C.c_void_p], C.c_int),
+    "lwse_resident_node_info": ([C.c_void_p, C.POINTER(R.NodeInfo)], C.c_int),
     "lwse_place_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
         C.c_int,
@@ -280,7 +281,7 @@ class Engine:
         self._chg = None
 
     _DT = {R.TABLE_LWS: R.LWS_REC, R.TABLE_GROUPS: R.GROUP_REC, R.TABLE_POD_STATE: R.POD_STATE,
-           R.TABLE_POD_IDENT: R.POD_IDENT, R.TABLE_PLACE_REQS: R.PLACE_REQ}
+           R.TABLE_POD_IDENT: R.POD_IDENT, R.TABLE_PLACE_REQS: R.PLACE_REQ, R.TABLE_NODES: R.NODE_REC}
 
     # ----------------------------------------------------------- resident tick
     def resident_arena(self, min_bytes: int = 0) -> np.ndarray:
@@ -373,6 +374,14 @@ class Engine:
         w = (C.c_uint32 * 4)()
         self._check(lib().lwse_resident_tick_info(self._h, w))
         return {"form": self.TICK_FORMS[w[0]], "indexed": bool(w[1]), "index_built": bool(w[2]), "graph": bool(w[3])}
+
+    def resident_node_info(self) -> dict:
+        """What the node-row patches of the most recently submitted tick did: ``rows_patched``,
+        ``index_built`` (its placement round rebuilt the domain-sorted node index first: a patch changed
+        whether a node is usable, or a usable node's domain) and ``n_usable`` (usable nodes after it)."""
+        info = R.NodeInfo()
+        self._check(lib().lwse_resident_node_info(self._h, C.byref(info)))
+        return {"rows_patched": info.rows_patched, "index_built": bool(info.index_built), "n_usable": info.n_usable}
 
     def resident_patch(self, which: int, rows, values):
         """Overwrite rows of a resident table (rows: uint32 indices, values: packed rows)."""

@@ -17,9 +17,17 @@ watch stream, so that a reconcile pass is ``lwse_resident_tick(patches)`` instea
   their set (separate informers do not order events between each other) are cached and encoded
   with it.  ``DELETED`` zeroes the object's LWS, group and pod rows (node occupancy stays exact)
   and makes its request rows inert; its rows are free again from the next ``flush()``;
-* an object that outgrows its slots moves to free rows; when the spare LWS rows, slot rows or
-  namespace ids run out ``needs_reload`` is set and the caller re-encodes everything
-  (``lwse_resident_load``), which lays objects out in (namespace, name) order again.
+* Node ``ADDED`` takes a vacant node row (freed by an earlier deletion, from the next ``flush()``
+  on, otherwise from the ``node_spare`` tail) and a new topology value the next spare domain id;
+  ``MODIFIED`` re-encodes the row in place; ``DELETED`` zeroes it (no request can use a zero row).
+  Domain ids are not reused before a reload.  Added and deleted nodes change which row a node name
+  means, so every object with a pod bound to that name is re-encoded in the same flush: its pods
+  become scheduled on the new row, or unscheduled / NODE_NOT_FOUND, and occupancy stays exact.
+  The node rows go out as ``TABLE_NODES`` patches;
+* an object that outgrows its slots moves to free rows; when the spare LWS rows, slot rows,
+  namespace ids, node rows or domain ids run out ``needs_reload`` is set and the caller re-encodes
+  everything (``lwse_resident_load`` / ``lwse_upload_nodes``), which lays objects out in
+  (namespace, name) order again.
 
 Rows that no object references (slack, vacant rows) are never read for a result: group rows are
 reached through ``lws.group_base/count``, pod rows through ``groups.pod_base/count``; unused
@@ -100,17 +108,29 @@ class IncrementalEncoder:
     """Resident tables + the slice of the informer cache they were encoded from."""
 
     def __init__(self, items: list, cluster: encoder.Cluster, topology_key: Optional[str] = None,
-                 namespaces: Optional[dict] = None, spare: float = 0.25):
+                 namespaces: Optional[dict] = None, spare: float = 0.25, node_spare: int = 0):
+        """``node_spare``: node rows and domain ids kept free for nodes and topology values that appear
+        later (0: the node table is exactly ``encoder.encode_nodes`` of the cluster's nodes)."""
         self.topology_key = topology_key
-        self.nodes = list(cluster.nodes)
-        self._encoded_nodes = encoder.encode_nodes(self.nodes, topology_key)
-        self.node_rec, self.domain_values, self.node_index = self._encoded_nodes
+        self.nodes = {n.name: n for n in cluster.nodes}  # node name → Node
+        rec, self.domain_values, self.node_index = encoder.encode_nodes(cluster.nodes, topology_key)
+        self.node_rec = R.aligned_empty(len(rec) + node_spare, R.NODE_REC)
+        self.node_rec[: len(rec)] = rec
+        self._encoded_nodes = (self.node_rec, self.domain_values, self.node_index)  # (updated in place)
+        self.n_domains = len(self.domain_values) + node_spare  # domain capacity: what upload_nodes takes
+        self._domain_ids = {v: d for d, v in enumerate(self.domain_values)}
+        self._node_end = len(rec)     # node rows below this one are in use or vacated
+        self._free_nodes: list = []   # vacated node rows
+        self._node_dirty: set = set()  # node rows written since the last flush
+        self._node_resident = self.node_rec.copy()
+        self._on_node: dict[str, dict] = {}  # node name → {object key: pods bound to that name}
         self.ns_ids = dict(namespaces or {})  # namespace name → dense id (exclusivity scope)
         self.items: dict[tuple, encoder.LwsItem] = {(it.lws.namespace, it.lws.name): it for it in items}
         self.pods: dict[tuple, dict] = {}  # (ns, set name) → {pod name: Pod}; also for sets not (yet) known
         self.sts: dict[tuple, dict] = {}   # (ns, set name) → {sts name: StatefulSet}  (the leader sts lives in the item)
         for p in cluster.pods:
             self.pods.setdefault((p.namespace, p.labels.get(api.SetNameLabelKey)), {})[p.name] = p
+            self._bind(p, 1)
         for s in cluster.statefulsets:
             self.sts.setdefault((s.namespace, s.labels.get(api.SetNameLabelKey)), {})[s.name] = s
         self.needs_reload = False
@@ -149,6 +169,20 @@ class IncrementalEncoder:
         self.n_namespaces = max(1, last_ns + 1, len(self.ns_ids)) + max(4, int(len(self.ns_ids) * spare))
 
     # ------------------------------------------------------------------ helpers
+    def _bind(self, pod: api.Pod, d: int):
+        """Count (d = 1) or forget (d = -1) the pod in the node-name → objects map."""
+        if pod.nodeName == "":
+            return
+        objs = self._on_node.setdefault(pod.nodeName, {})
+        key = self._set_key(pod)
+        n = objs.get(key, 0) + d
+        if n > 0:
+            objs[key] = n
+        else:
+            objs.pop(key, None)
+            if not objs:
+                del self._on_node[pod.nodeName]
+
     def _ns_id(self, namespace: str) -> int:
         return self.ns_ids.setdefault(namespace, len(self.ns_ids))
 
@@ -171,7 +205,7 @@ class IncrementalEncoder:
     def _encode_object(self, key) -> encoder.LwsTables:
         it = self.items[key]
         cl = encoder.Cluster(pods=list(self.pods.get(key, {}).values()),
-                             statefulsets=list(self.sts.get(key, {}).values()), nodes=self.nodes)
+                             statefulsets=list(self.sts.get(key, {}).values()))  # (the node table: _encoded_nodes)
         return encoder.encode_lws([it], cl, self.topology_key, encoded_nodes=self._encoded_nodes)
 
     def _object_requests(self, key, t: encoder.LwsTables, sl: Slots) -> np.ndarray:
@@ -313,10 +347,14 @@ class IncrementalEncoder:
         known (yet, or any more) are only cached."""
         key = self._set_key(pod)
         bucket = self.pods.setdefault(key, {})
+        old = bucket.get(pod.name)
+        if old is not None:
+            self._bind(old, -1)
         if kind == "DELETED":
             bucket.pop(pod.name, None)
         else:
             bucket[pod.name] = pod
+            self._bind(pod, 1)
         if key in self.items:
             self.dirty.add(key)
 
@@ -355,10 +393,59 @@ class IncrementalEncoder:
         self.items[key] = item
         self.dirty.add(key)
 
+    def node_event(self, kind: str, node: api.Node):
+        """ADDED | MODIFIED | DELETED of a Node.  A node's row changes at once (the objects re-encoded in
+        this flush see the new table); the rows go out with the next ``flush()``.  MODIFIED keeps the
+        row, and with it every object's rows: the device reads capacity, cordon and domain from the row."""
+        row = self.node_index.get(node.name)
+        if kind == "DELETED":
+            if row is None:
+                return
+            del self.node_index[node.name]
+            self.nodes.pop(node.name, None)
+            self.node_rec[row] = np.zeros(1, R.NODE_REC)
+            self._node_dirty.add(row)
+            self._freed.append((self._free_nodes, row, 1))
+            self._touch_bound(node.name)
+            return
+        val = node.labels.get(self.topology_key) if self.topology_key is not None else None
+        if val is not None and val not in self._domain_ids and len(self._domain_ids) >= self.n_domains:
+            self.needs_reload = True  # no spare domain id
+            return
+        if row is None:
+            row = _take(self._free_nodes, 1)
+            if row is None and self._node_end < len(self.node_rec):
+                row, self._node_end = self._node_end, self._node_end + 1
+            if row is None:
+                self.needs_reload = True  # no spare node row
+                return
+            self.node_index[node.name] = row
+            self._touch_bound(node.name)
+        self.nodes[node.name] = node
+        n_dom = len(self._domain_ids)
+        self.node_rec[row] = encoder.encode_node(node, self.topology_key, self._domain_ids)
+        if len(self._domain_ids) > n_dom:
+            self.domain_values.append(val)
+        self._node_dirty.add(row)
+
+    def _touch_bound(self, node_name: str):
+        """Objects with a pod bound to `node_name` are re-encoded in the next flush."""
+        for key in self._on_node.get(node_name, {}):
+            if key in self.items:
+                self.dirty.add(key)
+
     def flush(self) -> Patches:
         """Re-encode the dirty objects → the patch segments of one ``lwse_resident_tick``."""
         patches = Patches()
         patches._pending = {}
+        if self._node_dirty:
+            rows = np.array(sorted(self._node_dirty), dtype=np.int64)
+            a = self.node_rec[rows].view(np.uint8).reshape(len(rows), -1)
+            b = self._node_resident[rows].view(np.uint8).reshape(len(rows), -1)
+            changed = rows[(a != b).any(axis=1)]
+            self._node_resident[changed] = self.node_rec[changed]
+            patches.add(R.TABLE_NODES, changed.tolist(), self.node_rec[changed])
+            self._node_dirty.clear()
         for key in sorted(self._deleted):
             self._vacate(self.slots.pop(key), self._ns_id(key[0]), patches, whole=True)
         self._deleted.clear()
@@ -395,6 +482,10 @@ class IncrementalEncoder:
 
     def lws_row(self, namespace: str, name: str) -> int:
         return self.slots[(namespace, name)].lws_row
+
+    def node_row(self, name: str) -> Optional[int]:
+        """The node-table row of a node, or None for a node the table does not hold."""
+        return self.node_index.get(name)
 
     def object_of_lws_row(self, row: int) -> Optional[tuple]:
         """(namespace, name) of the object an LWS result row belongs to, or None for a vacant row."""

@@ -313,7 +313,7 @@ class Changes(C.Structure):
     ]
 
 
-TABLE_LWS, TABLE_GROUPS, TABLE_POD_STATE, TABLE_POD_IDENT, TABLE_PLACE_REQS = 0, 1, 2, 3, 4
+TABLE_LWS, TABLE_GROUPS, TABLE_POD_STATE, TABLE_POD_IDENT, TABLE_PLACE_REQS, TABLE_NODES = 0, 1, 2, 3, 4, 5
 PATCH_RANGE = 1 << 0
 TICK_MAX_SEGS = 8
 TICK_PLACE = 1 << 8
@@ -347,6 +347,17 @@ class Tick(C.Structure):
         ("place_out", C.c_void_p),
         ("n_place", C.c_uint32),
         ("place_rounds", C.c_uint32),
+    ]
+
+
+class NodeInfo(C.Structure):
+    """lwse_node_info: what the node-row patches of the last submitted tick did."""
+
+    _fields_ = [
+        ("rows_patched", C.c_uint32),
+        ("index_built", C.c_uint32),
+        ("n_usable", C.c_uint32),
+        ("reserved", C.c_uint32),
     ]
 
 
