@@ -117,6 +117,28 @@ func (e *Engine) Place(reqs *C.lwse_place_req, n uint32, occupancy *C.uint32_t, 
 // SweepDs advances every DisaggregatedSet by one reconcile.
 func (e *Engine) SweepDs(t *C.lwse_ds_tables) error { return e.check(C.lwse_sweep_ds_host(e.h, t)) }
 
+// DsResidentLoad makes the three DS input tables resident (spare rows included; the next DsTick
+// lists every DS).  It never waits for the LeaderWorkerSet ticks in flight.
+func (e *Engine) DsResidentLoad(t *C.lwse_ds_tables) error { return e.check(C.lwse_ds_resident_load(e.h, t)) }
+
+// DsTick applies the DS row patches of one pass of the DS work queue, sweeps every DS and returns
+// the DS rows whose decisions changed.  ch.ds_out / role_out / revrole_out are the full output
+// tables in engine-owned pinned memory (valid until the next DS call): read a listed DS's rows at its
+// role_base / rev_base.
+func (e *Engine) DsTick(segs []C.lwse_patch_seg, ch *C.lwse_ds_changes) ([]uint32, error) {
+	var p *C.lwse_patch_seg
+	if len(segs) > 0 {
+		p = &segs[0]
+	}
+	if err := e.check(C.lwse_ds_resident_tick(e.h, p, C.uint32_t(len(segs)), ch)); err != nil {
+		return nil, err
+	}
+	if ch.n_changed == 0 {
+		return nil, nil
+	}
+	return unsafe.Slice((*uint32)(unsafe.Pointer(ch.ds_rows)), int(ch.n_changed)), nil
+}
+
 // GroupKeys computes SHA-1 digests (20 bytes each) of n strings laid out CSR-style.
 func (e *Engine) GroupKeys(bytes *C.uint8_t, offsets *C.uint32_t, n uint32, digests *C.uint8_t) error {
 	return e.check(C.lwse_group_keys_host(e.h, bytes, offsets, C.uint32_t(n), digests))

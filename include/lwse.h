@@ -30,6 +30,8 @@
  *                      executor.go:199-302 (planner state / config / stability),
  *                      :330-398 (scaleDownOld), disaggregatedset_controller.go:
  *                      203-236 (cleanup predicate), service_manager.go:57-89
+ *   lwse_ds_resident_* the same arithmetic over resident DS tables, fed by DS and child-LWS
+ *                      watch events (disaggregatedset_controller.go:55-126, :273)
  *   lwse_group_keys_*  pkg/webhooks/pod_webhook.go:180-182 + pkg/utils/utils.go:39-43
  *                      (SHA-1 group / subgroup keys)
  *   lwse_subgroup_keys_*  pkg/webhooks/pod_webhook.go:249-255 (getSubGroupIndex) + :130,:151
@@ -373,13 +375,16 @@ typedef enum lwse_table {
   LWSE_TABLE_POD_STATE = 2, /* lwse_pod_state  */
   LWSE_TABLE_POD_IDENT = 3, /* lwse_pod_ident  */
   LWSE_TABLE_PLACE_REQS = 4, /* lwse_place_req (lwse_resident_place_load)  */
-  LWSE_TABLE_NODES = 5        /* lwse_node_rec: the table of the last lwse_upload_nodes.  Rows must be
+  LWSE_TABLE_NODES = 5,       /* lwse_node_rec: the table of the last lwse_upload_nodes.  Rows must be
                                  < its n_nodes: patches never change the table's size, so the caller
                                  reserves spare rows (flags = 0: no request can use them) at upload.
                                  A patched row means what an uploaded row means: a node is usable iff
                                  SCHEDULABLE, HAS_TOPOLOGY and domain_id < n_domains.  Multi-rank
                                  ticks (LWSE_TICK_SHARED_OCCUPANCY): every rank applies the same node
                                  patches in the same tick.                                      */
+  LWSE_TABLE_DS = 6,          /* lwse_ds_rec, lwse_ds_role_rec, lwse_ds_revrole_rec: the resident DS   */
+  LWSE_TABLE_DS_ROLES = 7,    /* tables (lwse_ds_resident_load).  Only lwse_ds_resident_tick takes     */
+  LWSE_TABLE_DS_REVROLES = 8  /* them; lwse_resident_patch / _tick reject them as any unknown table  */
 } lwse_table;
 
 /* Result rows that differ from the previous resident sweep (all rows after a load).
@@ -745,6 +750,49 @@ typedef struct lwse_ds_tables {
 
 LWSE_API int lwse_sweep_ds_host(lwse_engine* e, const lwse_ds_tables* host_tables);
 LWSE_API int lwse_sweep_ds_device(lwse_engine* e, const lwse_ds_tables* dev_tables, void* stream);
+
+/* ---- resident DS tables and the DS tick ---------------------------------------------------
+ * The DisaggregatedSet reconciler is a controller of its own (disaggregatedset_controller.go:55-126,
+ * its watches :273): DS objects and their child LeaderWorkerSets in, no pods.  Its tables stay
+ * resident like the LeaderWorkerSet tables, with their own tick: watch events in as row patches of
+ * the three tables below, the DS rows whose decisions changed out.  Replaces, per reconcile pass,
+ * the List of child LWS and the planner / executor arithmetic of every DS
+ * (disaggregatedset_controller.go:95-112,137-186,203-236; executor.go:85-124,199-398; planner.go:61-352).
+ *
+ * Both calls run on a DS stream of their own and never wait for, drain or drop the LeaderWorkerSet
+ * ticks in flight (the exception to the rule that every other lwse_resident_* call drains first);
+ * they touch neither the tick graphs nor the patch arena.  A load may allocate device and pinned
+ * memory (which waits for the device as cudaMalloc does, without dropping any tick's results). */
+/* (tables LWSE_TABLE_DS, LWSE_TABLE_DS_ROLES, LWSE_TABLE_DS_REVROLES: see lwse_table) */
+
+/* The outputs of a DS tick: views of engine-owned pinned memory, valid until the next
+ * lwse_ds_resident_* call.  ds_out / role_out / revrole_out are the FULL output tables, kept
+ * current: the rows of a listed DS are rewritten by the tick, every other DS's rows still hold its
+ * (unchanged) results.  A caller reads a changed DS's role and revision-role results in place, at
+ * that DS's role_base and rev_base. */
+typedef struct lwse_ds_changes {
+  const uint32_t* ds_rows;               /* [n_changed] DS rows whose decisions changed; order unspecified */
+  uint32_t n_changed;
+  uint32_t reserved;
+  const lwse_ds_out* ds_out;             /* [n_ds]       */
+  const lwse_ds_role_out* role_out;      /* [n_roles]    */
+  const lwse_ds_revrole_out* revrole_out;/* [n_revroles] */
+} lwse_ds_changes;
+
+/* Copy the three input tables of `host` to the device; they stay resident, and earlier DS results
+ * are forgotten (the next tick lists every DS).  Output pointers in `host` are ignored.  Table sizes
+ * are fixed from here on: the caller reserves spare rows (a zeroed DS row is a vacant DS). */
+LWSE_API int lwse_ds_resident_load(lwse_engine* e, const lwse_ds_tables* host);
+/* One DS reconcile pass: apply the patch segments (tables LWSE_TABLE_DS*; LWSE_PATCH_RANGE allowed;
+ * rows / values anywhere in host memory, at most LWSE_TICK_MAX_SEGS segments), sweep every DS over
+ * the resident tables, and report the DS whose lwse_ds_out row, role_out rows or revrole_out rows
+ * differ from the previous tick, plus every DS whose own lwse_ds_rec row was patched in this tick
+ * (a DS moved to other rows could otherwise compare equal to what those rows held).  Returns once
+ * the results are in pinned memory (it spins on a sequence word; no stream synchronize).
+ * LWSE_ERR_NOT_READY before lwse_ds_resident_load; LWSE_ERR_INVALID_ARG for NULL pointers, an
+ * unknown table, or a row at or beyond its table's size.  A failed call changes no table and no
+ * output. */
+LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, lwse_ds_changes* out);
 
 /* ------------------------------------------------------------------------- */
 /* Group / subgroup keys (SHA-1) and subgroup indices                        */

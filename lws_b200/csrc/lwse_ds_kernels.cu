@@ -161,7 +161,77 @@ __device__ bool compute_next_step(int n, const int* initial_old, const int* cur_
   return false;
 }
 
-__global__ void __launch_bounds__(128) ds_sweep_kernel(const lwse_ds_tables t) {
+// The resident DS tick (lwse_ds_resident_tick): t's outputs are this tick's output set; the
+// previous tick's results are in the other set (the sweep uses revrole_out as scratch inside
+// scaleDownOld, so it cannot be compared in place).
+struct DsTickArgs {
+  const lwse_ds_out* prev_ds_out;
+  const lwse_ds_role_out* prev_role_out;
+  const lwse_ds_revrole_out* prev_revrole_out;
+  lwse_ds_out* m_ds_out;  // pinned, mapped mirrors of the full output tables
+  lwse_ds_role_out* m_role_out;
+  lwse_ds_revrole_out* m_revrole_out;
+  uint8_t* marks;      // DS rows the tick's scatter patched (cleared here)
+  uint32_t* rows;      // pinned, mapped: the changed DS rows
+  uint32_t* count;     // device: rows appended so far (reset by the publishing CTA)
+  uint32_t* ticket;    // device: CTAs done (reset by the publishing CTA)
+  uint32_t* host_words;  // pinned, mapped: [0] changed rows, [1] sequence word
+  uint32_t seq;
+  uint32_t all;        // first tick after a load: every DS is listed
+};
+
+// After the sweep of DS d: list it when its ds_out row, a role_out row or a revrole_out row of its
+// ranges differs from the previous tick, when the scatter patched its own row, or on the first tick;
+// a listed DS's rows go to the pinned mirrors.  A BAD_TABLE row's ranges are not read.  The
+// kernel runs this in a second pass over the same rows (one thread owns the same DS in both), so
+// that nothing of it is live across the sweep's registers.
+__device__ __forceinline__ void ds_tick_diff(const lwse_ds_tables& t, const DsTickArgs& a, uint32_t d) {
+  const uint4 h0 = __ldg(reinterpret_cast<const uint4*>(t.ds + d) + 0);
+  const uint4 h1 = __ldg(reinterpret_cast<const uint4*>(t.ds + d) + 1);
+  const uint32_t role_base = h0.z, n = h0.w, rev_base = h1.y, nrr = (h1.z + 1u) * h0.w;
+  const uint8_t mark = a.marks[d];
+  if (mark) a.marks[d] = 0;
+  bool changed = a.all || mark;
+  const uint4 cur = *reinterpret_cast<const uint4*>(t.ds_out + d);
+  const bool bad = cur.x & LWSE_DOUT_BAD_TABLE;
+  if (!changed) {
+    const uint4 prev = __ldg(reinterpret_cast<const uint4*>(a.prev_ds_out + d));
+    changed = cur.x != prev.x || cur.y != prev.y || cur.z != prev.z || cur.w != prev.w;
+  }
+  const uint2* ro = reinterpret_cast<const uint2*>(t.role_out + role_base);
+  const uint2* pro = reinterpret_cast<const uint2*>(a.prev_role_out + role_base);
+  const int* rro = t.revrole_out + rev_base;
+  const int* prro = a.prev_revrole_out + rev_base;
+  if (!bad) {
+    for (uint32_t i = 0; i < n && !changed; i++) {
+      const uint2 x = ro[i], y = __ldg(pro + i);
+      changed = x.x != y.x || x.y != y.y;
+    }
+    for (uint32_t i = 0; i < nrr && !changed; i++) changed = rro[i] != __ldg(prro + i);
+  }
+  if (!changed) return;
+  *reinterpret_cast<uint4*>(a.m_ds_out + d) = cur;
+  if (!bad) {
+    uint2* mro = reinterpret_cast<uint2*>(a.m_role_out + role_base);
+    for (uint32_t i = 0; i < n; i++) mro[i] = ro[i];
+    int* mrro = a.m_revrole_out + rev_base;
+    for (uint32_t i = 0; i < nrr; i++) mrro[i] = rro[i];
+  }
+  // warp-aggregated append: one atomic per warp and call site
+  const unsigned m = __activemask();
+  const unsigned lane = threadIdx.x & 31u;
+  const int leader = __ffs(m) - 1;
+  uint32_t base = 0;
+  if ((int)lane == leader) base = atomicAdd(a.count, (uint32_t)__popc(m));
+  base = __shfl_sync(m, base, leader);
+  a.rows[base + __popc(m & ((1u << lane) - 1u))] = d;
+}
+
+// kTick = false: the stateless sweep (lwse_sweep_ds_*), `a` unused; its code is the same as before the
+// tick form existed.  kTick = true: the resident tick — diff, mirrors, change list, and the publish of
+// the count and sequence word by the last CTA (one system-scope release, as publish_lists_kernel).
+template <bool kTick>
+__global__ void __launch_bounds__(128) ds_sweep_kernel(const lwse_ds_tables t, const DsTickArgs a) {
   for (uint32_t d = blockIdx.x * blockDim.x + threadIdx.x; d < t.n_ds; d += gridDim.x * blockDim.x) {
     const uint4 h0 = ldg_stream(reinterpret_cast<const uint4*>(t.ds + d) + 0);
     const uint4 h1 = ldg_stream(reinterpret_cast<const uint4*>(t.ds + d) + 1);
@@ -312,6 +382,25 @@ __global__ void __launch_bounds__(128) ds_sweep_kernel(const lwse_ds_tables t) {
     }
     stg_stream(t.ds_out + d, make_uint4(oflags, drained, ready_revs, 0));
   }
+  if constexpr (kTick) {
+    for (uint32_t d = blockIdx.x * blockDim.x + threadIdx.x; d < t.n_ds; d += gridDim.x * blockDim.x) ds_tick_diff(t, a, d);
+    // the ticket orders every CTA's stores (bar.sync, then a gpu-scope release) before the last
+    // CTA's acquire; its system-scope release of the sequence word covers them all
+    __shared__ uint32_t s_last;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      uint32_t tk;
+      asm volatile("atom.add.acq_rel.gpu.global.u32 %0, [%1], 1;" : "=r"(tk) : "l"(a.ticket) : "memory");
+      s_last = tk == gridDim.x - 1u ? 1u : 0u;
+      if (s_last) {
+        volatile uint32_t* hw = a.host_words;
+        hw[0] = __ldcg(a.count);
+        *a.count = 0u;
+        *a.ticket = 0u;
+        asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(a.host_words + 1), "r"(a.seq) : "memory");
+      }
+    }
+  }
 }
 
 int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s, int* cuda_err) {
@@ -319,7 +408,38 @@ int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s, int* 
   if (t->n_ds == 0) return 0;
   const uint32_t want = (t->n_ds + 127u) / 128u;
   const uint32_t cap = (uint32_t)sm_count * 16u;
-  ds_sweep_kernel<<<want < cap ? want : cap, 128, 0, s>>>(*t);
+  ds_sweep_kernel<false><<<want < cap ? want : cap, 128, 0, s>>>(*t, DsTickArgs{});
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    *cuda_err = (int)e;
+    return -1;
+  }
+  return 1;
+}
+
+struct DsTickHost {  // (lwse_engine.cu)
+  const lwse_ds_out* prev_ds_out;
+  const lwse_ds_role_out* prev_role_out;
+  const lwse_ds_revrole_out* prev_revrole_out;
+  lwse_ds_out* m_ds_out;
+  lwse_ds_role_out* m_role_out;
+  lwse_ds_revrole_out* m_revrole_out;
+  uint8_t* marks;
+  uint32_t* rows;
+  uint32_t* counters;  // [0] count, [1] ticket
+  uint32_t* host_words;
+  uint32_t seq;
+  bool all;
+};
+
+int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  if (t->n_ds == 0) return 0;
+  const uint32_t want = (t->n_ds + 127u) / 128u;
+  const uint32_t cap = (uint32_t)sm_count * 16u;
+  const DsTickArgs a{h->prev_ds_out, h->prev_role_out, h->prev_revrole_out, h->m_ds_out, h->m_role_out, h->m_revrole_out,
+                     h->marks, h->rows, h->counters, h->counters + 1, h->host_words, h->seq, h->all ? 1u : 0u};
+  ds_sweep_kernel<true><<<want < cap ? want : cap, 128, 0, s>>>(*t, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     *cuda_err = (int)e;

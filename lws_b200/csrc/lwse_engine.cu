@@ -103,6 +103,21 @@ int launch_place_diff(const lwse_place_out* d_cur, lwse_place_out* d_prev, uint3
                       lwse_place_out* d_outs, uint32_t capacity, uint32_t* d_count, cudaStream_t s, int* cuda_err);
 // lwse_ds_kernels.cu
 int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s, int* cuda_err);
+struct DsTickHost {
+  const lwse_ds_out* prev_ds_out;
+  const lwse_ds_role_out* prev_role_out;
+  const lwse_ds_revrole_out* prev_revrole_out;
+  lwse_ds_out* m_ds_out;
+  lwse_ds_role_out* m_role_out;
+  lwse_ds_revrole_out* m_revrole_out;
+  uint8_t* marks;
+  uint32_t* rows;
+  uint32_t* counters;
+  uint32_t* host_words;
+  uint32_t seq;
+  bool all;
+};
+int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s, int* cuda_err);
 // lwse_sha1_kernels.cu
 int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,
                 int sm_count, cudaStream_t s, int* cuda_err);
@@ -275,6 +290,19 @@ struct lwse_engine {
   const uint32_t* place_counters = nullptr;  // device: counters / phase stamps of the last placement call
   const uint32_t* place_unpinned = nullptr;  // device: its unpinned-request count
   DevBuf ds, ds_roles, ds_revroles, ds_out, ds_role_out, ds_revrole_out;
+  // resident DS tables (lwse_ds_resident_*): their own stream, never ordered with the LWS ticks
+  cudaStream_t ds_stream = nullptr;
+  DevBuf rd_ds, rd_roles, rd_revroles;
+  DevBuf rd_out[2], rd_role_out[2], rd_revrole_out[2];  // output sets, alternating by tick parity
+  DevBuf rd_marks, rd_ones;          // DS rows the tick's scatter patched / a column of ones the scatter copies there
+  DevBuf rd_counters;                // [0] changed rows, [1] CTA ticket
+  PinBuf rd_pin;                     // [words | changed rows | ds_out | role_out | revrole_out] mirrors
+  size_t rd_off[4] = {};             // offsets of rows / ds_out / role_out / revrole_out in rd_pin
+  PinBuf rd_stage;                   // a tick's segments, staged for one H2D copy
+  DevBuf rd_stage_dev;
+  uint32_t rdn_ds = 0, rdn_roles = 0, rdn_revroles = 0;
+  uint32_t rd_seq = 0, rd_parity = 0;
+  bool rd_loaded = false, rd_all = false;
   DevBuf sha_bytes, sha_offsets, sha_digests, sha_ints;
   uint32_t* h_rounds = nullptr;  // pinned
   // peer exchange of the multi-GPU placement step (lwse_exchange_*)
@@ -486,9 +514,13 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->ds_role_out, &e->ds_revrole_out, &e->sha_bytes, &e->sha_offsets, &e->sha_digests, &e->sha_ints,
                       &e->r_lws, &e->r_groups, &e->r_pst, &e->r_pid, &e->r_lws_out, &e->r_group_out, &e->r_scan,
                       &e->r_counts, &e->r_occ, &e->r_preq, &e->r_pout, &e->r_pout_prev, &e->h_counts_dev, &e->place_ns_scratch,
-                      &e->arena_mirror, &e->stage_mirror, &e->chg_dev, &e->tdesc_dev};
+                      &e->arena_mirror, &e->stage_mirror, &e->chg_dev, &e->tdesc_dev,
+                      &e->rd_ds, &e->rd_roles, &e->rd_revroles, &e->rd_out[0], &e->rd_out[1], &e->rd_role_out[0],
+                      &e->rd_role_out[1], &e->rd_revrole_out[0], &e->rd_revrole_out[1], &e->rd_marks, &e->rd_ones,
+                      &e->rd_counters, &e->rd_stage_dev};
+    if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
     for (DevBuf* b : bufs) b->release();
-    PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc};
+    PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc, &e->rd_pin, &e->rd_stage};
     for (PinBuf* b : pins) b->release();
     if (e->ev_place) cudaEventDestroy(e->ev_place);
     if (e->h_rounds) cudaFreeHost(e->h_rounds);
@@ -503,6 +535,7 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
     if (e->ev_done) cudaEventDestroy(e->ev_done);
     if (e->ev_mid) cudaEventDestroy(e->ev_mid);
     if (e->pub_stream) cudaStreamDestroy(e->pub_stream);
+    if (e->ds_stream) cudaStreamDestroy(e->ds_stream);
     cudaStreamDestroy(e->side_stream);
     cudaStreamDestroy(e->stream);
   }
@@ -2297,6 +2330,185 @@ LWSE_API int lwse_sweep_ds_host(lwse_engine* e, const lwse_ds_tables* h) {
   if (o_ro) LWSE_CUDA(e, cudaMemcpyAsync(h->role_out, e->ds_role_out.p, o_ro, cudaMemcpyDeviceToHost, s));
   if (o_rr) LWSE_CUDA(e, cudaMemcpyAsync(h->revrole_out, e->ds_revrole_out.p, o_rr, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
+  return LWSE_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Resident DS tables and the DS tick
+// ---------------------------------------------------------------------------
+// Neither call touches the LeaderWorkerSet ticks in flight: everything runs on ds_stream, and the
+// only waits are on that stream (and on the DS tick's own sequence word).
+LWSE_API int lwse_ds_resident_load(lwse_engine* e, const lwse_ds_tables* h) {
+  if (!e || !h) return LWSE_ERR_INVALID_ARG;
+  if ((h->n_ds && !h->ds) || (h->n_roles && !h->roles) || (h->n_revroles && !h->revroles)) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  DeviceGuard guard(e->device);
+  if (!e->ds_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->ds_stream, cudaStreamNonBlocking));
+  cudaStream_t s = e->ds_stream;
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  e->rd_loaded = false;  // (until every copy below succeeded)
+  const size_t b_ds = (size_t)h->n_ds * sizeof(lwse_ds_rec), b_ro = (size_t)h->n_roles * sizeof(lwse_ds_role_rec),
+               b_rr = (size_t)h->n_revroles * sizeof(lwse_ds_revrole_rec);
+  const size_t o_ds = (size_t)h->n_ds * sizeof(lwse_ds_out), o_ro = (size_t)h->n_roles * sizeof(lwse_ds_role_out),
+               o_rr = (size_t)h->n_revroles * sizeof(lwse_ds_revrole_out);
+  LWSE_CUDA(e, e->rd_ds.reserve(b_ds + 16));
+  LWSE_CUDA(e, e->rd_roles.reserve(b_ro + 16));
+  LWSE_CUDA(e, e->rd_revroles.reserve(b_rr + 16));
+  for (int k = 0; k < 2; k++) {
+    LWSE_CUDA(e, e->rd_out[k].reserve(o_ds + 16));
+    LWSE_CUDA(e, e->rd_role_out[k].reserve(o_ro + 16));
+    LWSE_CUDA(e, e->rd_revrole_out[k].reserve(o_rr + 16));
+  }
+  LWSE_CUDA(e, e->rd_marks.reserve((size_t)h->n_ds + 16));
+  LWSE_CUDA(e, e->rd_ones.reserve((size_t)h->n_ds + 16));
+  LWSE_CUDA(e, e->rd_counters.reserve(64));
+  e->rd_off[0] = 256;                                     // [0] changed rows, [1] sequence word
+  e->rd_off[1] = e->rd_off[0] + align256((size_t)h->n_ds * 4 + 16);
+  e->rd_off[2] = e->rd_off[1] + align256(o_ds + 16);
+  e->rd_off[3] = e->rd_off[2] + align256(o_ro + 16);
+  LWSE_CUDA(e, e->rd_pin.reserve(e->rd_off[3] + align256(o_rr + 16)));
+  if (b_ds) LWSE_CUDA(e, cudaMemcpyAsync(e->rd_ds.p, h->ds, b_ds, cudaMemcpyHostToDevice, s));
+  if (b_ro) LWSE_CUDA(e, cudaMemcpyAsync(e->rd_roles.p, h->roles, b_ro, cudaMemcpyHostToDevice, s));
+  if (b_rr) LWSE_CUDA(e, cudaMemcpyAsync(e->rd_revroles.p, h->revroles, b_rr, cudaMemcpyHostToDevice, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->rd_marks.p, 0, (size_t)h->n_ds + 16, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->rd_ones.p, 1, (size_t)h->n_ds + 16, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->rd_counters.p, 0, 64, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  e->rdn_ds = h->n_ds;
+  e->rdn_roles = h->n_roles;
+  e->rdn_revroles = h->n_revroles;
+  e->rd_parity = 0;
+  e->rd_all = true;  // earlier results are forgotten: the first tick lists every DS
+  e->rd_loaded = true;
+  return LWSE_OK;
+}
+
+static bool ds_resident_table(const lwse_engine* e, uint32_t which, void** base, uint32_t* rows, uint32_t* row_bytes) {
+  switch (which) {
+    case LWSE_TABLE_DS: *base = e->rd_ds.p; *rows = e->rdn_ds; *row_bytes = sizeof(lwse_ds_rec); return true;
+    case LWSE_TABLE_DS_ROLES: *base = e->rd_roles.p; *rows = e->rdn_roles; *row_bytes = sizeof(lwse_ds_role_rec); return true;
+    case LWSE_TABLE_DS_REVROLES:
+      *base = e->rd_revroles.p; *rows = e->rdn_revroles; *row_bytes = sizeof(lwse_ds_revrole_rec); return true;
+    default: return false;
+  }
+}
+
+LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, lwse_ds_changes* out) {
+  if (!e || !out || (n_segs && !segs) || n_segs > LWSE_TICK_MAX_SEGS) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->rd_loaded) return LWSE_ERR_NOT_READY;
+  // every check before anything changes: a rejected tick leaves tables and outputs as they were
+  size_t need = 0;
+  for (uint32_t i = 0; i < n_segs; i++) {
+    const lwse_patch_seg& g = segs[i];
+    void* base;
+    uint32_t rows, rb;
+    if (!ds_resident_table(e, g.table, &base, &rows, &rb)) return LWSE_ERR_INVALID_ARG;
+    if (g.n == 0) continue;
+    if (!g.values) return LWSE_ERR_INVALID_ARG;
+    if (g.flags & LWSE_PATCH_RANGE) {
+      if ((uint64_t)g.first_row + g.n > rows) return LWSE_ERR_INVALID_ARG;
+    } else {
+      if (!g.rows) return LWSE_ERR_INVALID_ARG;
+      for (uint32_t k = 0; k < g.n; k++)
+        if (g.rows[k] >= rows) return LWSE_ERR_INVALID_ARG;
+      need += align256((size_t)g.n * 4);
+    }
+    need += align256((size_t)g.n * rb);
+  }
+  DeviceGuard guard(e->device);
+  cudaStream_t s = e->ds_stream;
+  if (need > e->rd_stage.cap || need > e->rd_stage_dev.cap) {  // (the previous DS tick is complete: nothing reads them)
+    LWSE_CUDA(e, e->rd_stage.reserve(need));
+    LWSE_CUDA(e, e->rd_stage_dev.reserve(e->rd_stage.cap));
+  }
+  // stage every segment, then one H2D copy; range segments go on from the device copy, scattered
+  // ones through scatter_rows_kernel, and every patched DS row is marked (the scatter copies a 1 there)
+  lwse::ScatterSegHost sc[2 * LWSE_TICK_MAX_SEGS];
+  int n_sc = 0;
+  struct RangeCopy { void* dst; const void* src; size_t bytes; uint32_t ds_first, ds_n; } rc[LWSE_TICK_MAX_SEGS];
+  int n_rc = 0;
+  size_t cursor = 0;
+  uint8_t* const hs = static_cast<uint8_t*>(e->rd_stage.h);
+  uint8_t* const ds_dev = static_cast<uint8_t*>(e->rd_stage_dev.p);
+  for (uint32_t i = 0; i < n_segs; i++) {
+    const lwse_patch_seg& g = segs[i];
+    if (g.n == 0) continue;
+    void* base;
+    uint32_t rows, rb;
+    ds_resident_table(e, g.table, &base, &rows, &rb);
+    const bool is_ds = g.table == LWSE_TABLE_DS;
+    if (g.flags & LWSE_PATCH_RANGE) {
+      memcpy(hs + cursor, g.values, (size_t)g.n * rb);
+      rc[n_rc++] = RangeCopy{static_cast<uint8_t*>(base) + (size_t)g.first_row * rb, ds_dev + cursor, (size_t)g.n * rb,
+                             g.first_row, is_ds ? g.n : 0u};
+      cursor += align256((size_t)g.n * rb);
+      continue;
+    }
+    memcpy(hs + cursor, g.rows, (size_t)g.n * 4);
+    const uint32_t* d_rows = reinterpret_cast<const uint32_t*>(ds_dev + cursor);
+    cursor += align256((size_t)g.n * 4);
+    memcpy(hs + cursor, g.values, (size_t)g.n * rb);
+    const void* d_vals = ds_dev + cursor;
+    cursor += align256((size_t)g.n * rb);
+    sc[n_sc++] = lwse::ScatterSegHost{base, rows, d_rows, d_vals, g.n, rb, false};
+    if (is_ds) sc[n_sc++] = lwse::ScatterSegHost{e->rd_marks.p, rows, d_rows, e->rd_ones.p, g.n, 1u, false};
+  }
+  int cuda_err = 0;
+  if (cursor) LWSE_CUDA(e, cudaMemcpyAsync(ds_dev, hs, cursor, cudaMemcpyHostToDevice, s));
+  for (int k = 0; k < n_rc; k++) {
+    LWSE_CUDA(e, cudaMemcpyAsync(rc[k].dst, rc[k].src, rc[k].bytes, cudaMemcpyDeviceToDevice, s));
+    if (rc[k].ds_n) LWSE_CUDA(e, cudaMemsetAsync(static_cast<uint8_t*>(e->rd_marks.p) + rc[k].ds_first, 1, rc[k].ds_n, s));
+  }
+  for (int k = 0; k < n_sc; k += 8) {  // (one launch takes up to eight segments)
+    const int launched = lwse::launch_scatter(sc + k, n_sc - k < 8 ? n_sc - k : 8, nullptr, 0, s, false, &cuda_err);
+    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+    e->launches += (uint64_t)launched;
+  }
+  const uint32_t p = e->rd_parity, q = p ^ 1u;
+  uint8_t* const pin_h = static_cast<uint8_t*>(e->rd_pin.h);
+  uint8_t* const pin_d = static_cast<uint8_t*>(e->rd_pin.d);
+  volatile uint32_t* hw = reinterpret_cast<volatile uint32_t*>(pin_h);
+  uint32_t n_changed = 0;
+  if (e->rdn_ds) {
+    lwse_ds_tables t{};
+    t.ds = (const lwse_ds_rec*)e->rd_ds.p;
+    t.n_ds = e->rdn_ds;
+    t.roles = (const lwse_ds_role_rec*)e->rd_roles.p;
+    t.n_roles = e->rdn_roles;
+    t.revroles = (const lwse_ds_revrole_rec*)e->rd_revroles.p;
+    t.n_revroles = e->rdn_revroles;
+    t.ds_out = (lwse_ds_out*)e->rd_out[p].p;
+    t.role_out = (lwse_ds_role_out*)e->rd_role_out[p].p;
+    t.revrole_out = (lwse_ds_revrole_out*)e->rd_revrole_out[p].p;
+    const uint32_t seq = ++e->rd_seq == 0 ? ++e->rd_seq : e->rd_seq;  // (0 is the word's initial value)
+    const lwse::DsTickHost a{(const lwse_ds_out*)e->rd_out[q].p, (const lwse_ds_role_out*)e->rd_role_out[q].p,
+                             (const lwse_ds_revrole_out*)e->rd_revrole_out[q].p,
+                             reinterpret_cast<lwse_ds_out*>(pin_d + e->rd_off[1]),
+                             reinterpret_cast<lwse_ds_role_out*>(pin_d + e->rd_off[2]),
+                             reinterpret_cast<lwse_ds_revrole_out*>(pin_d + e->rd_off[3]),
+                             (uint8_t*)e->rd_marks.p, reinterpret_cast<uint32_t*>(pin_d + e->rd_off[0]),
+                             (uint32_t*)e->rd_counters.p, reinterpret_cast<uint32_t*>(pin_d), seq, e->rd_all};
+    const int launched = lwse::launch_ds_tick(&t, &a, e->sm_count, s, &cuda_err);
+    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+    e->launches += (uint64_t)launched;
+    cudaError_t werr = cudaSuccess;
+    if (!wait_word(hw + 1, seq, s, &werr)) {
+      const cudaError_t a2 = cudaStreamSynchronize(s);
+      return fail_cuda(e, werr != cudaSuccess ? werr : a2 != cudaSuccess ? a2 : cudaErrorUnknown);
+    }
+    n_changed = hw[0];
+    e->rd_parity = q;
+    e->rd_all = false;
+  } else if (n_sc || n_rc) {
+    LWSE_CUDA(e, cudaStreamSynchronize(s));
+  }
+  out->ds_rows = reinterpret_cast<const uint32_t*>(pin_h + e->rd_off[0]);
+  out->n_changed = n_changed;
+  out->reserved = 0;
+  out->ds_out = reinterpret_cast<const lwse_ds_out*>(pin_h + e->rd_off[1]);
+  out->role_out = reinterpret_cast<const lwse_ds_role_out*>(pin_h + e->rd_off[2]);
+  out->revrole_out = reinterpret_cast<const lwse_ds_revrole_out*>(pin_h + e->rd_off[3]);
   return LWSE_OK;
 }
 

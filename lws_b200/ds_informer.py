@@ -1,0 +1,264 @@
+"""DisaggregatedSet and child-LeaderWorkerSet watch events → DS row patches.
+
+The reference's DS reconciler is a controller of its own: it watches DisaggregatedSets and the
+LeaderWorkerSets they own (disaggregatedset_controller.go:273) and never reads pods.  The engine
+keeps its three DS tables resident (``Engine.ds_resident_load``) and runs a DS tick of their own
+(``Engine.ds_resident_tick``); this module keeps those tables current from the two watch streams:
+
+* the tables are laid out in **slots**: every DS owns one DS row, a range of role rows and a range
+  of revision-role rows, each with some slack, so an event never moves another DS;
+* an event marks its DS dirty; ``flush()`` re-encodes just the dirty DS with the very function the
+  full encoder uses (``encoder.encode_ds([item])``), rebases the rows to the DS's slot ranges and
+  emits only the rows that differ from the resident ones.  Encoding one DS on its own gives it
+  creation ranks of its own (1, 2, … over its children's timestamps) instead of ranks over every
+  DS: the kernel only compares the ranks of one DS with each other (the newest-first revision
+  order of scaleDownOld, executor.go:283-302), so its results are the same;
+* child LeaderWorkerSets are keyed by (namespace, DS name, role, revision); children seen before
+  their DS (separate informers do not order events between each other) are cached and encoded
+  with it;
+* a DS ``ADDED`` takes a vacant DS row and ranges (first fit among freed ranges, otherwise from the
+  spare tail); a DS whose role or revision-role rows outgrow their range moves that range to a
+  first-fit one, and the old range is zeroed; ``DELETED`` zeroes the DS row and both ranges (a zero
+  DS row is a vacant DS).  Freed rows are reused from the next ``flush()`` on;
+* ``needs_reload`` is set only when spare DS rows, role rows or revision-role rows run out: the
+  caller then encodes everything again and calls ``Engine.ds_resident_load``.
+
+``object_of_ds_row``, ``role_names`` and ``old_revisions`` map a changed DS row, and its
+``revrole_out`` entries (old revision r, role i at ``rev_base + r * n_roles + i``; the target
+revision after the old ones), back to the objects.
+"""
+from __future__ import annotations
+
+from dataclasses import dataclass
+from typing import Optional
+
+import numpy as np
+
+from . import api, encoder
+from . import records as R
+from .informer import Patches, _give, _slack, _take
+
+
+@dataclass
+class DsSlots:
+    ds_row: int
+    role_base: int
+    role_cap: int
+    rev_base: int
+    rev_cap: int
+
+
+class DsIncrementalEncoder:
+    """Resident DS tables + the DS objects and child LeaderWorkerSets they were encoded from."""
+
+    def __init__(self, items: list, spare: float = 0.25):
+        """``items``: ``encoder.DsItem`` (their children included).  ``spare``: share of spare rows of
+        each table (DS rows, role rows, revision-role rows) kept for later objects and growth."""
+        self.items: dict[tuple, tuple] = {}      # (ns, name) → (DisaggregatedSet, target revision)
+        self.children: dict[tuple, dict] = {}    # (ns, DS name) → {(role, revision): ChildLWS}, List order
+        for it in items:
+            key = (it.ds.namespace, it.ds.name)
+            self.items[key] = (it.ds, it.revision)
+            bucket = self.children.setdefault(key, {})
+            for c in it.children:
+                bucket[(c.role, c.revision)] = c
+        fresh = {k: self._encode(k) for k in self.items}
+        self.slots: dict[tuple, DsSlots] = {}
+        r = v = 0
+        for i, k in enumerate(self.items):
+            rc, vc = _slack(len(fresh[k].roles)), _slack(len(fresh[k].revroles))
+            self.slots[k] = DsSlots(i, r, rc, v, vc)
+            r, v = r + rc, v + vc
+        n = len(self.items)
+        self.ds = R.aligned_empty(n + max(4, int(n * spare)), R.DS_REC)
+        self.roles = R.aligned_empty(r + max(16, int(r * spare)), R.DS_ROLE_REC)
+        self.revroles = R.aligned_empty(v + max(32, int(v * spare)), R.DS_REVROLE_REC)
+        self.n_ds, self.role_end, self.rev_end = n, r, v
+        self._free_ds: list = []
+        self._free_roles: list = []
+        self._free_revroles: list = []
+        self._freed: list = []  # (free list, base, length) released by this flush: free from the next one
+        self._ds_key: dict[int, tuple] = {}
+        self._meta: dict[int, tuple] = {}  # DS row → (role names, old revisions)
+        self.needs_reload = False
+        self.dirty: set = set()
+        self._deleted: set = set()
+        for k in self.items:
+            self._ds_key[self.slots[k].ds_row] = k
+            self._write(k, fresh[k], None)
+
+    # ------------------------------------------------------------------ helpers
+    def item(self, key) -> encoder.DsItem:
+        """The ``encoder.DsItem`` of a DS as the encoder holds it now."""
+        ds, rev = self.items[key]
+        return encoder.DsItem(ds, rev, list(self.children.get(key, {}).values()))
+
+    def _encode(self, key) -> encoder.DsTablesHost:
+        return encoder.encode_ds([self.item(key)])
+
+    @staticmethod
+    def _put(patches: Optional[Patches], table_id: int, table: np.ndarray, base: int, fresh_rows: np.ndarray):
+        """Write rows [base, base + n) of a table; with `patches`, emit the rows that changed."""
+        n = len(fresh_rows)
+        if n == 0:
+            return
+        cur = table[base: base + n]
+        if patches is None:
+            cur[:] = fresh_rows
+            return
+        a = np.ascontiguousarray(cur).view(np.uint8).reshape(n, -1)
+        b = np.ascontiguousarray(fresh_rows).view(np.uint8).reshape(n, -1)
+        diff = np.flatnonzero((a != b).any(axis=1))
+        if len(diff):
+            vals = R.aligned_empty(len(diff), table.dtype)
+            vals[:] = fresh_rows[diff]
+            cur[diff] = vals
+            rows, chunks = patches._pending.setdefault(table_id, ([], []))
+            rows.extend((diff + base).tolist())
+            chunks.append(vals)
+
+    def _alloc(self, free: list, end_attr: str, table: np.ndarray, cap: int) -> Optional[int]:
+        base = _take(free, cap)
+        end = getattr(self, end_attr)
+        if base is None and end + cap <= len(table):
+            base = end
+            setattr(self, end_attr, end + cap)
+        return base
+
+    def _write(self, key, t: encoder.DsTablesHost, patches: Optional[Patches]):
+        """Place the DS's fresh rows into its slots (moving an outgrown range); with `patches`, emit
+        the rows that changed."""
+        sl = self.slots[key]
+        n, nrr = len(t.roles), len(t.revroles)
+        if n > sl.role_cap:
+            cap = _slack(n)
+            base = self._alloc(self._free_roles, "role_end", self.roles, cap)
+            if base is None:
+                self.needs_reload = True
+                return
+            self._put(patches, R.TABLE_DS_ROLES, self.roles, sl.role_base, R.aligned_empty(sl.role_cap, R.DS_ROLE_REC))
+            self._freed.append((self._free_roles, sl.role_base, sl.role_cap))
+            sl.role_base, sl.role_cap = base, cap
+        if nrr > sl.rev_cap:
+            cap = _slack(nrr)
+            base = self._alloc(self._free_revroles, "rev_end", self.revroles, cap)
+            if base is None:
+                self.needs_reload = True
+                return
+            self._put(patches, R.TABLE_DS_REVROLES, self.revroles, sl.rev_base,
+                      R.aligned_empty(sl.rev_cap, R.DS_REVROLE_REC))
+            self._freed.append((self._free_revroles, sl.rev_base, sl.rev_cap))
+            sl.rev_base, sl.rev_cap = base, cap
+        row = t.ds.copy()
+        row["role_base"], row["rev_base"] = sl.role_base, sl.rev_base
+        # whole slot ranges: rows a shrinking DS no longer references go back to zero
+        roles = R.aligned_empty(sl.role_cap, R.DS_ROLE_REC)
+        roles[:n] = t.roles
+        revroles = R.aligned_empty(sl.rev_cap, R.DS_REVROLE_REC)
+        revroles[:nrr] = t.revroles
+        self._put(patches, R.TABLE_DS, self.ds, sl.ds_row, row)
+        self._put(patches, R.TABLE_DS_ROLES, self.roles, sl.role_base, roles)
+        self._put(patches, R.TABLE_DS_REVROLES, self.revroles, sl.rev_base, revroles)
+        self._meta[sl.ds_row] = (list(t.role_names[0]), list(t.old_revisions[0]))
+
+    def _create(self, key, t: encoder.DsTablesHost) -> bool:
+        """Slots for a new DS: a vacant DS row and free ranges.  False: nothing left, reload."""
+        row = _take(self._free_ds, 1)
+        if row is None and self.n_ds < len(self.ds):
+            row, self.n_ds = self.n_ds, self.n_ds + 1
+        if row is None:
+            return False
+        rc, vc = _slack(len(t.roles)), _slack(len(t.revroles))
+        r = self._alloc(self._free_roles, "role_end", self.roles, rc)
+        v = self._alloc(self._free_revroles, "rev_end", self.revroles, vc) if r is not None else None
+        if r is None or v is None:
+            self._freed.append((self._free_ds, row, 1))
+            if r is not None:
+                self._freed.append((self._free_roles, r, rc))
+            return False
+        self.slots[key] = DsSlots(row, r, rc, v, vc)
+        self._ds_key[row] = key
+        return True
+
+    def _vacate(self, key, patches: Patches):
+        """A deleted DS: its DS row and both ranges back to zero, free from the next flush."""
+        sl = self.slots.pop(key)
+        self._put(patches, R.TABLE_DS, self.ds, sl.ds_row, R.aligned_empty(1, R.DS_REC))
+        self._put(patches, R.TABLE_DS_ROLES, self.roles, sl.role_base, R.aligned_empty(sl.role_cap, R.DS_ROLE_REC))
+        self._put(patches, R.TABLE_DS_REVROLES, self.revroles, sl.rev_base, R.aligned_empty(sl.rev_cap, R.DS_REVROLE_REC))
+        self._ds_key.pop(sl.ds_row, None)
+        self._meta.pop(sl.ds_row, None)
+        self._freed += [(self._free_ds, sl.ds_row, 1), (self._free_roles, sl.role_base, sl.role_cap),
+                        (self._free_revroles, sl.rev_base, sl.rev_cap)]
+
+    # ------------------------------------------------------------------- events
+    def ds_event(self, kind: str, ds: api.DisaggregatedSet, revision: str):
+        """ADDED | MODIFIED | DELETED of a DisaggregatedSet; ``revision`` is its target revision
+        (ComputeRevision(spec.roles), as in ``encoder.DsItem``)."""
+        key = (ds.namespace, ds.name)
+        if kind == "DELETED":
+            if self.items.pop(key, None) is not None:
+                self.dirty.discard(key)
+                if key in self.slots:
+                    self._deleted.add(key)
+            return
+        self.items[key] = (ds, revision)
+        self._deleted.discard(key)  # (deleted and added again in one flush: it keeps its rows)
+        self.dirty.add(key)
+
+    def child_event(self, kind: str, namespace: str, ds_name: str, child: api.ChildLWS):
+        """ADDED | MODIFIED | DELETED of a LeaderWorkerSet owned by DS ``ds_name``: the child of
+        (role, revision).  Children of a DS not known (yet, or any more) are only cached."""
+        key = (namespace, ds_name)
+        bucket = self.children.setdefault(key, {})
+        if kind == "DELETED":
+            bucket.pop((child.role, child.revision), None)
+        else:
+            bucket[(child.role, child.revision)] = child
+        if key in self.items:
+            self.dirty.add(key)
+
+    def flush(self) -> Patches:
+        """Re-encode the dirty DS → the patch segments of one ``Engine.ds_resident_tick``."""
+        patches = Patches()
+        patches._pending = {}
+        for key in sorted(self._deleted):
+            self._vacate(key, patches)
+        self._deleted.clear()
+        for key in sorted(self.dirty):
+            t = self._encode(key)
+            if key not in self.slots and not self._create(key, t):
+                self.needs_reload = True
+                continue
+            self._write(key, t, patches)
+        self.dirty.clear()
+        for free, base, n in self._freed:  # rows given back in this flush may be patched in it: reuse from the next
+            _give(free, base, n)
+        self._freed.clear()
+        for table_id in (R.TABLE_DS, R.TABLE_DS_ROLES, R.TABLE_DS_REVROLES):
+            if table_id in patches._pending:
+                rows, chunks = patches._pending[table_id]
+                patches.add(table_id, rows, np.concatenate(chunks))
+        del patches._pending
+        return patches
+
+    # ------------------------------------------------------------------ results
+    def tables(self):
+        """(ds, roles, revroles): the whole allocation, spare rows included (what
+        ``Engine.ds_resident_load`` should take, so that new DS and moved ranges stay in range)."""
+        return self.ds, self.roles, self.revroles
+
+    def ds_row(self, namespace: str, name: str) -> int:
+        return self.slots[(namespace, name)].ds_row
+
+    def object_of_ds_row(self, row: int) -> Optional[tuple]:
+        """(namespace, name) of the DS a result row belongs to, or None for a vacant row."""
+        return self._ds_key.get(int(row))
+
+    def role_names(self, row: int) -> list:
+        """allRoleNames of the DS at `row`: spec roles, then removed roles (role_out / revrole_out order)."""
+        return self._meta[int(row)][0]
+
+    def old_revisions(self, row: int) -> list:
+        """The old revisions of the DS at `row` in revision-role row order (the target revision follows them)."""
+        return self._meta[int(row)][1]

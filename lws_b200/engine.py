@@ -83,6 +83,8 @@ SYMBOLS = {
     "lwse_exchange_status": ([C.c_void_p, C.POINTER(C.c_uint32)], C.c_int),
     "lwse_sweep_ds_host": ([C.c_void_p, C.POINTER(R.DsTables)], C.c_int),
     "lwse_sweep_ds_device": ([C.c_void_p, C.POINTER(R.DsTables), C.c_void_p], C.c_int),
+    "lwse_ds_resident_load": ([C.c_void_p, C.POINTER(R.DsTables)], C.c_int),
+    "lwse_ds_resident_tick": ([C.c_void_p, C.POINTER(R.PatchSeg), C.c_uint32, C.POINTER(R.DsChanges)], C.c_int),
     "lwse_group_keys_host": ([C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_subgroup_keys_host": (
         [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
@@ -482,6 +484,51 @@ class Engine:
             R.ptr(d_ds_out), R.ptr(d_role_out), R.ptr(d_revrole_out),
         )
         self._check(lib().lwse_sweep_ds_device(self._h, C.byref(t), stream))
+
+    # ------------------------------------------------------------ resident DS
+    _DS_DT = {R.TABLE_DS: R.DS_REC, R.TABLE_DS_ROLES: R.DS_ROLE_REC, R.TABLE_DS_REVROLES: R.DS_REVROLE_REC}
+
+    def ds_resident_load(self, ds, roles, revroles):
+        """Make the three DS input tables resident (sizes fixed until the next load; the next tick lists
+        every DS).  Never waits for the LeaderWorkerSet ticks in flight."""
+        assert ds.dtype == R.DS_REC and roles.dtype == R.DS_ROLE_REC and revroles.dtype == R.DS_REVROLE_REC
+        t = R.DsTables(R.ptr(ds) if len(ds) else None, len(ds), R.ptr(roles) if len(roles) else None, len(roles),
+                       R.ptr(revroles) if len(revroles) else None, len(revroles), None, None, None)
+        self._check(lib().lwse_ds_resident_load(self._h, C.byref(t)))
+        self._ds_shape = (len(ds), len(roles), len(revroles))
+
+    def ds_resident_tick(self, segments=()):
+        """One DS tick: ``segments`` as for ``make_tick`` ((table, rows, values), or (table, first_row,
+        values, True) for a range) of the tables TABLE_DS / TABLE_DS_ROLES / TABLE_DS_REVROLES; rows and
+        values may live anywhere in host memory.  → dict: ``rows`` (the DS rows whose decisions changed)
+        and ``ds_out`` / ``role_out`` / ``revrole_out``, views of the FULL output tables kept current in
+        engine-owned pinned memory (valid until the next DS call)."""
+        segs = (R.PatchSeg * max(len(segments), 1))()
+        keep = []
+        for i, sg in enumerate(segments):
+            if len(sg) == 4 and sg[3]:
+                table, first, values = sg[0], sg[1], np.ascontiguousarray(sg[2])
+                segs[i] = R.PatchSeg(table, R.PATCH_RANGE, len(values), int(first), None,
+                                     R.ptr(values) if len(values) else None)
+                keep.append(values)
+            else:
+                table, rows, values = sg[0], np.ascontiguousarray(sg[1], dtype=np.uint32), np.ascontiguousarray(sg[2])
+                assert len(rows) == len(values) and values.dtype == self._DS_DT.get(table, values.dtype)
+                segs[i] = R.PatchSeg(table, 0, len(rows), 0, R.ptr(rows) if len(rows) else None,
+                                     R.ptr(values) if len(rows) else None)
+                keep.append((rows, values))
+        ch = R.DsChanges()
+        self._check(lib().lwse_ds_resident_tick(self._h, segs, len(segments), C.byref(ch)))
+        n_ds, n_roles, n_rr = self._ds_shape
+
+        def view(ptr, n, dtype):
+            if not ptr or n == 0:
+                return np.zeros(0, dtype=dtype)
+            return np.frombuffer((C.c_uint8 * (n * np.dtype(dtype).itemsize)).from_address(ptr), dtype=dtype)
+
+        return {"rows": view(ch.ds_rows, min(ch.n_changed, n_ds), np.uint32), "n_changed": ch.n_changed,
+                "ds_out": view(ch.ds_out, n_ds, R.DS_OUT), "role_out": view(ch.role_out, n_roles, R.DS_ROLE_OUT),
+                "revrole_out": view(ch.revrole_out, n_rr, R.DS_REVROLE_OUT)}
 
     # ------------------------------------------------------------- group keys
     def group_keys_host(self, strings) -> np.ndarray:

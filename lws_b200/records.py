@@ -314,6 +314,7 @@ class Changes(C.Structure):
 
 
 TABLE_LWS, TABLE_GROUPS, TABLE_POD_STATE, TABLE_POD_IDENT, TABLE_PLACE_REQS, TABLE_NODES = 0, 1, 2, 3, 4, 5
+TABLE_DS, TABLE_DS_ROLES, TABLE_DS_REVROLES = 6, 7, 8  # lwse_ds_resident_tick only
 PATCH_RANGE = 1 << 0
 TICK_MAX_SEGS = 8
 TICK_PLACE = 1 << 8
@@ -369,6 +370,19 @@ class DsTables(C.Structure):
         ("n_roles", C.c_uint32),
         ("revroles", C.c_void_p),
         ("n_revroles", C.c_uint32),
+        ("ds_out", C.c_void_p),
+        ("role_out", C.c_void_p),
+        ("revrole_out", C.c_void_p),
+    ]
+
+
+class DsChanges(C.Structure):
+    """lwse_ds_changes: the changed DS rows and the full output mirrors of a DS tick (engine-owned pinned memory)."""
+
+    _fields_ = [
+        ("ds_rows", C.c_void_p),
+        ("n_changed", C.c_uint32),
+        ("reserved", C.c_uint32),
         ("ds_out", C.c_void_p),
         ("role_out", C.c_void_p),
         ("revrole_out", C.c_void_p),
