@@ -139,6 +139,16 @@ func (e *Engine) DsTick(segs []C.lwse_patch_seg, ch *C.lwse_ds_changes) ([]uint3
 	return unsafe.Slice((*uint32)(unsafe.Pointer(ch.ds_rows)), int(ch.n_changed)), nil
 }
 
+// DsTickInfo reports how the last DsTick read ready counts: whether it ran linked (a
+// LWSE_TABLE_DS_LINKS patch since DsResidentLoad: linked revision-role rows take their child's ready
+// count from the most recently submitted LWS tick), the rows that took that value, the linked rows
+// that fell back to their own, and the LWS ticks submitted when it read them.
+func (e *Engine) DsTickInfo() (C.lwse_ds_tick_info, error) {
+	var info C.lwse_ds_tick_info
+	err := e.check(C.lwse_ds_resident_tick_info(e.h, &info))
+	return info, err
+}
+
 // GroupKeys computes SHA-1 digests (20 bytes each) of n strings laid out CSR-style.
 func (e *Engine) GroupKeys(bytes *C.uint8_t, offsets *C.uint32_t, n uint32, digests *C.uint8_t) error {
 	return e.check(C.lwse_group_keys_host(e.h, bytes, offsets, C.uint32_t(n), digests))

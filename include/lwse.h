@@ -384,7 +384,9 @@ typedef enum lwse_table {
                                  patches in the same tick.                                      */
   LWSE_TABLE_DS = 6,          /* lwse_ds_rec, lwse_ds_role_rec, lwse_ds_revrole_rec: the resident DS   */
   LWSE_TABLE_DS_ROLES = 7,    /* tables (lwse_ds_resident_load).  Only lwse_ds_resident_tick takes     */
-  LWSE_TABLE_DS_REVROLES = 8  /* them; lwse_resident_patch / _tick reject them as any unknown table  */
+  LWSE_TABLE_DS_REVROLES = 8, /* them; lwse_resident_patch / _tick reject them as any unknown table  */
+  LWSE_TABLE_DS_LINKS = 9     /* lwse_ds_link, one row per revision-role row (see lwse_ds_link); the
+                                 same rules as the three DS tables                                  */
 } lwse_table;
 
 /* Result rows that differ from the previous resident sweep (all rows after a load).
@@ -793,6 +795,58 @@ LWSE_API int lwse_ds_resident_load(lwse_engine* e, const lwse_ds_tables* host);
  * unknown table, or a row at or beyond its table's size.  A failed call changes no table and no
  * output. */
 LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, lwse_ds_changes* out);
+
+/* ---- links from revision-role rows to resident child LeaderWorkerSets ----------------------
+ * A DS's children are ordinary LeaderWorkerSets named <ds>-<revision>-<role> (GenerateName,
+ * pkg/utils/disaggregatedset/utils.go:92-94).  When a child is also resident in this engine's LWS
+ * tables, the LWS tick has already computed the status.readyReplicas the DS tick needs
+ * (updateConditions, leaderworkerset_controller.go:478-480).  A link lets the DS tick read that value
+ * on the device instead of waiting for the status write, the watch event and a revision-role patch.
+ *
+ * LWSE_TABLE_DS_LINKS has one row per revision-role row, patched only through lwse_ds_resident_tick
+ * (scattered or as ranges).  lwse_ds_resident_load sets every lws_row to LWSE_NONE (the first tick
+ * after a load can send the whole table as one range).  Only status.readyReplicas is linked:
+ * replicas and initial replicas are spec fields the DS controller writes itself.
+ *
+ * The rule.  Revision-role row r with link (L, U) uses lws_out[L].ready_replicas of the resident LWS
+ * results when ALL of these hold, and its own ready_replicas otherwise:
+ *   - row r has LWSE_RR_EXISTS;
+ *   - LWS tables are resident (lwse_resident_load) and an LWS sweep was enqueued after the load and
+ *     after every patch of LWSE_TABLE_LWS rows that came without a sweep (lwse_resident_patch, or a
+ *     tick with LWSE_TICK_NO_SWEEP): until then the results do not belong to the resident LWS rows
+ *     (after a load they are all-ones rows);
+ *   - L < n_lws of the resident LWS table;
+ *   - the resident lwse_lws_rec[L].uid_hash == U (a row the LWS encoder has since given to another
+ *     object is harmless);
+ *   - lws_out[L].flags has none of LWSE_LOUT_IRREGULAR, _BAD_TABLE, _RUP_ERROR, _STATUS_ERROR: in each
+ *     case the reference never reaches Status().Update (Reconcile returns at :159-163, or
+ *     updateConditions fails), so the value the API server holds is the row's own one.
+ * Both objects must be on one engine: a child resident on another rank stays unlinked.
+ *
+ * Which LWS results.  A DS tick that has received a link patch since its load reads the results of
+ * everything enqueued on the engine's stream when it starts: the most recently submitted LWS tick (or
+ * lwse_resident_sweep), in flight or not.  It orders itself behind that work with one event and still
+ * never waits for, drains or drops an LWS tick, nor touches the tick graphs or the patch arena.  A DS
+ * tick that never received a link patch since its load waits on nothing. */
+typedef struct lwse_ds_link { /* 16 B */
+  uint64_t lws_uid_hash;      /* uid_hash of the child LWS (as in lwse_lws_rec)                      */
+  uint32_t lws_row;           /* its row in the resident LWS table, or LWSE_NONE: not linked        */
+  uint32_t reserved;           /* 0 (a patch with another value is rejected: LWSE_ERR_INVALID_ARG)  */
+} lwse_ds_link;
+
+/* How the last successful DS tick read ready counts (read-only; nothing waits). */
+typedef struct lwse_ds_tick_info { /* 24 B */
+  uint32_t linked;            /* 1: it ran the linked sweep (a link patch since the DS load)         */
+  uint32_t rows_from_lws;     /* existing revision-role rows that took the LWS tick's ready count    */
+  uint32_t rows_fallback;     /* linked rows (lws_row != LWSE_NONE) that used their own ready count   */
+                              /* (both counts cover the revision-role rows the sweep reads: the
+                                 (n_old_revs + 1) * n_roles rows of each DS whose row is not
+                                 LWSE_DOUT_BAD_TABLE; link rows outside them are not counted) */
+  uint32_t reserved;
+  uint64_t lws_ticks;         /* LWS ticks submitted (lwse_resident_tick*, _sweep) when it read the
+                                 LWS rows; 0 for an unlinked tick                                   */
+} lwse_ds_tick_info;
+LWSE_API int lwse_ds_resident_tick_info(lwse_engine* e, lwse_ds_tick_info* info);
 
 /* ------------------------------------------------------------------------- */
 /* Group / subgroup keys (SHA-1) and subgroup indices                        */

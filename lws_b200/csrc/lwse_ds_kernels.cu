@@ -178,7 +178,37 @@ struct DsTickArgs {
   uint32_t* host_words;  // pinned, mapped: [0] changed rows, [1] sequence word
   uint32_t seq;
   uint32_t all;        // first tick after a load: every DS is listed
+  // linked tick only (kLinked): the link table and the resident LWS rows it points into
+  const lwse_ds_link* links;  // [n_revroles]
+  const lwse_lws_rec* lws;    // resident LWS table and the results of the last LWS sweep enqueued
+  const lwse_lws_out* lws_out;
+  uint32_t n_lws;             // 0: no LWS tables or no results yet (every linked row falls back)
 };
+
+// The ready count a linked revision-role row uses (lwse.h, LWSE_TABLE_DS_LINKS): the child's
+// lws_out.ready_replicas when the row exists, its link names a row < n_lws, that row still holds the
+// same object (uid_hash) and its result went through Status().Update; else the row's own value.
+// Counts rows that took the LWS value (took) and linked rows that fell back (fell).  The LWS rows
+// are written by the LWS tick's kernels on the engine's stream (ordered before this kernel by an
+// event): ld.global.cg, and no L1 allocation for gathers nothing else in the kernel re-reads.
+__device__ __forceinline__ int linked_ready(const DsTickArgs& a, uint32_t row, bool exists, int own,
+                                            uint32_t& took, uint32_t& fell) {
+  const uint4 l = ldg_stream(a.links + row);  // {uid lo, uid hi, lws_row, reserved}
+  if (l.z == LWSE_NONE) return own;
+  if (exists && l.z < a.n_lws) {
+    const uint64_t uid = __ldcg(reinterpret_cast<const unsigned long long*>(&a.lws[l.z].uid_hash));
+    if (uid == u64_of(l.x, l.y)) {
+      const uint32_t f = __ldcg(&a.lws_out[l.z].flags);
+      constexpr uint32_t kNoUpdate = LWSE_LOUT_IRREGULAR | LWSE_LOUT_BAD_TABLE | LWSE_LOUT_RUP_ERROR | LWSE_LOUT_STATUS_ERROR;
+      if (!(f & kNoUpdate)) {
+        took++;
+        return __ldcg(&a.lws_out[l.z].ready_replicas);
+      }
+    }
+  }
+  fell++;
+  return own;
+}
 
 // After the sweep of DS d: list it when its ds_out row, a role_out row or a revrole_out row of its
 // ranges differs from the previous tick, when the scatter patched its own row, or on the first tick;
@@ -230,8 +260,11 @@ __device__ __forceinline__ void ds_tick_diff(const lwse_ds_tables& t, const DsTi
 // kTick = false: the stateless sweep (lwse_sweep_ds_*), `a` unused; its code is the same as before the
 // tick form existed.  kTick = true: the resident tick — diff, mirrors, change list, and the publish of
 // the count and sequence word by the last CTA (one system-scope release, as publish_lists_kernel).
-template <bool kTick>
+// kLinked (with kTick): every revision-role row's ready count goes through linked_ready, and the two
+// row counts are published beside the changed-row count.
+template <bool kTick, bool kLinked = false>
 __global__ void __launch_bounds__(128) ds_sweep_kernel(const lwse_ds_tables t, const DsTickArgs a) {
+  uint32_t took = 0, fell = 0;
   for (uint32_t d = blockIdx.x * blockDim.x + threadIdx.x; d < t.n_ds; d += gridDim.x * blockDim.x) {
     const uint4 h0 = ldg_stream(reinterpret_cast<const uint4*>(t.ds + d) + 0);
     const uint4 h1 = ldg_stream(reinterpret_cast<const uint4*>(t.ds + d) + 1);
@@ -258,8 +291,9 @@ __global__ void __launch_bounds__(128) ds_sweep_kernel(const lwse_ds_tables t, c
     for (int r = 0; r < V; r++) {
       bool any = false, all_drained = true, ready = true;
       for (int i = 0; i < n; i++) {
-        const uint4 x = ldg_stream(rr + r * n + i);
+        uint4 x = ldg_stream(rr + r * n + i);
         const bool exists = x.w & LWSE_RR_EXISTS;
+        if constexpr (kLinked) x.z = (uint32_t)linked_ready(a, rev_base + r * n + i, exists, (int)x.z, took, fell);
         rro[r * n + i] = exists ? (int)x.x : -1;
         if (i < S && (!exists || (int)x.z < 1)) ready = false;  // service_manager.go:62-67
         if (!exists) continue;
@@ -274,8 +308,9 @@ __global__ void __launch_bounds__(128) ds_sweep_kernel(const lwse_ds_tables t, c
     }
     bool new_ready = true, stable = true;
     for (int i = 0; i < n; i++) {
-      const uint4 x = ldg_stream(rr + V * n + i);
+      uint4 x = ldg_stream(rr + V * n + i);
       const bool exists = x.w & LWSE_RR_EXISTS;
+      if constexpr (kLinked) x.z = (uint32_t)linked_ready(a, rev_base + V * n + i, exists, (int)x.z, took, fell);
       rro[V * n + i] = exists ? (int)x.x : -1;
       const uint4 rl = ldg_cached(reinterpret_cast<const uint4*>(roles + i));  // {target, surge, unavail, flags}
       const bool in_spec = rl.w & LWSE_ROLE_IN_SPEC;
@@ -384,6 +419,14 @@ __global__ void __launch_bounds__(128) ds_sweep_kernel(const lwse_ds_tables t, c
   }
   if constexpr (kTick) {
     for (uint32_t d = blockIdx.x * blockDim.x + threadIdx.x; d < t.n_ds; d += gridDim.x * blockDim.x) ds_tick_diff(t, a, d);
+    if constexpr (kLinked) {  // (every lane of the block is here: the loops above have ended)
+      took = __reduce_add_sync(0xFFFFFFFFu, took);
+      fell = __reduce_add_sync(0xFFFFFFFFu, fell);
+      if ((threadIdx.x & 31u) == 0 && (took | fell)) {
+        atomicAdd(a.count + 2, took);
+        atomicAdd(a.count + 3, fell);
+      }
+    }
     // the ticket orders every CTA's stores (bar.sync, then a gpu-scope release) before the last
     // CTA's acquire; its system-scope release of the sequence word covers them all
     __shared__ uint32_t s_last;
@@ -397,6 +440,12 @@ __global__ void __launch_bounds__(128) ds_sweep_kernel(const lwse_ds_tables t, c
         hw[0] = __ldcg(a.count);
         *a.count = 0u;
         *a.ticket = 0u;
+        if constexpr (kLinked) {  // [2] rows that took the LWS value, [3] linked rows that fell back
+          hw[2] = __ldcg(a.count + 2);
+          hw[3] = __ldcg(a.count + 3);
+          a.count[2] = 0u;
+          a.count[3] = 0u;
+        }
         asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(a.host_words + 1), "r"(a.seq) : "memory");
       }
     }
@@ -430,6 +479,10 @@ struct DsTickHost {  // (lwse_engine.cu)
   uint32_t* host_words;
   uint32_t seq;
   bool all;
+  const lwse_ds_link* links;  // non-null: the linked instance
+  const lwse_lws_rec* lws;
+  const lwse_lws_out* lws_out;
+  uint32_t n_lws;
 };
 
 int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s, int* cuda_err) {
@@ -438,8 +491,12 @@ int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, c
   const uint32_t want = (t->n_ds + 127u) / 128u;
   const uint32_t cap = (uint32_t)sm_count * 16u;
   const DsTickArgs a{h->prev_ds_out, h->prev_role_out, h->prev_revrole_out, h->m_ds_out, h->m_role_out, h->m_revrole_out,
-                     h->marks, h->rows, h->counters, h->counters + 1, h->host_words, h->seq, h->all ? 1u : 0u};
-  ds_sweep_kernel<true><<<want < cap ? want : cap, 128, 0, s>>>(*t, a);
+                     h->marks, h->rows, h->counters, h->counters + 1, h->host_words, h->seq, h->all ? 1u : 0u,
+                     h->links, h->lws, h->lws_out, h->n_lws};
+  if (h->links)
+    ds_sweep_kernel<true, true><<<want < cap ? want : cap, 128, 0, s>>>(*t, a);
+  else
+    ds_sweep_kernel<true><<<want < cap ? want : cap, 128, 0, s>>>(*t, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     *cuda_err = (int)e;

@@ -116,6 +116,10 @@ struct DsTickHost {
   uint32_t* host_words;
   uint32_t seq;
   bool all;
+  const lwse_ds_link* links;
+  const lwse_lws_rec* lws;
+  const lwse_lws_out* lws_out;
+  uint32_t n_lws;
 };
 int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s, int* cuda_err);
 // lwse_sha1_kernels.cu
@@ -303,6 +307,12 @@ struct lwse_engine {
   uint32_t rdn_ds = 0, rdn_roles = 0, rdn_revroles = 0;
   uint32_t rd_seq = 0, rd_parity = 0;
   bool rd_loaded = false, rd_all = false;
+  DevBuf rd_links;                   // LWSE_TABLE_DS_LINKS: revision-role row → resident LWS row
+  bool rd_linked = false;            // a link patch arrived since the DS load: ticks run the linked sweep
+  cudaEvent_t ev_ds_link = nullptr;  // the engine's stream at the start of a linked DS tick
+  lwse_ds_tick_info last_ds_info{};  // lwse_ds_resident_tick_info
+  bool r_swept = false;              // r_lws_out holds the results of the resident LWS rows: a sweep was enqueued
+                                     // since lwse_resident_load and since any LWS-row patch without a sweep
   DevBuf sha_bytes, sha_offsets, sha_digests, sha_ints;
   uint32_t* h_rounds = nullptr;  // pinned
   // peer exchange of the multi-GPU placement step (lwse_exchange_*)
@@ -517,7 +527,7 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->arena_mirror, &e->stage_mirror, &e->chg_dev, &e->tdesc_dev,
                       &e->rd_ds, &e->rd_roles, &e->rd_revroles, &e->rd_out[0], &e->rd_out[1], &e->rd_role_out[0],
                       &e->rd_role_out[1], &e->rd_revrole_out[0], &e->rd_revrole_out[1], &e->rd_marks, &e->rd_ones,
-                      &e->rd_counters, &e->rd_stage_dev};
+                      &e->rd_counters, &e->rd_stage_dev, &e->rd_links};
     if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
     for (DevBuf* b : bufs) b->release();
     PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc, &e->rd_pin, &e->rd_stage};
@@ -536,6 +546,7 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
     if (e->ev_mid) cudaEventDestroy(e->ev_mid);
     if (e->pub_stream) cudaStreamDestroy(e->pub_stream);
     if (e->ds_stream) cudaStreamDestroy(e->ds_stream);
+    if (e->ev_ds_link) cudaEventDestroy(e->ev_ds_link);
     cudaStreamDestroy(e->side_stream);
     cudaStreamDestroy(e->stream);
   }
@@ -818,6 +829,7 @@ LWSE_API int lwse_resident_load(lwse_engine* e, const lwse_lws_tables* h) {
     const int drc = drain_ticks_locked(e);
     if (drc != LWSE_OK) return drc;
   }
+  e->r_swept = false;  // (the output rows are all-ones until the next sweep)
   cudaStream_t s = e->stream;
   const size_t b_lws = (size_t)h->n_lws * sizeof(lwse_lws_rec), b_grp = (size_t)h->n_groups * sizeof(lwse_group_rec);
   const size_t b_pst = (size_t)h->n_pods * sizeof(lwse_pod_state), b_pid = (size_t)h->n_pods * sizeof(lwse_pod_ident);
@@ -1119,6 +1131,7 @@ LWSE_API int lwse_resident_patch(lwse_engine* e, lwse_table which, const uint32_
     const int nrc = node_patches_locked(e, &seg, 1);
     if (nrc < 0) return nrc;
   }
+  if (which == LWSE_TABLE_LWS) e->r_swept = false;  // r_lws_out no longer belongs to these LWS rows
   bool wrote = false;
   const int rc = apply_patches_locked(e, &seg, 1, &wrote);
   if (rc != LWSE_OK) {
@@ -1714,6 +1727,10 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
     const int crc = check_segments(e, segs, n_segs);
     if (crc != LWSE_OK) return crc;
   }
+  // LWS rows patched without a sweep: r_lws_out no longer belongs to them (a row reused for another
+  // object would pass the linked DS tick's uid test with the previous object's results)
+  for (uint32_t i = 0; !do_sweep && i < n_segs; i++)
+    if (segs[i].table == LWSE_TABLE_LWS && segs[i].n) e->r_swept = false;
   // The round's form, decided before any patch is applied (it is part of a tick graph's key).  A request
   // table grouped by namespace — and not ungrouped by this tick's patches — runs the namespace kernels as
   // they are; any other table runs them through the namespace index, rebuilt when the namespace column
@@ -2064,6 +2081,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
       gts.published = true;
       gts.wrote = has_patches;
       e->t_submitted++;
+      if (do_sweep) e->r_swept = true;
       e->main_unforked = !do_place && (e->main_unforked || has_patches);
       record_info(true);
       return LWSE_OK;
@@ -2105,6 +2123,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
   ts.published = published;
   ts.wrote = wrote || wrote_side;
   e->t_submitted++;
+  if (do_sweep) e->r_swept = true;
   e->main_unforked = !do_place && (e->main_unforked || wrote);
   record_info(false);
   return LWSE_OK;
@@ -2359,6 +2378,7 @@ LWSE_API int lwse_ds_resident_load(lwse_engine* e, const lwse_ds_tables* h) {
     LWSE_CUDA(e, e->rd_role_out[k].reserve(o_ro + 16));
     LWSE_CUDA(e, e->rd_revrole_out[k].reserve(o_rr + 16));
   }
+  LWSE_CUDA(e, e->rd_links.reserve((size_t)h->n_revroles * sizeof(lwse_ds_link) + 16));
   LWSE_CUDA(e, e->rd_marks.reserve((size_t)h->n_ds + 16));
   LWSE_CUDA(e, e->rd_ones.reserve((size_t)h->n_ds + 16));
   LWSE_CUDA(e, e->rd_counters.reserve(64));
@@ -2370,6 +2390,8 @@ LWSE_API int lwse_ds_resident_load(lwse_engine* e, const lwse_ds_tables* h) {
   if (b_ds) LWSE_CUDA(e, cudaMemcpyAsync(e->rd_ds.p, h->ds, b_ds, cudaMemcpyHostToDevice, s));
   if (b_ro) LWSE_CUDA(e, cudaMemcpyAsync(e->rd_roles.p, h->roles, b_ro, cudaMemcpyHostToDevice, s));
   if (b_rr) LWSE_CUDA(e, cudaMemcpyAsync(e->rd_revroles.p, h->revroles, b_rr, cudaMemcpyHostToDevice, s));
+  // every link unlinked: lws_row = LWSE_NONE (all-ones rows)
+  LWSE_CUDA(e, cudaMemsetAsync(e->rd_links.p, 0xFF, (size_t)h->n_revroles * sizeof(lwse_ds_link), s));
   LWSE_CUDA(e, cudaMemsetAsync(e->rd_marks.p, 0, (size_t)h->n_ds + 16, s));
   LWSE_CUDA(e, cudaMemsetAsync(e->rd_ones.p, 1, (size_t)h->n_ds + 16, s));
   LWSE_CUDA(e, cudaMemsetAsync(e->rd_counters.p, 0, 64, s));
@@ -2379,6 +2401,8 @@ LWSE_API int lwse_ds_resident_load(lwse_engine* e, const lwse_ds_tables* h) {
   e->rdn_revroles = h->n_revroles;
   e->rd_parity = 0;
   e->rd_all = true;  // earlier results are forgotten: the first tick lists every DS
+  e->rd_linked = false;
+  e->last_ds_info = lwse_ds_tick_info{};
   e->rd_loaded = true;
   return LWSE_OK;
 }
@@ -2389,6 +2413,8 @@ static bool ds_resident_table(const lwse_engine* e, uint32_t which, void** base,
     case LWSE_TABLE_DS_ROLES: *base = e->rd_roles.p; *rows = e->rdn_roles; *row_bytes = sizeof(lwse_ds_role_rec); return true;
     case LWSE_TABLE_DS_REVROLES:
       *base = e->rd_revroles.p; *rows = e->rdn_revroles; *row_bytes = sizeof(lwse_ds_revrole_rec); return true;
+    case LWSE_TABLE_DS_LINKS:
+      *base = e->rd_links.p; *rows = e->rdn_revroles; *row_bytes = sizeof(lwse_ds_link); return true;
     default: return false;
   }
 }
@@ -2413,6 +2439,11 @@ LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, u
       for (uint32_t k = 0; k < g.n; k++)
         if (g.rows[k] >= rows) return LWSE_ERR_INVALID_ARG;
       need += align256((size_t)g.n * 4);
+    }
+    if (g.table == LWSE_TABLE_DS_LINKS) {  // reserved words must be zero
+      const lwse_ds_link* v = static_cast<const lwse_ds_link*>(g.values);
+      for (uint32_t k = 0; k < g.n; k++)
+        if (v[k].reserved != 0) return LWSE_ERR_INVALID_ARG;
     }
     need += align256((size_t)g.n * rb);
   }
@@ -2465,6 +2496,8 @@ LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, u
     if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
     e->launches += (uint64_t)launched;
   }
+  for (uint32_t i = 0; i < n_segs; i++)
+    if (segs[i].table == LWSE_TABLE_DS_LINKS && segs[i].n) e->rd_linked = true;
   const uint32_t p = e->rd_parity, q = p ^ 1u;
   uint8_t* const pin_h = static_cast<uint8_t*>(e->rd_pin.h);
   uint8_t* const pin_d = static_cast<uint8_t*>(e->rd_pin.d);
@@ -2482,13 +2515,26 @@ LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, u
     t.role_out = (lwse_ds_role_out*)e->rd_role_out[p].p;
     t.revrole_out = (lwse_ds_revrole_out*)e->rd_revrole_out[p].p;
     const uint32_t seq = ++e->rd_seq == 0 ? ++e->rd_seq : e->rd_seq;  // (0 is the word's initial value)
+    const bool linked = e->rd_linked;
+    if (linked) {
+      // The linked sweep reads r_lws / r_lws_out, which the LWS ticks write on the engine's stream: it
+      // waits for everything enqueued there now (the most recently submitted LWS tick, in flight or
+      // not) and nothing else — no drain, no dropped results.  The engine mutex is held until this call
+      // has its results, so no later LWS tick can overwrite those rows while the DS kernel reads them.
+      if (!e->ev_ds_link) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_ds_link, cudaEventDisableTiming));
+      LWSE_CUDA(e, cudaEventRecord(e->ev_ds_link, e->stream));
+      LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_ds_link, 0));
+    }
+    const bool lws_results = e->r_loaded && e->r_swept;  // (after a load, r_lws_out is all-ones until a sweep)
     const lwse::DsTickHost a{(const lwse_ds_out*)e->rd_out[q].p, (const lwse_ds_role_out*)e->rd_role_out[q].p,
                              (const lwse_ds_revrole_out*)e->rd_revrole_out[q].p,
                              reinterpret_cast<lwse_ds_out*>(pin_d + e->rd_off[1]),
                              reinterpret_cast<lwse_ds_role_out*>(pin_d + e->rd_off[2]),
                              reinterpret_cast<lwse_ds_revrole_out*>(pin_d + e->rd_off[3]),
                              (uint8_t*)e->rd_marks.p, reinterpret_cast<uint32_t*>(pin_d + e->rd_off[0]),
-                             (uint32_t*)e->rd_counters.p, reinterpret_cast<uint32_t*>(pin_d), seq, e->rd_all};
+                             (uint32_t*)e->rd_counters.p, reinterpret_cast<uint32_t*>(pin_d), seq, e->rd_all,
+                             linked ? (const lwse_ds_link*)e->rd_links.p : nullptr, (const lwse_lws_rec*)e->r_lws.p,
+                             (const lwse_lws_out*)e->r_lws_out.p, lws_results ? e->rn_lws : 0u};
     const int launched = lwse::launch_ds_tick(&t, &a, e->sm_count, s, &cuda_err);
     if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
     e->launches += (uint64_t)launched;
@@ -2500,8 +2546,10 @@ LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, u
     n_changed = hw[0];
     e->rd_parity = q;
     e->rd_all = false;
-  } else if (n_sc || n_rc) {
-    LWSE_CUDA(e, cudaStreamSynchronize(s));
+    e->last_ds_info = linked ? lwse_ds_tick_info{1u, hw[2], hw[3], 0u, e->t_submitted} : lwse_ds_tick_info{};
+  } else {
+    if (n_sc || n_rc) LWSE_CUDA(e, cudaStreamSynchronize(s));
+    e->last_ds_info = lwse_ds_tick_info{e->rd_linked ? 1u : 0u, 0u, 0u, 0u, 0u};
   }
   out->ds_rows = reinterpret_cast<const uint32_t*>(pin_h + e->rd_off[0]);
   out->n_changed = n_changed;
@@ -2509,6 +2557,13 @@ LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, u
   out->ds_out = reinterpret_cast<const lwse_ds_out*>(pin_h + e->rd_off[1]);
   out->role_out = reinterpret_cast<const lwse_ds_role_out*>(pin_h + e->rd_off[2]);
   out->revrole_out = reinterpret_cast<const lwse_ds_revrole_out*>(pin_h + e->rd_off[3]);
+  return LWSE_OK;
+}
+
+LWSE_API int lwse_ds_resident_tick_info(lwse_engine* e, lwse_ds_tick_info* info) {
+  if (!e || !info) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  *info = e->last_ds_info;
   return LWSE_OK;
 }
 

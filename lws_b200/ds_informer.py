@@ -26,6 +26,21 @@ keeps its three DS tables resident (``Engine.ds_resident_load``) and runs a DS t
 ``object_of_ds_row``, ``role_names`` and ``old_revisions`` map a changed DS row, and its
 ``revrole_out`` entries (old revision r, role i at ``rev_base + r * n_roles + i``; the target
 revision after the old ones), back to the objects.
+
+With ``links=`` (an ``informer.IncrementalEncoder`` of the same engine's LWS tables) the encoder also
+keeps ``links``, the ``TABLE_DS_LINKS`` table beside ``revroles``: revision-role row r of a DS links to
+the resident row and uid_hash of the LeaderWorkerSet named ``<ds>-<revision>-<role>`` in the DS's
+namespace (GenerateName, pkg/utils/disaggregatedset/utils.go:92-94), or holds ``lws_row = NONE``.  The
+DS tick then reads linked children's ready counts from the LWS tick on the device (lwse.h,
+``lwse_ds_link``).  Link rows follow the revision-role ranges (moved and freed ranges go back to
+``NONE``) and are emitted only where they differ.  The engine's load sets every link to ``NONE``: send
+``links`` whole with the first DS tick after ``Engine.ds_resident_load``, as the range segment
+``(TABLE_DS_LINKS, 0, links, True)``.  After an LWS ``flush()``, ``relink(lws.moved_keys)``
+has the next ``flush()`` re-link just the DS whose children took or gave back an LWS row or changed
+uid.  When the LWS encoder is rebuilt (its ``needs_reload``, then ``resident_load``), every row and
+uid may have changed: rebuild this encoder with ``links=`` the new LWS encoder and send ``links`` whole
+again (or ``relink`` every LWS key).  Without ``links=`` no link table exists and nothing emitted
+changes.
 """
 from __future__ import annotations
 
@@ -51,9 +66,11 @@ class DsSlots:
 class DsIncrementalEncoder:
     """Resident DS tables + the DS objects and child LeaderWorkerSets they were encoded from."""
 
-    def __init__(self, items: list, spare: float = 0.25):
+    def __init__(self, items: list, spare: float = 0.25, links=None):
         """``items``: ``encoder.DsItem`` (their children included).  ``spare``: share of spare rows of
-        each table (DS rows, role rows, revision-role rows) kept for later objects and growth."""
+        each table (DS rows, role rows, revision-role rows) kept for later objects and growth.
+        ``links``: a resolver with ``lws_link(namespace, name) -> (row, uid_hash) | None`` (the LWS
+        ``informer.IncrementalEncoder``); it turns on the link table."""
         self.items: dict[tuple, tuple] = {}      # (ns, name) → (DisaggregatedSet, target revision)
         self.children: dict[tuple, dict] = {}    # (ns, DS name) → {(role, revision): ChildLWS}, List order
         for it in items:
@@ -83,6 +100,14 @@ class DsIncrementalEncoder:
         self.needs_reload = False
         self.dirty: set = set()
         self._deleted: set = set()
+        self.resolver = links
+        self.links = None
+        if links is not None:
+            self.links = R.aligned_empty(len(self.revroles), R.DS_LINK)
+            self.links["lws_row"] = R.NONE
+            self._link_names: dict[tuple, set] = {}  # DS key → the (ns, LWS name) its rows resolve
+            self._linkers: dict[tuple, set] = {}     # (ns, LWS name) → DS keys that resolve it
+            self._relink: set = set()
         for k in self.items:
             self._ds_key[self.slots[k].ds_row] = k
             self._write(k, fresh[k], None)
@@ -147,6 +172,7 @@ class DsIncrementalEncoder:
                 return
             self._put(patches, R.TABLE_DS_REVROLES, self.revroles, sl.rev_base,
                       R.aligned_empty(sl.rev_cap, R.DS_REVROLE_REC))
+            self._unlink_range(patches, sl.rev_base, sl.rev_cap)
             self._freed.append((self._free_revroles, sl.rev_base, sl.rev_cap))
             sl.rev_base, sl.rev_cap = base, cap
         row = t.ds.copy()
@@ -160,6 +186,8 @@ class DsIncrementalEncoder:
         self._put(patches, R.TABLE_DS_ROLES, self.roles, sl.role_base, roles)
         self._put(patches, R.TABLE_DS_REVROLES, self.revroles, sl.rev_base, revroles)
         self._meta[sl.ds_row] = (list(t.role_names[0]), list(t.old_revisions[0]))
+        if self.links is not None:
+            self._put(patches, R.TABLE_DS_LINKS, self.links, sl.rev_base, self._resolve(key))
 
     def _create(self, key, t: encoder.DsTablesHost) -> bool:
         """Slots for a new DS: a vacant DS row and free ranges.  False: nothing left, reload."""
@@ -186,10 +214,59 @@ class DsIncrementalEncoder:
         self._put(patches, R.TABLE_DS, self.ds, sl.ds_row, R.aligned_empty(1, R.DS_REC))
         self._put(patches, R.TABLE_DS_ROLES, self.roles, sl.role_base, R.aligned_empty(sl.role_cap, R.DS_ROLE_REC))
         self._put(patches, R.TABLE_DS_REVROLES, self.revroles, sl.rev_base, R.aligned_empty(sl.rev_cap, R.DS_REVROLE_REC))
+        self._unlink_range(patches, sl.rev_base, sl.rev_cap)
+        if self.links is not None:
+            self._index_links(key, set())
         self._ds_key.pop(sl.ds_row, None)
         self._meta.pop(sl.ds_row, None)
         self._freed += [(self._free_ds, sl.ds_row, 1), (self._free_roles, sl.role_base, sl.role_cap),
                         (self._free_revroles, sl.rev_base, sl.rev_cap)]
+
+    # -------------------------------------------------------------------- links
+    def _unlink_range(self, patches: Optional[Patches], base: int, n: int):
+        """Link rows [base, base + n) back to NONE (a moved or freed revision-role range)."""
+        if self.links is not None:
+            none = R.aligned_empty(n, R.DS_LINK)
+            none["lws_row"] = R.NONE
+            self._put(patches, R.TABLE_DS_LINKS, self.links, base, none)
+
+    def _index_links(self, key, names: set):
+        for lk in self._link_names.pop(key, set()) - names:
+            users = self._linkers.get(lk)
+            if users is not None:
+                users.discard(key)
+                if not users:
+                    del self._linkers[lk]
+        for lk in names:
+            self._linkers.setdefault(lk, set()).add(key)
+        if names:
+            self._link_names[key] = names
+
+    def _resolve(self, key) -> np.ndarray:
+        """The link rows of the DS's whole revision-role range, resolved by child name now."""
+        sl = self.slots[key]
+        names, old = self._meta[sl.ds_row]
+        out = R.aligned_empty(sl.rev_cap, R.DS_LINK)
+        out["lws_row"] = R.NONE
+        ns, ds_name = key
+        used = set()
+        for r, rev in enumerate(old + [self.items[key][1]]):
+            for i, role in enumerate(names):
+                lk = (ns, f"{ds_name}-{rev}-{role}")  # GenerateName (utils.go:92-94)
+                used.add(lk)
+                got = self.resolver.lws_link(*lk)
+                if got is not None:
+                    out["lws_row"][r * len(names) + i] = got[0]
+                    out["lws_uid_hash"][r * len(names) + i] = got[1]
+        self._index_links(key, used)
+        return out
+
+    def relink(self, lws_keys):
+        """(ns, name) of LeaderWorkerSets whose resident row was taken or given back (the LWS
+        encoder's ``moved_keys`` after its ``flush()``): the next ``flush()`` re-links the DS whose
+        revision-role rows name them."""
+        for lk in lws_keys:
+            self._relink.update(self._linkers.get(lk, ()))
 
     # ------------------------------------------------------------------- events
     def ds_event(self, kind: str, ds: api.DisaggregatedSet, revision: str):
@@ -231,11 +308,16 @@ class DsIncrementalEncoder:
                 self.needs_reload = True
                 continue
             self._write(key, t, patches)
+        if self.links is not None:
+            for key in sorted(self._relink - self.dirty):
+                if key in self.slots and key in self.items:
+                    self._put(patches, R.TABLE_DS_LINKS, self.links, self.slots[key].rev_base, self._resolve(key))
+            self._relink.clear()
         self.dirty.clear()
         for free, base, n in self._freed:  # rows given back in this flush may be patched in it: reuse from the next
             _give(free, base, n)
         self._freed.clear()
-        for table_id in (R.TABLE_DS, R.TABLE_DS_ROLES, R.TABLE_DS_REVROLES):
+        for table_id in (R.TABLE_DS, R.TABLE_DS_ROLES, R.TABLE_DS_REVROLES, R.TABLE_DS_LINKS):
             if table_id in patches._pending:
                 rows, chunks = patches._pending[table_id]
                 patches.add(table_id, rows, np.concatenate(chunks))

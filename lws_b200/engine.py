@@ -85,6 +85,7 @@ SYMBOLS = {
     "lwse_sweep_ds_device": ([C.c_void_p, C.POINTER(R.DsTables), C.c_void_p], C.c_int),
     "lwse_ds_resident_load": ([C.c_void_p, C.POINTER(R.DsTables)], C.c_int),
     "lwse_ds_resident_tick": ([C.c_void_p, C.POINTER(R.PatchSeg), C.c_uint32, C.POINTER(R.DsChanges)], C.c_int),
+    "lwse_ds_resident_tick_info": ([C.c_void_p, C.POINTER(R.DsTickInfo)], C.c_int),
     "lwse_group_keys_host": ([C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_subgroup_keys_host": (
         [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
@@ -499,10 +500,13 @@ class Engine:
 
     def ds_resident_tick(self, segments=()):
         """One DS tick: ``segments`` as for ``make_tick`` ((table, rows, values), or (table, first_row,
-        values, True) for a range) of the tables TABLE_DS / TABLE_DS_ROLES / TABLE_DS_REVROLES; rows and
-        values may live anywhere in host memory.  → dict: ``rows`` (the DS rows whose decisions changed)
-        and ``ds_out`` / ``role_out`` / ``revrole_out``, views of the FULL output tables kept current in
-        engine-owned pinned memory (valid until the next DS call)."""
+        values, True) for a range) of the tables TABLE_DS / TABLE_DS_ROLES / TABLE_DS_REVROLES /
+        TABLE_DS_LINKS; rows and values may live anywhere in host memory.  Once a link patch arrived
+        (since the DS load), linked revision-role rows read their child's ready count from the
+        resident LWS results of the most recently submitted LWS tick (lwse.h, ``lwse_ds_link``).
+        → dict: ``rows`` (the DS rows whose decisions changed) and ``ds_out`` / ``role_out`` /
+        ``revrole_out``, views of the FULL output tables kept current in engine-owned pinned memory
+        (valid until the next DS call)."""
         segs = (R.PatchSeg * max(len(segments), 1))()
         keep = []
         for i, sg in enumerate(segments):
@@ -529,6 +533,16 @@ class Engine:
         return {"rows": view(ch.ds_rows, min(ch.n_changed, n_ds), np.uint32), "n_changed": ch.n_changed,
                 "ds_out": view(ch.ds_out, n_ds, R.DS_OUT), "role_out": view(ch.role_out, n_roles, R.DS_ROLE_OUT),
                 "revrole_out": view(ch.revrole_out, n_rr, R.DS_REVROLE_OUT)}
+
+    def ds_resident_tick_info(self) -> dict:
+        """How the last DS tick read ready counts: ``linked`` (it ran the linked sweep),
+        ``rows_from_lws`` (existing revision-role rows that took the LWS tick's value),
+        ``rows_fallback`` (linked rows that used their own ready count) and ``lws_ticks`` (LWS ticks
+        submitted when it read the LWS rows)."""
+        info = R.DsTickInfo()
+        self._check(lib().lwse_ds_resident_tick_info(self._h, C.byref(info)))
+        return {"linked": bool(info.linked), "rows_from_lws": info.rows_from_lws,
+                "rows_fallback": info.rows_fallback, "lws_ticks": info.lws_ticks}
 
     # ------------------------------------------------------------- group keys
     def group_keys_host(self, strings) -> np.ndarray:

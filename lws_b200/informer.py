@@ -136,6 +136,7 @@ class IncrementalEncoder:
         self.needs_reload = False
         self.dirty: set = set()
         self._deleted: set = set()  # objects deleted since the last flush whose rows are still resident
+        self.moved_keys: set = set()  # (ns, name) whose LWS row the last flush() took, gave back or re-uid'ed
         # ---- first layout: objects in (namespace id, name) order so that the request table is grouped by namespace
         keys = sorted(self.items, key=lambda k: (self._ns_id(k[0]), k))
         fresh = {k: self._encode_object(k) for k in keys}
@@ -446,15 +447,22 @@ class IncrementalEncoder:
             self._node_resident[changed] = self.node_rec[changed]
             patches.add(R.TABLE_NODES, changed.tolist(), self.node_rec[changed])
             self._node_dirty.clear()
+        self.moved_keys = set(self._deleted)
         for key in sorted(self._deleted):
             self._vacate(self.slots.pop(key), self._ns_id(key[0]), patches, whole=True)
         self._deleted.clear()
         for key in sorted(self.dirty):
             t = self._encode_object(key)
-            if key not in self.slots and not self._create(key, t):
-                self.needs_reload = True
-                continue
+            if key not in self.slots:
+                if not self._create(key, t):
+                    self.needs_reload = True
+                    continue
+                self.moved_keys.add(key)
+            row = self.slots[key].lws_row
+            uid = int(self.lws["uid_hash"][row])
             self._write_object(key, t, patches)
+            if int(self.lws["uid_hash"][row]) != uid:  # the object was replaced under its name (a new uid)
+                self.moved_keys.add(key)
         self.dirty.clear()
         for free, base, n in self._freed:  # rows given back in this flush may be patched in it: reuse from the next
             _give(free, base, n)
@@ -482,6 +490,16 @@ class IncrementalEncoder:
 
     def lws_row(self, namespace: str, name: str) -> int:
         return self.slots[(namespace, name)].lws_row
+
+    def lws_link(self, namespace: str, name: str) -> Optional[tuple]:
+        """(LWS row, uid_hash) of a LeaderWorkerSet as the resident table holds it after the last
+        ``flush()``, or None when no row holds it: what a DS revision-role row links to
+        (``ds_informer.DsIncrementalEncoder(links=...)``).  ``moved_keys`` names the objects for which
+        the answer changed in the last ``flush()``: created, deleted, or given a new uid."""
+        sl = self.slots.get((namespace, name))
+        if sl is None:
+            return None
+        return sl.lws_row, int(self.lws["uid_hash"][sl.lws_row])
 
     def node_row(self, name: str) -> Optional[int]:
         """The node-table row of a node, or None for a node the table does not hold."""

@@ -280,6 +280,10 @@ DS_ROLE_OUT = np.dtype([("next_old", "<i4"), ("next_new", "<i4")], align=False)
 assert DS_ROLE_OUT.itemsize == 8
 DS_REVROLE_OUT = np.dtype("<i4")
 
+# lwse_ds_link: revision-role row → its child's row in the resident LWS table (TABLE_DS_LINKS)
+DS_LINK = np.dtype([("lws_uid_hash", "<u8"), ("lws_row", "<u4"), ("reserved", "<u4")], align=False)
+assert DS_LINK.itemsize == 16
+
 
 # --------------------------------------------------------------------------- #
 # ctypes bundles (lwse_lws_tables / lwse_ds_tables / lwse_config)
@@ -315,6 +319,7 @@ class Changes(C.Structure):
 
 TABLE_LWS, TABLE_GROUPS, TABLE_POD_STATE, TABLE_POD_IDENT, TABLE_PLACE_REQS, TABLE_NODES = 0, 1, 2, 3, 4, 5
 TABLE_DS, TABLE_DS_ROLES, TABLE_DS_REVROLES = 6, 7, 8  # lwse_ds_resident_tick only
+TABLE_DS_LINKS = 9  # lwse_ds_resident_tick only: DS_LINK rows, one per revision-role row
 PATCH_RANGE = 1 << 0
 TICK_MAX_SEGS = 8
 TICK_PLACE = 1 << 8
@@ -386,6 +391,18 @@ class DsChanges(C.Structure):
         ("ds_out", C.c_void_p),
         ("role_out", C.c_void_p),
         ("revrole_out", C.c_void_p),
+    ]
+
+
+class DsTickInfo(C.Structure):
+    """lwse_ds_tick_info: how the last DS tick read ready counts."""
+
+    _fields_ = [
+        ("linked", C.c_uint32),
+        ("rows_from_lws", C.c_uint32),
+        ("rows_fallback", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("lws_ticks", C.c_uint64),
     ]
 
 
