@@ -149,6 +149,15 @@ func (e *Engine) DsTickInfo() (C.lwse_ds_tick_info, error) {
 	return info, err
 }
 
+// Forecast replays the rest of every DS rollout from the resident DS tables as the last DsTick left
+// them, assuming every child becomes ready before each reconcile: per DS the flags, cycles and
+// trajectory offset, per role the peak replicas, availability floor and final counts, and (when
+// out.steps is set) the {old, new} rows of each step.  It changes no DsTick output and never waits for
+// LeaderWorkerSet ticks; a status or kubectl surface reads it, not Reconcile().
+func (e *Engine) Forecast(out *C.lwse_ds_forecast_out) error {
+	return e.check(C.lwse_ds_resident_forecast(e.h, out))
+}
+
 // GroupKeys computes SHA-1 digests (20 bytes each) of n strings laid out CSR-style.
 func (e *Engine) GroupKeys(bytes *C.uint8_t, offsets *C.uint32_t, n uint32, digests *C.uint8_t) error {
 	return e.check(C.lwse_group_keys_host(e.h, bytes, offsets, C.uint32_t(n), digests))

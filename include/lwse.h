@@ -848,6 +848,82 @@ typedef struct lwse_ds_tick_info { /* 24 B */
 } lwse_ds_tick_info;
 LWSE_API int lwse_ds_resident_tick_info(lwse_engine* e, lwse_ds_tick_info* info);
 
+/* ---- rollout forecast ---------------------------------------------------------------------
+ * The rest of every DS rollout, replayed on the device from the current rows: the reconcile cycles
+ * the DS controller would run if every child became ready before each cycle (simulateAllReady,
+ * executor_test.go:190-201).  One cycle of one DS, on a private copy of its rows:
+ *   1. every existing revision-role row gets ready_replicas = replicas;
+ *   2. the DS is swept with the arithmetic of lwse_sweep_ds_* (the same device code);
+ *   3. old revisions in drained_revs are deleted: their rows stop existing;
+ *   4. on LWSE_DOUT_INIT every existing old row gets initial_replicas = replicas (SetInitialReplicas,
+ *      executor.go:100-112) and the DS gets LWSE_DS_HAS_NEW_REVISION;
+ *   5. every existing row takes its revrole_out value as replicas (a nil spec.replicas takes a value);
+ *      a new-revision row that does not exist and has revrole_out >= 0 is created with that value
+ *      (initRollingUpdate at 0, or reconcileSimple creating a missing role).
+ * The replay stops at the first cycle that changes nothing (no replica value, no created or deleted
+ * row, no INIT), or after the cycle cap min(2*M + 12, LWSE_DS_FORECAST_MAX_CYCLES), M being the largest
+ * of any role's target_replicas and any role's sum over the DS's existing rows of max(replicas,
+ * initial_replicas) (ComputeAllSteps' 2*max + 10, planner.go:355-385, plus the INIT and cleanup
+ * cycles).  Per role, old = sum of replicas over existing old-revision rows, new = the new revision's
+ * replicas (0 when absent); sums are 64-bit and stored clamped to int32.  A DS that is not on the
+ * rolling path (LWSE_DOUT_ROLLING of a sweep of its current rows) runs no cycle.  DS whose row ranges
+ * overlap another DS's give unspecified results, as for the sweep. */
+#define LWSE_DS_FORECAST_MAX_CYCLES 65536u
+
+typedef struct lwse_ds_forecast { /* per DS, 16 B */
+  uint32_t flags;      /* LWSE_DSF_* */
+  uint32_t cycles;     /* cycles that changed something */
+  uint32_t step_base;  /* first trajectory row of this DS: rows of the DS before it, in DS order
+                          (saturates at 0xFFFFFFFF)                                           */
+  uint32_t n_steps;    /* cycles that changed some role's old or new count: n_steps * n_roles rows */
+} lwse_ds_forecast;
+
+#define LWSE_DSF_ROLLING (1u << 0)    /* the current rows are on the rolling path                  */
+#define LWSE_DSF_WAITING (1u << 1)    /* …with a new revision that is not stable: the first cycle
+                                         assumes it becomes ready                                    */
+#define LWSE_DSF_DONE (1u << 2)       /* rolling, and stopped with no old replicas left and every
+                                         spec role's new count at its target                         */
+#define LWSE_DSF_UNFINISHED (1u << 3) /* rolling, and stopped with work left or at the cycle cap    */
+#define LWSE_DSF_TRUNCATED (1u << 4)  /* its trajectory did not fit in step_capacity: none of its
+                                         rows were written (the summaries are exact)                 */
+#define LWSE_DSF_BAD_TABLE (1u << 6)  /* as LWSE_DOUT_BAD_TABLE; nothing else is set               */
+
+typedef struct lwse_ds_forecast_role { /* per role row, 16 B (zero for rows of no valid DS) */
+  int32_t peak_replicas;   /* max of old + new now and of old_k + new_{k+1} over cycles k (scaleUpNew
+                              runs before scaleDownOld, executor.go:163-166)                   */
+  int32_t floor_available; /* min of old + new now and of old_{k+1} + new_k over cycles k (drained pods
+                              are gone, new ones are not ready yet)                            */
+  int32_t final_old;       /* old and new after the last cycle (now, for a DS that runs none)  */
+  int32_t final_new;
+} lwse_ds_forecast_role;
+
+/* Trajectory rows are lwse_ds_role_out rows {next_old, next_new} = {old, new} after a cycle that
+ * changed some role's count, one per role; a DS's n_steps * n_roles rows are contiguous at step_base,
+ * step-major.  A DS whose rows do not all fit below step_capacity gets LWSE_DSF_TRUNCATED and writes
+ * none; no row at or beyond step_capacity is written, and no DS writes outside its own n_steps * n_roles
+ * rows (also where overlapping row ranges make the results unspecified). */
+typedef struct lwse_ds_forecast_out {
+  lwse_ds_forecast* ds;              /* [n_ds]                                                */
+  lwse_ds_forecast_role* roles;      /* [n_roles]                                             */
+  lwse_ds_role_out* steps;           /* [step_capacity], or NULL: summaries only              */
+  uint32_t step_capacity;
+  uint32_t n_steps_written;          /* out: trajectory rows written                          */
+  uint64_t n_steps_needed;           /* out: rows every DS's trajectory needs                 */
+} lwse_ds_forecast_out;
+
+/* Stateless: host tables in (output pointers of `host` ignored), host outputs out.  LWSE_ERR_INVALID_ARG
+ * for NULL tables or outputs. */
+LWSE_API int lwse_ds_forecast_host(lwse_engine* e, const lwse_ds_tables* host, lwse_ds_forecast_out* out);
+/* Over the resident DS tables as the last lwse_ds_resident_tick (or the load) left them.  Runs on the
+ * DS stream under the engine mutex, with scratch of its own: it changes no resident table, no DS tick
+ * output, change list or counter, and never drains or drops LeaderWorkerSet ticks.  Links are ignored
+ * (the forecast assumes readiness).  The scratch is sized by the tables and by the trajectory rows
+ * written (never by step_capacity) and only grows: a call that needs more of it than any call before
+ * allocates device memory, which waits for the device as cudaMalloc / cudaFree do (as
+ * lwse_ds_resident_load); every other call waits only on the DS stream.  LWSE_ERR_NOT_READY before
+ * lwse_ds_resident_load; LWSE_ERR_INVALID_ARG for NULL outputs. */
+LWSE_API int lwse_ds_resident_forecast(lwse_engine* e, lwse_ds_forecast_out* out);
+
 /* ------------------------------------------------------------------------- */
 /* Group / subgroup keys (SHA-1) and subgroup indices                        */
 /* ------------------------------------------------------------------------- */

@@ -257,8 +257,193 @@ __device__ __forceinline__ void ds_tick_diff(const lwse_ds_tables& t, const DsTi
   a.rows[base + __popc(m & ((1u << lane) - 1u))] = d;
 }
 
-// kTick = false: the stateless sweep (lwse_sweep_ds_*), `a` unused; its code is the same as before the
-// tick form existed.  kTick = true: the resident tick — diff, mirrors, change list, and the publish of
+// The table checks of one DS (BAD_TABLE when they fail): its ranges lie inside the tables.
+__device__ __forceinline__ bool ds_rows_ok(const lwse_ds_tables& t, const uint4 h0, const uint4 h1) {
+  const uint32_t role_base = h0.z, n_roles = h0.w, n_spec = h1.x, rev_base = h1.y, n_old = h1.z;
+  return !(n_roles > LWSE_DS_MAX_ROLES || n_spec > n_roles || n_old > LWSE_DS_MAX_OLD_REVS ||
+           (uint64_t)role_base + n_roles > t.n_roles ||
+           (uint64_t)rev_base + (uint64_t)(n_old + 1u) * n_roles > t.n_revroles);
+}
+
+// How the sweep body reads revision-role rows.  The sweep and the tick read input tables that
+// nothing in the kernel writes: ld.global.nc.  The forecast rewrites its scratch copy of the rows
+// between the cycles of one kernel, so it reads them with coherent loads, ordered after the thread's
+// own stores (the memory clobber: the compiler moves no store of a row past them).
+struct RrLoadNc {
+  static __device__ __forceinline__ uint4 row(const uint4* p) { return ldg_stream(p); }
+  static __device__ __forceinline__ uint32_t flags(const uint32_t* p) { return __ldg(p); }
+};
+struct RrLoadCoherent {
+  static __device__ __forceinline__ uint4 row(const uint4* p) {
+    uint4 r;
+    asm volatile("ld.global.v4.u32 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
+                 : "l"(p)
+                 : "memory");
+    return r;
+  }
+  static __device__ __forceinline__ uint32_t flags(const uint32_t* p) {
+    uint32_t r;
+    asm volatile("ld.global.u32 %0, [%1];" : "=r"(r) : "l"(p) : "memory");
+    return r;
+  }
+};
+
+// One DS of the sweep (h0, h1: its lwse_ds_rec): writes its ds_out, role_out and revrole_out rows
+// and returns {ds_out.flags, ds_out.drained_revs}.  Shared by the sweep, the tick and the forecast.
+template <class Ld, bool kLinked>
+__device__ __forceinline__ uint2 ds_sweep_one(const lwse_ds_tables& t, const DsTickArgs& a, const uint32_t d,
+                                              const uint4 h0, const uint4 h1, uint32_t& took, uint32_t& fell) {
+  const uint32_t role_base = h0.z, n_roles = h0.w, n_spec = h1.x, rev_base = h1.y, n_old = h1.z, dflags = h1.w;
+  uint32_t oflags = 0, drained = 0, ready_revs = 0;
+  const int n = (int)n_roles, S = (int)n_spec, V = (int)n_old;
+  if (!ds_rows_ok(t, h0, h1)) {
+    stg_stream(t.ds_out + d, make_uint4(LWSE_DOUT_BAD_TABLE, 0, 0, 0));
+    return make_uint2(LWSE_DOUT_BAD_TABLE, 0);
+  }
+  const lwse_ds_role_rec* roles = t.roles + role_base;
+  const uint4* rr = reinterpret_cast<const uint4*>(t.revroles + rev_base);  // {replicas, initial, ready, flags}
+  lwse_ds_role_out* ro = t.role_out + role_base;
+  lwse_ds_revrole_out* rro = t.revrole_out + rev_base;
+
+  int initial_old[MAXR], cur_old[MAXR], cur_new[MAXR], target[MAXR];
+  RuConfig cfg[MAXR];
+  for (int i = 0; i < n; i++) initial_old[i] = cur_old[i] = cur_new[i] = target[i] = 0;
+
+  // one pass over the old revisions: totals, cleanup predicate, service readiness, defaults
+  int total_old_spec = 0;
+  for (int r = 0; r < V; r++) {
+    bool any = false, all_drained = true, ready = true;
+    for (int i = 0; i < n; i++) {
+      uint4 x = Ld::row(rr + r * n + i);
+      const bool exists = x.w & LWSE_RR_EXISTS;
+      if constexpr (kLinked) x.z = (uint32_t)linked_ready(a, rev_base + r * n + i, exists, (int)x.z, took, fell);
+      rro[r * n + i] = exists ? (int)x.x : -1;
+      if (i < S && (!exists || (int)x.z < 1)) ready = false;  // service_manager.go:62-67
+      if (!exists) continue;
+      any = true;
+      if (((x.w & LWSE_RR_REPLICAS_NIL) ? 0 : (int)x.x) != 0) all_drained = false;  // :222-225
+      cur_old[i] += (int)x.x;                                                        // utils.go:167-175
+      initial_old[i] += (int)x.y >= 0 ? (int)x.y : (int)x.x;                         // utils.go:177-190
+      if (i < S) total_old_spec += (int)x.x;
+    }
+    if (any && all_drained) drained |= 1u << r;
+    if (ready) ready_revs |= 1u << r;
+  }
+  bool new_ready = true, stable = true;
+  for (int i = 0; i < n; i++) {
+    uint4 x = Ld::row(rr + V * n + i);
+    const bool exists = x.w & LWSE_RR_EXISTS;
+    if constexpr (kLinked) x.z = (uint32_t)linked_ready(a, rev_base + V * n + i, exists, (int)x.z, took, fell);
+    rro[V * n + i] = exists ? (int)x.x : -1;
+    const uint4 rl = ldg_cached(reinterpret_cast<const uint4*>(roles + i));  // {target, surge, unavail, flags}
+    const bool in_spec = rl.w & LWSE_ROLE_IN_SPEC;
+    if (i < S) {
+      if (!exists || (int)x.z < 1) new_ready = false;
+      if (!exists || (int)x.x != (int)x.z) stable = false;  // isRevisionStable executor.go:270-281
+    }
+    if (in_spec) {
+      if (exists) cur_new[i] = (int)x.x;
+      target[i] = (int)rl.x;
+    }
+    // extractRollingUpdateConfig executor.go:235-260
+    cfg[i].ms = 1;
+    cfg[i].mu = 0;
+    if (in_spec && (rl.w & LWSE_ROLE_HAS_ROLLING_CONFIG)) {
+      const int replicas = (int)rl.x;
+      const int surge = (rl.w & LWSE_ROLE_SURGE_INVALID)
+                            ? 0
+                            : scaled_value((int)rl.y, rl.w & LWSE_ROLE_SURGE_IS_PERCENT, replicas, true);
+      const int unav = (rl.w & LWSE_ROLE_UNAVAIL_INVALID)
+                           ? 0
+                           : scaled_value((int)rl.z, rl.w & LWSE_ROLE_UNAVAIL_IS_PERCENT, replicas, false);
+      if (unav > 0) {
+        cfg[i].mu = unav;
+        cfg[i].ms = surge;
+      } else if (surge > 0) {
+        cfg[i].ms = surge;
+      }
+    }
+    ro[i].next_old = -1;
+    ro[i].next_new = -1;
+  }
+  if (new_ready) oflags |= LWSE_DOUT_NEW_READY;
+
+  if (!(V > 0 && total_old_spec > 0)) {
+    // reconcileSimple disaggregatedset_controller.go:137-186
+    for (int i = 0; i < S; i++) rro[V * n + i] = target[i];
+  } else {
+    oflags |= LWSE_DOUT_ROLLING;
+    if (!(dflags & LWSE_DS_HAS_NEW_REVISION)) {
+      oflags |= LWSE_DOUT_INIT;  // initRollingUpdate executor.go:85-124
+      for (int i = 0; i < S; i++) rro[V * n + i] = 0;
+    } else if (stable) {
+      oflags |= LWSE_DOUT_STABLE;
+      int past[MAXR], new_[MAXR];
+      if (!compute_next_step(n, initial_old, cur_old, cur_new, target, cfg, past, new_)) {
+        oflags |= LWSE_DOUT_COMPLETE;
+      } else {
+        oflags |= LWSE_DOUT_STEP;
+        for (int i = 0; i < n; i++) {
+          ro[i].next_old = past[i];
+          ro[i].next_new = new_[i];
+          // scaleUpNew executor.go:306-328
+          if ((__ldg(&roles[i].flags) & LWSE_ROLE_IN_SPEC) && cur_new[i] < new_[i]) rro[V * n + i] = new_[i];
+        }
+        // scaleDownOld executor.go:330-398, revisions newest-first (:283-302)
+        int budget[MAXR];
+        for (int i = 0; i < n; i++) budget[i] = cur_old[i] - past[i];
+        uint32_t done_mask = 0;
+        for (int k = 0; k < V; k++) {
+          bool all_zero = true;
+          for (int i = 0; i < n; i++)
+            if (budget[i] > 0) all_zero = false;
+          if (all_zero) break;
+          // next newest revision not yet handled (stable: lowest row on equal stamps)
+          int r = -1;
+          uint32_t best_ts = 0;
+          for (int c = 0; c < V; c++) {
+            if (done_mask & (1u << c)) continue;
+            uint32_t ts = 0;
+            for (int i = 0; i < n; i++) {
+              const uint32_t w = Ld::flags(&t.revroles[rev_base + c * n + i].flags);
+              if (w & LWSE_RR_EXISTS) ts = max(ts, w >> LWSE_RR_TS_SHIFT);
+            }
+            if (r < 0 || ts > best_ts) {
+              r = c;
+              best_ts = ts;
+            }
+          }
+          done_mask |= 1u << r;
+          int new_rep[MAXR], planned[MAXR];
+          uint32_t trig = 0;
+          for (int i = 0; i < n; i++) {
+            planned[i] = 0;
+            new_rep[i] = 0;
+            const int rep = rro[r * n + i];
+            if (rep < 0) continue;
+            const int drain = min(budget[i], rep);
+            planned[i] = drain;
+            new_rep[i] = rep - drain;
+            if (new_rep[i] == 0) trig |= 1u << i;
+          }
+          for (int i = 0; i < n; i++) {
+            const int rep = rro[r * n + i];
+            if (rep < 0) continue;
+            const int nr = trig ? 0 : new_rep[i];  // coordinated drain :366-373
+            if (rep <= nr) continue;
+            rro[r * n + i] = nr;
+            if ((trig & (1u << i)) || !trig) budget[i] -= planned[i];  // :392-394
+          }
+        }
+      }
+    }
+  }
+  stg_stream(t.ds_out + d, make_uint4(oflags, drained, ready_revs, 0));
+  return make_uint2(oflags, drained);
+}
+
+// kTick = false: the stateless sweep (lwse_sweep_ds_*), `a` unused.  kTick = true: the resident tick — diff, mirrors, change list, and the publish of
 // the count and sequence word by the last CTA (one system-scope release, as publish_lists_kernel).
 // kLinked (with kTick): every revision-role row's ready count goes through linked_ready, and the two
 // row counts are published beside the changed-row count.
@@ -268,154 +453,7 @@ __global__ void __launch_bounds__(128) ds_sweep_kernel(const lwse_ds_tables t, c
   for (uint32_t d = blockIdx.x * blockDim.x + threadIdx.x; d < t.n_ds; d += gridDim.x * blockDim.x) {
     const uint4 h0 = ldg_stream(reinterpret_cast<const uint4*>(t.ds + d) + 0);
     const uint4 h1 = ldg_stream(reinterpret_cast<const uint4*>(t.ds + d) + 1);
-    const uint32_t role_base = h0.z, n_roles = h0.w, n_spec = h1.x, rev_base = h1.y, n_old = h1.z, dflags = h1.w;
-    uint32_t oflags = 0, drained = 0, ready_revs = 0;
-    const int n = (int)n_roles, S = (int)n_spec, V = (int)n_old;
-    if (n_roles > LWSE_DS_MAX_ROLES || n_spec > n_roles || n_old > LWSE_DS_MAX_OLD_REVS ||
-        (uint64_t)role_base + n_roles > t.n_roles ||
-        (uint64_t)rev_base + (uint64_t)(n_old + 1u) * n_roles > t.n_revroles) {
-      stg_stream(t.ds_out + d, make_uint4(LWSE_DOUT_BAD_TABLE, 0, 0, 0));
-      continue;
-    }
-    const lwse_ds_role_rec* roles = t.roles + role_base;
-    const uint4* rr = reinterpret_cast<const uint4*>(t.revroles + rev_base);  // {replicas, initial, ready, flags}
-    lwse_ds_role_out* ro = t.role_out + role_base;
-    lwse_ds_revrole_out* rro = t.revrole_out + rev_base;
-
-    int initial_old[MAXR], cur_old[MAXR], cur_new[MAXR], target[MAXR];
-    RuConfig cfg[MAXR];
-    for (int i = 0; i < n; i++) initial_old[i] = cur_old[i] = cur_new[i] = target[i] = 0;
-
-    // one pass over the old revisions: totals, cleanup predicate, service readiness, defaults
-    int total_old_spec = 0;
-    for (int r = 0; r < V; r++) {
-      bool any = false, all_drained = true, ready = true;
-      for (int i = 0; i < n; i++) {
-        uint4 x = ldg_stream(rr + r * n + i);
-        const bool exists = x.w & LWSE_RR_EXISTS;
-        if constexpr (kLinked) x.z = (uint32_t)linked_ready(a, rev_base + r * n + i, exists, (int)x.z, took, fell);
-        rro[r * n + i] = exists ? (int)x.x : -1;
-        if (i < S && (!exists || (int)x.z < 1)) ready = false;  // service_manager.go:62-67
-        if (!exists) continue;
-        any = true;
-        if (((x.w & LWSE_RR_REPLICAS_NIL) ? 0 : (int)x.x) != 0) all_drained = false;  // :222-225
-        cur_old[i] += (int)x.x;                                                        // utils.go:167-175
-        initial_old[i] += (int)x.y >= 0 ? (int)x.y : (int)x.x;                         // utils.go:177-190
-        if (i < S) total_old_spec += (int)x.x;
-      }
-      if (any && all_drained) drained |= 1u << r;
-      if (ready) ready_revs |= 1u << r;
-    }
-    bool new_ready = true, stable = true;
-    for (int i = 0; i < n; i++) {
-      uint4 x = ldg_stream(rr + V * n + i);
-      const bool exists = x.w & LWSE_RR_EXISTS;
-      if constexpr (kLinked) x.z = (uint32_t)linked_ready(a, rev_base + V * n + i, exists, (int)x.z, took, fell);
-      rro[V * n + i] = exists ? (int)x.x : -1;
-      const uint4 rl = ldg_cached(reinterpret_cast<const uint4*>(roles + i));  // {target, surge, unavail, flags}
-      const bool in_spec = rl.w & LWSE_ROLE_IN_SPEC;
-      if (i < S) {
-        if (!exists || (int)x.z < 1) new_ready = false;
-        if (!exists || (int)x.x != (int)x.z) stable = false;  // isRevisionStable executor.go:270-281
-      }
-      if (in_spec) {
-        if (exists) cur_new[i] = (int)x.x;
-        target[i] = (int)rl.x;
-      }
-      // extractRollingUpdateConfig executor.go:235-260
-      cfg[i].ms = 1;
-      cfg[i].mu = 0;
-      if (in_spec && (rl.w & LWSE_ROLE_HAS_ROLLING_CONFIG)) {
-        const int replicas = (int)rl.x;
-        const int surge = (rl.w & LWSE_ROLE_SURGE_INVALID)
-                              ? 0
-                              : scaled_value((int)rl.y, rl.w & LWSE_ROLE_SURGE_IS_PERCENT, replicas, true);
-        const int unav = (rl.w & LWSE_ROLE_UNAVAIL_INVALID)
-                             ? 0
-                             : scaled_value((int)rl.z, rl.w & LWSE_ROLE_UNAVAIL_IS_PERCENT, replicas, false);
-        if (unav > 0) {
-          cfg[i].mu = unav;
-          cfg[i].ms = surge;
-        } else if (surge > 0) {
-          cfg[i].ms = surge;
-        }
-      }
-      ro[i].next_old = -1;
-      ro[i].next_new = -1;
-    }
-    if (new_ready) oflags |= LWSE_DOUT_NEW_READY;
-
-    if (!(V > 0 && total_old_spec > 0)) {
-      // reconcileSimple disaggregatedset_controller.go:137-186
-      for (int i = 0; i < S; i++) rro[V * n + i] = target[i];
-    } else {
-      oflags |= LWSE_DOUT_ROLLING;
-      if (!(dflags & LWSE_DS_HAS_NEW_REVISION)) {
-        oflags |= LWSE_DOUT_INIT;  // initRollingUpdate executor.go:85-124
-        for (int i = 0; i < S; i++) rro[V * n + i] = 0;
-      } else if (stable) {
-        oflags |= LWSE_DOUT_STABLE;
-        int past[MAXR], new_[MAXR];
-        if (!compute_next_step(n, initial_old, cur_old, cur_new, target, cfg, past, new_)) {
-          oflags |= LWSE_DOUT_COMPLETE;
-        } else {
-          oflags |= LWSE_DOUT_STEP;
-          for (int i = 0; i < n; i++) {
-            ro[i].next_old = past[i];
-            ro[i].next_new = new_[i];
-            // scaleUpNew executor.go:306-328
-            if ((__ldg(&roles[i].flags) & LWSE_ROLE_IN_SPEC) && cur_new[i] < new_[i]) rro[V * n + i] = new_[i];
-          }
-          // scaleDownOld executor.go:330-398, revisions newest-first (:283-302)
-          int budget[MAXR];
-          for (int i = 0; i < n; i++) budget[i] = cur_old[i] - past[i];
-          uint32_t done_mask = 0;
-          for (int k = 0; k < V; k++) {
-            bool all_zero = true;
-            for (int i = 0; i < n; i++)
-              if (budget[i] > 0) all_zero = false;
-            if (all_zero) break;
-            // next newest revision not yet handled (stable: lowest row on equal stamps)
-            int r = -1;
-            uint32_t best_ts = 0;
-            for (int c = 0; c < V; c++) {
-              if (done_mask & (1u << c)) continue;
-              uint32_t ts = 0;
-              for (int i = 0; i < n; i++) {
-                const uint32_t w = __ldg(&t.revroles[rev_base + c * n + i].flags);
-                if (w & LWSE_RR_EXISTS) ts = max(ts, w >> LWSE_RR_TS_SHIFT);
-              }
-              if (r < 0 || ts > best_ts) {
-                r = c;
-                best_ts = ts;
-              }
-            }
-            done_mask |= 1u << r;
-            int new_rep[MAXR], planned[MAXR];
-            uint32_t trig = 0;
-            for (int i = 0; i < n; i++) {
-              planned[i] = 0;
-              new_rep[i] = 0;
-              const int rep = rro[r * n + i];
-              if (rep < 0) continue;
-              const int drain = min(budget[i], rep);
-              planned[i] = drain;
-              new_rep[i] = rep - drain;
-              if (new_rep[i] == 0) trig |= 1u << i;
-            }
-            for (int i = 0; i < n; i++) {
-              const int rep = rro[r * n + i];
-              if (rep < 0) continue;
-              const int nr = trig ? 0 : new_rep[i];  // coordinated drain :366-373
-              if (rep <= nr) continue;
-              rro[r * n + i] = nr;
-              if ((trig & (1u << i)) || !trig) budget[i] -= planned[i];  // :392-394
-            }
-          }
-        }
-      }
-    }
-    stg_stream(t.ds_out + d, make_uint4(oflags, drained, ready_revs, 0));
+    ds_sweep_one<RrLoadNc, kLinked>(t, a, d, h0, h1, took, fell);
   }
   if constexpr (kTick) {
     for (uint32_t d = blockIdx.x * blockDim.x + threadIdx.x; d < t.n_ds; d += gridDim.x * blockDim.x) ds_tick_diff(t, a, d);
@@ -450,6 +488,283 @@ __global__ void __launch_bounds__(128) ds_sweep_kernel(const lwse_ds_tables t, c
       }
     }
   }
+}
+
+// ---- rollout forecast (lwse_ds_forecast_*): the cycle rules are in lwse.h ----
+struct DsForecastArgs {
+  lwse_ds_revrole_rec* rows;            // scratch copy of the revision-role table (same row numbers)
+  lwse_ds_out* s_ds_out;                // the sweep body's outputs for the replay (scratch)
+  lwse_ds_role_out* s_role_out;
+  lwse_ds_revrole_out* s_revrole_out;
+  lwse_ds_forecast* fc;                 // [n_ds]
+  lwse_ds_forecast_role* fc_role;       // [n_roles]
+  lwse_ds_role_out* steps;              // [step_capacity] (write pass only)
+  uint32_t step_capacity;
+  unsigned long long* totals;           // scan: [0] rows needed, [1] rows written
+};
+
+__device__ __forceinline__ int clamp32(long long v) {
+  return (int)max(min(v, (long long)INT32_MAX), (long long)INT32_MIN);
+}
+
+// Per-role old (existing old-revision rows) and new (the new revision's row) counts of a DS's rows.
+__device__ __forceinline__ void ds_role_counts(const uint4* rows, int n, int V, long long* old_c, long long* new_c) {
+  for (int i = 0; i < n; i++) old_c[i] = new_c[i] = 0;
+  for (int r = 0; r <= V; r++)
+    for (int i = 0; i < n; i++) {
+      const uint4 x = rows[r * n + i];
+      if (!(x.w & LWSE_RR_EXISTS)) continue;
+      if (r < V)
+        old_c[i] += (int)x.x;
+      else
+        new_c[i] = (int)x.x;
+    }
+}
+
+// The replay of DS d.  kWrite = false: summaries, and the DS's trajectory row count in step_base
+// (the scan turns it into an offset).  kWrite = true: replays the DS again and writes its rows.
+// The thread owns the DS's scratch rows, so nothing is shared between threads.
+template <bool kWrite>
+__device__ void ds_forecast_one(const lwse_ds_tables& in, const DsForecastArgs& f, const uint32_t d) {
+  const uint4 h0 = ldg_stream(reinterpret_cast<const uint4*>(in.ds + d) + 0);
+  uint4 h1 = ldg_stream(reinterpret_cast<const uint4*>(in.ds + d) + 1);
+  if (!ds_rows_ok(in, h0, h1)) {
+    if (!kWrite) f.fc[d] = lwse_ds_forecast{LWSE_DSF_BAD_TABLE, 0u, 0u, 0u};
+    return;
+  }
+  // The write pass writes at most the n_steps rows the summary pass counted and the scan reserved
+  // below step_capacity.  Its replay finds the same steps, except where DS row ranges overlap (their
+  // threads then share scratch rows and the results are unspecified): the bound keeps every store
+  // inside the DS's own reserved rows even then.
+  uint32_t step_base = 0, step_limit = 0;
+  if constexpr (kWrite) {
+    const lwse_ds_forecast c = f.fc[d];
+    if (c.n_steps == 0 || (c.flags & LWSE_DSF_TRUNCATED)) return;
+    step_base = c.step_base;
+    step_limit = c.n_steps;
+  }
+  const uint32_t role_base = h0.z, rev_base = h1.y;
+  const int n = (int)h0.w, S = (int)h1.x, V = (int)h1.z, nrr = (V + 1) * n;
+  const lwse_ds_role_rec* roles = in.roles + role_base;
+  const uint4* src = reinterpret_cast<const uint4*>(in.revroles + rev_base);
+  uint4* rows = reinterpret_cast<uint4*>(f.rows + rev_base);  // {replicas, initial, ready, flags}
+
+  // private copy of the rows; the cap's M; the newest creation rank
+  long long mx[MAXR];
+  for (int i = 0; i < n; i++) mx[i] = 0;
+  uint32_t rank = 0;
+  for (int k = 0; k < nrr; k++) {
+    const uint4 x = ldg_stream(src + k);
+    rows[k] = x;
+    if (x.w & LWSE_RR_EXISTS) {
+      mx[k % n] += max((int)x.x, (int)x.y);
+      rank = max(rank, x.w >> LWSE_RR_TS_SHIFT);
+    }
+  }
+  long long M = 0;
+  for (int i = 0; i < n; i++) M = max(M, max(mx[i], (long long)__ldg(&roles[i].target_replicas)));
+  const uint32_t cap = (uint32_t)min(2 * M + 12, (long long)LWSE_DS_FORECAST_MAX_CYCLES);
+
+  long long old_c[MAXR], new_c[MAXR], peak[MAXR], floor_[MAXR];
+  ds_role_counts(rows, n, V, old_c, new_c);
+  for (int i = 0; i < n; i++) peak[i] = floor_[i] = old_c[i] + new_c[i];
+
+  lwse_ds_tables t = in;
+  t.revroles = f.rows;
+  t.ds_out = f.s_ds_out;
+  t.role_out = f.s_role_out;
+  t.revrole_out = f.s_revrole_out;
+  const DsTickArgs none{};
+  uint32_t unused = 0;
+  // the current rows as they are: the rolling path, and whether the new revision is stable
+  const uint2 now = ds_sweep_one<RrLoadCoherent, false>(t, none, d, h0, h1, unused, unused);
+  uint32_t flags = 0, cycles = 0, n_steps = 0;
+  const lwse_ds_revrole_out* rro = f.s_revrole_out + rev_base;
+  if (now.x & LWSE_DOUT_ROLLING) {
+    flags = LWSE_DSF_ROLLING;
+    if (!(now.x & (LWSE_DOUT_INIT | LWSE_DOUT_STABLE))) flags |= LWSE_DSF_WAITING;
+    bool stopped = false;
+    for (uint32_t c = 0; c < cap; c++) {
+      for (int k = 0; k < nrr; k++) {  // 1. every child ready
+        uint4 x = rows[k];
+        if (x.w & LWSE_RR_EXISTS) {
+          x.z = x.x;
+          rows[k] = x;
+        }
+      }
+      const uint2 o = ds_sweep_one<RrLoadCoherent, false>(t, none, d, h0, h1, unused, unused);  // 2.
+      bool changed = false;
+      for (int r = 0; r < V; r++) {  // 3. cleanupDrainedLWS
+        if (!((o.y >> r) & 1u)) continue;
+        changed = true;
+        for (int i = 0; i < n; i++) {
+          uint4 x = rows[r * n + i];
+          x.w &= ~LWSE_RR_EXISTS;
+          rows[r * n + i] = x;
+        }
+      }
+      if (o.x & LWSE_DOUT_INIT) {  // 4. initRollingUpdate
+        changed = true;
+        h1.w |= LWSE_DS_HAS_NEW_REVISION;
+        for (int k = 0; k < V * n; k++) {
+          uint4 x = rows[k];
+          if (x.w & LWSE_RR_EXISTS) {
+            x.y = x.x;
+            rows[k] = x;
+          }
+        }
+      }
+      for (int k = 0; k < nrr; k++) {  // 5. the decided replicas
+        const int v = rro[k];
+        if (v < 0) continue;
+        uint4 x = rows[k];
+        if (x.w & LWSE_RR_EXISTS) {
+          if ((int)x.x == v && !(x.w & LWSE_RR_REPLICAS_NIL)) continue;
+          x.x = (uint32_t)v;
+          x.w &= ~LWSE_RR_REPLICAS_NIL;
+        } else if (k >= V * n) {
+          x = make_uint4((uint32_t)v, 0xFFFFFFFFu, 0u, LWSE_RR_EXISTS | (rank << LWSE_RR_TS_SHIFT));
+        } else {
+          continue;
+        }
+        rows[k] = x;
+        changed = true;
+      }
+      if (!changed) {
+        stopped = true;
+        break;
+      }
+      cycles++;
+      long long nold[MAXR], nnew[MAXR];
+      ds_role_counts(rows, n, V, nold, nnew);
+      bool step = false;
+      for (int i = 0; i < n; i++) {
+        if (nold[i] != old_c[i] || nnew[i] != new_c[i]) step = true;
+        peak[i] = max(peak[i], old_c[i] + nnew[i]);
+        floor_[i] = min(floor_[i], nold[i] + new_c[i]);
+        old_c[i] = nold[i];
+        new_c[i] = nnew[i];
+      }
+      if (step) {
+        if constexpr (kWrite) {
+          uint2* out = reinterpret_cast<uint2*>(f.steps + step_base + n_steps * (uint32_t)n);
+          for (int i = 0; i < n; i++) out[i] = make_uint2((uint32_t)clamp32(nold[i]), (uint32_t)clamp32(nnew[i]));
+        }
+        n_steps++;
+        if constexpr (kWrite) {
+          if (n_steps == step_limit) return;  // every reserved row is written: the rest is the summary pass's
+        }
+      }
+    }
+    bool done = stopped;
+    for (int i = 0; i < n; i++) {
+      if (old_c[i] != 0) done = false;
+      if (i < S && new_c[i] != (long long)__ldg(&roles[i].target_replicas)) done = false;
+    }
+    flags |= done ? LWSE_DSF_DONE : LWSE_DSF_UNFINISHED;
+  }
+  if constexpr (!kWrite) {
+    f.fc[d] = lwse_ds_forecast{flags, cycles, n_steps * (uint32_t)n, n_steps};
+    for (int i = 0; i < n; i++)
+      f.fc_role[role_base + i] =
+          lwse_ds_forecast_role{clamp32(peak[i]), clamp32(floor_[i]), clamp32(old_c[i]), clamp32(new_c[i])};
+  }
+}
+
+template <bool kWrite>
+__global__ void __launch_bounds__(128) ds_forecast_kernel(const lwse_ds_tables in, const DsForecastArgs f) {
+  for (uint32_t d = blockIdx.x * blockDim.x + threadIdx.x; d < in.n_ds; d += gridDim.x * blockDim.x)
+    ds_forecast_one<kWrite>(in, f, d);
+}
+
+// One CTA: step_base (a row count after the summary pass) becomes the exclusive prefix over the DS in
+// row order; with a trajectory buffer, DS whose rows end beyond step_capacity get TRUNCATED.
+// totals[0] = rows needed, totals[1] = rows written.
+constexpr int kScanThreads = 1024;
+__global__ void __launch_bounds__(kScanThreads) ds_forecast_scan_kernel(lwse_ds_forecast* fc, uint32_t n_ds,
+                                                                        uint32_t capacity, int has_steps,
+                                                                        unsigned long long* totals) {
+  __shared__ unsigned long long s_warp[kScanThreads / 32];
+  const uint32_t per = (n_ds + kScanThreads - 1) / kScanThreads;
+  const uint32_t lo = min(n_ds, threadIdx.x * per), hi = min(n_ds, lo + per);
+  unsigned long long sum = 0;
+  for (uint32_t d = lo; d < hi; d++) sum += fc[d].step_base;
+  // block-wide exclusive scan of the per-thread sums
+  const unsigned lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  unsigned long long incl = sum;
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+    if ((int)lane >= o) incl += v;
+  }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    unsigned long long w = s_warp[lane], wi = w;
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long v = __shfl_up_sync(0xFFFFFFFFu, wi, o);
+      if ((int)lane >= o) wi += v;
+    }
+    s_warp[lane] = wi - w;
+  }
+  __syncthreads();
+  unsigned long long base = s_warp[warp] + incl - sum, written = 0;
+  for (uint32_t d = lo; d < hi; d++) {
+    lwse_ds_forecast c = fc[d];
+    const unsigned long long rows = c.step_base;
+    c.step_base = (uint32_t)min(base, 0xFFFFFFFFull);
+    if (has_steps && rows) {
+      if (base + rows > capacity)
+        c.flags |= LWSE_DSF_TRUNCATED;
+      else
+        written += rows;
+    }
+    fc[d] = c;
+    base += rows;
+  }
+  if (threadIdx.x == kScanThreads - 1) totals[0] = base;
+  written = __reduce_add_sync(0xFFFFFFFFu, (unsigned)written);  // (< 2^32: bounded by capacity)
+  if (lane == 0 && written) atomicAdd(totals + 1, written);
+}
+
+struct DsForecastHost {  // (lwse_engine.cu)
+  lwse_ds_revrole_rec* rows;
+  lwse_ds_out* s_ds_out;
+  lwse_ds_role_out* s_role_out;
+  lwse_ds_revrole_out* s_revrole_out;
+  lwse_ds_forecast* fc;
+  lwse_ds_forecast_role* fc_role;
+  lwse_ds_role_out* steps;  // the write pass's rows (device scratch)
+  uint32_t step_capacity;
+  bool want_steps;  // a trajectory is asked for: the scan marks what does not fit in step_capacity
+  unsigned long long* totals;  // device, 2 words, zeroed by the caller
+};
+
+// write_pass = false: the summary pass and the scan.  write_pass = true: the write pass into h->steps,
+// which holds the rows the scan counted as written.  Both on stream s.
+int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s,
+                       int* cuda_err) {
+  *cuda_err = 0;
+  if (t->n_ds == 0) return 0;
+  const uint32_t want = (t->n_ds + 127u) / 128u;
+  const uint32_t cap = (uint32_t)sm_count * 16u;
+  const uint32_t grid = want < cap ? want : cap;
+  const DsForecastArgs f{h->rows, h->s_ds_out, h->s_role_out, h->s_revrole_out, h->fc, h->fc_role,
+                         h->steps, h->step_capacity, h->totals};
+  int launched;
+  if (write_pass) {
+    ds_forecast_kernel<true><<<grid, 128, 0, s>>>(*t, f);
+    launched = 1;
+  } else {
+    ds_forecast_kernel<false><<<grid, 128, 0, s>>>(*t, f);
+    ds_forecast_scan_kernel<<<1, kScanThreads, 0, s>>>(h->fc, t->n_ds, h->step_capacity, h->want_steps ? 1 : 0, h->totals);
+    launched = 2;
+  }
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    *cuda_err = (int)e;
+    return -1;
+  }
+  return launched;
 }
 
 int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s, int* cuda_err) {

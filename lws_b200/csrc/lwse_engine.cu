@@ -122,6 +122,20 @@ struct DsTickHost {
   uint32_t n_lws;
 };
 int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s, int* cuda_err);
+struct DsForecastHost {
+  lwse_ds_revrole_rec* rows;
+  lwse_ds_out* s_ds_out;
+  lwse_ds_role_out* s_role_out;
+  lwse_ds_revrole_out* s_revrole_out;
+  lwse_ds_forecast* fc;
+  lwse_ds_forecast_role* fc_role;
+  lwse_ds_role_out* steps;  // the write pass's rows (device scratch)
+  uint32_t step_capacity;
+  bool want_steps;  // a trajectory is asked for: the scan marks what does not fit in step_capacity
+  unsigned long long* totals;
+};
+int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s,
+                       int* cuda_err);
 // lwse_sha1_kernels.cu
 int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,
                 int sm_count, cudaStream_t s, int* cuda_err);
@@ -311,6 +325,10 @@ struct lwse_engine {
   bool rd_linked = false;            // a link patch arrived since the DS load: ticks run the linked sweep
   cudaEvent_t ev_ds_link = nullptr;  // the engine's stream at the start of a linked DS tick
   lwse_ds_tick_info last_ds_info{};  // lwse_ds_resident_tick_info
+  // rollout forecast (lwse_ds_forecast_*): a private copy of the revision-role rows, the replay's sweep
+  // outputs, the forecast rows and the trajectory; never the DS tick's buffers
+  DevBuf fc_rows, fc_ds_out, fc_role_out, fc_revrole_out, fc_ds, fc_roles, fc_steps, fc_totals;
+  PinBuf fc_words;                   // the two totals, copied back
   bool r_swept = false;              // r_lws_out holds the results of the resident LWS rows: a sweep was enqueued
                                      // since lwse_resident_load and since any LWS-row patch without a sweep
   DevBuf sha_bytes, sha_offsets, sha_digests, sha_ints;
@@ -527,10 +545,11 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->arena_mirror, &e->stage_mirror, &e->chg_dev, &e->tdesc_dev,
                       &e->rd_ds, &e->rd_roles, &e->rd_revroles, &e->rd_out[0], &e->rd_out[1], &e->rd_role_out[0],
                       &e->rd_role_out[1], &e->rd_revrole_out[0], &e->rd_revrole_out[1], &e->rd_marks, &e->rd_ones,
-                      &e->rd_counters, &e->rd_stage_dev, &e->rd_links};
+                      &e->rd_counters, &e->rd_stage_dev, &e->rd_links, &e->fc_rows, &e->fc_ds_out, &e->fc_role_out,
+                      &e->fc_revrole_out, &e->fc_ds, &e->fc_roles, &e->fc_steps, &e->fc_totals};
     if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
     for (DevBuf* b : bufs) b->release();
-    PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc, &e->rd_pin, &e->rd_stage};
+    PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc, &e->rd_pin, &e->rd_stage, &e->fc_words};
     for (PinBuf* b : pins) b->release();
     if (e->ev_place) cudaEventDestroy(e->ev_place);
     if (e->h_rounds) cudaFreeHost(e->h_rounds);
@@ -2565,6 +2584,110 @@ LWSE_API int lwse_ds_resident_tick_info(lwse_engine* e, lwse_ds_tick_info* info)
   std::lock_guard<std::mutex> lock(e->mu);
   *info = e->last_ds_info;
   return LWSE_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Rollout forecast
+// ---------------------------------------------------------------------------
+static int check_forecast_out(const lwse_ds_forecast_out* out, uint32_t n_ds, uint32_t n_roles) {
+  if (!out || (n_ds && !out->ds) || (n_roles && !out->roles)) return LWSE_ERR_INVALID_ARG;
+  return LWSE_OK;
+}
+
+// The forecast of the device tables `d` (sizes in d), on stream s, into the host outputs `out`.
+// Everything it writes on the device is its own scratch; returns once `out` is filled.  The summary
+// pass and the scan run first; the trajectory buffer is then sized by the rows that fit (not by
+// step_capacity), so scratch grows only when a forecast needs more than any before it.
+static int forecast_locked(lwse_engine* e, const lwse_ds_tables& d, lwse_ds_forecast_out* out, cudaStream_t s) {
+  const uint32_t cap = out->steps ? out->step_capacity : 0u;
+  LWSE_CUDA(e, e->fc_rows.reserve((size_t)d.n_revroles * sizeof(lwse_ds_revrole_rec) + 16));
+  LWSE_CUDA(e, e->fc_ds_out.reserve((size_t)d.n_ds * sizeof(lwse_ds_out) + 16));
+  LWSE_CUDA(e, e->fc_role_out.reserve((size_t)d.n_roles * sizeof(lwse_ds_role_out) + 16));
+  LWSE_CUDA(e, e->fc_revrole_out.reserve((size_t)d.n_revroles * sizeof(lwse_ds_revrole_out) + 16));
+  LWSE_CUDA(e, e->fc_ds.reserve((size_t)d.n_ds * sizeof(lwse_ds_forecast) + 16));
+  LWSE_CUDA(e, e->fc_roles.reserve((size_t)d.n_roles * sizeof(lwse_ds_forecast_role) + 16));
+  LWSE_CUDA(e, e->fc_totals.reserve(16));
+  LWSE_CUDA(e, e->fc_words.reserve(16));
+  const size_t b_fc = (size_t)d.n_ds * sizeof(lwse_ds_forecast), b_fr = (size_t)d.n_roles * sizeof(lwse_ds_forecast_role);
+  // role rows of no valid DS read as zero
+  if (b_fr) LWSE_CUDA(e, cudaMemsetAsync(e->fc_roles.p, 0, b_fr, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->fc_totals.p, 0, 16, s));
+  lwse::DsForecastHost h{(lwse_ds_revrole_rec*)e->fc_rows.p, (lwse_ds_out*)e->fc_ds_out.p,
+                         (lwse_ds_role_out*)e->fc_role_out.p, (lwse_ds_revrole_out*)e->fc_revrole_out.p,
+                         (lwse_ds_forecast*)e->fc_ds.p, (lwse_ds_forecast_role*)e->fc_roles.p,
+                         nullptr, cap, out->steps != nullptr, (unsigned long long*)e->fc_totals.p};
+  int cuda_err = 0;
+  int launched = lwse::launch_ds_forecast(&d, &h, false, e->sm_count, s, &cuda_err);
+  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+  e->launches += (uint64_t)launched;
+  uint64_t* words = static_cast<uint64_t*>(e->fc_words.h);
+  LWSE_CUDA(e, cudaMemcpyAsync(words, e->fc_totals.p, 16, cudaMemcpyDeviceToHost, s));
+  if (b_fc) LWSE_CUDA(e, cudaMemcpyAsync(out->ds, e->fc_ds.p, b_fc, cudaMemcpyDeviceToHost, s));
+  if (b_fr) LWSE_CUDA(e, cudaMemcpyAsync(out->roles, e->fc_roles.p, b_fr, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  // the DS whose rows fit come first in DS order: the written rows are [0, n_steps_written), and
+  // n_steps_written <= step_capacity
+  const uint32_t written = d.n_ds ? (uint32_t)words[1] : 0u;
+  const uint64_t needed = d.n_ds ? words[0] : 0u;
+  if (written) {
+    LWSE_CUDA(e, e->fc_steps.reserve((size_t)written * sizeof(lwse_ds_role_out) + 16));
+    h.steps = (lwse_ds_role_out*)e->fc_steps.p;
+    launched = lwse::launch_ds_forecast(&d, &h, true, e->sm_count, s, &cuda_err);
+    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+    e->launches += (uint64_t)launched;
+    LWSE_CUDA(e, cudaMemcpyAsync(out->steps, e->fc_steps.p, (size_t)written * sizeof(lwse_ds_role_out),
+                                 cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaStreamSynchronize(s));
+  }
+  out->n_steps_written = written;
+  out->n_steps_needed = needed;
+  return LWSE_OK;
+}
+
+LWSE_API int lwse_ds_forecast_host(lwse_engine* e, const lwse_ds_tables* h, lwse_ds_forecast_out* out) {
+  if (!e || !h) return LWSE_ERR_INVALID_ARG;
+  if ((h->n_ds && !h->ds) || (h->n_roles && !h->roles) || (h->n_revroles && !h->revroles)) return LWSE_ERR_INVALID_ARG;
+  if (!aligned16(h->ds) || !aligned16(h->roles) || !aligned16(h->revroles)) return LWSE_ERR_INVALID_ARG;
+  int rc = check_forecast_out(out, h->n_ds, h->n_roles);
+  if (rc != LWSE_OK) return rc;
+  std::lock_guard<std::mutex> lock(e->mu);
+  DeviceGuard guard(e->device);
+  cudaStream_t s = e->stream;
+  const size_t b_ds = (size_t)h->n_ds * sizeof(lwse_ds_rec), b_ro = (size_t)h->n_roles * sizeof(lwse_ds_role_rec),
+               b_rr = (size_t)h->n_revroles * sizeof(lwse_ds_revrole_rec);
+  LWSE_CUDA(e, e->ds.reserve(b_ds + 16));
+  LWSE_CUDA(e, e->ds_roles.reserve(b_ro + 16));
+  LWSE_CUDA(e, e->ds_revroles.reserve(b_rr + 16));
+  if (b_ds) LWSE_CUDA(e, cudaMemcpyAsync(e->ds.p, h->ds, b_ds, cudaMemcpyHostToDevice, s));
+  if (b_ro) LWSE_CUDA(e, cudaMemcpyAsync(e->ds_roles.p, h->roles, b_ro, cudaMemcpyHostToDevice, s));
+  if (b_rr) LWSE_CUDA(e, cudaMemcpyAsync(e->ds_revroles.p, h->revroles, b_rr, cudaMemcpyHostToDevice, s));
+  lwse_ds_tables d{};
+  d.ds = (const lwse_ds_rec*)e->ds.p;
+  d.n_ds = h->n_ds;
+  d.roles = (const lwse_ds_role_rec*)e->ds_roles.p;
+  d.n_roles = h->n_roles;
+  d.revroles = (const lwse_ds_revrole_rec*)e->ds_revroles.p;
+  d.n_revroles = h->n_revroles;
+  return forecast_locked(e, d, out, s);
+}
+
+// On the DS stream, over rd_ds / rd_roles / rd_revroles as the last DS tick left them; the tick's
+// output sets, marks, counters, pinned mirrors and links are not touched.
+LWSE_API int lwse_ds_resident_forecast(lwse_engine* e, lwse_ds_forecast_out* out) {
+  if (!e) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->rd_loaded) return LWSE_ERR_NOT_READY;
+  int rc = check_forecast_out(out, e->rdn_ds, e->rdn_roles);
+  if (rc != LWSE_OK) return rc;
+  DeviceGuard guard(e->device);
+  lwse_ds_tables d{};
+  d.ds = (const lwse_ds_rec*)e->rd_ds.p;
+  d.n_ds = e->rdn_ds;
+  d.roles = (const lwse_ds_role_rec*)e->rd_roles.p;
+  d.n_roles = e->rdn_roles;
+  d.revroles = (const lwse_ds_revrole_rec*)e->rd_revroles.p;
+  d.n_revroles = e->rdn_revroles;
+  return forecast_locked(e, d, out, e->ds_stream);
 }
 
 // ---------------------------------------------------------------------------

@@ -344,3 +344,24 @@ class DsIncrementalEncoder:
     def old_revisions(self, row: int) -> list:
         """The old revisions of the DS at `row` in revision-role row order (the target revision follows them)."""
         return self._meta[int(row)][1]
+
+    def forecast_of(self, forecast: dict, namespace: str, name: str) -> dict:
+        """One DS's rollout forecast (``Engine.ds_resident_forecast`` over ``tables()``), by name:
+        the flags, cycle and step counts, and per role name its peak replicas, availability floor,
+        final old / new counts and trajectory [(old, new), ...] (empty without trajectory rows, or
+        when the DS's rows did not fit)."""
+        row = self.ds_row(namespace, name)
+        fc = forecast["ds"][row]
+        role_base = int(self.ds[row]["role_base"])
+        names = self.role_names(row)
+        n, base, n_steps = len(names), int(fc["step_base"]), int(fc["n_steps"])
+        steps = forecast.get("steps")
+        have = steps is not None and not fc["flags"] & R.DSF_TRUNCATED and base + n_steps * n <= len(steps)
+        roles = {}
+        for i, role in enumerate(names):
+            r = forecast["roles"][role_base + i]
+            traj = ([(int(steps[base + s * n + i]["next_old"]), int(steps[base + s * n + i]["next_new"]))
+                     for s in range(n_steps)] if have else [])
+            roles[role] = {"peak_replicas": int(r["peak_replicas"]), "floor_available": int(r["floor_available"]),
+                           "final_old": int(r["final_old"]), "final_new": int(r["final_new"]), "trajectory": traj}
+        return {"flags": int(fc["flags"]), "cycles": int(fc["cycles"]), "n_steps": n_steps, "roles": roles}

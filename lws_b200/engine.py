@@ -86,6 +86,8 @@ SYMBOLS = {
     "lwse_ds_resident_load": ([C.c_void_p, C.POINTER(R.DsTables)], C.c_int),
     "lwse_ds_resident_tick": ([C.c_void_p, C.POINTER(R.PatchSeg), C.c_uint32, C.POINTER(R.DsChanges)], C.c_int),
     "lwse_ds_resident_tick_info": ([C.c_void_p, C.POINTER(R.DsTickInfo)], C.c_int),
+    "lwse_ds_forecast_host": ([C.c_void_p, C.POINTER(R.DsTables), C.POINTER(R.DsForecastOut)], C.c_int),
+    "lwse_ds_resident_forecast": ([C.c_void_p, C.POINTER(R.DsForecastOut)], C.c_int),
     "lwse_group_keys_host": ([C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_subgroup_keys_host": (
         [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
@@ -543,6 +545,44 @@ class Engine:
         self._check(lib().lwse_ds_resident_tick_info(self._h, C.byref(info)))
         return {"linked": bool(info.linked), "rows_from_lws": info.rows_from_lws,
                 "rows_fallback": info.rows_fallback, "lws_ticks": info.lws_ticks}
+
+    # ------------------------------------------------------- rollout forecast
+    def _ds_forecast(self, call, n_ds, n_roles, steps, step_capacity):
+        fc = R.aligned_empty(n_ds, R.DS_FORECAST)
+        fr = R.aligned_empty(n_roles, R.DS_FORECAST_ROLE)
+        traj = None
+        if steps:
+            if step_capacity is None:  # every DS's rows fit: at most the cycle cap per DS (sized by a first pass)
+                probe = R.DsForecastOut(R.ptr(fc) if n_ds else None, R.ptr(fr) if n_roles else None, None, 0, 0, 0)
+                self._check(call(probe))
+                step_capacity = int(probe.n_steps_needed)
+            traj = R.aligned_empty(max(int(step_capacity), 1), R.DS_ROLE_OUT)
+        out = R.DsForecastOut(R.ptr(fc) if n_ds else None, R.ptr(fr) if n_roles else None,
+                              R.ptr(traj) if traj is not None else None, int(step_capacity or 0), 0, 0)
+        self._check(call(out))
+        return {"ds": fc, "roles": fr, "steps": traj[: out.n_steps_written] if traj is not None else None,
+                "n_steps_written": out.n_steps_written, "n_steps_needed": out.n_steps_needed}
+
+    def ds_forecast_host(self, ds, roles, revroles, steps=True, step_capacity=None):
+        """lwse_ds_forecast_host: the rest of every DS rollout, replayed from these host tables with
+        every child ready before each cycle (lwse.h, "rollout forecast").  → dict: ``ds`` (DS_FORECAST
+        per DS), ``roles`` (DS_FORECAST_ROLE per role row), ``steps`` (DS_ROLE_OUT {old, new} trajectory
+        rows, DS d's at ``ds[d]["step_base"]``; None when ``steps`` is False), ``n_steps_written``,
+        ``n_steps_needed``.  ``step_capacity`` None sizes the buffer so that every trajectory fits: it
+        runs a summaries-only call first (a second summary pass) to learn the rows needed; callers
+        that forecast repeatedly pass a capacity instead."""
+        assert ds.dtype == R.DS_REC and roles.dtype == R.DS_ROLE_REC and revroles.dtype == R.DS_REVROLE_REC
+        t = R.DsTables(R.ptr(ds) if len(ds) else None, len(ds), R.ptr(roles) if len(roles) else None, len(roles),
+                       R.ptr(revroles) if len(revroles) else None, len(revroles), None, None, None)
+        return self._ds_forecast(lambda o: lib().lwse_ds_forecast_host(self._h, C.byref(t), C.byref(o)),
+                                 len(ds), len(roles), steps, step_capacity)
+
+    def ds_resident_forecast(self, steps=True, step_capacity=None):
+        """lwse_ds_resident_forecast: as ``ds_forecast_host`` over the resident DS tables as the last DS
+        tick left them.  Changes no DS tick output and never waits for the LeaderWorkerSet ticks."""
+        n_ds, n_roles, _ = getattr(self, "_ds_shape", (0, 0, 0))
+        return self._ds_forecast(lambda o: lib().lwse_ds_resident_forecast(self._h, C.byref(o)),
+                                 n_ds, n_roles, steps, step_capacity)
 
     # ------------------------------------------------------------- group keys
     def group_keys_host(self, strings) -> np.ndarray:

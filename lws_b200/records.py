@@ -284,6 +284,23 @@ DS_REVROLE_OUT = np.dtype("<i4")
 DS_LINK = np.dtype([("lws_uid_hash", "<u8"), ("lws_row", "<u4"), ("reserved", "<u4")], align=False)
 assert DS_LINK.itemsize == 16
 
+# rollout forecast (lwse_ds_forecast_*): per DS, per role row; trajectory rows are DS_ROLE_OUT {old, new}
+DS_FORECAST = np.dtype(
+    [("flags", "<u4"), ("cycles", "<u4"), ("step_base", "<u4"), ("n_steps", "<u4")], align=False
+)
+assert DS_FORECAST.itemsize == 16
+DS_FORECAST_ROLE = np.dtype(
+    [("peak_replicas", "<i4"), ("floor_available", "<i4"), ("final_old", "<i4"), ("final_new", "<i4")], align=False
+)
+assert DS_FORECAST_ROLE.itemsize == 16
+DSF_ROLLING = 1 << 0
+DSF_WAITING = 1 << 1
+DSF_DONE = 1 << 2
+DSF_UNFINISHED = 1 << 3
+DSF_TRUNCATED = 1 << 4
+DSF_BAD_TABLE = 1 << 6
+DS_FORECAST_MAX_CYCLES = 65536
+
 
 # --------------------------------------------------------------------------- #
 # ctypes bundles (lwse_lws_tables / lwse_ds_tables / lwse_config)
@@ -403,6 +420,19 @@ class DsTickInfo(C.Structure):
         ("rows_fallback", C.c_uint32),
         ("reserved", C.c_uint32),
         ("lws_ticks", C.c_uint64),
+    ]
+
+
+class DsForecastOut(C.Structure):
+    """lwse_ds_forecast_out: where a forecast goes, and the trajectory rows it wrote / needed."""
+
+    _fields_ = [
+        ("ds", C.c_void_p),
+        ("roles", C.c_void_p),
+        ("steps", C.c_void_p),
+        ("step_capacity", C.c_uint32),
+        ("n_steps_written", C.c_uint32),
+        ("n_steps_needed", C.c_uint64),
     ]
 
 
