@@ -530,6 +530,101 @@ typedef struct lwse_node_info {
 } lwse_node_info;
 LWSE_API int lwse_resident_node_info(lwse_engine* e, lwse_node_info* info);
 
+/* ---- rolling-update forecast ----------------------------------------------------------------
+ * The rest of every LeaderWorkerSet rolling update, replayed on the device from the current LWS rows
+ * and group results: the controller writes (partition, replicas) to the leader StatefulSet
+ * (rollingUpdateParameters, leaderworkerset_controller.go:280-373, with the partition walk :643-673),
+ * and the model is an ideal StatefulSet controller and kubelet: after each write every group the
+ * StatefulSet would roll is ready.  The replay runs on a private copy of the object's flag bytes (the
+ * low five bits of lwse_group_out.flags: STATE_READY, STATE_UPDATED, COUNTED, COND_READY, COND_UPDATED).
+ *
+ * An object has C = max(group_count, sts_replicas, replicas + surge) slots, surge being maxSurge scaled
+ * and clamped to [0, replicas] (:307); slot idx < group_count starts as group idx's flag byte, the
+ * others (room for surge groups) at 0.  One cycle:
+ *   1. pass: the LWS pass of lwse_sweep_lws_* (the same device code) over the private row and slots
+ *      gives (p', n') = (sts_partition, sts_replicas) and the status;
+ *   2. apply: the row takes STS_EXISTS, ANNOT_VALID, sts_replicas = n', sts_partition = p',
+ *      sts_replicas_annotation = replicas and loses UPDATED (what the server-side apply writes,
+ *      :375-411, :831-853); slot idx >= n' becomes 0 (the group is gone); slot idx < n' becomes
+ *      STATE_READY|COUNTED|COND_READY, plus STATE_UPDATED|COND_UPDATED when idx >= p' or the old byte
+ *      had COND_UPDATED (only ordinals >= partition take the new revision; a missing pod below the
+ *      partition is recreated at the old one);
+ *   3. stop at the first apply that changes no slot and no row field, or after the cycle cap
+ *      min(2*C + 8, LWSE_LWS_FORECAST_MAX_CYCLES), or when n' > C (possible only with a negative
+ *      maxUnavailable): the replay is then UNFINISHED.
+ * Spec edits during the replay are not modelled.  The pass of the current rows runs first; an object
+ * whose pass reports LWSE_LOUT_RUP_ERROR, _STATUS_ERROR or _IRREGULAR, or whose C exceeds
+ * LWSE_LWS_FORECAST_MAX_SLOTS, runs no cycle (LWSE_LWSF_NOT_FORECAST); one with LWSE_LOUT_BAD_TABLE
+ * gets LWSE_LWSF_BAD_TABLE.  Both leave every other field 0 except step_base, which holds the running
+ * offset like every object's (such an object has no rows). */
+#define LWSE_LWS_FORECAST_MAX_CYCLES 65536u
+#define LWSE_LWS_FORECAST_MAX_SLOTS (1u << 20)
+
+typedef struct lwse_lws_forecast { /* per LWS, 32 B */
+  uint32_t flags;            /* LWSE_LWSF_* */
+  uint32_t cycles;           /* cycles whose apply changed something (= n_steps)                      */
+  uint32_t step_base;        /* first trajectory row of this object: rows of the objects before it, in
+                                row order (saturates at 0xFFFFFFFF)                                    */
+  uint32_t n_steps;          /* trajectory rows of this object                                         */
+  int32_t peak_sts_replicas; /* max of the StatefulSet's replicas now (0 without one) and every n'     */
+  int32_t floor_ready;       /* min of the ready count now (the pass of the current rows) and, for each
+                                cycle, the slots idx < n' that are COUNTED and COND_READY and are not
+                                being replaced (idx >= p' without COND_UPDATED) before its apply       */
+  int32_t final_partition;   /* (p', n') of the last pass: what the StatefulSet holds when the replay  */
+  int32_t final_replicas;    /* stopped, what the controller writes next when it did not               */
+} lwse_lws_forecast;
+
+#define LWSE_LWSF_ROLLING (1u << 0)      /* the pass of the current rows is UpdateInProgress            */
+#define LWSE_LWSF_WAITING (1u << 1)      /* the first cycle assumes groups that are not ready now become
+                                            ready: its apply set STATE_READY or COND_READY on a slot    */
+#define LWSE_LWSF_DONE (1u << 2)         /* stopped, and the last pass has LWSE_LOUT_UPDATE_DONE        */
+#define LWSE_LWSF_UNFINISHED (1u << 3)   /* stopped by the cycle cap or by n' > C                       */
+#define LWSE_LWSF_TRUNCATED (1u << 4)    /* its trajectory did not fit in step_capacity: none of its
+                                            rows were written (the summary is exact)                    */
+#define LWSE_LWSF_HELD (1u << 5)         /* stopped with final_partition > 0 equal to the spec's
+                                            rollingUpdateConfiguration.partition (the clamp :285-288)   */
+#define LWSE_LWSF_BAD_TABLE (1u << 6)    /* as LWSE_LOUT_BAD_TABLE                                      */
+#define LWSE_LWSF_NOT_FORECAST (1u << 7) /* see above                                                   */
+
+/* One trajectory row: the pass after a cycle whose apply changed something (16 B).  An object's
+ * n_steps rows are contiguous at step_base, in cycle order; the last one is the state the replay
+ * stopped in (for a stopped replay). */
+typedef struct lwse_lws_forecast_step {
+  int32_t partition;
+  int32_t sts_replicas;
+  int32_t ready_replicas;
+  int32_t updated_replicas;
+} lwse_lws_forecast_step;
+
+/* An object whose rows do not all fit below step_capacity gets LWSE_LWSF_TRUNCATED and writes none;
+ * no row at or beyond step_capacity is written, and no object writes outside its own n_steps rows. */
+typedef struct lwse_lws_forecast_out {
+  lwse_lws_forecast* lws;           /* [n_lws]                                                */
+  lwse_lws_forecast_step* steps;    /* [step_capacity], or NULL: summaries only               */
+  uint32_t step_capacity;
+  uint32_t n_steps_written;         /* out: trajectory rows written                           */
+  uint64_t n_steps_needed;          /* out: rows every object's trajectory needs              */
+} lwse_lws_forecast_out;
+
+/* Stateless: n_lws object rows and the n_groups group result rows of a sweep of the same tables
+ * (only the low five flag bits are read), host memory.  LWSE_ERR_INVALID_ARG for NULL or misaligned
+ * tables or outputs; LWSE_ERR_UNSUPPORTED when the objects' slots (C rounded up to 8, summed) reach 2^31.
+ * The kernels check every access to their private slots and to the trajectory rows against the sizes
+ * the scans gave; an access they refuse would be an engine defect, and fails the call with LWSE_ERR_CUDA
+ * and lwse_last_cuda_error() == cudaErrorAssert (710). */
+LWSE_API int lwse_lws_forecast_host(lwse_engine* e, const lwse_lws_rec* lws, uint32_t n_lws,
+                                    const lwse_group_out* group_out, uint32_t n_groups, lwse_lws_forecast_out* out);
+/* Over the resident LWS rows and the resident group results.  The call snapshots both on the engine's
+ * stream (device-to-device copies behind the most recently submitted tick, in flight or not) and
+ * replays on a stream of its own, with scratch of its own: it never waits for, drains or drops a tick,
+ * and touches no tick graph, arena, change list or output.  The scratch only grows (a call that needs
+ * more than any before allocates, which waits for the device as cudaMalloc does).  LWSE_ERR_NOT_READY
+ * before lwse_resident_load, and while the group results do not belong to the resident rows: after a
+ * load, and after a patch of LWS, group or pod rows made without a sweep (lwse_resident_patch, or a
+ * tick with LWSE_TICK_NO_SWEEP), until the next sweep is enqueued.  LWSE_ERR_INVALID_ARG for NULL
+ * outputs; LWSE_ERR_UNSUPPORTED and LWSE_ERR_CUDA as for lwse_lws_forecast_host. */
+LWSE_API int lwse_resident_forecast(lwse_engine* e, lwse_lws_forecast_out* out);
+
 /* ------------------------------------------------------------------------- */
 /* Placement (build-defined spec — the reference has no node scoring)        */
 /* ------------------------------------------------------------------------- */

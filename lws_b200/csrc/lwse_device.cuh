@@ -121,6 +121,116 @@ __device__ __forceinline__ void pdl_launch_dependents() {
 }
 __device__ __forceinline__ void pdl_wait_prior() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
+// ---- the trajectory layout of the rollout forecasts (lwse_ds_forecast_*, lwse_lws_forecast_*) ----
+constexpr int kForecastScanThreads = 1024;
+
+// Exclusive prefix over one CTA of kForecastScanThreads threads of one value per thread.
+__device__ __forceinline__ unsigned long long cta_exclusive_scan(const unsigned long long sum) {
+  __shared__ unsigned long long s_warp[kForecastScanThreads / 32];
+  const unsigned lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  unsigned long long incl = sum;
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+    if ((int)lane >= o) incl += v;
+  }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    unsigned long long w = s_warp[lane], wi = w;
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long v = __shfl_up_sync(0xFFFFFFFFu, wi, o);
+      if ((int)lane >= o) wi += v;
+    }
+    s_warp[lane] = wi - w;
+  }
+  __syncthreads();
+  return s_warp[warp] + incl - sum;
+}
+
+// An exclusive prefix over n items in three launches (Op::count(i) = item i's count):
+//   scan_block_sums_kernel  one CTA per kForecastScanThreads consecutive items (coalesced): their sum
+//   scan_carry_kernel       one CTA: the block sums become exclusive block offsets; *total = the sum
+//   scan_apply_kernel       every item's offset to Op::apply(i, offset, count), whose results are summed
+//                           into *acc (nullable; the sum of one warp must fit 32 bits)
+// sums: forecast_scan_words(n) words of device scratch.
+inline uint32_t forecast_scan_words(uint32_t n) { return (n + kForecastScanThreads - 1) / kForecastScanThreads; }
+
+template <class Op>
+__global__ void __launch_bounds__(kForecastScanThreads) scan_block_sums_kernel(const Op op, uint32_t n,
+                                                                               unsigned long long* sums) {
+  const uint32_t i = blockIdx.x * kForecastScanThreads + threadIdx.x;
+  const unsigned long long v = i < n ? op.count(i) : 0ull;
+  const unsigned long long ex = cta_exclusive_scan(v);
+  if (threadIdx.x == kForecastScanThreads - 1) sums[blockIdx.x] = ex + v;
+}
+
+template <class Op>  // (only to give each user its own instance)
+__global__ void __launch_bounds__(kForecastScanThreads) scan_carry_kernel(unsigned long long* sums, uint32_t n_blocks,
+                                                                          unsigned long long* total) {
+  __shared__ unsigned long long s_chunk;
+  unsigned long long carry = 0;
+  for (uint32_t b0 = 0; b0 < n_blocks; b0 += kForecastScanThreads) {
+    const uint32_t b = b0 + threadIdx.x;
+    const unsigned long long v = b < n_blocks ? sums[b] : 0ull;
+    const unsigned long long ex = cta_exclusive_scan(v);
+    if (b < n_blocks) sums[b] = carry + ex;
+    if (threadIdx.x == kForecastScanThreads - 1) s_chunk = ex + v;
+    __syncthreads();
+    carry += s_chunk;
+    __syncthreads();  // (s_chunk and the scan's shared words are rewritten by the next chunk)
+  }
+  if (threadIdx.x == 0) *total = carry;
+}
+
+template <class Op>
+__global__ void __launch_bounds__(kForecastScanThreads) scan_apply_kernel(const Op op, uint32_t n,
+                                                                          const unsigned long long* sums,
+                                                                          unsigned long long* acc) {
+  const uint32_t i = blockIdx.x * kForecastScanThreads + threadIdx.x;
+  const unsigned long long v = i < n ? op.count(i) : 0ull;
+  const unsigned long long base = cta_exclusive_scan(v) + sums[blockIdx.x];
+  const unsigned long long r = i < n ? op.apply(i, base, v) : 0ull;
+  if (acc != nullptr) {
+    const unsigned w = __reduce_add_sync(0xFFFFFFFFu, (unsigned)r);
+    if ((threadIdx.x & 31u) == 0 && w) atomicAdd(acc, (unsigned long long)w);
+  }
+}
+
+template <class Op>
+inline cudaError_t launch_forecast_scan(const Op& op, uint32_t n, unsigned long long* sums, unsigned long long* total,
+                                        unsigned long long* acc, cudaStream_t s) {
+  const uint32_t blocks = forecast_scan_words(n);
+  if (blocks) scan_block_sums_kernel<Op><<<blocks, kForecastScanThreads, 0, s>>>(op, n, sums);
+  scan_carry_kernel<Op><<<1, kForecastScanThreads, 0, s>>>(sums, blocks, total);
+  if (blocks) scan_apply_kernel<Op><<<blocks, kForecastScanThreads, 0, s>>>(op, n, sums, acc);
+  return cudaGetLastError();
+}
+
+// The trajectory layout: step_base (a row count after the summary pass) becomes the exclusive prefix over
+// the objects in row order, saturated to 32 bits; with a trajectory buffer, objects whose rows end beyond
+// step_capacity get kTruncated.  Total: rows needed; acc: rows written (< 2^32: bounded by capacity).
+template <class Rec, uint32_t kTruncated>
+struct StepLayoutOp {
+  Rec* fc;
+  uint32_t capacity;
+  int has_steps;
+  __device__ __forceinline__ unsigned long long count(uint32_t i) const { return fc[i].step_base; }
+  __device__ __forceinline__ unsigned long long apply(uint32_t i, unsigned long long base,
+                                                      unsigned long long rows) const {
+    Rec c = fc[i];
+    c.step_base = (uint32_t)min(base, 0xFFFFFFFFull);
+    unsigned long long written = 0;
+    if (has_steps && rows) {
+      if (base + rows > capacity)
+        c.flags |= kTruncated;
+      else
+        written = rows;
+    }
+    fc[i] = c;
+    return written;
+  }
+};
+
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
                               bool pdl, Args&&... args) {

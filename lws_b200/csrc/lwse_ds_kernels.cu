@@ -677,55 +677,6 @@ __global__ void __launch_bounds__(128) ds_forecast_kernel(const lwse_ds_tables i
     ds_forecast_one<kWrite>(in, f, d);
 }
 
-// One CTA: step_base (a row count after the summary pass) becomes the exclusive prefix over the DS in
-// row order; with a trajectory buffer, DS whose rows end beyond step_capacity get TRUNCATED.
-// totals[0] = rows needed, totals[1] = rows written.
-constexpr int kScanThreads = 1024;
-__global__ void __launch_bounds__(kScanThreads) ds_forecast_scan_kernel(lwse_ds_forecast* fc, uint32_t n_ds,
-                                                                        uint32_t capacity, int has_steps,
-                                                                        unsigned long long* totals) {
-  __shared__ unsigned long long s_warp[kScanThreads / 32];
-  const uint32_t per = (n_ds + kScanThreads - 1) / kScanThreads;
-  const uint32_t lo = min(n_ds, threadIdx.x * per), hi = min(n_ds, lo + per);
-  unsigned long long sum = 0;
-  for (uint32_t d = lo; d < hi; d++) sum += fc[d].step_base;
-  // block-wide exclusive scan of the per-thread sums
-  const unsigned lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  unsigned long long incl = sum;
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned long long v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-    if ((int)lane >= o) incl += v;
-  }
-  if (lane == 31) s_warp[warp] = incl;
-  __syncthreads();
-  if (warp == 0) {
-    unsigned long long w = s_warp[lane], wi = w;
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned long long v = __shfl_up_sync(0xFFFFFFFFu, wi, o);
-      if ((int)lane >= o) wi += v;
-    }
-    s_warp[lane] = wi - w;
-  }
-  __syncthreads();
-  unsigned long long base = s_warp[warp] + incl - sum, written = 0;
-  for (uint32_t d = lo; d < hi; d++) {
-    lwse_ds_forecast c = fc[d];
-    const unsigned long long rows = c.step_base;
-    c.step_base = (uint32_t)min(base, 0xFFFFFFFFull);
-    if (has_steps && rows) {
-      if (base + rows > capacity)
-        c.flags |= LWSE_DSF_TRUNCATED;
-      else
-        written += rows;
-    }
-    fc[d] = c;
-    base += rows;
-  }
-  if (threadIdx.x == kScanThreads - 1) totals[0] = base;
-  written = __reduce_add_sync(0xFFFFFFFFu, (unsigned)written);  // (< 2^32: bounded by capacity)
-  if (lane == 0 && written) atomicAdd(totals + 1, written);
-}
-
 struct DsForecastHost {  // (lwse_engine.cu)
   lwse_ds_revrole_rec* rows;
   lwse_ds_out* s_ds_out;
@@ -756,8 +707,10 @@ int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool wr
     launched = 1;
   } else {
     ds_forecast_kernel<false><<<grid, 128, 0, s>>>(*t, f);
-    ds_forecast_scan_kernel<<<1, kScanThreads, 0, s>>>(h->fc, t->n_ds, h->step_capacity, h->want_steps ? 1 : 0, h->totals);
-    launched = 2;
+    // (totals[2..] holds the scan's block sums)
+    launch_forecast_scan(StepLayoutOp<lwse_ds_forecast, LWSE_DSF_TRUNCATED>{h->fc, h->step_capacity, h->want_steps ? 1 : 0},
+                         t->n_ds, h->totals + 2, h->totals + 0, h->totals + 1, s);
+    launched = 4;
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {

@@ -136,6 +136,24 @@ struct DsForecastHost {
 };
 int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s,
                        int* cuda_err);
+// lwse_lws_forecast_kernels.cu
+struct LwsForecastHost {
+  const lwse_lws_rec* lws;
+  uint32_t n_lws;
+  const lwse_group_out* group_out;
+  uint32_t n_groups;
+  unsigned long long* slot_off;
+  uint8_t* slots;
+  uint32_t n_slots;
+  lwse_lws_forecast* fc;
+  lwse_lws_forecast_step* steps;  // the write pass's rows (device scratch)
+  uint32_t steps_rows;
+  uint32_t step_capacity;
+  bool want_steps;  // a trajectory is asked for: the scan marks what does not fit in step_capacity
+  unsigned long long* totals;
+};
+int launch_lws_forecast_slots(const LwsForecastHost* h, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_lws_forecast(const LwsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s, int* cuda_err);
 // lwse_sha1_kernels.cu
 int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,
                 int sm_count, cudaStream_t s, int* cuda_err);
@@ -331,6 +349,14 @@ struct lwse_engine {
   PinBuf fc_words;                   // the two totals, copied back
   bool r_swept = false;              // r_lws_out holds the results of the resident LWS rows: a sweep was enqueued
                                      // since lwse_resident_load and since any LWS-row patch without a sweep
+  bool r_groups_swept = false;       // r_group_out holds the results of the resident rows: as r_swept, for
+                                     // patches of LWS, group and pod rows
+  // rolling-update forecast (lwse_lws_forecast_*): a snapshot of the LWS rows and group results, the private
+  // flag slots, the forecast rows and the trajectory, on a stream of its own; never a tick's buffers
+  cudaStream_t lf_stream = nullptr;
+  cudaEvent_t ev_lf = nullptr;       // the engine's stream where a resident forecast takes its snapshot
+  DevBuf lf_lws, lf_group_out, lf_slot_off, lf_slots, lf_fc, lf_steps, lf_totals;
+  PinBuf lf_words;                   // the three totals, copied back
   DevBuf sha_bytes, sha_offsets, sha_digests, sha_ints;
   uint32_t* h_rounds = nullptr;  // pinned
   // peer exchange of the multi-GPU placement step (lwse_exchange_*)
@@ -546,10 +572,12 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->rd_ds, &e->rd_roles, &e->rd_revroles, &e->rd_out[0], &e->rd_out[1], &e->rd_role_out[0],
                       &e->rd_role_out[1], &e->rd_revrole_out[0], &e->rd_revrole_out[1], &e->rd_marks, &e->rd_ones,
                       &e->rd_counters, &e->rd_stage_dev, &e->rd_links, &e->fc_rows, &e->fc_ds_out, &e->fc_role_out,
-                      &e->fc_revrole_out, &e->fc_ds, &e->fc_roles, &e->fc_steps, &e->fc_totals};
+                      &e->fc_revrole_out, &e->fc_ds, &e->fc_roles, &e->fc_steps, &e->fc_totals,
+                      &e->lf_lws, &e->lf_group_out, &e->lf_slot_off, &e->lf_slots, &e->lf_fc, &e->lf_steps, &e->lf_totals};
     if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
+    if (e->lf_stream) cudaStreamSynchronize(e->lf_stream);
     for (DevBuf* b : bufs) b->release();
-    PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc, &e->rd_pin, &e->rd_stage, &e->fc_words};
+    PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc, &e->rd_pin, &e->rd_stage, &e->fc_words, &e->lf_words};
     for (PinBuf* b : pins) b->release();
     if (e->ev_place) cudaEventDestroy(e->ev_place);
     if (e->h_rounds) cudaFreeHost(e->h_rounds);
@@ -566,6 +594,8 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
     if (e->pub_stream) cudaStreamDestroy(e->pub_stream);
     if (e->ds_stream) cudaStreamDestroy(e->ds_stream);
     if (e->ev_ds_link) cudaEventDestroy(e->ev_ds_link);
+    if (e->lf_stream) cudaStreamDestroy(e->lf_stream);
+    if (e->ev_lf) cudaEventDestroy(e->ev_lf);
     cudaStreamDestroy(e->side_stream);
     cudaStreamDestroy(e->stream);
   }
@@ -849,6 +879,7 @@ LWSE_API int lwse_resident_load(lwse_engine* e, const lwse_lws_tables* h) {
     if (drc != LWSE_OK) return drc;
   }
   e->r_swept = false;  // (the output rows are all-ones until the next sweep)
+  e->r_groups_swept = false;
   cudaStream_t s = e->stream;
   const size_t b_lws = (size_t)h->n_lws * sizeof(lwse_lws_rec), b_grp = (size_t)h->n_groups * sizeof(lwse_group_rec);
   const size_t b_pst = (size_t)h->n_pods * sizeof(lwse_pod_state), b_pid = (size_t)h->n_pods * sizeof(lwse_pod_ident);
@@ -1151,6 +1182,7 @@ LWSE_API int lwse_resident_patch(lwse_engine* e, lwse_table which, const uint32_
     if (nrc < 0) return nrc;
   }
   if (which == LWSE_TABLE_LWS) e->r_swept = false;  // r_lws_out no longer belongs to these LWS rows
+  if (which <= LWSE_TABLE_POD_IDENT) e->r_groups_swept = false;  // nor r_group_out to the group and pod rows
   bool wrote = false;
   const int rc = apply_patches_locked(e, &seg, 1, &wrote);
   if (rc != LWSE_OK) {
@@ -1748,8 +1780,10 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
   }
   // LWS rows patched without a sweep: r_lws_out no longer belongs to them (a row reused for another
   // object would pass the linked DS tick's uid test with the previous object's results)
-  for (uint32_t i = 0; !do_sweep && i < n_segs; i++)
+  for (uint32_t i = 0; !do_sweep && i < n_segs; i++) {
     if (segs[i].table == LWSE_TABLE_LWS && segs[i].n) e->r_swept = false;
+    if (segs[i].table <= LWSE_TABLE_POD_IDENT && segs[i].n) e->r_groups_swept = false;
+  }
   // The round's form, decided before any patch is applied (it is part of a tick graph's key).  A request
   // table grouped by namespace — and not ungrouped by this tick's patches — runs the namespace kernels as
   // they are; any other table runs them through the namespace index, rebuilt when the namespace column
@@ -2100,7 +2134,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
       gts.published = true;
       gts.wrote = has_patches;
       e->t_submitted++;
-      if (do_sweep) e->r_swept = true;
+      if (do_sweep) e->r_swept = e->r_groups_swept = true;
       e->main_unforked = !do_place && (e->main_unforked || has_patches);
       record_info(true);
       return LWSE_OK;
@@ -2142,7 +2176,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
   ts.published = published;
   ts.wrote = wrote || wrote_side;
   e->t_submitted++;
-  if (do_sweep) e->r_swept = true;
+  if (do_sweep) e->r_swept = e->r_groups_swept = true;
   e->main_unforked = !do_place && (e->main_unforked || wrote);
   record_info(false);
   return LWSE_OK;
@@ -2606,7 +2640,7 @@ static int forecast_locked(lwse_engine* e, const lwse_ds_tables& d, lwse_ds_fore
   LWSE_CUDA(e, e->fc_revrole_out.reserve((size_t)d.n_revroles * sizeof(lwse_ds_revrole_out) + 16));
   LWSE_CUDA(e, e->fc_ds.reserve((size_t)d.n_ds * sizeof(lwse_ds_forecast) + 16));
   LWSE_CUDA(e, e->fc_roles.reserve((size_t)d.n_roles * sizeof(lwse_ds_forecast_role) + 16));
-  LWSE_CUDA(e, e->fc_totals.reserve(16));
+  LWSE_CUDA(e, e->fc_totals.reserve(16 + (size_t)lwse::forecast_scan_words(d.n_ds) * 8));  // + the scan's block sums
   LWSE_CUDA(e, e->fc_words.reserve(16));
   const size_t b_fc = (size_t)d.n_ds * sizeof(lwse_ds_forecast), b_fr = (size_t)d.n_roles * sizeof(lwse_ds_forecast_role);
   // role rows of no valid DS read as zero
@@ -2688,6 +2722,119 @@ LWSE_API int lwse_ds_resident_forecast(lwse_engine* e, lwse_ds_forecast_out* out
   d.revroles = (const lwse_ds_revrole_rec*)e->rd_revroles.p;
   d.n_revroles = e->rdn_revroles;
   return forecast_locked(e, d, out, e->ds_stream);
+}
+
+// ---- rolling-update forecast of the LeaderWorkerSets ----
+// The forecast of device rows h.lws / h.group_out (sizes in h) on stream s into the host outputs `out`.
+// Everything it writes on the device is its own scratch; returns once `out` is filled.  The slot layout
+// comes first (it sizes the private flag bytes), then the summary pass and the scan; the trajectory
+// buffer is sized by the rows that fit (not by step_capacity), so scratch only grows when a forecast
+// needs more than any before it.
+static int lws_forecast_locked(lwse_engine* e, lwse::LwsForecastHost& h, lwse_lws_forecast_out* out, cudaStream_t s) {
+  h.step_capacity = out->steps ? out->step_capacity : 0u;
+  h.want_steps = out->steps != nullptr;
+  LWSE_CUDA(e, e->lf_slot_off.reserve((size_t)h.n_lws * 8 + 16));
+  LWSE_CUDA(e, e->lf_fc.reserve((size_t)h.n_lws * sizeof(lwse_lws_forecast) + 16));
+  LWSE_CUDA(e, e->lf_totals.reserve(32 + (size_t)lwse::forecast_scan_words(h.n_lws) * 8));  // + the scans' block sums
+  LWSE_CUDA(e, e->lf_words.reserve(32));
+  LWSE_CUDA(e, cudaMemsetAsync(e->lf_totals.p, 0, 32, s));
+  h.slot_off = (unsigned long long*)e->lf_slot_off.p;
+  h.fc = (lwse_lws_forecast*)e->lf_fc.p;
+  h.totals = (unsigned long long*)e->lf_totals.p;
+  uint64_t* words = static_cast<uint64_t*>(e->lf_words.h);
+  int cuda_err = 0;
+  int launched = lwse::launch_lws_forecast_slots(&h, e->sm_count, s, &cuda_err);
+  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+  e->launches += (uint64_t)launched;
+  LWSE_CUDA(e, cudaMemcpyAsync(words, e->lf_totals.p, 32, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint64_t n_slots = h.n_lws ? words[2] : 0u;
+  if (n_slots >= 0x80000000ull) return LWSE_ERR_UNSUPPORTED;  // the pass indexes its slots with int32 offsets
+  LWSE_CUDA(e, e->lf_slots.reserve((size_t)n_slots + 16));
+  h.slots = (uint8_t*)e->lf_slots.p;
+  h.n_slots = (uint32_t)n_slots;
+  h.steps = nullptr;
+  h.steps_rows = 0;
+  launched = lwse::launch_lws_forecast(&h, false, e->sm_count, s, &cuda_err);
+  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+  e->launches += (uint64_t)launched;
+  const size_t b_fc = (size_t)h.n_lws * sizeof(lwse_lws_forecast);
+  LWSE_CUDA(e, cudaMemcpyAsync(words, e->lf_totals.p, 32, cudaMemcpyDeviceToHost, s));
+  if (b_fc) LWSE_CUDA(e, cudaMemcpyAsync(out->lws, e->lf_fc.p, b_fc, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  // the objects whose rows fit come first in row order: the written rows are [0, n_steps_written)
+  if (words[3]) return fail_cuda(e, cudaErrorAssert);  // a bounds check refused an access (an engine defect)
+  const uint32_t written = h.n_lws ? (uint32_t)words[1] : 0u;
+  const uint64_t needed = h.n_lws ? words[0] : 0u;
+  if (written) {
+    LWSE_CUDA(e, e->lf_steps.reserve((size_t)written * sizeof(lwse_lws_forecast_step) + 16));
+    h.steps = (lwse_lws_forecast_step*)e->lf_steps.p;
+    h.steps_rows = written;
+    launched = lwse::launch_lws_forecast(&h, true, e->sm_count, s, &cuda_err);
+    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+    e->launches += (uint64_t)launched;
+    LWSE_CUDA(e, cudaMemcpyAsync(words, e->lf_totals.p, 32, cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaMemcpyAsync(out->steps, e->lf_steps.p, (size_t)written * sizeof(lwse_lws_forecast_step),
+                                 cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaStreamSynchronize(s));
+    if (words[3]) return fail_cuda(e, cudaErrorAssert);
+  }
+  out->n_steps_written = written;
+  out->n_steps_needed = needed;
+  return LWSE_OK;
+}
+
+static int lws_forecast_stream(lwse_engine* e) {
+  if (!e->lf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->lf_stream, cudaStreamNonBlocking));
+  return LWSE_OK;
+}
+
+LWSE_API int lwse_lws_forecast_host(lwse_engine* e, const lwse_lws_rec* lws, uint32_t n_lws,
+                                    const lwse_group_out* group_out, uint32_t n_groups, lwse_lws_forecast_out* out) {
+  if (!e || !out || (n_lws && (!lws || !out->lws)) || (n_groups && !group_out)) return LWSE_ERR_INVALID_ARG;
+  if (!aligned16(lws) || !aligned16(group_out)) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  DeviceGuard guard(e->device);
+  int rc = lws_forecast_stream(e);
+  if (rc != LWSE_OK) return rc;
+  cudaStream_t s = e->lf_stream;
+  const size_t b_lws = (size_t)n_lws * sizeof(lwse_lws_rec), b_go = (size_t)n_groups * sizeof(lwse_group_out);
+  LWSE_CUDA(e, e->lf_lws.reserve(b_lws + 16));
+  LWSE_CUDA(e, e->lf_group_out.reserve(b_go + 16));
+  if (b_lws) LWSE_CUDA(e, cudaMemcpyAsync(e->lf_lws.p, lws, b_lws, cudaMemcpyHostToDevice, s));
+  if (b_go) LWSE_CUDA(e, cudaMemcpyAsync(e->lf_group_out.p, group_out, b_go, cudaMemcpyHostToDevice, s));
+  lwse::LwsForecastHost h{};
+  h.lws = (const lwse_lws_rec*)e->lf_lws.p;
+  h.n_lws = n_lws;
+  h.group_out = (const lwse_group_out*)e->lf_group_out.p;
+  h.n_groups = n_groups;
+  return lws_forecast_locked(e, h, out, s);
+}
+
+// Snapshot on the engine's stream, replay on lf_stream: the ticks in flight keep running, and none of
+// their buffers is written.
+LWSE_API int lwse_resident_forecast(lwse_engine* e, lwse_lws_forecast_out* out) {
+  if (!e) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->r_loaded || !e->r_groups_swept) return LWSE_ERR_NOT_READY;
+  if (!out || (e->rn_lws && !out->lws)) return LWSE_ERR_INVALID_ARG;
+  DeviceGuard guard(e->device);
+  int rc = lws_forecast_stream(e);
+  if (rc != LWSE_OK) return rc;
+  if (!e->ev_lf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_lf, cudaEventDisableTiming));
+  const size_t b_lws = (size_t)e->rn_lws * sizeof(lwse_lws_rec), b_go = (size_t)e->rn_groups * sizeof(lwse_group_out);
+  LWSE_CUDA(e, e->lf_lws.reserve(b_lws + 16));
+  LWSE_CUDA(e, e->lf_group_out.reserve(b_go + 16));
+  if (b_lws) LWSE_CUDA(e, cudaMemcpyAsync(e->lf_lws.p, e->r_lws.p, b_lws, cudaMemcpyDeviceToDevice, e->stream));
+  if (b_go) LWSE_CUDA(e, cudaMemcpyAsync(e->lf_group_out.p, e->r_group_out.p, b_go, cudaMemcpyDeviceToDevice, e->stream));
+  LWSE_CUDA(e, cudaEventRecord(e->ev_lf, e->stream));
+  LWSE_CUDA(e, cudaStreamWaitEvent(e->lf_stream, e->ev_lf, 0));
+  lwse::LwsForecastHost h{};
+  h.lws = (const lwse_lws_rec*)e->lf_lws.p;
+  h.n_lws = e->rn_lws;
+  h.group_out = (const lwse_group_out*)e->lf_group_out.p;
+  h.n_groups = e->rn_groups;
+  return lws_forecast_locked(e, h, out, e->lf_stream);
 }
 
 // ---------------------------------------------------------------------------

@@ -88,6 +88,9 @@ SYMBOLS = {
     "lwse_ds_resident_tick_info": ([C.c_void_p, C.POINTER(R.DsTickInfo)], C.c_int),
     "lwse_ds_forecast_host": ([C.c_void_p, C.POINTER(R.DsTables), C.POINTER(R.DsForecastOut)], C.c_int),
     "lwse_ds_resident_forecast": ([C.c_void_p, C.POINTER(R.DsForecastOut)], C.c_int),
+    "lwse_lws_forecast_host": (
+        [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(R.LwsForecastOut)], C.c_int),
+    "lwse_resident_forecast": ([C.c_void_p, C.POINTER(R.LwsForecastOut)], C.c_int),
     "lwse_group_keys_host": ([C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_subgroup_keys_host": (
         [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
@@ -132,6 +135,15 @@ def lib() -> C.CDLL:
 
 def shard_of(uid_hash: int, n_shards: int) -> int:
     return lib().lwse_shard_of(uid_hash, n_shards)
+
+
+def _aligned16(a: np.ndarray) -> np.ndarray:
+    """``a`` itself when it is contiguous at a 16-byte aligned base, else an aligned copy."""
+    if a.flags.c_contiguous and a.ctypes.data % 16 == 0:
+        return a
+    b = R.aligned_empty(len(a), a.dtype)
+    b[:] = a
+    return b
 
 
 class Engine:
@@ -583,6 +595,45 @@ class Engine:
         n_ds, n_roles, _ = getattr(self, "_ds_shape", (0, 0, 0))
         return self._ds_forecast(lambda o: lib().lwse_ds_resident_forecast(self._h, C.byref(o)),
                                  n_ds, n_roles, steps, step_capacity)
+
+    # ------------------------------------------- rolling-update forecast (LWS)
+    def _lws_forecast(self, call, n_lws, steps, step_capacity):
+        fc = R.aligned_empty(n_lws, R.LWS_FORECAST)
+        traj = None
+        if steps:
+            if step_capacity is None:  # every object's rows fit (sized by a summaries-only call)
+                probe = R.LwsForecastOut(R.ptr(fc) if n_lws else None, None, 0, 0, 0)
+                self._check(call(probe))
+                step_capacity = int(probe.n_steps_needed)
+            traj = R.aligned_empty(max(int(step_capacity), 1), R.LWS_FORECAST_STEP)
+        out = R.LwsForecastOut(R.ptr(fc) if n_lws else None, R.ptr(traj) if traj is not None else None,
+                               int(step_capacity or 0), 0, 0)
+        self._check(call(out))
+        return {"lws": fc, "steps": traj[: out.n_steps_written] if traj is not None else None,
+                "n_steps_written": out.n_steps_written, "n_steps_needed": out.n_steps_needed}
+
+    def lws_forecast(self, lws, group_out, steps=True, step_capacity=None):
+        """lwse_lws_forecast_host: the rest of every LeaderWorkerSet rolling update, replayed from these
+        object rows and the group result rows of a sweep of the same tables (lwse.h, "rolling-update
+        forecast").  → dict: ``lws`` (LWS_FORECAST per object), ``steps`` (LWS_FORECAST_STEP trajectory
+        rows, object i's at ``lws[i]["step_base"]``; None when ``steps`` is False), ``n_steps_written``,
+        ``n_steps_needed``.  ``step_capacity`` None sizes the buffer so that every trajectory fits, with
+        a summaries-only call first; callers that forecast repeatedly pass a capacity instead."""
+        assert lws.dtype == R.LWS_REC and group_out.dtype == R.GROUP_OUT
+        lws, group_out = _aligned16(lws), _aligned16(group_out)
+        return self._lws_forecast(
+            lambda o: lib().lwse_lws_forecast_host(self._h, R.ptr(lws) if len(lws) else None, len(lws),
+                                                   R.ptr(group_out) if len(group_out) else None, len(group_out),
+                                                   C.byref(o)),
+            len(lws), steps, step_capacity)
+
+    def resident_forecast(self, steps=True, step_capacity=None):
+        """lwse_resident_forecast: as ``lws_forecast`` over the resident LWS rows and the group results of
+        the most recently submitted sweep, in flight or not; waits for no tick and changes none.  Raises
+        (NOT_READY) before a sweep after a load, or after LWS / group / pod patches made without one."""
+        n_lws = getattr(self, "_resident_shape", (0, 0))[0]
+        return self._lws_forecast(lambda o: lib().lwse_resident_forecast(self._h, C.byref(o)), n_lws, steps,
+                                  step_capacity)
 
     # ------------------------------------------------------------- group keys
     def group_keys_host(self, strings) -> np.ndarray:

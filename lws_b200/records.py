@@ -301,6 +301,28 @@ DSF_TRUNCATED = 1 << 4
 DSF_BAD_TABLE = 1 << 6
 DS_FORECAST_MAX_CYCLES = 65536
 
+# rolling-update forecast of the LeaderWorkerSets (lwse_lws_forecast_*): per LWS, and the trajectory rows
+LWS_FORECAST = np.dtype(
+    [("flags", "<u4"), ("cycles", "<u4"), ("step_base", "<u4"), ("n_steps", "<u4"), ("peak_sts_replicas", "<i4"),
+     ("floor_ready", "<i4"), ("final_partition", "<i4"), ("final_replicas", "<i4")], align=False
+)
+assert LWS_FORECAST.itemsize == 32
+LWS_FORECAST_STEP = np.dtype(
+    [("partition", "<i4"), ("sts_replicas", "<i4"), ("ready_replicas", "<i4"), ("updated_replicas", "<i4")],
+    align=False
+)
+assert LWS_FORECAST_STEP.itemsize == 16
+LWSF_ROLLING = 1 << 0
+LWSF_WAITING = 1 << 1
+LWSF_DONE = 1 << 2
+LWSF_UNFINISHED = 1 << 3
+LWSF_TRUNCATED = 1 << 4
+LWSF_HELD = 1 << 5
+LWSF_BAD_TABLE = 1 << 6
+LWSF_NOT_FORECAST = 1 << 7
+LWS_FORECAST_MAX_CYCLES = 65536
+LWS_FORECAST_MAX_SLOTS = 1 << 20
+
 
 # --------------------------------------------------------------------------- #
 # ctypes bundles (lwse_lws_tables / lwse_ds_tables / lwse_config)
@@ -429,6 +451,18 @@ class DsForecastOut(C.Structure):
     _fields_ = [
         ("ds", C.c_void_p),
         ("roles", C.c_void_p),
+        ("steps", C.c_void_p),
+        ("step_capacity", C.c_uint32),
+        ("n_steps_written", C.c_uint32),
+        ("n_steps_needed", C.c_uint64),
+    ]
+
+
+class LwsForecastOut(C.Structure):
+    """lwse_lws_forecast_out: where an LWS forecast goes, and the trajectory rows it wrote / needed."""
+
+    _fields_ = [
+        ("lws", C.c_void_p),
         ("steps", C.c_void_p),
         ("step_capacity", C.c_uint32),
         ("n_steps_written", C.c_uint32),
