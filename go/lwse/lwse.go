@@ -158,6 +158,15 @@ func (e *Engine) Forecast(out *C.lwse_ds_forecast_out) error {
 	return e.check(C.lwse_ds_resident_forecast(e.h, out))
 }
 
+// PlaceWhatIf answers "what would the placement round give with these node and request patches and
+// these extra requests?" over the resident tables without changing them: the resident rows whose
+// placement would change (with their current and hypothetical rows), the rows of the extra requests,
+// and lost / moved / gained counts.  It never waits for or drops a tick.  A validating webhook calls it
+// on LWS create / scale-up with an exclusive topology, a kubectl drain planner with cordon segments.
+func (e *Engine) PlaceWhatIf(q *C.lwse_place_whatif) error {
+	return e.check(C.lwse_resident_place_whatif(e.h, q))
+}
+
 // GroupKeys computes SHA-1 digests (20 bytes each) of n strings laid out CSR-style.
 func (e *Engine) GroupKeys(bytes *C.uint8_t, offsets *C.uint32_t, n uint32, digests *C.uint8_t) error {
 	return e.check(C.lwse_group_keys_host(e.h, bytes, offsets, C.uint32_t(n), digests))

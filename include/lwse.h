@@ -707,6 +707,75 @@ LWSE_API int lwse_reconcile_host(lwse_engine* e, const lwse_lws_tables* host, co
                                  uint32_t n_reqs, const uint32_t* occupancy, uint32_t n_namespaces,
                                  lwse_place_out* place_out);
 
+/* ---- placement what-if -----------------------------------------------------------------------
+ * "If these nodes were cordoned / relabelled / resized, or these requests changed or were added, what
+ * would the placement round give?" — answered on the resident tables without changing them.
+ *
+ * The what-if round is the round the placement spec computes over: the resident node rows with the
+ * NODES patches applied, the resident occupancy counters, the resident request rows with the PLACE_REQS
+ * patches applied followed by the `extra` rows, and n_namespaces namespaces.  Requests with
+ * ns >= n_namespaces get the tick's UNSCHEDULABLE row; extra row i has row index (and key) rn_reqs + i,
+ * where rn_reqs is the resident request count.  Identity patches are not taken: node deletion and
+ * eviction move occupancy, which a what-if never does.
+ *
+ * The baseline ("before") is the rows of the most recently submitted tick that ran LWSE_TICK_PLACE, in
+ * flight or not.  For a query without extra rows and with the resident n_namespaces, `after` equals byte
+ * for byte the rows a tick with the same segments and LWSE_TICK_PLACE computes, and {rows} is that
+ * tick's place change list.
+ *
+ * Namespaces are independent sub-problems over one capacity snapshot: without node patches the call
+ * solves only the TOUCHED namespaces (old and new namespace of every patched request row, the namespace
+ * of every extra row, and the namespaces n_namespaces adds) and every other row keeps its baseline row;
+ * with node patches it solves every namespace.  Node patches that change a node's usability or the
+ * domain of a usable node (the tick's rule) build a what-if node index; others use the resident one.
+ *
+ * Isolation: the call runs under the engine mutex, on a stream of its own with scratch of its own,
+ * behind everything the engine's stream holds (the most recently submitted tick with both branches
+ * joined).  It never drains, waits for the results of, or drops a tick, and touches no tick graph,
+ * arena region, change list, resident table, node index, output row, occupancy counter or tick info.
+ * Its segments are copied into a pinned staging buffer of its own.  Its scratch only grows (a call that
+ * needs more than any before allocates, which waits for the device as cudaMalloc does).
+ *
+ * Returns LWSE_ERR_NOT_READY before lwse_resident_place_load, before the first tick with
+ * LWSE_TICK_PLACE, and while the rows of that tick do not belong to the resident tables: after node,
+ * request or identity rows were patched by a tick without LWSE_TICK_PLACE, by lwse_resident_patch, or
+ * replaced by lwse_upload_nodes / lwse_resident_load, until the next tick with it.  An empty resident
+ * request table is ready after such a tick too (its baseline is empty): a what-if with extra rows only
+ * is the admission check of the first exclusive object.  LWSE_ERR_INVALID_ARG for a NULL
+ * query, more than LWSE_TICK_MAX_SEGS segments, a table other than LWSE_TABLE_NODES or
+ * LWSE_TABLE_PLACE_REQS, a scattered row at or beyond its table, n_namespaces == 0 with no resident
+ * count, or a NULL buffer with a count > 0; LWSE_ERR_BAD_TABLE for a range segment beyond its table (as
+ * a tick).  LWSE_ERR_UNSUPPORTED when rn_reqs + n_extra >= 2^24 (row keys are 24-bit) and on an
+ * engine with a peer exchange (the shared-occupancy round).  The scan form is not offered (it gives
+ * the same rows by spec); where a tick would run the general form (the domains do not fit one CTA, or
+ * LWSE_PLACE_FORM=general) the what-if does too. */
+typedef struct lwse_place_whatif {
+  /* in */
+  const lwse_patch_seg* segs;     /* LWSE_TABLE_NODES and LWSE_TABLE_PLACE_REQS only, the packing of a
+                                     tick's segments, host memory                                      */
+  uint32_t n_segs;
+  const lwse_place_req* extra;    /* hypothetical new requests: rows rn_reqs .. rn_reqs + n_extra - 1   */
+  uint32_t n_extra;
+  uint32_t n_namespaces;          /* 0 = the resident count; may be larger (new namespaces)            */
+  uint32_t capacity;              /* rows the change buffers below hold                                */
+  uint32_t* rows;                 /* [capacity]: resident rows whose row differs from the baseline      */
+  lwse_place_out* before;         /* [capacity]: their baseline rows                                    */
+  lwse_place_out* after;          /* [capacity]: their what-if rows                                     */
+  lwse_place_out* extra_out;      /* [n_extra], always written                                          */
+  /* out */
+  uint32_t n_changed;             /* every resident row that differs (rows beyond capacity not listed;
+                                     order unspecified)                                                */
+  uint32_t n_lost;                /* PLACED before and not after (resident rows)                       */
+  uint32_t n_moved;               /* PLACED in both, in another domain                                  */
+  uint32_t n_gained;              /* not PLACED before, PLACED after                                    */
+  uint32_t n_placed;              /* PLACED / UNSCHEDULABLE / CONFLICT rows of the whole what-if round, */
+  uint32_t n_unschedulable;       /* extra rows included                                                */
+  uint32_t n_conflict;
+  uint32_t namespaces_solved;     /* namespaces the namespace form solved (0 for the general form)      */
+  uint32_t form;                  /* LWSE_TICK_FORM_NAMESPACE or LWSE_TICK_FORM_GENERAL                 */
+} lwse_place_whatif;
+LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q);
+
 /* ------------------------------------------------------------------------- */
 /* Peer exchange: the multi-GPU placement step without a collective library  */
 /* ------------------------------------------------------------------------- */

@@ -3,6 +3,7 @@
 // library: every sweep is a CUDA kernel launch or the call fails.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <cstdlib>
@@ -101,6 +102,11 @@ int launch_node_index(const lwse_node_rec* d_nodes, uint32_t n_nodes, uint32_t n
                       bool pdl, int* cuda_err);
 int launch_place_diff(const lwse_place_out* d_cur, lwse_place_out* d_prev, uint32_t n, uint32_t* d_rows,
                       lwse_place_out* d_outs, uint32_t capacity, uint32_t* d_count, cudaStream_t s, int* cuda_err);
+int launch_place_whatif_index(const lwse_place_req* d_reqs, uint32_t n_reqs, uint32_t n_namespaces, const uint8_t* d_touched,
+                              uint32_t n_nodes, uint32_t n_domains, void* d_scratch, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_place_whatif_diff(const lwse_place_out* d_before, const lwse_place_out* d_after, uint32_t n_resident, uint32_t n_total,
+                             uint32_t* d_rows, lwse_place_out* d_outs_before, lwse_place_out* d_outs_after, uint32_t capacity,
+                             uint32_t* d_counts, int sm_count, cudaStream_t s, int* cuda_err);
 // lwse_ds_kernels.cu
 int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s, int* cuda_err);
 struct DsTickHost {
@@ -357,6 +363,20 @@ struct lwse_engine {
   cudaEvent_t ev_lf = nullptr;       // the engine's stream where a resident forecast takes its snapshot
   DevBuf lf_lws, lf_group_out, lf_slot_off, lf_slots, lf_fc, lf_steps, lf_totals;
   PinBuf lf_words;                   // the three totals, copied back
+  bool r_place_current = false;      // r_pout holds the round of the resident node, request and identity rows: a
+                                     // tick with LWSE_TICK_PLACE was submitted since lwse_resident_place_load and
+                                     // since any patch of those rows made without a round
+  // placement what-if (lwse_resident_place_whatif): patched copies of the node and request rows, the what-if
+  // round's rows, its own node index and round scratch, on a stream of its own; never a tick's buffers
+  cudaStream_t wf_stream = nullptr;
+  cudaEvent_t ev_wf = nullptr;       // the engine's stream where a what-if takes its snapshot
+  cudaEvent_t ev_wf_t0 = nullptr, ev_wf_t1 = nullptr;  // (LWSE_WHATIF_TIMING=1) around the last what-if's device work
+  bool wf_timed = false;
+  DevBuf wf_nodes, wf_reqs, wf_out, wf_dom_first, wf_node_order, wf_node_pos, wf_node_ix, wf_touched, wf_round, wf_list;
+  PinBuf wf_stage;                   // the call's segments, extra rows and namespace mask (the scatter reads them here)
+  PinBuf wf_words;                   // the counts, copied back
+  uint32_t wf_geometry[4] = {0, 0, 0, 0};  // (n_reqs, n_namespaces, nodes, domains) the round scratch was laid out for
+  uint32_t wf_calls = 0;
   DevBuf sha_bytes, sha_offsets, sha_digests, sha_ints;
   uint32_t* h_rounds = nullptr;  // pinned
   // peer exchange of the multi-GPU placement step (lwse_exchange_*)
@@ -573,11 +593,15 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->rd_role_out[1], &e->rd_revrole_out[0], &e->rd_revrole_out[1], &e->rd_marks, &e->rd_ones,
                       &e->rd_counters, &e->rd_stage_dev, &e->rd_links, &e->fc_rows, &e->fc_ds_out, &e->fc_role_out,
                       &e->fc_revrole_out, &e->fc_ds, &e->fc_roles, &e->fc_steps, &e->fc_totals,
-                      &e->lf_lws, &e->lf_group_out, &e->lf_slot_off, &e->lf_slots, &e->lf_fc, &e->lf_steps, &e->lf_totals};
+                      &e->lf_lws, &e->lf_group_out, &e->lf_slot_off, &e->lf_slots, &e->lf_fc, &e->lf_steps, &e->lf_totals,
+                      &e->wf_nodes, &e->wf_reqs, &e->wf_out, &e->wf_dom_first, &e->wf_node_order, &e->wf_node_pos,
+                      &e->wf_node_ix, &e->wf_touched, &e->wf_round, &e->wf_list};
     if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
     if (e->lf_stream) cudaStreamSynchronize(e->lf_stream);
+    if (e->wf_stream) cudaStreamSynchronize(e->wf_stream);
     for (DevBuf* b : bufs) b->release();
-    PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc, &e->rd_pin, &e->rd_stage, &e->fc_words, &e->lf_words};
+    PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc, &e->rd_pin, &e->rd_stage, &e->fc_words, &e->lf_words,
+                      &e->wf_stage, &e->wf_words};
     for (PinBuf* b : pins) b->release();
     if (e->ev_place) cudaEventDestroy(e->ev_place);
     if (e->h_rounds) cudaFreeHost(e->h_rounds);
@@ -596,6 +620,10 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
     if (e->ev_ds_link) cudaEventDestroy(e->ev_ds_link);
     if (e->lf_stream) cudaStreamDestroy(e->lf_stream);
     if (e->ev_lf) cudaEventDestroy(e->ev_lf);
+    if (e->wf_stream) cudaStreamDestroy(e->wf_stream);
+    if (e->ev_wf) cudaEventDestroy(e->ev_wf);
+    if (e->ev_wf_t0) cudaEventDestroy(e->ev_wf_t0);
+    if (e->ev_wf_t1) cudaEventDestroy(e->ev_wf_t1);
     cudaStreamDestroy(e->side_stream);
     cudaStreamDestroy(e->stream);
   }
@@ -609,6 +637,13 @@ LWSE_API uint64_t lwse_launch_count(const lwse_engine* e) { return e ? e->launch
 // A node a placement request can use: schedulable, labelled with the topology key, a domain in range.
 static bool node_usable(const lwse_node_rec& nd, uint32_t n_domains) {
   return (nd.flags & LWSE_NODE_SCHEDULABLE) && (nd.flags & LWSE_NODE_HAS_TOPOLOGY) && nd.domain_id < n_domains;
+}
+
+// The node-index rule (ticks and what-ifs alike): a patch needs a new domain-sorted index when it changes
+// whether the node is usable, or the domain of a usable node.  Capacity-only patches keep the index.
+static bool node_patch_moves_index(const lwse_node_rec& old, const lwse_node_rec& now, uint32_t n_domains) {
+  const bool was = node_usable(old, n_domains), is = node_usable(now, n_domains);
+  return was != is || (is && old.domain_id != now.domain_id);
 }
 
 // The domain-sorted node index (dom_first / node_order / node_pos), rebuilt on `s` from the device node
@@ -649,7 +684,7 @@ static int node_patches_locked(lwse_engine* e, const lwse_patch_seg* segs, uint3
       if (row >= e->n_nodes) continue;  // (the scatter kernel skips it too)
       lwse_node_rec& old = e->h_nodes[row];
       const bool was = node_usable(old, e->n_domains), is = node_usable(v[k], e->n_domains);
-      if (was != is || (is && old.domain_id != v[k].domain_id)) e->node_index_stale = true;
+      if (node_patch_moves_index(old, v[k], e->n_domains)) e->node_index_stale = true;
       e->n_usable = e->n_usable - (was ? 1u : 0u) + (is ? 1u : 0u);
       old = v[k];
       n_rows++;
@@ -686,6 +721,7 @@ LWSE_API int lwse_upload_nodes(lwse_engine* e, const lwse_node_rec* nodes, uint3
                                  cudaMemcpyHostToDevice, e->stream));
   e->n_nodes = n_nodes;
   e->n_domains = n_domains;
+  e->r_place_current = false;  // (the rows of the last round were computed over the previous node table)
   e->h_nodes.assign(nodes, nodes + n_nodes);
   e->n_usable = 0;
   for (const lwse_node_rec& nd : e->h_nodes) e->n_usable += node_usable(nd, n_domains) ? 1u : 0u;
@@ -880,6 +916,7 @@ LWSE_API int lwse_resident_load(lwse_engine* e, const lwse_lws_tables* h) {
   }
   e->r_swept = false;  // (the output rows are all-ones until the next sweep)
   e->r_groups_swept = false;
+  e->r_place_current = false;  // (a new identity column: new occupancy counters)
   cudaStream_t s = e->stream;
   const size_t b_lws = (size_t)h->n_lws * sizeof(lwse_lws_rec), b_grp = (size_t)h->n_groups * sizeof(lwse_group_rec);
   const size_t b_pst = (size_t)h->n_pods * sizeof(lwse_pod_state), b_pid = (size_t)h->n_pods * sizeof(lwse_pod_ident);
@@ -1183,6 +1220,8 @@ LWSE_API int lwse_resident_patch(lwse_engine* e, lwse_table which, const uint32_
   }
   if (which == LWSE_TABLE_LWS) e->r_swept = false;  // r_lws_out no longer belongs to these LWS rows
   if (which <= LWSE_TABLE_POD_IDENT) e->r_groups_swept = false;  // nor r_group_out to the group and pod rows
+  if (which == LWSE_TABLE_NODES || which == LWSE_TABLE_PLACE_REQS || which == LWSE_TABLE_POD_IDENT)
+    e->r_place_current = false;  // nor r_pout to the rows a round reads
   bool wrote = false;
   const int rc = apply_patches_locked(e, &seg, 1, &wrote);
   if (rc != LWSE_OK) {
@@ -1568,6 +1607,19 @@ LWSE_API int lwse_exchange_status(lwse_engine* e, uint32_t* error_out) {
   return LWSE_OK;
 }
 
+// Measurement aid (not part of lwse.h): with LWSE_WHATIF_TIMING=1, the device time of the last what-if on its
+// stream, from behind the snapshot event to the end of the diff kernel (the copies back to the host excluded).
+extern "C" __attribute__((visibility("default"))) int lwse_debug_whatif_device_us(lwse_engine* e, float* us) {
+  if (!e || !us) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->wf_timed) return LWSE_ERR_NOT_READY;
+  DeviceGuard guard(e->device);
+  float ms = 0.f;
+  LWSE_CUDA(e, cudaEventElapsedTime(&ms, e->ev_wf_t0, e->ev_wf_t1));
+  *us = ms * 1000.f;
+  return LWSE_OK;
+}
+
 // Tuning aid (not part of lwse.h): phase timestamps of the most recent placement kernel.
 extern "C" __attribute__((visibility("default"))) int lwse_debug_place_trace(lwse_engine* e, uint64_t* out16) {
   if (!e || !out16 || !e->place_scratch.p || e->place_calls == 0) return LWSE_ERR_NOT_READY;
@@ -1688,6 +1740,7 @@ LWSE_API int lwse_resident_place_load(lwse_engine* e, const lwse_place_req* reqs
   e->rn_reqs = n_reqs;
   e->rn_namespaces = n_namespaces;
   e->r_place_loaded = true;
+  e->r_place_current = false;  // (no round over these rows yet)
   e->r_place_grouped = grouped_by_namespace(reqs, n_reqs);
   e->r_ns_index_ok = false;  // an ungrouped table: the first tick builds the namespace index
   e->r_req_ns.resize(n_reqs);
@@ -1754,6 +1807,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
 // Enqueue one tick (nothing waits): slot = t_submitted & 1.  At most two ticks are in flight.
 static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, uint32_t flags) {
   const int rc = tick_submit_body(e, segs, n_segs, flags);
+  if (rc != LWSE_OK) e->r_place_current = false;  // (its patches may or may not have been applied)
   if (rc != LWSE_OK && segs) {
     // A tick that fails once its node rows are in the mirror (a CUDA error, no staging memory) may or may
     // not have patched them on the device: the next round rebuilds the index from the device rows.
@@ -1773,6 +1827,8 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
   uint8_t* chg_v = static_cast<uint8_t*>(e->chg_dev.p) + slot * e->chg_bytes;  // the device-memory lists (of this slot) the kernels append to
   uint32_t* cnt = static_cast<uint32_t*>(e->r_counts.p) + slot * 16u;          // and their counters
   const bool do_place = (flags & LWSE_TICK_PLACE) && e->r_place_loaded && e->rn_reqs > 0;
+  // a tick that asks for a round leaves r_pout current for the resident rows (trivially so for an empty table)
+  const bool round_asked = (flags & LWSE_TICK_PLACE) && e->r_place_loaded;
   const bool do_sweep = !(flags & LWSE_TICK_NO_SWEEP) && (e->rn_lws || e->rn_groups);
   {
     const int crc = check_segments(e, segs, n_segs);
@@ -1784,6 +1840,11 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
     if (segs[i].table == LWSE_TABLE_LWS && segs[i].n) e->r_swept = false;
     if (segs[i].table <= LWSE_TABLE_POD_IDENT && segs[i].n) e->r_groups_swept = false;
   }
+  // as r_swept, for the placement rows: node, request and identity rows patched without a round
+  for (uint32_t i = 0; !round_asked && i < n_segs; i++)
+    if (segs[i].n && (segs[i].table == LWSE_TABLE_NODES || segs[i].table == LWSE_TABLE_PLACE_REQS ||
+                      segs[i].table == LWSE_TABLE_POD_IDENT))
+      e->r_place_current = false;
   // The round's form, decided before any patch is applied (it is part of a tick graph's key).  A request
   // table grouped by namespace — and not ungrouped by this tick's patches — runs the namespace kernels as
   // they are; any other table runs them through the namespace index, rebuilt when the namespace column
@@ -2135,6 +2196,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
       gts.wrote = has_patches;
       e->t_submitted++;
       if (do_sweep) e->r_swept = e->r_groups_swept = true;
+      if (round_asked) e->r_place_current = true;
       e->main_unforked = !do_place && (e->main_unforked || has_patches);
       record_info(true);
       return LWSE_OK;
@@ -2177,6 +2239,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
   ts.wrote = wrote || wrote_side;
   e->t_submitted++;
   if (do_sweep) e->r_swept = e->r_groups_swept = true;
+  if (round_asked) e->r_place_current = true;
   e->main_unforked = !do_place && (e->main_unforked || wrote);
   record_info(false);
   return LWSE_OK;
@@ -2338,6 +2401,259 @@ LWSE_API int lwse_resident_node_info(lwse_engine* e, lwse_node_info* info) {
   if (!e || !info) return LWSE_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(e->mu);
   *info = e->last_node_info;
+  return LWSE_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Placement what-if
+// ---------------------------------------------------------------------------
+// Patched copies of the node and request rows in what-if scratch, the round over them on wf_stream
+// (only the touched namespaces in the namespace form), then one diff kernel against the baseline rows
+// (r_pout, read in place: nothing writes them while the call holds the mutex).  The resident node
+// index is read in place unless the node patches need another one.
+LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->r_loaded || !e->r_place_loaded || !e->r_place_current || e->n_nodes == 0 || e->n_domains == 0)
+    return LWSE_ERR_NOT_READY;
+  if (e->xch_world > 0) return LWSE_ERR_UNSUPPORTED;
+  if ((q->n_segs && !q->segs) || q->n_segs > LWSE_TICK_MAX_SEGS || (q->n_extra && (!q->extra || !q->extra_out)) ||
+      (q->capacity && (!q->rows || !q->before || !q->after)))
+    return LWSE_ERR_INVALID_ARG;
+  const uint32_t n_ns = q->n_namespaces ? q->n_namespaces : e->rn_namespaces;
+  if (n_ns == 0) return LWSE_ERR_INVALID_ARG;
+  const uint32_t rn = e->rn_reqs;
+  if ((uint64_t)rn + q->n_extra >= (1ull << 24)) return LWSE_ERR_UNSUPPORTED;
+  const uint32_t n_total = rn + q->n_extra;
+  for (uint32_t i = 0; i < q->n_segs; i++)
+    if (q->segs[i].n && q->segs[i].table != LWSE_TABLE_NODES && q->segs[i].table != LWSE_TABLE_PLACE_REQS)
+      return LWSE_ERR_INVALID_ARG;
+  {
+    const int crc = check_segments(e, q->segs, q->n_segs);
+    if (crc != LWSE_OK) return crc;
+  }
+  // the touched namespaces and the node-index decision (the tick's rule, over the mirror, which stays as it is)
+  std::vector<uint8_t> touched(n_ns, 0);
+  for (uint32_t v = e->rn_namespaces; v < n_ns; v++) touched[v] = 1;  // (their resident rows were UNSCHEDULABLE)
+  bool node_rows = false, node_rebuild = false;
+  size_t stage_need = align256((size_t)n_ns) + align256((size_t)q->n_extra * sizeof(lwse_place_req));
+  std::unordered_map<uint32_t, lwse_node_rec> node_now;  // rows patched earlier in this call
+  for (uint32_t i = 0; i < q->n_segs; i++) {
+    const lwse_patch_seg& g = q->segs[i];
+    if (g.n == 0) continue;
+    const bool range = (g.flags & LWSE_PATCH_RANGE) != 0;
+    const uint32_t rb = g.table == LWSE_TABLE_NODES ? (uint32_t)sizeof(lwse_node_rec) : (uint32_t)sizeof(lwse_place_req);
+    const uint32_t n_rows = g.table == LWSE_TABLE_NODES ? e->n_nodes : rn;
+    stage_need += align256((size_t)g.n * 4) + align256((size_t)g.n * rb);
+    for (uint32_t k = 0; k < g.n; k++) {
+      const uint32_t row = range ? g.first_row + k : g.rows[k];
+      if (row >= n_rows) return LWSE_ERR_INVALID_ARG;
+      if (g.table == LWSE_TABLE_NODES) {
+        node_rows = true;
+        const lwse_node_rec& v = static_cast<const lwse_node_rec*>(g.values)[k];
+        auto it = node_now.find(row);
+        const lwse_node_rec& old = it != node_now.end() ? it->second : e->h_nodes[row];
+        if (node_patch_moves_index(old, v, e->n_domains)) node_rebuild = true;
+        node_now[row] = v;
+      } else {
+        const uint32_t nv = static_cast<const lwse_place_req*>(g.values)[k].ns, ov = e->r_req_ns[row];
+        if (nv < n_ns) touched[nv] = 1;
+        if (ov < n_ns) touched[ov] = 1;
+      }
+    }
+  }
+  for (uint32_t i = 0; i < q->n_extra; i++)
+    if (q->extra[i].ns < n_ns) touched[q->extra[i].ns] = 1;
+  if (node_rows) std::fill(touched.begin(), touched.end(), (uint8_t)1);  // (capacities or domains moved under every namespace)
+  // (a resident index behind the resident rows — node patches, and no round since because the request table is
+  // empty — is not read either: the what-if builds its own)
+  if (e->node_index_stale) node_rebuild = true;
+  uint32_t n_touched = 0;
+  for (uint8_t t : touched) n_touched += t;
+
+  DeviceGuard guard(e->device);
+  if (!e->wf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->wf_stream, cudaStreamNonBlocking));
+  if (!e->ev_wf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_wf, cudaEventDisableTiming));
+  cudaStream_t s = e->wf_stream;
+  // staging (the previous call synchronized its stream: the buffer is free)
+  LWSE_CUDA(e, e->wf_stage.reserve(stage_need));
+  LWSE_CUDA(e, e->wf_words.reserve(64));
+  uint8_t* st_h = static_cast<uint8_t*>(e->wf_stage.h);
+  size_t cursor = 0;
+  auto stage = [&](const void* src, size_t bytes) -> size_t {
+    const size_t at = cursor;
+    if (bytes) memcpy(st_h + at, src, bytes);
+    cursor += align256(bytes);
+    return at;
+  };
+  const bool ns_form = g_place_form_env != 0 && lwse::place_ns_supported(e->n_nodes, e->n_domains);
+  const size_t b_nodes = (size_t)e->n_nodes * sizeof(lwse_node_rec);
+  const size_t b_out = (size_t)n_total * sizeof(lwse_place_out);
+  LWSE_CUDA(e, e->wf_reqs.reserve((size_t)n_total * sizeof(lwse_place_req) + 16));
+  LWSE_CUDA(e, e->wf_out.reserve(b_out + 16));
+  LWSE_CUDA(e, e->wf_touched.reserve((size_t)n_ns + 16));
+  const uint32_t list_cap = q->capacity < rn ? q->capacity : rn;  // (at most rn rows can differ)
+  LWSE_CUDA(e, e->wf_list.reserve(64 + 16 + (size_t)list_cap * (4 + 2 * sizeof(lwse_place_out))));
+  if (node_rows) LWSE_CUDA(e, e->wf_nodes.reserve(b_nodes + 16));
+  if (node_rebuild) {
+    const size_t order_padded = ((size_t)(e->n_nodes + 255u) / 256u + 1u) * 1024u;
+    const size_t ix_bytes = lwse::node_index_scratch_bytes(e->n_domains);
+    LWSE_CUDA(e, e->wf_dom_first.reserve(((size_t)e->n_domains + 1) * 4 + 16));
+    LWSE_CUDA(e, e->wf_node_order.reserve(order_padded + 16));
+    LWSE_CUDA(e, e->wf_node_pos.reserve((size_t)e->n_nodes * 4 + 16));
+    LWSE_CUDA(e, e->wf_node_ix.reserve(ix_bytes));
+    // The build wants its per-domain counts at zero.  A build leaves them so but not its cursors, and their
+    // places move with n_domains (counts at [0, n), cursors at [n, 2n)): cleared before every build, as
+    // lwse_upload_nodes clears the resident ones.  The padding of the order rows stays zero.
+    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_ix.p, 0, ix_bytes, s));
+    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_order.p, 0, order_padded, s));
+  }
+  size_t round_bytes = 0;
+  bool round_fresh = false;
+  if (ns_form) {
+    round_bytes = lwse::place_ns_scratch_bytes(e->n_nodes, e->n_domains, n_total, n_ns);
+    const void* before = e->wf_round.p;
+    LWSE_CUDA(e, e->wf_round.reserve(round_bytes));
+    const uint32_t geometry[4] = {n_total, n_ns, e->n_nodes, e->n_domains};
+    round_fresh = before != e->wf_round.p || memcmp(geometry, e->wf_geometry, sizeof(geometry)) != 0;
+    memcpy(e->wf_geometry, geometry, sizeof(geometry));
+  } else {
+    round_bytes = lwse::place_scratch_bytes(e->n_nodes, e->n_domains, n_total, n_ns);
+    LWSE_CUDA(e, e->wf_round.reserve(round_bytes));
+    e->wf_geometry[0] = e->wf_geometry[1] = e->wf_geometry[2] = e->wf_geometry[3] = 0;  // (the general form re-initialises it)
+  }
+
+  // the snapshot: behind everything on the engine's stream, both branches of every tick submitted so far joined
+  LWSE_CUDA(e, cudaEventRecord(e->ev_wf, e->stream));
+  LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_wf, 0));
+  static const bool timing = [] {  // LWSE_WHATIF_TIMING=1: CUDA events on the what-if stream (measurements)
+    const char* v = getenv("LWSE_WHATIF_TIMING");
+    return v && atoi(v) != 0;
+  }();
+  e->wf_timed = false;
+  if (timing) {
+    if (!e->ev_wf_t0) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t0));
+    if (!e->ev_wf_t1) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t1));
+    LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t0, s));
+  }
+  lwse_node_rec* d_nodes = (lwse_node_rec*)e->nodes.p;
+  lwse_place_req* d_reqs = (lwse_place_req*)e->wf_reqs.p;
+  lwse_place_out* d_out = (lwse_place_out*)e->wf_out.p;
+  if (node_rows) {
+    LWSE_CUDA(e, cudaMemcpyAsync(e->wf_nodes.p, e->nodes.p, b_nodes, cudaMemcpyDeviceToDevice, s));
+    d_nodes = (lwse_node_rec*)e->wf_nodes.p;
+  }
+  if (rn) {
+    LWSE_CUDA(e, cudaMemcpyAsync(d_reqs, e->r_preq.p, (size_t)rn * sizeof(lwse_place_req), cudaMemcpyDeviceToDevice, s));
+    LWSE_CUDA(e, cudaMemcpyAsync(d_out, e->r_pout.p, (size_t)rn * sizeof(lwse_place_out), cudaMemcpyDeviceToDevice, s));
+  }
+  if (q->n_extra) {
+    const size_t at = stage(q->extra, (size_t)q->n_extra * sizeof(lwse_place_req));
+    LWSE_CUDA(e, cudaMemcpyAsync(d_reqs + rn, st_h + at, (size_t)q->n_extra * sizeof(lwse_place_req), cudaMemcpyHostToDevice, s));
+    LWSE_CUDA(e, cudaMemsetAsync(d_out + rn, 0, (size_t)q->n_extra * sizeof(lwse_place_out), s));
+  }
+  {
+    const size_t at = stage(touched.data(), n_ns);
+    LWSE_CUDA(e, cudaMemcpyAsync(e->wf_touched.p, st_h + at, n_ns, cudaMemcpyHostToDevice, s));
+  }
+  // the segments, into the copies: ranges by DMA first, then one scatter of the rest (as a tick applies them)
+  lwse::ScatterSegHost sc[LWSE_TICK_MAX_SEGS];
+  int n_sc = 0;
+  for (uint32_t i = 0; i < q->n_segs; i++) {
+    const lwse_patch_seg& g = q->segs[i];
+    if (g.n == 0) continue;
+    const bool is_nodes = g.table == LWSE_TABLE_NODES;
+    const uint32_t rb = is_nodes ? (uint32_t)sizeof(lwse_node_rec) : (uint32_t)sizeof(lwse_place_req);
+    void* table = is_nodes ? (void*)d_nodes : (void*)d_reqs;
+    const size_t vat = stage(g.values, (size_t)g.n * rb);
+    if (g.flags & LWSE_PATCH_RANGE) {
+      LWSE_CUDA(e, cudaMemcpyAsync(static_cast<uint8_t*>(table) + (size_t)g.first_row * rb, st_h + vat, (size_t)g.n * rb,
+                                   cudaMemcpyHostToDevice, s));
+      continue;
+    }
+    const size_t rat = stage(g.rows, (size_t)g.n * 4);
+    uint8_t* st_d = static_cast<uint8_t*>(e->wf_stage.d);
+    sc[n_sc++] = lwse::ScatterSegHost{table, is_nodes ? (uint64_t)e->n_nodes : (uint64_t)rn,
+                                      reinterpret_cast<const uint32_t*>(st_d + rat), st_d + vat, g.n, rb, false};
+  }
+  int cuda_err = 0;
+  if (n_sc) {
+    const int launched = lwse::launch_scatter(sc, n_sc, nullptr, 0, s, false, &cuda_err);
+    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+    e->launches += (uint64_t)launched;
+  }
+  const uint32_t* dom_first = (const uint32_t*)e->dom_first.p;
+  const uint32_t* node_order = (const uint32_t*)e->node_order.p;
+  const uint32_t* node_pos = (const uint32_t*)e->node_pos.p;
+  if (node_rebuild) {
+    const int launched = lwse::launch_node_index(d_nodes, e->n_nodes, e->n_domains, (uint32_t*)e->wf_dom_first.p,
+                                                 (uint32_t*)e->wf_node_order.p, (uint32_t*)e->wf_node_pos.p, e->wf_node_ix.p,
+                                                 e->sm_count, s, false, &cuda_err);
+    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+    e->launches += (uint64_t)launched;
+    dom_first = (const uint32_t*)e->wf_dom_first.p;
+    node_order = (const uint32_t*)e->wf_node_order.p;
+    node_pos = (const uint32_t*)e->wf_node_pos.p;
+  }
+  if (ns_form) {
+    if (round_fresh) LWSE_CUDA(e, cudaMemsetAsync(e->wf_round.p, 0, round_bytes, s));  // (index counts and counters start at zero)
+    int launched = lwse::launch_place_whatif_index(d_reqs, n_total, n_ns, (const uint8_t*)e->wf_touched.p, e->n_nodes, e->n_domains,
+                                                   e->wf_round.p, e->sm_count, s, &cuda_err);
+    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+    e->launches += (uint64_t)launched;
+    launched = lwse::launch_place_ns(d_nodes, dom_first, node_order, e->n_nodes, e->n_domains, d_reqs, n_total,
+                                     (const uint32_t*)e->r_occ.p, 1, 0, n_ns, d_out, e->wf_round.p, round_bytes, false,
+                                     e->wf_calls++, false, e->sm_count, s, &cuda_err, nullptr, false, nullptr, nullptr,
+                                     lwse::kNsIndexReuse);
+    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+    e->launches += (uint64_t)launched;
+  } else {
+    const int launched = lwse::launch_place(d_nodes, dom_first, node_order, node_pos, e->n_nodes, e->n_domains, d_reqs, n_total,
+                                            (const uint32_t*)e->r_occ.p, n_ns, d_out, e->wf_round.p, round_bytes, nullptr,
+                                            e->sm_count, s, &cuda_err, 0u, true, 1, n_total, 0, nullptr, nullptr, nullptr, false);
+    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+    e->launches += (uint64_t)launched;
+  }
+  // the diff against the baseline, the counts
+  // (layout: [counts: 16 words] [rows: list_cap] [before: list_cap] [after: list_cap], the 16-byte rows aligned)
+  uint32_t* d_counts = (uint32_t*)e->wf_list.p;
+  uint32_t* d_rows = d_counts + 16;
+  lwse_place_out* d_before =
+      reinterpret_cast<lwse_place_out*>(static_cast<uint8_t*>(e->wf_list.p) + 64 + (((size_t)list_cap * 4 + 15) & ~(size_t)15));
+  lwse_place_out* d_after = d_before + list_cap;
+  LWSE_CUDA(e, cudaMemsetAsync(d_counts, 0, 64, s));
+  {
+    const int launched = lwse::launch_place_whatif_diff((const lwse_place_out*)e->r_pout.p, d_out, rn, n_total, d_rows, d_before,
+                                                        d_after, list_cap, d_counts, e->sm_count, s, &cuda_err);
+    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+    e->launches += (uint64_t)launched;
+  }
+  if (timing) {
+    LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t1, s));
+    e->wf_timed = true;
+  }
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_counts, 32, cudaMemcpyDeviceToHost, s));
+  if (q->n_extra)
+    LWSE_CUDA(e, cudaMemcpyAsync(q->extra_out, d_out + rn, (size_t)q->n_extra * sizeof(lwse_place_out), cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint32_t n_changed = words[0];
+  const uint32_t listed = n_changed < list_cap ? n_changed : list_cap;
+  if (listed) {
+    LWSE_CUDA(e, cudaMemcpyAsync(q->rows, d_rows, (size_t)listed * 4, cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaMemcpyAsync(q->before, d_before, (size_t)listed * sizeof(lwse_place_out), cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaMemcpyAsync(q->after, d_after, (size_t)listed * sizeof(lwse_place_out), cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaStreamSynchronize(s));
+  }
+  q->n_changed = n_changed;
+  q->n_lost = words[1];
+  q->n_moved = words[2];
+  q->n_gained = words[3];
+  q->n_placed = words[4];
+  q->n_unschedulable = words[5];
+  q->n_conflict = words[6];
+  q->namespaces_solved = ns_form ? n_touched : 0u;
+  q->form = ns_form ? LWSE_TICK_FORM_NAMESPACE : LWSE_TICK_FORM_GENERAL;
   return LWSE_OK;
 }
 

@@ -991,4 +991,155 @@ cudaError_t set_place_ns_carveout(int pct) {  // see set_sweep_carveout (lwse_lw
   return e;
 }
 
+// --------------------------------------------------------------------------
+// what-if rounds (lwse_resident_place_whatif)
+// --------------------------------------------------------------------------
+// The what-if solves only the namespaces its patches touch: the namespace index it builds holds the
+// rows of touched namespaces alone, so the namespace kernel's CTAs of the others see an empty range
+// and its output keeps their rows (a copy of the baseline).  Exact, because namespaces share nothing
+// but the capacity snapshot, which a what-if does not change.  The same count -> scan -> fill as the
+// tick's index, with a mask: separate kernels, so that the tick's instances stay as they are.
+struct WhatIfIndexArgs {
+  const lwse_place_req* reqs;
+  const uint8_t* touched;  // n_namespaces: 1 = solve this namespace
+  uint32_t* ns_count;
+  uint32_t* ns_cursor;
+  uint32_t* ns_rows;
+  uint32_t n_reqs, n_namespaces;
+};
+
+__device__ __forceinline__ uint32_t whatif_ns_of(const WhatIfIndexArgs& a, uint32_t i) {
+  if (i >= a.n_reqs) return LWSE_NONE;
+  const uint32_t v = __ldcg(reinterpret_cast<const uint32_t*>(a.reqs + i) + 5);  // .ns (rows the scatter just patched)
+  return (v < a.n_namespaces && a.touched[v]) ? v : LWSE_NONE;
+}
+
+__global__ void __launch_bounds__(256) place_whatif_count_kernel(const WhatIfIndexArgs a) {
+  const uint32_t lane = threadIdx.x & 31u, stride = gridDim.x * blockDim.x;
+  for (uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; base < a.n_reqs; base += stride) {
+    const uint32_t v = whatif_ns_of(a, base + lane);
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, v);
+    if (v != LWSE_NONE && lane == (uint32_t)__ffs(peers) - 1u) atomicAdd(a.ns_count + v, (uint32_t)__popc(peers));
+  }
+}
+
+__global__ void __launch_bounds__(256) place_whatif_fill_kernel(const WhatIfIndexArgs a) {
+  const uint32_t lane = threadIdx.x & 31u, stride = gridDim.x * blockDim.x;
+  for (uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; base < a.n_reqs; base += stride) {
+    const uint32_t i = base + lane, v = whatif_ns_of(a, i);
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, v);
+    const uint32_t leader = (uint32_t)__ffs(peers) - 1u;
+    uint32_t pos = 0;
+    if (v != LWSE_NONE && lane == leader) pos = atomicAdd(a.ns_cursor + v, (uint32_t)__popc(peers));
+    pos = __shfl_sync(0xFFFFFFFFu, pos, (int)leader);
+    if (v != LWSE_NONE) a.ns_rows[pos + (uint32_t)__popc(peers & ((1u << lane) - 1u))] = i;
+  }
+}
+
+// The masked namespace index in the namespace-form scratch `d_scratch` (laid out as launch_place_ns
+// lays it out for the same geometry; ns_count zero before, and again after).  Returns kernels launched or -1.
+int launch_place_whatif_index(const lwse_place_req* d_reqs, uint32_t n_reqs, uint32_t n_namespaces, const uint8_t* d_touched,
+                              uint32_t n_nodes, uint32_t n_domains, void* d_scratch, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  const NsLayout l = ns_layout(n_nodes, n_domains, n_reqs, n_namespaces);
+  uint8_t* base = static_cast<uint8_t*>(d_scratch);
+  WhatIfIndexArgs a{};
+  a.reqs = d_reqs;
+  a.touched = d_touched;
+  a.ns_count = reinterpret_cast<uint32_t*>(base + l.ns_count);
+  a.ns_cursor = reinterpret_cast<uint32_t*>(base + l.ns_cursor);
+  a.ns_rows = reinterpret_cast<uint32_t*>(base + l.ns_rows);
+  a.n_reqs = n_reqs;
+  a.n_namespaces = n_namespaces;
+  uint64_t grid = ((uint64_t)n_reqs + 255) / 256;
+  if (grid < 1) grid = 1;
+  if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
+  place_whatif_count_kernel<<<(unsigned)grid, 256, 0, s>>>(a);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) {
+    place_index_scan_kernel<<<1, kIndexScanThreads, 0, s>>>(
+        IndexScanArgs{a.ns_count, reinterpret_cast<uint32_t*>(base + l.ns_first), a.ns_cursor, n_namespaces});
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) {
+    place_whatif_fill_kernel<<<(unsigned)grid, 256, 0, s>>>(a);
+    e = cudaGetLastError();
+  }
+  if (e != cudaSuccess) {
+    *cuda_err = (int)e;
+    return -1;
+  }
+  return 3;
+}
+
+// The what-if's diff against the baseline and its counts.  counts: [0] changed rows [1] lost [2] moved
+// [3] gained (resident rows) [4] PLACED [5] UNSCHEDULABLE [6] CONFLICT (every row, extra rows included).
+// Each warp reduces its counts before the one atomic per counter, and appends its changed rows with one
+// atomic (rows at or beyond `capacity` are counted, not listed).
+struct WhatIfDiffArgs {
+  const lwse_place_out* before;  // n_resident
+  const lwse_place_out* after;   // n_total
+  uint32_t* rows;
+  lwse_place_out* outs_before;
+  lwse_place_out* outs_after;
+  uint32_t* counts;
+  uint32_t capacity, n_resident, n_total;
+};
+
+__global__ void __launch_bounds__(256) place_whatif_diff_kernel(const WhatIfDiffArgs a) {
+  const uint32_t lane = threadIdx.x & 31u, stride = gridDim.x * blockDim.x;
+  uint32_t c[6] = {0u, 0u, 0u, 0u, 0u, 0u};
+  for (uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; base < a.n_total; base += stride) {
+    const uint32_t r = base + lane;
+    bool changed = false;
+    uint4 v = make_uint4(0u, 0u, 0u, 0u), o = v;
+    if (r < a.n_total) {
+      v = __ldcg(reinterpret_cast<const uint4*>(a.after + r));
+      c[3] += (v.z & LWSE_PLACE_PLACED) ? 1u : 0u;
+      c[4] += (v.z & LWSE_PLACE_UNSCHEDULABLE) ? 1u : 0u;
+      c[5] += (v.z & LWSE_PLACE_CONFLICT) ? 1u : 0u;
+      if (r < a.n_resident) {
+        o = __ldcg(reinterpret_cast<const uint4*>(a.before + r));
+        changed = v.x != o.x || v.y != o.y || v.z != o.z || v.w != o.w;
+        const bool was = (o.z & LWSE_PLACE_PLACED) != 0u, is = (v.z & LWSE_PLACE_PLACED) != 0u;
+        c[0] += (was && !is) ? 1u : 0u;
+        c[1] += (was && is && o.x != v.x) ? 1u : 0u;
+        c[2] += (!was && is) ? 1u : 0u;
+      }
+    }
+    const uint32_t mask = __ballot_sync(0xFFFFFFFFu, changed);
+    if (mask == 0u) continue;  // warp-uniform
+    uint32_t at = 0;
+    if (lane == 0) at = atomicAdd(a.counts, (uint32_t)__popc(mask));
+    at = __shfl_sync(0xFFFFFFFFu, at, 0) + (uint32_t)__popc(mask & ((1u << lane) - 1u));
+    if (changed && at < a.capacity) {
+      a.rows[at] = r;
+      *reinterpret_cast<uint4*>(a.outs_before + at) = o;
+      *reinterpret_cast<uint4*>(a.outs_after + at) = v;
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 6; k++) {
+    const uint32_t sum = __reduce_add_sync(0xFFFFFFFFu, c[k]);
+    if (lane == 0 && sum) atomicAdd(a.counts + 1 + k, sum);
+  }
+}
+
+int launch_place_whatif_diff(const lwse_place_out* d_before, const lwse_place_out* d_after, uint32_t n_resident, uint32_t n_total,
+                             uint32_t* d_rows, lwse_place_out* d_outs_before, lwse_place_out* d_outs_after, uint32_t capacity,
+                             uint32_t* d_counts, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  const WhatIfDiffArgs a{d_before, d_after, d_rows, d_outs_before, d_outs_after, d_counts, capacity, n_resident, n_total};
+  uint64_t grid = ((uint64_t)n_total + 255) / 256;
+  if (grid < 1) grid = 1;
+  if (grid > (uint64_t)sm_count * 4u) grid = (uint64_t)sm_count * 4u;
+  place_whatif_diff_kernel<<<(unsigned)grid, 256, 0, s>>>(a);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    *cuda_err = (int)e;
+    return -1;
+  }
+  return 1;
+}
+
 }  // namespace lwse

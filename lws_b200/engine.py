@@ -43,6 +43,7 @@ SYMBOLS = {
     "lwse_resident_occupancy": ([C.c_void_p, C.c_void_p], C.c_int),
     "lwse_resident_tick_info": ([C.c_void_p, C.c_void_p], C.c_int),
     "lwse_resident_node_info": ([C.c_void_p, C.POINTER(R.NodeInfo)], C.c_int),
+    "lwse_resident_place_whatif": ([C.c_void_p, C.POINTER(R.PlaceWhatIf)], C.c_int),
     "lwse_place_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
         C.c_int,
@@ -399,6 +400,36 @@ class Engine:
         info = R.NodeInfo()
         self._check(lib().lwse_resident_node_info(self._h, C.byref(info)))
         return {"rows_patched": info.rows_patched, "index_built": bool(info.index_built), "n_usable": info.n_usable}
+
+    def resident_place_whatif(self, segs=(), extra=None, n_namespaces=0, capacity=None):
+        """lwse_resident_place_whatif: the placement round over the resident tables with ``segs`` (NODES and
+        PLACE_REQS segments, as ``make_tick`` takes them) applied and the ``extra`` request rows appended —
+        nothing resident changes, and no tick is waited for.  ``capacity`` None lists every changed row.
+        → dict: ``rows`` / ``before`` / ``after`` (the resident rows that differ from the last round, with
+        both rows), ``extra_out`` (the rows of the extra requests), the counters of ``records.PLACE_WHATIF``
+        and ``form`` (namespace | general)."""
+        tick = self.make_tick(segs)
+        n_res = getattr(self, "_n_place", 0)
+        extra = R.aligned_empty(0, R.PLACE_REQ) if extra is None else _aligned16(np.asarray(extra, dtype=R.PLACE_REQ))
+        cap = n_res if capacity is None else int(capacity)
+        rows = np.zeros(max(cap, 1), np.uint32)
+        before, after = R.aligned_empty(max(cap, 1), R.PLACE_OUT), R.aligned_empty(max(cap, 1), R.PLACE_OUT)
+        extra_out = R.aligned_empty(max(len(extra), 1), R.PLACE_OUT)
+        q = R.PlaceWhatIf()
+        q.segs = C.cast(tick.segs, C.c_void_p) if len(segs) else None
+        q.n_segs = len(segs)
+        q.extra = R.ptr(extra) if len(extra) else None
+        q.n_extra = len(extra)
+        q.n_namespaces = int(n_namespaces)
+        q.capacity = cap
+        q.rows, q.before, q.after = R.ptr(rows), R.ptr(before), R.ptr(after)
+        q.extra_out = R.ptr(extra_out) if len(extra) else None
+        self._check(lib().lwse_resident_place_whatif(self._h, C.byref(q)))
+        n = min(q.n_changed, cap)
+        out = {"rows": rows[:n], "before": before[:n], "after": after[:n], "extra_out": extra_out[: len(extra)],
+               "form": self.TICK_FORMS[q.form]}
+        out.update({k: getattr(q, k) for k in R.PLACE_WHATIF})
+        return out
 
     def resident_patch(self, which: int, rows, values):
         """Overwrite rows of a resident table (rows: uint32 indices, values: packed rows)."""

@@ -474,6 +474,69 @@ class IncrementalEncoder:
         del patches._pending
         return patches
 
+    # ------------------------------------------------------------- what-if
+    # Segments and extra rows for ``Engine.resident_place_whatif``, built from the state of the last
+    # ``flush()``.  None of them changes the encoder: no namespace id, slot, spare row or node row is
+    # taken.  They model node cordons and capacity changes and new exclusive groups; they do not model
+    # node deletion or eviction, which move occupancy (the what-if takes no identity patches).
+    def _whatif_nodes(self, names, edit) -> tuple:
+        rows = np.array(sorted({self.node_index[n] for n in names}), dtype=np.uint32)
+        vals = R.aligned_empty(len(rows), R.NODE_REC)
+        vals[:] = self._node_resident[rows]
+        edit(vals)
+        return R.TABLE_NODES, rows, vals
+
+    def whatif_cordon(self, node_names) -> tuple:
+        """A NODES segment of the named nodes' resident rows with NODE_SCHEDULABLE cleared."""
+        def cordon(v):
+            v["flags"] &= ~np.uint16(R.NODE_SCHEDULABLE)
+        return self._whatif_nodes(node_names, cordon)
+
+    def whatif_capacity(self, node_name: str, capacity: int) -> tuple:
+        """A NODES segment that sets one node's capacity (pods it can hold)."""
+        def resize(v):
+            v["capacity"] = capacity
+        return self._whatif_nodes([node_name], resize)
+
+    @staticmethod
+    def _whatif_requests(uid_hash: int, size: int, ns: int, group_indices) -> np.ndarray:
+        """Request rows of an exclusive object's groups whose leader pods exist and are not scheduled, with
+        the priority and key mix of ``encoder.encode_place_requests`` (the same function computes them)."""
+        gidx = np.asarray(list(group_indices), dtype=np.int64)
+        if len(gidx) == 0:
+            return R.aligned_empty(0, R.PLACE_REQ)
+        lws = R.aligned_empty(1, R.LWS_REC)
+        lws["uid_hash"], lws["size"], lws["flags"] = uid_hash, size, R.LWS_EXCLUSIVE_TOPOLOGY
+        groups = R.aligned_empty(int(gidx.max()) + 1, R.GROUP_REC)
+        groups["leader_node"] = R.NONE
+        groups["flags"][gidx] = R.GRP_POD_PRESENT
+        reqs = encoder.encode_place_requests(lws, groups)
+        reqs["ns"] = ns
+        return reqs
+
+    def whatif_new_lws(self, item: encoder.LwsItem) -> tuple:
+        """Extra rows for a LeaderWorkerSet that is not resident, created with its ``replicas`` groups
+        (indices 0 .. replicas-1, leaders not yet scheduled) → (rows, n_namespaces to pass).  A namespace
+        the encoder has not seen gets the id the next flush would give it; n_namespaces covers it."""
+        t = encoder.encode_lws([item], encoder.Cluster(pods=[], statefulsets=[]), self.topology_key,
+                               encoded_nodes=self._encoded_nodes)
+        ns = self.ns_ids.get(item.lws.namespace, len(self.ns_ids))
+        n_ns = max(self.n_namespaces, ns + 1)
+        if not len(t.lws) or not (int(t.lws["flags"][0]) & R.LWS_EXCLUSIVE_TOPOLOGY):
+            return R.aligned_empty(0, R.PLACE_REQ), n_ns
+        return self._whatif_requests(int(t.lws["uid_hash"][0]), int(t.lws["size"][0]), ns,
+                                     range(max(item.lws.replicas, 0))), n_ns
+
+    def whatif_scale(self, key: tuple, replicas: int) -> np.ndarray:
+        """Extra rows for the groups a resident object would add when scaled to ``replicas``: indices from
+        its current ``replicas`` up (leaders not yet scheduled).  Empty for a scale-down or a
+        non-exclusive object."""
+        row = self.slots[key].lws_row
+        if not (int(self.lws["flags"][row]) & R.LWS_EXCLUSIVE_TOPOLOGY):
+            return R.aligned_empty(0, R.PLACE_REQ)
+        return self._whatif_requests(int(self.lws["uid_hash"][row]), int(self.lws["size"][row]), self.ns_ids[key[0]],
+                                     range(self.items[key].lws.replicas, replicas))
+
     # ------------------------------------------------------------------ results
     def tables(self):
         """(lws, groups, pod_state, pod_ident, reqs) trimmed to the rows in use (+ spare already laid out)."""

@@ -470,6 +470,38 @@ class LwsForecastOut(C.Structure):
     ]
 
 
+class PlaceWhatIf(C.Structure):
+    """lwse_place_whatif: a hypothetical placement round over the resident tables (segments and extra
+    rows in, changed rows and the PLACE_WHATIF counters out)."""
+
+    _fields_ = [
+        ("segs", C.c_void_p),
+        ("n_segs", C.c_uint32),
+        ("extra", C.c_void_p),
+        ("n_extra", C.c_uint32),
+        ("n_namespaces", C.c_uint32),
+        ("capacity", C.c_uint32),
+        ("rows", C.c_void_p),
+        ("before", C.c_void_p),
+        ("after", C.c_void_p),
+        ("extra_out", C.c_void_p),
+        ("n_changed", C.c_uint32),
+        ("n_lost", C.c_uint32),
+        ("n_moved", C.c_uint32),
+        ("n_gained", C.c_uint32),
+        ("n_placed", C.c_uint32),
+        ("n_unschedulable", C.c_uint32),
+        ("n_conflict", C.c_uint32),
+        ("namespaces_solved", C.c_uint32),
+        ("form", C.c_uint32),
+    ]
+
+
+# the counters of a what-if, as Engine.resident_place_whatif returns them
+PLACE_WHATIF = ("n_changed", "n_lost", "n_moved", "n_gained", "n_placed", "n_unschedulable", "n_conflict",
+                "namespaces_solved")
+
+
 class Config(C.Structure):
     _fields_ = [
         ("abi_version", C.c_uint32),
