@@ -504,7 +504,7 @@ LWSE_API int lwse_resident_occupancy(lwse_engine* e, uint32_t* occupancy_out);
  * namespace runs the namespace-parallel form; one that is not (a patch moved a request to another
  * namespace) runs the same form through a namespace index the device builds, rebuilt by the ticks
  * whose patches change a request's namespace.  The general form only runs where the namespace form
- * cannot: too many domains for one CTA's shared memory, or LWSE_PLACE_FORM=general. */
+ * cannot: too many domains for one CTA's shared memory. */
 typedef struct lwse_tick_info {
   uint32_t place_form;  /* LWSE_TICK_FORM_*                                                   */
   uint32_t indexed;     /* 1: the namespace form read the requests through the namespace index */
@@ -747,8 +747,8 @@ LWSE_API int lwse_reconcile_host(lwse_engine* e, const lwse_lws_tables* host, co
  * count, or a NULL buffer with a count > 0; LWSE_ERR_BAD_TABLE for a range segment beyond its table (as
  * a tick).  LWSE_ERR_UNSUPPORTED when rn_reqs + n_extra >= 2^24 (row keys are 24-bit) and on an
  * engine with a peer exchange (the shared-occupancy round).  The scan form is not offered (it gives
- * the same rows by spec); where a tick would run the general form (the domains do not fit one CTA, or
- * LWSE_PLACE_FORM=general) the what-if does too. */
+ * the same rows by spec); where a tick would run the general form (the domains do not fit one CTA) the
+ * what-if does too. */
 typedef struct lwse_place_whatif {
   /* in */
   const lwse_patch_seg* segs;     /* LWSE_TABLE_NODES and LWSE_TABLE_PLACE_REQS only, the packing of a

@@ -39,8 +39,6 @@ struct PublishListHost {
 int launch_publish(const PublishListHost* lists, const uint32_t* d_extra, uint32_t* h_words, uint32_t seq_slot,
                    uint32_t seq, uint32_t* d_ticket, uint32_t expected_rows, cudaStream_t s, int* cuda_err,
                    uint32_t* d_clear, uint32_t n_clear, bool pdl);
-cudaError_t set_sweep_carveout(int pct);
-cudaError_t set_place_ns_carveout(int pct);
 int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uint32_t n_nodes,
                      void* scratch, int sm_count, cudaStream_t s, int* cuda_err, const SweepChangeLists* cl,
                      uint32_t* d_event_count = nullptr, int first_mode = 1);
@@ -310,10 +308,8 @@ struct lwse_engine {
   int use_graph = 1;                 // LWSE_TICK_GRAPH: 0 never, 1 when a tick is in flight (default), 2 always
   uint64_t graph_ticks = 0;
   cudaEvent_t ev_pub = nullptr;      // behind the previous tick's publish kernel: the next tick's side stream starts there
-  int tick_order = 0;                // LWSE_TICK_ORDER (A/B of the tick's enqueue order, see tick_locked)
   uint32_t* h_counts = nullptr;      // pinned, 2 words
   DevBuf h_counts_dev;               // event-pod count of the host entry point's sweep
-  bool no_zero_copy = false;         // LWSE_NO_ZERO_COPY=1: always upload the identity column
   uint32_t place_calls = 0;          // selects the scratch half
   uint32_t place_geometry[4] = {0, 0, 0, 0};  // (n_reqs, n_namespaces, nodes, domains) the scratch was laid out for
   cudaEvent_t ev_place = nullptr;    // end of the last placement call: the next one (any stream) orders behind it
@@ -547,19 +543,8 @@ LWSE_API int lwse_create(const lwse_config* cfg, lwse_engine** out) {
     return LWSE_ERR_OOM;
   }
   {
-    const char* v = getenv("LWSE_NO_ZERO_COPY");
-    e->no_zero_copy = v && atoi(v) != 0;
-    const char* o = getenv("LWSE_TICK_ORDER");
-    e->tick_order = o ? atoi(o) : 0;
-    if (e->tick_order < 0 || e->tick_order > 2) e->tick_order = 0;
     const char* g = getenv("LWSE_TICK_GRAPH");
     e->use_graph = g ? atoi(g) : 1;
-    const char* c = getenv("LWSE_SMEM_CARVEOUT");  // percent of the maximum shared memory, every tick kernel alike
-    if (c && atoi(c) >= 0 && atoi(c) <= 100) {
-      (void)lwse::set_sweep_carveout(atoi(c));
-      (void)lwse::set_place_ns_carveout(atoi(c));
-      (void)cudaGetLastError();
-    }
   }
   *out = e;
   return LWSE_OK;
@@ -817,7 +802,7 @@ static int sweep_host_locked(lwse_engine* e, const lwse_lws_tables* h, const std
     //    synchronize; the first sweep of a table is optimistic).
     const bool reuse = (h->flags & LWSE_SWEEP_REUSE_POD_IDENT) && e->ident_rows == h->n_pods && !ident_moved;
     const void* mapped = nullptr;
-    if (!reuse && !e->no_zero_copy && !want_occ) {
+    if (!reuse && !want_occ) {
       cudaPointerAttributes attr;
       if (cudaPointerGetAttributes(&attr, h->pod_ident) == cudaSuccess && attr.type == cudaMemoryTypeHost)
         mapped = attr.devicePointer;
@@ -1124,14 +1109,10 @@ static int apply_patches_locked(lwse_engine* e, const lwse_patch_seg* segs, uint
     // Few patch bytes: the scatter kernel reads them in place over PCIe (one round trip, no copy
     // launch).  Many: one DMA copy per pinned buffer of the span this call uses, then the kernel
     // reads device memory — the copy engine moves large spans several times faster than SM reads of host memory.
-    static const long dma_threshold = [] {
-      const char* v = getenv("LWSE_PATCH_DMA_BYTES");
-      return v ? atol(v) : 16384L;
-    }();
+    constexpr long kDmaBytes = 16384;
     size_t total = 0;
     for (int k = 0; k < n_sc; k++) total += (size_t)sc[k].n * (4u + sc[k].row_bytes);
-    const long dma_from = dma_threshold < 0 ? -1 : (dma_min_bytes > dma_threshold ? dma_min_bytes : dma_threshold);
-    if (dma_from >= 0 && total >= (size_t)dma_from) {
+    if (total >= (size_t)(dma_min_bytes > kDmaBytes ? dma_min_bytes : kDmaBytes)) {
       struct Span { const PinBuf* pin; DevBuf* mirror; uintptr_t lo, hi; } spans[2] = {
           {&e->arena, &e->arena_mirror, UINTPTR_MAX, 0}, {&e->stage, &e->stage_mirror, UINTPTR_MAX, 0}};
       auto touch = [&](const void* dptr, size_t bytes) {
@@ -1252,11 +1233,6 @@ LWSE_API int lwse_resident_outputs(lwse_engine* e, lwse_lws_out* lws_out, lwse_g
 // Placement
 // ---------------------------------------------------------------------------
 constexpr uint32_t kFormGeneral = 0, kFormGrouped = 1, kFormScan = 2;
-static const int g_place_form_env = [] {  // LWSE_PLACE_FORM=general|grouped|scan: A/B measurements
-  const char* v = getenv("LWSE_PLACE_FORM");
-  if (!v) return -1;
-  return v[0] == 'g' && v[1] == 'e' ? 0 : v[0] == 's' ? 2 : 1;
-}();
 
 // The namespace-parallel form (request table grouped by namespace): condense kernel + one CTA per
 // namespace.  `first_pdl`: nothing on the stream right before writes the request table.  `index` other
@@ -1314,8 +1290,6 @@ static int place_locked(lwse_engine* e, const lwse_place_req* d_reqs, uint32_t n
                         lwse::PlaceNsIndex index = lwse::kNsIndexNone) {
   if ((n_reqs && (!d_reqs || !d_out)) || n_namespaces == 0) return LWSE_ERR_INVALID_ARG;
   if (e->n_nodes == 0 || e->n_domains == 0) return LWSE_ERR_NOT_READY;
-  if (g_place_form_env == 0) form = kFormGeneral;
-  if (g_place_form_env == 2 && form != kFormGeneral) form = kFormScan;
   if (diffed) *diffed = false;
   if (form != kFormGeneral && n_parts <= 1 && lwse::place_ns_supported(e->n_nodes, e->n_domains)) {
     if (diffed) *diffed = changes != nullptr;
@@ -1699,7 +1673,7 @@ LWSE_API int lwse_reconcile_host(lwse_engine* e, const lwse_lws_tables* h, const
     const int prc = place_locked(e, (const lwse_place_req*)e->place_reqs.p, n_reqs, (const uint32_t*)e->place_occ.p, n_namespaces,
                                  (lwse_place_out*)e->place_out.p, nullptr, ps, 1, n_reqs, 0, false, form);
     if (prc != LWSE_OK) return prc;
-    if (promised && g_place_form_env != 0 && e->place_scans_ptr != nullptr) {  // (the namespace kernels ran: their counter block)
+    if (promised && e->place_scans_ptr != nullptr) {  // (the namespace kernels ran: their counter block)
       LWSE_CUDA(e, cudaMemcpyAsync(e->h_rounds + 8, e->place_rounds_ptr + 2, 4, cudaMemcpyDeviceToHost, ps));
       check_order = true;
     }
@@ -1859,19 +1833,37 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
       ns_moves = row < e->rn_reqs && v[k].ns != e->r_req_ns[row];
     }
   }
-  const bool ns_form = do_place && g_place_form_env != 0 && lwse::place_ns_supported(e->n_nodes, e->n_domains);
+  const bool ns_form = do_place && lwse::place_ns_supported(e->n_nodes, e->n_domains);
   const bool indexed = ns_form && !(e->r_place_grouped && !ns_moves);
   const lwse::PlaceNsIndex ns_index = !indexed                              ? lwse::kNsIndexNone
                                       : (ns_moves || !e->r_ns_index_ok) ? lwse::kNsIndexBuild
                                                                           : lwse::kNsIndexReuse;
-  const bool scan_form = (flags & LWSE_SWEEP_PLACE_SCAN) || g_place_form_env == 2;
+  const bool scan_form = (flags & LWSE_SWEEP_PLACE_SCAN) != 0;
   // Node rows: the mirror decides, before anything is enqueued, whether this tick's round rebuilds the node
   // index (also part of a tick graph's key).  A tick without a round leaves a stale index to the next one.
   const int node_rows = node_patches_locked(e, segs, n_segs);
   if (node_rows < 0) return node_rows;
   const bool node_rebuild = do_place && e->node_index_stale;
   e->last_node_info = lwse_node_info{(uint32_t)node_rows, node_rebuild ? 1u : 0u, e->n_usable, 0u};
-  auto record_info = [&](bool graph) {
+  // sequence numbers count the ticks that end in a publish kernel (the device counts the same ones)
+  uint32_t seq = 0;
+  if (do_sweep || do_place) {
+    seq = ++e->tick_seq;
+    if (seq == 0) seq = ++e->tick_seq;
+  }
+  // The bookkeeping that closes a submitted tick.  `wrote_any`: the tick patched a table; `wrote_main`: it
+  // patched a table on the engine's stream.
+  auto close_submit = [&](bool published, bool wrote_any, bool wrote_main, bool graph) {
+    lwse_engine::TickSlot& ts = e->tslot[slot];
+    ts.seq = seq;
+    ts.do_sweep = do_sweep;
+    ts.do_place = do_place;
+    ts.published = published;
+    ts.wrote = wrote_any;
+    e->t_submitted++;
+    if (do_sweep) e->r_swept = e->r_groups_swept = true;
+    if (round_asked) e->r_place_current = true;
+    e->main_unforked = !do_place && (e->main_unforked || wrote_main);
     lwse_tick_info& ti = e->last_tick_info;
     ti.place_form = !do_place ? LWSE_TICK_FORM_NONE
                     : !ns_form ? LWSE_TICK_FORM_GENERAL
@@ -1882,12 +1874,6 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
     ti.graph = graph ? 1u : 0u;
     if (indexed) e->r_ns_index_ok = true;  // (also after a replay, which enqueues no call that would say so)
   };
-  // sequence numbers count the ticks that end in a publish kernel (the device counts the same ones)
-  uint32_t seq = 0;
-  if (do_sweep || do_place) {
-    seq = ++e->tick_seq;
-    if (seq == 0) seq = ++e->tick_seq;
-  }
   {
     const size_t ub = stage_bytes_upper_bound(segs, n_segs);
     if (ub > e->stage.cap) {  // rare: only segments outside the arena are staged
@@ -1925,14 +1911,6 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
   int rc = LWSE_OK;
   int cuda_err = 0;
   cudaStream_t ps = e->side_stream;
-  // Enqueue order (every call costs microseconds of host time, and the copy of the pod patches is the
-  // head of the critical path):
-  //   0 (default)  copy of the pod patches; the round's launches on the side stream while the copy
-  //                engine works; then the scatter and the sweep behind the copy
-  //   1            the round's launches first, then copy + scatter + sweep (segments in the arena only)
-  //   2            copy + scatter, the round, the sweep
-  // With identity or node patches the round forks behind the main scatter (it reads the occupancy
-  // counters and the node rows).
   bool all_in_place = true;  // no segment needs the staging buffer
   for (uint32_t i = 0; i < n_segs; i++) {
     if (!segs[i].n || (segs[i].flags & LWSE_PATCH_RANGE)) continue;
@@ -1942,8 +1920,6 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
     if (!resident_table(e, segs[i].table, &tb, &trows, &rb)) return LWSE_ERR_INVALID_ARG;
     if (!rows_in_place(e, segs[i]) || !values_in_place(e, segs[i], rb)) all_in_place = false;
   }
-  int order = fork_behind_main ? 2 : e->tick_order;
-  if (order == 1 && !all_in_place) order = 0;  // (the two calls share the staging buffer: main part first)
   if (in_flight) {
     // a tick is still running.  Its DMA may still read the staging buffer: segments outside the arena
     // wait for it.  Its publish kernel (the last thing on the engine's stream) still has to copy and
@@ -1970,6 +1946,14 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
     return apply_patches_locked(e, segs, n_segs, &wrote_side, kSideTables, ps, stage_used, nullptr, /*dma_min_bytes=*/65536);
   };
   lwse::PublishListHost pl[3] = {};
+  // the publish kernel's entry for this slot's change list k: 0 LWS rows, 1 group rows, 2 placement rows
+  auto publish_list = [&](int k) -> lwse::PublishListHost {
+    const uint32_t capacity[3] = {e->rn_lws, e->rn_groups, e->rn_reqs};
+    const uint32_t out_bytes[3] = {sizeof(lwse_lws_out), sizeof(lwse_group_out), sizeof(lwse_place_out)};
+    return {reinterpret_cast<uint32_t*>(chg_v + e->chg_off[2 * k]), chg_v + e->chg_off[2 * k + 1],
+            reinterpret_cast<uint32_t*>(chg_d + e->chg_off[2 * k]), chg_d + e->chg_off[2 * k + 1], cnt + (k == 2 ? 4 : k),
+            capacity[k], out_bytes[k]};
+  };
   int sweep_first_mode = -1;      // -1: 2 behind this tick's scatter kernel, else 1 (see launch_lws_sweep)
   bool place_first_pdl = true;    // the round's first kernel follows a kernel on the side stream
   void* place_mid_event = nullptr;  // (graph capture) recorded between the condense and the namespace kernel
@@ -1997,10 +1981,8 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
                                           &cuda_err, &cl, nullptr, sweep_first_mode >= 0 ? sweep_first_mode : (wrote ? 2 : 1));
     if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
     e->launches += (uint64_t)launched;
-    pl[0] = {cl.lws_rows, cl.lws_out, reinterpret_cast<uint32_t*>(chg_d + e->chg_off[0]), chg_d + e->chg_off[1],
-             cnt + 0, e->rn_lws, (uint32_t)sizeof(lwse_lws_out)};
-    pl[1] = {cl.group_rows, cl.group_out, reinterpret_cast<uint32_t*>(chg_d + e->chg_off[2]), chg_d + e->chg_off[3],
-             cnt + 1, e->rn_groups, (uint32_t)sizeof(lwse_group_out)};
+    pl[0] = publish_list(0);
+    pl[1] = publish_list(1);
     return LWSE_OK;
   };
   auto enqueue_place = [&]() -> int {
@@ -2028,8 +2010,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
       if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
       e->launches += (uint64_t)launched;
     }
-    pl[2] = {changes.rows, changes.outs, reinterpret_cast<uint32_t*>(chg_d + e->chg_off[4]), chg_d + e->chg_off[5], changes.count,
-             e->rn_reqs, (uint32_t)sizeof(lwse_place_out)};
+    pl[2] = publish_list(2);
     e->tick_place_ns = diffed;
     return LWSE_OK;
   };
@@ -2174,53 +2155,32 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
       e->graph_ticks++;
       if (shared_occ) e->xch_step++;  // (the replayed push kernel advanced the device counter by one)
       if (!pl[0].count && do_sweep) {  // (replayed without capturing: the lists the graph's kernels append to)
-        pl[0] = {reinterpret_cast<uint32_t*>(chg_v + e->chg_off[0]), chg_v + e->chg_off[1], reinterpret_cast<uint32_t*>(chg_d + e->chg_off[0]),
-                 chg_d + e->chg_off[1], cnt + 0, e->rn_lws, (uint32_t)sizeof(lwse_lws_out)};
-        pl[1] = {reinterpret_cast<uint32_t*>(chg_v + e->chg_off[2]), chg_v + e->chg_off[3], reinterpret_cast<uint32_t*>(chg_d + e->chg_off[2]),
-                 chg_d + e->chg_off[3], cnt + 1, e->rn_groups, (uint32_t)sizeof(lwse_group_out)};
+        pl[0] = publish_list(0);
+        pl[1] = publish_list(1);
       }
-      if (!pl[2].count && do_place)
-        pl[2] = {reinterpret_cast<uint32_t*>(chg_v + e->chg_off[4]), chg_v + e->chg_off[5], reinterpret_cast<uint32_t*>(chg_d + e->chg_off[4]),
-                 chg_d + e->chg_off[5], cnt + 4, e->rn_reqs, (uint32_t)sizeof(lwse_place_out)};
+      if (!pl[2].count && do_place) pl[2] = publish_list(2);
       if (do_place) {
         e->tick_place_ns = tg.place_ns;
         e->place_rounds_ptr = tg.rounds_ptr;
       }
       rc = enqueue_publish();
       if (rc != LWSE_OK) return rc;
-      lwse_engine::TickSlot& gts = e->tslot[slot];
-      gts.seq = seq;
-      gts.do_sweep = do_sweep;
-      gts.do_place = do_place;
-      gts.published = true;
-      gts.wrote = has_patches;
-      e->t_submitted++;
-      if (do_sweep) e->r_swept = e->r_groups_swept = true;
-      if (round_asked) e->r_place_current = true;
-      e->main_unforked = !do_place && (e->main_unforked || has_patches);
-      record_info(true);
+      close_submit(true, has_patches, has_patches, true);
       return LWSE_OK;
     }
   }
-  if (order == 1) {
-    rc = apply_side();
-    if (rc == LWSE_OK && do_place) rc = enqueue_place();
-    if (rc == LWSE_OK) rc = apply_main(false);
-    if (rc == LWSE_OK && do_sweep) rc = enqueue_sweep();
-  } else if (order == 0) {
-    rc = apply_main(true);
-    if (rc == LWSE_OK) rc = apply_side();
-    if (rc == LWSE_OK && do_place && wrote) rc = enqueue_place();
-    if (rc == LWSE_OK) rc = launch_scatter_plan(e, main_plan, s);
-    if (rc == LWSE_OK && do_sweep) rc = enqueue_sweep();
-    if (rc == LWSE_OK && do_place && !wrote) rc = enqueue_place();
-  } else {
-    rc = apply_main(false);
-    if (rc == LWSE_OK) rc = apply_side();
-    if (rc == LWSE_OK && do_place && wrote) rc = enqueue_place();
-    if (rc == LWSE_OK && do_sweep) rc = enqueue_sweep();
-    if (rc == LWSE_OK && do_place && !wrote) rc = enqueue_place();
-  }
+  // Eager enqueue order.  Every call costs microseconds of host time and the copy of the pod patches
+  // heads the critical path, so that copy is enqueued first; the round's launches follow on the side
+  // stream while the copy engine works, then the main scatter and the sweep behind the copy.  A round
+  // that forks behind the main scatter (identity or node patches: it reads the occupancy counters and
+  // the node rows) needs that scatter enqueued before it, so the scatter is not deferred then.
+  const bool defer_scatter = !fork_behind_main;
+  rc = apply_main(defer_scatter);
+  if (rc == LWSE_OK) rc = apply_side();
+  if (rc == LWSE_OK && do_place && wrote) rc = enqueue_place();
+  if (rc == LWSE_OK && defer_scatter) rc = launch_scatter_plan(e, main_plan, s);
+  if (rc == LWSE_OK && do_sweep) rc = enqueue_sweep();
+  if (rc == LWSE_OK && do_place && !wrote) rc = enqueue_place();
   if (rc != LWSE_OK) return rc;
   if (do_place || wrote_side) {
     LWSE_CUDA(e, cudaEventRecord(e->ev_join, ps));
@@ -2231,17 +2191,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
     rc = enqueue_publish();
     if (rc != LWSE_OK) return rc;
   }
-  lwse_engine::TickSlot& ts = e->tslot[slot];
-  ts.seq = seq;
-  ts.do_sweep = do_sweep;
-  ts.do_place = do_place;
-  ts.published = published;
-  ts.wrote = wrote || wrote_side;
-  e->t_submitted++;
-  if (do_sweep) e->r_swept = e->r_groups_swept = true;
-  if (round_asked) e->r_place_current = true;
-  e->main_unforked = !do_place && (e->main_unforked || wrote);
-  record_info(false);
+  close_submit(published, wrote || wrote_side, wrote, false);
   return LWSE_OK;
 }
 
@@ -2486,7 +2436,7 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
     cursor += align256(bytes);
     return at;
   };
-  const bool ns_form = g_place_form_env != 0 && lwse::place_ns_supported(e->n_nodes, e->n_domains);
+  const bool ns_form = lwse::place_ns_supported(e->n_nodes, e->n_domains);
   const size_t b_nodes = (size_t)e->n_nodes * sizeof(lwse_node_rec);
   const size_t b_out = (size_t)n_total * sizeof(lwse_place_out);
   LWSE_CUDA(e, e->wf_reqs.reserve((size_t)n_total * sizeof(lwse_place_req) + 16));

@@ -557,12 +557,7 @@ struct DirectBits {
   }
 };
 
-#ifdef LWSE_FUSED_MAXNREG  // build-time experiment switch, see lwse_place_ns_kernels.cu
-#define LWSE_FUSED_BOUNDS __maxnreg__(LWSE_FUSED_MAXNREG)
-#else
-#define LWSE_FUSED_BOUNDS __launch_bounds__(kFusedThreads, 3)
-#endif
-__global__ void LWSE_FUSED_BOUNDS group_fused_kernel(const GroupSweepArgs a) {
+__global__ void __launch_bounds__(kFusedThreads, 3) group_fused_kernel(const GroupSweepArgs a) {
   __shared__ uint32_t s_pend[kWinWords], s_ev[kWinWords];
   __shared__ uint32_t s_pair[kPairCap];  // tid << 16 | pod index relative to the window start
   __shared__ uint4 s_ctx4[kFusedThreads];
@@ -768,21 +763,11 @@ __global__ void __launch_bounds__(256) lws_sweep_kernel(const LwsSweepArgs a) {
 // --------------------------------------------------------------------------
 // launchers
 // --------------------------------------------------------------------------
-// LWSE_NO_PDL=1 turns programmatic dependent launch off (A/B measurements).
-static const bool g_pdl = [] {
-  const char* v = getenv("LWSE_NO_PDL");
-  return !(v && v[0] == '1');
-}();
-
 int pick_tile(uint64_t items, uint64_t owners) {  // (also the forecast's tile, lwse_lws_forecast_kernels.cu)
   // Lanes per object: a lane handles 8 groups per 64-bit word, and every lane of a tile runs the
   // object-level logic (the five cases, the walk) itself — one lane per object until objects
   // average more than 64 groups, then next power of two >= avg / 64, in [1, 32].
-  static const uint64_t div = [] {
-    const char* v = getenv("LWSE_LWS_TILE_DIV");
-    const int d = v ? atoi(v) : 64;
-    return (uint64_t)(d < 1 ? 1 : d);
-  }();
+  constexpr uint64_t div = 64;
   if (owners == 0) return 1;
   const uint64_t avg = ((items + owners - 1) / owners + div - 1) / div;
   int w = 1;
@@ -805,8 +790,7 @@ static cudaError_t launch_group(const GroupSweepArgs& a, int sm_count, cudaStrea
   constexpr uint32_t kTilesPerBlock = kGroupThreads / W;
   (void)sm_count;
   const uint32_t want = (a.n_groups + kTilesPerBlock - 1) / kTilesPerBlock;
-  return launch_pdl(group_sweep_kernel<W>, dim3(want < (1u << 20) ? want : (1u << 20)), dim3(kGroupThreads), 0, s,
-                    g_pdl, a);
+  return launch_pdl(group_sweep_kernel<W>, dim3(want < (1u << 20) ? want : (1u << 20)), dim3(kGroupThreads), 0, s, true, a);
 }
 
 template <int W>
@@ -815,7 +799,7 @@ static cudaError_t launch_lws(const LwsSweepArgs& a, int sm_count, cudaStream_t 
   static uint32_t resident = 0;
   if (resident == 0) resident = resident_ctas(lws_sweep_kernel<W>, sm_count);
   const uint32_t want = (a.n_lws + kTilesPerBlock - 1) / kTilesPerBlock;
-  return launch_pdl(lws_sweep_kernel<W>, dim3(want < resident ? want : resident), dim3(256), 0, s, g_pdl, a);
+  return launch_pdl(lws_sweep_kernel<W>, dim3(want < resident ? want : resident), dim3(256), 0, s, true, a);
 }
 
 constexpr int kScanUnroll = 4;  // 128-bit loads per lane per chunk: 4 x 512 B = 2 KB in flight per warp
@@ -863,19 +847,11 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
   // lanes per group: one per bitmap word of an average group, in {1, 2, 4, 8}
   const uint64_t avg_pods = t->n_groups ? (t->n_pods + t->n_groups - 1) / t->n_groups : 0;
   const int w = avg_pods > 2048 ? 8 : avg_pods > 1024 ? 4 : avg_pods > 512 ? 2 : 1;
-  static const bool no_fuse = [] {
-    const char* v = getenv("LWSE_NO_FUSE");
-    return v && atoi(v) != 0;
-  }();
   // scan + group pass in one kernel: mid-sized groups, both passes wanted.  Upper bound: the pod
   // window of 256 consecutive groups has to fit the CTA's bitmap window of 65 536 pods.  Lower bound:
   // with a handful of pods per group a CTA of 256 groups streams only 2-4 KB of state and the
   // kernel is all per-group work, and the scan and the group pass as two kernels are faster.
-  static const uint64_t fuse_min_pods = [] {
-    const char* v = getenv("LWSE_FUSE_MIN_PODS");
-    return v ? (uint64_t)atol(v) : (uint64_t)16;
-  }();
-  const bool fused = group_pass && avg_pods <= 256 && avg_pods >= fuse_min_pods && !no_fuse && !(t->flags & LWSE_SWEEP_SKIP_POD_SCAN);
+  const bool fused = group_pass && avg_pods <= 256 && avg_pods >= 16 && !(t->flags & LWSE_SWEEP_SKIP_POD_SCAN);
   if (t->node_occupancy && n_nodes && !(t->flags & LWSE_SWEEP_SKIP_POD_SCAN)) {
     e = cudaMemsetAsync(t->node_occupancy, 0, (size_t)n_nodes * sizeof(uint32_t), s);
     if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
@@ -894,7 +870,7 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
     if (cl && cl->group_rows) a.changes = ChangeList{cl->group_rows, cl->group_out, cl->counts + 1, cl->group_capacity};
     const uint32_t grid = (t->n_groups + kFusedThreads - 1) / kFusedThreads;
     // (a memset / occupancy kernel right before: an ordinary launch orders behind it)
-    const bool pdl = g_pdl && !t->node_occupancy && first_mode != 0;
+    const bool pdl = !t->node_occupancy && first_mode != 0;
     if (pdl && first_mode == 2) a.sweep_flags |= kSweepWaitAtTop;
     e = launch_pdl(group_fused_kernel, dim3(grid), dim3(kFusedThreads), 0, s, pdl, a);
     if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
@@ -907,7 +883,7 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
     const uint64_t chunks = (t->n_pods + 512ull * kScanUnroll - 1) / (512ull * kScanUnroll);
     const uint64_t want = (chunks + 7) / 8;
     const uint32_t grid = (uint32_t)(want < (1u << 20) ? want : (1u << 20));
-    e = launch_pdl(pod_scan_kernel<kScanUnroll>, dim3(grid), dim3(256), 0, s, g_pdl && first_pdl && !t->node_occupancy && !d_event_count, a);
+    e = launch_pdl(pod_scan_kernel<kScanUnroll>, dim3(grid), dim3(256), 0, s, first_pdl && !t->node_occupancy && !d_event_count, a);
     if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
     launches++;
   }
@@ -970,7 +946,6 @@ struct PublishArgs {
   uint32_t seq_slot;
   uint32_t seq;
   uint32_t* ticket;
-  uint32_t fence_each;     // A/B: every CTA fences at system scope as well
   // clear: device words zeroed after `extra` was read (the tick slot's block of placement counters)
   uint32_t* clear;
   uint32_t n_clear;
@@ -1010,7 +985,6 @@ __global__ void __launch_bounds__(kPublishThreads) publish_lists_kernel(const Pu
   bool last = true;
   if (gridDim.x > 1) {
     if (threadIdx.x == 0) {
-      if (a.fence_each) __threadfence_system();
       uint32_t t;  // release at gpu scope: the CTA's stores (ordered before this by bar.sync) happen-before the ticket
       asm volatile("atom.add.acq_rel.gpu.global.u32 %0, [%1], 1;" : "=r"(t) : "l"(a.ticket) : "memory");
       s_last = t == gridDim.x - 1u ? 1u : 0u;
@@ -1062,15 +1036,10 @@ int launch_publish(const PublishListHost* lists, const uint32_t* d_extra, uint32
   a.ticket = d_ticket;
   a.clear = d_clear;
   a.n_clear = d_clear ? n_clear : 0u;
-  static const bool fence_each = [] {
-    const char* v = getenv("LWSE_PUBLISH_FENCE_EACH");
-    return v && atoi(v) != 0;
-  }();
-  a.fence_each = fence_each ? 1u : 0u;
   // ONE CTA for the usual few thousand rows (no ticket stage then); more when the previous tick reported many
   unsigned grid = expected_rows / 8192u + 1u;
   if (grid > 32u) grid = 32u;
-  const cudaError_t e = launch_pdl(publish_lists_kernel, dim3(grid), dim3(kPublishThreads), 0, s, g_pdl && pdl, a);
+  const cudaError_t e = launch_pdl(publish_lists_kernel, dim3(grid), dim3(kPublishThreads), 0, s, pdl, a);
   if (e != cudaSuccess) {
     *cuda_err = (int)e;
     return -1;
@@ -1216,7 +1185,7 @@ bool write_scatter_desc(void* h_desc, const ScatterSegHost* segs, int n_segs, ui
 }
 int launch_scatter_desc(const void* d_desc, int sm_count, cudaStream_t s, bool pdl, int* cuda_err) {
   *cuda_err = 0;
-  const cudaError_t e = launch_pdl(scatter_rows_desc_kernel, dim3((unsigned)sm_count * 4u), dim3(256), 0, s, pdl && g_pdl,
+  const cudaError_t e = launch_pdl(scatter_rows_desc_kernel, dim3((unsigned)sm_count * 4u), dim3(256), 0, s, pdl,
                                    static_cast<const ScatterArgs*>(d_desc));
   if (e != cudaSuccess) {
     *cuda_err = (int)e;
@@ -1237,7 +1206,7 @@ int launch_scatter(const ScatterSegHost* segs, int n_segs, uint32_t* d_occupancy
   const uint64_t work = a.total_work;
   uint64_t grid = (work + 255) / 256;
   if (grid > (uint64_t)kSmCount * 16u) grid = (uint64_t)kSmCount * 16u;
-  const cudaError_t e = launch_pdl(scatter_rows_kernel, dim3((unsigned)grid), dim3(256), 0, s, pdl && g_pdl, a);
+  const cudaError_t e = launch_pdl(scatter_rows_kernel, dim3((unsigned)grid), dim3(256), 0, s, pdl, a);
   if (e != cudaSuccess) {
     *cuda_err = (int)e;
     return -1;
@@ -1258,28 +1227,6 @@ int launch_occupancy(const lwse_pod_ident* d_ident, uint64_t n_pods, uint32_t* d
   e = cudaGetLastError();
   if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
   return 1;
-}
-
-// LWSE_SMEM_CARVEOUT (experiment switch, engine creation): one preferred shared-memory carveout (percent of the
-// SM's maximum) for every kernel of a tick, so that CTAs of the sweep and of the placement round never ask the SM
-// for different L1 / shared-memory splits.
-cudaError_t set_sweep_carveout(int pct) {
-  cudaError_t e = cudaSuccess;
-  auto set = [&](const void* k) {
-    const cudaError_t r = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-    if (r != cudaSuccess) e = r;
-  };
-  set((const void*)group_fused_kernel);
-  set((const void*)lws_sweep_kernel<1>);
-  set((const void*)lws_sweep_kernel<2>);
-  set((const void*)lws_sweep_kernel<4>);
-  set((const void*)lws_sweep_kernel<8>);
-  set((const void*)lws_sweep_kernel<16>);
-  set((const void*)lws_sweep_kernel<32>);
-  set((const void*)scatter_rows_kernel);
-  set((const void*)scatter_rows_desc_kernel);
-  set((const void*)publish_lists_kernel);
-  return e;
 }
 
 }  // namespace lwse

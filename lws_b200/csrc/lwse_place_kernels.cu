@@ -496,10 +496,6 @@ int launch_place(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, cons
 
   // One cluster while every request can have its own warp within a few passes; beyond that a
   // cooperative grid with one warp per request, at most one CTA per SM.
-  static const int env_path = [] {  // tuning / tests: 1 = always the cluster, 2 = always the grid
-    const char* v = getenv("LWSE_PLACE_PATH");
-    return v ? atoi(v) : 0;
-  }();
   // (phase 0 and the scratch reset are grid-stride loops: tables that 4096 threads cannot sweep in
   // a few passes go to the grid as well.)  What decides is the number of UNPINNED requests — pinned
   // ones cost one claim in phase 0 — and the host does not know it: the previous call's count,
@@ -512,8 +508,7 @@ int launch_place(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, cons
                                        : n_reqs;
   const bool small = (few_reqs || (expect_unpinned <= kClusterCtas * kPlaceWarps * 2u && n_reqs <= (1u << 14))) &&
                      n_nodes <= (1u << 16) && (uint64_t)n_namespaces * hold_stride_of(n_domains) <= (1u << 16);
-  const bool cluster = env_path == 1 || (env_path != 2 && small);
-  if (cluster) {
+  if (small) {
     // 16 CTAs x 256 threads where the device can co-schedule a 16-CTA cluster (non-portable size:
     // probed once per device), else 8 x 512: the same 128 warps on twice the SMs — the rounds are
     // bound by the instruction issue of the warps sharing a scheduler.
@@ -524,9 +519,7 @@ int launch_place(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, cons
     int& probed = wide_by_device[dev & 63];
     if (probed == 0) {
       probed = 1;
-      const char* v = getenv("LWSE_PLACE_CLUSTER16");
-      if (!(v && atoi(v) == 0) &&
-          cudaFuncSetAttribute(place_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
+      if (cudaFuncSetAttribute(place_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) {
         cudaLaunchConfig_t probe{};
         probe.gridDim = dim3(16);
         probe.blockDim = dim3(256);

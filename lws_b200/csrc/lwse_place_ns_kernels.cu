@@ -412,18 +412,10 @@ __device__ __forceinline__ void diff_row(const PlaceNsArgs& a, uint32_t r, const
   }
 }
 
-// Register budget: LWSE_NS_MAXNREG (build-time experiment switch) caps the kernel with __maxnreg__ instead of
-// __launch_bounds__ (the two cannot be combined) so that a CTA of this kernel and CTAs of the sweep fit one SM's
-// register file side by side in a tick.
-#ifdef LWSE_NS_MAXNREG
-#define LWSE_NS_BOUNDS __maxnreg__(LWSE_NS_MAXNREG)
-#else
-#define LWSE_NS_BOUNDS __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
-#endif
 // kIndexed: the requests of a namespace are reached through the index (ns_rows); results, keys and the
 // unpinned list carry the request ROW either way.
 template <bool kScan, bool kIndexed>
-__global__ void LWSE_NS_BOUNDS
+__global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
     place_ns_kernel(const PlaceNsArgs a, const __grid_constant__ CUtensorMap words_map) {
   extern __shared__ uint8_t s_dyn[];
   // layout (from a 128-byte aligned base: the TMA destination):
@@ -921,11 +913,7 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
     map_for = a.g_words;
     map_rows = l.word_rows;
   }
-  static const bool no_tensor_map = [] {
-    const char* v = getenv("LWSE_PLACE_NO_TENSOR_MAP");
-    return v && atoi(v) != 0;
-  }();
-  a.use_tensor_map = (a.stage_words && map_ok && !no_tensor_map) ? 1u : 0u;
+  a.use_tensor_map = (a.stage_words && map_ok) ? 1u : 0u;
 
   int launched = 2;
   // first_pdl: the predecessor on the stream is a kernel — programmatically dependent then (every
@@ -975,20 +963,6 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
     if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
   }
   return launched;
-}
-
-cudaError_t set_place_ns_carveout(int pct) {  // see set_sweep_carveout (lwse_lws_kernels.cu)
-  cudaError_t e = cudaSuccess;
-  auto set = [&](const void* k) {
-    const cudaError_t r = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-    if (r != cudaSuccess) e = r;
-  };
-  set((const void*)place_condense_kernel);
-  set((const void*)place_ns_kernel<false, false>);
-  set((const void*)place_ns_kernel<true, false>);
-  set((const void*)place_ns_kernel<false, true>);
-  set((const void*)place_ns_kernel<true, true>);
-  return e;
 }
 
 // --------------------------------------------------------------------------

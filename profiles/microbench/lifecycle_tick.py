@@ -1,8 +1,7 @@
 """C3 resident tick at 1 % churn on a request table grouped by namespace and on the same table made
 ungrouped (1 % of the requests moved to tail rows, two namespaces interleaved — what creating and
-deleting LeaderWorkerSets in place leaves behind).  The two alternate in one process; the ungrouped
-table is also timed with LWSE_PLACE_FORM=general in a subprocess (the form such a table ran before
-the namespace index).  Per case: the synchronous tick (lwse_resident_tick, wall clock around a call
+deleting LeaderWorkerSets in place leaves behind).  The two alternate in one process.  Per case: the
+synchronous tick (lwse_resident_tick, wall clock around a call
 that returns after the device finished) and the pipelined tick (two in flight, as bench.py's headline).
 Every case's final placement rows are checked against the spec oracle.
 
@@ -111,7 +110,6 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=300)
     ap.add_argument("--repeats", type=int, default=3)
-    ap.add_argument("--only", choices=["both", "ungrouped"], default="both")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     t = synth.make("C3", 1.0, seed=synth.SEED)
@@ -119,18 +117,8 @@ def main():
     eng.upload_nodes(t.nodes, t.n_domains)
     flags = t.flags | R.TICK_PLACE
     reqs = t.place_requests()
-    cases = {}
-    if args.only == "both":
-        cases["grouped"] = Case(eng, t, reqs, flags)
-    cases["ungrouped"] = Case(eng, t, ungroup(reqs), flags)
+    cases = {"grouped": Case(eng, t, reqs, flags), "ungrouped": Case(eng, t, ungroup(reqs), flags)}
     res = measure(cases, args.steps, args.repeats)
-    if args.only == "ungrouped":
-        print(json.dumps(res))
-        return
-    env = dict(os.environ, LWSE_PLACE_FORM="general")
-    sub = subprocess.run([sys.executable, os.path.abspath(__file__), "--only", "ungrouped", "--steps", str(args.steps),
-                          "--repeats", str(args.repeats)], env=env, capture_output=True, text=True, check=True)
-    res["ungrouped_general_form"] = json.loads(sub.stdout.strip().splitlines()[-1])["ungrouped"]
     res["config"] = {"workload": "C3", "scale": 1.0, "churn_pods": 0.01, "churn_reqs": 0.01, "steps": args.steps,
                      "repeats": args.repeats, "n_requests": int(len(reqs)), **gpu_info()}
     line = json.dumps(res)
