@@ -827,6 +827,13 @@ LWSE_API int lwse_exchange_status(lwse_engine* e, uint32_t* error_out);
 /* DisaggregatedSet sweep                                                    */
 /* ------------------------------------------------------------------------- */
 #define LWSE_DS_MAX_ROLES 10u /* api/disaggregatedset/v1: 2..10 roles             */
+/* The limits of one DS: n_roles <= LWSE_DS_MAX_ROLES counts the removed roles too (roles of old
+ * revisions that left the spec), so a DS with 10 spec roles that renamed one has 11 and is past it;
+ * n_old_revs <= LWSE_DS_MAX_OLD_REVS; n_spec_roles <= n_roles; both ranges inside their tables.
+ * A DS past any of them is reported LWSE_DOUT_BAD_TABLE (LWSE_DSF_BAD_TABLE by the forecast), not
+ * reconciled: its role and revision-role rows are neither read nor written by the sweep, the DS
+ * tick or the forecast (their role_out / revrole_out rows keep what the output tables held), and
+ * no other DS's results change. */
 
 /* One DisaggregatedSet (32 B). */
 typedef struct lwse_ds_rec {
