@@ -10,6 +10,7 @@
 // integer floor / ceil division (DESIGN.md "float vs int"); the CPU oracle keeps
 // the float form, so parity tests compare the two formulations.
 #include "lwse_device.cuh"
+#include "lwse_launch.cuh"
 
 namespace lwse {
 
@@ -677,19 +678,6 @@ __global__ void __launch_bounds__(128) ds_forecast_kernel(const lwse_ds_tables i
     ds_forecast_one<kWrite>(in, f, d);
 }
 
-struct DsForecastHost {  // (lwse_engine.cu)
-  lwse_ds_revrole_rec* rows;
-  lwse_ds_out* s_ds_out;
-  lwse_ds_role_out* s_role_out;
-  lwse_ds_revrole_out* s_revrole_out;
-  lwse_ds_forecast* fc;
-  lwse_ds_forecast_role* fc_role;
-  lwse_ds_role_out* steps;  // the write pass's rows (device scratch)
-  uint32_t step_capacity;
-  bool want_steps;  // a trajectory is asked for: the scan marks what does not fit in step_capacity
-  unsigned long long* totals;  // device, 2 words, zeroed by the caller
-};
-
 // write_pass = false: the summary pass and the scan.  write_pass = true: the write pass into h->steps,
 // which holds the rows the scan counted as written.  Both on stream s.
 int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s,
@@ -733,25 +721,6 @@ int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s, int* 
   }
   return 1;
 }
-
-struct DsTickHost {  // (lwse_engine.cu)
-  const lwse_ds_out* prev_ds_out;
-  const lwse_ds_role_out* prev_role_out;
-  const lwse_ds_revrole_out* prev_revrole_out;
-  lwse_ds_out* m_ds_out;
-  lwse_ds_role_out* m_role_out;
-  lwse_ds_revrole_out* m_revrole_out;
-  uint8_t* marks;
-  uint32_t* rows;
-  uint32_t* counters;  // [0] count, [1] ticket
-  uint32_t* host_words;
-  uint32_t seq;
-  bool all;
-  const lwse_ds_link* links;  // non-null: the linked instance
-  const lwse_lws_rec* lws;
-  const lwse_lws_out* lws_out;
-  uint32_t n_lws;
-};
 
 int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s, int* cuda_err) {
   *cuda_err = 0;

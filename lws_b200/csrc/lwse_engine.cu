@@ -15,162 +15,7 @@
 #include <new>
 
 #include "lwse_device.cuh"
-
-namespace lwse {
-// lwse_lws_kernels.cu
-struct SweepChangeLists {
-  uint32_t* lws_rows = nullptr;
-  lwse_lws_out* lws_out = nullptr;
-  uint32_t lws_capacity = 0;
-  uint32_t* group_rows = nullptr;
-  lwse_group_out* group_out = nullptr;
-  uint32_t group_capacity = 0;
-  uint32_t* counts = nullptr;
-};
-struct PublishListHost {
-  const uint32_t* src_rows;
-  const void* src_outs;
-  uint32_t* dst_rows;
-  void* dst_outs;
-  uint32_t* count;
-  uint32_t capacity;
-  uint32_t out_bytes;
-};
-int launch_publish(const PublishListHost* lists, const uint32_t* d_extra, uint32_t* h_words, uint32_t seq_slot,
-                   uint32_t seq, uint32_t* d_ticket, uint32_t expected_rows, cudaStream_t s, int* cuda_err,
-                   uint32_t* d_clear, uint32_t n_clear, bool pdl);
-int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uint32_t n_nodes,
-                     void* scratch, int sm_count, cudaStream_t s, int* cuda_err, const SweepChangeLists* cl,
-                     uint32_t* d_event_count = nullptr, int first_mode = 1);
-size_t lws_sweep_scratch_bytes(uint64_t n_pods, uint32_t n_groups);
-struct ScatterSegHost {
-  void* table;
-  uint64_t table_rows;
-  const uint32_t* rows;
-  const void* values;
-  uint32_t n;
-  uint32_t row_bytes;
-  bool is_ident;
-};
-int launch_scatter(const ScatterSegHost* segs, int n_segs, uint32_t* d_occupancy, uint32_t n_nodes, cudaStream_t s,
-                   bool pdl, int* cuda_err);
-size_t scatter_desc_bytes();
-bool write_scatter_desc(void* h_desc, const ScatterSegHost* segs, int n_segs, uint32_t* d_occupancy, uint32_t n_nodes);
-int launch_scatter_desc(const void* d_desc, int sm_count, cudaStream_t s, bool pdl, int* cuda_err);
-int launch_ident_prefetch(const uint8_t* d_state, uint64_t n_pods, const lwse_pod_ident* mapped_host_ident,
-                          lwse_pod_ident* d_ident, int sm_count, cudaStream_t s, int* cuda_err);
-int launch_occupancy(const lwse_pod_ident* d_ident, uint64_t n_pods, uint32_t* d_occupancy, uint32_t n_nodes, int sm_count,
-                     cudaStream_t s, int* cuda_err);
-// lwse_place_kernels.cu
-int launch_place(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, const uint32_t* d_node_order,
-                 const uint32_t* d_node_pos, uint32_t n_nodes, uint32_t n_domains,
-                 const lwse_place_req* d_reqs, uint32_t n_reqs, const uint32_t* d_occupancy,
-                 uint32_t n_namespaces, lwse_place_out* d_out, void* d_scratch, size_t scratch_bytes,
-                 uint32_t* h_rounds, int sm_count, cudaStream_t s, int* cuda_err, uint32_t call_index,
-                 bool fresh, uint32_t n_parts, uint32_t reqs_per_part, uint64_t part_stride_bytes,
-                 uint32_t* h_unpinned, const uint32_t** d_counters_out, const uint32_t** d_unpinned_out,
-                 bool after_push);
-size_t place_scratch_bytes(uint32_t n_nodes, uint32_t n_domains, uint32_t n_reqs, uint32_t n_namespaces);
-size_t place_ns_scratch_bytes(uint32_t n_nodes, uint32_t n_domains, uint32_t n_reqs, uint32_t n_namespaces);
-struct PlaceNsChanges {  // a tick's placement change list (device memory); prev == null: off
-  lwse_place_out* prev;
-  uint32_t* rows;
-  lwse_place_out* outs;
-  uint32_t* count;
-  uint32_t capacity;
-  int tick_slot;    // see lwse_place_ns_kernels.cu
-  void* mid_event;
-};
-struct PlaceNsExchange {
-  const unsigned long long* step_ctr;
-  uint64_t half_bytes;
-  bool lagged;
-};
-enum PlaceNsIndex : uint32_t { kNsIndexNone = 0, kNsIndexReuse = 1, kNsIndexBuild = 2 };
-bool place_ns_supported(uint32_t n_nodes, uint32_t n_domains);
-int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, const uint32_t* d_node_order, uint32_t n_nodes,
-                    uint32_t n_domains, const lwse_place_req* d_reqs, uint32_t n_reqs,
-                    const uint32_t* d_occupancy, uint32_t n_parts, uint64_t part_stride_bytes, uint32_t n_namespaces,
-                    lwse_place_out* d_out, void* d_scratch, size_t scratch_bytes, bool fresh, uint32_t call_index, bool scan,
-                    int sm_count, cudaStream_t s, int* cuda_err, const uint32_t** d_counters_out, bool first_pdl,
-                    const PlaceNsChanges* changes, const PlaceNsExchange* xch, PlaceNsIndex index);
-size_t node_index_scratch_bytes(uint32_t n_domains);
-int launch_node_index(const lwse_node_rec* d_nodes, uint32_t n_nodes, uint32_t n_domains, uint32_t* d_dom_first,
-                      uint32_t* d_node_order, uint32_t* d_node_pos, void* d_scratch, int sm_count, cudaStream_t s,
-                      bool pdl, int* cuda_err);
-int launch_place_diff(const lwse_place_out* d_cur, lwse_place_out* d_prev, uint32_t n, uint32_t* d_rows,
-                      lwse_place_out* d_outs, uint32_t capacity, uint32_t* d_count, cudaStream_t s, int* cuda_err);
-int launch_place_whatif_index(const lwse_place_req* d_reqs, uint32_t n_reqs, uint32_t n_namespaces, const uint8_t* d_touched,
-                              uint32_t n_nodes, uint32_t n_domains, void* d_scratch, int sm_count, cudaStream_t s, int* cuda_err);
-int launch_place_whatif_diff(const lwse_place_out* d_before, const lwse_place_out* d_after, uint32_t n_resident, uint32_t n_total,
-                             uint32_t* d_rows, lwse_place_out* d_outs_before, lwse_place_out* d_outs_after, uint32_t capacity,
-                             uint32_t* d_counts, int sm_count, cudaStream_t s, int* cuda_err);
-// lwse_ds_kernels.cu
-int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s, int* cuda_err);
-struct DsTickHost {
-  const lwse_ds_out* prev_ds_out;
-  const lwse_ds_role_out* prev_role_out;
-  const lwse_ds_revrole_out* prev_revrole_out;
-  lwse_ds_out* m_ds_out;
-  lwse_ds_role_out* m_role_out;
-  lwse_ds_revrole_out* m_revrole_out;
-  uint8_t* marks;
-  uint32_t* rows;
-  uint32_t* counters;
-  uint32_t* host_words;
-  uint32_t seq;
-  bool all;
-  const lwse_ds_link* links;
-  const lwse_lws_rec* lws;
-  const lwse_lws_out* lws_out;
-  uint32_t n_lws;
-};
-int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s, int* cuda_err);
-struct DsForecastHost {
-  lwse_ds_revrole_rec* rows;
-  lwse_ds_out* s_ds_out;
-  lwse_ds_role_out* s_role_out;
-  lwse_ds_revrole_out* s_revrole_out;
-  lwse_ds_forecast* fc;
-  lwse_ds_forecast_role* fc_role;
-  lwse_ds_role_out* steps;  // the write pass's rows (device scratch)
-  uint32_t step_capacity;
-  bool want_steps;  // a trajectory is asked for: the scan marks what does not fit in step_capacity
-  unsigned long long* totals;
-};
-int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s,
-                       int* cuda_err);
-// lwse_lws_forecast_kernels.cu
-struct LwsForecastHost {
-  const lwse_lws_rec* lws;
-  uint32_t n_lws;
-  const lwse_group_out* group_out;
-  uint32_t n_groups;
-  unsigned long long* slot_off;
-  uint8_t* slots;
-  uint32_t n_slots;
-  lwse_lws_forecast* fc;
-  lwse_lws_forecast_step* steps;  // the write pass's rows (device scratch)
-  uint32_t steps_rows;
-  uint32_t step_capacity;
-  bool want_steps;  // a trajectory is asked for: the scan marks what does not fit in step_capacity
-  unsigned long long* totals;
-};
-int launch_lws_forecast_slots(const LwsForecastHost* h, int sm_count, cudaStream_t s, int* cuda_err);
-int launch_lws_forecast(const LwsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s, int* cuda_err);
-// lwse_sha1_kernels.cu
-int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,
-                int sm_count, cudaStream_t s, int* cuda_err);
-int launch_subgroup_keys(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, const int32_t* d_pod_count,
-                         const int32_t* d_subgroup_size, const int32_t* d_worker_index, int32_t* d_index_out,
-                         uint8_t* d_digests, int sm_count, cudaStream_t s, int* cuda_err);
-// lwse_exchange_kernels.cu
-int launch_exchange_push(const void* d_local_part, uint8_t* const* d_peer_base, void* d_local_base,
-                         uint64_t part_bytes, uint64_t part_stride, uint64_t half_bytes, uint64_t flags_offset,
-                         uint64_t step, uint64_t wait_step, uint32_t world, uint32_t rank, cudaStream_t s, int* cuda_err,
-                         bool lagged);
-}  // namespace lwse
-
+#include "lwse_launch.cuh"
 
 namespace {
 
@@ -297,7 +142,7 @@ struct lwse_engine {
     const uint32_t* rounds_ptr = nullptr;  // where its round counts
   };
   std::unordered_map<uint32_t, TickGraph> tick_graphs;
-  PinBuf tdesc;                      // 2 slots x 512 B: the scatter's segment descriptors of the tick of that parity
+  PinBuf tdesc;                      // 2 slots x kScatterDescBytes: the scatter's segment descriptors of the tick of that parity
   DevBuf tdesc_dev;                  // device copy (the copy node at the root of a tick graph fills it)
   cudaStream_t copy_stream = nullptr;  // the patch copy of a replayed tick: overlaps the previous tick's kernels
   cudaEvent_t ev_dma = nullptr;
@@ -389,6 +234,15 @@ int fail_cuda(lwse_engine* e, cudaError_t err) {
   e->last_cuda_error = (int)err;
   (void)cudaGetLastError();  // clear the sticky-free error state
   return err == cudaErrorMemoryAllocation ? LWSE_ERR_OOM : LWSE_ERR_CUDA;
+}
+
+// The result of a launcher (kernels launched, or -1 with its CUDA error): counts the kernels, or fails.
+int count_launch(lwse_engine* e, int launched, int cuda_err) {
+  if (launched >= 0) {
+    e->launches += (uint64_t)launched;
+    return LWSE_OK;
+  }
+  return fail_cuda(e, (cudaError_t)cuda_err);
 }
 
 #define LWSE_CUDA(e, call)                                \
@@ -641,8 +495,7 @@ static int build_node_index_locked(lwse_engine* e, cudaStream_t s, bool pdl, boo
   const int launched = lwse::launch_node_index((const lwse_node_rec*)e->nodes.p, e->n_nodes, e->n_domains, (uint32_t*)e->dom_first.p,
                                                (uint32_t*)e->node_order.p, (uint32_t*)e->node_pos.p, e->node_ix.p, e->sm_count, s,
                                                pdl, &cuda_err);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   e->node_index_stale = false;
   if (built) *built = true;
   return LWSE_OK;
@@ -720,8 +573,7 @@ LWSE_API int lwse_upload_nodes(lwse_engine* e, const lwse_node_rec* nodes, uint3
     int cuda_err = 0;
     int launched = lwse::launch_occupancy((const lwse_pod_ident*)e->r_pid.p, e->rn_pods, (uint32_t*)e->r_occ.p, n_nodes,
                                           e->sm_count, e->stream, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
   LWSE_CUDA(e, cudaStreamSynchronize(e->stream));
   e->place_ns_geometry[0] = e->place_ns_geometry[1] = e->place_ns_geometry[2] = e->place_ns_geometry[3] = 0;
@@ -739,8 +591,7 @@ static int sweep_device_locked(lwse_engine* e, const lwse_lws_tables* t, cudaStr
   int cuda_err = 0;
   int launched = lwse::launch_lws_sweep(t, (const lwse_node_rec*)e->nodes.p, e->n_nodes,
                                         e->scan_scratch.p, e->sm_count, s, &cuda_err, nullptr);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   return LWSE_OK;
 }
 
@@ -815,8 +666,7 @@ static int sweep_host_locked(lwse_engine* e, const lwse_lws_tables* h, const std
       LWSE_CUDA(e, cudaStreamWaitEvent(e->side_stream, e->ev_fork, 0));
       int launched = lwse::launch_ident_prefetch((const uint8_t*)e->pod_state.p, h->n_pods, (const lwse_pod_ident*)mapped,
                                                  (lwse_pod_ident*)e->pod_ident.p, e->sm_count, e->side_stream, &cuda_err);
-      if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-      e->launches += (uint64_t)launched;
+      if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
       LWSE_CUDA(e, cudaEventRecord(e->ev_join, e->side_stream));
       prefetching = true;
       e->ident_rows = ~0ull;  // the device copy holds the event pods' rows only
@@ -837,8 +687,7 @@ static int sweep_host_locked(lwse_engine* e, const lwse_lws_tables* h, const std
   int launched = lwse::launch_lws_sweep(&d, (const lwse_node_rec*)e->nodes.p, e->n_nodes, e->scan_scratch.p, e->sm_count,
                                         s, &cuda_err, nullptr, counted ? (uint32_t*)e->h_counts_dev.p : nullptr,
                                         /*first_pdl=*/false);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
 
   // group results first: they are complete while the LWS pass still runs
   if (b_go) LWSE_CUDA(e, cudaMemcpyAsync(h->group_out, e->group_out.p, b_go, cudaMemcpyDeviceToHost, s));
@@ -927,8 +776,7 @@ LWSE_API int lwse_resident_load(lwse_engine* e, const lwse_lws_tables* h) {
     int cuda_err = 0;
     int launched = lwse::launch_occupancy((const lwse_pod_ident*)e->r_pid.p, h->n_pods, (uint32_t*)e->r_occ.p, e->n_nodes,
                                           e->sm_count, s, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   e->rn_lws = h->n_lws;
@@ -1004,14 +852,12 @@ static int launch_scatter_plan(lwse_engine* e, const ScatterPlan& p, cudaStream_
   int cuda_err = 0;
   if (p.n) {
     int launched = lwse::launch_scatter(p.sc, p.n, e->n_nodes ? (uint32_t*)e->r_occ.p : nullptr, e->n_nodes, s, true, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
   if (p.recount && e->n_nodes) {
     int launched = lwse::launch_occupancy((const lwse_pod_ident*)e->r_pid.p, e->rn_pods, (uint32_t*)e->r_occ.p, e->n_nodes,
                                           e->sm_count, s, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
   return LWSE_OK;
 }
@@ -1264,9 +1110,8 @@ static int place_grouped_locked(lwse_engine* e, const lwse_place_req* d_reqs, ui
                                        d_occupancy, n_parts, part_stride_bytes, n_namespaces, d_out, e->place_ns_scratch.p,
                                        scratch, fresh, e->place_ns_calls++, scan, e->sm_count, s, &cuda_err, &counters,
                                        (first_pdl || built) && !fresh, changes, xch, index);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   e->r_ns_index_ok = index != lwse::kNsIndexNone;  // (a grouped call writes its own ns_first over the index's)
-  e->launches += (uint64_t)launched;
   e->place_rounds_ptr = counters;
   e->place_scans_ptr = counters + 3;
   if (eager && !changes) {  // (a tick — `changes` — returns only after the host has seen the round complete)
@@ -1321,8 +1166,7 @@ static int place_locked(lwse_engine* e, const lwse_place_req* d_reqs, uint32_t n
                                     scratch, rounds_out ? e->h_rounds : nullptr, e->sm_count, s, &cuda_err,
                                     e->place_calls++, fresh, n_parts, reqs_per_part, part_stride_bytes,
                                     e->h_rounds + 2, &e->place_counters, &e->place_unpinned, after_push);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   e->place_rounds_ptr = e->place_counters + 3;
   e->place_scans_ptr = nullptr;
   if (rounds_out) *rounds_out = e->h_rounds[0];
@@ -1532,8 +1376,7 @@ static int shared_occupancy_place_locked(lwse_engine* e, const lwse_place_req* d
                                             e->xch_reqs_off,  // the occupancy block of a part: n_nodes counters, 16-byte padded
                                             e->xch_stride, e->xch_half, e->xch_flags_off, step, read_step, e->xch_world,
                                             e->xch_rank, ps, &cuda_err, lagged);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   if (n_reqs == 0) return LWSE_OK;
   const lwse::PlaceNsExchange xch{reinterpret_cast<const unsigned long long*>(static_cast<const uint8_t*>(e->xch.p) + e->xch_flags_off +
                                                                               (uint64_t)e->xch_world * 8u + 16u),
@@ -1754,8 +1597,8 @@ struct TickCounts {
   uint32_t n_lws = 0, n_groups = 0, n_place = 0, rounds = 0;
 };
 
-static inline uint8_t* d_desc_of(lwse_engine* e, uint32_t slot, size_t desc_bytes) {
-  return static_cast<uint8_t*>(e->tdesc_dev.p) + slot * desc_bytes;
+static inline uint8_t* d_desc_of(lwse_engine* e, uint32_t slot) {
+  return static_cast<uint8_t*>(e->tdesc_dev.p) + slot * lwse::kScatterDescBytes;
 }
 
 // The checks apply_patches_locked makes on a tick's segments, all of them before anything (the node-table
@@ -1979,8 +1822,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
     cl.counts = cnt;
     int launched = lwse::launch_lws_sweep(&d, (const lwse_node_rec*)e->nodes.p, e->n_nodes, e->r_scan.p, e->sm_count, s,
                                           &cuda_err, &cl, nullptr, sweep_first_mode >= 0 ? sweep_first_mode : (wrote ? 2 : 1));
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
     pl[0] = publish_list(0);
     pl[1] = publish_list(1);
     return LWSE_OK;
@@ -2007,8 +1849,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
     if (!diffed) {
       int launched = lwse::launch_place_diff((const lwse_place_out*)e->r_pout.p, changes.prev, e->rn_reqs, changes.rows,
                                              changes.outs, changes.capacity, changes.count, ps, &cuda_err);
-      if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-      e->launches += (uint64_t)launched;
+      if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
     }
     pl[2] = publish_list(2);
     e->tick_place_ns = diffed;
@@ -2024,8 +1865,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
     int launched = lwse::launch_publish(pl, do_place ? e->place_rounds_ptr : nullptr, hw_dev, 4, seq, cnt + 2,
                                         e->last_changed[0] + e->last_changed[1], e->pub_stream, &cuda_err,
                                         ns_counters ? const_cast<uint32_t*>(e->place_rounds_ptr) : nullptr, 8u, /*pdl=*/false);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
     LWSE_CUDA(e, cudaEventRecord(e->ev_pub, e->pub_stream));
     return LWSE_OK;
   };
@@ -2068,15 +1908,14 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
       if (rc != LWSE_OK) return rc;
       if (gp.eager_only || gp.recount) replay = false;
     }
-    const size_t desc_bytes = 512;
-    if (replay && (lwse::scatter_desc_bytes() > desc_bytes || e->tdesc.reserve(2 * desc_bytes) != cudaSuccess ||
-                   e->tdesc_dev.reserve(2 * desc_bytes) != cudaSuccess)) {
+    const size_t desc_bytes = lwse::kScatterDescBytes;
+    if (replay && (e->tdesc.reserve(2 * desc_bytes) != cudaSuccess || e->tdesc_dev.reserve(2 * desc_bytes) != cudaSuccess)) {
       (void)cudaGetLastError();
       replay = false;
     }
     if (replay) {
       uint8_t* h_desc = static_cast<uint8_t*>(e->tdesc.h) + slot * desc_bytes;
-      uint8_t* d_desc = static_cast<uint8_t*>(e->tdesc_dev.p) + slot * desc_bytes;
+      uint8_t* d_desc = d_desc_of(e, slot);
       if (has_patches && !lwse::write_scatter_desc(h_desc, gp.sc, gp.n, e->n_nodes ? (uint32_t*)e->r_occ.p : nullptr, e->n_nodes))
         replay = false;
       if (replay && !tg.exec) {
@@ -2144,7 +1983,7 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
         if (gp.dma)
           LWSE_CUDA(e, cudaMemcpyAsync(static_cast<uint8_t*>(e->arena_mirror.p) + gp.lo, static_cast<const uint8_t*>(e->arena.h) + gp.lo,
                                        gp.hi - gp.lo, cudaMemcpyHostToDevice, e->copy_stream));
-        LWSE_CUDA(e, cudaMemcpyAsync(d_desc_of(e, slot, desc_bytes), static_cast<uint8_t*>(e->tdesc.h) + slot * desc_bytes, desc_bytes,
+        LWSE_CUDA(e, cudaMemcpyAsync(d_desc_of(e, slot), static_cast<uint8_t*>(e->tdesc.h) + slot * desc_bytes, desc_bytes,
                                      cudaMemcpyHostToDevice, e->copy_stream));
         LWSE_CUDA(e, cudaEventRecord(e->ev_dma, e->copy_stream));
         LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_dma, 0));
@@ -2529,8 +2368,7 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
   int cuda_err = 0;
   if (n_sc) {
     const int launched = lwse::launch_scatter(sc, n_sc, nullptr, 0, s, false, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
   const uint32_t* dom_first = (const uint32_t*)e->dom_first.p;
   const uint32_t* node_order = (const uint32_t*)e->node_order.p;
@@ -2539,8 +2377,7 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
     const int launched = lwse::launch_node_index(d_nodes, e->n_nodes, e->n_domains, (uint32_t*)e->wf_dom_first.p,
                                                  (uint32_t*)e->wf_node_order.p, (uint32_t*)e->wf_node_pos.p, e->wf_node_ix.p,
                                                  e->sm_count, s, false, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
     dom_first = (const uint32_t*)e->wf_dom_first.p;
     node_order = (const uint32_t*)e->wf_node_order.p;
     node_pos = (const uint32_t*)e->wf_node_pos.p;
@@ -2549,20 +2386,17 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
     if (round_fresh) LWSE_CUDA(e, cudaMemsetAsync(e->wf_round.p, 0, round_bytes, s));  // (index counts and counters start at zero)
     int launched = lwse::launch_place_whatif_index(d_reqs, n_total, n_ns, (const uint8_t*)e->wf_touched.p, e->n_nodes, e->n_domains,
                                                    e->wf_round.p, e->sm_count, s, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
     launched = lwse::launch_place_ns(d_nodes, dom_first, node_order, e->n_nodes, e->n_domains, d_reqs, n_total,
                                      (const uint32_t*)e->r_occ.p, 1, 0, n_ns, d_out, e->wf_round.p, round_bytes, false,
                                      e->wf_calls++, false, e->sm_count, s, &cuda_err, nullptr, false, nullptr, nullptr,
                                      lwse::kNsIndexReuse);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   } else {
     const int launched = lwse::launch_place(d_nodes, dom_first, node_order, node_pos, e->n_nodes, e->n_domains, d_reqs, n_total,
                                             (const uint32_t*)e->r_occ.p, n_ns, d_out, e->wf_round.p, round_bytes, nullptr,
                                             e->sm_count, s, &cuda_err, 0u, true, 1, n_total, 0, nullptr, nullptr, nullptr, false);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
   // the diff against the baseline, the counts
   // (layout: [counts: 16 words] [rows: list_cap] [before: list_cap] [after: list_cap], the 16-byte rows aligned)
@@ -2575,8 +2409,7 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
   {
     const int launched = lwse::launch_place_whatif_diff((const lwse_place_out*)e->r_pout.p, d_out, rn, n_total, d_rows, d_before,
                                                         d_after, list_cap, d_counts, e->sm_count, s, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
   if (timing) {
     LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t1, s));
@@ -2628,8 +2461,7 @@ LWSE_API int lwse_sweep_ds_device(lwse_engine* e, const lwse_ds_tables* t, void*
   cudaStream_t s = stream ? (cudaStream_t)stream : e->stream;
   int cuda_err = 0;
   int launched = lwse::launch_ds_sweep(t, e->sm_count, s, &cuda_err);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   return LWSE_OK;
 }
 
@@ -2662,8 +2494,7 @@ LWSE_API int lwse_sweep_ds_host(lwse_engine* e, const lwse_ds_tables* h) {
   d.revrole_out = (lwse_ds_revrole_out*)e->ds_revrole_out.p;
   int cuda_err = 0;
   int launched = lwse::launch_ds_sweep(&d, e->sm_count, s, &cuda_err);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   if (o_ds) LWSE_CUDA(e, cudaMemcpyAsync(h->ds_out, e->ds_out.p, o_ds, cudaMemcpyDeviceToHost, s));
   if (o_ro) LWSE_CUDA(e, cudaMemcpyAsync(h->role_out, e->ds_role_out.p, o_ro, cudaMemcpyDeviceToHost, s));
   if (o_rr) LWSE_CUDA(e, cudaMemcpyAsync(h->revrole_out, e->ds_revrole_out.p, o_rr, cudaMemcpyDeviceToHost, s));
@@ -2812,8 +2643,7 @@ LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, u
   }
   for (int k = 0; k < n_sc; k += 8) {  // (one launch takes up to eight segments)
     const int launched = lwse::launch_scatter(sc + k, n_sc - k < 8 ? n_sc - k : 8, nullptr, 0, s, false, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
   for (uint32_t i = 0; i < n_segs; i++)
     if (segs[i].table == LWSE_TABLE_DS_LINKS && segs[i].n) e->rd_linked = true;
@@ -2855,8 +2685,7 @@ LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, u
                              linked ? (const lwse_ds_link*)e->rd_links.p : nullptr, (const lwse_lws_rec*)e->r_lws.p,
                              (const lwse_lws_out*)e->r_lws_out.p, lws_results ? e->rn_lws : 0u};
     const int launched = lwse::launch_ds_tick(&t, &a, e->sm_count, s, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
     cudaError_t werr = cudaSuccess;
     if (!wait_word(hw + 1, seq, s, &werr)) {
       const cudaError_t a2 = cudaStreamSynchronize(s);
@@ -2918,8 +2747,7 @@ static int forecast_locked(lwse_engine* e, const lwse_ds_tables& d, lwse_ds_fore
                          nullptr, cap, out->steps != nullptr, (unsigned long long*)e->fc_totals.p};
   int cuda_err = 0;
   int launched = lwse::launch_ds_forecast(&d, &h, false, e->sm_count, s, &cuda_err);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   uint64_t* words = static_cast<uint64_t*>(e->fc_words.h);
   LWSE_CUDA(e, cudaMemcpyAsync(words, e->fc_totals.p, 16, cudaMemcpyDeviceToHost, s));
   if (b_fc) LWSE_CUDA(e, cudaMemcpyAsync(out->ds, e->fc_ds.p, b_fc, cudaMemcpyDeviceToHost, s));
@@ -2933,8 +2761,7 @@ static int forecast_locked(lwse_engine* e, const lwse_ds_tables& d, lwse_ds_fore
     LWSE_CUDA(e, e->fc_steps.reserve((size_t)written * sizeof(lwse_ds_role_out) + 16));
     h.steps = (lwse_ds_role_out*)e->fc_steps.p;
     launched = lwse::launch_ds_forecast(&d, &h, true, e->sm_count, s, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
     LWSE_CUDA(e, cudaMemcpyAsync(out->steps, e->fc_steps.p, (size_t)written * sizeof(lwse_ds_role_out),
                                  cudaMemcpyDeviceToHost, s));
     LWSE_CUDA(e, cudaStreamSynchronize(s));
@@ -3010,8 +2837,7 @@ static int lws_forecast_locked(lwse_engine* e, lwse::LwsForecastHost& h, lwse_lw
   uint64_t* words = static_cast<uint64_t*>(e->lf_words.h);
   int cuda_err = 0;
   int launched = lwse::launch_lws_forecast_slots(&h, e->sm_count, s, &cuda_err);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(words, e->lf_totals.p, 32, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   const uint64_t n_slots = h.n_lws ? words[2] : 0u;
@@ -3022,8 +2848,7 @@ static int lws_forecast_locked(lwse_engine* e, lwse::LwsForecastHost& h, lwse_lw
   h.steps = nullptr;
   h.steps_rows = 0;
   launched = lwse::launch_lws_forecast(&h, false, e->sm_count, s, &cuda_err);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   const size_t b_fc = (size_t)h.n_lws * sizeof(lwse_lws_forecast);
   LWSE_CUDA(e, cudaMemcpyAsync(words, e->lf_totals.p, 32, cudaMemcpyDeviceToHost, s));
   if (b_fc) LWSE_CUDA(e, cudaMemcpyAsync(out->lws, e->lf_fc.p, b_fc, cudaMemcpyDeviceToHost, s));
@@ -3037,8 +2862,7 @@ static int lws_forecast_locked(lwse_engine* e, lwse::LwsForecastHost& h, lwse_lw
     h.steps = (lwse_lws_forecast_step*)e->lf_steps.p;
     h.steps_rows = written;
     launched = lwse::launch_lws_forecast(&h, true, e->sm_count, s, &cuda_err);
-    if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-    e->launches += (uint64_t)launched;
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
     LWSE_CUDA(e, cudaMemcpyAsync(words, e->lf_totals.p, 32, cudaMemcpyDeviceToHost, s));
     LWSE_CUDA(e, cudaMemcpyAsync(out->steps, e->lf_steps.p, (size_t)written * sizeof(lwse_lws_forecast_step),
                                  cudaMemcpyDeviceToHost, s));
@@ -3110,8 +2934,7 @@ static int group_keys_locked(lwse_engine* e, const uint8_t* d_bytes, const uint3
                              uint8_t* d_digests, cudaStream_t s) {
   int cuda_err = 0;
   int launched = lwse::launch_sha1(d_bytes, d_offsets, n, d_digests, e->sm_count, s, &cuda_err);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   return LWSE_OK;
 }
 
@@ -3157,8 +2980,7 @@ LWSE_API int lwse_subgroup_keys_device(lwse_engine* e, const uint8_t* d_bytes, c
   int cuda_err = 0;
   int launched = lwse::launch_subgroup_keys(d_bytes, d_offsets, n, d_pod_count, d_subgroup_size, d_worker_index, d_index_out,
                                             d_digests, e->sm_count, stream ? (cudaStream_t)stream : e->stream, &cuda_err);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   return LWSE_OK;
 }
 
@@ -3188,8 +3010,7 @@ LWSE_API int lwse_subgroup_keys_host(lwse_engine* e, const uint8_t* bytes, const
   int launched = lwse::launch_subgroup_keys((const uint8_t*)e->sha_bytes.p, (const uint32_t*)e->sha_offsets.p, n, d_int, d_int + n,
                                             d_int + 2 * (size_t)n, d_int + 3 * (size_t)n, (uint8_t*)e->sha_digests.p,
                                             e->sm_count, s, &cuda_err);
-  if (launched < 0) return fail_cuda(e, (cudaError_t)cuda_err);
-  e->launches += (uint64_t)launched;
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(index_out, d_int + 3 * (size_t)n, b_int, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(digests, e->sha_digests.p, (size_t)n * 20, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));

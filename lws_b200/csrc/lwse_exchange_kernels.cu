@@ -20,6 +20,7 @@
 // which on B's stream comes after B's round of tick s - 2 — the last reader of buffer (s - 3) % 3
 // = s % 3.
 #include "lwse_device.cuh"
+#include "lwse_launch.cuh"
 
 namespace lwse {
 

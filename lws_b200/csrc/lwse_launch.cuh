@@ -1,0 +1,195 @@
+// The interface between the engine (lwse_engine.cu) and the kernel files (lwse_*_kernels.cu): every
+// launcher, scratch-size function and argument struct one file defines and another calls.  Host
+// declarations only.  Each struct is defined here and nowhere else, so that the engine and the
+// kernel that reads it cannot disagree on its layout.
+//
+// A launcher enqueues its kernels on the stream it is given and returns the number of kernels it
+// launched (>= 0), or -1 with *cuda_err set.
+#pragma once
+
+#include <cuda_runtime.h>
+#include <stddef.h>
+#include <stdint.h>
+
+#include "../../include/lwse.h"
+
+namespace lwse {
+
+// ---- lwse_lws_kernels.cu ----
+int pick_tile(uint64_t items, uint64_t owners);  // lanes per object of the LWS pass (and of the forecast)
+
+struct SweepChangeLists {  // device (or mapped host) pointers; all null = off
+  uint32_t* lws_rows = nullptr;
+  lwse_lws_out* lws_out = nullptr;
+  uint32_t lws_capacity = 0;
+  uint32_t* group_rows = nullptr;
+  lwse_group_out* group_out = nullptr;
+  uint32_t group_capacity = 0;
+  uint32_t* counts = nullptr;  // device: [0] lws, [1] groups; zeroed by the caller (a tick's publish kernel resets them)
+};
+int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uint32_t n_nodes,
+                     void* scratch, int sm_count, cudaStream_t s, int* cuda_err, const SweepChangeLists* cl,
+                     uint32_t* d_event_count = nullptr, int first_mode = 1);
+size_t lws_sweep_scratch_bytes(uint64_t n_pods, uint32_t n_groups);
+
+struct PublishListHost {
+  const uint32_t* src_rows;
+  const void* src_outs;
+  uint32_t* dst_rows;
+  void* dst_outs;
+  uint32_t* count;   // null = skip this slot
+  uint32_t capacity;
+  uint32_t out_bytes;
+};
+int launch_publish(const PublishListHost* lists, const uint32_t* d_extra, uint32_t* h_words, uint32_t seq_slot,
+                   uint32_t seq, uint32_t* d_ticket, uint32_t expected_rows, cudaStream_t s, int* cuda_err,
+                   uint32_t* d_clear, uint32_t n_clear, bool pdl);
+
+struct ScatterSegHost {
+  void* table;
+  uint64_t table_rows;
+  const uint32_t* rows;
+  const void* values;
+  uint32_t n;
+  uint32_t row_bytes;
+  bool is_ident;
+};
+int launch_scatter(const ScatterSegHost* segs, int n_segs, uint32_t* d_occupancy, uint32_t n_nodes, cudaStream_t s,
+                   bool pdl, int* cuda_err);
+// Bytes of one scatter descriptor block of a graph tick (write_scatter_desc / launch_scatter_desc); the
+// kernel file asserts that its argument block fits.
+constexpr size_t kScatterDescBytes = 512;
+bool write_scatter_desc(void* h_desc, const ScatterSegHost* segs, int n_segs, uint32_t* d_occupancy, uint32_t n_nodes);
+int launch_scatter_desc(const void* d_desc, int sm_count, cudaStream_t s, bool pdl, int* cuda_err);
+int launch_ident_prefetch(const uint8_t* d_state, uint64_t n_pods, const lwse_pod_ident* mapped_host_ident,
+                          lwse_pod_ident* d_ident, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_occupancy(const lwse_pod_ident* d_ident, uint64_t n_pods, uint32_t* d_occupancy, uint32_t n_nodes, int sm_count,
+                     cudaStream_t s, int* cuda_err);
+
+// ---- lwse_place_kernels.cu ----
+int launch_place(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, const uint32_t* d_node_order,
+                 const uint32_t* d_node_pos, uint32_t n_nodes, uint32_t n_domains,
+                 const lwse_place_req* d_reqs, uint32_t n_reqs, const uint32_t* d_occupancy,
+                 uint32_t n_namespaces, lwse_place_out* d_out, void* d_scratch, size_t scratch_bytes,
+                 uint32_t* h_rounds, int sm_count, cudaStream_t s, int* cuda_err, uint32_t call_index,
+                 bool fresh, uint32_t n_parts, uint32_t reqs_per_part, uint64_t part_stride_bytes,
+                 uint32_t* h_unpinned, const uint32_t** d_counters_out, const uint32_t** d_unpinned_out,
+                 bool after_push);
+size_t place_scratch_bytes(uint32_t n_nodes, uint32_t n_domains, uint32_t n_reqs, uint32_t n_namespaces);
+int launch_place_diff(const lwse_place_out* d_cur, lwse_place_out* d_prev, uint32_t n, uint32_t* d_rows,
+                      lwse_place_out* d_outs, uint32_t capacity, uint32_t* d_count, cudaStream_t s, int* cuda_err);
+
+// ---- lwse_place_ns_kernels.cu ----
+struct PlaceNsChanges {  // a tick's change list (device memory); prev == null: off
+  lwse_place_out* prev;
+  uint32_t* rows;
+  lwse_place_out* outs;
+  uint32_t* count;
+  uint32_t capacity;
+  int tick_slot;  // 0 / 1: the round's counters live in the tick slot's own block, which the tick's publish
+                  // kernel clears after reading (two ticks may be in flight); -1: the two alternating blocks
+  void* mid_event;  // cudaEvent_t or null: recorded between the condense and the namespace kernel (a tick graph
+                    // holds the sweep back until then, so that both branches reach the SMs together)
+};
+
+struct PlaceNsExchange {  // multi-rank: d_occupancy is the base of the exchange buffers (see PlaceNsArgs::xch_step)
+  const unsigned long long* step_ctr;
+  uint64_t half_bytes;
+  bool lagged;
+};
+
+// index: kNsIndexNone = the request table is grouped by namespace; otherwise the indexed form, with the
+// index kept in the scratch (kNsIndexReuse: as the last build left it — the caller knows the namespace
+// column has not changed since; kNsIndexBuild: built first).
+enum PlaceNsIndex : uint32_t { kNsIndexNone = 0, kNsIndexReuse = 1, kNsIndexBuild = 2 };
+
+bool place_ns_supported(uint32_t n_nodes, uint32_t n_domains);
+int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, const uint32_t* d_node_order, uint32_t n_nodes,
+                    uint32_t n_domains, const lwse_place_req* d_reqs, uint32_t n_reqs,
+                    const uint32_t* d_occupancy, uint32_t n_parts, uint64_t part_stride_bytes, uint32_t n_namespaces,
+                    lwse_place_out* d_out, void* d_scratch, size_t scratch_bytes, bool fresh, uint32_t call_index, bool scan,
+                    int sm_count, cudaStream_t s, int* cuda_err, const uint32_t** d_counters_out, bool first_pdl,
+                    const PlaceNsChanges* changes, const PlaceNsExchange* xch, PlaceNsIndex index);
+size_t place_ns_scratch_bytes(uint32_t n_nodes, uint32_t n_domains, uint32_t n_reqs, uint32_t n_namespaces);
+size_t node_index_scratch_bytes(uint32_t n_domains);
+int launch_node_index(const lwse_node_rec* d_nodes, uint32_t n_nodes, uint32_t n_domains, uint32_t* d_dom_first,
+                      uint32_t* d_node_order, uint32_t* d_node_pos, void* d_scratch, int sm_count, cudaStream_t s,
+                      bool pdl, int* cuda_err);
+int launch_place_whatif_index(const lwse_place_req* d_reqs, uint32_t n_reqs, uint32_t n_namespaces, const uint8_t* d_touched,
+                              uint32_t n_nodes, uint32_t n_domains, void* d_scratch, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_place_whatif_diff(const lwse_place_out* d_before, const lwse_place_out* d_after, uint32_t n_resident, uint32_t n_total,
+                             uint32_t* d_rows, lwse_place_out* d_outs_before, lwse_place_out* d_outs_after, uint32_t capacity,
+                             uint32_t* d_counts, int sm_count, cudaStream_t s, int* cuda_err);
+
+// ---- lwse_ds_kernels.cu ----
+int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s, int* cuda_err);
+
+struct DsTickHost {
+  const lwse_ds_out* prev_ds_out;
+  const lwse_ds_role_out* prev_role_out;
+  const lwse_ds_revrole_out* prev_revrole_out;
+  lwse_ds_out* m_ds_out;
+  lwse_ds_role_out* m_role_out;
+  lwse_ds_revrole_out* m_revrole_out;
+  uint8_t* marks;
+  uint32_t* rows;
+  uint32_t* counters;  // [0] count, [1] ticket
+  uint32_t* host_words;
+  uint32_t seq;
+  bool all;
+  const lwse_ds_link* links;  // non-null: the linked instance
+  const lwse_lws_rec* lws;
+  const lwse_lws_out* lws_out;
+  uint32_t n_lws;
+};
+int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s, int* cuda_err);
+
+struct DsForecastHost {
+  lwse_ds_revrole_rec* rows;
+  lwse_ds_out* s_ds_out;
+  lwse_ds_role_out* s_role_out;
+  lwse_ds_revrole_out* s_revrole_out;
+  lwse_ds_forecast* fc;
+  lwse_ds_forecast_role* fc_role;
+  lwse_ds_role_out* steps;  // the write pass's rows (device scratch)
+  uint32_t step_capacity;
+  bool want_steps;  // a trajectory is asked for: the scan marks what does not fit in step_capacity
+  unsigned long long* totals;  // device, 2 words, zeroed by the caller
+};
+int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s,
+                       int* cuda_err);
+
+// ---- lwse_lws_forecast_kernels.cu ----
+struct LwsForecastHost {
+  const lwse_lws_rec* lws;
+  uint32_t n_lws;
+  const lwse_group_out* group_out;
+  uint32_t n_groups;
+  unsigned long long* slot_off;  // [n_lws]
+  uint8_t* slots;                // n_slots bytes (+ 8), sized after launch_lws_forecast_slots
+  uint32_t n_slots;
+  lwse_lws_forecast* fc;
+  lwse_lws_forecast_step* steps;  // the write pass's rows (device scratch)
+  uint32_t steps_rows;            // rows of `steps`
+  uint32_t step_capacity;
+  bool want_steps;               // a trajectory is asked for: the scan marks what does not fit
+  unsigned long long* totals;    // device: [0] rows needed, [1] rows written, [2] slots, [3] refused accesses
+                                 // (zeroed by the caller), then forecast_scan_words(n_lws) words for the scans
+};
+int launch_lws_forecast_slots(const LwsForecastHost* h, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_lws_forecast(const LwsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s, int* cuda_err);
+
+// ---- lwse_sha1_kernels.cu ----
+int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,
+                int sm_count, cudaStream_t s, int* cuda_err);
+int launch_subgroup_keys(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, const int32_t* d_pod_count,
+                         const int32_t* d_subgroup_size, const int32_t* d_worker_index, int32_t* d_index_out,
+                         uint8_t* d_digests, int sm_count, cudaStream_t s, int* cuda_err);
+
+// ---- lwse_exchange_kernels.cu ----
+int launch_exchange_push(const void* d_local_part, uint8_t* const* d_peer_base, void* d_local_base,
+                         uint64_t part_bytes, uint64_t part_stride, uint64_t half_bytes, uint64_t flags_offset,
+                         uint64_t step, uint64_t wait_step, uint32_t world, uint32_t rank, cudaStream_t s, int* cuda_err,
+                         bool lagged);
+
+}  // namespace lwse

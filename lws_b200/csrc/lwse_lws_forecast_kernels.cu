@@ -8,11 +8,10 @@
 //   scan (three kernels)           trajectory offsets, TRUNCATED (lwse_device.cuh)
 //   lws_forecast_kernel<W, true>   the replay again, writing the rows the scan reserved
 #include "lwse_device.cuh"
+#include "lwse_launch.cuh"
 #include "lwse_lws_pass.cuh"
 
 namespace lwse {
-
-int pick_tile(uint64_t items, uint64_t owners);  // lwse_lws_kernels.cu
 
 struct LwsForecastArgs {
   const lwse_lws_rec* lws;
@@ -201,23 +200,6 @@ __global__ void __launch_bounds__(256) lws_forecast_kernel(const LwsForecastArgs
   for (uint32_t i = blockIdx.x * kTilesPerBlock + threadIdx.x / W; i < a.n_lws; i += n_tiles)
     lws_forecast_one<W, kWrite>(a, i, lane);
 }
-
-struct LwsForecastHost {  // (lwse_engine.cu)
-  const lwse_lws_rec* lws;
-  uint32_t n_lws;
-  const lwse_group_out* group_out;
-  uint32_t n_groups;
-  unsigned long long* slot_off;  // [n_lws]
-  uint8_t* slots;                // n_slots bytes (+ 8), sized after launch_lws_forecast_slots
-  uint32_t n_slots;
-  lwse_lws_forecast* fc;
-  lwse_lws_forecast_step* steps;  // the write pass's rows (device scratch)
-  uint32_t steps_rows;            // rows of `steps`
-  uint32_t step_capacity;
-  bool want_steps;               // a trajectory is asked for: the scan marks what does not fit
-  unsigned long long* totals;    // device: [0] rows needed, [1] rows written, [2] slots, [3] refused accesses
-                                 // (zeroed by the caller), then forecast_scan_words(n_lws) words for the scans
-};
 
 static LwsForecastArgs forecast_args(const LwsForecastHost* h) {
   return LwsForecastArgs{h->lws,  h->n_lws, h->group_out, h->n_groups,   h->slot_off,

@@ -26,6 +26,7 @@
 #include <cstring>
 
 #include "lwse_device.cuh"
+#include "lwse_launch.cuh"
 #include "lwse_lws_pass.cuh"
 
 namespace lwse {
@@ -812,16 +813,6 @@ size_t lws_sweep_scratch_bytes(uint64_t n_pods, uint32_t n_groups) {
 
 // Returns the number of kernels launched (>=0) or -1 with *cuda_err set.
 // scratch: lws_sweep_scratch_bytes(n_pods, n_groups) bytes of device memory.
-struct SweepChangeLists {  // device (or mapped host) pointers; all null = off
-  uint32_t* lws_rows = nullptr;
-  lwse_lws_out* lws_out = nullptr;
-  uint32_t lws_capacity = 0;
-  uint32_t* group_rows = nullptr;
-  lwse_group_out* group_out = nullptr;
-  uint32_t group_capacity = 0;
-  uint32_t* counts = nullptr;  // device: [0] lws, [1] groups; zeroed by the caller (a tick's publish kernel resets them)
-};
-
 // first_pdl: the sweep's first kernel may start before the previous kernel on the stream has
 // finished (it reads only input tables before its griddepcontrol.wait) — false when that previous
 // kernel WRITES the input tables (the patch scatter of a tick).
@@ -1010,16 +1001,6 @@ __global__ void __launch_bounds__(kPublishThreads) publish_lists_kernel(const Pu
   }
 }
 
-struct PublishListHost {
-  const uint32_t* src_rows;
-  const void* src_outs;
-  uint32_t* dst_rows;
-  void* dst_outs;
-  uint32_t* count;   // null = skip this slot
-  uint32_t capacity;
-  uint32_t out_bytes;
-};
-
 // lists[0..2]: the three slots (host_words[k] receives the count of slot k).
 int launch_publish(const PublishListHost* lists, const uint32_t* d_extra, uint32_t* h_words, uint32_t seq_slot,
                    uint32_t seq, uint32_t* d_ticket, uint32_t expected_rows, cudaStream_t s, int* cuda_err,
@@ -1071,6 +1052,7 @@ struct ScatterArgs {
   uint32_t* occupancy;  // nullable
   uint32_t n_nodes;
 };
+static_assert(sizeof(ScatterArgs) <= kScatterDescBytes, "a graph tick's descriptor slot holds the scatter's arguments");
 
 __device__ __forceinline__ void scatter_body(const ScatterArgs& a) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.total_work; i += gridDim.x * blockDim.x) {
@@ -1141,16 +1123,6 @@ __global__ void __launch_bounds__(256) scatter_rows_desc_kernel(const ScatterArg
   scatter_body(s_a);
 }
 
-struct ScatterSegHost {
-  void* table;
-  uint64_t table_rows;
-  const uint32_t* rows;
-  const void* values;
-  uint32_t n;
-  uint32_t row_bytes;
-  bool is_ident;
-};
-
 // Segment list -> kernel arguments.  false: more than kMaxScatterSegs segments, a row width the kernel
 // does not handle, or more than 2^32 work items.
 static bool fill_scatter_args(const ScatterSegHost* segs, int n_segs, uint32_t* d_occupancy, uint32_t n_nodes, ScatterArgs* out) {
@@ -1174,9 +1146,8 @@ static bool fill_scatter_args(const ScatterSegHost* segs, int n_segs, uint32_t* 
   return true;
 }
 
-// Graph form: the descriptor block (scatter_desc_bytes() bytes, written by write_scatter_desc into a
-// pinned slot and copied to d_desc by a node of the graph) and a fixed grid.
-size_t scatter_desc_bytes() { return sizeof(ScatterArgs); }
+// Graph form: the descriptor block (written by write_scatter_desc into a pinned slot of kScatterDescBytes
+// and copied to d_desc by a node of the graph) and a fixed grid.
 bool write_scatter_desc(void* h_desc, const ScatterSegHost* segs, int n_segs, uint32_t* d_occupancy, uint32_t n_nodes) {
   ScatterArgs a{};
   if (!fill_scatter_args(segs, n_segs, d_occupancy, n_nodes, &a)) return false;

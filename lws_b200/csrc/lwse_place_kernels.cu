@@ -27,6 +27,7 @@
 #include <cstdlib>
 
 #include "lwse_device.cuh"
+#include "lwse_launch.cuh"
 
 namespace cg = cooperative_groups;
 

@@ -48,6 +48,7 @@
 #include <cstdlib>
 
 #include "lwse_device.cuh"
+#include "lwse_launch.cuh"
 
 namespace lwse {
 
@@ -734,24 +735,6 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
 // --------------------------------------------------------------------------
 // launcher
 // --------------------------------------------------------------------------
-struct PlaceNsChanges {  // a tick's change list (device memory); prev == null: off
-  lwse_place_out* prev;
-  uint32_t* rows;
-  lwse_place_out* outs;
-  uint32_t* count;
-  uint32_t capacity;
-  int tick_slot;  // 0 / 1: the round's counters live in the tick slot's own block, which the tick's publish
-                  // kernel clears after reading (two ticks may be in flight); -1: the two alternating blocks
-  void* mid_event;  // cudaEvent_t or null: recorded between the condense and the namespace kernel (a tick graph
-                    // holds the sweep back until then, so that both branches reach the SMs together)
-};
-
-struct PlaceNsExchange {  // multi-rank: d_occupancy is the base of the exchange buffers (see PlaceNsArgs::xch_step)
-  const unsigned long long* step_ctr;
-  uint64_t half_bytes;
-  bool lagged;
-};
-
 static size_t up256(size_t v) { return (v + 255) / 256 * 256; }
 
 // scratch: [words (rows x 1 KB)] [nodes2 (same)] [dom_free] [ns_first] [unpinned] [counters: 2 blocks of 8 words]
@@ -824,11 +807,6 @@ static bool encode_words_map(CUtensorMap* map, void* g_words, uint32_t word_rows
   return fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, g_words, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-
-// index: kNsIndexNone = the request table is grouped by namespace; otherwise the indexed form, with the
-// index kept in the scratch (kNsIndexReuse: as the last build left it — the caller knows the namespace
-// column has not changed since; kNsIndexBuild: built first).
-enum PlaceNsIndex : uint32_t { kNsIndexNone = 0, kNsIndexReuse = 1, kNsIndexBuild = 2 };
 
 // Returns kernels launched or -1.  `fresh`: the scratch was (re)allocated: zero it first.
 int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, const uint32_t* d_node_order, uint32_t n_nodes,

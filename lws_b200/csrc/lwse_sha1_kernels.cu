@@ -14,6 +14,7 @@
 // The subgroup form appends "/<index>" itself: getSubGroupIndex (:249-255) is evaluated on the
 // device, in C's truncating division like Go's, and the decimal suffix never exists in memory.
 #include "lwse_device.cuh"
+#include "lwse_launch.cuh"
 
 namespace lwse {
 
