@@ -787,20 +787,20 @@ static uint32_t resident_ctas(K kernel, int sm_count) {
 }
 
 template <int W>
-static cudaError_t launch_group(const GroupSweepArgs& a, int sm_count, cudaStream_t s) {
+static cudaError_t launch_group(const GroupSweepArgs& a, int sm_count, cudaStream_t s, bool pdl) {
   constexpr uint32_t kTilesPerBlock = kGroupThreads / W;
   (void)sm_count;
   const uint32_t want = (a.n_groups + kTilesPerBlock - 1) / kTilesPerBlock;
-  return launch_pdl(group_sweep_kernel<W>, dim3(want < (1u << 20) ? want : (1u << 20)), dim3(kGroupThreads), 0, s, true, a);
+  return launch_pdl(group_sweep_kernel<W>, dim3(want < (1u << 20) ? want : (1u << 20)), dim3(kGroupThreads), 0, s, pdl, a);
 }
 
 template <int W>
-static cudaError_t launch_lws(const LwsSweepArgs& a, int sm_count, cudaStream_t s) {
+static cudaError_t launch_lws(const LwsSweepArgs& a, int sm_count, cudaStream_t s, bool pdl) {
   constexpr uint32_t kTilesPerBlock = 256 / W;
   static uint32_t resident = 0;
   if (resident == 0) resident = resident_ctas(lws_sweep_kernel<W>, sm_count);
   const uint32_t want = (a.n_lws + kTilesPerBlock - 1) / kTilesPerBlock;
-  return launch_pdl(lws_sweep_kernel<W>, dim3(want < resident ? want : resident), dim3(256), 0, s, true, a);
+  return launch_pdl(lws_sweep_kernel<W>, dim3(want < resident ? want : resident), dim3(256), 0, s, pdl, a);
 }
 
 constexpr int kScanUnroll = 4;  // 128-bit loads per lane per chunk: 4 x 512 B = 2 KB in flight per warp
@@ -825,7 +825,11 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
   //      kernel does not write them)
   //   2  programmatically dependent, waits at its top (the predecessor kernel — a tick's patch
   //      scatter — WRITES the input tables)
+  // Only the fused kernel can wait at its top.  The group pass and the LWS pass read input rows
+  // before their wait, so when one of them is the sweep's first kernel (no pod rows: no scan; no
+  // group rows: no group pass) mode 2 launches it as an ordinary launch.
   const bool first_pdl = first_mode == 1;
+  const bool behind_writer = first_mode == 2;
   *cuda_err = 0;
   int launches = 0;
   cudaError_t e = cudaSuccess;
@@ -882,11 +886,12 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
     GroupSweepArgs a{t->lws,   t->groups, t->pod_state, t->pod_ident, pending_bits, event_bits, d_nodes,
                      t->group_out, gflag8, t->n_pods, t->n_lws, t->n_groups, n_nodes, t->flags, ChangeList{}, nullptr};
     if (cl && cl->group_rows) a.changes = ChangeList{cl->group_rows, cl->group_out, cl->counts + 1, cl->group_capacity};
+    const bool pdl = !(behind_writer && launches == 0);
     switch (w) {
-      case 8: e = launch_group<8>(a, sm_count, s); break;
-      case 4: e = launch_group<4>(a, sm_count, s); break;
-      case 2: e = launch_group<2>(a, sm_count, s); break;
-      default: e = launch_group<1>(a, sm_count, s); break;
+      case 8: e = launch_group<8>(a, sm_count, s, pdl); break;
+      case 4: e = launch_group<4>(a, sm_count, s, pdl); break;
+      case 2: e = launch_group<2>(a, sm_count, s, pdl); break;
+      default: e = launch_group<1>(a, sm_count, s, pdl); break;
     }
     if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
     launches++;
@@ -894,13 +899,14 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
   if (t->n_lws && !(t->flags & LWSE_SWEEP_SKIP_LWS_PASS)) {
     LwsSweepArgs a{t->lws, gflag8, t->lws_out, t->n_lws, t->n_groups, t->flags, ChangeList{}};
     if (cl && cl->lws_rows) a.changes = ChangeList{cl->lws_rows, cl->lws_out, cl->counts + 0, cl->lws_capacity};
+    const bool pdl = !(behind_writer && launches == 0);
     switch (pick_tile(t->n_groups, t->n_lws)) {
-      case 1: e = launch_lws<1>(a, sm_count, s); break;
-      case 2: e = launch_lws<2>(a, sm_count, s); break;
-      case 4: e = launch_lws<4>(a, sm_count, s); break;
-      case 8: e = launch_lws<8>(a, sm_count, s); break;
-      case 16: e = launch_lws<16>(a, sm_count, s); break;
-      default: e = launch_lws<32>(a, sm_count, s); break;
+      case 1: e = launch_lws<1>(a, sm_count, s, pdl); break;
+      case 2: e = launch_lws<2>(a, sm_count, s, pdl); break;
+      case 4: e = launch_lws<4>(a, sm_count, s, pdl); break;
+      case 8: e = launch_lws<8>(a, sm_count, s, pdl); break;
+      case 16: e = launch_lws<16>(a, sm_count, s, pdl); break;
+      default: e = launch_lws<32>(a, sm_count, s, pdl); break;
     }
     if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
     launches++;
