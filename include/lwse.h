@@ -32,6 +32,8 @@
  *                      203-236 (cleanup predicate), service_manager.go:57-89
  *   lwse_ds_resident_* the same arithmetic over resident DS tables, fed by DS and child-LWS
  *                      watch events (disaggregatedset_controller.go:55-126, :273)
+ *   lwse_resident_drain_*  pod_controller.go:204-266 (handleRestartPolicy), :268-295, :338-362 over
+ *                      the resident tables with the pods of drained nodes deleting
  *   lwse_group_keys_*  pkg/webhooks/pod_webhook.go:180-182 + pkg/utils/utils.go:39-43
  *                      (SHA-1 group / subgroup keys)
  *   lwse_subgroup_keys_*  pkg/webhooks/pod_webhook.go:249-255 (getSubGroupIndex) + :130,:151
@@ -775,6 +777,77 @@ typedef struct lwse_place_whatif {
   uint32_t form;                  /* LWSE_TICK_FORM_NAMESPACE or LWSE_TICK_FORM_GENERAL                 */
 } lwse_place_whatif;
 LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q);
+
+/* ---- drain what-if ------------------------------------------------------------------------------
+ * "If I drain these nodes, which LeaderWorkerSet groups restart?" — answered on the resident tables
+ * without changing them.  With RecreateGroupOnPodRestart / RecreateGroupAfterStart, evicting one pod of
+ * a group deletes its leader and so recreates the whole group (handleRestartPolicy,
+ * pod_controller.go:204-266, behind the pending gate of pendingPodsInGroup :338-362 and the owner chain
+ * of workerPodBelongsToLeader :268-295).
+ *
+ * Definition: for a set D of node rows, the what-if rows are the group result rows of a sweep of the
+ * resident tables (the sweep flags of the most recently submitted sweep) with two changes — the rows the
+ * informer produces when eviction sets deletionTimestamp on every pod bound to those nodes:
+ *   - LWSE_POD_DELETING is set in the state byte of every pod whose identity row has LWSE_PODID_SCHEDULED
+ *     and a node field in D;
+ *   - LWSE_GRP_POD_DELETING is set on every group row whose leader_node is in D.
+ * Nothing else changes.  The LWS pass reads only the five low flag bits of a group result row, which
+ * eviction changes on no row, so the LWS result rows do not change and only group rows are returned.
+ *
+ * The baseline ("before") is the group results of the most recently submitted sweep, in flight or not:
+ * the rows lwse_resident_forecast snapshots, under the same readiness rule.
+ *
+ * Isolation: as lwse_resident_place_whatif — under the engine mutex, on the what-if stream behind an event
+ * recorded on the engine's stream, with scratch of its own (a copy of the pod-state column and of the
+ * group rows, the sweep's bitmaps and result rows); it never drains, waits for the results of, or drops a
+ * tick, and touches no tick graph, arena, change list, resident table, output row, occupancy counter, node
+ * index or tick info.  The scratch only grows.
+ *
+ * Multi-rank engines: both calls see only this rank's objects.  Every count is a sum over groups and a
+ * group lives on one rank, so the sum of the ranks' answers is the cluster's answer.
+ *
+ * Returns LWSE_ERR_NOT_READY before lwse_resident_load, before a node table is uploaded, and while the
+ * group results do not belong to the resident rows (after a load, and after a patch of LWS, group or pod
+ * rows made without a sweep, until the next sweep is enqueued).  LWSE_ERR_INVALID_ARG for a NULL query, a
+ * node row at or beyond n_nodes, or a NULL buffer with a count > 0.  Duplicate node rows are allowed. */
+typedef struct lwse_drain_whatif {
+  /* in */
+  const uint32_t* nodes;      /* [n_nodes] node rows of D, host memory                                  */
+  uint32_t n_nodes;
+  uint32_t capacity;          /* rows the change buffers below hold                                     */
+  uint32_t* rows;             /* [capacity]: group rows whose result differs from the baseline          */
+  lwse_group_out* before;     /* [capacity]: their baseline rows                                        */
+  lwse_group_out* after;      /* [capacity]: their what-if rows                                         */
+  /* out */
+  uint32_t n_changed;         /* every group row that differs (rows beyond capacity not listed; order
+                                 unspecified)                                                          */
+  uint32_t n_pods_evicted;    /* identity rows scheduled on a node of D                                 */
+  uint32_t n_leaders_evicted; /* group rows whose leader_node is in D                                   */
+  uint32_t n_groups_restarted;/* LWSE_GOUT_DELETE_LEADER | LWSE_GOUT_LEADER_DELETING clear before, set
+                                 after                                                                 */
+  uint32_t n_ready_restarted; /* of those, the groups with LWSE_GOUT_COND_READY in the baseline         */
+  uint32_t reserved;
+  uint64_t n_pods_recreated;  /* sum of pod_count over the restarted groups                             */
+} lwse_drain_whatif;
+LWSE_API int lwse_resident_drain_whatif(lwse_engine* e, lwse_drain_whatif* q);
+
+/* The drain cost of every node of the resident node table: row n holds the totals of
+ * lwse_resident_drain_whatif with D = {n}, all nodes in one pass (32 B per node).  Exact in one pass: take
+ * a group whose baseline has neither restart bit.  Draining n restarts it iff some pod of the group bound
+ * to n passes handleRestartPolicy with its deleting bit set; that per-pod verdict reads only the pod's
+ * state byte and identity row, the group row and the group's pending state (none of which the deletion of
+ * other pods changes), and the leader's deleting bit only chooses between DELETE_LEADER and
+ * LEADER_DELETING.  A group that already has a restart bit never counts.  Same readiness, isolation and
+ * errors as lwse_resident_drain_whatif; `out` holds n_nodes rows of host memory. */
+typedef struct lwse_drain_cost {
+  uint32_t pods;             /* n_pods_evicted = lwse_resident_occupancy[n]                             */
+  uint32_t leaders;          /* n_leaders_evicted                                                       */
+  uint32_t groups_restarted; /* n_groups_restarted                                                      */
+  uint32_t ready_restarted;  /* n_ready_restarted                                                       */
+  uint64_t pods_recreated;   /* n_pods_recreated                                                        */
+  uint64_t reserved;
+} lwse_drain_cost;
+LWSE_API int lwse_resident_drain_cost(lwse_engine* e, lwse_drain_cost* out);
 
 /* ------------------------------------------------------------------------- */
 /* Peer exchange: the multi-GPU placement step without a collective library  */

@@ -218,6 +218,10 @@ struct lwse_engine {
   PinBuf wf_words;                   // the counts, copied back
   uint32_t wf_geometry[4] = {0, 0, 0, 0};  // (n_reqs, n_namespaces, nodes, domains) the round scratch was laid out for
   uint32_t wf_calls = 0;
+  // drain what-if / drain cost (lwse_resident_drain_*): on the what-if stream, copies of the state column and the
+  // group rows, the sweep's bitmaps and group rows, the node mask, the change list and the cost rows
+  DevBuf dr_state, dr_groups, dr_out, dr_scan, dr_mask, dr_list, dr_cost;
+  uint32_t r_sweep_flags = 0;        // LWSE_SWEEP_GANG of the most recently submitted sweep (r_group_out's flags)
   DevBuf sha_bytes, sha_offsets, sha_digests, sha_ints;
   uint32_t* h_rounds = nullptr;  // pinned
   // peer exchange of the multi-GPU placement step (lwse_exchange_*)
@@ -434,7 +438,8 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->fc_revrole_out, &e->fc_ds, &e->fc_roles, &e->fc_steps, &e->fc_totals,
                       &e->lf_lws, &e->lf_group_out, &e->lf_slot_off, &e->lf_slots, &e->lf_fc, &e->lf_steps, &e->lf_totals,
                       &e->wf_nodes, &e->wf_reqs, &e->wf_out, &e->wf_dom_first, &e->wf_node_order, &e->wf_node_pos,
-                      &e->wf_node_ix, &e->wf_touched, &e->wf_round, &e->wf_list};
+                      &e->wf_node_ix, &e->wf_touched, &e->wf_round, &e->wf_list,
+                      &e->dr_state, &e->dr_groups, &e->dr_out, &e->dr_scan, &e->dr_mask, &e->dr_list, &e->dr_cost};
     if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
     if (e->lf_stream) cudaStreamSynchronize(e->lf_stream);
     if (e->wf_stream) cudaStreamSynchronize(e->wf_stream);
@@ -1704,7 +1709,10 @@ static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t
     ts.published = published;
     ts.wrote = wrote_any;
     e->t_submitted++;
-    if (do_sweep) e->r_swept = e->r_groups_swept = true;
+    if (do_sweep) {
+      e->r_swept = e->r_groups_swept = true;
+      e->r_sweep_flags = flags & LWSE_SWEEP_GANG;
+    }
     if (round_asked) e->r_place_current = true;
     e->main_unforked = !do_place && (e->main_unforked || wrote_main);
     lwse_tick_info& ti = e->last_tick_info;
@@ -2196,6 +2204,15 @@ LWSE_API int lwse_resident_node_info(lwse_engine* e, lwse_node_info* info) {
 // ---------------------------------------------------------------------------
 // Placement what-if
 // ---------------------------------------------------------------------------
+// LWSE_WHATIF_TIMING=1: CUDA events around the device work of every what-if (lwse_debug_whatif_device_us)
+static bool whatif_timing() {
+  static const bool on = [] {
+    const char* v = getenv("LWSE_WHATIF_TIMING");
+    return v && atoi(v) != 0;
+  }();
+  return on;
+}
+
 // Patched copies of the node and request rows in what-if scratch, the round over them on wf_stream
 // (only the touched namespaces in the namespace form), then one diff kernel against the baseline rows
 // (r_pout, read in place: nothing writes them while the call holds the mutex).  The resident node
@@ -2315,10 +2332,7 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
   // the snapshot: behind everything on the engine's stream, both branches of every tick submitted so far joined
   LWSE_CUDA(e, cudaEventRecord(e->ev_wf, e->stream));
   LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_wf, 0));
-  static const bool timing = [] {  // LWSE_WHATIF_TIMING=1: CUDA events on the what-if stream (measurements)
-    const char* v = getenv("LWSE_WHATIF_TIMING");
-    return v && atoi(v) != 0;
-  }();
+  const bool timing = whatif_timing();
   e->wf_timed = false;
   if (timing) {
     if (!e->ev_wf_t0) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t0));
@@ -2437,6 +2451,142 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
   q->n_conflict = words[6];
   q->namespaces_solved = ns_form ? n_touched : 0u;
   q->form = ns_form ? LWSE_TICK_FORM_NAMESPACE : LWSE_TICK_FORM_GENERAL;
+  return LWSE_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Drain what-if and drain cost
+// ---------------------------------------------------------------------------
+// Both on wf_stream behind an event on the engine's stream (the most recently submitted tick, both branches
+// joined), reading the resident tables and the baseline group results in place: nothing writes them while
+// the call holds the mutex, and the call synchronizes its stream before it returns.
+static int drain_begin_locked(lwse_engine* e) {
+  if (!e->wf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->wf_stream, cudaStreamNonBlocking));
+  if (!e->ev_wf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_wf, cudaEventDisableTiming));
+  LWSE_CUDA(e, cudaEventRecord(e->ev_wf, e->stream));
+  LWSE_CUDA(e, cudaStreamWaitEvent(e->wf_stream, e->ev_wf, 0));
+  e->wf_timed = false;
+  if (whatif_timing()) {
+    if (!e->ev_wf_t0) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t0));
+    if (!e->ev_wf_t1) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t1));
+    LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t0, e->wf_stream));
+  }
+  return LWSE_OK;
+}
+
+static int drain_end_locked(lwse_engine* e) {
+  if (whatif_timing()) {
+    LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t1, e->wf_stream));
+    e->wf_timed = true;
+  }
+  return LWSE_OK;
+}
+
+// Copies of the state column and the group rows, the mark kernel on them, the sweep's group pass over
+// {resident LWS rows, copied groups, copied states, resident identity rows} into rows of its own (the LWS
+// pass is skipped: it reads only flag bits eviction does not change), then the diff against the baseline.
+LWSE_API int lwse_resident_drain_whatif(lwse_engine* e, lwse_drain_whatif* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->r_loaded || e->n_nodes == 0 || !e->r_groups_swept) return LWSE_ERR_NOT_READY;
+  if ((q->n_nodes && !q->nodes) || (q->capacity && (!q->rows || !q->before || !q->after))) return LWSE_ERR_INVALID_ARG;
+  for (uint32_t i = 0; i < q->n_nodes; i++)
+    if (q->nodes[i] >= e->n_nodes) return LWSE_ERR_INVALID_ARG;
+  const uint32_t ng = e->rn_groups, nn = e->n_nodes;
+  const uint64_t np = e->rn_pods;
+  const uint32_t list_cap = q->capacity < ng ? q->capacity : ng;  // (at most ng rows can differ)
+  DeviceGuard guard(e->device);
+  LWSE_CUDA(e, e->wf_stage.reserve((size_t)nn));  // (the previous what-if synchronized its stream: free)
+  LWSE_CUDA(e, e->wf_words.reserve(64));
+  LWSE_CUDA(e, e->dr_state.reserve((size_t)np + 16));
+  LWSE_CUDA(e, e->dr_groups.reserve((size_t)ng * sizeof(lwse_group_rec) + 16));
+  LWSE_CUDA(e, e->dr_out.reserve((size_t)ng * sizeof(lwse_group_out) + 16));
+  LWSE_CUDA(e, e->dr_scan.reserve(lwse::lws_sweep_scratch_bytes(np, ng)));
+  LWSE_CUDA(e, e->dr_mask.reserve((size_t)nn + 16));
+  // (layout: [counts: 16 words] [rows: list_cap] [before: list_cap] [after: list_cap], the 16-byte rows aligned)
+  const size_t rows_bytes = ((size_t)list_cap * 4 + 15) & ~(size_t)15;
+  LWSE_CUDA(e, e->dr_list.reserve(64 + rows_bytes + (size_t)list_cap * 2 * sizeof(lwse_group_out)));
+  uint8_t* mask = static_cast<uint8_t*>(e->wf_stage.h);
+  memset(mask, 0, nn);
+  for (uint32_t i = 0; i < q->n_nodes; i++) mask[q->nodes[i]] = 1;
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* d_counts = (uint32_t*)e->dr_list.p;
+  uint32_t* d_rows = d_counts + 16;
+  lwse_group_out* d_before = reinterpret_cast<lwse_group_out*>(static_cast<uint8_t*>(e->dr_list.p) + 64 + rows_bytes);
+  lwse_group_out* d_after = d_before + list_cap;
+  if (np) LWSE_CUDA(e, cudaMemcpyAsync(e->dr_state.p, e->r_pst.p, (size_t)np, cudaMemcpyDeviceToDevice, s));
+  if (ng) LWSE_CUDA(e, cudaMemcpyAsync(e->dr_groups.p, e->r_groups.p, (size_t)ng * sizeof(lwse_group_rec), cudaMemcpyDeviceToDevice, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(e->dr_mask.p, mask, nn, cudaMemcpyHostToDevice, s));
+  LWSE_CUDA(e, cudaMemsetAsync(d_counts, 0, 64, s));
+  int cuda_err = 0;
+  int launched = lwse::launch_drain_mark((const uint8_t*)e->dr_mask.p, nn, (const lwse_pod_ident*)e->r_pid.p, (uint8_t*)e->dr_state.p,
+                                         np, (lwse_group_rec*)e->dr_groups.p, ng, d_counts, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  lwse_lws_tables d{};
+  d.lws = (const lwse_lws_rec*)e->r_lws.p;
+  d.n_lws = e->rn_lws;
+  d.groups = (const lwse_group_rec*)e->dr_groups.p;
+  d.n_groups = ng;
+  d.pod_state = (const lwse_pod_state*)e->dr_state.p;
+  d.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
+  d.n_pods = np;
+  d.group_out = (lwse_group_out*)e->dr_out.p;
+  d.flags = e->r_sweep_flags | LWSE_SWEEP_SKIP_LWS_PASS;
+  launched = lwse::launch_lws_sweep(&d, (const lwse_node_rec*)e->nodes.p, nn, e->dr_scan.p, e->sm_count, s, &cuda_err, nullptr,
+                                    nullptr, /*first_mode=*/0);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  launched = lwse::launch_drain_diff((const lwse_group_out*)e->r_group_out.p, (const lwse_group_out*)e->dr_out.p,
+                                     (const lwse_group_rec*)e->r_groups.p, ng, d_rows, d_before, d_after, list_cap, d_counts,
+                                     e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_counts, 32, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint32_t n_changed = words[0];
+  const uint32_t listed = n_changed < list_cap ? n_changed : list_cap;
+  if (listed) {
+    LWSE_CUDA(e, cudaMemcpyAsync(q->rows, d_rows, (size_t)listed * 4, cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaMemcpyAsync(q->before, d_before, (size_t)listed * sizeof(lwse_group_out), cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaMemcpyAsync(q->after, d_after, (size_t)listed * sizeof(lwse_group_out), cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaStreamSynchronize(s));
+  }
+  q->n_changed = n_changed;
+  q->n_pods_evicted = words[1];
+  q->n_leaders_evicted = words[2];
+  q->n_groups_restarted = words[3];
+  q->n_ready_restarted = words[4];
+  uint64_t recreated = 0;
+  memcpy(&recreated, words + 6, 8);
+  q->n_pods_recreated = recreated;
+  return LWSE_OK;
+}
+
+// Every node in one pass: the rows start as {pods = the resident occupancy counter, zeros}, then
+// drain_cost_kernel adds each group's restart to the nodes it would restart from.
+LWSE_API int lwse_resident_drain_cost(lwse_engine* e, lwse_drain_cost* out) {
+  if (!e) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->r_loaded || e->n_nodes == 0 || !e->r_groups_swept) return LWSE_ERR_NOT_READY;
+  if (!out) return LWSE_ERR_INVALID_ARG;
+  const uint32_t nn = e->n_nodes;
+  DeviceGuard guard(e->device);
+  LWSE_CUDA(e, e->dr_cost.reserve((size_t)nn * sizeof(lwse_drain_cost) + 16));
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  lwse_drain_cost* d_cost = (lwse_drain_cost*)e->dr_cost.p;
+  LWSE_CUDA(e, cudaMemsetAsync(d_cost, 0, (size_t)nn * sizeof(lwse_drain_cost), s));
+  LWSE_CUDA(e, cudaMemcpy2DAsync(d_cost, sizeof(lwse_drain_cost), e->r_occ.p, 4, 4, nn, cudaMemcpyDeviceToDevice, s));
+  int cuda_err = 0;
+  const int launched = lwse::launch_drain_cost((const lwse_lws_rec*)e->r_lws.p, e->rn_lws, (const lwse_group_rec*)e->r_groups.p,
+                                               e->rn_groups, (const uint8_t*)e->r_pst.p, (const lwse_pod_ident*)e->r_pid.p,
+                                               e->rn_pods, (const lwse_group_out*)e->r_group_out.p, d_cost, nn, e->sm_count, s,
+                                               &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(out, d_cost, (size_t)nn * sizeof(lwse_drain_cost), cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
   return LWSE_OK;
 }
 

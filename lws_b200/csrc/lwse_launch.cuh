@@ -179,6 +179,20 @@ struct LwsForecastHost {
 int launch_lws_forecast_slots(const LwsForecastHost* h, int sm_count, cudaStream_t s, int* cuda_err);
 int launch_lws_forecast(const LwsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s, int* cuda_err);
 
+// ---- lwse_drain_kernels.cu ----
+// The drain what-if's counters (device, 16 words, zeroed by the caller): [0] changed rows [1] pods evicted
+// [2] leaders evicted [3] groups restarted [4] ready groups restarted [6..7] pods recreated (u64).
+int launch_drain_mark(const uint8_t* d_mask, uint32_t n_nodes, const lwse_pod_ident* d_ident, uint8_t* d_state, uint64_t n_pods,
+                      lwse_group_rec* d_groups, uint32_t n_groups, uint32_t* d_counts, int sm_count, cudaStream_t s,
+                      int* cuda_err);
+int launch_drain_diff(const lwse_group_out* d_before, const lwse_group_out* d_after, const lwse_group_rec* d_groups,
+                      uint32_t n_groups, uint32_t* d_rows, lwse_group_out* d_outs_before, lwse_group_out* d_outs_after,
+                      uint32_t capacity, uint32_t* d_counts, int sm_count, cudaStream_t s, int* cuda_err);
+// d_cost: n_nodes rows with `pods` filled in and every other field zero.
+int launch_drain_cost(const lwse_lws_rec* d_lws, uint32_t n_lws, const lwse_group_rec* d_groups, uint32_t n_groups,
+                      const uint8_t* d_state, const lwse_pod_ident* d_ident, uint64_t n_pods, const lwse_group_out* d_baseline,
+                      lwse_drain_cost* d_cost, uint32_t n_nodes, int sm_count, cudaStream_t s, int* cuda_err);
+
 // ---- lwse_sha1_kernels.cu ----
 int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,
                 int sm_count, cudaStream_t s, int* cuda_err);

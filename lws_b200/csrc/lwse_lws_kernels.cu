@@ -28,6 +28,7 @@
 #include "lwse_device.cuh"
 #include "lwse_launch.cuh"
 #include "lwse_lws_pass.cuh"
+#include "lwse_restart.cuh"
 
 namespace lwse {
 
@@ -249,40 +250,6 @@ struct GlobalBits {
   __device__ __forceinline__ uint32_t event(uint32_t w) const { return __ldcg(event_bits + w); }
 };
 
-// What deciding one event pod needs from its group (pod_controller.go:233-257).
-struct VisitCtx {
-  uint32_t rev_lo, rev_hi;  // leader pod's revision hash
-  uint32_t leader_uid, wsts_uid;
-  uint32_t pod_base;
-  uint32_t bits;  // kLeaderFound | kChainOk | kLeaderDeleting
-};
-constexpr uint32_t kLeaderFound = 1u, kChainOk = 2u, kLeaderDeleting = 4u;
-constexpr uint32_t kAccLeaderCand = 0x80000000u;
-
-// handleRestartPolicy (:204-266) for ONE pod that has a restart / deletion event, policy checks
-// already done: returns the verdict bits it contributes; *cand = it would recreate the group.
-__device__ __forceinline__ uint32_t visit_pod(const VisitCtx& c, uint32_t state, const uint4 id, bool& cand) {
-  uint32_t acc = 0;
-  bool deleting;
-  if (state & LWSE_POD_IS_LEADER) {
-    cand = true;  // leader = pod (:251)
-    deleting = state & LWSE_POD_DELETING;
-    acc |= kAccLeaderCand;
-  } else if (!(id.w & LWSE_PODID_NAME_OK)) {
-    cand = false;
-    return LWSE_GOUT_RESTART_ERROR;  // :230
-  } else {
-    const uint32_t kind = (state & LWSE_POD_OWNER_MASK) >> LWSE_POD_OWNER_SHIFT;
-    // workerPodBelongsToLeader :268-295
-    const bool belongs = (state & LWSE_POD_OWNER_NAME_MATCH) &&
-                         ((kind == 1u && id.z == c.leader_uid) || (kind == 2u && id.z == c.wsts_uid && (c.bits & kChainOk)));
-    cand = (c.bits & kLeaderFound) && id.x == c.rev_lo && id.y == c.rev_hi && belongs;  // :233, :239
-    deleting = c.bits & kLeaderDeleting;
-  }
-  if (!cand) return 0;
-  return acc | (deleting ? LWSE_GOUT_LEADER_DELETING : LWSE_GOUT_DELETE_LEADER);  // :255 / :259
-}
-
 // First part of the group pass for group g (row ca..cd, first 16 bytes of its owner L):
 // pendingPodsInGroup (:338-362) from the pending bitmap and the decision whether the group's
 // event pods have to be visited at all.
@@ -297,11 +264,10 @@ template <int W, class Bits>
 __device__ __forceinline__ GroupPre group_pre(const Bits& bits, uint32_t lane, const uint4 ca, const uint4 cb,
                                               const uint4 cc, const uint4 cd, const uint4 L) {
   GroupPre r;
-  const uint32_t pod_base = cc.z, pod_count = cc.w, gflags = cd.y;
+  const uint32_t pod_base = cc.z, pod_count = cc.w;
   const int32_t size = (int32_t)L.z;
   const uint32_t lflags = L.w;
-  const uint32_t policy = (lflags & LWSE_LWS_RESTART_MASK) >> LWSE_LWS_RESTART_SHIFT;
-  const bool policy_on = policy == LWSE_RESTART_ON_POD_RESTART || policy == LWSE_RESTART_AFTER_START;
+  const bool policy_on = restart_policy_on(lflags);
   r.oflags = 0;
   r.pod_end = pod_base + pod_count;  // <= n_pods < 2^32 (checked by the entry points)
   r.w_first = pod_base >> 5;
@@ -319,21 +285,9 @@ __device__ __forceinline__ GroupPre group_pre(const Bits& bits, uint32_t lane, c
   any_bits = tile_or<W>(any_bits);
   const bool pending = (uint32_t)size != pod_count || (any_bits & 1u);
   if (pending) r.oflags |= LWSE_GOUT_PENDING;
-  // :222 skip when pending ∧ (AfterStart ∨ annotation)
-  const bool suppressed =
-      pending && (policy == LWSE_RESTART_AFTER_START || (lflags & LWSE_LWS_RECREATE_AFTER_START_ANNOT));
+  const bool suppressed = restart_suppressed(pending, lflags);
   r.visit = (any_bits & 2u) && policy_on && !suppressed;
-  constexpr uint32_t kChain = LWSE_GRP_WSTS_FOUND | LWSE_GRP_WSTS_OWNER_IS_POD | LWSE_GRP_WSTS_OWNER_NAME_MATCH;
-  r.ctx.rev_lo = ca.x;
-  r.ctx.rev_hi = ca.y;
-  r.ctx.leader_uid = cb.z;
-  r.ctx.wsts_uid = cb.w;
-  r.ctx.pod_base = pod_base;
-  r.ctx.bits = 0;
-  if ((gflags & (LWSE_GRP_POD_PRESENT | LWSE_GRP_POD_NAME_MATCH)) == (LWSE_GRP_POD_PRESENT | LWSE_GRP_POD_NAME_MATCH))
-    r.ctx.bits |= kLeaderFound;  // :233
-  if ((gflags & kChain) == kChain && cc.x == cb.z) r.ctx.bits |= kChainOk;  // sts owner uid == leader uid
-  if (gflags & LWSE_GRP_POD_DELETING) r.ctx.bits |= kLeaderDeleting;
+  visit_ctx_of(r.ctx, ca, cb, cc, cd);
   return r;
 }
 

@@ -44,6 +44,8 @@ SYMBOLS = {
     "lwse_resident_tick_info": ([C.c_void_p, C.c_void_p], C.c_int),
     "lwse_resident_node_info": ([C.c_void_p, C.POINTER(R.NodeInfo)], C.c_int),
     "lwse_resident_place_whatif": ([C.c_void_p, C.POINTER(R.PlaceWhatIf)], C.c_int),
+    "lwse_resident_drain_whatif": ([C.c_void_p, C.POINTER(R.DrainWhatIf)], C.c_int),
+    "lwse_resident_drain_cost": ([C.c_void_p, C.c_void_p], C.c_int),
     "lwse_place_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
         C.c_int,
@@ -430,6 +432,35 @@ class Engine:
                "form": self.TICK_FORMS[q.form]}
         out.update({k: getattr(q, k) for k in R.PLACE_WHATIF})
         return out
+
+    def resident_drain_whatif(self, nodes, capacity=None):
+        """lwse_resident_drain_whatif: the group rows of a sweep of the resident tables with every pod scheduled
+        on one of the node rows ``nodes`` (and every leader whose group row names one) deleting — nothing
+        resident changes, and no tick is waited for.  ``capacity`` None lists every changed row.
+        → dict: ``rows`` / ``before`` / ``after`` (the group rows that differ from the last sweep, with both
+        rows) and the counters of ``records.DRAIN_WHATIF``."""
+        nodes = np.ascontiguousarray(nodes, dtype=np.uint32)
+        n_res = getattr(self, "_resident_shape", (0, 0))[1]
+        cap = n_res if capacity is None else int(capacity)
+        rows = np.zeros(max(cap, 1), np.uint32)
+        before, after = R.aligned_empty(max(cap, 1), R.GROUP_OUT), R.aligned_empty(max(cap, 1), R.GROUP_OUT)
+        q = R.DrainWhatIf()
+        q.nodes = R.ptr(nodes) if len(nodes) else None
+        q.n_nodes = len(nodes)
+        q.capacity = cap
+        q.rows, q.before, q.after = R.ptr(rows), R.ptr(before), R.ptr(after)
+        self._check(lib().lwse_resident_drain_whatif(self._h, C.byref(q)))
+        n = min(q.n_changed, cap)
+        out = {"rows": rows[:n], "before": before[:n], "after": after[:n]}
+        out.update({k: getattr(q, k) for k in R.DRAIN_WHATIF})
+        return out
+
+    def resident_drain_cost(self) -> np.ndarray:
+        """lwse_resident_drain_cost: one ``records.DRAIN_COST`` row per node of the resident node table, row n
+        holding the counters ``resident_drain_whatif([n])`` returns — every node in one pass."""
+        out = R.aligned_empty(max(self.n_nodes, 1), R.DRAIN_COST)
+        self._check(lib().lwse_resident_drain_cost(self._h, R.ptr(out)))
+        return out[: self.n_nodes]
 
     def resident_patch(self, which: int, rows, values):
         """Overwrite rows of a resident table (rows: uint32 indices, values: packed rows)."""

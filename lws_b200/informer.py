@@ -537,6 +537,31 @@ class IncrementalEncoder:
         return self._whatif_requests(int(self.lws["uid_hash"][row]), int(self.lws["size"][row]), self.ns_ids[key[0]],
                                      range(self.items[key].lws.replicas, replicas))
 
+    def whatif_drain(self, node_names) -> np.ndarray:
+        """The node rows of the named nodes, for ``Engine.resident_drain_whatif`` (sorted, each once)."""
+        return np.array(sorted({self.node_index[n] for n in node_names}), dtype=np.uint32)
+
+    def drain_place_query(self, result: dict, node_names) -> list:
+        """Segments for ``Engine.resident_place_whatif`` that ask where the groups a drain restarts would go:
+        a NODES segment that cordons the drained nodes (``whatif_cordon``) and a PLACE_REQS segment that unpins
+        (leader_node = NONE) the request rows of the groups ``result`` (a ``resident_drain_whatif`` answer for
+        the same nodes) restarts and of the groups whose leader is on a drained node.  A request row is its
+        group's row.
+
+        The answer is conservative: the placement what-if never moves occupancy, so the pods of a restarting
+        group on nodes that are not drained still count against those nodes."""
+        drained = self.whatif_drain(node_names)
+        restart = np.uint32(R.GOUT_DELETE_LEADER | R.GOUT_LEADER_DELETING)
+        hit = ((result["before"]["flags"] & restart) == 0) & ((result["after"]["flags"] & restart) != 0)
+        rows = set(result["rows"][hit].tolist())
+        owned = np.flatnonzero(self._group_lws[: len(self.groups)] >= 0)
+        rows |= set(owned[np.isin(self.groups["leader_node"][owned], drained)].tolist())
+        rows = np.array(sorted(rows), dtype=np.uint32)
+        vals = R.aligned_empty(len(rows), R.PLACE_REQ)
+        vals[:] = self.reqs[rows]
+        vals["leader_node"] = R.NONE
+        return [self.whatif_cordon(node_names), (R.TABLE_PLACE_REQS, rows, vals)]
+
     # ------------------------------------------------------------------ results
     def tables(self):
         """(lws, groups, pod_state, pod_ident, reqs) trimmed to the rows in use (+ spare already laid out)."""

@@ -502,6 +502,40 @@ PLACE_WHATIF = ("n_changed", "n_lost", "n_moved", "n_gained", "n_placed", "n_uns
                 "namespaces_solved")
 
 
+class DrainWhatIf(C.Structure):
+    """lwse_drain_whatif: the group rows of a sweep with the pods of a set of nodes deleting (node rows in,
+    changed group rows and the DRAIN_WHATIF counters out)."""
+
+    _fields_ = [
+        ("nodes", C.c_void_p),
+        ("n_nodes", C.c_uint32),
+        ("capacity", C.c_uint32),
+        ("rows", C.c_void_p),
+        ("before", C.c_void_p),
+        ("after", C.c_void_p),
+        ("n_changed", C.c_uint32),
+        ("n_pods_evicted", C.c_uint32),
+        ("n_leaders_evicted", C.c_uint32),
+        ("n_groups_restarted", C.c_uint32),
+        ("n_ready_restarted", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("n_pods_recreated", C.c_uint64),
+    ]
+
+
+# the counters of a drain what-if, as Engine.resident_drain_whatif returns them
+DRAIN_WHATIF = ("n_changed", "n_pods_evicted", "n_leaders_evicted", "n_groups_restarted", "n_ready_restarted",
+                "n_pods_recreated")
+
+# lwse_drain_cost: per node, the totals of a drain what-if of that node alone
+DRAIN_COST = np.dtype(
+    [("pods", "<u4"), ("leaders", "<u4"), ("groups_restarted", "<u4"), ("ready_restarted", "<u4"),
+     ("pods_recreated", "<u8"), ("reserved", "<u8")],
+    align=False,
+)
+assert DRAIN_COST.itemsize == 32
+
+
 class Config(C.Structure):
     _fields_ = [
         ("abi_version", C.c_uint32),
