@@ -78,6 +78,12 @@ struct PinBuf {
   }
 };
 
+// What the placement branch of a tick decided when it was enqueued; a tick graph keeps it for its replays.
+struct TickPlaceResult {
+  bool place_ns = false;                 // the round runs the namespace kernels (counters in the slot's block)
+  const uint32_t* rounds_ptr = nullptr;  // device: where the round counts
+};
+
 }  // namespace
 
 struct lwse_engine {
@@ -138,8 +144,7 @@ struct lwse_engine {
     uint32_t seen = 0;      // eager ticks with this key so far (the first one lets every buffer settle)
     uint32_t kernels = 0;   // kernel nodes (launch accounting)
     bool failed = false;    // capture or instantiation failed once: this key stays eager
-    bool place_ns = false;  // its round runs the namespace kernels (counters in the slot's block)
-    const uint32_t* rounds_ptr = nullptr;  // where its round counts
+    TickPlaceResult place;  // of the captured placement branch
   };
   std::unordered_map<uint32_t, TickGraph> tick_graphs;
   PinBuf tdesc;                      // 2 slots x kScatterDescBytes: the scatter's segment descriptors of the tick of that parity
@@ -149,7 +154,6 @@ struct lwse_engine {
   cudaStream_t pub_stream = nullptr;   // the publish kernels: tick k+1 starts while tick k's changed rows travel to the host
   cudaEvent_t ev_done = nullptr;       // behind the last kernel of a tick on the engine's stream (both branches joined)
   cudaEvent_t ev_mid = nullptr;        // (graph capture) between the condense and the namespace kernel
-  bool tick_place_ns = false;          // the last enqueue_place() ran the namespace kernels (their counters are per slot)
   int use_graph = 1;                 // LWSE_TICK_GRAPH: 0 never, 1 when a tick is in flight (default), 2 always
   uint64_t graph_ticks = 0;
   cudaEvent_t ev_pub = nullptr;      // behind the previous tick's publish kernel: the next tick's side stream starts there
@@ -506,36 +510,6 @@ static int build_node_index_locked(lwse_engine* e, cudaStream_t s, bool pdl, boo
   return LWSE_OK;
 }
 
-// Node-row patches of a tick (or of lwse_resident_patch), before any of them is applied: checks the
-// segments, brings the host mirror up to date and marks the index stale when a row's usability, or the
-// domain of a usable row, changed.  Capacity-only patches keep the index.  Returns the rows patched or < 0.
-static int node_patches_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs) {
-  uint32_t n_rows = 0;
-  for (uint32_t i = 0; i < n_segs; i++) {
-    const lwse_patch_seg& g = segs[i];
-    if (g.table != LWSE_TABLE_NODES || g.n == 0) continue;
-    if (e->n_nodes == 0) return LWSE_ERR_NOT_READY;
-    if (!g.values || (!(g.flags & LWSE_PATCH_RANGE) && !g.rows)) return LWSE_ERR_INVALID_ARG;
-    if ((g.flags & LWSE_PATCH_RANGE) && (uint64_t)g.first_row + g.n > e->n_nodes) return LWSE_ERR_BAD_TABLE;
-  }
-  for (uint32_t i = 0; i < n_segs; i++) {
-    const lwse_patch_seg& g = segs[i];
-    if (g.table != LWSE_TABLE_NODES) continue;
-    const lwse_node_rec* v = static_cast<const lwse_node_rec*>(g.values);
-    for (uint32_t k = 0; k < g.n; k++) {
-      const uint32_t row = (g.flags & LWSE_PATCH_RANGE) ? g.first_row + k : g.rows[k];
-      if (row >= e->n_nodes) continue;  // (the scatter kernel skips it too)
-      lwse_node_rec& old = e->h_nodes[row];
-      const bool was = node_usable(old, e->n_domains), is = node_usable(v[k], e->n_domains);
-      if (node_patch_moves_index(old, v[k], e->n_domains)) e->node_index_stale = true;
-      e->n_usable = e->n_usable - (was ? 1u : 0u) + (is ? 1u : 0u);
-      old = v[k];
-      n_rows++;
-    }
-  }
-  return (int)n_rows;
-}
-
 LWSE_API int lwse_upload_nodes(lwse_engine* e, const lwse_node_rec* nodes, uint32_t n_nodes,
                                uint32_t n_domains) {
   if (!e || (n_nodes && !nodes) || !aligned16(nodes)) return LWSE_ERR_INVALID_ARG;
@@ -838,20 +812,213 @@ static bool values_in_place(const lwse_engine* e, const lwse_patch_seg& g, uint3
          (rb == 1 ? (reinterpret_cast<uintptr_t>(g.values) & 3u) == 0 : aligned16(g.values));
 }
 
-// Enqueue the patch segments of a tick on the engine's stream.  *wrote = some table changed
-// (the sweep's first kernel then has to wait for the scatter kernel to finish).
-// `tables`: bit t set = apply the segments of lwse_table t (a tick applies the placement request
-// patches on the side stream, where the round that reads them runs, and the rest on the engine's
-// stream); `stage_base`: where in the staging buffer this call may put copies.
-struct ScatterPlan {  // a prepared scatter launch (apply_patches_locked with `defer`): the copy is enqueued, the kernel is not
+// What one walk over the segments of a tick (or of lwse_resident_patch, of a what-if) finds: every argument
+// check, and what the caller decides from.  The walk writes nothing; commit_segments does, once it passed.
+struct SegSummary {
+  uint32_t tables = 0;       // bit t: a segment of lwse_table t has rows
+  bool any_range = false;    // a LWSE_PATCH_RANGE segment has rows
+  bool all_in_place = true;  // no scattered segment needs the staging buffer
+  size_t stage_bytes = 0;    // staging the segments outside the arena need
+  bool ns_moves = false;     // a request row moves to another namespace
+  uint32_t node_rows = 0;    // node rows patched (rows inside the table: the scatter kernel skips the others too)
+  bool node_moves = false;   // one of them changes whether its node is usable, or the domain of a usable node
+};
+
+static int summarize_segments(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, SegSummary* out) {
+  SegSummary ss;
+  if (n_segs && (!segs || n_segs > LWSE_TICK_MAX_SEGS)) return LWSE_ERR_INVALID_ARG;
+  for (uint32_t i = 0; i < n_segs; i++) {
+    const lwse_patch_seg& g = segs[i];
+    void* base;
+    uint64_t rows;
+    uint32_t rb;
+    if (!resident_table(e, g.table, &base, &rows, &rb)) return LWSE_ERR_INVALID_ARG;
+    if (g.n == 0) continue;
+    const bool range = (g.flags & LWSE_PATCH_RANGE) != 0;
+    if (!g.values || (!range && !g.rows)) return LWSE_ERR_INVALID_ARG;
+    if (range && (uint64_t)g.first_row + g.n > rows) return LWSE_ERR_BAD_TABLE;
+    ss.tables |= 1u << g.table;
+    if (range) {
+      ss.any_range = true;
+    } else {
+      if (!rows_in_place(e, g)) ss.stage_bytes += align256((size_t)g.n * 4);
+      if (!values_in_place(e, g, rb)) ss.stage_bytes += align256((size_t)g.n * rb);
+    }
+    if (g.table == LWSE_TABLE_PLACE_REQS) {
+      const lwse_place_req* v = static_cast<const lwse_place_req*>(g.values);
+      for (uint32_t k = 0; k < g.n && !ss.ns_moves; k++) {
+        const uint32_t row = range ? g.first_row + k : g.rows[k];
+        ss.ns_moves = row < e->rn_reqs && v[k].ns != e->r_req_ns[row];
+      }
+    } else if (g.table == LWSE_TABLE_NODES) {
+      // (a row patched twice is compared with the mirror both times: some step of old -> v1 -> v2 moves the
+      // index exactly when v1 or v2 differs from old in what the index is sorted by)
+      const lwse_node_rec* v = static_cast<const lwse_node_rec*>(g.values);
+      for (uint32_t k = 0; k < g.n; k++) {
+        const uint32_t row = range ? g.first_row + k : g.rows[k];
+        if (row >= e->n_nodes) continue;
+        ss.node_rows++;
+        if (node_patch_moves_index(e->h_nodes[row], v[k], e->n_domains)) ss.node_moves = true;
+      }
+    }
+  }
+  ss.all_in_place = ss.stage_bytes == 0;
+  *out = ss;
+  return LWSE_OK;
+}
+
+// The host mirrors follow the segments, once all of them passed their checks: the node table's (and the
+// usable-node count; the index is stale when a row moved it) and the request table's namespace column.  A
+// request that moves to another namespace breaks the grouping the fast placement kernels rely on, and the
+// namespace index of an ungrouped table.
+static void commit_segments(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, const SegSummary& ss) {
+  if (ss.node_moves) e->node_index_stale = true;
+  for (uint32_t i = 0; i < n_segs; i++) {
+    const lwse_patch_seg& g = segs[i];
+    const bool nodes = g.table == LWSE_TABLE_NODES && ss.node_rows, reqs = g.table == LWSE_TABLE_PLACE_REQS && ss.ns_moves;
+    if (!nodes && !reqs) continue;
+    for (uint32_t k = 0; k < g.n; k++) {
+      const uint32_t row = (g.flags & LWSE_PATCH_RANGE) ? g.first_row + k : g.rows[k];
+      if (nodes && row < e->n_nodes) {
+        const lwse_node_rec& now = static_cast<const lwse_node_rec*>(g.values)[k];
+        e->n_usable = e->n_usable - (node_usable(e->h_nodes[row], e->n_domains) ? 1u : 0u) + (node_usable(now, e->n_domains) ? 1u : 0u);
+        e->h_nodes[row] = now;
+      } else if (reqs && row < e->rn_reqs && static_cast<const lwse_place_req*>(g.values)[k].ns != e->r_req_ns[row]) {
+        e->r_req_ns[row] = static_cast<const lwse_place_req*>(g.values)[k].ns;
+        e->r_place_grouped = false;
+        e->r_ns_index_ok = false;
+      }
+    }
+  }
+}
+
+// Which resident outputs stop belonging to the resident rows when rows of `tables` are patched and no sweep
+// (`swept` false) / no placement round (`placed` false) follows in the same tick.  r_lws_out: the LWS rows (a
+// row reused for another object would pass the linked DS tick's uid test with the previous object's results);
+// r_group_out: the LWS, group and pod rows; r_pout: the node, request and identity rows a round reads.
+static void mark_outputs_stale(lwse_engine* e, uint32_t tables, bool swept, bool placed) {
+  constexpr uint32_t kGroupInputs = (1u << LWSE_TABLE_LWS) | (1u << LWSE_TABLE_GROUPS) | (1u << LWSE_TABLE_POD_STATE) | (1u << LWSE_TABLE_POD_IDENT);
+  constexpr uint32_t kRoundInputs = (1u << LWSE_TABLE_NODES) | (1u << LWSE_TABLE_PLACE_REQS) | (1u << LWSE_TABLE_POD_IDENT);
+  if (!swept && (tables & (1u << LWSE_TABLE_LWS))) e->r_swept = false;
+  if (!swept && (tables & kGroupInputs)) e->r_groups_swept = false;
+  if (!placed && (tables & kRoundInputs)) e->r_place_current = false;
+}
+
+// Room in the staging buffer for the segments that lie outside the arena (rare).  Growing replaces the
+// buffer, so nothing may still be reading it.
+static int reserve_stage(lwse_engine* e, size_t bytes) {
+  if (bytes <= e->stage.cap) return LWSE_OK;
+  LWSE_CUDA(e, cudaStreamSynchronize(e->stream));
+  LWSE_CUDA(e, cudaStreamSynchronize(e->side_stream));
+  LWSE_CUDA(e, e->stage.reserve(bytes));
+  return LWSE_OK;
+}
+
+// A prepared scatter: where the kernel reads each segment, and the copies that go in front of it.
+struct ScatterPlan {
+  struct Copy {
+    void* dst;
+    const void* src;
+    size_t bytes;
+  };
   lwse::ScatterSegHost sc[LWSE_TICK_MAX_SEGS];
   int n = 0;
-  bool recount = false;
-  // with `plan_only`: nothing was enqueued at all; the arena span [lo, hi) still has to be copied
-  // to the mirror (dma), or — staged segments, range segments — the plan cannot be replayed (eager_only)
-  bool dma = false, eager_only = false;
-  size_t lo = 0, hi = 0;
+  Copy ranges[LWSE_TICK_MAX_SEGS];  // range segments: one DMA copy straight into the table, in segment order
+  int n_ranges = 0;
+  Copy spans[2];                    // the arena / staging spans the kernel reads from their device mirrors
+  int n_spans = 0;
+  bool recount = false;             // a range copy rewrote identity rows: the occupancy is counted again
+  size_t stage_end = 0;             // the staging buffer is free from here on
 };
+
+// Host only: resolves the segments of `tables` (bit t set = lwse_table t; a tick applies the placement request
+// patches on the side stream, where the round that reads them runs, and the rest on the engine's stream) to
+// device pointers.  Segments outside the arena are copied into the staging buffer from `stage_base` on (the
+// caller reserved the room).  Nothing is enqueued.
+static int plan_scatter(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, uint32_t tables, size_t stage_base,
+                        size_t dma_min_bytes, ScatterPlan* plan) {
+  *plan = ScatterPlan{};
+  lwse::ScatterSegHost* sc = plan->sc;
+  size_t cursor = stage_base, total = 0;
+  for (uint32_t i = 0; i < n_segs; i++) {
+    const lwse_patch_seg& g = segs[i];
+    if (g.n == 0 || !((tables >> g.table) & 1u)) continue;
+    void* base;
+    uint64_t rows;
+    uint32_t rb;
+    if (!resident_table(e, g.table, &base, &rows, &rb)) continue;  // (summarize_segments turns such a segment away)
+    if (g.flags & LWSE_PATCH_RANGE) {
+      plan->ranges[plan->n_ranges++] = {static_cast<uint8_t*>(base) + (size_t)g.first_row * rb, g.values, (size_t)g.n * rb};
+      if (g.table == LWSE_TABLE_POD_IDENT) plan->recount = true;
+      continue;
+    }
+    const void* src[2] = {g.rows, g.values};
+    const size_t bytes[2] = {(size_t)g.n * 4, (size_t)g.n * rb};
+    const bool in_place[2] = {rows_in_place(e, g), values_in_place(e, g, rb)};
+    const void* dev[2];
+    for (int c = 0; c < 2; c++) {
+      if (in_place[c]) {
+        dev[c] = e->arena.dev_of(static_cast<const uint8_t*>(src[c]));
+        continue;
+      }
+      if (cursor + bytes[c] > e->stage.cap) return LWSE_ERR_OOM;
+      memcpy(static_cast<uint8_t*>(e->stage.h) + cursor, src[c], bytes[c]);
+      dev[c] = static_cast<uint8_t*>(e->stage.d) + cursor;
+      cursor += align256(bytes[c]);
+    }
+    sc[plan->n++] = lwse::ScatterSegHost{base, rows, static_cast<const uint32_t*>(dev[0]), dev[1], g.n, rb, g.table == LWSE_TABLE_POD_IDENT};
+    total += bytes[0] + bytes[1];
+  }
+  plan->stage_end = cursor;
+  // Few patch bytes: the scatter kernel reads them in place over PCIe (one round trip, no copy
+  // launch).  Many: one DMA copy per pinned buffer of the span this plan uses, then the kernel
+  // reads device memory — the copy engine moves large spans several times faster than SM reads of host memory.
+  constexpr size_t kDmaBytes = 16384;
+  if (plan->n == 0 || total < (dma_min_bytes > kDmaBytes ? dma_min_bytes : kDmaBytes)) return LWSE_OK;
+  struct Span { const PinBuf* pin; DevBuf* mirror; uintptr_t lo, hi; } spans[2] = {
+      {&e->arena, &e->arena_mirror, UINTPTR_MAX, 0}, {&e->stage, &e->stage_mirror, UINTPTR_MAX, 0}};
+  auto touch = [&](const void* dptr, size_t bytes) {
+    for (Span& sp : spans) {
+      const uintptr_t d0 = reinterpret_cast<uintptr_t>(sp.pin->d), a = reinterpret_cast<uintptr_t>(dptr);
+      if (sp.pin->d && a >= d0 && a + bytes <= d0 + sp.pin->cap) {
+        sp.lo = a - d0 < sp.lo ? a - d0 : sp.lo;
+        sp.hi = a - d0 + bytes > sp.hi ? a - d0 + bytes : sp.hi;
+      }
+    }
+  };
+  for (int k = 0; k < plan->n; k++) {
+    touch(sc[k].rows, (size_t)sc[k].n * 4);
+    touch(sc[k].values, (size_t)sc[k].n * sc[k].row_bytes);
+  }
+  for (Span& sp : spans) {
+    if (sp.hi <= sp.lo) continue;
+    if (sp.mirror->cap < sp.pin->cap) {  // (first use, or the pinned buffer grew)
+      LWSE_CUDA(e, cudaStreamSynchronize(e->stream));
+      LWSE_CUDA(e, cudaStreamSynchronize(e->side_stream));
+      LWSE_CUDA(e, cudaStreamSynchronize(e->copy_stream));
+      LWSE_CUDA(e, sp.mirror->reserve(sp.pin->cap));
+    }
+    plan->spans[plan->n_spans++] = {static_cast<uint8_t*>(sp.mirror->p) + sp.lo, static_cast<const uint8_t*>(sp.pin->h) + sp.lo, sp.hi - sp.lo};
+    const uintptr_t d0 = reinterpret_cast<uintptr_t>(sp.pin->d), m0 = reinterpret_cast<uintptr_t>(sp.mirror->p);
+    for (int k = 0; k < plan->n; k++) {
+      uintptr_t a = reinterpret_cast<uintptr_t>(sc[k].rows);
+      if (a >= d0 && a < d0 + sp.pin->cap) sc[k].rows = reinterpret_cast<const uint32_t*>(m0 + (a - d0));
+      a = reinterpret_cast<uintptr_t>(sc[k].values);
+      if (a >= d0 && a < d0 + sp.pin->cap) sc[k].values = reinterpret_cast<const void*>(m0 + (a - d0));
+    }
+  }
+  return LWSE_OK;
+}
+
+// The copies of a plan, on `s`: the range segments in segment order, then the mirrored spans.  The scatter
+// kernel (launch_scatter_plan, or a tick graph's first node) goes behind all of them.
+static int enqueue_scatter_copies(lwse_engine* e, const ScatterPlan& p, cudaStream_t s) {
+  for (int k = 0; k < p.n_ranges; k++)
+    LWSE_CUDA(e, cudaMemcpyAsync(p.ranges[k].dst, p.ranges[k].src, p.ranges[k].bytes, cudaMemcpyHostToDevice, s));
+  for (int k = 0; k < p.n_spans; k++)
+    LWSE_CUDA(e, cudaMemcpyAsync(p.spans[k].dst, p.spans[k].src, p.spans[k].bytes, cudaMemcpyHostToDevice, s));
+  return LWSE_OK;
+}
 
 static int launch_scatter_plan(lwse_engine* e, const ScatterPlan& p, cudaStream_t s) {
   int cuda_err = 0;
@@ -865,166 +1032,6 @@ static int launch_scatter_plan(lwse_engine* e, const ScatterPlan& p, cudaStream_
     if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
   return LWSE_OK;
-}
-
-static int apply_patches_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, bool* wrote,
-                                uint32_t tables = 0xFFFFFFFFu, cudaStream_t s = nullptr, size_t stage_base = 0,
-                                size_t* stage_used = nullptr, long dma_min_bytes = 0, ScatterPlan* defer = nullptr,
-                                bool plan_only = false) {
-  *wrote = false;
-  if (stage_used) *stage_used = stage_base;
-  if (n_segs == 0) return LWSE_OK;
-  if (!segs || n_segs > LWSE_TICK_MAX_SEGS) return LWSE_ERR_INVALID_ARG;
-  if (!s) s = e->stream;
-  // room for every segment that is not in the arena
-  size_t need = 0;
-  for (uint32_t i = 0; i < n_segs; i++) {
-    void* base;
-    uint64_t rows;
-    uint32_t rb;
-    if (!resident_table(e, segs[i].table, &base, &rows, &rb)) return LWSE_ERR_INVALID_ARG;
-    if (segs[i].n == 0 || !((tables >> segs[i].table) & 1u)) continue;
-    if (!segs[i].values || (!(segs[i].flags & LWSE_PATCH_RANGE) && !segs[i].rows)) return LWSE_ERR_INVALID_ARG;
-    if (segs[i].flags & LWSE_PATCH_RANGE) {
-      if ((uint64_t)segs[i].first_row + segs[i].n > rows) return LWSE_ERR_BAD_TABLE;
-      continue;
-    }
-    if (!rows_in_place(e, segs[i])) need += align256((size_t)segs[i].n * 4);
-    if (!values_in_place(e, segs[i], rb)) need += align256((size_t)segs[i].n * rb);
-  }
-  if (stage_base + need > e->stage.cap) {
-    if (stage_base) return LWSE_ERR_OOM;  // (the tick sizes the buffer for both of its calls up front)
-    LWSE_CUDA(e, cudaStreamSynchronize(e->stream));
-    LWSE_CUDA(e, cudaStreamSynchronize(e->side_stream));
-    LWSE_CUDA(e, e->stage.reserve(need));
-  }
-  ScatterPlan plan;
-  lwse::ScatterSegHost* sc = plan.sc;
-  int n_sc = 0;
-  size_t cursor = stage_base;
-  bool recount = false;
-  for (uint32_t i = 0; i < n_segs; i++) {
-    const lwse_patch_seg& g = segs[i];
-    if (g.n == 0 || !((tables >> g.table) & 1u)) continue;
-    void* base;
-    uint64_t rows;
-    uint32_t rb;
-    resident_table(e, g.table, &base, &rows, &rb);
-    *wrote = true;
-    if (g.table == LWSE_TABLE_PLACE_REQS) {
-      // a request that moves to another namespace breaks the grouping the fast placement kernels rely on,
-      // and the namespace index of an ungrouped table
-      const lwse_place_req* v = static_cast<const lwse_place_req*>(g.values);
-      for (uint32_t k = 0; k < g.n; k++) {
-        const uint32_t row = (g.flags & LWSE_PATCH_RANGE) ? g.first_row + k : g.rows[k];
-        if (row < e->rn_reqs && v[k].ns != e->r_req_ns[row]) {
-          e->r_req_ns[row] = v[k].ns;
-          e->r_place_grouped = false;
-          e->r_ns_index_ok = false;
-        }
-      }
-    }
-    if (g.flags & LWSE_PATCH_RANGE) {  // one DMA copy straight into the table
-      if (plan_only) {
-        plan.eager_only = true;
-        continue;
-      }
-      LWSE_CUDA(e, cudaMemcpyAsync(static_cast<uint8_t*>(base) + (size_t)g.first_row * rb, g.values, (size_t)g.n * rb,
-                                   cudaMemcpyHostToDevice, s));
-      if (g.table == LWSE_TABLE_POD_IDENT) recount = true;
-      continue;
-    }
-    const uint32_t* d_rows;
-    const void* d_vals;
-    if (rows_in_place(e, g)) {
-      d_rows = e->arena.dev_of(g.rows);
-    } else {
-      if (plan_only) plan.eager_only = true;
-      uint8_t* dst = static_cast<uint8_t*>(e->stage.h) + cursor;
-      memcpy(dst, g.rows, (size_t)g.n * 4);
-      d_rows = reinterpret_cast<const uint32_t*>(static_cast<uint8_t*>(e->stage.d) + cursor);
-      cursor += align256((size_t)g.n * 4);
-    }
-    if (values_in_place(e, g, rb)) {
-      d_vals = e->arena.dev_of(static_cast<const uint8_t*>(g.values));
-    } else {
-      if (plan_only) plan.eager_only = true;
-      uint8_t* dst = static_cast<uint8_t*>(e->stage.h) + cursor;
-      memcpy(dst, g.values, (size_t)g.n * rb);
-      d_vals = static_cast<uint8_t*>(e->stage.d) + cursor;
-      cursor += align256((size_t)g.n * rb);
-    }
-    sc[n_sc++] = lwse::ScatterSegHost{base, rows, d_rows, d_vals, g.n, rb, g.table == LWSE_TABLE_POD_IDENT};
-  }
-  if (n_sc) {
-    // Few patch bytes: the scatter kernel reads them in place over PCIe (one round trip, no copy
-    // launch).  Many: one DMA copy per pinned buffer of the span this call uses, then the kernel
-    // reads device memory — the copy engine moves large spans several times faster than SM reads of host memory.
-    constexpr long kDmaBytes = 16384;
-    size_t total = 0;
-    for (int k = 0; k < n_sc; k++) total += (size_t)sc[k].n * (4u + sc[k].row_bytes);
-    if (total >= (size_t)(dma_min_bytes > kDmaBytes ? dma_min_bytes : kDmaBytes)) {
-      struct Span { const PinBuf* pin; DevBuf* mirror; uintptr_t lo, hi; } spans[2] = {
-          {&e->arena, &e->arena_mirror, UINTPTR_MAX, 0}, {&e->stage, &e->stage_mirror, UINTPTR_MAX, 0}};
-      auto touch = [&](const void* dptr, size_t bytes) {
-        for (Span& sp : spans) {
-          const uintptr_t d0 = reinterpret_cast<uintptr_t>(sp.pin->d), a = reinterpret_cast<uintptr_t>(dptr);
-          if (sp.pin->d && a >= d0 && a + bytes <= d0 + sp.pin->cap) {
-            sp.lo = a - d0 < sp.lo ? a - d0 : sp.lo;
-            sp.hi = a - d0 + bytes > sp.hi ? a - d0 + bytes : sp.hi;
-          }
-        }
-      };
-      for (int k = 0; k < n_sc; k++) {
-        touch(sc[k].rows, (size_t)sc[k].n * 4);
-        touch(sc[k].values, (size_t)sc[k].n * sc[k].row_bytes);
-      }
-      for (Span& sp : spans) {
-        if (sp.hi <= sp.lo) continue;
-        if (sp.mirror->cap < sp.pin->cap) {  // (first use, or the pinned buffer grew)
-          LWSE_CUDA(e, cudaStreamSynchronize(e->stream));
-          LWSE_CUDA(e, cudaStreamSynchronize(e->side_stream));
-          LWSE_CUDA(e, cudaStreamSynchronize(e->copy_stream));
-          LWSE_CUDA(e, sp.mirror->reserve(sp.pin->cap));
-        }
-        if (plan_only) {
-          if (sp.pin == &e->stage) {
-            plan.eager_only = true;
-          } else {
-            plan.dma = true;
-            plan.lo = sp.lo;
-            plan.hi = sp.hi;
-          }
-        } else {
-          LWSE_CUDA(e, cudaMemcpyAsync(static_cast<uint8_t*>(sp.mirror->p) + sp.lo, static_cast<const uint8_t*>(sp.pin->h) + sp.lo,
-                                       sp.hi - sp.lo, cudaMemcpyHostToDevice, s));
-        }
-        const uintptr_t d0 = reinterpret_cast<uintptr_t>(sp.pin->d), m0 = reinterpret_cast<uintptr_t>(sp.mirror->p);
-        for (int k = 0; k < n_sc; k++) {
-          uintptr_t a = reinterpret_cast<uintptr_t>(sc[k].rows);
-          if (a >= d0 && a < d0 + sp.pin->cap) sc[k].rows = reinterpret_cast<const uint32_t*>(m0 + (a - d0));
-          a = reinterpret_cast<uintptr_t>(sc[k].values);
-          if (a >= d0 && a < d0 + sp.pin->cap) sc[k].values = reinterpret_cast<const void*>(m0 + (a - d0));
-        }
-      }
-    }
-  }
-  plan.n = n_sc;
-  plan.recount = recount;
-  if (stage_used) *stage_used = cursor;
-  if (defer) {
-    *defer = plan;
-    return LWSE_OK;
-  }
-  return launch_scatter_plan(e, plan, s);
-}
-
-// bytes of staging the segments of a tick need in the worst case (nothing in the arena)
-static size_t stage_bytes_upper_bound(const lwse_patch_seg* segs, uint32_t n_segs) {
-  size_t need = 0;
-  for (uint32_t i = 0; i < n_segs; i++)
-    if (segs && !(segs[i].flags & LWSE_PATCH_RANGE)) need += align256((size_t)segs[i].n * 4) + align256((size_t)segs[i].n * 64);
-  return need;
 }
 
 LWSE_API int lwse_resident_patch(lwse_engine* e, lwse_table which, const uint32_t* rows, const void* values,
@@ -1044,18 +1051,17 @@ LWSE_API int lwse_resident_patch(lwse_engine* e, lwse_table which, const uint32_
   seg.n = n;
   seg.rows = rows;
   seg.values = values;
-  if (which == LWSE_TABLE_NODES) {
-    // the round of the last placement call may still read the rows (and it reads them on another stream)
-    if (e->place_pending) LWSE_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_place, 0));
-    const int nrc = node_patches_locked(e, &seg, 1);
-    if (nrc < 0) return nrc;
-  }
-  if (which == LWSE_TABLE_LWS) e->r_swept = false;  // r_lws_out no longer belongs to these LWS rows
-  if (which <= LWSE_TABLE_POD_IDENT) e->r_groups_swept = false;  // nor r_group_out to the group and pod rows
-  if (which == LWSE_TABLE_NODES || which == LWSE_TABLE_PLACE_REQS || which == LWSE_TABLE_POD_IDENT)
-    e->r_place_current = false;  // nor r_pout to the rows a round reads
-  bool wrote = false;
-  const int rc = apply_patches_locked(e, &seg, 1, &wrote);
+  SegSummary ss;
+  if (const int crc = summarize_segments(e, &seg, 1, &ss); crc != LWSE_OK) return crc;
+  // the round of the last placement call may still read the node rows (and it reads them on another stream)
+  if (which == LWSE_TABLE_NODES && e->place_pending) LWSE_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_place, 0));
+  commit_segments(e, &seg, 1, ss);
+  mark_outputs_stale(e, ss.tables, false, false);
+  ScatterPlan plan;
+  int rc = reserve_stage(e, ss.stage_bytes);
+  if (rc == LWSE_OK) rc = plan_scatter(e, &seg, 1, ss.tables, 0, 0, &plan);
+  if (rc == LWSE_OK) rc = enqueue_scatter_copies(e, plan, e->stream);
+  if (rc == LWSE_OK) rc = launch_scatter_plan(e, plan, e->stream);
   if (rc != LWSE_OK) {
     if (which == LWSE_TABLE_NODES) e->node_index_stale = true;  // (see tick_submit_locked)
     return rc;
@@ -1606,29 +1612,401 @@ static inline uint8_t* d_desc_of(lwse_engine* e, uint32_t slot) {
   return static_cast<uint8_t*>(e->tdesc_dev.p) + slot * lwse::kScatterDescBytes;
 }
 
-// The checks apply_patches_locked makes on a tick's segments, all of them before anything (the node-table
-// mirror included) changes.
-static int check_segments(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs) {
-  if (n_segs == 0) return LWSE_OK;
-  if (!segs || n_segs > LWSE_TICK_MAX_SEGS) return LWSE_ERR_INVALID_ARG;
-  for (uint32_t i = 0; i < n_segs; i++) {
-    const lwse_patch_seg& g = segs[i];
-    void* base;
-    uint64_t rows;
-    uint32_t rb;
-    if (!resident_table(e, g.table, &base, &rows, &rb)) return LWSE_ERR_INVALID_ARG;
-    if (g.n == 0) continue;
-    if (!g.values || (!(g.flags & LWSE_PATCH_RANGE) && !g.rows)) return LWSE_ERR_INVALID_ARG;
-    if ((g.flags & LWSE_PATCH_RANGE) && (uint64_t)g.first_row + g.n > rows) return LWSE_ERR_BAD_TABLE;
+// The patches of a tick go where their readers run: the placement request table is read only by the round
+// on the side stream, everything else by the sweep on the engine's stream.
+constexpr uint32_t kSideTables = 1u << LWSE_TABLE_PLACE_REQS;
+
+// Every decision of one tick, made by plan_tick before anything is enqueued.  The enqueue functions, the
+// graph key, lwse_tick_info and the slot's bookkeeping all read it and nothing else.
+struct TickPlan {
+  uint32_t slot = 0;         // t_submitted & 1: which pinned lists, words and counters the tick uses
+  bool in_flight = false;    // the previous tick has not been waited for yet
+  bool do_sweep = false, do_place = false;
+  bool round_asked = false;  // LWSE_TICK_PLACE on a loaded request table: r_pout is current afterwards (trivially so for an empty table)
+  uint32_t sweep_flags = 0;  // LWSE_SWEEP_GANG
+  // The round's form.  A request table grouped by namespace — and not ungrouped by this tick's patches — runs
+  // the namespace kernels as they are; any other table runs them through the namespace index, rebuilt when the
+  // namespace column changed since the last build.  The general form only where the namespace form cannot run.
+  bool ns_form = false, scan_form = false, indexed = false;
+  lwse::PlaceNsIndex ns_index = lwse::kNsIndexNone;
+  bool shared_occ = false, lagged = false;  // LWSE_TICK_SHARED_OCCUPANCY (and its LWSE_EXCHANGE_LAGGED)
+  bool has_patches = false, has_ident = false, has_side = false;
+  bool wrote_main = false;   // a table is patched on the engine's stream
+  uint32_t node_rows = 0;
+  bool node_rebuild = false;  // the round rebuilds the node index (a tick without a round leaves a stale index to the next one)
+  // A round forks behind the engine's stream when it reads what the main scatter writes — identity-row patches
+  // move occupancy counts, node-row patches change the nodes — or when an earlier tick without a round patched
+  // tables there that no round has been ordered behind yet.
+  bool prior_unforked = false, fork_behind_main = false;
+  // LWSE_TICK_GRAPH: 1 = replay when the previous tick is still in flight — the pipelined use, where the host's
+  // enqueue time is what limits the rate; a lone tick is faster kernel by kernel, because its round starts
+  // while the copy engine still moves the pod patches; 2 = always; 0 = never.  Only ticks whose patches all lie
+  // in the arena, and whose round takes the namespace form, are replayed.
+  bool graph_ok = false;
+};
+
+static TickPlan plan_tick(const lwse_engine* e, const SegSummary& ss, uint32_t flags) {
+  TickPlan p;
+  p.slot = (uint32_t)(e->t_submitted & 1u);
+  p.in_flight = e->t_submitted != e->t_waited;
+  p.round_asked = (flags & LWSE_TICK_PLACE) && e->r_place_loaded;
+  p.do_place = p.round_asked && e->rn_reqs > 0;
+  p.do_sweep = !(flags & LWSE_TICK_NO_SWEEP) && (e->rn_lws || e->rn_groups);
+  p.sweep_flags = flags & LWSE_SWEEP_GANG;
+  p.ns_form = p.do_place && lwse::place_ns_supported(e->n_nodes, e->n_domains);
+  p.scan_form = (flags & LWSE_SWEEP_PLACE_SCAN) != 0;
+  p.indexed = p.ns_form && !(e->r_place_grouped && !ss.ns_moves);
+  p.ns_index = !p.indexed                             ? lwse::kNsIndexNone
+               : (ss.ns_moves || !e->r_ns_index_ok) ? lwse::kNsIndexBuild
+                                                      : lwse::kNsIndexReuse;
+  p.shared_occ = (flags & LWSE_TICK_SHARED_OCCUPANCY) != 0;
+  p.lagged = p.shared_occ && (flags & LWSE_EXCHANGE_LAGGED);
+  p.has_patches = ss.tables != 0;
+  p.has_ident = (ss.tables & (1u << LWSE_TABLE_POD_IDENT)) != 0;
+  p.has_side = (ss.tables & kSideTables) != 0;
+  p.wrote_main = (ss.tables & ~kSideTables) != 0;
+  p.node_rows = ss.node_rows;
+  p.node_rebuild = p.do_place && (e->node_index_stale || ss.node_moves);
+  p.prior_unforked = p.do_place && e->main_unforked;
+  p.fork_behind_main = p.has_ident || p.node_rows > 0 || p.prior_unforked;
+  p.graph_ok = (e->use_graph >= 2 || (e->use_graph == 1 && p.in_flight)) && ss.all_in_place && !ss.any_range &&
+               (!p.shared_occ || (p.do_place && e->xch_connected)) && (p.do_sweep || p.do_place) &&
+               !(p.has_side && !p.do_place) && (!p.do_place || p.ns_form);
+  return p;
+}
+
+// One graph per shape of the tick and slot: every decision that changes what a replayable tick enqueues has
+// its bit here.  (has_ident, has_side and the forks do not: a graph's one scatter takes every table, and its
+// round always forks behind it.)
+static uint32_t graph_key(const TickPlan& p) {
+  enum { kPatches, kSweep, kPlace, kGang, kScan, kSlot, kSharedOcc, kLagged, kIndexed, kIndexBuild, kNodeRows, kNodeRebuild };
+  auto bit = [](bool on, int at) { return (on ? 1u : 0u) << at; };
+  return bit(p.has_patches, kPatches) | bit(p.do_sweep, kSweep) | bit(p.do_place, kPlace) | bit(p.sweep_flags != 0, kGang) |
+         bit(p.scan_form, kScan) | bit(p.slot != 0, kSlot) | bit(p.shared_occ, kSharedOcc) | bit(p.lagged, kLagged) |
+         bit(p.indexed, kIndexed) | bit(p.ns_index == lwse::kNsIndexBuild, kIndexBuild) | bit(p.node_rows > 0, kNodeRows) |
+         bit(p.node_rebuild, kNodeRebuild);
+}
+
+static lwse_tick_info tick_info(const TickPlan& p, bool graph) {
+  lwse_tick_info ti{};
+  ti.place_form = !p.do_place   ? LWSE_TICK_FORM_NONE
+                  : !p.ns_form  ? LWSE_TICK_FORM_GENERAL
+                  : p.scan_form ? LWSE_TICK_FORM_SCAN
+                                : LWSE_TICK_FORM_NAMESPACE;
+  ti.indexed = p.indexed ? 1u : 0u;
+  ti.index_built = p.ns_index == lwse::kNsIndexBuild ? 1u : 0u;
+  ti.graph = graph ? 1u : 0u;
+  return ti;
+}
+
+// The bookkeeping that closes a submitted tick.
+static void close_submit(lwse_engine* e, const TickPlan& p, uint32_t seq, bool graph) {
+  lwse_engine::TickSlot& ts = e->tslot[p.slot];
+  ts.seq = seq;
+  ts.do_sweep = p.do_sweep;
+  ts.do_place = p.do_place;
+  ts.published = p.do_sweep || p.do_place;
+  ts.wrote = p.has_patches;
+  e->t_submitted++;
+  if (p.do_sweep) {
+    e->r_swept = e->r_groups_swept = true;
+    e->r_sweep_flags = p.sweep_flags;
+  }
+  if (p.round_asked) e->r_place_current = true;
+  e->main_unforked = !p.do_place && (e->main_unforked || p.wrote_main);
+  e->last_tick_info = tick_info(p, graph);
+  if (p.indexed) e->r_ns_index_ok = true;  // (also after a replay, which enqueues no call that would say so)
+}
+
+// One tick slot's buffers: its words in pinned memory, its pinned change lists (both as the device sees them),
+// the device-memory lists the kernels append to, and their counters.
+struct SlotBufs {
+  uint32_t* words;
+  uint8_t *chg_pinned, *chg_dev;
+  uint32_t* counts;
+};
+static SlotBufs slot_bufs(const lwse_engine* e, uint32_t slot) {
+  return {static_cast<uint32_t*>(e->tickw.d) + slot * 16u, static_cast<uint8_t*>(e->chg.d) + slot * e->chg_bytes,
+          static_cast<uint8_t*>(e->chg_dev.p) + slot * e->chg_bytes, static_cast<uint32_t*>(e->r_counts.p) + slot * 16u};
+}
+
+// `first_mode`: how the sweep's first kernel is launched (see launch_lws_sweep): 2 behind this tick's scatter
+// kernel alone (programmatic: it waits at its top), 1 eager with nothing to wait for, 0 behind an event or as a
+// graph's first node (ordinary).
+static int enqueue_sweep(lwse_engine* e, const TickPlan& p, int first_mode) {
+  const SlotBufs b = slot_bufs(e, p.slot);
+  lwse_lws_tables d{};
+  d.lws = (const lwse_lws_rec*)e->r_lws.p;
+  d.n_lws = e->rn_lws;
+  d.groups = (const lwse_group_rec*)e->r_groups.p;
+  d.n_groups = e->rn_groups;
+  d.pod_state = (const lwse_pod_state*)e->r_pst.p;
+  d.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
+  d.n_pods = e->rn_pods;
+  d.lws_out = (lwse_lws_out*)e->r_lws_out.p;
+  d.group_out = (lwse_group_out*)e->r_group_out.p;
+  d.flags = p.sweep_flags;
+  lwse::SweepChangeLists cl;
+  cl.lws_rows = reinterpret_cast<uint32_t*>(b.chg_dev + e->chg_off[0]);
+  cl.lws_out = reinterpret_cast<lwse_lws_out*>(b.chg_dev + e->chg_off[1]);
+  cl.lws_capacity = e->rn_lws;
+  cl.group_rows = reinterpret_cast<uint32_t*>(b.chg_dev + e->chg_off[2]);
+  cl.group_out = reinterpret_cast<lwse_group_out*>(b.chg_dev + e->chg_off[3]);
+  cl.group_capacity = e->rn_groups;
+  cl.counts = b.counts;
+  int cuda_err = 0;
+  const int launched = lwse::launch_lws_sweep(&d, (const lwse_node_rec*)e->nodes.p, e->n_nodes, e->r_scan.p, e->sm_count,
+                                              e->stream, &cuda_err, &cl, nullptr, first_mode);
+  return count_launch(e, launched, cuda_err);
+}
+
+// How the round's first kernels are launched.  Eagerly the first one follows a kernel on the side stream; in a
+// graph capture it follows an event (an ordinary launch), and `mid_event` is recorded between the condense and
+// the namespace kernel.
+struct PlaceLaunch {
+  bool first_pdl;
+  void* mid_event;
+};
+
+static int enqueue_place(lwse_engine* e, const TickPlan& p, const PlaceLaunch& how, TickPlaceResult* res) {
+  const SlotBufs b = slot_bufs(e, p.slot);
+  cudaStream_t ps = e->side_stream;
+  const uint32_t form = !p.ns_form ? kFormGeneral : p.scan_form ? kFormScan : kFormGrouped;
+  // the namespace kernels append the changed rows themselves; the general form gets a diff kernel
+  const lwse::PlaceNsChanges changes{(lwse_place_out*)e->r_pout_prev.p, reinterpret_cast<uint32_t*>(b.chg_dev + e->chg_off[4]),
+                                     reinterpret_cast<lwse_place_out*>(b.chg_dev + e->chg_off[5]), b.counts + 4, e->rn_reqs,
+                                     (int)p.slot, how.mid_event};
+  bool diffed = false;
+  int rc;
+  if (p.shared_occ) {  // multi-rank: this rank's counters go to the peers, the round sees the sum
+    if (!e->xch_connected) return LWSE_ERR_NOT_READY;
+    rc = shared_occupancy_place_locked(e, (const lwse_place_req*)e->r_preq.p, e->rn_reqs, (const uint32_t*)e->r_occ.p,
+                                       e->rn_namespaces, (lwse_place_out*)e->r_pout.p, form, p.lagged, ps, &changes, p.ns_index);
+    diffed = rc == LWSE_OK;
+  } else {
+    rc = place_locked(e, (const lwse_place_req*)e->r_preq.p, e->rn_reqs, (const uint32_t*)e->r_occ.p, e->rn_namespaces,
+                      (lwse_place_out*)e->r_pout.p, nullptr, ps, 1, e->rn_reqs, 0, false, form, how.first_pdl, &changes, &diffed,
+                      p.ns_index);
+  }
+  if (rc != LWSE_OK) return rc;
+  if (!diffed) {
+    int cuda_err = 0;
+    const int launched = lwse::launch_place_diff((const lwse_place_out*)e->r_pout.p, changes.prev, e->rn_reqs, changes.rows,
+                                                 changes.outs, changes.capacity, changes.count, ps, &cuda_err);
+    if (const int drc = count_launch(e, launched, cuda_err); drc != LWSE_OK) return drc;
+  }
+  *res = TickPlaceResult{diffed, e->place_rounds_ptr};
+  return LWSE_OK;
+}
+
+// The tick's last step, on the publish stream: behind everything the tick enqueued on the engine's
+// stream (both branches joined there), so the NEXT tick's kernels do not wait for the copy of this
+// tick's changed rows to the host.  ONE kernel copies all change lists out (0 LWS rows, 1 group rows,
+// 2 placement rows); lists, counters and the round's counter block are per slot.
+static int enqueue_publish(lwse_engine* e, const TickPlan& p, uint32_t seq, const TickPlaceResult& placed) {
+  const SlotBufs b = slot_bufs(e, p.slot);
+  const uint32_t capacity[3] = {e->rn_lws, e->rn_groups, e->rn_reqs};
+  const uint32_t out_bytes[3] = {sizeof(lwse_lws_out), sizeof(lwse_group_out), sizeof(lwse_place_out)};
+  lwse::PublishListHost pl[3] = {};
+  for (int k = 0; k < 3; k++)
+    if (k == 2 ? p.do_place : p.do_sweep)
+      pl[k] = {reinterpret_cast<uint32_t*>(b.chg_dev + e->chg_off[2 * k]), b.chg_dev + e->chg_off[2 * k + 1],
+               reinterpret_cast<uint32_t*>(b.chg_pinned + e->chg_off[2 * k]), b.chg_pinned + e->chg_off[2 * k + 1],
+               b.counts + (k == 2 ? 4 : k), capacity[k], out_bytes[k]};
+  LWSE_CUDA(e, cudaEventRecord(e->ev_done, e->stream));
+  LWSE_CUDA(e, cudaStreamWaitEvent(e->pub_stream, e->ev_done, 0));
+  const uint32_t* rounds = p.do_place ? placed.rounds_ptr : nullptr;
+  int cuda_err = 0;
+  const int launched = lwse::launch_publish(pl, rounds, b.words, 4, seq, b.counts + 2, e->last_changed[0] + e->last_changed[1],
+                                            e->pub_stream, &cuda_err,
+                                            p.do_place && placed.place_ns ? const_cast<uint32_t*>(rounds) : nullptr, 8u, /*pdl=*/false);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaEventRecord(e->ev_pub, e->pub_stream));
+  return LWSE_OK;
+}
+
+// The graph of plan `p`, captured from the same enqueue functions on capturing streams:
+//   scatter (from the slot's descriptor block) -> condense -> { fused -> LWS pass  ||  namespace kernel }.
+// Returns an error only when the streams could not be drained; a capture that fails leaves tg.exec null and
+// the key eager for good (the streams are usable again after EndCapture).
+static int capture_tick_graph(lwse_engine* e, const TickPlan& p, lwse_engine::TickGraph& tg) {
+  cudaStream_t s = e->stream, ps = e->side_stream;
+  cudaError_t ce = cudaStreamSynchronize(s);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(ps);
+  if (ce != cudaSuccess) return fail_cuda(e, ce);
+  const uint64_t launches_before = e->launches;
+  int crc = LWSE_OK;
+  TickPlaceResult placed;
+  ce = cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed);
+  if (ce == cudaSuccess) {
+    auto cap = [&](cudaError_t x) { if (crc == LWSE_OK && x != cudaSuccess) { ce = x; crc = LWSE_ERR_CUDA; } };
+    if (p.has_patches) {  // the graph's first node: an ordinary launch
+      int err = 0;
+      const int launched = lwse::launch_scatter_desc(d_desc_of(e, p.slot), e->sm_count, s, /*pdl=*/false, &err);
+      if (launched < 0) cap((cudaError_t)err); else e->launches += (uint64_t)launched;
+    }
+    if (p.do_place) {  // the round forks behind the scatter (it reads the request rows and the occupancy counters)
+      cap(cudaEventRecord(e->ev_fork, s));
+      cap(cudaStreamWaitEvent(ps, e->ev_fork, 0));
+      // The fused sweep kernel fills every SM (3 CTAs of 256 x 77 registers) the moment it starts
+      // and the namespace kernel's CTAs (512 x 53 registers) then wait for CTAs to retire: hold
+      // the sweep back until the (short) condense kernel is done, so that both reach the SMs together.
+      if (crc == LWSE_OK) crc = enqueue_place(e, p, PlaceLaunch{false, p.do_sweep ? (void*)e->ev_mid : nullptr}, &placed);
+      if (p.do_sweep && placed.place_ns) cap(cudaStreamWaitEvent(s, e->ev_mid, 0));
+    }
+    if (crc == LWSE_OK && p.do_sweep) crc = enqueue_sweep(e, p, (p.has_patches && !placed.place_ns) ? 2 : 0);
+    if (p.do_place) {
+      cap(cudaEventRecord(e->ev_join, ps));
+      cap(cudaStreamWaitEvent(s, e->ev_join, 0));
+    }
+    cudaGraph_t graph = nullptr;
+    const cudaError_t ee = cudaStreamEndCapture(s, &graph);
+    if (ee != cudaSuccess || graph == nullptr) cap(ee != cudaSuccess ? ee : cudaErrorUnknown);
+    if (crc == LWSE_OK) cap(cudaGraphInstantiate(&tg.exec, graph, 0));
+    if (graph) cudaGraphDestroy(graph);
+  } else {
+    crc = LWSE_ERR_CUDA;
+  }
+  tg.kernels = (uint32_t)(e->launches - launches_before);
+  e->launches = launches_before;
+  if (crc != LWSE_OK || !tg.exec) {
+    (void)cudaGetLastError();
+    if (tg.exec) cudaGraphExecDestroy(tg.exec);
+    tg.exec = nullptr;
+    tg.failed = true;
+    e->node_index_stale = e->node_index_stale || p.node_rebuild;  // (the eager run builds it)
+  } else {
+    tg.place = placed;
   }
   return LWSE_OK;
 }
 
-static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, uint32_t flags);
+// Enqueueing a tick kernel by kernel costs ~10 runtime calls of microseconds each (launches with
+// attributes and 200-400 bytes of parameters): more host time than the GPU needs for the tick.
+// A tick whose plan allows it (graph_ok) is therefore replayed as ONE graph per key, from the second tick
+// of that key on: the first runs eagerly, so that every buffer settles.
+// What changes from tick to tick travels outside the graph, on the copy stream, so that the
+// copies of tick k+1 overlap the kernels of tick k: the patch bytes (arena span -> mirror, one scatter for
+// every table behind one copy) and the scatter's segment descriptors (a 512-byte block, pinned slot ->
+// device).  The publish kernel follows on the publish stream, launched with the tick's sequence number.
+// *done: the tick was enqueued; otherwise the caller enqueues it eagerly.
+static int replay_tick(lwse_engine* e, const TickPlan& p, const lwse_patch_seg* segs, uint32_t n_segs, uint32_t seq, bool* done) {
+  *done = false;
+  lwse_engine::TickGraph& tg = e->tick_graphs[graph_key(p)];
+  if (tg.seen++ == 0 || tg.failed) return LWSE_OK;
+  ScatterPlan gp;
+  if (const int rc = plan_scatter(e, segs, n_segs, 0xFFFFFFFFu, 0, 0, &gp); rc != LWSE_OK) return rc;
+  const size_t desc_bytes = lwse::kScatterDescBytes;
+  if (e->tdesc.reserve(2 * desc_bytes) != cudaSuccess || e->tdesc_dev.reserve(2 * desc_bytes) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return LWSE_OK;
+  }
+  uint8_t* h_desc = static_cast<uint8_t*>(e->tdesc.h) + p.slot * desc_bytes;
+  if (p.has_patches && !lwse::write_scatter_desc(h_desc, gp.sc, gp.n, e->n_nodes ? (uint32_t*)e->r_occ.p : nullptr, e->n_nodes))
+    return LWSE_OK;
+  if (!tg.exec) {
+    if (const int rc = capture_tick_graph(e, p, tg); rc != LWSE_OK) return rc;
+    if (!tg.exec) return LWSE_OK;
+  }
+  if (p.has_patches) {
+    if (const int rc = enqueue_scatter_copies(e, gp, e->copy_stream); rc != LWSE_OK) return rc;
+    LWSE_CUDA(e, cudaMemcpyAsync(d_desc_of(e, p.slot), h_desc, desc_bytes, cudaMemcpyHostToDevice, e->copy_stream));
+    LWSE_CUDA(e, cudaEventRecord(e->ev_dma, e->copy_stream));
+    LWSE_CUDA(e, cudaStreamWaitEvent(e->stream, e->ev_dma, 0));
+  }
+  LWSE_CUDA(e, cudaGraphLaunch(tg.exec, e->stream));
+  e->launches += tg.kernels;
+  if (p.node_rebuild) e->node_index_stale = false;  // (the graph's round built it)
+  e->graph_ticks++;
+  if (p.shared_occ) e->xch_step++;  // (the replayed push kernel advanced the device counter by one)
+  if (p.do_place) e->place_rounds_ptr = tg.place.rounds_ptr;
+  if (const int rc = enqueue_publish(e, p, seq, tg.place); rc != LWSE_OK) return rc;
+  close_submit(e, p, seq, true);
+  *done = true;
+  return LWSE_OK;
+}
 
-// Enqueue one tick (nothing waits): slot = t_submitted & 1.  At most two ticks are in flight.
+// The eager enqueue order.  Every call costs microseconds of host time and the copy of the pod patches
+// heads the critical path, so that copy is enqueued first; the round's launches follow on the side
+// stream while the copy engine works — it starts behind its own few request rows (read in place over PCIe:
+// no copy-engine launch) and is mostly done when the sweep needs the SMs — then the main scatter and the
+// sweep behind the copy.  A round that forks behind the main scatter needs that scatter enqueued before it,
+// so the scatter keeps its place in front then.
+static int enqueue_tick_eager(lwse_engine* e, const TickPlan& p, const lwse_patch_seg* segs, uint32_t n_segs, uint32_t seq) {
+  cudaStream_t s = e->stream, ps = e->side_stream;
+  const bool scatter_last = !p.fork_behind_main;
+  ScatterPlan main_plan, side_plan;
+  int rc = plan_scatter(e, segs, n_segs, ~kSideTables, 0, 0, &main_plan);
+  if (rc == LWSE_OK) rc = enqueue_scatter_copies(e, main_plan, s);
+  if (rc == LWSE_OK && !scatter_last) rc = launch_scatter_plan(e, main_plan, s);
+  if (rc != LWSE_OK) return rc;
+  if (p.fork_behind_main && (p.wrote_main || p.prior_unforked) && (p.has_side || p.do_place)) {
+    LWSE_CUDA(e, cudaEventRecord(e->ev_fork, s));
+    LWSE_CUDA(e, cudaStreamWaitEvent(ps, e->ev_fork, 0));
+  }
+  if (p.has_side) {
+    rc = plan_scatter(e, segs, n_segs, kSideTables, main_plan.stage_end, /*dma_min_bytes=*/65536, &side_plan);
+    if (rc == LWSE_OK) rc = enqueue_scatter_copies(e, side_plan, ps);
+    if (rc == LWSE_OK) rc = launch_scatter_plan(e, side_plan, ps);
+  }
+  const PlaceLaunch how{/*first_pdl=*/true, /*mid_event=*/nullptr};
+  TickPlaceResult placed;
+  if (rc == LWSE_OK && p.do_place && p.wrote_main) rc = enqueue_place(e, p, how, &placed);
+  if (rc == LWSE_OK && scatter_last) rc = launch_scatter_plan(e, main_plan, s);
+  if (rc == LWSE_OK && p.do_sweep) rc = enqueue_sweep(e, p, p.wrote_main ? 2 : 1);
+  if (rc == LWSE_OK && p.do_place && !p.wrote_main) rc = enqueue_place(e, p, how, &placed);
+  if (rc != LWSE_OK) return rc;
+  if (p.do_place || p.has_side) {
+    LWSE_CUDA(e, cudaEventRecord(e->ev_join, ps));
+    LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_join, 0));
+  }
+  if (p.do_sweep || p.do_place) {
+    rc = enqueue_publish(e, p, seq, placed);
+    if (rc != LWSE_OK) return rc;
+  }
+  close_submit(e, p, seq, false);
+  return LWSE_OK;
+}
+
+// Decide one tick, then enqueue it (nothing waits): slot = t_submitted & 1.  At most two ticks are in flight.
+// Argument errors come back before anything changes.
+static int submit_tick(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, uint32_t flags) {
+  if (e->t_submitted - e->t_waited >= 2) return LWSE_ERR_NOT_READY;  // wait for the oldest tick first
+  SegSummary ss;
+  if (const int rc = summarize_segments(e, segs, n_segs, &ss); rc != LWSE_OK) return rc;
+  const TickPlan p = plan_tick(e, ss, flags);
+  mark_outputs_stale(e, ss.tables, p.do_sweep, p.round_asked);
+  commit_segments(e, segs, n_segs, ss);
+  e->last_node_info = lwse_node_info{p.node_rows, p.node_rebuild ? 1u : 0u, e->n_usable, 0u};
+  // sequence numbers count the ticks that end in a publish kernel (the device counts the same ones)
+  uint32_t seq = 0;
+  if (p.do_sweep || p.do_place) {
+    seq = ++e->tick_seq;
+    if (seq == 0) seq = ++e->tick_seq;
+  }
+  if (const int rc = reserve_stage(e, ss.stage_bytes); rc != LWSE_OK) return rc;
+  if (p.in_flight) {
+    // a tick is still running.  Its DMA may still read the staging buffer: segments outside the arena
+    // wait for it.
+    if (!ss.all_in_place) {
+      LWSE_CUDA(e, cudaStreamSynchronize(e->stream));
+      LWSE_CUDA(e, cudaStreamSynchronize(e->side_stream));
+    }
+    // the general placement kernel keeps its counters in two alternating scratch halves (a call resets
+    // the half the next one uses): its round may not start before the previous tick's publish kernel
+    // has read them.  (The namespace kernels count in the tick slot's own block.)
+    if (p.do_place && !p.ns_form) LWSE_CUDA(e, cudaStreamWaitEvent(e->side_stream, e->ev_pub, 0));
+  }
+  if (p.graph_ok) {
+    bool done = false;
+    const int rc = replay_tick(e, p, segs, n_segs, seq, &done);
+    if (rc != LWSE_OK || done) return rc;
+  }
+  return enqueue_tick_eager(e, p, segs, n_segs, seq);
+}
+
 static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, uint32_t flags) {
-  const int rc = tick_submit_body(e, segs, n_segs, flags);
+  const int rc = submit_tick(e, segs, n_segs, flags);
   if (rc != LWSE_OK) e->r_place_current = false;  // (its patches may or may not have been applied)
   if (rc != LWSE_OK && segs) {
     // A tick that fails once its node rows are in the mirror (a CUDA error, no staging memory) may or may
@@ -1637,409 +2015,6 @@ static int tick_submit_locked(lwse_engine* e, const lwse_patch_seg* segs, uint32
       if (segs[i].table == LWSE_TABLE_NODES && segs[i].n) e->node_index_stale = true;
   }
   return rc;
-}
-
-static int tick_submit_body(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, uint32_t flags) {
-  if (e->t_submitted - e->t_waited >= 2) return LWSE_ERR_NOT_READY;  // wait for the oldest tick first
-  const bool in_flight = e->t_submitted != e->t_waited;
-  const uint32_t slot = (uint32_t)(e->t_submitted & 1u);
-  cudaStream_t s = e->stream;
-  uint32_t* hw_dev = static_cast<uint32_t*>(e->tickw.d) + slot * 16u;
-  uint8_t* chg_d = static_cast<uint8_t*>(e->chg.d) + slot * e->chg_bytes;  // the pinned lists of this slot, as the device sees them
-  uint8_t* chg_v = static_cast<uint8_t*>(e->chg_dev.p) + slot * e->chg_bytes;  // the device-memory lists (of this slot) the kernels append to
-  uint32_t* cnt = static_cast<uint32_t*>(e->r_counts.p) + slot * 16u;          // and their counters
-  const bool do_place = (flags & LWSE_TICK_PLACE) && e->r_place_loaded && e->rn_reqs > 0;
-  // a tick that asks for a round leaves r_pout current for the resident rows (trivially so for an empty table)
-  const bool round_asked = (flags & LWSE_TICK_PLACE) && e->r_place_loaded;
-  const bool do_sweep = !(flags & LWSE_TICK_NO_SWEEP) && (e->rn_lws || e->rn_groups);
-  {
-    const int crc = check_segments(e, segs, n_segs);
-    if (crc != LWSE_OK) return crc;
-  }
-  // LWS rows patched without a sweep: r_lws_out no longer belongs to them (a row reused for another
-  // object would pass the linked DS tick's uid test with the previous object's results)
-  for (uint32_t i = 0; !do_sweep && i < n_segs; i++) {
-    if (segs[i].table == LWSE_TABLE_LWS && segs[i].n) e->r_swept = false;
-    if (segs[i].table <= LWSE_TABLE_POD_IDENT && segs[i].n) e->r_groups_swept = false;
-  }
-  // as r_swept, for the placement rows: node, request and identity rows patched without a round
-  for (uint32_t i = 0; !round_asked && i < n_segs; i++)
-    if (segs[i].n && (segs[i].table == LWSE_TABLE_NODES || segs[i].table == LWSE_TABLE_PLACE_REQS ||
-                      segs[i].table == LWSE_TABLE_POD_IDENT))
-      e->r_place_current = false;
-  // The round's form, decided before any patch is applied (it is part of a tick graph's key).  A request
-  // table grouped by namespace — and not ungrouped by this tick's patches — runs the namespace kernels as
-  // they are; any other table runs them through the namespace index, rebuilt when the namespace column
-  // changed since the last build.  The general form only where the namespace form cannot run.
-  bool ns_moves = false;
-  for (uint32_t i = 0; do_place && i < n_segs && !ns_moves; i++) {
-    const lwse_patch_seg& g = segs[i];
-    if (g.table != LWSE_TABLE_PLACE_REQS || g.n == 0 || !g.values || (!(g.flags & LWSE_PATCH_RANGE) && !g.rows)) continue;
-    const lwse_place_req* v = static_cast<const lwse_place_req*>(g.values);
-    for (uint32_t k = 0; k < g.n && !ns_moves; k++) {
-      const uint32_t row = (g.flags & LWSE_PATCH_RANGE) ? g.first_row + k : g.rows[k];
-      ns_moves = row < e->rn_reqs && v[k].ns != e->r_req_ns[row];
-    }
-  }
-  const bool ns_form = do_place && lwse::place_ns_supported(e->n_nodes, e->n_domains);
-  const bool indexed = ns_form && !(e->r_place_grouped && !ns_moves);
-  const lwse::PlaceNsIndex ns_index = !indexed                              ? lwse::kNsIndexNone
-                                      : (ns_moves || !e->r_ns_index_ok) ? lwse::kNsIndexBuild
-                                                                          : lwse::kNsIndexReuse;
-  const bool scan_form = (flags & LWSE_SWEEP_PLACE_SCAN) != 0;
-  // Node rows: the mirror decides, before anything is enqueued, whether this tick's round rebuilds the node
-  // index (also part of a tick graph's key).  A tick without a round leaves a stale index to the next one.
-  const int node_rows = node_patches_locked(e, segs, n_segs);
-  if (node_rows < 0) return node_rows;
-  const bool node_rebuild = do_place && e->node_index_stale;
-  e->last_node_info = lwse_node_info{(uint32_t)node_rows, node_rebuild ? 1u : 0u, e->n_usable, 0u};
-  // sequence numbers count the ticks that end in a publish kernel (the device counts the same ones)
-  uint32_t seq = 0;
-  if (do_sweep || do_place) {
-    seq = ++e->tick_seq;
-    if (seq == 0) seq = ++e->tick_seq;
-  }
-  // The bookkeeping that closes a submitted tick.  `wrote_any`: the tick patched a table; `wrote_main`: it
-  // patched a table on the engine's stream.
-  auto close_submit = [&](bool published, bool wrote_any, bool wrote_main, bool graph) {
-    lwse_engine::TickSlot& ts = e->tslot[slot];
-    ts.seq = seq;
-    ts.do_sweep = do_sweep;
-    ts.do_place = do_place;
-    ts.published = published;
-    ts.wrote = wrote_any;
-    e->t_submitted++;
-    if (do_sweep) {
-      e->r_swept = e->r_groups_swept = true;
-      e->r_sweep_flags = flags & LWSE_SWEEP_GANG;
-    }
-    if (round_asked) e->r_place_current = true;
-    e->main_unforked = !do_place && (e->main_unforked || wrote_main);
-    lwse_tick_info& ti = e->last_tick_info;
-    ti.place_form = !do_place ? LWSE_TICK_FORM_NONE
-                    : !ns_form ? LWSE_TICK_FORM_GENERAL
-                    : scan_form ? LWSE_TICK_FORM_SCAN
-                                : LWSE_TICK_FORM_NAMESPACE;
-    ti.indexed = indexed ? 1u : 0u;
-    ti.index_built = ns_index == lwse::kNsIndexBuild ? 1u : 0u;
-    ti.graph = graph ? 1u : 0u;
-    if (indexed) e->r_ns_index_ok = true;  // (also after a replay, which enqueues no call that would say so)
-  };
-  {
-    const size_t ub = stage_bytes_upper_bound(segs, n_segs);
-    if (ub > e->stage.cap) {  // rare: only segments outside the arena are staged
-      bool all_in_arena = true;
-      for (uint32_t i = 0; i < n_segs; i++)
-        if (segs[i].n && !(segs[i].flags & LWSE_PATCH_RANGE) &&
-            (!rows_in_place(e, segs[i]) || !e->arena.holds(segs[i].values, 1)))
-          all_in_arena = false;
-      if (!all_in_arena) {
-        LWSE_CUDA(e, cudaStreamSynchronize(s));
-        LWSE_CUDA(e, cudaStreamSynchronize(e->side_stream));
-        LWSE_CUDA(e, e->stage.reserve(ub));
-      }
-    }
-  }
-  // Patches go where their readers run: the placement request table is read only by the round on
-  // the side stream, everything else by the sweep on the engine's stream — the round then starts
-  // behind its own few rows (read in place over PCIe: no copy-engine launch) while the copy engine
-  // still moves the pod patches, and is mostly done when the sweep needs the SMs.  Identity-row
-  // patches move occupancy counts and node-row patches change the nodes, both of which the round
-  // reads: with either in the tick it forks behind the main scatter.  ONE publish kernel behind the
-  // join copies all change lists out.
-  constexpr uint32_t kSideTables = 1u << LWSE_TABLE_PLACE_REQS;
-  bool has_ident = false, has_side = false;
-  for (uint32_t i = 0; i < n_segs; i++) {
-    if (segs[i].n && segs[i].table == LWSE_TABLE_POD_IDENT) has_ident = true;
-    if (segs[i].n && segs[i].table == LWSE_TABLE_PLACE_REQS) has_side = true;
-  }
-  // (a round also forks behind the engine's stream when an earlier tick without a round patched tables there
-  // that no round has been ordered behind yet: its node rows and occupancy counters may still be in flight)
-  const bool prior_unforked = do_place && e->main_unforked;
-  const bool fork_behind_main = has_ident || node_rows > 0 || prior_unforked;
-  bool wrote = false, wrote_side = false;
-  size_t stage_used = 0;
-  int rc = LWSE_OK;
-  int cuda_err = 0;
-  cudaStream_t ps = e->side_stream;
-  bool all_in_place = true;  // no segment needs the staging buffer
-  for (uint32_t i = 0; i < n_segs; i++) {
-    if (!segs[i].n || (segs[i].flags & LWSE_PATCH_RANGE)) continue;
-    void* tb;
-    uint64_t trows;
-    uint32_t rb = 0;
-    if (!resident_table(e, segs[i].table, &tb, &trows, &rb)) return LWSE_ERR_INVALID_ARG;
-    if (!rows_in_place(e, segs[i]) || !values_in_place(e, segs[i], rb)) all_in_place = false;
-  }
-  if (in_flight) {
-    // a tick is still running.  Its DMA may still read the staging buffer: segments outside the arena
-    // wait for it.  Its publish kernel (the last thing on the engine's stream) still has to copy and
-    // reset the placement change list the side stream appends to: the side stream starts behind it.
-    if (!all_in_place) {
-      LWSE_CUDA(e, cudaStreamSynchronize(s));
-      LWSE_CUDA(e, cudaStreamSynchronize(ps));
-    }
-    // the general placement kernel keeps its counters in two alternating scratch halves (a call resets
-    // the half the next one uses): its round may not start before the previous tick's publish kernel
-    // has read them.  (The namespace kernels count in the tick slot's own block.)
-    if (do_place && !ns_form) LWSE_CUDA(e, cudaStreamWaitEvent(ps, e->ev_pub, 0));
-  }
-  ScatterPlan main_plan;
-  auto apply_main = [&](bool defer) -> int {
-    return apply_patches_locked(e, segs, n_segs, &wrote, ~kSideTables, s, 0, &stage_used, 0, defer ? &main_plan : nullptr);
-  };
-  auto apply_side = [&]() -> int {
-    if (fork_behind_main && (wrote || prior_unforked) && (has_side || do_place)) {
-      LWSE_CUDA(e, cudaEventRecord(e->ev_fork, s));
-      LWSE_CUDA(e, cudaStreamWaitEvent(ps, e->ev_fork, 0));
-    }
-    if (!has_side) return LWSE_OK;
-    return apply_patches_locked(e, segs, n_segs, &wrote_side, kSideTables, ps, stage_used, nullptr, /*dma_min_bytes=*/65536);
-  };
-  lwse::PublishListHost pl[3] = {};
-  // the publish kernel's entry for this slot's change list k: 0 LWS rows, 1 group rows, 2 placement rows
-  auto publish_list = [&](int k) -> lwse::PublishListHost {
-    const uint32_t capacity[3] = {e->rn_lws, e->rn_groups, e->rn_reqs};
-    const uint32_t out_bytes[3] = {sizeof(lwse_lws_out), sizeof(lwse_group_out), sizeof(lwse_place_out)};
-    return {reinterpret_cast<uint32_t*>(chg_v + e->chg_off[2 * k]), chg_v + e->chg_off[2 * k + 1],
-            reinterpret_cast<uint32_t*>(chg_d + e->chg_off[2 * k]), chg_d + e->chg_off[2 * k + 1], cnt + (k == 2 ? 4 : k),
-            capacity[k], out_bytes[k]};
-  };
-  int sweep_first_mode = -1;      // -1: 2 behind this tick's scatter kernel, else 1 (see launch_lws_sweep)
-  bool place_first_pdl = true;    // the round's first kernel follows a kernel on the side stream
-  void* place_mid_event = nullptr;  // (graph capture) recorded between the condense and the namespace kernel
-  auto enqueue_sweep = [&]() -> int {
-    lwse_lws_tables d{};
-    d.lws = (const lwse_lws_rec*)e->r_lws.p;
-    d.n_lws = e->rn_lws;
-    d.groups = (const lwse_group_rec*)e->r_groups.p;
-    d.n_groups = e->rn_groups;
-    d.pod_state = (const lwse_pod_state*)e->r_pst.p;
-    d.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
-    d.n_pods = e->rn_pods;
-    d.lws_out = (lwse_lws_out*)e->r_lws_out.p;
-    d.group_out = (lwse_group_out*)e->r_group_out.p;
-    d.flags = flags & LWSE_SWEEP_GANG;
-    lwse::SweepChangeLists cl;
-    cl.lws_rows = reinterpret_cast<uint32_t*>(chg_v + e->chg_off[0]);
-    cl.lws_out = reinterpret_cast<lwse_lws_out*>(chg_v + e->chg_off[1]);
-    cl.lws_capacity = e->rn_lws;
-    cl.group_rows = reinterpret_cast<uint32_t*>(chg_v + e->chg_off[2]);
-    cl.group_out = reinterpret_cast<lwse_group_out*>(chg_v + e->chg_off[3]);
-    cl.group_capacity = e->rn_groups;
-    cl.counts = cnt;
-    int launched = lwse::launch_lws_sweep(&d, (const lwse_node_rec*)e->nodes.p, e->n_nodes, e->r_scan.p, e->sm_count, s,
-                                          &cuda_err, &cl, nullptr, sweep_first_mode >= 0 ? sweep_first_mode : (wrote ? 2 : 1));
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-    pl[0] = publish_list(0);
-    pl[1] = publish_list(1);
-    return LWSE_OK;
-  };
-  auto enqueue_place = [&]() -> int {
-    const uint32_t form = !ns_form ? kFormGeneral : (flags & LWSE_SWEEP_PLACE_SCAN) ? kFormScan : kFormGrouped;
-    // the namespace kernels append the changed rows themselves; the general form gets a diff kernel
-    const lwse::PlaceNsChanges changes{(lwse_place_out*)e->r_pout_prev.p, reinterpret_cast<uint32_t*>(chg_v + e->chg_off[4]),
-                                       reinterpret_cast<lwse_place_out*>(chg_v + e->chg_off[5]), cnt + 4, e->rn_reqs, (int)slot,
-                                       place_mid_event};
-    bool diffed = false;
-    if (flags & LWSE_TICK_SHARED_OCCUPANCY) {  // multi-rank: this rank's counters go to the peers, the round sees the sum
-      if (!e->xch_connected) return LWSE_ERR_NOT_READY;
-      rc = shared_occupancy_place_locked(e, (const lwse_place_req*)e->r_preq.p, e->rn_reqs, (const uint32_t*)e->r_occ.p,
-                                         e->rn_namespaces, (lwse_place_out*)e->r_pout.p, form,
-                                         (flags & LWSE_EXCHANGE_LAGGED) != 0, ps, &changes, ns_index);
-      diffed = rc == LWSE_OK;
-    } else {
-      rc = place_locked(e, (const lwse_place_req*)e->r_preq.p, e->rn_reqs, (const uint32_t*)e->r_occ.p, e->rn_namespaces,
-                        (lwse_place_out*)e->r_pout.p, nullptr, ps, 1, e->rn_reqs, 0, false, form, place_first_pdl, &changes,
-                        &diffed, ns_index);
-    }
-    if (rc != LWSE_OK) return rc;
-    if (!diffed) {
-      int launched = lwse::launch_place_diff((const lwse_place_out*)e->r_pout.p, changes.prev, e->rn_reqs, changes.rows,
-                                             changes.outs, changes.capacity, changes.count, ps, &cuda_err);
-      if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-    }
-    pl[2] = publish_list(2);
-    e->tick_place_ns = diffed;
-    return LWSE_OK;
-  };
-  // The tick's last step, on the publish stream: behind everything the tick enqueued on the engine's
-  // stream (both branches joined there), so the NEXT tick's kernels do not wait for the copy of this
-  // tick's changed rows to the host.  Lists, counters and the round's counter block are per slot.
-  auto enqueue_publish = [&]() -> int {
-    LWSE_CUDA(e, cudaEventRecord(e->ev_done, s));
-    LWSE_CUDA(e, cudaStreamWaitEvent(e->pub_stream, e->ev_done, 0));
-    const bool ns_counters = do_place && e->tick_place_ns;
-    int launched = lwse::launch_publish(pl, do_place ? e->place_rounds_ptr : nullptr, hw_dev, 4, seq, cnt + 2,
-                                        e->last_changed[0] + e->last_changed[1], e->pub_stream, &cuda_err,
-                                        ns_counters ? const_cast<uint32_t*>(e->place_rounds_ptr) : nullptr, 8u, /*pdl=*/false);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-    LWSE_CUDA(e, cudaEventRecord(e->ev_pub, e->pub_stream));
-    return LWSE_OK;
-  };
-  // ---- replay as a CUDA graph --------------------------------------------------------------
-  // Enqueueing a tick kernel by kernel costs ~10 runtime calls of microseconds each (launches with
-  // attributes and 200-400 bytes of parameters): more host time than the GPU needs for the tick.
-  // A tick whose patches lie in the arena is therefore replayed as ONE graph per (shape of the
-  // tick, slot):   scatter -> condense -> { fused -> LWS pass  ||  namespace kernel }.
-  // What changes from tick to tick travels outside the graph, on the copy stream, so that the
-  // copies of tick k+1 overlap the kernels of tick k: the patch bytes (arena span -> mirror) and
-  // the scatter's segment descriptors (a 512-byte block, pinned slot -> device).  The publish
-  // kernel follows on the publish stream, launched with the tick's sequence number.
-  bool any_range = false;
-  for (uint32_t i = 0; i < n_segs; i++)
-    if (segs[i].n && (segs[i].flags & LWSE_PATCH_RANGE)) any_range = true;
-  // (LWSE_TICK_GRAPH: 1 = replay when the previous tick is still in flight — the pipelined use, where the
-  //  host's enqueue time is what limits the rate; a lone tick is faster kernel by kernel, because its
-  //  round starts while the copy engine still moves the pod patches; 2 = always; 0 = never)
-  const bool shared_occ = (flags & LWSE_TICK_SHARED_OCCUPANCY) != 0;
-  const bool graph_ok = (e->use_graph >= 2 || (e->use_graph == 1 && in_flight)) && all_in_place && !any_range &&
-                        (!shared_occ || (do_place && e->xch_connected)) &&
-                        (do_sweep || do_place) && !(has_side && !do_place) &&
-                        (!do_place || ns_form);
-  if (graph_ok) {
-    bool has_patches = false;
-    for (uint32_t i = 0; i < n_segs; i++)
-      if (segs[i].n) has_patches = true;
-    const uint32_t key = (has_patches ? 1u : 0u) | (do_sweep ? 8u : 0u) | (do_place ? 16u : 0u) |
-                         ((flags & LWSE_SWEEP_GANG) ? 32u : 0u) | ((flags & LWSE_SWEEP_PLACE_SCAN) ? 64u : 0u) | (slot << 8) |
-                         (shared_occ ? 512u : 0u) | ((shared_occ && (flags & LWSE_EXCHANGE_LAGGED)) ? 1024u : 0u) |
-                         (indexed ? 2048u : 0u) | (ns_index == lwse::kNsIndexBuild ? 4096u : 0u) |
-                         (node_rows > 0 ? 8192u : 0u) | (node_rebuild ? 16384u : 0u);
-    lwse_engine::TickGraph& tg = e->tick_graphs[key];
-    bool replay = !tg.failed && tg.seen >= 1;  // the first tick of a shape runs eagerly: every buffer settles
-    tg.seen++;
-    ScatterPlan gp;
-    if (replay) {
-      bool w = false;  // one plan for every table: one scatter launch behind one copy of the arena span
-      rc = apply_patches_locked(e, segs, n_segs, &w, 0xFFFFFFFFu, s, 0, nullptr, 0, &gp, /*plan_only=*/true);
-      if (rc != LWSE_OK) return rc;
-      if (gp.eager_only || gp.recount) replay = false;
-    }
-    const size_t desc_bytes = lwse::kScatterDescBytes;
-    if (replay && (e->tdesc.reserve(2 * desc_bytes) != cudaSuccess || e->tdesc_dev.reserve(2 * desc_bytes) != cudaSuccess)) {
-      (void)cudaGetLastError();
-      replay = false;
-    }
-    if (replay) {
-      uint8_t* h_desc = static_cast<uint8_t*>(e->tdesc.h) + slot * desc_bytes;
-      uint8_t* d_desc = d_desc_of(e, slot);
-      if (has_patches && !lwse::write_scatter_desc(h_desc, gp.sc, gp.n, e->n_nodes ? (uint32_t*)e->r_occ.p : nullptr, e->n_nodes))
-        replay = false;
-      if (replay && !tg.exec) {
-        // ---- capture: the same enqueue functions, on capturing streams ----
-        cudaError_t ce = cudaStreamSynchronize(s);
-        if (ce == cudaSuccess) ce = cudaStreamSynchronize(ps);
-        if (ce != cudaSuccess) return fail_cuda(e, ce);
-        const uint64_t launches_before = e->launches;
-        int crc = LWSE_OK;
-        ce = cudaStreamBeginCapture(s, cudaStreamCaptureModeRelaxed);
-        if (ce == cudaSuccess) {
-          auto cap = [&](cudaError_t x) { if (crc == LWSE_OK && x != cudaSuccess) { ce = x; crc = LWSE_ERR_CUDA; } };
-          if (has_patches) {  // the graph's first node: an ordinary launch
-            int err = 0;
-            const int launched = lwse::launch_scatter_desc(d_desc, e->sm_count, s, /*pdl=*/false, &err);
-            if (launched < 0) cap((cudaError_t)err); else e->launches += (uint64_t)launched;
-          }
-          if (do_place) {  // the round forks behind the scatter (it reads the request rows and the occupancy counters)
-            cap(cudaEventRecord(e->ev_fork, s));
-            cap(cudaStreamWaitEvent(ps, e->ev_fork, 0));
-            place_first_pdl = false;  // (behind an event: an ordinary launch)
-            // The fused sweep kernel fills every SM (3 CTAs of 256 x 77 registers) the moment it starts
-            // and the namespace kernel's CTAs (512 x 53 registers) then wait for CTAs to retire: hold
-            // the sweep back until the (short) condense kernel is done, so that both reach the SMs together.
-            place_mid_event = do_sweep ? (void*)e->ev_mid : nullptr;
-            if (crc == LWSE_OK) crc = enqueue_place();
-            if (do_sweep && e->tick_place_ns) cap(cudaStreamWaitEvent(s, e->ev_mid, 0));
-            place_mid_event = nullptr;
-          }
-          // behind the scatter kernel alone: programmatic, waits at its top; behind an event / first node: ordinary
-          sweep_first_mode = (has_patches && !(do_place && e->tick_place_ns)) ? 2 : 0;
-          if (crc == LWSE_OK && do_sweep) crc = enqueue_sweep();
-          if (do_place) {
-            cap(cudaEventRecord(e->ev_join, ps));
-            cap(cudaStreamWaitEvent(s, e->ev_join, 0));
-          }
-          cudaGraph_t graph = nullptr;
-          const cudaError_t ee = cudaStreamEndCapture(s, &graph);
-          if (ee != cudaSuccess || graph == nullptr) cap(ee != cudaSuccess ? ee : cudaErrorUnknown);
-          if (crc == LWSE_OK) cap(cudaGraphInstantiate(&tg.exec, graph, 0));
-          if (graph) cudaGraphDestroy(graph);
-        } else {
-          crc = LWSE_ERR_CUDA;
-        }
-        tg.kernels = (uint32_t)(e->launches - launches_before);
-        e->launches = launches_before;
-        sweep_first_mode = -1;
-        place_first_pdl = true;
-        if (crc != LWSE_OK || !tg.exec) {  // this shape stays eager; the streams are usable again after EndCapture
-          (void)cudaGetLastError();
-          if (tg.exec) cudaGraphExecDestroy(tg.exec);
-          tg.exec = nullptr;
-          tg.failed = true;
-          replay = false;
-          pl[0] = pl[1] = pl[2] = lwse::PublishListHost{};
-          e->node_index_stale = e->node_index_stale || node_rebuild;  // (the eager run below builds it)
-        } else {
-          tg.place_ns = e->tick_place_ns;
-          tg.rounds_ptr = e->place_rounds_ptr;
-        }
-      }
-    }
-    if (replay) {
-      if (has_patches) {  // patch bytes (arena span -> mirror) and the descriptor block, on the copy stream
-        if (gp.dma)
-          LWSE_CUDA(e, cudaMemcpyAsync(static_cast<uint8_t*>(e->arena_mirror.p) + gp.lo, static_cast<const uint8_t*>(e->arena.h) + gp.lo,
-                                       gp.hi - gp.lo, cudaMemcpyHostToDevice, e->copy_stream));
-        LWSE_CUDA(e, cudaMemcpyAsync(d_desc_of(e, slot), static_cast<uint8_t*>(e->tdesc.h) + slot * desc_bytes, desc_bytes,
-                                     cudaMemcpyHostToDevice, e->copy_stream));
-        LWSE_CUDA(e, cudaEventRecord(e->ev_dma, e->copy_stream));
-        LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_dma, 0));
-      }
-      LWSE_CUDA(e, cudaGraphLaunch(tg.exec, s));
-      e->launches += tg.kernels;
-      if (node_rebuild) e->node_index_stale = false;  // (the graph's round built it)
-      e->graph_ticks++;
-      if (shared_occ) e->xch_step++;  // (the replayed push kernel advanced the device counter by one)
-      if (!pl[0].count && do_sweep) {  // (replayed without capturing: the lists the graph's kernels append to)
-        pl[0] = publish_list(0);
-        pl[1] = publish_list(1);
-      }
-      if (!pl[2].count && do_place) pl[2] = publish_list(2);
-      if (do_place) {
-        e->tick_place_ns = tg.place_ns;
-        e->place_rounds_ptr = tg.rounds_ptr;
-      }
-      rc = enqueue_publish();
-      if (rc != LWSE_OK) return rc;
-      close_submit(true, has_patches, has_patches, true);
-      return LWSE_OK;
-    }
-  }
-  // Eager enqueue order.  Every call costs microseconds of host time and the copy of the pod patches
-  // heads the critical path, so that copy is enqueued first; the round's launches follow on the side
-  // stream while the copy engine works, then the main scatter and the sweep behind the copy.  A round
-  // that forks behind the main scatter (identity or node patches: it reads the occupancy counters and
-  // the node rows) needs that scatter enqueued before it, so the scatter is not deferred then.
-  const bool defer_scatter = !fork_behind_main;
-  rc = apply_main(defer_scatter);
-  if (rc == LWSE_OK) rc = apply_side();
-  if (rc == LWSE_OK && do_place && wrote) rc = enqueue_place();
-  if (rc == LWSE_OK && defer_scatter) rc = launch_scatter_plan(e, main_plan, s);
-  if (rc == LWSE_OK && do_sweep) rc = enqueue_sweep();
-  if (rc == LWSE_OK && do_place && !wrote) rc = enqueue_place();
-  if (rc != LWSE_OK) return rc;
-  if (do_place || wrote_side) {
-    LWSE_CUDA(e, cudaEventRecord(e->ev_join, ps));
-    LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_join, 0));
-  }
-  const bool published = do_sweep || do_place;
-  if (published) {
-    rc = enqueue_publish();
-    if (rc != LWSE_OK) return rc;
-  }
-  close_submit(published, wrote || wrote_side, wrote, false);
-  return LWSE_OK;
 }
 
 // The oldest tick in flight: spin on its sequence word (the tick's only wait), report its counts.
@@ -2234,16 +2209,14 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
   for (uint32_t i = 0; i < q->n_segs; i++)
     if (q->segs[i].n && q->segs[i].table != LWSE_TABLE_NODES && q->segs[i].table != LWSE_TABLE_PLACE_REQS)
       return LWSE_ERR_INVALID_ARG;
-  {
-    const int crc = check_segments(e, q->segs, q->n_segs);
-    if (crc != LWSE_OK) return crc;
-  }
-  // the touched namespaces and the node-index decision (the tick's rule, over the mirror, which stays as it is)
+  SegSummary ss;
+  if (const int crc = summarize_segments(e, q->segs, q->n_segs, &ss); crc != LWSE_OK) return crc;
+  // the node-index decision is the tick's, over the mirror, which stays as it is; then the touched namespaces
+  const bool node_rows = (ss.tables & (1u << LWSE_TABLE_NODES)) != 0;
+  bool node_rebuild = ss.node_moves;
   std::vector<uint8_t> touched(n_ns, 0);
   for (uint32_t v = e->rn_namespaces; v < n_ns; v++) touched[v] = 1;  // (their resident rows were UNSCHEDULABLE)
-  bool node_rows = false, node_rebuild = false;
   size_t stage_need = align256((size_t)n_ns) + align256((size_t)q->n_extra * sizeof(lwse_place_req));
-  std::unordered_map<uint32_t, lwse_node_rec> node_now;  // rows patched earlier in this call
   for (uint32_t i = 0; i < q->n_segs; i++) {
     const lwse_patch_seg& g = q->segs[i];
     if (g.n == 0) continue;
@@ -2254,14 +2227,7 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
     for (uint32_t k = 0; k < g.n; k++) {
       const uint32_t row = range ? g.first_row + k : g.rows[k];
       if (row >= n_rows) return LWSE_ERR_INVALID_ARG;
-      if (g.table == LWSE_TABLE_NODES) {
-        node_rows = true;
-        const lwse_node_rec& v = static_cast<const lwse_node_rec*>(g.values)[k];
-        auto it = node_now.find(row);
-        const lwse_node_rec& old = it != node_now.end() ? it->second : e->h_nodes[row];
-        if (node_patch_moves_index(old, v, e->n_domains)) node_rebuild = true;
-        node_now[row] = v;
-      } else {
+      if (g.table == LWSE_TABLE_PLACE_REQS) {
         const uint32_t nv = static_cast<const lwse_place_req*>(g.values)[k].ns, ov = e->r_req_ns[row];
         if (nv < n_ns) touched[nv] = 1;
         if (ov < n_ns) touched[ov] = 1;
