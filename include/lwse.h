@@ -33,7 +33,9 @@
  *   lwse_ds_resident_* the same arithmetic over resident DS tables, fed by DS and child-LWS
  *                      watch events (disaggregatedset_controller.go:55-126, :273)
  *   lwse_resident_drain_*  pod_controller.go:204-266 (handleRestartPolicy), :268-295, :338-362 over
- *                      the resident tables with the pods of drained nodes deleting
+ *                      the resident tables with the pods of drained nodes deleting;
+ *                      lwse_resident_drain_budget* adds a build-defined availability floor from
+ *                      leaderworkerset_controller.go:302 (the reference has no drain budget)
  *   lwse_group_keys_*  pkg/webhooks/pod_webhook.go:180-182 + pkg/utils/utils.go:39-43
  *                      (SHA-1 group / subgroup keys)
  *   lwse_subgroup_keys_*  pkg/webhooks/pod_webhook.go:249-255 (getSubGroupIndex) + :130,:151
@@ -848,6 +850,106 @@ typedef struct lwse_drain_cost {
   uint64_t reserved;
 } lwse_drain_cost;
 LWSE_API int lwse_resident_drain_cost(lwse_engine* e, lwse_drain_cost* out);
+
+/* ---- drain budget -------------------------------------------------------------------------------
+ * "Does this drain take a LeaderWorkerSet below its availability floor?"  LeaderWorkerSet has no
+ * disruption budget of its own; the one number that says how many groups an object may lose is
+ * rollingUpdateConfiguration.maxUnavailable, which the controller respects on rolling updates
+ * (leaderworkerset_controller.go:302, :366-369, :650-673).  The reference has no drain budget: the
+ * definition below is this build's own (DESIGN.md §3.5, "Drain budget").
+ *
+ * Definition.  An LWS row L is EVALUATED when its baseline result row has none of LWSE_LOUT_BAD_TABLE,
+ * _IRREGULAR, _RUP_ERROR, _STATUS_ERROR and its row has no LWSE_LWS_INTSTR_INVALID.  For an evaluated L:
+ *   floor        = max(0, replicas - mu), mu = maxUnavailable scaled against replicas, rounded down (:302),
+ *                  clamped to int32;
+ *   ready_before = lws_out[L].ready_replicas of the baseline (the results of the most recently submitted
+ *                  sweep, the rows lwse_resident_drain_whatif diffs against).
+ * The groups of L are the rows g of its group range (inside the group table) with lws_index == L.  For a
+ * drain set D of node rows a group is RESTARTED exactly as lwse_resident_drain_whatif defines it (neither
+ * restart bit in its baseline row, one in its what-if row), and
+ *   lost         = restarted groups of L whose baseline row has LWSE_GOUT_COND_READY (counted into
+ *                  readyReplicas, :455-458);  ready_after = ready_before - lost;
+ *   BREACHED        lost > 0 and ready_after < floor;
+ *   ALREADY_BELOW   ready_before < floor, whether or not D touches L;
+ *   LOSES_AVAILABLE the baseline condition is Available and a lost group has index g - group_base <
+ *                   replicas (readyNonBurstWorkerCount falls below replicas, :494).
+ * L is TOUCHED when any group of L restarts.  A touched L that is not evaluated is listed with
+ * LWSE_DRAINB_NOT_EVALUATED (floor 0) and counts in n_touched / lws_touched only.
+ *
+ * Drain sets: LWSE_DRAIN_NODES takes node rows (as lwse_resident_drain_whatif); LWSE_DRAIN_DOMAINS takes
+ * domain ids below the resident n_domains and drains every node row whose domain_id is one of them — by
+ * domain_id alone, so cordoned and unschedulable nodes belong to their domain, and a node whose domain_id
+ * is LWSE_NONE or >= n_domains belongs to none.
+ *
+ * Readiness, isolation and errors: as lwse_resident_drain_whatif (the what-if stream, the engine mutex,
+ * scratch of its own that only grows; no tick, graph, arena, change list, resident table, output row,
+ * occupancy counter, node index or tick info is touched).  LWSE_ERR_INVALID_ARG also for a scope other
+ * than the two, and for a domain id >= n_domains.  Multi-rank engines: an LWS lives on one rank, so every
+ * count sums across ranks' answers and min_margin is the min of theirs. */
+#define LWSE_DRAIN_NODES 0u
+#define LWSE_DRAIN_DOMAINS 1u
+
+#define LWSE_DRAINB_NOT_EVALUATED (1u << 0)
+#define LWSE_DRAINB_BREACHED (1u << 1)
+#define LWSE_DRAINB_ALREADY_BELOW (1u << 2)
+#define LWSE_DRAINB_LOSES_AVAILABLE (1u << 3)
+
+/* One touched LWS row of a drain (32 B). */
+typedef struct lwse_drain_budget {
+  uint32_t lws;               /* LWS row                                                                */
+  uint32_t flags;             /* LWSE_DRAINB_*                                                           */
+  int32_t replicas;           /* spec.replicas                                                           */
+  int32_t floor;              /* 0 when not evaluated                                                    */
+  int32_t ready_before;
+  int32_t ready_after;        /* ready_before - lost, clamped to int32                                   */
+  uint32_t groups_restarted;  /* restarted groups of L, ready or not                                     */
+  uint32_t reserved;
+} lwse_drain_budget;
+
+/* The set form: the touched LWS rows of one drain set, and its totals. */
+typedef struct lwse_drain_budget_query {
+  /* in */
+  const uint32_t* ids;        /* [n_ids] node rows or domain ids (by scope), host memory; duplicates allowed */
+  uint32_t n_ids;
+  uint32_t scope;             /* LWSE_DRAIN_NODES or LWSE_DRAIN_DOMAINS                                  */
+  uint32_t capacity;          /* rows `rows` holds                                                       */
+  uint32_t reserved;
+  lwse_drain_budget* rows;    /* [capacity]: touched LWS rows (beyond capacity not listed; order unspecified) */
+  /* out */
+  uint32_t n_touched;         /* every touched LWS row, listed or not                                    */
+  uint32_t n_breached;
+  uint32_t n_loses_available;
+  uint32_t n_already_below;   /* evaluated rows below their floor, touched or not                       */
+  uint32_t n_pods_evicted;    /* the five totals of lwse_drain_whatif for the same node set              */
+  uint32_t n_leaders_evicted;
+  uint32_t n_groups_restarted;
+  uint32_t n_ready_restarted;
+  uint64_t n_pods_recreated;
+} lwse_drain_budget_query;
+LWSE_API int lwse_resident_drain_budget(lwse_engine* e, lwse_drain_budget_query* q);
+
+/* The per-key form: one row per node (LWSE_DRAIN_NODES, n_nodes rows) or per domain (LWSE_DRAIN_DOMAINS,
+ * n_domains rows), row k holding the answer of the set form for the node k or for the nodes of domain k
+ * (48 B).  The first 32 bytes are an lwse_drain_cost row: for scope NODES they equal
+ * lwse_resident_drain_cost byte for byte.  Exact in one pass per key by the drain cost's argument: draining
+ * D restarts a group iff some pod of the group bound to a node of D passes the restart verdict with its
+ * deleting bit set, so lost(L, key) is the number of distinct COND_READY groups of L with such a pod on the
+ * key.  The (LWS, key) pairs are gathered in an open-addressing table in scratch sized from a counting pass
+ * (one host synchronisation); an insert the table refuses fails the call with LWSE_ERR_OOM.  `out` holds the
+ * rows in host memory. */
+typedef struct lwse_drain_budget_cost {
+  uint32_t pods;              /* the lwse_drain_cost totals of the key                                   */
+  uint32_t leaders;
+  uint32_t groups_restarted;
+  uint32_t ready_restarted;
+  uint64_t pods_recreated;
+  uint64_t reserved;
+  uint32_t lws_touched;       /* n_touched of the set form for this key                                  */
+  uint32_t lws_breached;
+  uint32_t lws_loses_available;
+  int32_t min_margin;         /* min over touched evaluated L of ready_after - floor; INT32_MAX for none */
+} lwse_drain_budget_cost;
+LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lwse_drain_budget_cost* out);
 
 /* ------------------------------------------------------------------------- */
 /* Peer exchange: the multi-GPU placement step without a collective library  */

@@ -11,6 +11,18 @@
 //                       the group pass (lwse_restart.cuh) with the deleting bit set, and the group's
 //                       restart nodes deduplicated (__match_any_sync per batch, a per-warp list across
 //                       batches) before one atomic per (group, node) pair and field.
+//
+// Drain budget (lwse_resident_drain_budget*):
+//   drain_domain_mask_kernel   the node mask of a set of domains, from the node rows' domain_id.
+//   drain_budget_kernel        the set form, after the what-if's mark → sweep → diff: one warp per LWS row over
+//                              its group range, the what-if rows against the baseline; touched rows appended
+//                              with one atomic per LWS, the totals reduced per warp before one atomic each.
+//   drain_budget_walk_kernel   the per-key form: drain_cost_kernel's walk (same gate, visit_pod, dedup) with
+//                              the key = the node or its domain.  <false> adds the cost totals per key and
+//                              counts the pairs; <true> adds every fresh (group, key) pair of a group that
+//                              belongs to its LWS row into an open-addressing (LWS, key) table.
+//   drain_budget_keys_init_kernel / drain_budget_finish_kernel   the key rows' pods and min_margin start; each
+//                              table entry turned into its key's lws_touched / breached / loses / min_margin.
 #include "lwse_device.cuh"
 #include "lwse_launch.cuh"
 #include "lwse_restart.cuh"
@@ -247,6 +259,331 @@ int launch_drain_cost(const lwse_lws_rec* d_lws, uint32_t n_lws, const lwse_grou
   const DrainCostArgs a{d_lws, d_groups, d_state, d_ident, d_baseline, d_cost, n_pods, n_lws, n_groups, n_nodes};
   drain_cost_kernel<<<grid_for(n_groups, kCostThreads / 32, (uint32_t)sm_count * 8u), kCostThreads, 0, s>>>(a);
   return launched_or_fail(1, cuda_err);
+}
+
+// --------------------------------------------------------------------------
+// drain budget (lwse_resident_drain_budget*): the definitions are in lwse.h
+// --------------------------------------------------------------------------
+// What the budget of one LWS row needs from its row and its baseline result row.
+struct LwsBudget {
+  uint32_t gbase, gcount;  // the group range; gcount = 0 when it lies outside the group table
+  int32_t replicas, floor, ready_before;
+  bool evaluated, available;
+};
+
+constexpr uint32_t kBudgetExcluded = LWSE_LOUT_BAD_TABLE | LWSE_LOUT_IRREGULAR | LWSE_LOUT_RUP_ERROR | LWSE_LOUT_STATUS_ERROR;
+
+__device__ __forceinline__ int32_t clamp_i32(int64_t v) {
+  return (int32_t)(v < INT32_MIN ? (int64_t)INT32_MIN : (v > INT32_MAX ? (int64_t)INT32_MAX : v));
+}
+
+__device__ __forceinline__ LwsBudget budget_of(const lwse_lws_rec* lws, const lwse_lws_out* lws_out, uint32_t L,
+                                               uint32_t n_groups) {
+  const uint4* row = reinterpret_cast<const uint4*>(lws + L);
+  const uint4 r0 = ldg_cached(row + 0), r1 = ldg_cached(row + 1), r3 = ldg_cached(row + 3);
+  const uint4* orow = reinterpret_cast<const uint4*>(lws_out + L);
+  const uint4 o0 = __ldg(orow + 0), o1 = __ldg(orow + 1);
+  const uint32_t lflags = r0.w, oflags = o1.z;
+  LwsBudget b;
+  b.replicas = (int32_t)r1.x;
+  b.gbase = r3.z;
+  b.gcount = (uint64_t)r3.z + r3.w <= n_groups ? r3.w : 0u;
+  b.evaluated = !(oflags & kBudgetExcluded) && !(lflags & LWSE_LWS_INTSTR_INVALID);
+  b.available = ((oflags & LWSE_LOUT_COND_MASK) >> LWSE_LOUT_COND_SHIFT) == LWSE_COND_AVAILABLE;
+  b.ready_before = (int32_t)o0.w;
+  const int32_t mu = scaled_value((int32_t)r1.w, lflags & LWSE_LWS_UNAVAIL_IS_PERCENT, b.replicas, false);  // :302
+  const int64_t fl = (int64_t)b.replicas - mu;
+  b.floor = b.evaluated ? clamp_i32(fl < 0 ? 0 : fl) : 0;
+  return b;
+}
+
+// The drain mask of a set of domains: node n is drained iff its domain_id is a marked id below n_domains.
+struct DrainDomainMaskArgs {
+  const uint8_t* domains;  // n_domains bytes, 1 = the domain is drained
+  const lwse_node_rec* nodes;
+  uint8_t* mask;           // n_nodes bytes
+  uint32_t n_nodes, n_domains;
+};
+
+__global__ void __launch_bounds__(256) drain_domain_mask_kernel(const DrainDomainMaskArgs a) {
+  for (uint32_t n = blockIdx.x * blockDim.x + threadIdx.x; n < a.n_nodes; n += gridDim.x * blockDim.x) {
+    const uint32_t d = __ldg(&a.nodes[n].domain_id);
+    a.mask[n] = (d < a.n_domains && __ldg(a.domains + d)) ? 1u : 0u;
+  }
+}
+
+int launch_drain_domain_mask(const uint8_t* d_domains, uint32_t n_domains, const lwse_node_rec* d_nodes, uint32_t n_nodes,
+                             uint8_t* d_mask, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  const DrainDomainMaskArgs a{d_domains, d_nodes, d_mask, n_nodes, n_domains};
+  drain_domain_mask_kernel<<<grid_for(n_nodes, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(a);
+  return launched_or_fail(1, cuda_err);
+}
+
+// The set form: one warp per LWS row over its group range, the what-if rows against the baseline.
+struct DrainBudgetArgs {
+  const lwse_lws_rec* lws;
+  const lwse_lws_out* lws_out;   // the baseline
+  const lwse_group_rec* groups;  // lws_index of every row
+  const lwse_group_out* before;  // the baseline
+  const lwse_group_out* after;   // the what-if's sweep
+  lwse_drain_budget* rows;
+  uint32_t* counts;  // [8] touched (the append cursor) [9] breached [10] loses available [11] already below
+  uint32_t capacity, n_lws, n_groups;
+};
+
+__global__ void __launch_bounds__(256) drain_budget_kernel(const DrainBudgetArgs a) {
+  constexpr uint32_t kFull = 0xFFFFFFFFu;
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t n_warps = gridDim.x * (blockDim.x / 32);
+  uint32_t breached = 0, loses = 0, below = 0;  // lane 0's
+  for (uint32_t L = (blockIdx.x * blockDim.x + threadIdx.x) / 32; L < a.n_lws; L += n_warps) {
+    const LwsBudget b = budget_of(a.lws, a.lws_out, L, a.n_groups);
+    uint32_t restarted = 0, lost = 0, lost_nb = 0;
+    for (uint32_t i = lane; i < b.gcount; i += 32) {
+      const uint32_t g = b.gbase + i;
+      if (__ldg(&a.groups[g].lws_index) != L) continue;
+      const uint32_t o = __ldcg(&a.before[g].flags), v = __ldcg(&a.after[g].flags);
+      if (!(o & kRestartBits) && (v & kRestartBits)) {
+        restarted++;
+        if (o & LWSE_GOUT_COND_READY) {
+          lost++;
+          if ((int64_t)i < b.replicas) lost_nb++;
+        }
+      }
+    }
+    restarted = __reduce_add_sync(kFull, restarted);
+    lost = __reduce_add_sync(kFull, lost);
+    lost_nb = __reduce_add_sync(kFull, lost_nb);
+    if (lane != 0) continue;
+    const int32_t after = clamp_i32((int64_t)b.ready_before - lost);
+    uint32_t flags = 0;
+    if (!b.evaluated) {
+      flags = LWSE_DRAINB_NOT_EVALUATED;
+    } else {
+      if (b.ready_before < b.floor) flags |= LWSE_DRAINB_ALREADY_BELOW;
+      if (lost > 0 && after < b.floor) flags |= LWSE_DRAINB_BREACHED;
+      if (b.available && lost_nb > 0) flags |= LWSE_DRAINB_LOSES_AVAILABLE;
+      below += (flags & LWSE_DRAINB_ALREADY_BELOW) ? 1u : 0u;
+    }
+    if (restarted == 0) continue;
+    breached += (flags & LWSE_DRAINB_BREACHED) ? 1u : 0u;
+    loses += (flags & LWSE_DRAINB_LOSES_AVAILABLE) ? 1u : 0u;
+    const uint32_t at = atomicAdd(a.counts + 8, 1u);
+    if (at < a.capacity) {
+      uint4* out = reinterpret_cast<uint4*>(a.rows + at);
+      out[0] = make_uint4(L, flags, (uint32_t)b.replicas, (uint32_t)b.floor);
+      out[1] = make_uint4((uint32_t)b.ready_before, (uint32_t)after, restarted, 0u);
+    }
+  }
+  if (lane == 0 && breached) atomicAdd(a.counts + 9, breached);
+  if (lane == 0 && loses) atomicAdd(a.counts + 10, loses);
+  if (lane == 0 && below) atomicAdd(a.counts + 11, below);
+}
+
+int launch_drain_budget(const lwse_lws_rec* d_lws, const lwse_lws_out* d_lws_out, uint32_t n_lws, const lwse_group_rec* d_groups,
+                        const lwse_group_out* d_before, const lwse_group_out* d_after, uint32_t n_groups,
+                        lwse_drain_budget* d_rows, uint32_t capacity, uint32_t* d_counts, int sm_count, cudaStream_t s,
+                        int* cuda_err) {
+  *cuda_err = 0;
+  if (n_lws == 0) return 0;
+  const DrainBudgetArgs a{d_lws, d_lws_out, d_groups, d_before, d_after, d_rows, d_counts, capacity, n_lws, n_groups};
+  drain_budget_kernel<<<grid_for(n_lws, 256 / 32, (uint32_t)sm_count * 8u), 256, 0, s>>>(a);
+  return launched_or_fail(1, cuda_err);
+}
+
+// The per-key form.  The walk is drain_cost_kernel's with the restart node mapped to its key (the node, or
+// its domain); the first pass adds the cost totals and counts the (group, key) pairs of groups that belong
+// to their LWS row, the second inserts those pairs into an (LWS, key) table, and the finish pass turns
+// every table entry into its key's budget columns.
+struct DrainBudgetCostArgs {
+  const lwse_lws_rec* lws;
+  const lwse_lws_out* lws_out;
+  const lwse_group_rec* groups;
+  const uint8_t* pod_state;
+  const lwse_pod_ident* pod_ident;
+  const lwse_group_out* baseline;
+  const lwse_node_rec* nodes;    // scope DOMAINS: key = nodes[node].domain_id when < n_domains; null: key = node
+  lwse_drain_budget_cost* cost;  // n_keys rows
+  unsigned long long* keys;      // the table: LWS row << 32 | key, kEmptyKey when free
+  uint4* vals;                   // {groups restarted, ready groups restarted, of those with index < replicas, 0}
+  uint32_t* counts;              // [0..1] pairs (u64), [2] refused inserts
+  uint64_t n_pods;
+  uint32_t n_lws, n_groups, n_nodes, n_domains, table_mask;
+};
+
+constexpr unsigned long long kEmptyKey = ~0ull;
+
+__device__ __forceinline__ uint32_t key_of_node(const DrainBudgetCostArgs& a, uint32_t node) {
+  if (node >= a.n_nodes) return LWSE_NONE;
+  if (!a.nodes) return node;
+  const uint32_t d = __ldg(&a.nodes[node].domain_id);
+  return d < a.n_domains ? d : LWSE_NONE;
+}
+
+__device__ __forceinline__ uint32_t restart_key(const DrainBudgetCostArgs& a, const VisitCtx& ctx, uint32_t p, bool valid) {
+  if (!valid) return LWSE_NONE;
+  const uint4 id = ldg_stream(a.pod_ident + p);
+  const uint32_t node = id.w >> LWSE_PODID_NODE_SHIFT;
+  if (!(id.w & LWSE_PODID_SCHEDULED) || node >= a.n_nodes) return LWSE_NONE;
+  bool cand;
+  (void)visit_pod(ctx, (uint32_t)__ldg(a.pod_state + p) | LWSE_POD_DELETING, id, cand);
+  return cand ? key_of_node(a, node) : LWSE_NONE;
+}
+
+__device__ __forceinline__ uint32_t table_slot(unsigned long long k, uint32_t mask) {
+  k ^= k >> 33;
+  k *= 0xFF51AFD7ED558CCDull;
+  k ^= k >> 33;
+  return (uint32_t)k & mask;
+}
+
+__device__ __forceinline__ void table_add(const DrainBudgetCostArgs& a, unsigned long long k, uint32_t ready, uint32_t ready_nb) {
+  uint32_t h = table_slot(k, a.table_mask);
+  for (uint32_t probe = 0; probe <= a.table_mask; probe++, h = (h + 1u) & a.table_mask) {
+    const unsigned long long prev = atomicCAS(a.keys + h, kEmptyKey, k);
+    if (prev == kEmptyKey || prev == k) {
+      atomicAdd(&a.vals[h].x, 1u);
+      if (ready) atomicAdd(&a.vals[h].y, 1u);
+      if (ready_nb) atomicAdd(&a.vals[h].z, 1u);
+      return;
+    }
+  }
+  atomicAdd(a.counts + 2, 1u);  // full: the call fails
+}
+
+template <bool kInsert>
+__global__ void __launch_bounds__(kCostThreads) drain_budget_walk_kernel(const DrainBudgetCostArgs a) {
+  __shared__ uint32_t s_list[kCostThreads / 32][kCostList];
+  constexpr uint32_t kFull = 0xFFFFFFFFu;
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const uint32_t lt = (1u << lane) - 1u;
+  uint32_t* list = s_list[warp];
+  const uint32_t n_warps = gridDim.x * (kCostThreads / 32);
+  unsigned long long pairs = 0;
+  for (uint32_t g = blockIdx.x * (kCostThreads / 32) + warp; g < a.n_groups; g += n_warps) {
+    const uint4* row = reinterpret_cast<const uint4*>(a.groups + g);
+    const uint4 ca = ldg_stream(row + 0), cb = ldg_stream(row + 1), cc = ldg_stream(row + 2), cd = ldg_stream(row + 3);
+    const uint32_t leader_node = cc.y, pod_base = cc.z, pod_count = cc.w, lws_index = cd.x;
+    if (!kInsert && lane == 0) {
+      const uint32_t lk = key_of_node(a, leader_node);
+      if (lk != LWSE_NONE) atomicAdd(&a.cost[lk].leaders, 1u);
+    }
+    if (lws_index >= a.n_lws || (uint64_t)pod_base + pod_count > a.n_pods || pod_count == 0) continue;
+    const uint32_t before = __ldcs(&a.baseline[g].flags);
+    if (before & kRestartBits) continue;
+    const uint4 L = ldg_cached(a.lws + lws_index);
+    const uint32_t lflags = L.w;
+    if (!restart_policy_on(lflags)) continue;
+    bool pending = (uint32_t)(int32_t)L.z != pod_count;
+    if (!pending && restart_suppressed(true, lflags)) {
+      for (uint32_t i0 = 0; i0 < pod_count && !pending; i0 += 32) {
+        const uint32_t st = i0 + lane < pod_count ? (uint32_t)__ldg(a.pod_state + pod_base + i0 + lane) : 0u;
+        pending = __any_sync(kFull, (st & LWSE_POD_PHASE_MASK) == LWSE_POD_PHASE_PENDING);
+      }
+    }
+    if (restart_suppressed(pending, lflags)) continue;
+    // the group belongs to its LWS row when the row's range is inside the table and holds g
+    const uint4* lrow = reinterpret_cast<const uint4*>(a.lws + lws_index);
+    const uint4 l1 = ldg_cached(lrow + 1), l3 = ldg_cached(lrow + 3);
+    const uint32_t index = g - l3.z;
+    const bool member = (uint64_t)l3.z + l3.w <= a.n_groups && g >= l3.z && index < l3.w;
+    if (kInsert && !member) continue;
+    VisitCtx ctx;
+    visit_ctx_of(ctx, ca, cb, cc, cd);
+    const bool ready = (before & LWSE_GOUT_COND_READY) != 0u;
+    const bool ready_nb = ready && (int64_t)index < (int64_t)(int32_t)l1.x;
+    uint32_t n_list = 0;
+    bool listed = true;
+    for (uint32_t b0 = 0; b0 < pod_count; b0 += 32) {
+      const uint32_t key = restart_key(a, ctx, pod_base + b0 + lane, b0 + lane < pod_count);
+      const uint32_t peers = __match_any_sync(kFull, key);
+      bool fresh = key != LWSE_NONE && lane == (uint32_t)(__ffs(peers) - 1);
+      if (listed) {
+        for (uint32_t j = 0; j < n_list; j++) fresh &= list[j] != key;
+        const uint32_t add = __ballot_sync(kFull, fresh);
+        if (n_list + (uint32_t)__popc(add) <= kCostList) {
+          __syncwarp();
+          if (fresh) list[n_list + (uint32_t)__popc(add & lt)] = key;
+          __syncwarp();
+          n_list += (uint32_t)__popc(add);
+        } else {
+          listed = false;
+        }
+      }
+      if (!listed) {
+        for (uint32_t e0 = 0; e0 < b0; e0 += 32) {
+          const uint32_t k2 = restart_key(a, ctx, pod_base + e0 + lane, true);
+          for (int j = 0; j < 32; j++) fresh &= __shfl_sync(kFull, k2, j) != key;
+        }
+      }
+      if (!fresh) continue;
+      if (kInsert) {
+        table_add(a, (unsigned long long)lws_index << 32 | key, ready, ready_nb);
+      } else {
+        lwse_drain_budget_cost* c = a.cost + key;
+        atomicAdd(&c->groups_restarted, 1u);
+        if (ready) atomicAdd(&c->ready_restarted, 1u);
+        atomicAdd(reinterpret_cast<unsigned long long*>(&c->pods_recreated), (unsigned long long)pod_count);
+        pairs += member ? 1u : 0u;
+      }
+    }
+  }
+  if (!kInsert) {
+    pairs = warp_sum_u64(pairs);
+    if (lane == 0 && pairs) atomicAdd(reinterpret_cast<unsigned long long*>(a.counts), pairs);
+  }
+}
+
+// Every key row starts as {pods of its nodes, zeros, min_margin = INT32_MAX}; `cost` is zeroed by the caller.
+__global__ void __launch_bounds__(256) drain_budget_keys_init_kernel(const DrainBudgetCostArgs a, const uint32_t* occupancy,
+                                                                     uint32_t n_keys) {
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_keys || i < a.n_nodes; i += stride) {
+    if (i < n_keys) a.cost[i].min_margin = INT32_MAX;
+    if (i < a.n_nodes) {
+      const uint32_t k = key_of_node(a, i), pods = __ldg(occupancy + i);
+      if (k != LWSE_NONE && pods) atomicAdd(&a.cost[k].pods, pods);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) drain_budget_finish_kernel(const DrainBudgetCostArgs a) {
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t h = blockIdx.x * blockDim.x + threadIdx.x; h <= a.table_mask; h += stride) {
+    const unsigned long long k = a.keys[h];
+    if (k == kEmptyKey) continue;
+    const uint32_t L = (uint32_t)(k >> 32), key = (uint32_t)k;
+    const uint4 v = a.vals[h];
+    lwse_drain_budget_cost* c = a.cost + key;
+    atomicAdd(&c->lws_touched, 1u);
+    const LwsBudget b = budget_of(a.lws, a.lws_out, L, a.n_groups);
+    if (!b.evaluated) continue;
+    const int64_t after = (int64_t)b.ready_before - v.y;
+    if (v.y > 0 && after < b.floor) atomicAdd(&c->lws_breached, 1u);
+    if (b.available && v.z > 0) atomicAdd(&c->lws_loses_available, 1u);
+    atomicMin(&c->min_margin, clamp_i32((int64_t)clamp_i32(after) - b.floor));
+  }
+}
+
+int launch_drain_budget_cost(const DrainBudgetCostLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  const DrainBudgetCostArgs a{p->lws, p->lws_out, p->groups, p->pod_state, p->pod_ident, p->baseline,
+                              p->by_domain ? p->nodes : nullptr, p->cost, p->keys, p->vals, p->counts,
+                              p->n_pods, p->n_lws, p->n_groups, p->n_nodes, p->n_domains, p->table_mask};
+  const unsigned walk_grid = grid_for(p->n_groups, kCostThreads / 32, (uint32_t)sm_count * 8u);
+  switch (pass) {
+    case 0: {
+      const uint32_t n = p->n_keys > p->n_nodes ? p->n_keys : p->n_nodes;
+      drain_budget_keys_init_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(a, p->occupancy, p->n_keys);
+      if (p->n_groups) drain_budget_walk_kernel<false><<<walk_grid, kCostThreads, 0, s>>>(a);
+      return launched_or_fail(p->n_groups ? 2 : 1, cuda_err);
+    }
+    default:
+      drain_budget_walk_kernel<true><<<walk_grid, kCostThreads, 0, s>>>(a);
+      drain_budget_finish_kernel<<<grid_for((uint64_t)p->table_mask + 1, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(a);
+      return launched_or_fail(2, cuda_err);
+  }
 }
 
 }  // namespace lwse

@@ -225,6 +225,9 @@ struct lwse_engine {
   // drain what-if / drain cost (lwse_resident_drain_*): on the what-if stream, copies of the state column and the
   // group rows, the sweep's bitmaps and group rows, the node mask, the change list and the cost rows
   DevBuf dr_state, dr_groups, dr_out, dr_scan, dr_mask, dr_list, dr_cost;
+  // drain budget (lwse_resident_drain_budget*): the domain mask, the touched rows, the key rows, the (LWS, key)
+  // table and its counters
+  DevBuf dr_domains, dr_brows, dr_bcost, dr_table, dr_bwords;
   uint32_t r_sweep_flags = 0;        // LWSE_SWEEP_GANG of the most recently submitted sweep (r_group_out's flags)
   DevBuf sha_bytes, sha_offsets, sha_digests, sha_ints;
   uint32_t* h_rounds = nullptr;  // pinned
@@ -443,7 +446,8 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->lf_lws, &e->lf_group_out, &e->lf_slot_off, &e->lf_slots, &e->lf_fc, &e->lf_steps, &e->lf_totals,
                       &e->wf_nodes, &e->wf_reqs, &e->wf_out, &e->wf_dom_first, &e->wf_node_order, &e->wf_node_pos,
                       &e->wf_node_ix, &e->wf_touched, &e->wf_round, &e->wf_list,
-                      &e->dr_state, &e->dr_groups, &e->dr_out, &e->dr_scan, &e->dr_mask, &e->dr_list, &e->dr_cost};
+                      &e->dr_state, &e->dr_groups, &e->dr_out, &e->dr_scan, &e->dr_mask, &e->dr_list, &e->dr_cost,
+                      &e->dr_domains, &e->dr_brows, &e->dr_bcost, &e->dr_table, &e->dr_bwords};
     if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
     if (e->lf_stream) cudaStreamSynchronize(e->lf_stream);
     if (e->wf_stream) cudaStreamSynchronize(e->wf_stream);
@@ -2448,43 +2452,31 @@ static int drain_end_locked(lwse_engine* e) {
   return LWSE_OK;
 }
 
-// Copies of the state column and the group rows, the mark kernel on them, the sweep's group pass over
-// {resident LWS rows, copied groups, copied states, resident identity rows} into rows of its own (the LWS
-// pass is skipped: it reads only flag bits eviction does not change), then the diff against the baseline.
-LWSE_API int lwse_resident_drain_whatif(lwse_engine* e, lwse_drain_whatif* q) {
-  if (!e || !q) return LWSE_ERR_INVALID_ARG;
-  std::lock_guard<std::mutex> lock(e->mu);
-  if (!e->r_loaded || e->n_nodes == 0 || !e->r_groups_swept) return LWSE_ERR_NOT_READY;
-  if ((q->n_nodes && !q->nodes) || (q->capacity && (!q->rows || !q->before || !q->after))) return LWSE_ERR_INVALID_ARG;
-  for (uint32_t i = 0; i < q->n_nodes; i++)
-    if (q->nodes[i] >= e->n_nodes) return LWSE_ERR_INVALID_ARG;
-  const uint32_t ng = e->rn_groups, nn = e->n_nodes;
+// The scratch of the what-if's sweep (lwse_resident_drain_whatif and the set form of the drain budget).
+static int reserve_drain_sweep(lwse_engine* e) {
+  const uint32_t ng = e->rn_groups;
   const uint64_t np = e->rn_pods;
-  const uint32_t list_cap = q->capacity < ng ? q->capacity : ng;  // (at most ng rows can differ)
-  DeviceGuard guard(e->device);
-  LWSE_CUDA(e, e->wf_stage.reserve((size_t)nn));  // (the previous what-if synchronized its stream: free)
+  LWSE_CUDA(e, e->wf_stage.reserve((size_t)e->n_nodes));  // (the previous what-if synchronized its stream: free)
   LWSE_CUDA(e, e->wf_words.reserve(64));
   LWSE_CUDA(e, e->dr_state.reserve((size_t)np + 16));
   LWSE_CUDA(e, e->dr_groups.reserve((size_t)ng * sizeof(lwse_group_rec) + 16));
   LWSE_CUDA(e, e->dr_out.reserve((size_t)ng * sizeof(lwse_group_out) + 16));
   LWSE_CUDA(e, e->dr_scan.reserve(lwse::lws_sweep_scratch_bytes(np, ng)));
-  LWSE_CUDA(e, e->dr_mask.reserve((size_t)nn + 16));
-  // (layout: [counts: 16 words] [rows: list_cap] [before: list_cap] [after: list_cap], the 16-byte rows aligned)
-  const size_t rows_bytes = ((size_t)list_cap * 4 + 15) & ~(size_t)15;
-  LWSE_CUDA(e, e->dr_list.reserve(64 + rows_bytes + (size_t)list_cap * 2 * sizeof(lwse_group_out)));
-  uint8_t* mask = static_cast<uint8_t*>(e->wf_stage.h);
-  memset(mask, 0, nn);
-  for (uint32_t i = 0; i < q->n_nodes; i++) mask[q->nodes[i]] = 1;
-  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, e->dr_mask.reserve((size_t)e->n_nodes + 16));
+  return LWSE_OK;
+}
+
+// Copies of the state column and the group rows, the mark kernel on them (the node mask in dr_mask), the
+// sweep's group pass over {resident LWS rows, copied groups, copied states, resident identity rows} into
+// dr_out (the LWS pass is skipped: it reads only flag bits eviction does not change), then the diff against
+// the baseline; on wf_stream, after the caller zeroed the 16 counters at d_counts.
+static int enqueue_drain_sweep(lwse_engine* e, uint32_t* d_counts, uint32_t* d_rows, lwse_group_out* d_before,
+                               lwse_group_out* d_after, uint32_t list_cap) {
+  const uint32_t ng = e->rn_groups, nn = e->n_nodes;
+  const uint64_t np = e->rn_pods;
   cudaStream_t s = e->wf_stream;
-  uint32_t* d_counts = (uint32_t*)e->dr_list.p;
-  uint32_t* d_rows = d_counts + 16;
-  lwse_group_out* d_before = reinterpret_cast<lwse_group_out*>(static_cast<uint8_t*>(e->dr_list.p) + 64 + rows_bytes);
-  lwse_group_out* d_after = d_before + list_cap;
   if (np) LWSE_CUDA(e, cudaMemcpyAsync(e->dr_state.p, e->r_pst.p, (size_t)np, cudaMemcpyDeviceToDevice, s));
   if (ng) LWSE_CUDA(e, cudaMemcpyAsync(e->dr_groups.p, e->r_groups.p, (size_t)ng * sizeof(lwse_group_rec), cudaMemcpyDeviceToDevice, s));
-  LWSE_CUDA(e, cudaMemcpyAsync(e->dr_mask.p, mask, nn, cudaMemcpyHostToDevice, s));
-  LWSE_CUDA(e, cudaMemsetAsync(d_counts, 0, 64, s));
   int cuda_err = 0;
   int launched = lwse::launch_drain_mark((const uint8_t*)e->dr_mask.p, nn, (const lwse_pod_ident*)e->r_pid.p, (uint8_t*)e->dr_state.p,
                                          np, (lwse_group_rec*)e->dr_groups.p, ng, d_counts, e->sm_count, s, &cuda_err);
@@ -2505,7 +2497,35 @@ LWSE_API int lwse_resident_drain_whatif(lwse_engine* e, lwse_drain_whatif* q) {
   launched = lwse::launch_drain_diff((const lwse_group_out*)e->r_group_out.p, (const lwse_group_out*)e->dr_out.p,
                                      (const lwse_group_rec*)e->r_groups.p, ng, d_rows, d_before, d_after, list_cap, d_counts,
                                      e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  return count_launch(e, launched, cuda_err);
+}
+
+LWSE_API int lwse_resident_drain_whatif(lwse_engine* e, lwse_drain_whatif* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->r_loaded || e->n_nodes == 0 || !e->r_groups_swept) return LWSE_ERR_NOT_READY;
+  if ((q->n_nodes && !q->nodes) || (q->capacity && (!q->rows || !q->before || !q->after))) return LWSE_ERR_INVALID_ARG;
+  for (uint32_t i = 0; i < q->n_nodes; i++)
+    if (q->nodes[i] >= e->n_nodes) return LWSE_ERR_INVALID_ARG;
+  const uint32_t ng = e->rn_groups, nn = e->n_nodes;
+  const uint32_t list_cap = q->capacity < ng ? q->capacity : ng;  // (at most ng rows can differ)
+  DeviceGuard guard(e->device);
+  if (const int rc = reserve_drain_sweep(e); rc != LWSE_OK) return rc;
+  // (layout: [counts: 16 words] [rows: list_cap] [before: list_cap] [after: list_cap], the 16-byte rows aligned)
+  const size_t rows_bytes = ((size_t)list_cap * 4 + 15) & ~(size_t)15;
+  LWSE_CUDA(e, e->dr_list.reserve(64 + rows_bytes + (size_t)list_cap * 2 * sizeof(lwse_group_out)));
+  uint8_t* mask = static_cast<uint8_t*>(e->wf_stage.h);
+  memset(mask, 0, nn);
+  for (uint32_t i = 0; i < q->n_nodes; i++) mask[q->nodes[i]] = 1;
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* d_counts = (uint32_t*)e->dr_list.p;
+  uint32_t* d_rows = d_counts + 16;
+  lwse_group_out* d_before = reinterpret_cast<lwse_group_out*>(static_cast<uint8_t*>(e->dr_list.p) + 64 + rows_bytes);
+  lwse_group_out* d_after = d_before + list_cap;
+  LWSE_CUDA(e, cudaMemcpyAsync(e->dr_mask.p, mask, nn, cudaMemcpyHostToDevice, s));
+  LWSE_CUDA(e, cudaMemsetAsync(d_counts, 0, 64, s));
+  if (const int rc = enqueue_drain_sweep(e, d_counts, d_rows, d_before, d_after, list_cap); rc != LWSE_OK) return rc;
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_counts, 32, cudaMemcpyDeviceToHost, s));
@@ -2553,6 +2573,147 @@ LWSE_API int lwse_resident_drain_cost(lwse_engine* e, lwse_drain_cost* out) {
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(out, d_cost, (size_t)nn * sizeof(lwse_drain_cost), cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
+  return LWSE_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Drain budget
+// ---------------------------------------------------------------------------
+static bool drain_budget_ready(const lwse_engine* e) {
+  return e->r_loaded && e->n_nodes != 0 && e->r_groups_swept && e->r_swept;
+}
+
+// The set form: the drain what-if's sweep over the node mask (the given node rows, or the nodes of the given
+// domains, built on the device), the diff's totals without a change list, then drain_budget_kernel over
+// every LWS row.
+LWSE_API int lwse_resident_drain_budget(lwse_engine* e, lwse_drain_budget_query* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!drain_budget_ready(e)) return LWSE_ERR_NOT_READY;
+  if (q->scope != LWSE_DRAIN_NODES && q->scope != LWSE_DRAIN_DOMAINS) return LWSE_ERR_INVALID_ARG;
+  if ((q->n_ids && !q->ids) || (q->capacity && !q->rows)) return LWSE_ERR_INVALID_ARG;
+  const bool by_domain = q->scope == LWSE_DRAIN_DOMAINS;
+  const uint32_t nn = e->n_nodes, nd = e->n_domains, n_keys = by_domain ? nd : nn;
+  for (uint32_t i = 0; i < q->n_ids; i++)
+    if (q->ids[i] >= n_keys) return LWSE_ERR_INVALID_ARG;
+  const uint32_t nl = e->rn_lws;
+  const uint32_t list_cap = q->capacity < nl ? q->capacity : nl;
+  DeviceGuard guard(e->device);
+  if (const int rc = reserve_drain_sweep(e); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, e->wf_stage.reserve((size_t)n_keys));
+  LWSE_CUDA(e, e->dr_list.reserve(64));
+  LWSE_CUDA(e, e->dr_brows.reserve((size_t)list_cap * sizeof(lwse_drain_budget) + 16));
+  if (by_domain) LWSE_CUDA(e, e->dr_domains.reserve((size_t)nd + 16));
+  uint8_t* mask = static_cast<uint8_t*>(e->wf_stage.h);
+  memset(mask, 0, n_keys);
+  for (uint32_t i = 0; i < q->n_ids; i++) mask[q->ids[i]] = 1;
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* d_counts = (uint32_t*)e->dr_list.p;
+  lwse_drain_budget* d_rows = (lwse_drain_budget*)e->dr_brows.p;
+  int cuda_err = 0;
+  if (by_domain) {
+    if (nd) LWSE_CUDA(e, cudaMemcpyAsync(e->dr_domains.p, mask, nd, cudaMemcpyHostToDevice, s));
+    const int launched = lwse::launch_drain_domain_mask((const uint8_t*)e->dr_domains.p, nd, (const lwse_node_rec*)e->nodes.p, nn,
+                                                        (uint8_t*)e->dr_mask.p, e->sm_count, s, &cuda_err);
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  } else {
+    LWSE_CUDA(e, cudaMemcpyAsync(e->dr_mask.p, mask, nn, cudaMemcpyHostToDevice, s));
+  }
+  LWSE_CUDA(e, cudaMemsetAsync(d_counts, 0, 64, s));
+  if (const int rc = enqueue_drain_sweep(e, d_counts, nullptr, nullptr, nullptr, 0); rc != LWSE_OK) return rc;
+  const int launched = lwse::launch_drain_budget((const lwse_lws_rec*)e->r_lws.p, (const lwse_lws_out*)e->r_lws_out.p, nl,
+                                                 (const lwse_group_rec*)e->r_groups.p, (const lwse_group_out*)e->r_group_out.p,
+                                                 (const lwse_group_out*)e->dr_out.p, e->rn_groups, d_rows, list_cap, d_counts,
+                                                 e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_counts, 64, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint32_t n_touched = words[8];
+  const uint32_t listed = n_touched < list_cap ? n_touched : list_cap;
+  if (listed) {
+    LWSE_CUDA(e, cudaMemcpyAsync(q->rows, d_rows, (size_t)listed * sizeof(lwse_drain_budget), cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaStreamSynchronize(s));
+  }
+  q->n_touched = n_touched;
+  q->n_breached = words[9];
+  q->n_loses_available = words[10];
+  q->n_already_below = words[11];
+  q->n_pods_evicted = words[1];
+  q->n_leaders_evicted = words[2];
+  q->n_groups_restarted = words[3];
+  q->n_ready_restarted = words[4];
+  uint64_t recreated = 0;
+  memcpy(&recreated, words + 6, 8);
+  q->n_pods_recreated = recreated;
+  return LWSE_OK;
+}
+
+// The per-key form: the key rows and the pair count (pass 0), one host synchronisation to size the (LWS, key)
+// table from that count (a power of two at least twice it, so linear probing always finds a slot), then the
+// table and the key rows' budget columns (pass 1).
+LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lwse_drain_budget_cost* out) {
+  if (!e) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!drain_budget_ready(e)) return LWSE_ERR_NOT_READY;
+  if (!out || (scope != LWSE_DRAIN_NODES && scope != LWSE_DRAIN_DOMAINS)) return LWSE_ERR_INVALID_ARG;
+  const bool by_domain = scope == LWSE_DRAIN_DOMAINS;
+  const uint32_t nn = e->n_nodes, n_keys = by_domain ? e->n_domains : nn;
+  const size_t cost_bytes = (size_t)n_keys * sizeof(lwse_drain_budget_cost);
+  DeviceGuard guard(e->device);
+  LWSE_CUDA(e, e->dr_bcost.reserve(cost_bytes + 16));
+  LWSE_CUDA(e, e->dr_bwords.reserve(64));
+  LWSE_CUDA(e, e->wf_words.reserve(64));
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  lwse::DrainBudgetCostLaunch p{};
+  p.lws = (const lwse_lws_rec*)e->r_lws.p;
+  p.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
+  p.groups = (const lwse_group_rec*)e->r_groups.p;
+  p.pod_state = (const uint8_t*)e->r_pst.p;
+  p.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
+  p.baseline = (const lwse_group_out*)e->r_group_out.p;
+  p.nodes = (const lwse_node_rec*)e->nodes.p;
+  p.occupancy = (const uint32_t*)e->r_occ.p;
+  p.cost = (lwse_drain_budget_cost*)e->dr_bcost.p;
+  p.counts = (uint32_t*)e->dr_bwords.p;
+  p.n_pods = e->rn_pods;
+  p.n_lws = e->rn_lws;
+  p.n_groups = e->rn_groups;
+  p.n_nodes = nn;
+  p.n_domains = e->n_domains;
+  p.n_keys = n_keys;
+  p.by_domain = by_domain;
+  LWSE_CUDA(e, cudaMemsetAsync(p.cost, 0, cost_bytes, s));
+  LWSE_CUDA(e, cudaMemsetAsync(p.counts, 0, 64, s));
+  int cuda_err = 0;
+  int launched = lwse::launch_drain_budget_cost(&p, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 16, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  uint64_t pairs = 0;
+  memcpy(&pairs, words, 8);
+  if (pairs) {
+    if (pairs > (1ull << 30)) return LWSE_ERR_OOM;  // (the table index is 32-bit)
+    uint64_t slots = 256;
+    while (slots < 2 * pairs) slots <<= 1;
+    LWSE_CUDA(e, e->dr_table.reserve((size_t)slots * (sizeof(unsigned long long) + sizeof(uint4))));
+    p.keys = (unsigned long long*)e->dr_table.p;
+    p.vals = reinterpret_cast<uint4*>(p.keys + slots);
+    p.table_mask = (uint32_t)(slots - 1);
+    LWSE_CUDA(e, cudaMemsetAsync(p.keys, 0xFF, (size_t)slots * sizeof(unsigned long long), s));
+    LWSE_CUDA(e, cudaMemsetAsync(p.vals, 0, (size_t)slots * sizeof(uint4), s));
+    launched = lwse::launch_drain_budget_cost(&p, 1, e->sm_count, s, &cuda_err);
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  }
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  if (n_keys) LWSE_CUDA(e, cudaMemcpyAsync(out, p.cost, cost_bytes, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 16, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  if (words[2]) return LWSE_ERR_OOM;  // an insert the table refused: no answer rather than a wrong one
   return LWSE_OK;
 }
 

@@ -192,6 +192,37 @@ int launch_drain_diff(const lwse_group_out* d_before, const lwse_group_out* d_af
 int launch_drain_cost(const lwse_lws_rec* d_lws, uint32_t n_lws, const lwse_group_rec* d_groups, uint32_t n_groups,
                       const uint8_t* d_state, const lwse_pod_ident* d_ident, uint64_t n_pods, const lwse_group_out* d_baseline,
                       lwse_drain_cost* d_cost, uint32_t n_nodes, int sm_count, cudaStream_t s, int* cuda_err);
+// The node mask of a set of domains (d_domains: n_domains bytes, 1 = drained) into d_mask (n_nodes bytes).
+int launch_drain_domain_mask(const uint8_t* d_domains, uint32_t n_domains, const lwse_node_rec* d_nodes, uint32_t n_nodes,
+                             uint8_t* d_mask, int sm_count, cudaStream_t s, int* cuda_err);
+// The drain budget's set form over a what-if sweep (d_after) against the baseline: touched rows appended to
+// d_rows (up to capacity); counters [8] touched [9] breached [10] loses available [11] already below.
+int launch_drain_budget(const lwse_lws_rec* d_lws, const lwse_lws_out* d_lws_out, uint32_t n_lws, const lwse_group_rec* d_groups,
+                        const lwse_group_out* d_before, const lwse_group_out* d_after, uint32_t n_groups,
+                        lwse_drain_budget* d_rows, uint32_t capacity, uint32_t* d_counts, int sm_count, cudaStream_t s,
+                        int* cuda_err);
+// The drain budget's per-key form.  Pass 0: the key rows (cost zeroed by the caller) get their pods and cost
+// totals, and counts[0..1] (u64, zeroed by the caller) the (group, key) pairs the table must hold.  Pass 1
+// (keys all-ones and vals zeroed by the caller, table_mask + 1 a power of two > the pairs): the (LWS, key)
+// table, then the budget columns of the key rows; counts[2] = inserts the table refused.
+struct DrainBudgetCostLaunch {
+  const lwse_lws_rec* lws;
+  const lwse_lws_out* lws_out;
+  const lwse_group_rec* groups;
+  const uint8_t* pod_state;
+  const lwse_pod_ident* pod_ident;
+  const lwse_group_out* baseline;
+  const lwse_node_rec* nodes;
+  const uint32_t* occupancy;
+  lwse_drain_budget_cost* cost;
+  unsigned long long* keys;
+  uint4* vals;
+  uint32_t* counts;
+  uint64_t n_pods;
+  uint32_t n_lws, n_groups, n_nodes, n_domains, n_keys, table_mask;
+  bool by_domain;
+};
+int launch_drain_budget_cost(const DrainBudgetCostLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
 
 // ---- lwse_sha1_kernels.cu ----
 int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,

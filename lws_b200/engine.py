@@ -46,6 +46,8 @@ SYMBOLS = {
     "lwse_resident_place_whatif": ([C.c_void_p, C.POINTER(R.PlaceWhatIf)], C.c_int),
     "lwse_resident_drain_whatif": ([C.c_void_p, C.POINTER(R.DrainWhatIf)], C.c_int),
     "lwse_resident_drain_cost": ([C.c_void_p, C.c_void_p], C.c_int),
+    "lwse_resident_drain_budget": ([C.c_void_p, C.POINTER(R.DrainBudgetQuery)], C.c_int),
+    "lwse_resident_drain_budget_cost": ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_place_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
         C.c_int,
@@ -461,6 +463,40 @@ class Engine:
         out = R.aligned_empty(max(self.n_nodes, 1), R.DRAIN_COST)
         self._check(lib().lwse_resident_drain_cost(self._h, R.ptr(out)))
         return out[: self.n_nodes]
+
+    _DRAIN_SCOPES = {"nodes": R.DRAIN_NODES, "domains": R.DRAIN_DOMAINS}
+
+    def resident_drain_budget(self, nodes=None, domains=None, capacity=None):
+        """lwse_resident_drain_budget: the LeaderWorkerSet rows a drain of the node rows ``nodes`` — or of every
+        node in the domain ids ``domains`` — touches, each with its availability floor, ready count before
+        and after, and ``records.DRAINB_*`` flags.  Give exactly one of the two.  ``capacity`` None lists every
+        touched row.  → dict: ``rows`` (``records.DRAIN_BUDGET``) and the totals of
+        ``records.DRAIN_BUDGET_TOTALS``."""
+        if (nodes is None) == (domains is None):
+            raise ValueError("give node rows or domain ids")
+        ids = np.ascontiguousarray(nodes if domains is None else domains, dtype=np.uint32)
+        n_res = getattr(self, "_resident_shape", (0, 0))[0]
+        cap = n_res if capacity is None else int(capacity)
+        rows = R.aligned_empty(max(cap, 1), R.DRAIN_BUDGET)
+        q = R.DrainBudgetQuery()
+        q.ids = R.ptr(ids) if len(ids) else None
+        q.n_ids = len(ids)
+        q.scope = R.DRAIN_NODES if domains is None else R.DRAIN_DOMAINS
+        q.capacity = cap
+        q.rows = R.ptr(rows)
+        self._check(lib().lwse_resident_drain_budget(self._h, C.byref(q)))
+        out = {"rows": rows[: min(q.n_touched, cap)]}
+        out.update({k: getattr(q, k) for k in R.DRAIN_BUDGET_TOTALS})
+        return out
+
+    def resident_drain_budget_cost(self, scope: str = "nodes") -> np.ndarray:
+        """lwse_resident_drain_budget_cost: one ``records.DRAIN_BUDGET_COST`` row per node (``scope="nodes"``) or
+        per domain (``"domains"``), row k holding the answer ``resident_drain_budget`` gives for that key alone
+        — every key in one call."""
+        n = self.n_nodes if scope == "nodes" else self.n_domains
+        out = R.aligned_empty(max(n, 1), R.DRAIN_BUDGET_COST)
+        self._check(lib().lwse_resident_drain_budget_cost(self._h, self._DRAIN_SCOPES[scope], R.ptr(out)))
+        return out[:n]
 
     def resident_patch(self, which: int, rows, values):
         """Overwrite rows of a resident table (rows: uint32 indices, values: packed rows)."""

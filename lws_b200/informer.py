@@ -541,6 +541,27 @@ class IncrementalEncoder:
         """The node rows of the named nodes, for ``Engine.resident_drain_whatif`` (sorted, each once)."""
         return np.array(sorted({self.node_index[n] for n in node_names}), dtype=np.uint32)
 
+    def whatif_drain_domains(self, topology_values) -> np.ndarray:
+        """The domain ids of the named topology values, for ``Engine.resident_drain_budget(domains=...)``
+        (sorted, each once).  A value no node row has carried is a KeyError."""
+        unknown = sorted({v for v in topology_values if v not in self._domain_ids})
+        if unknown:
+            raise KeyError(f"unknown topology values: {unknown}")
+        return np.array(sorted({self._domain_ids[v] for v in topology_values}), dtype=np.uint32)
+
+    def drain_budget_report(self, result: dict) -> list:
+        """The touched objects of a ``resident_drain_budget`` answer as dicts: ``namespace`` and ``name`` (None
+        for a row no object holds), then the row's fields, its ``records.DRAINB_*`` flags named."""
+        names = {R.DRAINB_NOT_EVALUATED: "not_evaluated", R.DRAINB_BREACHED: "breached",
+                 R.DRAINB_ALREADY_BELOW: "already_below", R.DRAINB_LOSES_AVAILABLE: "loses_available"}
+        out = []
+        for r in result["rows"]:
+            key = self.object_of_lws_row(int(r["lws"]))
+            out.append({"namespace": key[0] if key else None, "name": key[1] if key else None,
+                        **{f: int(r[f]) for f in R.DRAIN_BUDGET.names if f != "reserved"},
+                        "conditions": [n for bit, n in names.items() if int(r["flags"]) & bit]})
+        return out
+
     def drain_place_query(self, result: dict, node_names) -> list:
         """Segments for ``Engine.resident_place_whatif`` that ask where the groups a drain restarts would go:
         a NODES segment that cordons the drained nodes (``whatif_cordon``) and a PLACE_REQS segment that unpins

@@ -535,6 +535,54 @@ DRAIN_COST = np.dtype(
 )
 assert DRAIN_COST.itemsize == 32
 
+# drain budget (lwse_resident_drain_budget*): the drain set's scope and the flags of a touched LWS row
+DRAIN_NODES, DRAIN_DOMAINS = 0, 1
+DRAINB_NOT_EVALUATED = 1 << 0
+DRAINB_BREACHED = 1 << 1
+DRAINB_ALREADY_BELOW = 1 << 2
+DRAINB_LOSES_AVAILABLE = 1 << 3
+
+# lwse_drain_budget: one touched LWS row of a drain
+DRAIN_BUDGET = np.dtype(
+    [("lws", "<u4"), ("flags", "<u4"), ("replicas", "<i4"), ("floor", "<i4"), ("ready_before", "<i4"),
+     ("ready_after", "<i4"), ("groups_restarted", "<u4"), ("reserved", "<u4")],
+    align=False,
+)
+assert DRAIN_BUDGET.itemsize == 32
+
+# lwse_drain_budget_cost: per node or per domain, the DRAIN_COST totals and the budget columns
+DRAIN_BUDGET_COST = np.dtype(DRAIN_COST.descr + [("lws_touched", "<u4"), ("lws_breached", "<u4"),
+                                                 ("lws_loses_available", "<u4"), ("min_margin", "<i4")])
+assert DRAIN_BUDGET_COST.itemsize == 48
+
+
+class DrainBudgetQuery(C.Structure):
+    """lwse_drain_budget_query: the touched LWS rows of one drain set (node rows or domain ids in, the
+    DRAIN_BUDGET rows and the DRAIN_BUDGET_TOTALS out)."""
+
+    _fields_ = [
+        ("ids", C.c_void_p),
+        ("n_ids", C.c_uint32),
+        ("scope", C.c_uint32),
+        ("capacity", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("rows", C.c_void_p),
+        ("n_touched", C.c_uint32),
+        ("n_breached", C.c_uint32),
+        ("n_loses_available", C.c_uint32),
+        ("n_already_below", C.c_uint32),
+        ("n_pods_evicted", C.c_uint32),
+        ("n_leaders_evicted", C.c_uint32),
+        ("n_groups_restarted", C.c_uint32),
+        ("n_ready_restarted", C.c_uint32),
+        ("n_pods_recreated", C.c_uint64),
+    ]
+
+
+# the totals of a drain budget query, as Engine.resident_drain_budget returns them
+DRAIN_BUDGET_TOTALS = ("n_touched", "n_breached", "n_loses_available", "n_already_below", "n_pods_evicted",
+                       "n_leaders_evicted", "n_groups_restarted", "n_ready_restarted", "n_pods_recreated")
+
 
 class Config(C.Structure):
     _fields_ = [
