@@ -861,7 +861,7 @@ LWSE_API int lwse_resident_drain_cost(lwse_engine* e, lwse_drain_cost* out);
  * Definition.  An LWS row L is EVALUATED when its baseline result row has none of LWSE_LOUT_BAD_TABLE,
  * _IRREGULAR, _RUP_ERROR, _STATUS_ERROR and its row has no LWSE_LWS_INTSTR_INVALID.  For an evaluated L:
  *   floor        = max(0, replicas - mu), mu = maxUnavailable scaled against replicas, rounded down (:302),
- *                  clamped to int32;
+ *                  in 64 bits as Go's int (mu is never truncated to int32); the floor is clamped to int32;
  *   ready_before = lws_out[L].ready_replicas of the baseline (the results of the most recently submitted
  *                  sweep, the rows lwse_resident_drain_whatif diffs against).
  * The groups of L are the rows g of its group range (inside the group table) with lws_index == L.  For a

@@ -277,6 +277,15 @@ __device__ __forceinline__ int32_t clamp_i32(int64_t v) {
   return (int32_t)(v < INT32_MIN ? (int64_t)INT32_MIN : (v > INT32_MAX ? (int64_t)INT32_MAX : v));
 }
 
+// scaled_value (lwse_device.cuh) rounded down, kept in 64 bits as Go's int: the floor's mu must not wrap
+// when a percentage above 100 of a large replicas passes int32.  (The sweep keeps its int32(mu), :313.)
+__device__ __forceinline__ int64_t unavailable_i64(int32_t val, bool is_percent, int32_t total) {
+  if (!is_percent) return val;
+  const int64_t num = (int64_t)val * (int64_t)total;
+  const int64_t q = num / 100;
+  return (num - q * 100 != 0 && num < 0) ? q - 1 : q;
+}
+
 __device__ __forceinline__ LwsBudget budget_of(const lwse_lws_rec* lws, const lwse_lws_out* lws_out, uint32_t L,
                                                uint32_t n_groups) {
   const uint4* row = reinterpret_cast<const uint4*>(lws + L);
@@ -291,7 +300,7 @@ __device__ __forceinline__ LwsBudget budget_of(const lwse_lws_rec* lws, const lw
   b.evaluated = !(oflags & kBudgetExcluded) && !(lflags & LWSE_LWS_INTSTR_INVALID);
   b.available = ((oflags & LWSE_LOUT_COND_MASK) >> LWSE_LOUT_COND_SHIFT) == LWSE_COND_AVAILABLE;
   b.ready_before = (int32_t)o0.w;
-  const int32_t mu = scaled_value((int32_t)r1.w, lflags & LWSE_LWS_UNAVAIL_IS_PERCENT, b.replicas, false);  // :302
+  const int64_t mu = unavailable_i64((int32_t)r1.w, lflags & LWSE_LWS_UNAVAIL_IS_PERCENT, b.replicas);  // :302
   const int64_t fl = (int64_t)b.replicas - mu;
   b.floor = b.evaluated ? clamp_i32(fl < 0 ? 0 : fl) : 0;
   return b;
