@@ -127,6 +127,9 @@ __device__ __forceinline__ void lws_forecast_one(const LwsForecastArgs& a, const
   int32_t floor_ready = (int32_t)o.v0.w;
   uint32_t n_steps = 0;
   bool stopped = false;
+  // A guard, not a stop the replay reaches: after the first apply p' and n' never rise, and a cycle that
+  // leaves both as they were changes nothing, so an object stops within about C cycles (DESIGN.md).
+  // MAX_CYCLES binds for C >= 2^15.
   const uint32_t cap = (uint32_t)min(2 * C + 8, (long long)LWSE_LWS_FORECAST_MAX_CYCLES);
   for (uint32_t c = 0; c < cap; c++) {
     // the pass's reads of the slots (by any lane of the tile) come before this cycle's stores
