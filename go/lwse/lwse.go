@@ -167,6 +167,21 @@ func (e *Engine) PlaceWhatIf(q *C.lwse_place_whatif) error {
 	return e.check(C.lwse_resident_place_whatif(e.h, q))
 }
 
+// DsDrain answers "does draining these nodes or topology domains take an inference service down, or
+// stall its rollout?" over the resident LWS and DS tables: the DisaggregatedSets whose linked child
+// LeaderWorkerSets lose ready groups, with SERVICE_LOST / OLD_SERVICE_LOST / STALLS verdicts and their
+// ds_out rows before and after.  A drain or maintenance controller calls it before cordoning a rack or
+// zone, a kubectl drain dry-run plugin to report the services at risk.
+func (e *Engine) DsDrain(q *C.lwse_ds_drain_query) error {
+	return e.check(C.lwse_resident_ds_drain(e.h, q))
+}
+
+// DsDrainCost gives DsDrain's counts for every node (scope LWSE_DRAIN_NODES) or every domain
+// (LWSE_DRAIN_DOMAINS) in one call, to rank maintenance candidates.
+func (e *Engine) DsDrainCost(scope uint32, out *C.lwse_ds_drain_cost) error {
+	return e.check(C.lwse_resident_ds_drain_cost(e.h, C.uint32_t(scope), out))
+}
+
 // GroupKeys computes SHA-1 digests (20 bytes each) of n strings laid out CSR-style.
 func (e *Engine) GroupKeys(bytes *C.uint8_t, offsets *C.uint32_t, n uint32, digests *C.uint8_t) error {
 	return e.check(C.lwse_group_keys_host(e.h, bytes, offsets, C.uint32_t(n), digests))

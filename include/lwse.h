@@ -36,6 +36,8 @@
  *                      the resident tables with the pods of drained nodes deleting;
  *                      lwse_resident_drain_budget* adds a build-defined availability floor from
  *                      leaderworkerset_controller.go:302 (the reference has no drain budget)
+ *   lwse_resident_ds_drain*  the drain budget's lost groups through the DS links into the DS sweep:
+ *                      service_manager.go:57-89, :174-189 (serving), executor.go:270-281 (stable)
  *   lwse_group_keys_*  pkg/webhooks/pod_webhook.go:180-182 + pkg/utils/utils.go:39-43
  *                      (SHA-1 group / subgroup keys)
  *   lwse_subgroup_keys_*  pkg/webhooks/pod_webhook.go:249-255 (getSubGroupIndex) + :130,:151
@@ -1269,6 +1271,109 @@ LWSE_API int lwse_ds_forecast_host(lwse_engine* e, const lwse_ds_tables* host, l
  * lwse_ds_resident_load); every other call waits only on the DS stream.  LWSE_ERR_NOT_READY before
  * lwse_ds_resident_load; LWSE_ERR_INVALID_ARG for NULL outputs. */
 LWSE_API int lwse_ds_resident_forecast(lwse_engine* e, lwse_ds_forecast_out* out);
+
+/* ---- DS drain ------------------------------------------------------------------------------
+ * "Does this drain take an inference service down, or stall its rollout?"  A DisaggregatedSet serves
+ * while every spec role of a revision has a ready replica (service_manager.go:57-89, :174-189: the sweep's
+ * LWSE_DOUT_NEW_READY and ready_revs), and its rollout advances only while the target revision is stable,
+ * replicas == readyReplicas on every spec role (isRevisionStable, executor.go:270-281: LWSE_DOUT_STABLE).
+ * A drain can break either while every child LeaderWorkerSet stays above its own drain-budget floor.  The
+ * reference has no drain logic: the definition below is this build's own (DESIGN.md §3.5, "DS drain").
+ *
+ * Definition.  Drain sets and lost(L, D) are those of lwse_resident_drain_budget: lost(L, D) is the number
+ * of groups of LWS row L restarted by D whose baseline group row has LWSE_GOUT_COND_READY, against the
+ * results of the most recently submitted LWS sweep.  For a revision-role row r of a DS that is not
+ * LWSE_DOUT_BAD_TABLE, among the (n_old_revs + 1) * n_roles rows the sweep reads:
+ *   ready_before(r)  the value the linked DS sweep reads (the link rule of lwse_ds_link): the child's baseline
+ *                    lws_out[L].ready_replicas when r TAKES THE LWS VALUE, else r's own ready_replicas;
+ *   ready_after(r)   ready_before(r) - lost(L, D) for a row that takes the LWS value (computed in 64 bits,
+ *                    clamped to int32; several rows linked to one L all see the same lost), else ready_before.
+ * The BEFORE and AFTER sweeps are linked DS sweeps of the resident DS tables (the DS tick's device code) with
+ * ready_before and with ready_after.  "Before" is recomputed from the current LWS baseline, not read from the
+ * last DS tick, so the two differ by the drain alone.  Per DS:
+ *   LWSE_DSD_TOUCHED           some row that takes the LWS value has lost > 0;
+ *   LWSE_DSD_SERVICE_LOST      NEW_READY before, not after;
+ *   LWSE_DSD_OLD_SERVICE_LOST  ready_revs before & ~ready_revs after != 0;
+ *   LWSE_DSD_STALLS            STABLE before, not after;
+ *   LWSE_DSD_CHANGED           a ds_out row, or (not BAD_TABLE) a role_out or revrole_out row of the DS differs.
+ *   rows_touched               rows that take the LWS value and have lost > 0 (removed roles included);
+ *   rows_zeroed                of those, the rows with ready_before >= 1 and ready_after < 1.
+ * Only the ready column moves between the two sweeps, so a DS that is not touched is not changed either.
+ *
+ * Readiness and errors: LWSE_ERR_NOT_READY unless the drain budget is ready (as lwse_resident_drain_budget)
+ * and DS tables are resident (lwse_ds_resident_load).  With no link patch since the DS load every row falls
+ * back: nothing is touched and rows_linked is 0.  LWSE_ERR_INVALID_ARG as for lwse_resident_drain_budget.
+ * Isolation: the what-if stream under the engine mutex, behind an event on the engine's stream and one on
+ * the DS stream, with scratch of its own that only grows; no tick, graph, arena, change list, resident LWS
+ * or DS table, DS tick output or mirror, link table, occupancy counter, node index or tick info is touched.
+ * Multi-rank engines: a DS and its children live on one rank, so every count sums over the ranks.  DS whose row
+ * ranges overlap give results as unspecified as the sweep's; every write of both calls stays in their scratch
+ * (a row read by k DS counts k times, and the per-key form sizes its scratch from that count). */
+#define LWSE_DSD_TOUCHED (1u << 0)
+#define LWSE_DSD_SERVICE_LOST (1u << 1)
+#define LWSE_DSD_OLD_SERVICE_LOST (1u << 2)
+#define LWSE_DSD_STALLS (1u << 3)
+#define LWSE_DSD_CHANGED (1u << 4)
+
+/* One touched DS of a drain (64 B). */
+typedef struct lwse_ds_drain {
+  uint32_t ds;                /* DS row                                                                  */
+  uint32_t flags;             /* LWSE_DSD_*                                                              */
+  uint32_t rows_touched;
+  uint32_t rows_zeroed;
+  uint32_t new_zeroed_roles;  /* bit i: spec role i's row of the new revision is zeroed (the roles that take
+                                 its service down when SERVICE_LOST)                                     */
+  uint32_t old_zeroed_roles;  /* bit i: spec role i is zeroed in an old revision whose ready_revs bit falls
+                                 (the union over those revisions)                                        */
+  uint32_t reserved[2];
+  lwse_ds_out before;         /* its ds_out row in the before and the after sweep                        */
+  lwse_ds_out after;
+} lwse_ds_drain;
+
+/* The set form: the touched DS of one drain set, and its totals. */
+typedef struct lwse_ds_drain_query {
+  /* in */
+  const uint32_t* ids;        /* [n_ids] node rows or domain ids (by scope), host memory; duplicates allowed */
+  uint32_t n_ids;
+  uint32_t scope;             /* LWSE_DRAIN_NODES or LWSE_DRAIN_DOMAINS                                  */
+  uint32_t capacity;          /* rows `rows` holds                                                       */
+  uint32_t reserved;
+  lwse_ds_drain* rows;        /* [capacity]: touched DS (beyond capacity not listed; order unspecified)  */
+  lwse_ds_role_out* role_out; /* [n_roles] or NULL: the after sweep's full role_out (rows no DS's sweep
+                                 writes read 0)                                                          */
+  lwse_ds_revrole_out* revrole_out; /* [n_revroles] or NULL: the after sweep's full revrole_out (as role_out) */
+  /* out */
+  uint32_t n_touched;         /* every touched DS, listed or not                                         */
+  uint32_t n_service_lost;
+  uint32_t n_old_service_lost;
+  uint32_t n_stalled;
+  uint32_t n_changed;
+  uint32_t rows_touched;      /* summed over the touched DS                                              */
+  uint32_t rows_zeroed;
+  uint32_t rows_linked;       /* rows that take the LWS value, touched or not                            */
+} lwse_ds_drain_query;
+LWSE_API int lwse_resident_ds_drain(lwse_engine* e, lwse_ds_drain_query* q);
+
+/* The per-key form: one row per node (LWSE_DRAIN_NODES, n_nodes rows) or per domain (LWSE_DRAIN_DOMAINS,
+ * n_domains rows), row k holding what lwse_resident_ds_drain gives for the node k or the nodes of domain k
+ * (32 B; LWSE_DSD_CHANGED has no column: it needs the whole sweep).  Exact in one pass: lost(L, k) is the
+ * drain budget's per-key count, and only the ready column differs between the two sweeps, so NEW_READY
+ * falls iff a spec row of the new revision has ready_before >= 1 > ready_after, an old revision's ready bit
+ * iff one of its spec rows does, and STABLE iff a spec row of the new revision changes its ready count (before
+ * the drain ready == replicas there).  Each verdict is an OR over (row, key) facts gated by the DS's flags in
+ * the before sweep.  The (LWS, key) and (DS, key) pairs are gathered in open-addressing tables in scratch,
+ * each sized from a counting pass (one host synchronisation each); an insert a table refuses fails the call
+ * with LWSE_ERR_OOM.  Readiness, isolation and errors as lwse_resident_ds_drain; `out` is host memory. */
+typedef struct lwse_ds_drain_cost {
+  uint32_t ds_touched;        /* n_touched of the set form for this key                                  */
+  uint32_t ds_service_lost;
+  uint32_t ds_old_service_lost;
+  uint32_t ds_stalled;
+  uint32_t rows_touched;
+  uint32_t rows_zeroed;
+  uint32_t reserved[2];
+} lwse_ds_drain_cost;
+LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds_drain_cost* out);
 
 /* ------------------------------------------------------------------------- */
 /* Group / subgroup keys (SHA-1) and subgroup indices                        */

@@ -588,11 +588,153 @@ int launch_drain_budget_cost(const DrainBudgetCostLaunch* p, int pass, int sm_co
       if (p->n_groups) drain_budget_walk_kernel<false><<<walk_grid, kCostThreads, 0, s>>>(a);
       return launched_or_fail(p->n_groups ? 2 : 1, cuda_err);
     }
-    default:
+    case 1:
       drain_budget_walk_kernel<true><<<walk_grid, kCostThreads, 0, s>>>(a);
       drain_budget_finish_kernel<<<grid_for((uint64_t)p->table_mask + 1, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(a);
       return launched_or_fail(2, cuda_err);
+    default:  // the table alone, for the DS drain's per-key form
+      drain_budget_walk_kernel<true><<<walk_grid, kCostThreads, 0, s>>>(a);
+      return launched_or_fail(1, cuda_err);
   }
+}
+
+// --------------------------------------------------------------------------
+// DS drain (lwse_resident_ds_drain*): the definitions are in lwse.h
+// --------------------------------------------------------------------------
+//   ds_drain_lost_kernel     the set form: one warp per LWS row over its group range (as drain_budget_kernel),
+//                            lost[L] and the after copy of its lws_out row (ready_replicas - lost, clamped).
+//   ds_drain_pairs_kernel    the per-key form: (row, key) pairs = the linked rows of L summed over the (LWS, key)
+//                            entries with lost > 0.
+//   ds_drain_insert_kernel   one thread per (LWS, key) entry with lost > 0, over the rows linked to L: the key
+//                            row's rows_touched / rows_zeroed, and the row's facts ORed into the (DS, key) table.
+//   ds_drain_finish_kernel   every (DS, key) entry gated by the DS's before flags into its key's DS columns.
+struct DsDrainLostArgs {
+  const lwse_lws_rec* lws;
+  const lwse_lws_out* lws_out;
+  const lwse_group_rec* groups;
+  const lwse_group_out* before;
+  const lwse_group_out* after;
+  uint32_t* lost;
+  lwse_lws_out* lws_after;
+  uint32_t n_lws, n_groups;
+};
+
+__global__ void __launch_bounds__(256) ds_drain_lost_kernel(const DsDrainLostArgs a) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t n_warps = gridDim.x * (blockDim.x / 32);
+  for (uint32_t L = (blockIdx.x * blockDim.x + threadIdx.x) / 32; L < a.n_lws; L += n_warps) {
+    const uint4 r3 = ldg_cached(reinterpret_cast<const uint4*>(a.lws + L) + 3);
+    const uint32_t gbase = r3.z, gcount = (uint64_t)r3.z + r3.w <= a.n_groups ? r3.w : 0u;
+    uint32_t lost = 0;
+    for (uint32_t i = lane; i < gcount; i += 32) {
+      const uint32_t g = gbase + i;
+      if (__ldg(&a.groups[g].lws_index) != L) continue;
+      const uint32_t o = __ldcg(&a.before[g].flags), v = __ldcg(&a.after[g].flags);
+      lost += (!(o & kRestartBits) && (v & kRestartBits) && (o & LWSE_GOUT_COND_READY)) ? 1u : 0u;
+    }
+    lost = __reduce_add_sync(0xFFFFFFFFu, lost);
+    if (lane > 1) continue;
+    const uint4* src = reinterpret_cast<const uint4*>(a.lws_out + L);
+    uint4 v = __ldg(src + lane);
+    if (lane == 0) {
+      a.lost[L] = lost;
+      v.w = (uint32_t)clamp_i32((int64_t)(int32_t)v.w - lost);  // ready_replicas
+    }
+    reinterpret_cast<uint4*>(a.lws_after + L)[lane] = v;
+  }
+}
+
+int launch_ds_drain_lost(const lwse_lws_rec* d_lws, const lwse_lws_out* d_lws_out, uint32_t n_lws, const lwse_group_rec* d_groups,
+                         const lwse_group_out* d_before, const lwse_group_out* d_after, uint32_t n_groups, uint32_t* d_lost,
+                         lwse_lws_out* d_lws_after, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  if (n_lws == 0) return 0;
+  const DsDrainLostArgs a{d_lws, d_lws_out, d_groups, d_before, d_after, d_lost, d_lws_after, n_lws, n_groups};
+  ds_drain_lost_kernel<<<grid_for(n_lws, 256 / 32, (uint32_t)sm_count * 8u), 256, 0, s>>>(a);
+  return launched_or_fail(1, cuda_err);
+}
+
+constexpr uint32_t kDsdNewZeroed = 1u << 0;   // a spec row of the new revision falls below 1 ready
+constexpr uint32_t kDsdNewChanged = 1u << 1;  // a spec row of the new revision changes its ready count
+
+__global__ void __launch_bounds__(256) ds_drain_pairs_kernel(const DsDrainCostLaunch p) {
+  unsigned long long pairs = 0;
+  for (uint32_t h = blockIdx.x * blockDim.x + threadIdx.x; h <= p.lws_mask; h += gridDim.x * blockDim.x) {
+    const unsigned long long k = __ldg(p.lws_keys + h);
+    if (k == kEmptyKey || __ldg(&p.lws_vals[h].y) == 0) continue;
+    const uint32_t L = (uint32_t)(k >> 32);
+    pairs += __ldg(p.first + L + 1) - __ldg(p.first + L);
+  }
+  pairs = warp_sum_u64(pairs);
+  if ((threadIdx.x & 31u) == 0 && pairs) atomicAdd(reinterpret_cast<unsigned long long*>(p.counts), pairs);
+}
+
+__global__ void __launch_bounds__(256) ds_drain_insert_kernel(const DsDrainCostLaunch p) {
+  for (uint32_t h = blockIdx.x * blockDim.x + threadIdx.x; h <= p.lws_mask; h += gridDim.x * blockDim.x) {
+    const unsigned long long k = __ldg(p.lws_keys + h);
+    if (k == kEmptyKey) continue;
+    const uint32_t lost = __ldg(&p.lws_vals[h].y);
+    if (lost == 0) continue;
+    const uint32_t L = (uint32_t)(k >> 32), key = (uint32_t)k;
+    uint32_t touched = 0, zeroed = 0;
+    for (uint32_t j = __ldg(p.first + L), end = __ldg(p.first + L + 1); j < end; j++) {
+      const uint4 e = __ldg(p.entries + j);  // {DS row, slot | spec, ready_before, 0}
+      const int32_t rb = (int32_t)e.z, ra = clamp_i32((int64_t)rb - lost);
+      const bool zero = rb >= 1 && ra < 1;
+      touched++;
+      zeroed += zero ? 1u : 0u;
+      uint32_t bits = 0, old_mask = 0;
+      if (e.y & kDsDrainSpec) {
+        const uint32_t slot = e.y & 0xFFu;
+        if (slot == kDsDrainNewSlot)
+          bits = (zero ? kDsdNewZeroed : 0u) | (ra != rb ? kDsdNewChanged : 0u);
+        else if (zero)
+          old_mask = 1u << slot;
+      }
+      const unsigned long long dk = (unsigned long long)e.x << 32 | key;
+      uint32_t t = table_slot(dk, p.table_mask);
+      bool placed = false;
+      for (uint32_t probe = 0; probe <= p.table_mask; probe++, t = (t + 1u) & p.table_mask) {
+        const unsigned long long prev = atomicCAS(p.keys + t, kEmptyKey, dk);
+        if (prev == kEmptyKey || prev == dk) {
+          if (bits) atomicOr(&p.vals[t].x, bits);
+          if (old_mask) atomicOr(&p.vals[t].y, old_mask);
+          placed = true;
+          break;
+        }
+      }
+      if (!placed) atomicAdd(p.counts + 2, 1u);  // full: the call fails
+    }
+    atomicAdd(&p.cost[key].rows_touched, touched);
+    if (zeroed) atomicAdd(&p.cost[key].rows_zeroed, zeroed);
+  }
+}
+
+__global__ void __launch_bounds__(256) ds_drain_finish_kernel(const DsDrainCostLaunch p) {
+  for (uint32_t h = blockIdx.x * blockDim.x + threadIdx.x; h <= p.table_mask; h += gridDim.x * blockDim.x) {
+    const unsigned long long k = p.keys[h];
+    if (k == kEmptyKey) continue;
+    const uint32_t d = (uint32_t)(k >> 32), key = (uint32_t)k;
+    const uint2 v = p.vals[h];
+    const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.before + d));  // {flags, drained_revs, ready_revs, 0}
+    lwse_ds_drain_cost* c = p.cost + key;
+    atomicAdd(&c->ds_touched, 1u);
+    if ((v.x & kDsdNewZeroed) && (b.x & LWSE_DOUT_NEW_READY)) atomicAdd(&c->ds_service_lost, 1u);
+    if (v.y & b.z) atomicAdd(&c->ds_old_service_lost, 1u);
+    if ((v.x & kDsdNewChanged) && (b.x & LWSE_DOUT_STABLE)) atomicAdd(&c->ds_stalled, 1u);
+  }
+}
+
+int launch_ds_drain_cost(const DsDrainCostLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  const unsigned lws_grid = grid_for((uint64_t)p->lws_mask + 1, 256, (uint32_t)sm_count * 8u);
+  if (pass == 0) {
+    ds_drain_pairs_kernel<<<lws_grid, 256, 0, s>>>(*p);
+    return launched_or_fail(1, cuda_err);
+  }
+  ds_drain_insert_kernel<<<lws_grid, 256, 0, s>>>(*p);
+  ds_drain_finish_kernel<<<grid_for((uint64_t)p->table_mask + 1, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p);
+  return launched_or_fail(2, cuda_err);
 }
 
 }  // namespace lwse

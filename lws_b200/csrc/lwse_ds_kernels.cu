@@ -742,4 +742,198 @@ int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, c
   return 1;
 }
 
+// ---- DS drain (lwse_resident_ds_drain*): the definitions are in lwse.h ----
+//   ds_sweep_kernel<false, true>  the before and the after sweep: the linked sweep body without the tick's
+//                                 diff, mirrors and publish, reading ready counts from the baseline lws_out or
+//                                 from its copy with the drain's lost groups taken off.
+//   ds_drain_diff_kernel          one thread per DS: its rows' link rule against lost[L] (rows touched / zeroed
+//                                 / linked), the two sweeps' rows compared, the verdicts; touched DS appended
+//                                 with one atomic per warp, the totals reduced per warp.
+//   ds_drain_links_kernel         the per-key form's reverse link index (count, then fill behind the scan).
+static unsigned ds_grid(uint32_t n_ds, int sm_count) {
+  const uint32_t want = (n_ds + 127u) / 128u, cap = (uint32_t)sm_count * 16u;
+  return want < cap ? want : cap;
+}
+
+// The LWS row whose ready count revision-role row `row` takes under the link rule (linked_ready), or LWSE_NONE.
+__device__ __forceinline__ uint32_t ds_drain_link_of(const DsDrainLink& lk, uint32_t row, bool exists) {
+  if (!exists) return LWSE_NONE;
+  const uint4 l = ldg_stream(lk.links + row);  // {uid lo, uid hi, lws_row, reserved}
+  if (l.z >= lk.n_lws) return LWSE_NONE;       // (LWSE_NONE included)
+  const uint64_t uid = __ldg(reinterpret_cast<const unsigned long long*>(&lk.lws[l.z].uid_hash));
+  if (uid != u64_of(l.x, l.y)) return LWSE_NONE;
+  constexpr uint32_t kNoUpdate = LWSE_LOUT_IRREGULAR | LWSE_LOUT_BAD_TABLE | LWSE_LOUT_RUP_ERROR | LWSE_LOUT_STATUS_ERROR;
+  return (__ldg(&lk.lws_out[l.z].flags) & kNoUpdate) ? LWSE_NONE : l.z;
+}
+
+__device__ __forceinline__ bool u4_ne(const uint4 a, const uint4 b) { return a.x != b.x || a.y != b.y || a.z != b.z || a.w != b.w; }
+
+__global__ void __launch_bounds__(128, 4) ds_drain_diff_kernel(const lwse_ds_tables t, const DsDrainLink lk, const DsDrainDiffHost h) {
+  uint32_t service = 0, old_service = 0, stalled = 0, changed_n = 0, rows_touched = 0, rows_zeroed = 0, linked = 0;
+  const uint32_t lane = threadIdx.x & 31u;
+  for (uint32_t d = blockIdx.x * blockDim.x + threadIdx.x; d < t.n_ds; d += gridDim.x * blockDim.x) {
+    const uint4 h0 = ldg_stream(reinterpret_cast<const uint4*>(t.ds + d) + 0);
+    const uint4 h1 = ldg_stream(reinterpret_cast<const uint4*>(t.ds + d) + 1);
+    const uint4 after = __ldcg(reinterpret_cast<const uint4*>(t.ds_out + d));
+    const uint4 before = __ldcg(reinterpret_cast<const uint4*>(h.before_ds_out + d));
+    bool changed = u4_ne(after, before);
+    uint32_t touched = 0, zeroed = 0, new_zeroed = 0, old_zeroed = 0;
+    if (!(before.x & LWSE_DOUT_BAD_TABLE)) {  // (BAD_TABLE in both sweeps, or in neither)
+      const uint32_t role_base = h0.z, n = h0.w, S = h1.x, rev_base = h1.y, V = h1.z, nrr = (h1.z + 1u) * h0.w;
+      const uint32_t fell = before.z & ~after.z;  // old revisions whose service the drain takes down
+      for (uint32_t k = 0; k < nrr; k++) {
+        const uint32_t row = rev_base + k;
+        const uint32_t L = ds_drain_link_of(lk, row, __ldg(&t.revroles[row].flags) & LWSE_RR_EXISTS);
+        if (L == LWSE_NONE) continue;
+        linked++;
+        const uint32_t lost = __ldg(h.lost + L);
+        if (lost == 0) continue;
+        touched++;
+        const int32_t rb = __ldg(&lk.lws_out[L].ready_replicas);
+        const int64_t ra = (int64_t)rb - lost;
+        if (!(rb >= 1 && ra < 1)) continue;
+        zeroed++;
+        const uint32_t r = k / n, i = k - r * n;
+        if (i >= S) continue;  // (a removed role serves nothing)
+        if (r == V)
+          new_zeroed |= 1u << i;
+        else if ((fell >> r) & 1u)
+          old_zeroed |= 1u << i;
+      }
+      const uint2* ro = reinterpret_cast<const uint2*>(t.role_out + role_base);
+      const uint2* pro = reinterpret_cast<const uint2*>(h.before_role_out + role_base);
+      for (uint32_t i = 0; i < n && !changed; i++) {
+        const uint2 x = __ldcg(ro + i), y = __ldcg(pro + i);
+        changed = x.x != y.x || x.y != y.y;
+      }
+      for (uint32_t i = 0; i < nrr && !changed; i++)
+        changed = __ldcg(t.revrole_out + rev_base + i) != __ldcg(h.before_revrole_out + rev_base + i);
+    }
+    if (touched == 0) continue;  // (only the ready column of touched rows differs: an untouched DS is unchanged)
+    uint32_t flags = LWSE_DSD_TOUCHED;
+    if ((before.x & LWSE_DOUT_NEW_READY) && !(after.x & LWSE_DOUT_NEW_READY)) flags |= LWSE_DSD_SERVICE_LOST;
+    if (before.z & ~after.z) flags |= LWSE_DSD_OLD_SERVICE_LOST;
+    if ((before.x & LWSE_DOUT_STABLE) && !(after.x & LWSE_DOUT_STABLE)) flags |= LWSE_DSD_STALLS;
+    if (changed) flags |= LWSE_DSD_CHANGED;
+    service += (flags & LWSE_DSD_SERVICE_LOST) ? 1u : 0u;
+    old_service += (flags & LWSE_DSD_OLD_SERVICE_LOST) ? 1u : 0u;
+    stalled += (flags & LWSE_DSD_STALLS) ? 1u : 0u;
+    changed_n += changed ? 1u : 0u;
+    rows_touched += touched;
+    rows_zeroed += zeroed;
+    // warp-aggregated append: one atomic per warp
+    const unsigned m = __activemask();
+    const int leader = __ffs(m) - 1;
+    uint32_t at = 0;
+    if ((int)lane == leader) at = atomicAdd(h.counts + 16, (uint32_t)__popc(m));
+    at = __shfl_sync(m, at, leader) + (uint32_t)__popc(m & ((1u << lane) - 1u));
+    if (at < h.capacity) {
+      uint4* out = reinterpret_cast<uint4*>(h.rows + at);
+      out[0] = make_uint4(d, flags, touched, zeroed);
+      out[1] = make_uint4(new_zeroed, old_zeroed, 0u, 0u);
+      out[2] = before;
+      out[3] = after;
+    }
+  }
+  // (every lane of the warp is here: the loop above has ended)
+  service = __reduce_add_sync(0xFFFFFFFFu, service);
+  old_service = __reduce_add_sync(0xFFFFFFFFu, old_service);
+  stalled = __reduce_add_sync(0xFFFFFFFFu, stalled);
+  changed_n = __reduce_add_sync(0xFFFFFFFFu, changed_n);
+  rows_touched = __reduce_add_sync(0xFFFFFFFFu, rows_touched);
+  rows_zeroed = __reduce_add_sync(0xFFFFFFFFu, rows_zeroed);
+  linked = __reduce_add_sync(0xFFFFFFFFu, linked);
+  if (lane != 0) return;
+  if (service) atomicAdd(h.counts + 17, service);
+  if (old_service) atomicAdd(h.counts + 18, old_service);
+  if (stalled) atomicAdd(h.counts + 19, stalled);
+  if (changed_n) atomicAdd(h.counts + 20, changed_n);
+  if (rows_touched) atomicAdd(h.counts + 21, rows_touched);
+  if (rows_zeroed) atomicAdd(h.counts + 22, rows_zeroed);
+  if (linked) atomicAdd(h.counts + 23, linked);
+}
+
+// kFill = false: count[L] += the rows that take L's value, and *total (64-bit) += every such row (the entries the
+// fill writes: a row in the ranges of several DS counts once per DS).  kFill = true: each row's entry at
+// cursor[L]++, written only below capacity (the caller sized `entries` from *total, so every entry fits).
+template <bool kFill>
+__global__ void __launch_bounds__(128) ds_drain_links_kernel(const lwse_ds_tables t, const DsDrainLink lk, uint32_t* count,
+                                                            uint32_t* cursor, uint4* entries, uint32_t capacity,
+                                                            unsigned long long* total) {
+  unsigned long long rows = 0;
+  for (uint32_t d = blockIdx.x * blockDim.x + threadIdx.x; d < t.n_ds; d += gridDim.x * blockDim.x) {
+    const uint4 h0 = ldg_stream(reinterpret_cast<const uint4*>(t.ds + d) + 0);
+    const uint4 h1 = ldg_stream(reinterpret_cast<const uint4*>(t.ds + d) + 1);
+    if (!ds_rows_ok(t, h0, h1)) continue;
+    const uint32_t n = h0.w, S = h1.x, rev_base = h1.y, V = h1.z;
+    for (uint32_t r = 0; r <= V; r++)
+      for (uint32_t i = 0; i < n; i++) {
+        const uint32_t row = rev_base + r * n + i;
+        const uint32_t L = ds_drain_link_of(lk, row, __ldg(&t.revroles[row].flags) & LWSE_RR_EXISTS);
+        if (L == LWSE_NONE) continue;
+        if (!kFill) {
+          atomicAdd(count + L, 1u);
+          rows++;
+        } else {
+          const uint32_t at = atomicAdd(cursor + L, 1u);
+          const uint32_t info = (r == V ? kDsDrainNewSlot : r) | (i < S ? kDsDrainSpec : 0u);
+          if (at < capacity) entries[at] = make_uint4(d, info, (uint32_t)__ldg(&lk.lws_out[L].ready_replicas), 0u);
+        }
+      }
+  }
+  if (!kFill) {
+    // (every lane of the warp is here: the loop above has ended)
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) rows += __shfl_xor_sync(0xFFFFFFFFu, rows, off);
+    if ((threadIdx.x & 31u) == 0 && rows) atomicAdd(total, rows);
+  }
+}
+
+int launch_ds_drain_sweep(const lwse_ds_tables* t, const DsDrainLink* lk, const lwse_lws_out* ready_from, int sm_count,
+                          cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  if (t->n_ds == 0) return 0;
+  DsTickArgs a{};
+  a.links = lk->links;
+  a.lws = lk->lws;
+  a.lws_out = ready_from;
+  a.n_lws = lk->n_lws;
+  ds_sweep_kernel<false, true><<<ds_grid(t->n_ds, sm_count), 128, 0, s>>>(*t, a);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    *cuda_err = (int)e;
+    return -1;
+  }
+  return 1;
+}
+
+int launch_ds_drain_diff(const lwse_ds_tables* t, const DsDrainLink* lk, const DsDrainDiffHost* h, int sm_count,
+                         cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  if (t->n_ds == 0) return 0;
+  ds_drain_diff_kernel<<<ds_grid(t->n_ds, sm_count), 128, 0, s>>>(*t, *lk, *h);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    *cuda_err = (int)e;
+    return -1;
+  }
+  return 1;
+}
+
+int launch_ds_drain_links(const lwse_ds_tables* t, const DsDrainLink* lk, uint32_t* count, uint32_t* cursor, uint4* entries,
+                          uint32_t capacity, unsigned long long* total, bool fill, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  if (t->n_ds == 0) return 0;
+  if (fill)
+    ds_drain_links_kernel<true><<<ds_grid(t->n_ds, sm_count), 128, 0, s>>>(*t, *lk, count, cursor, entries, capacity, total);
+  else
+    ds_drain_links_kernel<false><<<ds_grid(t->n_ds, sm_count), 128, 0, s>>>(*t, *lk, count, cursor, entries, capacity, total);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    *cuda_err = (int)e;
+    return -1;
+  }
+  return 1;
+}
+
 }  // namespace lwse

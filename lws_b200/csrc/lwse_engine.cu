@@ -228,6 +228,10 @@ struct lwse_engine {
   // drain budget (lwse_resident_drain_budget*): the domain mask, the touched rows, the key rows, the (LWS, key)
   // table and its counters
   DevBuf dr_domains, dr_brows, dr_bcost, dr_table, dr_bwords;
+  // DS drain (lwse_resident_ds_drain*): lost[L] and the after copy of lws_out, the before / after sweep outputs, the
+  // touched DS rows, the reverse link index (count | first | cursor) and its entries, the key rows, the (DS, key) table
+  DevBuf dd_lost, dd_lws_after, dd_out[2], dd_role_out[2], dd_revrole_out[2], dd_rows, dd_index, dd_entries, dd_cost, dd_table;
+  cudaEvent_t ev_dd = nullptr;       // the DS stream where a DS drain starts
   uint32_t r_sweep_flags = 0;        // LWSE_SWEEP_GANG of the most recently submitted sweep (r_group_out's flags)
   DevBuf sha_bytes, sha_offsets, sha_digests, sha_ints;
   uint32_t* h_rounds = nullptr;  // pinned
@@ -302,6 +306,7 @@ int check_lws_tables(const lwse_lws_tables* t) {
 extern "C" {
 
 static int drain_ticks_locked(lwse_engine* e);  // waits for (and drops the results of) every tick in flight
+static bool ds_resident_table(const lwse_engine* e, uint32_t which, void** base, uint32_t* rows, uint32_t* row_bytes);
 
 LWSE_API uint32_t lwse_abi_version(void) { return LWSE_ABI_VERSION; }
 
@@ -447,7 +452,10 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->wf_nodes, &e->wf_reqs, &e->wf_out, &e->wf_dom_first, &e->wf_node_order, &e->wf_node_pos,
                       &e->wf_node_ix, &e->wf_touched, &e->wf_round, &e->wf_list,
                       &e->dr_state, &e->dr_groups, &e->dr_out, &e->dr_scan, &e->dr_mask, &e->dr_list, &e->dr_cost,
-                      &e->dr_domains, &e->dr_brows, &e->dr_bcost, &e->dr_table, &e->dr_bwords};
+                      &e->dr_domains, &e->dr_brows, &e->dr_bcost, &e->dr_table, &e->dr_bwords,
+                      &e->dd_lost, &e->dd_lws_after, &e->dd_out[0], &e->dd_out[1], &e->dd_role_out[0], &e->dd_role_out[1],
+                      &e->dd_revrole_out[0], &e->dd_revrole_out[1], &e->dd_rows, &e->dd_index, &e->dd_entries, &e->dd_cost,
+                      &e->dd_table};
     if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
     if (e->lf_stream) cudaStreamSynchronize(e->lf_stream);
     if (e->wf_stream) cudaStreamSynchronize(e->wf_stream);
@@ -476,6 +484,7 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
     if (e->ev_wf) cudaEventDestroy(e->ev_wf);
     if (e->ev_wf_t0) cudaEventDestroy(e->ev_wf_t0);
     if (e->ev_wf_t1) cudaEventDestroy(e->ev_wf_t1);
+    if (e->ev_dd) cudaEventDestroy(e->ev_dd);
     cudaStreamDestroy(e->side_stream);
     cudaStreamDestroy(e->stream);
   }
@@ -1449,6 +1458,31 @@ extern "C" __attribute__((visibility("default"))) int lwse_debug_whatif_device_u
   float ms = 0.f;
   LWSE_CUDA(e, cudaEventElapsedTime(&ms, e->ev_wf_t0, e->ev_wf_t1));
   *us = ms * 1000.f;
+  return LWSE_OK;
+}
+
+// Test aid (not part of lwse.h): copies the first n_rows rows of a resident input table (LWSE_TABLE_LWS, _GROUPS,
+// _POD_STATE, _POD_IDENT, or a DS table including LWSE_TABLE_DS_LINKS) to host memory, after the device is idle.
+// Tests read the tables back to check that a call left them as they were.
+extern "C" __attribute__((visibility("default"))) int lwse_debug_resident_read(lwse_engine* e, uint32_t table, void* out,
+                                                                               uint32_t n_rows) {
+  if (!e || (n_rows && !out)) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  void* base = nullptr;
+  uint32_t rows = 0, rb = 0;
+  switch (table) {
+    case LWSE_TABLE_LWS: base = e->r_lws.p; rows = e->rn_lws; rb = sizeof(lwse_lws_rec); break;
+    case LWSE_TABLE_GROUPS: base = e->r_groups.p; rows = e->rn_groups; rb = sizeof(lwse_group_rec); break;
+    case LWSE_TABLE_POD_STATE: base = e->r_pst.p; rows = (uint32_t)e->rn_pods; rb = 1; break;
+    case LWSE_TABLE_POD_IDENT: base = e->r_pid.p; rows = (uint32_t)e->rn_pods; rb = sizeof(lwse_pod_ident); break;
+    default:
+      if (!e->rd_loaded || !ds_resident_table(e, table, &base, &rows, &rb)) return LWSE_ERR_INVALID_ARG;
+  }
+  if (table <= LWSE_TABLE_POD_IDENT && !e->r_loaded) return LWSE_ERR_NOT_READY;
+  if (n_rows > rows) return LWSE_ERR_INVALID_ARG;
+  DeviceGuard guard(e->device);
+  LWSE_CUDA(e, cudaDeviceSynchronize());
+  if (n_rows) LWSE_CUDA(e, cudaMemcpy(out, base, (size_t)n_rows * rb, cudaMemcpyDeviceToHost));
   return LWSE_OK;
 }
 
@@ -2583,6 +2617,22 @@ static bool drain_budget_ready(const lwse_engine* e) {
   return e->r_loaded && e->n_nodes != 0 && e->r_groups_swept && e->r_swept;
 }
 
+// The node mask of a drain set in dr_mask, on wf_stream: `mask` (host) marks node rows, or domain ids whose
+// nodes the device marks.
+static int enqueue_drain_set(lwse_engine* e, const uint8_t* mask, bool by_domain) {
+  const uint32_t nn = e->n_nodes, nd = e->n_domains;
+  cudaStream_t s = e->wf_stream;
+  if (!by_domain) {
+    LWSE_CUDA(e, cudaMemcpyAsync(e->dr_mask.p, mask, nn, cudaMemcpyHostToDevice, s));
+    return LWSE_OK;
+  }
+  if (nd) LWSE_CUDA(e, cudaMemcpyAsync(e->dr_domains.p, mask, nd, cudaMemcpyHostToDevice, s));
+  int cuda_err = 0;
+  const int launched = lwse::launch_drain_domain_mask((const uint8_t*)e->dr_domains.p, nd, (const lwse_node_rec*)e->nodes.p, nn,
+                                                      (uint8_t*)e->dr_mask.p, e->sm_count, s, &cuda_err);
+  return count_launch(e, launched, cuda_err);
+}
+
 // The set form: the drain what-if's sweep over the node mask (the given node rows, or the nodes of the given
 // domains, built on the device), the diff's totals without a change list, then drain_budget_kernel over
 // every LWS row.
@@ -2611,17 +2661,10 @@ LWSE_API int lwse_resident_drain_budget(lwse_engine* e, lwse_drain_budget_query*
   cudaStream_t s = e->wf_stream;
   uint32_t* d_counts = (uint32_t*)e->dr_list.p;
   lwse_drain_budget* d_rows = (lwse_drain_budget*)e->dr_brows.p;
-  int cuda_err = 0;
-  if (by_domain) {
-    if (nd) LWSE_CUDA(e, cudaMemcpyAsync(e->dr_domains.p, mask, nd, cudaMemcpyHostToDevice, s));
-    const int launched = lwse::launch_drain_domain_mask((const uint8_t*)e->dr_domains.p, nd, (const lwse_node_rec*)e->nodes.p, nn,
-                                                        (uint8_t*)e->dr_mask.p, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  } else {
-    LWSE_CUDA(e, cudaMemcpyAsync(e->dr_mask.p, mask, nn, cudaMemcpyHostToDevice, s));
-  }
+  if (const int rc = enqueue_drain_set(e, mask, by_domain); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemsetAsync(d_counts, 0, 64, s));
   if (const int rc = enqueue_drain_sweep(e, d_counts, nullptr, nullptr, nullptr, 0); rc != LWSE_OK) return rc;
+  int cuda_err = 0;
   const int launched = lwse::launch_drain_budget((const lwse_lws_rec*)e->r_lws.p, (const lwse_lws_out*)e->r_lws_out.p, nl,
                                                  (const lwse_group_rec*)e->r_groups.p, (const lwse_group_out*)e->r_group_out.p,
                                                  (const lwse_group_out*)e->dr_out.p, e->rn_groups, d_rows, list_cap, d_counts,
@@ -2714,6 +2757,262 @@ LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lws
   LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 16, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   if (words[2]) return LWSE_ERR_OOM;  // an insert the table refused: no answer rather than a wrong one
+  return LWSE_OK;
+}
+
+// ---------------------------------------------------------------------------
+// DS drain
+// ---------------------------------------------------------------------------
+static bool ds_drain_ready(const lwse_engine* e) { return drain_budget_ready(e) && e->rd_loaded; }
+
+// drain_begin_locked, with the what-if stream also behind the DS stream (the last DS tick or load: nothing is
+// in flight there while the mutex is held, but the call does not depend on that).
+static int ds_drain_begin_locked(lwse_engine* e) {
+  if (!e->wf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->wf_stream, cudaStreamNonBlocking));
+  if (!e->ev_dd) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_dd, cudaEventDisableTiming));
+  LWSE_CUDA(e, cudaEventRecord(e->ev_dd, e->ds_stream));
+  LWSE_CUDA(e, cudaStreamWaitEvent(e->wf_stream, e->ev_dd, 0));
+  return drain_begin_locked(e);
+}
+
+// The resident DS tables with output set k of the DS drain's scratch (0: before, 1: after).
+static lwse_ds_tables ds_drain_tables(const lwse_engine* e, int k) {
+  lwse_ds_tables t{};
+  t.ds = (const lwse_ds_rec*)e->rd_ds.p;
+  t.n_ds = e->rdn_ds;
+  t.roles = (const lwse_ds_role_rec*)e->rd_roles.p;
+  t.n_roles = e->rdn_roles;
+  t.revroles = (const lwse_ds_revrole_rec*)e->rd_revroles.p;
+  t.n_revroles = e->rdn_revroles;
+  t.ds_out = (lwse_ds_out*)e->dd_out[k].p;
+  t.role_out = (lwse_ds_role_out*)e->dd_role_out[k].p;
+  t.revrole_out = (lwse_ds_revrole_out*)e->dd_revrole_out[k].p;
+  return t;
+}
+
+// The link table and the baseline LWS results (drain_budget_ready: they belong to the resident LWS rows).
+static lwse::DsDrainLink ds_drain_link(const lwse_engine* e) {
+  return lwse::DsDrainLink{(const lwse_ds_link*)e->rd_links.p, (const lwse_lws_rec*)e->r_lws.p,
+                           (const lwse_lws_out*)e->r_lws_out.p, e->rn_lws};
+}
+
+static int reserve_ds_drain_outputs(lwse_engine* e, int sets) {
+  for (int k = 0; k < sets; k++) {
+    LWSE_CUDA(e, e->dd_out[k].reserve((size_t)e->rdn_ds * sizeof(lwse_ds_out) + 16));
+    LWSE_CUDA(e, e->dd_role_out[k].reserve((size_t)e->rdn_roles * sizeof(lwse_ds_role_out) + 16));
+    LWSE_CUDA(e, e->dd_revrole_out[k].reserve((size_t)e->rdn_revroles * sizeof(lwse_ds_revrole_out) + 16));
+  }
+  return LWSE_OK;
+}
+
+// Output set k zeroed (rows no DS's sweep writes read 0), then the linked sweep into it reading ready counts
+// from `ready_from`; on wf_stream.
+static int enqueue_ds_drain_sweep(lwse_engine* e, int k, const lwse_lws_out* ready_from) {
+  cudaStream_t s = e->wf_stream;
+  const lwse_ds_tables t = ds_drain_tables(e, k);
+  LWSE_CUDA(e, cudaMemsetAsync(t.role_out, 0, (size_t)t.n_roles * sizeof(lwse_ds_role_out) + 16, s));
+  LWSE_CUDA(e, cudaMemsetAsync(t.revrole_out, 0, (size_t)t.n_revroles * sizeof(lwse_ds_revrole_out) + 16, s));
+  const lwse::DsDrainLink lk = ds_drain_link(e);
+  int cuda_err = 0;
+  const int launched = lwse::launch_ds_drain_sweep(&t, &lk, ready_from, e->sm_count, s, &cuda_err);
+  return count_launch(e, launched, cuda_err);
+}
+
+// The set form: the drain budget's mark → sweep (what-if group rows), lost[L] and the after copy of lws_out,
+// the before and the after linked DS sweep, then one diff kernel over every DS.
+LWSE_API int lwse_resident_ds_drain(lwse_engine* e, lwse_ds_drain_query* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!ds_drain_ready(e)) return LWSE_ERR_NOT_READY;
+  if (q->scope != LWSE_DRAIN_NODES && q->scope != LWSE_DRAIN_DOMAINS) return LWSE_ERR_INVALID_ARG;
+  if ((q->n_ids && !q->ids) || (q->capacity && !q->rows)) return LWSE_ERR_INVALID_ARG;
+  const bool by_domain = q->scope == LWSE_DRAIN_DOMAINS;
+  const uint32_t nn = e->n_nodes, nd = e->n_domains, n_keys = by_domain ? nd : nn;
+  for (uint32_t i = 0; i < q->n_ids; i++)
+    if (q->ids[i] >= n_keys) return LWSE_ERR_INVALID_ARG;
+  const uint32_t nl = e->rn_lws, nds = e->rdn_ds;
+  const uint32_t list_cap = q->capacity < nds ? q->capacity : nds;
+  DeviceGuard guard(e->device);
+  if (const int rc = reserve_drain_sweep(e); rc != LWSE_OK) return rc;
+  if (const int rc = reserve_ds_drain_outputs(e, 2); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, e->wf_stage.reserve((size_t)n_keys));
+  LWSE_CUDA(e, e->wf_words.reserve(128));
+  LWSE_CUDA(e, e->dr_list.reserve(128));
+  if (by_domain) LWSE_CUDA(e, e->dr_domains.reserve((size_t)nd + 16));
+  LWSE_CUDA(e, e->dd_lost.reserve((size_t)nl * 4 + 16));
+  LWSE_CUDA(e, e->dd_lws_after.reserve((size_t)nl * sizeof(lwse_lws_out) + 16));
+  LWSE_CUDA(e, e->dd_rows.reserve((size_t)list_cap * sizeof(lwse_ds_drain) + 16));
+  uint8_t* mask = static_cast<uint8_t*>(e->wf_stage.h);
+  memset(mask, 0, n_keys);
+  for (uint32_t i = 0; i < q->n_ids; i++) mask[q->ids[i]] = 1;
+  if (const int rc = ds_drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* d_counts = (uint32_t*)e->dr_list.p;
+  if (const int rc = enqueue_drain_set(e, mask, by_domain); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemsetAsync(d_counts, 0, 128, s));
+  if (const int rc = enqueue_drain_sweep(e, d_counts, nullptr, nullptr, nullptr, 0); rc != LWSE_OK) return rc;
+  int cuda_err = 0;
+  int launched = lwse::launch_ds_drain_lost((const lwse_lws_rec*)e->r_lws.p, (const lwse_lws_out*)e->r_lws_out.p, nl,
+                                            (const lwse_group_rec*)e->r_groups.p, (const lwse_group_out*)e->r_group_out.p,
+                                            (const lwse_group_out*)e->dr_out.p, e->rn_groups, (uint32_t*)e->dd_lost.p,
+                                            (lwse_lws_out*)e->dd_lws_after.p, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_ds_drain_sweep(e, 0, (const lwse_lws_out*)e->r_lws_out.p); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_ds_drain_sweep(e, 1, (const lwse_lws_out*)e->dd_lws_after.p); rc != LWSE_OK) return rc;
+  const lwse_ds_tables after = ds_drain_tables(e, 1);
+  const lwse::DsDrainLink lk = ds_drain_link(e);
+  const lwse::DsDrainDiffHost h{(const lwse_ds_out*)e->dd_out[0].p, (const lwse_ds_role_out*)e->dd_role_out[0].p,
+                                (const lwse_ds_revrole_out*)e->dd_revrole_out[0].p, (const uint32_t*)e->dd_lost.p,
+                                (lwse_ds_drain*)e->dd_rows.p, list_cap, d_counts};
+  launched = lwse::launch_ds_drain_diff(&after, &lk, &h, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_counts, 128, cudaMemcpyDeviceToHost, s));
+  if (q->role_out && e->rdn_roles)
+    LWSE_CUDA(e, cudaMemcpyAsync(q->role_out, after.role_out, (size_t)e->rdn_roles * sizeof(lwse_ds_role_out), cudaMemcpyDeviceToHost, s));
+  if (q->revrole_out && e->rdn_revroles)
+    LWSE_CUDA(e, cudaMemcpyAsync(q->revrole_out, after.revrole_out, (size_t)e->rdn_revroles * sizeof(lwse_ds_revrole_out),
+                                 cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint32_t n_touched = words[16];
+  const uint32_t listed = n_touched < list_cap ? n_touched : list_cap;
+  if (listed) {
+    LWSE_CUDA(e, cudaMemcpyAsync(q->rows, e->dd_rows.p, (size_t)listed * sizeof(lwse_ds_drain), cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaStreamSynchronize(s));
+  }
+  q->n_touched = n_touched;
+  q->n_service_lost = words[17];
+  q->n_old_service_lost = words[18];
+  q->n_stalled = words[19];
+  q->n_changed = words[20];
+  q->rows_touched = words[21];
+  q->rows_zeroed = words[22];
+  q->rows_linked = words[23];
+  return LWSE_OK;
+}
+
+// The per-key form: the before sweep, the reverse link index's counts and scan, and the drain budget's key rows
+// and pair count; one host synchronisation to size the index entries and the (LWS, key) table; the index fill,
+// that table alone and the (row, key) pair count; a second synchronisation to size the (DS, key) table; then the
+// insert and finish passes.
+LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds_drain_cost* out) {
+  if (!e) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!ds_drain_ready(e)) return LWSE_ERR_NOT_READY;
+  if (!out || (scope != LWSE_DRAIN_NODES && scope != LWSE_DRAIN_DOMAINS)) return LWSE_ERR_INVALID_ARG;
+  const bool by_domain = scope == LWSE_DRAIN_DOMAINS;
+  const uint32_t nn = e->n_nodes, n_keys = by_domain ? e->n_domains : nn, nl = e->rn_lws;
+  const size_t cost_bytes = (size_t)n_keys * sizeof(lwse_ds_drain_cost);
+  DeviceGuard guard(e->device);
+  if (const int rc = reserve_ds_drain_outputs(e, 1); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, e->dr_bcost.reserve((size_t)n_keys * sizeof(lwse_drain_budget_cost) + 16));
+  LWSE_CUDA(e, e->dr_bwords.reserve(64));
+  LWSE_CUDA(e, e->wf_words.reserve(64));
+  LWSE_CUDA(e, e->dd_cost.reserve(cost_bytes + 16));
+  LWSE_CUDA(e, e->dd_index.reserve((size_t)(nl + 1) * 3 * 4 + 16));
+  if (const int rc = ds_drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  int cuda_err = 0;
+  // the before sweep (its ds_out gates the verdicts) and the reverse link index
+  if (const int rc = enqueue_ds_drain_sweep(e, 0, (const lwse_lws_out*)e->r_lws_out.p); rc != LWSE_OK) return rc;
+  const lwse_ds_tables t = ds_drain_tables(e, 0);
+  const lwse::DsDrainLink lk = ds_drain_link(e);
+  uint32_t* d_count = (uint32_t*)e->dd_index.p;
+  uint32_t* d_first = d_count + (nl + 1);
+  uint32_t* d_cursor = d_first + (nl + 1);
+  uint32_t* d_words = (uint32_t*)e->dr_bwords.p;  // [0..1] (group, key) pairs [2] refused; [8..9] (row, key) pairs
+                                                  // [10] refused; [12..13] reverse-index entries (all u64 but [2], [10])
+  LWSE_CUDA(e, cudaMemsetAsync(d_words, 0, 64, s));
+  LWSE_CUDA(e, cudaMemsetAsync(d_count, 0, (size_t)(nl + 1) * 4, s));
+  int launched = lwse::launch_ds_drain_links(&t, &lk, d_count, d_cursor, nullptr, 0, (unsigned long long*)(d_words + 12),
+                                             false, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  launched = lwse::launch_index_scan(d_count, d_first, d_cursor, nl, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  // the drain budget's (LWS, key) table: vals.y = lost(L, key)
+  lwse::DrainBudgetCostLaunch p{};
+  p.lws = (const lwse_lws_rec*)e->r_lws.p;
+  p.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
+  p.groups = (const lwse_group_rec*)e->r_groups.p;
+  p.pod_state = (const uint8_t*)e->r_pst.p;
+  p.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
+  p.baseline = (const lwse_group_out*)e->r_group_out.p;
+  p.nodes = (const lwse_node_rec*)e->nodes.p;
+  p.occupancy = (const uint32_t*)e->r_occ.p;
+  p.cost = (lwse_drain_budget_cost*)e->dr_bcost.p;
+  p.counts = d_words;
+  p.n_pods = e->rn_pods;
+  p.n_lws = nl;
+  p.n_groups = e->rn_groups;
+  p.n_nodes = nn;
+  p.n_domains = e->n_domains;
+  p.n_keys = n_keys;
+  p.by_domain = by_domain;
+  lwse::DsDrainCostLaunch c{};
+  c.first = d_first;
+  c.before = t.ds_out;
+  c.cost = (lwse_ds_drain_cost*)e->dd_cost.p;
+  c.counts = p.counts + 8;
+  LWSE_CUDA(e, cudaMemsetAsync(p.cost, 0, (size_t)n_keys * sizeof(lwse_drain_budget_cost), s));
+  LWSE_CUDA(e, cudaMemsetAsync(c.cost, 0, cost_bytes, s));
+  launched = lwse::launch_drain_budget_cost(&p, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 64, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  uint64_t pairs = 0, n_entries = 0;
+  memcpy(&pairs, words, 8);
+  memcpy(&n_entries, words + 12, 8);
+  // The index holds one entry per (DS, row that takes the LWS value): a row inside the ranges of several DS
+  // counts once for each, so the entries are sized from this count, not from the revision-role table.
+  if (n_entries > (1ull << 30)) return LWSE_ERR_OOM;  // (the index is 32-bit)
+  LWSE_CUDA(e, e->dd_entries.reserve((size_t)n_entries * sizeof(uint4) + 16));
+  c.entries = (const uint4*)e->dd_entries.p;
+  launched = lwse::launch_ds_drain_links(&t, &lk, d_count, d_cursor, (uint4*)e->dd_entries.p, (uint32_t)n_entries, nullptr,
+                                         true, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (pairs) {
+    if (pairs > (1ull << 30)) return LWSE_ERR_OOM;  // (the table index is 32-bit)
+    uint64_t slots = 256;
+    while (slots < 2 * pairs) slots <<= 1;
+    LWSE_CUDA(e, e->dr_table.reserve((size_t)slots * (sizeof(unsigned long long) + sizeof(uint4))));
+    p.keys = (unsigned long long*)e->dr_table.p;
+    p.vals = reinterpret_cast<uint4*>(p.keys + slots);
+    p.table_mask = (uint32_t)(slots - 1);
+    LWSE_CUDA(e, cudaMemsetAsync(p.keys, 0xFF, (size_t)slots * sizeof(unsigned long long), s));
+    LWSE_CUDA(e, cudaMemsetAsync(p.vals, 0, (size_t)slots * sizeof(uint4), s));
+    launched = lwse::launch_drain_budget_cost(&p, 2, e->sm_count, s, &cuda_err);
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    c.lws_keys = p.keys;
+    c.lws_vals = p.vals;
+    c.lws_mask = p.table_mask;
+    launched = lwse::launch_ds_drain_cost(&c, 0, e->sm_count, s, &cuda_err);
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 64, cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaStreamSynchronize(s));
+    if (words[2]) return LWSE_ERR_OOM;  // an insert the (LWS, key) table refused
+    uint64_t ds_pairs = 0;
+    memcpy(&ds_pairs, words + 8, 8);
+    if (ds_pairs) {
+      if (ds_pairs > (1ull << 30)) return LWSE_ERR_OOM;
+      uint64_t ds_slots = 256;
+      while (ds_slots < 2 * ds_pairs) ds_slots <<= 1;
+      LWSE_CUDA(e, e->dd_table.reserve((size_t)ds_slots * (sizeof(unsigned long long) + sizeof(uint2))));
+      c.keys = (unsigned long long*)e->dd_table.p;
+      c.vals = reinterpret_cast<uint2*>(c.keys + ds_slots);
+      c.table_mask = (uint32_t)(ds_slots - 1);
+      LWSE_CUDA(e, cudaMemsetAsync(c.keys, 0xFF, (size_t)ds_slots * sizeof(unsigned long long), s));
+      LWSE_CUDA(e, cudaMemsetAsync(c.vals, 0, (size_t)ds_slots * sizeof(uint2), s));
+      launched = lwse::launch_ds_drain_cost(&c, 1, e->sm_count, s, &cuda_err);
+      if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    }
+  }
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  if (n_keys) LWSE_CUDA(e, cudaMemcpyAsync(out, c.cost, cost_bytes, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 64, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  if (words[10]) return LWSE_ERR_OOM;  // an insert the (DS, key) table refused: no answer rather than a wrong one
   return LWSE_OK;
 }
 

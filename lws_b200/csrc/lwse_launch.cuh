@@ -112,6 +112,9 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
                     const PlaceNsChanges* changes, const PlaceNsExchange* xch, PlaceNsIndex index);
 size_t place_ns_scratch_bytes(uint32_t n_nodes, uint32_t n_domains, uint32_t n_reqs, uint32_t n_namespaces);
 size_t node_index_scratch_bytes(uint32_t n_domains);
+// The index block's scan (one CTA): first[0..n] = the exclusive scan of count[0..n) and its total, cursor = first,
+// count back to zero.
+int launch_index_scan(uint32_t* d_count, uint32_t* d_first, uint32_t* d_cursor, uint32_t n, cudaStream_t s, int* cuda_err);
 int launch_node_index(const lwse_node_rec* d_nodes, uint32_t n_nodes, uint32_t n_domains, uint32_t* d_dom_first,
                       uint32_t* d_node_order, uint32_t* d_node_pos, void* d_scratch, int sm_count, cudaStream_t s,
                       bool pdl, int* cuda_err);
@@ -158,6 +161,41 @@ struct DsForecastHost {
 };
 int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s,
                        int* cuda_err);
+
+// DS drain (lwse_resident_ds_drain*): the link table and the baseline LWS rows it points into.
+struct DsDrainLink {
+  const lwse_ds_link* links;
+  const lwse_lws_rec* lws;
+  const lwse_lws_out* lws_out;  // the baseline results (ready_before)
+  uint32_t n_lws;
+};
+// A linked DS sweep of t into t's outputs, reading ready counts from `ready_from` (the baseline, or its copy
+// with the drain's lost groups taken off) through the link rule of `lk`.
+int launch_ds_drain_sweep(const lwse_ds_tables* t, const DsDrainLink* lk, const lwse_lws_out* ready_from, int sm_count,
+                          cudaStream_t s, int* cuda_err);
+// The set form's diff: t's outputs (after) against `before`; touched DS appended to rows (up to capacity).
+// counts (device, zeroed by the caller): [16] touched (the append cursor) [17] service lost [18] old service
+// lost [19] stalled [20] changed [21] rows touched [22] rows zeroed [23] rows linked.
+struct DsDrainDiffHost {
+  const lwse_ds_out* before_ds_out;
+  const lwse_ds_role_out* before_role_out;
+  const lwse_ds_revrole_out* before_revrole_out;
+  const uint32_t* lost;  // [n_lws]
+  lwse_ds_drain* rows;
+  uint32_t capacity;
+  uint32_t* counts;
+};
+int launch_ds_drain_diff(const lwse_ds_tables* t, const DsDrainLink* lk, const DsDrainDiffHost* h, int sm_count,
+                         cudaStream_t s, int* cuda_err);
+// The reverse link index of the per-key form: LWS row → the revision-role rows that take its value, once per DS
+// whose ranges hold the row (DS ranges may overlap).  fill = false: count[L] += rows per L (count zeroed by the
+// caller) and *total (u64, zeroed by the caller) += all of them.  fill = true: every such row's entry
+// {DS row, slot (0xFF: the new revision) | 0x100 when a spec role, ready_before, 0} at cursor[L]++, written only
+// below capacity (entries holds capacity rows; the caller sizes it from *total).
+int launch_ds_drain_links(const lwse_ds_tables* t, const DsDrainLink* lk, uint32_t* count, uint32_t* cursor, uint4* entries,
+                          uint32_t capacity, unsigned long long* total, bool fill, int sm_count, cudaStream_t s, int* cuda_err);
+constexpr uint32_t kDsDrainNewSlot = 0xFFu;
+constexpr uint32_t kDsDrainSpec = 0x100u;
 
 // ---- lwse_lws_forecast_kernels.cu ----
 struct LwsForecastHost {
@@ -222,7 +260,31 @@ struct DrainBudgetCostLaunch {
   uint32_t n_lws, n_groups, n_nodes, n_domains, n_keys, table_mask;
   bool by_domain;
 };
+// Pass 2: the (LWS, key) table alone (pass 1 without the budget columns).
 int launch_drain_budget_cost(const DrainBudgetCostLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
+// The DS drain's set form: lost[L] (the drain budget's lost groups of every LWS row, d_after a what-if sweep
+// against the baseline d_before) and d_lws_after, a copy of d_lws_out with ready_replicas - lost[L].
+int launch_ds_drain_lost(const lwse_lws_rec* d_lws, const lwse_lws_out* d_lws_out, uint32_t n_lws, const lwse_group_rec* d_groups,
+                         const lwse_group_out* d_before, const lwse_group_out* d_after, uint32_t n_groups, uint32_t* d_lost,
+                         lwse_lws_out* d_lws_after, int sm_count, cudaStream_t s, int* cuda_err);
+// The DS drain's per-key form over the drain budget's (LWS, key) table (vals.y = lost(L, key)) and the reverse
+// link index.  Pass 0: counts[0..1] (u64, zeroed by the caller) = the (row, key) pairs.  Pass 1 (keys all-ones
+// and vals zeroed by the caller, table_mask + 1 a power of two > the pairs): the (DS, key) table, the key rows'
+// rows_touched / rows_zeroed, then the DS columns; counts[2] = inserts the table refused.
+struct DsDrainCostLaunch {
+  const unsigned long long* lws_keys;
+  const uint4* lws_vals;
+  uint32_t lws_mask;
+  const uint32_t* first;  // [n_lws + 1]
+  const uint4* entries;
+  const lwse_ds_out* before;  // the before sweep's ds_out
+  lwse_ds_drain_cost* cost;   // n_keys rows, zeroed by the caller
+  unsigned long long* keys;   // the (DS, key) table: DS row << 32 | key
+  uint2* vals;                // {bits, old revisions with a zeroed spec row}
+  uint32_t table_mask;
+  uint32_t* counts;
+};
+int launch_ds_drain_cost(const DsDrainCostLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
 
 // ---- lwse_sha1_kernels.cu ----
 int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,

@@ -1024,6 +1024,17 @@ int launch_place_whatif_index(const lwse_place_req* d_reqs, uint32_t n_reqs, uin
   return 3;
 }
 
+int launch_index_scan(uint32_t* d_count, uint32_t* d_first, uint32_t* d_cursor, uint32_t n, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  place_index_scan_kernel<<<1, kIndexScanThreads, 0, s>>>(IndexScanArgs{d_count, d_first, d_cursor, n});
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    *cuda_err = (int)e;
+    return -1;
+  }
+  return 1;
+}
+
 // The what-if's diff against the baseline and its counts.  counts: [0] changed rows [1] lost [2] moved
 // [3] gained (resident rows) [4] PLACED [5] UNSCHEDULABLE [6] CONFLICT (every row, extra rows included).
 // Each warp reduces its counts before the one atomic per counter, and appends its changed rows with one

@@ -345,6 +345,37 @@ class DsIncrementalEncoder:
         """The old revisions of the DS at `row` in revision-role row order (the target revision follows them)."""
         return self._meta[int(row)][1]
 
+    def ds_drain_report(self, result: dict) -> list:
+        """The touched DisaggregatedSets of a ``resident_ds_drain`` answer as dicts: ``namespace`` and ``name``
+        (None for a row no DS holds), ``rows_touched`` / ``rows_zeroed``, the ``records.DSD_*`` flags named in
+        ``conditions``, ``service_lost`` ({"revision": the target revision, "roles": its spec roles the drain
+        takes to zero ready replicas}, or None) and ``old_service_lost`` (one {"revision", "roles"} per old
+        revision that loses its service; a DS row carries one role mask for all of them, so each lists the
+        roles zeroed in any of those revisions)."""
+        names = {R.DSD_TOUCHED: "touched", R.DSD_SERVICE_LOST: "service_lost",
+                 R.DSD_OLD_SERVICE_LOST: "old_service_lost", R.DSD_STALLS: "stalls", R.DSD_CHANGED: "changed"}
+        out = []
+        for r in result["rows"]:
+            row, flags = int(r["ds"]), int(r["flags"])
+            key = self.object_of_ds_row(row)
+            roles = self.role_names(row) if key else []
+            old = self.old_revisions(row) if key else []
+
+            def named(mask):
+                return [role for i, role in enumerate(roles) if (mask >> i) & 1]
+
+            fell = int(r["before"]["ready_revs"]) & ~int(r["after"]["ready_revs"])
+            service = None
+            if key and flags & R.DSD_SERVICE_LOST:
+                service = {"revision": self.items[key][1], "roles": named(int(r["new_zeroed_roles"]))}
+            out.append({"namespace": key[0] if key else None, "name": key[1] if key else None,
+                        "rows_touched": int(r["rows_touched"]), "rows_zeroed": int(r["rows_zeroed"]),
+                        "conditions": [n for bit, n in names.items() if flags & bit],
+                        "service_lost": service,
+                        "old_service_lost": [{"revision": rev, "roles": named(int(r["old_zeroed_roles"]))}
+                                             for i, rev in enumerate(old) if (fell >> i) & 1]})
+        return out
+
     def forecast_of(self, forecast: dict, namespace: str, name: str) -> dict:
         """One DS's rollout forecast (``Engine.ds_resident_forecast`` over ``tables()``), by name:
         the flags, cycle and step counts, and per role name its peak replicas, availability floor,

@@ -48,6 +48,8 @@ SYMBOLS = {
     "lwse_resident_drain_cost": ([C.c_void_p, C.c_void_p], C.c_int),
     "lwse_resident_drain_budget": ([C.c_void_p, C.POINTER(R.DrainBudgetQuery)], C.c_int),
     "lwse_resident_drain_budget_cost": ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
+    "lwse_resident_ds_drain": ([C.c_void_p, C.POINTER(R.DsDrainQuery)], C.c_int),
+    "lwse_resident_ds_drain_cost": ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_place_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
         C.c_int,
@@ -496,6 +498,46 @@ class Engine:
         n = self.n_nodes if scope == "nodes" else self.n_domains
         out = R.aligned_empty(max(n, 1), R.DRAIN_BUDGET_COST)
         self._check(lib().lwse_resident_drain_budget_cost(self._h, self._DRAIN_SCOPES[scope], R.ptr(out)))
+        return out[:n]
+
+    def resident_ds_drain(self, nodes=None, domains=None, capacity=None, outputs=False):
+        """lwse_resident_ds_drain: the DisaggregatedSets a drain of the node rows ``nodes`` — or of every node in
+        the domain ids ``domains`` — touches through their linked child LeaderWorkerSets, each with its
+        ``records.DSD_*`` verdicts and its ds_out row in the before and the after sweep.  Give exactly one of the
+        two.  ``capacity`` None lists every touched DS; ``outputs`` also returns the after sweep's full
+        ``role_out`` / ``revrole_out``.  → dict: ``rows`` (``records.DS_DRAIN``) and the totals of
+        ``records.DS_DRAIN_TOTALS``."""
+        if (nodes is None) == (domains is None):
+            raise ValueError("give node rows or domain ids")
+        ids = np.ascontiguousarray(nodes if domains is None else domains, dtype=np.uint32)
+        n_ds, n_roles, n_rr = getattr(self, "_ds_shape", (0, 0, 0))
+        cap = n_ds if capacity is None else int(capacity)
+        rows = R.aligned_empty(max(cap, 1), R.DS_DRAIN)
+        q = R.DsDrainQuery()
+        q.ids = R.ptr(ids) if len(ids) else None
+        q.n_ids = len(ids)
+        q.scope = R.DRAIN_NODES if domains is None else R.DRAIN_DOMAINS
+        q.capacity = cap
+        q.rows = R.ptr(rows)
+        role_out = revrole_out = None
+        if outputs:
+            role_out = R.aligned_empty(max(n_roles, 1), R.DS_ROLE_OUT)
+            revrole_out = R.aligned_empty(max(n_rr, 1), R.DS_REVROLE_OUT)
+            q.role_out, q.revrole_out = R.ptr(role_out), R.ptr(revrole_out)
+        self._check(lib().lwse_resident_ds_drain(self._h, C.byref(q)))
+        out = {"rows": rows[: min(q.n_touched, cap)]}
+        out.update({k: getattr(q, k) for k in R.DS_DRAIN_TOTALS})
+        if outputs:
+            out["role_out"], out["revrole_out"] = role_out[:n_roles], revrole_out[:n_rr]
+        return out
+
+    def resident_ds_drain_cost(self, scope: str = "nodes") -> np.ndarray:
+        """lwse_resident_ds_drain_cost: one ``records.DS_DRAIN_COST`` row per node (``scope="nodes"``) or per
+        domain (``"domains"``), row k holding the counts ``resident_ds_drain`` gives for that key alone — every
+        key in one call."""
+        n = self.n_nodes if scope == "nodes" else self.n_domains
+        out = R.aligned_empty(max(n, 1), R.DS_DRAIN_COST)
+        self._check(lib().lwse_resident_ds_drain_cost(self._h, self._DRAIN_SCOPES[scope], R.ptr(out)))
         return out[:n]
 
     def resident_patch(self, which: int, rows, values):

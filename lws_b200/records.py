@@ -584,6 +584,59 @@ DRAIN_BUDGET_TOTALS = ("n_touched", "n_breached", "n_loses_available", "n_alread
                        "n_leaders_evicted", "n_groups_restarted", "n_ready_restarted", "n_pods_recreated")
 
 
+# DS drain (lwse_resident_ds_drain*): the flags of a touched DS
+DSD_TOUCHED = 1 << 0
+DSD_SERVICE_LOST = 1 << 1
+DSD_OLD_SERVICE_LOST = 1 << 2
+DSD_STALLS = 1 << 3
+DSD_CHANGED = 1 << 4
+
+# lwse_ds_drain: one touched DS of a drain, with its ds_out row in the before and the after sweep
+DS_DRAIN = np.dtype(
+    [("ds", "<u4"), ("flags", "<u4"), ("rows_touched", "<u4"), ("rows_zeroed", "<u4"), ("new_zeroed_roles", "<u4"),
+     ("old_zeroed_roles", "<u4"), ("reserved", "<u4", (2,)), ("before", DS_OUT), ("after", DS_OUT)],
+    align=False,
+)
+assert DS_DRAIN.itemsize == 64
+
+# lwse_ds_drain_cost: per node or per domain, the set form's DS counts for that key alone
+DS_DRAIN_COST = np.dtype(
+    [("ds_touched", "<u4"), ("ds_service_lost", "<u4"), ("ds_old_service_lost", "<u4"), ("ds_stalled", "<u4"),
+     ("rows_touched", "<u4"), ("rows_zeroed", "<u4"), ("reserved", "<u4", (2,))],
+    align=False,
+)
+assert DS_DRAIN_COST.itemsize == 32
+
+
+class DsDrainQuery(C.Structure):
+    """lwse_ds_drain_query: the touched DisaggregatedSets of one drain set (node rows or domain ids in, the
+    DS_DRAIN rows, optionally the after sweep's full role_out / revrole_out, and the DS_DRAIN_TOTALS out)."""
+
+    _fields_ = [
+        ("ids", C.c_void_p),
+        ("n_ids", C.c_uint32),
+        ("scope", C.c_uint32),
+        ("capacity", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("rows", C.c_void_p),
+        ("role_out", C.c_void_p),
+        ("revrole_out", C.c_void_p),
+        ("n_touched", C.c_uint32),
+        ("n_service_lost", C.c_uint32),
+        ("n_old_service_lost", C.c_uint32),
+        ("n_stalled", C.c_uint32),
+        ("n_changed", C.c_uint32),
+        ("rows_touched", C.c_uint32),
+        ("rows_zeroed", C.c_uint32),
+        ("rows_linked", C.c_uint32),
+    ]
+
+
+# the totals of a DS drain query, as Engine.resident_ds_drain returns them
+DS_DRAIN_TOTALS = ("n_touched", "n_service_lost", "n_old_service_lost", "n_stalled", "n_changed", "rows_touched",
+                   "rows_zeroed", "rows_linked")
+
+
 class Config(C.Structure):
     _fields_ = [
         ("abi_version", C.c_uint32),
