@@ -2966,14 +2966,15 @@ LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds
   memcpy(&n_entries, words + 12, 8);
   // The index holds one entry per (DS, row that takes the LWS value): a row inside the ranges of several DS
   // counts once for each, so the entries are sized from this count, not from the revision-role table.
+  // Both refusals come before the next launch: nothing is left in flight on wf_stream when the call returns.
   if (n_entries > (1ull << 30)) return LWSE_ERR_OOM;  // (the index is 32-bit)
+  if (pairs > (1ull << 30)) return LWSE_ERR_OOM;      // (the table index is 32-bit)
   LWSE_CUDA(e, e->dd_entries.reserve((size_t)n_entries * sizeof(uint4) + 16));
   c.entries = (const uint4*)e->dd_entries.p;
   launched = lwse::launch_ds_drain_links(&t, &lk, d_count, d_cursor, (uint4*)e->dd_entries.p, (uint32_t)n_entries, nullptr,
                                          true, e->sm_count, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   if (pairs) {
-    if (pairs > (1ull << 30)) return LWSE_ERR_OOM;  // (the table index is 32-bit)
     uint64_t slots = 256;
     while (slots < 2 * pairs) slots <<= 1;
     LWSE_CUDA(e, e->dr_table.reserve((size_t)slots * (sizeof(unsigned long long) + sizeof(uint4))));
