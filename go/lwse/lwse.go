@@ -167,6 +167,17 @@ func (e *Engine) PlaceWhatIf(q *C.lwse_place_whatif) error {
 	return e.check(C.lwse_resident_place_whatif(e.h, q))
 }
 
+// RolloutWhatIf answers "if this LeaderWorkerSet edit were pushed, what would its rollout do?" over the
+// resident tables without changing them: per proposal (a resident row and the row the edited object
+// would encode to) the controller's first write, and the forecast of the rollout it starts — controller
+// writes, peak leader StatefulSet replicas, the ready-group floor, and whether it finishes or stops at
+// the spec partition.  It never waits for or drops a tick.  A kubectl plugin or a validating webhook
+// calls it on a template, replicas or rollout-settings edit; a fleet image bump asks one proposal per
+// object in one call.
+func (e *Engine) RolloutWhatIf(q *C.lwse_rollout_whatif) error {
+	return e.check(C.lwse_resident_rollout_whatif(e.h, q))
+}
+
 // DsDrain answers "does draining these nodes or topology domains take an inference service down, or
 // stall its rollout?" over the resident LWS and DS tables: the DisaggregatedSets whose linked child
 // LeaderWorkerSets lose ready groups, with SERVICE_LOST / OLD_SERVICE_LOST / STALLS verdicts and their

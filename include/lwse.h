@@ -32,6 +32,9 @@
  *                      203-236 (cleanup predicate), service_manager.go:57-89
  *   lwse_ds_resident_* the same arithmetic over resident DS tables, fed by DS and child-LWS
  *                      watch events (disaggregatedset_controller.go:55-126, :273)
+ *   lwse_resident_rollout_whatif  the sweep and the forecast above over a proposed LWS row: the
+ *                      encoder's leaderWorkerSetUpdated (leaderworkerset_controller.go:150-159,
+ *                      :325-332) into rollingUpdateParameters (:280-373), Case 4 (:351-361)
  *   lwse_resident_drain_*  pod_controller.go:204-266 (handleRestartPolicy), :268-295, :338-362 over
  *                      the resident tables with the pods of drained nodes deleting;
  *                      lwse_resident_drain_budget* adds a build-defined availability floor from
@@ -630,6 +633,47 @@ LWSE_API int lwse_lws_forecast_host(lwse_engine* e, const lwse_lws_rec* lws, uin
  * tick with LWSE_TICK_NO_SWEEP), until the next sweep is enqueued.  LWSE_ERR_INVALID_ARG for NULL
  * outputs; LWSE_ERR_UNSUPPORTED and LWSE_ERR_CUDA as for lwse_lws_forecast_host. */
 LWSE_API int lwse_resident_forecast(lwse_engine* e, lwse_lws_forecast_out* out);
+
+/* ---- rollout what-if ------------------------------------------------------------------------
+ * What a proposed edit of a LeaderWorkerSet would make the controller do, before the edit reaches the
+ * API server.  A query is a list of proposals (row L_i, lwse_lws_rec P_i), i = 0 .. n-1, each answered on
+ * its own as if it were the only edit; several proposals may name the same row (to compare settings).
+ *   - Ranges: P_i's group_base and group_count are ignored and taken from the resident row L_i (a
+ *     what-if moves no group rows).  Every other field is the caller's: rev_hash, flags (LWSE_LWS_UPDATED,
+ *     the percent, restart, startup and exclusive bits, INTSTR_INVALID, IRREGULAR), replicas, partition,
+ *     max_surge, max_unavailable, size, subgroup_size and the sts_* fields.  A template edit is rev_hash
+ *     set to the new revision's hash plus LWSE_LWS_UPDATED (what the encoder writes for
+ *     leaderWorkerSetUpdated, leaderworkerset_controller.go:150-159, :325-332); a scale is a changed
+ *     replicas, which Case 4 (:351-361) compares with the annotation the row already carries.
+ *   - now[i]: the lwse_lws_out row of L_i in a sweep of the resident tables with row L_i replaced by the
+ *     proposal, under the flags of the most recently submitted sweep: what the controller writes first.
+ *   - fc.lws[i] and the trajectory: lwse_resident_forecast's row of L_i over the same replaced tables (the
+ *     same rules, cap, flags and fields).  Proposal i's trajectory rows are contiguous at step_base; the
+ *     offsets run over the proposals in query order, with the TRUNCATED / step_capacity /
+ *     n_steps_written / n_steps_needed contract of lwse_lws_forecast_out.
+ *   - A group row inside L_i's range whose lws_index is not L_i keeps the result the resident sweep gave
+ *     it (its owner and pods are unchanged), so the answer is exactly the full replaced-table sweep's; only
+ *     the range rows L_i owns are recomputed.
+ *   - A resident row whose range lies outside the group table gets LWSE_LOUT_BAD_TABLE /
+ *     LWSE_LWSF_BAD_TABLE, as the sweep and the forecast give it, and gathers no group rows.
+ * Readiness, isolation and scratch as lwse_resident_forecast: LWSE_ERR_NOT_READY before
+ * lwse_resident_load and while the group results do not belong to the resident rows; the call holds the
+ * engine mutex, runs on a stream of its own behind an event on the engine's stream (it sees the most
+ * recently submitted tick, in flight or not), reads the resident tables in place, and never waits for,
+ * drains or drops a tick or touches a graph, arena, change list, output, occupancy counter, node index or
+ * tick info.  LWSE_ERR_INVALID_ARG for NULL or misaligned arrays or a row >= n_lws.  LWSE_ERR_UNSUPPORTED
+ * when the proposals' slots reach 2^31 (as the forecast refuses), or when the gathered group rows (the
+ * named rows' group_count summed over the proposals whose range lies inside the table) reach 2^32; an
+ * unsupported call writes nothing.  n == 0 is a valid empty answer. */
+typedef struct lwse_rollout_whatif {
+  const uint32_t* rows;      /* [n] resident LWS rows                                */
+  const lwse_lws_rec* recs;  /* [n] proposed rows, 16-byte aligned                   */
+  uint32_t n;
+  uint32_t reserved;
+  lwse_lws_out* now;         /* [n] out                                              */
+  lwse_lws_forecast_out fc;  /* fc.lws [n]; fc.steps [step_capacity] or NULL          */
+} lwse_rollout_whatif;
+LWSE_API int lwse_resident_rollout_whatif(lwse_engine* e, lwse_rollout_whatif* q);
 
 /* ------------------------------------------------------------------------- */
 /* Placement (build-defined spec — the reference has no node scoring)        */

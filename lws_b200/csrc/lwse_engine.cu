@@ -208,6 +208,10 @@ struct lwse_engine {
   cudaEvent_t ev_lf = nullptr;       // the engine's stream where a resident forecast takes its snapshot
   DevBuf lf_lws, lf_group_out, lf_slot_off, lf_slots, lf_fc, lf_steps, lf_totals;
   PinBuf lf_words;                   // the three totals, copied back
+  // rollout what-if (lwse_resident_rollout_whatif): on lf_stream, the proposals' rows and their resident rows, the
+  // layout's offsets and block sums, the gathered group rows with their foreign-row record, the sweep's results
+  // and scratch; the forecast that follows uses the lf_* scratch above
+  DevBuf rw_rows, rw_lws, rw_off, rw_sums, rw_groups, rw_src, rw_group_out, rw_now, rw_scan;
   bool r_place_current = false;      // r_pout holds the round of the resident node, request and identity rows: a
                                      // tick with LWSE_TICK_PLACE was submitted since lwse_resident_place_load and
                                      // since any patch of those rows made without a round
@@ -455,7 +459,8 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->dr_domains, &e->dr_brows, &e->dr_bcost, &e->dr_table, &e->dr_bwords,
                       &e->dd_lost, &e->dd_lws_after, &e->dd_out[0], &e->dd_out[1], &e->dd_role_out[0], &e->dd_role_out[1],
                       &e->dd_revrole_out[0], &e->dd_revrole_out[1], &e->dd_rows, &e->dd_index, &e->dd_entries, &e->dd_cost,
-                      &e->dd_table};
+                      &e->dd_table, &e->rw_rows, &e->rw_lws, &e->rw_off, &e->rw_sums, &e->rw_groups, &e->rw_src,
+                      &e->rw_group_out, &e->rw_now, &e->rw_scan};
     if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
     if (e->lf_stream) cudaStreamSynchronize(e->lf_stream);
     if (e->wf_stream) cudaStreamSynchronize(e->wf_stream);
@@ -3502,6 +3507,103 @@ LWSE_API int lwse_resident_forecast(lwse_engine* e, lwse_lws_forecast_out* out) 
   h.group_out = (const lwse_group_out*)e->lf_group_out.p;
   h.n_groups = e->rn_groups;
   return lws_forecast_locked(e, h, out, e->lf_stream);
+}
+
+// ---- rollout what-if ----
+// On lf_stream behind an event on the engine's stream; reads the resident rows, groups, pods and group
+// results in place (the mutex keeps the next tick out until the call returns).  The layout sizes the
+// gathered group table at one synchronisation; the gather, the sweep's group pass, the restore of the
+// foreign-owned rows and the LWS pass follow, then the forecast over the proposals' rows.  `now` is copied
+// out last, so that a refused forecast writes nothing.
+LWSE_API int lwse_resident_rollout_whatif(lwse_engine* e, lwse_rollout_whatif* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->r_loaded || !e->r_groups_swept) return LWSE_ERR_NOT_READY;
+  const uint32_t n = q->n;
+  if (n && (!q->rows || !q->recs || !q->now || !q->fc.lws)) return LWSE_ERR_INVALID_ARG;
+  if (!aligned16(q->recs)) return LWSE_ERR_INVALID_ARG;
+  for (uint32_t i = 0; i < n; i++)
+    if (q->rows[i] >= e->rn_lws) return LWSE_ERR_INVALID_ARG;
+  if (n == 0) {
+    q->fc.n_steps_written = 0;
+    q->fc.n_steps_needed = 0;
+    return LWSE_OK;
+  }
+  DeviceGuard guard(e->device);
+  if (const int rc = lws_forecast_stream(e); rc != LWSE_OK) return rc;
+  if (!e->ev_lf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_lf, cudaEventDisableTiming));
+  cudaStream_t s = e->lf_stream;
+  LWSE_CUDA(e, e->rw_rows.reserve((size_t)n * 4 + 16));
+  LWSE_CUDA(e, e->rw_lws.reserve((size_t)n * sizeof(lwse_lws_rec) + 16));
+  LWSE_CUDA(e, e->rw_off.reserve((size_t)n * 8 + 16));
+  LWSE_CUDA(e, e->rw_sums.reserve(16 + (size_t)lwse::forecast_scan_words(n) * 8));  // [0] total, then the block sums
+  LWSE_CUDA(e, e->lf_words.reserve(32));
+  LWSE_CUDA(e, cudaMemcpyAsync(e->rw_rows.p, q->rows, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(e->rw_lws.p, q->recs, (size_t)n * sizeof(lwse_lws_rec), cudaMemcpyHostToDevice, s));
+  LWSE_CUDA(e, cudaEventRecord(e->ev_lf, e->stream));
+  LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_lf, 0));
+  unsigned long long* d_sums = (unsigned long long*)e->rw_sums.p;
+  lwse::RolloutWhatifHost h{};
+  h.lws = (const lwse_lws_rec*)e->r_lws.p;
+  h.groups = (const lwse_group_rec*)e->r_groups.p;
+  h.n_groups = e->rn_groups;
+  h.rows = (const uint32_t*)e->rw_rows.p;
+  h.n = n;
+  h.off = (unsigned long long*)e->rw_off.p;
+  h.s_lws = (lwse_lws_rec*)e->rw_lws.p;
+  int cuda_err = 0;
+  int launched = lwse::launch_rollout_whatif_layout(&h, d_sums + 2, d_sums, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  uint64_t* words = static_cast<uint64_t*>(e->lf_words.h);
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_sums, 8, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint64_t gathered = words[0];
+  if (gathered >= 0x100000000ull) return LWSE_ERR_UNSUPPORTED;  // the scratch rows are indexed with uint32
+  const uint32_t ng = (uint32_t)gathered;
+  const uint64_t np = e->rn_pods;
+  LWSE_CUDA(e, e->rw_groups.reserve((size_t)ng * sizeof(lwse_group_rec) + 16));
+  LWSE_CUDA(e, e->rw_src.reserve((size_t)ng * 4 + 16));
+  LWSE_CUDA(e, e->rw_group_out.reserve((size_t)ng * sizeof(lwse_group_out) + 16));
+  LWSE_CUDA(e, e->rw_now.reserve((size_t)n * sizeof(lwse_lws_out) + 16));
+  LWSE_CUDA(e, e->rw_scan.reserve(lwse::lws_sweep_scratch_bytes(np, ng)));
+  h.s_groups = (lwse_group_rec*)e->rw_groups.p;
+  h.s_src = (uint32_t*)e->rw_src.p;
+  launched = lwse::launch_rollout_whatif_gather(&h, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  // the group pass over {proposal rows, gathered groups, resident pods}, no occupancy
+  lwse_lws_tables d{};
+  d.lws = (const lwse_lws_rec*)e->rw_lws.p;
+  d.n_lws = n;
+  d.groups = (const lwse_group_rec*)e->rw_groups.p;
+  d.n_groups = ng;
+  d.pod_state = (const lwse_pod_state*)e->r_pst.p;
+  d.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
+  d.n_pods = np;
+  d.lws_out = (lwse_lws_out*)e->rw_now.p;
+  d.group_out = (lwse_group_out*)e->rw_group_out.p;
+  d.flags = e->r_sweep_flags | LWSE_SWEEP_SKIP_LWS_PASS;
+  const lwse_node_rec* nodes = (const lwse_node_rec*)e->nodes.p;
+  launched = lwse::launch_lws_sweep(&d, nodes, e->n_nodes, e->rw_scan.p, e->sm_count, s, &cuda_err, nullptr, nullptr,
+                                    /*first_mode=*/0);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  // the rows other objects own keep the resident sweep's result, where the forecast and the LWS pass read it
+  launched = lwse::launch_rollout_whatif_restore(h.s_src, (const lwse_group_out*)e->r_group_out.p, d.group_out,
+                                                 lwse::lws_sweep_flag_column(e->rw_scan.p, np), ng, e->sm_count, s,
+                                                 &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  d.flags = e->r_sweep_flags | LWSE_SWEEP_SKIP_GROUP_PASS | LWSE_SWEEP_SKIP_POD_SCAN;  // the LWS pass alone
+  launched = lwse::launch_lws_sweep(&d, nodes, e->n_nodes, e->rw_scan.p, e->sm_count, s, &cuda_err, nullptr, nullptr,
+                                    /*first_mode=*/0);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  lwse::LwsForecastHost f{};
+  f.lws = (const lwse_lws_rec*)e->rw_lws.p;
+  f.n_lws = n;
+  f.group_out = (const lwse_group_out*)e->rw_group_out.p;
+  f.n_groups = ng;
+  if (const int rc = lws_forecast_locked(e, f, &q->fc, s); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(q->now, e->rw_now.p, (size_t)n * sizeof(lwse_lws_out), cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  return LWSE_OK;
 }
 
 // ---------------------------------------------------------------------------

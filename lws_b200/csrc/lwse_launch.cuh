@@ -31,6 +31,9 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
                      void* scratch, int sm_count, cudaStream_t s, int* cuda_err, const SweepChangeLists* cl,
                      uint32_t* d_event_count = nullptr, int first_mode = 1);
 size_t lws_sweep_scratch_bytes(uint64_t n_pods, uint32_t n_groups);
+// The sweep scratch's flag column: one byte per group row, the low five bits of its group_out.flags, which
+// the group pass writes and the LWS pass reads.
+uint8_t* lws_sweep_flag_column(void* scratch, uint64_t n_pods);
 
 struct PublishListHost {
   const uint32_t* src_rows;
@@ -216,6 +219,27 @@ struct LwsForecastHost {
 };
 int launch_lws_forecast_slots(const LwsForecastHost* h, int sm_count, cudaStream_t s, int* cuda_err);
 int launch_lws_forecast(const LwsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s, int* cuda_err);
+
+// ---- lwse_rollout_whatif_kernels.cu ----
+struct RolloutWhatifHost {
+  const lwse_lws_rec* lws;        // the resident rows
+  const lwse_group_rec* groups;   // the resident group rows
+  uint32_t n_groups;
+  const uint32_t* rows;           // [n] the proposals' resident rows (< n_lws, checked by the engine)
+  uint32_t n;
+  unsigned long long* off;        // [n] each proposal's first scratch group row (the layout writes them)
+  lwse_lws_rec* s_lws;            // [n] the proposed rows; the gather sets group_base / group_count
+  lwse_group_rec* s_groups;       // the gathered group rows
+  uint32_t* s_src;                // per gathered row: the resident row of a foreign-owned row, else LWSE_NONE
+};
+// The layout: off[i] = the exclusive prefix of the proposals' gathered rows, *total = their sum (u64).
+// sums: forecast_scan_words(n) words.
+int launch_rollout_whatif_layout(const RolloutWhatifHost* h, unsigned long long* sums, unsigned long long* total,
+                                 cudaStream_t s, int* cuda_err);
+int launch_rollout_whatif_gather(const RolloutWhatifHost* h, int sm_count, cudaStream_t s, int* cuda_err);
+// The foreign-owned rows' baseline results into d_out and the sweep's flag column (lws_sweep_flag_column).
+int launch_rollout_whatif_restore(const uint32_t* d_src, const lwse_group_out* d_baseline, lwse_group_out* d_out,
+                                  uint8_t* d_gflag8, uint32_t n_rows, int sm_count, cudaStream_t s, int* cuda_err);
 
 // ---- lwse_drain_kernels.cu ----
 // The drain what-if's counters (device, 16 words, zeroed by the caller): [0] changed rows [1] pods evicted

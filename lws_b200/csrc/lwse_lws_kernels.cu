@@ -764,6 +764,9 @@ static uint64_t bitmap_words(uint64_t n_pods) { return ((n_pods + 31u) / 32u + 3
 size_t lws_sweep_scratch_bytes(uint64_t n_pods, uint32_t n_groups) {
   return (size_t)(2 * bitmap_words(n_pods) * sizeof(uint32_t) + (((uint64_t)n_groups + 7u) & ~7ull) + 256);
 }
+uint8_t* lws_sweep_flag_column(void* scratch, uint64_t n_pods) {
+  return reinterpret_cast<uint8_t*>(static_cast<uint32_t*>(scratch) + 2 * bitmap_words(n_pods));
+}
 
 // Returns the number of kernels launched (>=0) or -1 with *cuda_err set.
 // scratch: lws_sweep_scratch_bytes(n_pods, n_groups) bytes of device memory.

@@ -98,6 +98,7 @@ SYMBOLS = {
     "lwse_lws_forecast_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(R.LwsForecastOut)], C.c_int),
     "lwse_resident_forecast": ([C.c_void_p, C.POINTER(R.LwsForecastOut)], C.c_int),
+    "lwse_resident_rollout_whatif": ([C.c_void_p, C.POINTER(R.RolloutWhatIf)], C.c_int),
     "lwse_group_keys_host": ([C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_subgroup_keys_host": (
         [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int),
@@ -774,6 +775,31 @@ class Engine:
         n_lws = getattr(self, "_resident_shape", (0, 0))[0]
         return self._lws_forecast(lambda o: lib().lwse_resident_forecast(self._h, C.byref(o)), n_lws, steps,
                                   step_capacity)
+
+    def resident_rollout_whatif(self, rows, recs, steps=True, step_capacity=None):
+        """lwse_resident_rollout_whatif: for each proposal (resident row ``rows[i]``, proposed LWS_REC
+        ``recs[i]``), the controller's first write (``now``, LWS_OUT) and the forecast of the rollout it
+        would start, each as if it were the only edit (lwse.h, "rollout what-if").  The proposals'
+        group_base / group_count are taken from the resident rows.  → ``now`` plus what
+        ``resident_forecast`` returns, with one ``lws`` row per proposal and the trajectory offsets running
+        over the proposals in order.  Changes nothing resident and waits for no tick."""
+        rows = np.ascontiguousarray(rows, dtype=np.uint32)
+        recs = np.asarray(recs)
+        assert recs.dtype == R.LWS_REC and len(recs) == len(rows)
+        recs = _aligned16(recs)
+        now = R.aligned_empty(len(rows), R.LWS_OUT)
+        n = len(rows)
+
+        def call(o):
+            q = R.RolloutWhatIf(R.ptr(rows) if n else None, R.ptr(recs) if n else None, n, 0,
+                                R.ptr(now) if n else None, o)
+            rc = lib().lwse_resident_rollout_whatif(self._h, C.byref(q))
+            o.n_steps_written, o.n_steps_needed = q.fc.n_steps_written, q.fc.n_steps_needed
+            return rc
+
+        out = self._lws_forecast(call, n, steps, step_capacity)
+        out["now"] = now
+        return out
 
     # ------------------------------------------------------------- group keys
     def group_keys_host(self, strings) -> np.ndarray:

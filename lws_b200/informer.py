@@ -38,7 +38,7 @@ engine's resident tick runs the placement round through a namespace index (DESIG
 """
 from __future__ import annotations
 
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from typing import Optional
 
 import numpy as np
@@ -536,6 +536,22 @@ class IncrementalEncoder:
             return R.aligned_empty(0, R.PLACE_REQ)
         return self._whatif_requests(int(self.lws["uid_hash"][row]), int(self.lws["size"][row]), self.ns_ids[key[0]],
                                      range(self.items[key].lws.replicas, replicas))
+
+    def whatif_rollout(self, item: encoder.LwsItem) -> tuple:
+        """A proposal for ``Engine.resident_rollout_whatif``: ``item`` is what ``lws_event`` would take for
+        the edit (with its own ``revision_key`` and ``lws_updated``), encoded with the object's cached pods
+        and StatefulSets as the next ``flush()`` would encode it → (LWS row, LWS_REC row).  Nothing in the
+        encoder changes.  KeyError for an object that is not resident."""
+        key = (item.lws.namespace, item.lws.name)
+        sl = self.slots[key]
+        if item.leader_sts is None:  # as lws_event: the cached leader StatefulSet
+            item = replace(item, leader_sts=self.items[key].leader_sts)
+        cl = encoder.Cluster(pods=list(self.pods.get(key, {}).values()),
+                             statefulsets=list(self.sts.get(key, {}).values()))
+        t = encoder.encode_lws([item], cl, self.topology_key, encoded_nodes=self._encoded_nodes)
+        rec = t.lws.copy()
+        rec["group_base"] = sl.group_base
+        return sl.lws_row, rec[0]
 
     def whatif_drain(self, node_names) -> np.ndarray:
         """The node rows of the named nodes, for ``Engine.resident_drain_whatif`` (sorted, each once)."""

@@ -470,6 +470,20 @@ class LwsForecastOut(C.Structure):
     ]
 
 
+class RolloutWhatIf(C.Structure):
+    """lwse_rollout_whatif: proposed LWS rows for resident rows in; the controller's first write and the
+    forecast of the rollout each proposal would start out."""
+
+    _fields_ = [
+        ("rows", C.c_void_p),
+        ("recs", C.c_void_p),
+        ("n", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("now", C.c_void_p),
+        ("fc", LwsForecastOut),
+    ]
+
+
 class PlaceWhatIf(C.Structure):
     """lwse_place_whatif: a hypothetical placement round over the resident tables (segments and extra
     rows in, changed rows and the PLACE_WHATIF counters out)."""
