@@ -178,6 +178,16 @@ func (e *Engine) RolloutWhatIf(q *C.lwse_rollout_whatif) error {
 	return e.check(C.lwse_resident_rollout_whatif(e.h, q))
 }
 
+// DsRolloutWhatIf answers "if this DisaggregatedSet edit were pushed, what would its rollout do?" over the
+// resident DS tables without changing them: per proposal (a DS row, NEW_REVISION for a template edit, ROLES with
+// new role rows for a scale or new rollout settings) the DS controller's first decision, read through the child
+// links as the DS tick reads them, and the forecast of the rollout it starts — steps, peak replicas and the
+// availability floor per role.  It never waits for or drops a tick.  A validating webhook calls it on a DS update;
+// a fleet image bump asks one proposal per DS in one call.
+func (e *Engine) DsRolloutWhatIf(q *C.lwse_ds_rollout_whatif) error {
+	return e.check(C.lwse_resident_ds_rollout_whatif(e.h, q))
+}
+
 // DsDrain answers "does draining these nodes or topology domains take an inference service down, or
 // stall its rollout?" over the resident LWS and DS tables: the DisaggregatedSets whose linked child
 // LeaderWorkerSets lose ready groups, with SERVICE_LOST / OLD_SERVICE_LOST / STALLS verdicts and their

@@ -35,6 +35,9 @@
  *   lwse_resident_rollout_whatif  the sweep and the forecast above over a proposed LWS row: the
  *                      encoder's leaderWorkerSetUpdated (leaderworkerset_controller.go:150-159,
  *                      :325-332) into rollingUpdateParameters (:280-373), Case 4 (:351-361)
+ *   lwse_resident_ds_rollout_whatif  the DS sweep and forecast above over the rows a proposed DS edit
+ *                      encodes to: a new ComputeRevision(spec.roles) (utils.go:173-199) retires the
+ *                      target revision into the old ones (GroupByRevision, utils.go:192-211)
  *   lwse_resident_drain_*  pod_controller.go:204-266 (handleRestartPolicy), :268-295, :338-362 over
  *                      the resident tables with the pods of drained nodes deleting;
  *                      lwse_resident_drain_budget* adds a build-defined availability floor from
@@ -1315,6 +1318,76 @@ LWSE_API int lwse_ds_forecast_host(lwse_engine* e, const lwse_ds_tables* host, l
  * lwse_ds_resident_load); every other call waits only on the DS stream.  LWSE_ERR_NOT_READY before
  * lwse_ds_resident_load; LWSE_ERR_INVALID_ARG for NULL outputs. */
 LWSE_API int lwse_ds_resident_forecast(lwse_engine* e, lwse_ds_forecast_out* out);
+
+/* ---- DS rollout what-if -------------------------------------------------------------------
+ * What a proposed edit of a DisaggregatedSet would make the DS controller do, before the edit reaches the
+ * API server: a new image (a template edit, so a new target revision), a scale, or new maxSurge /
+ * maxUnavailable.  A query is a list of proposals, each answered on its own as if it were the only edit;
+ * several proposals may name the same DS (to compare settings).  For proposal i on resident DS row D
+ * (n roles, V old revisions, header flags h) the proposed rows P_i are:
+ *   - BAD_TABLE: D's resident row fails the sweep's limits or range test.  now[i] = {LWSE_DOUT_BAD_TABLE,
+ *     0, 0, 0}, fc.ds[i].flags = LWSE_DSF_BAD_TABLE, its role rows in now_roles and fc.roles are 0 and
+ *     nothing is gathered.  (A vacant, zeroed row is answered as the sweep answers it.)
+ *   - Roles: D's n resident role rows, or with LWSE_DSP_ROLES the n rows at q->roles[i*10 .. i*10+n),
+ *     in the resident order (spec roles, then removed roles); n_spec_roles stays the resident one.  A
+ *     scale (target_replicas) or new rollout settings: ComputeRevision hashes only role names and templates
+ *     (utils.go:173-199), so neither changes the revision.
+ *   - Revision-role rows without LWSE_DSP_NEW_REVISION: D's (V+1)*n rows as they are.
+ *   - With LWSE_DSP_NEW_REVISION, when h has LWSE_DS_HAS_NEW_REVISION, the target revision retires:
+ *     V' = V + 1; old revisions 0..V-1 as resident; old revision V is D's current new-revision rows,
+ *     unchanged; the new revision's n rows are absent {0, -1, 0, 0}; LWSE_DS_HAS_NEW_REVISION is cleared.
+ *     V' > LWSE_DS_MAX_OLD_REVS makes the proposal BAD_TABLE, as the sweep reports the re-encoded DS.
+ *   - With LWSE_DSP_NEW_REVISION, without LWSE_DS_HAS_NEW_REVISION: the target revision has no children to
+ *     retire; V' = V and the rows are unchanged.
+ *   - Links: a proposed row copied from resident row r carries r's link row; rows the edit creates carry
+ *     none.  `now` follows the DS tick's link state: the rows are linked only after a link patch since the
+ *     DS load, and LWS results count only while the LWS tables are loaded and swept.
+ * P_i is exactly what the encoder writes for the edited object (same children, new target revision) when
+ * the retired revision's children come last in List order; any other List order only permutes old
+ * revisions.
+ *   - now[i], now_roles[i*10 + j]: the ds_out / role_out rows of the linked DS sweep of P_i with the DS
+ *     tick's device code and link rule: what the DS controller does first.  The bits of drained_revs /
+ *     ready_revs number P_i's old revisions (the retired revision is bit V).
+ *   - fc: lwse_ds_resident_forecast's rules over P_i (links ignored, as there), into fc.ds[i] and
+ *     fc.roles[i*10 + j].  Proposal i's trajectory rows are contiguous at step_base, the offsets running
+ *     over the proposals in query order, with the TRUNCATED / step_capacity / n_steps_written /
+ *     n_steps_needed contract of lwse_ds_forecast_out.
+ * Role rows j >= n of a proposal read 0 in now_roles and fc.roles.
+ * Readiness and errors: LWSE_ERR_NOT_READY before lwse_ds_resident_load.  LWSE_ERR_INVALID_ARG for a NULL q;
+ * n > 0 with NULL proposals, now, fc.ds or fc.roles; a LWSE_DSP_ROLES proposal with NULL or misaligned roles;
+ * ds >= n_ds; unknown flag bits; reserved != 0.  LWSE_ERR_UNSUPPORTED when n > LWSE_DS_WHATIF_MAX_PROPOSALS
+ * (checked before any array is read: the gathered rows then always index with uint32).  A failed call
+ * writes nothing; n == 0 is a valid empty answer.
+ * Isolation as lwse_resident_ds_drain: the what-if stream under the engine mutex, behind an event on the DS
+ * stream and one on the engine's stream (it sees the last DS tick and the most recently submitted LWS tick,
+ * in flight or not), with scratch of its own that only grows.  It touches no tick, graph, arena, change
+ * list, resident LWS or DS table, link table, DS tick output, mirror or marks, tick info or counter, and
+ * never waits for, drains or drops an LWS tick.
+ * Out of scope: edits that add, remove or rename a role (they change allRoleNames and the row layout;
+ * re-encode the object and call lwse_ds_forecast_host), edits that move a role between the spec and the removed
+ * roles (n_spec_roles stays the resident one), and DS whose children live on another rank (each
+ * rank answers its own DS). */
+typedef struct lwse_ds_proposal { /* 8 B */
+  uint32_t ds;                    /* resident DS row */
+  uint32_t flags;                 /* LWSE_DSP_* */
+} lwse_ds_proposal;
+#define LWSE_DSP_NEW_REVISION (1u << 0) /* the edit changes ComputeRevision(spec.roles): a template edit */
+#define LWSE_DSP_ROLES (1u << 1)        /* proposal i's role rows are q->roles[i*LWSE_DS_MAX_ROLES ..]  */
+/* floor((2^32 - 1) / ((LWSE_DS_MAX_OLD_REVS + 1) * LWSE_DS_MAX_ROLES)) */
+#define LWSE_DS_WHATIF_MAX_PROPOSALS 13015052u
+
+typedef struct lwse_ds_rollout_whatif {
+  const lwse_ds_proposal* proposals; /* [n] */
+  const lwse_ds_role_rec* roles;     /* [n * LWSE_DS_MAX_ROLES], 16-byte aligned; read only for LWSE_DSP_ROLES
+                                        proposals (may be NULL when none has it) */
+  uint32_t n;
+  uint32_t reserved;                 /* 0 */
+  lwse_ds_out* now;                  /* [n] out */
+  lwse_ds_role_out* now_roles;       /* [n * LWSE_DS_MAX_ROLES] out, or NULL */
+  lwse_ds_forecast_out fc;           /* fc.ds [n], fc.roles [n * LWSE_DS_MAX_ROLES], fc.steps [step_capacity] or
+                                        NULL */
+} lwse_ds_rollout_whatif;
+LWSE_API int lwse_resident_ds_rollout_whatif(lwse_engine* e, lwse_ds_rollout_whatif* q);
 
 /* ---- DS drain ------------------------------------------------------------------------------
  * "Does this drain take an inference service down, or stall its rollout?"  A DisaggregatedSet serves

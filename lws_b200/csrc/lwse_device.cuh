@@ -112,6 +112,15 @@ __device__ __forceinline__ int32_t scaled_value(int32_t val, bool is_percent, in
   return (int32_t)q;
 }
 
+// The table checks of one DS (BAD_TABLE when they fail): its ranges lie inside the tables.  The DS sweep,
+// tick, forecast and drain, and the DS rollout what-if, which decides the same way for a proposal.
+__device__ __forceinline__ bool ds_rows_ok(const lwse_ds_tables& t, const uint4 h0, const uint4 h1) {
+  const uint32_t role_base = h0.z, n_roles = h0.w, n_spec = h1.x, rev_base = h1.y, n_old = h1.z;
+  return !(n_roles > LWSE_DS_MAX_ROLES || n_spec > n_roles || n_old > LWSE_DS_MAX_OLD_REVS ||
+           (uint64_t)role_base + n_roles > t.n_roles ||
+           (uint64_t)rev_base + (uint64_t)(n_old + 1u) * n_roles > t.n_revroles);
+}
+
 // Programmatic dependent launch (PDL): the kernels of one sweep are launched
 // with programmatic stream serialization, call pdl_launch_dependents() first
 // thing (the next kernel may start its own prologue) and pdl_wait_prior()

@@ -258,14 +258,6 @@ __device__ __forceinline__ void ds_tick_diff(const lwse_ds_tables& t, const DsTi
   a.rows[base + __popc(m & ((1u << lane) - 1u))] = d;
 }
 
-// The table checks of one DS (BAD_TABLE when they fail): its ranges lie inside the tables.
-__device__ __forceinline__ bool ds_rows_ok(const lwse_ds_tables& t, const uint4 h0, const uint4 h1) {
-  const uint32_t role_base = h0.z, n_roles = h0.w, n_spec = h1.x, rev_base = h1.y, n_old = h1.z;
-  return !(n_roles > LWSE_DS_MAX_ROLES || n_spec > n_roles || n_old > LWSE_DS_MAX_OLD_REVS ||
-           (uint64_t)role_base + n_roles > t.n_roles ||
-           (uint64_t)rev_base + (uint64_t)(n_old + 1u) * n_roles > t.n_revroles);
-}
-
 // How the sweep body reads revision-role rows.  The sweep and the tick read input tables that
 // nothing in the kernel writes: ld.global.nc.  The forecast rewrites its scratch copy of the rows
 // between the cycles of one kernel, so it reads them with coherent loads, ordered after the thread's

@@ -236,6 +236,12 @@ struct lwse_engine {
   // touched DS rows, the reverse link index (count | first | cursor) and its entries, the key rows, the (DS, key) table
   DevBuf dd_lost, dd_lws_after, dd_out[2], dd_role_out[2], dd_revrole_out[2], dd_rows, dd_index, dd_entries, dd_cost, dd_table;
   cudaEvent_t ev_dd = nullptr;       // the DS stream where a DS drain starts
+  // DS rollout what-if (lwse_resident_ds_rollout_whatif): on the what-if stream, the proposals and the query's role
+  // rows, the layout's counts, offsets and block sums, the proposed DS, role, revision-role and link rows, and the
+  // linked sweep's outputs; the forecast that follows uses the fc_* scratch above
+  DevBuf dw_props, dw_qroles, dw_count, dw_off, dw_sums, dw_ds, dw_roles, dw_revroles, dw_links, dw_now, dw_role_out,
+      dw_revrole_out;
+  PinBuf dw_words;                   // the layout's total, copied back
   uint32_t r_sweep_flags = 0;        // LWSE_SWEEP_GANG of the most recently submitted sweep (r_group_out's flags)
   DevBuf sha_bytes, sha_offsets, sha_digests, sha_ints;
   uint32_t* h_rounds = nullptr;  // pinned
@@ -460,13 +466,15 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->dd_lost, &e->dd_lws_after, &e->dd_out[0], &e->dd_out[1], &e->dd_role_out[0], &e->dd_role_out[1],
                       &e->dd_revrole_out[0], &e->dd_revrole_out[1], &e->dd_rows, &e->dd_index, &e->dd_entries, &e->dd_cost,
                       &e->dd_table, &e->rw_rows, &e->rw_lws, &e->rw_off, &e->rw_sums, &e->rw_groups, &e->rw_src,
-                      &e->rw_group_out, &e->rw_now, &e->rw_scan};
+                      &e->rw_group_out, &e->rw_now, &e->rw_scan, &e->dw_props, &e->dw_qroles, &e->dw_count, &e->dw_off,
+                      &e->dw_sums, &e->dw_ds, &e->dw_roles, &e->dw_revroles, &e->dw_links, &e->dw_now, &e->dw_role_out,
+                      &e->dw_revrole_out};
     if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
     if (e->lf_stream) cudaStreamSynchronize(e->lf_stream);
     if (e->wf_stream) cudaStreamSynchronize(e->wf_stream);
     for (DevBuf* b : bufs) b->release();
     PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc, &e->rd_pin, &e->rd_stage, &e->fc_words, &e->lf_words,
-                      &e->wf_stage, &e->wf_words};
+                      &e->wf_stage, &e->wf_words, &e->dw_words};
     for (PinBuf* b : pins) b->release();
     if (e->ev_place) cudaEventDestroy(e->ev_place);
     if (e->h_rounds) cudaFreeHost(e->h_rounds);
@@ -3397,6 +3405,106 @@ LWSE_API int lwse_ds_resident_forecast(lwse_engine* e, lwse_ds_forecast_out* out
   d.revroles = (const lwse_ds_revrole_rec*)e->rd_revroles.p;
   d.n_revroles = e->rdn_revroles;
   return forecast_locked(e, d, out, e->ds_stream);
+}
+
+// ---- DS rollout what-if ----
+// On wf_stream behind an event on the DS stream and one on the engine's stream (ds_drain_begin_locked); reads the
+// resident DS rows, link rows and LWS results in place (the mutex keeps the next tick of either kind out until the
+// call returns).  The layout sizes the gathered tables at one synchronisation; the gather, the linked sweep of the
+// proposed rows and the forecast over them follow.  `now` is copied out last.
+LWSE_API int lwse_resident_ds_rollout_whatif(lwse_engine* e, lwse_ds_rollout_whatif* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->rd_loaded) return LWSE_ERR_NOT_READY;
+  if (q->reserved) return LWSE_ERR_INVALID_ARG;
+  const uint32_t n = q->n;
+  if (n > LWSE_DS_WHATIF_MAX_PROPOSALS) return LWSE_ERR_UNSUPPORTED;
+  if (n && (!q->proposals || !q->now || !q->fc.ds || !q->fc.roles)) return LWSE_ERR_INVALID_ARG;
+  bool any_roles = false;
+  for (uint32_t i = 0; i < n; i++) {
+    const lwse_ds_proposal p = q->proposals[i];
+    if (p.ds >= e->rdn_ds || (p.flags & ~(LWSE_DSP_NEW_REVISION | LWSE_DSP_ROLES))) return LWSE_ERR_INVALID_ARG;
+    any_roles |= (p.flags & LWSE_DSP_ROLES) != 0;
+  }
+  if (any_roles && (!q->roles || !aligned16(q->roles))) return LWSE_ERR_INVALID_ARG;
+  if (n == 0) {
+    q->fc.n_steps_written = 0;
+    q->fc.n_steps_needed = 0;
+    return LWSE_OK;
+  }
+  DeviceGuard guard(e->device);
+  if (!e->wf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->wf_stream, cudaStreamNonBlocking));
+  cudaStream_t s = e->wf_stream;
+  const size_t nr = (size_t)n * LWSE_DS_MAX_ROLES;
+  LWSE_CUDA(e, e->dw_props.reserve((size_t)n * sizeof(lwse_ds_proposal) + 16));
+  if (any_roles) LWSE_CUDA(e, e->dw_qroles.reserve(nr * sizeof(lwse_ds_role_rec) + 16));
+  LWSE_CUDA(e, e->dw_count.reserve((size_t)n * 4 + 16));
+  LWSE_CUDA(e, e->dw_off.reserve((size_t)n * 4 + 16));
+  LWSE_CUDA(e, e->dw_sums.reserve(16 + (size_t)lwse::forecast_scan_words(n) * 8));  // [0] total, then the block sums
+  LWSE_CUDA(e, e->dw_ds.reserve((size_t)n * sizeof(lwse_ds_rec) + 16));
+  LWSE_CUDA(e, e->dw_roles.reserve(nr * sizeof(lwse_ds_role_rec) + 16));
+  LWSE_CUDA(e, e->dw_now.reserve((size_t)n * sizeof(lwse_ds_out) + 16));
+  LWSE_CUDA(e, e->dw_role_out.reserve(nr * sizeof(lwse_ds_role_out) + 16));
+  LWSE_CUDA(e, e->dw_words.reserve(16));
+  LWSE_CUDA(e, cudaMemcpyAsync(e->dw_props.p, q->proposals, (size_t)n * sizeof(lwse_ds_proposal), cudaMemcpyHostToDevice, s));
+  if (any_roles)
+    LWSE_CUDA(e, cudaMemcpyAsync(e->dw_qroles.p, q->roles, nr * sizeof(lwse_ds_role_rec), cudaMemcpyHostToDevice, s));
+  if (const int rc = ds_drain_begin_locked(e); rc != LWSE_OK) return rc;
+  lwse::DsWhatifHost h{};
+  h.t.ds = (const lwse_ds_rec*)e->rd_ds.p;
+  h.t.n_ds = e->rdn_ds;
+  h.t.roles = (const lwse_ds_role_rec*)e->rd_roles.p;
+  h.t.n_roles = e->rdn_roles;
+  h.t.revroles = (const lwse_ds_revrole_rec*)e->rd_revroles.p;
+  h.t.n_revroles = e->rdn_revroles;
+  h.links = (const lwse_ds_link*)e->rd_links.p;
+  h.proposals = (const lwse_ds_proposal*)e->dw_props.p;
+  h.q_roles = any_roles ? (const lwse_ds_role_rec*)e->dw_qroles.p : nullptr;
+  h.n = n;
+  h.count = (uint32_t*)e->dw_count.p;
+  h.off = (uint32_t*)e->dw_off.p;
+  h.s_ds = (lwse_ds_rec*)e->dw_ds.p;
+  h.s_roles = (lwse_ds_role_rec*)e->dw_roles.p;
+  unsigned long long* d_sums = (unsigned long long*)e->dw_sums.p;
+  int cuda_err = 0;
+  int launched = lwse::launch_ds_whatif_layout(&h, d_sums + 2, d_sums, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  uint64_t* words = static_cast<uint64_t*>(e->dw_words.h);
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_sums, 8, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint32_t nrr = (uint32_t)words[0];  // <= 330 n < 2^32 (the cap on n)
+  LWSE_CUDA(e, e->dw_revroles.reserve((size_t)nrr * sizeof(lwse_ds_revrole_rec) + 16));
+  LWSE_CUDA(e, e->dw_links.reserve((size_t)nrr * sizeof(lwse_ds_link) + 16));
+  LWSE_CUDA(e, e->dw_revrole_out.reserve((size_t)nrr * sizeof(lwse_ds_revrole_out) + 16));
+  h.s_revroles = (lwse_ds_revrole_rec*)e->dw_revroles.p;
+  h.s_links = (lwse_ds_link*)e->dw_links.p;
+  launched = lwse::launch_ds_whatif_gather(&h, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  // the DS tick's first decision over the proposed rows: the linked sweep under the tick's link state (linked only
+  // after a link patch since the DS load; LWS results only while the LWS rows are loaded and swept)
+  lwse_ds_tables t{};
+  t.ds = (const lwse_ds_rec*)e->dw_ds.p;
+  t.n_ds = n;
+  t.roles = (const lwse_ds_role_rec*)e->dw_roles.p;
+  t.n_roles = (uint32_t)nr;
+  t.revroles = (const lwse_ds_revrole_rec*)e->dw_revroles.p;
+  t.n_revroles = nrr;
+  t.ds_out = (lwse_ds_out*)e->dw_now.p;
+  t.role_out = (lwse_ds_role_out*)e->dw_role_out.p;
+  t.revrole_out = (lwse_ds_revrole_out*)e->dw_revrole_out.p;
+  LWSE_CUDA(e, cudaMemsetAsync(t.role_out, 0, nr * sizeof(lwse_ds_role_out), s));  // role rows no sweep writes read 0
+  const bool lws_results = e->rd_linked && e->r_loaded && e->r_swept;
+  const lwse::DsDrainLink lk{(const lwse_ds_link*)e->dw_links.p, (const lwse_lws_rec*)e->r_lws.p,
+                             (const lwse_lws_out*)e->r_lws_out.p, lws_results ? e->rn_lws : 0u};
+  launched = lwse::launch_ds_drain_sweep(&t, &lk, lk.lws_out, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = forecast_locked(e, t, &q->fc, s); rc != LWSE_OK) return rc;
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(q->now, t.ds_out, (size_t)n * sizeof(lwse_ds_out), cudaMemcpyDeviceToHost, s));
+  if (q->now_roles)
+    LWSE_CUDA(e, cudaMemcpyAsync(q->now_roles, t.role_out, nr * sizeof(lwse_ds_role_out), cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  return LWSE_OK;
 }
 
 // ---- rolling-update forecast of the LeaderWorkerSets ----

@@ -241,6 +241,27 @@ int launch_rollout_whatif_gather(const RolloutWhatifHost* h, int sm_count, cudaS
 int launch_rollout_whatif_restore(const uint32_t* d_src, const lwse_group_out* d_baseline, lwse_group_out* d_out,
                                   uint8_t* d_gflag8, uint32_t n_rows, int sm_count, cudaStream_t s, int* cuda_err);
 
+// ---- lwse_ds_whatif_kernels.cu ----
+struct DsWhatifHost {
+  lwse_ds_tables t;                   // the resident DS tables (inputs only)
+  const lwse_ds_link* links;          // the resident link table, [t.n_revroles]
+  const lwse_ds_proposal* proposals;  // [n] (ds < t.n_ds and known flags, checked by the engine)
+  const lwse_ds_role_rec* q_roles;    // [n * LWSE_DS_MAX_ROLES] the query's role rows, or null when no proposal
+                                      // has LWSE_DSP_ROLES
+  uint32_t n;
+  uint32_t* count;                    // [n] revision-role rows each proposal gathers (the count kernel writes them)
+  uint32_t* off;                      // [n] its first scratch revision-role row (the layout writes them)
+  lwse_ds_rec* s_ds;                  // [n] the proposed DS rows
+  lwse_ds_role_rec* s_roles;          // [n * LWSE_DS_MAX_ROLES] their role rows, proposal i's at i * 10
+  lwse_ds_revrole_rec* s_revroles;    // the gathered revision-role rows ...
+  lwse_ds_link* s_links;              // ... and their link rows
+};
+// The layout: count[i], then off[i] = their exclusive prefix and *total = their sum (u64, < 2^32 for
+// n <= LWSE_DS_WHATIF_MAX_PROPOSALS).  sums: forecast_scan_words(n) words.
+int launch_ds_whatif_layout(const DsWhatifHost* h, unsigned long long* sums, unsigned long long* total, int sm_count,
+                            cudaStream_t s, int* cuda_err);
+int launch_ds_whatif_gather(const DsWhatifHost* h, int sm_count, cudaStream_t s, int* cuda_err);
+
 // ---- lwse_drain_kernels.cu ----
 // The drain what-if's counters (device, 16 words, zeroed by the caller): [0] changed rows [1] pods evicted
 // [2] leaders evicted [3] groups restarted [4] ready groups restarted [6..7] pods recreated (u64).

@@ -376,21 +376,77 @@ class DsIncrementalEncoder:
                                              for i, rev in enumerate(old) if (fell >> i) & 1]})
         return out
 
+    def whatif_rollout(self, ds: api.DisaggregatedSet, revision: str) -> tuple:
+        """A proposal for ``Engine.resident_ds_rollout_whatif``: ``ds`` is the edited object and ``revision`` its
+        ComputeRevision(spec.roles), as ``ds_event`` would take them.  The edited object is encoded with the
+        DS's cached children, the retired target revision's children last in List order, as the next
+        ``flush()`` would encode it once the edit lands.  → (DS_PROPOSAL, DS_MAX_ROLES DS_ROLE_REC rows, the
+        encoded role rows first): DSP_NEW_REVISION iff ``revision`` is not the current target, DSP_ROLES iff
+        the role rows differ from the resident ones.  Nothing in the encoder changes.  KeyError for a DS that
+        is not resident; ValueError for an edit that changes allRoleNames or which of them are in the spec (add,
+        remove or rename a role, also one whose children remain, or take a removed role back into the spec) or
+        whose revision names an old revision that still has children (re-encode and use
+        ``Engine.ds_forecast_host`` for those)."""
+        key = (ds.namespace, ds.name)
+        sl = self.slots[key]
+        current = self.items[key][1]
+        kids = list(self.children.get(key, {}).values())
+        if revision != current and any(c.revision == revision for c in kids):
+            raise ValueError(f"{key}: revision {revision} still has children")
+        kids = [c for c in kids if c.revision != current] + [c for c in kids if c.revision == current]
+        t = encoder.encode_ds([encoder.DsItem(ds, revision, kids)])
+        names = self.role_names(sl.ds_row)
+        if list(t.role_names[0]) != names:
+            raise ValueError(f"{key}: the edit changes the roles {names} to {list(t.role_names[0])}")
+        # allRoleNames alone misses a spec role dropped while its children remain (it stays, as a removed role)
+        # and a removed role taken back into the spec: the spec / removed split moves, which a proposal keeps
+        n_spec = int(self.ds[sl.ds_row]["n_spec_roles"])
+        if int(t.ds[0]["n_spec_roles"]) != n_spec:
+            raise ValueError(f"{key}: the edit changes the spec roles {names[:n_spec]} to "
+                             f"{names[:int(t.ds[0]['n_spec_roles'])]}")
+        n = len(names)
+        roles = R.aligned_empty(R.DS_MAX_ROLES, R.DS_ROLE_REC)
+        roles[:n] = t.roles
+        flags = R.DSP_NEW_REVISION if revision != current else 0
+        if roles[:n].tobytes() != self.roles[sl.role_base: sl.role_base + n].tobytes():
+            flags |= R.DSP_ROLES
+        p = np.zeros(1, R.DS_PROPOSAL)
+        p[0] = (sl.ds_row, flags)
+        return p[0], roles
+
+    def whatif_of(self, answer: dict, i: int, namespace: str, name: str) -> dict:
+        """Proposal i of a ``resident_ds_rollout_whatif`` answer on the named DS, as ``forecast_of`` names a
+        forecast, plus ``now`` (the DS_OUT row) and per role its ``next`` (old, new) from ``now_roles``.  A
+        template edit adds the retired target revision as the last old revision (bit len(old_revisions) of
+        drained_revs / ready_revs)."""
+        names = self.role_names(self.ds_row(namespace, name))
+        n, base = len(names), i * R.DS_MAX_ROLES
+        out = self._named(answer["ds"][i], answer["roles"][base: base + n], answer.get("steps"), names)
+        out["now"] = answer["now"][i]
+        for j, role in enumerate(names):
+            r = answer["now_roles"][base + j]
+            out["roles"][role]["next"] = (int(r["next_old"]), int(r["next_new"]))
+        return out
+
     def forecast_of(self, forecast: dict, namespace: str, name: str) -> dict:
         """One DS's rollout forecast (``Engine.ds_resident_forecast`` over ``tables()``), by name:
         the flags, cycle and step counts, and per role name its peak replicas, availability floor,
         final old / new counts and trajectory [(old, new), ...] (empty without trajectory rows, or
         when the DS's rows did not fit)."""
         row = self.ds_row(namespace, name)
-        fc = forecast["ds"][row]
         role_base = int(self.ds[row]["role_base"])
         names = self.role_names(row)
+        return self._named(forecast["ds"][row], forecast["roles"][role_base: role_base + len(names)],
+                           forecast.get("steps"), names)
+
+    @staticmethod
+    def _named(fc, role_rows, steps, names) -> dict:
+        """A forecast row and its role rows, by role name (``forecast_of``, ``whatif_of``)."""
         n, base, n_steps = len(names), int(fc["step_base"]), int(fc["n_steps"])
-        steps = forecast.get("steps")
         have = steps is not None and not fc["flags"] & R.DSF_TRUNCATED and base + n_steps * n <= len(steps)
         roles = {}
         for i, role in enumerate(names):
-            r = forecast["roles"][role_base + i]
+            r = role_rows[i]
             traj = ([(int(steps[base + s * n + i]["next_old"]), int(steps[base + s * n + i]["next_new"]))
                      for s in range(n_steps)] if have else [])
             roles[role] = {"peak_replicas": int(r["peak_replicas"]), "floor_available": int(r["floor_available"]),

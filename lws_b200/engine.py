@@ -95,6 +95,7 @@ SYMBOLS = {
     "lwse_ds_resident_tick_info": ([C.c_void_p, C.POINTER(R.DsTickInfo)], C.c_int),
     "lwse_ds_forecast_host": ([C.c_void_p, C.POINTER(R.DsTables), C.POINTER(R.DsForecastOut)], C.c_int),
     "lwse_ds_resident_forecast": ([C.c_void_p, C.POINTER(R.DsForecastOut)], C.c_int),
+    "lwse_resident_ds_rollout_whatif": ([C.c_void_p, C.POINTER(R.DsRolloutWhatIf)], C.c_int),
     "lwse_lws_forecast_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(R.LwsForecastOut)], C.c_int),
     "lwse_resident_forecast": ([C.c_void_p, C.POINTER(R.LwsForecastOut)], C.c_int),
@@ -736,6 +737,36 @@ class Engine:
         n_ds, n_roles, _ = getattr(self, "_ds_shape", (0, 0, 0))
         return self._ds_forecast(lambda o: lib().lwse_ds_resident_forecast(self._h, C.byref(o)),
                                  n_ds, n_roles, steps, step_capacity)
+
+    def resident_ds_rollout_whatif(self, proposals, roles=None, steps=True, step_capacity=None):
+        """lwse_resident_ds_rollout_whatif: for each proposal (DS_PROPOSAL: a resident DS row and DSP_* flags)
+        the DS controller's first decision over the rows the edit would encode to (``now``, DS_OUT, and
+        ``now_roles``, DS_ROLE_OUT, DS_MAX_ROLES rows per proposal) and the forecast of the rollout it would
+        start, each as if it were the only edit (lwse.h, "DS rollout what-if").  ``roles``: DS_ROLE_REC rows,
+        DS_MAX_ROLES per proposal (an (n, DS_MAX_ROLES) or flat array), read for DSP_ROLES proposals.  → ``now``,
+        ``now_roles`` plus what ``ds_resident_forecast`` returns, with one ``ds`` row and DS_MAX_ROLES ``roles``
+        rows per proposal and the trajectory offsets running over the proposals in order.  Changes nothing
+        resident and waits for no tick."""
+        props = np.ascontiguousarray(proposals)
+        assert props.dtype == R.DS_PROPOSAL
+        n, nr = len(props), len(props) * R.DS_MAX_ROLES
+        if roles is not None:
+            roles = np.asarray(roles).reshape(-1)
+            assert roles.dtype == R.DS_ROLE_REC and len(roles) == nr
+            roles = _aligned16(roles)
+        now = R.aligned_empty(n, R.DS_OUT)
+        now_roles = R.aligned_empty(nr, R.DS_ROLE_OUT)
+
+        def call(o):
+            q = R.DsRolloutWhatIf(R.ptr(props) if n else None, R.ptr(roles) if roles is not None and n else None, n, 0,
+                                  R.ptr(now) if n else None, R.ptr(now_roles) if n else None, o)
+            rc = lib().lwse_resident_ds_rollout_whatif(self._h, C.byref(q))
+            o.n_steps_written, o.n_steps_needed = q.fc.n_steps_written, q.fc.n_steps_needed
+            return rc
+
+        out = self._ds_forecast(call, n, nr, steps, step_capacity)
+        out["now"], out["now_roles"] = now, now_roles
+        return out
 
     # ------------------------------------------- rolling-update forecast (LWS)
     def _lws_forecast(self, call, n_lws, steps, step_capacity):

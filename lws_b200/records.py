@@ -301,6 +301,14 @@ DSF_TRUNCATED = 1 << 4
 DSF_BAD_TABLE = 1 << 6
 DS_FORECAST_MAX_CYCLES = 65536
 
+# DS rollout what-if (lwse_resident_ds_rollout_whatif): one proposal per DS edit; with DSP_ROLES its role rows
+# are rows [i * DS_MAX_ROLES, i * DS_MAX_ROLES + n_roles) of the query's role table
+DS_PROPOSAL = np.dtype([("ds", "<u4"), ("flags", "<u4")], align=False)
+assert DS_PROPOSAL.itemsize == 8
+DSP_NEW_REVISION = 1 << 0
+DSP_ROLES = 1 << 1
+DS_WHATIF_MAX_PROPOSALS = (2**32 - 1) // ((DS_MAX_OLD_REVS + 1) * DS_MAX_ROLES)
+
 # rolling-update forecast of the LeaderWorkerSets (lwse_lws_forecast_*): per LWS, and the trajectory rows
 LWS_FORECAST = np.dtype(
     [("flags", "<u4"), ("cycles", "<u4"), ("step_base", "<u4"), ("n_steps", "<u4"), ("peak_sts_replicas", "<i4"),
@@ -481,6 +489,21 @@ class RolloutWhatIf(C.Structure):
         ("reserved", C.c_uint32),
         ("now", C.c_void_p),
         ("fc", LwsForecastOut),
+    ]
+
+
+class DsRolloutWhatIf(C.Structure):
+    """lwse_ds_rollout_whatif: proposed DS edits in; the DS controller's first decision and the forecast of
+    the rollout each proposal would start out."""
+
+    _fields_ = [
+        ("proposals", C.c_void_p),
+        ("roles", C.c_void_p),
+        ("n", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("now", C.c_void_p),
+        ("now_roles", C.c_void_p),
+        ("fc", DsForecastOut),
     ]
 
 
