@@ -203,6 +203,14 @@ func (e *Engine) DsDrainCost(scope uint32, out *C.lwse_ds_drain_cost) error {
 	return e.check(C.lwse_resident_ds_drain_cost(e.h, C.uint32_t(scope), out))
 }
 
+// DrainPlaceCost answers "if I drain this node or this domain, do the groups it restarts find a new
+// exclusive domain?" for every node (scope LWSE_DRAIN_NODES) or every domain (LWSE_DRAIN_DOMAINS) in one
+// call: restarted groups, unpinned requests, those left without a domain (stranded), others that lose theirs
+// (bumped) and the placement what-if's counts.  A maintenance controller ranks the next rack to drain with it.
+func (e *Engine) DrainPlaceCost(scope uint32, out *C.lwse_drain_place_cost) error {
+	return e.check(C.lwse_resident_drain_place_cost(e.h, C.uint32_t(scope), out))
+}
+
 // GroupKeys computes SHA-1 digests (20 bytes each) of n strings laid out CSR-style.
 func (e *Engine) GroupKeys(bytes *C.uint8_t, offsets *C.uint32_t, n uint32, digests *C.uint8_t) error {
 	return e.check(C.lwse_group_keys_host(e.h, bytes, offsets, C.uint32_t(n), digests))

@@ -1000,6 +1000,54 @@ typedef struct lwse_drain_budget_cost {
 } lwse_drain_budget_cost;
 LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lwse_drain_budget_cost* out);
 
+/* ---- drain placement ----------------------------------------------------------------------------
+ * "If I drain this node or this domain, do the groups it restarts find a new exclusive domain?" — for every
+ * node (LWSE_DRAIN_NODES, n_nodes rows) or every domain (LWSE_DRAIN_DOMAINS, n_domains rows) in one call.
+ *
+ * Definition.  Key k names a node row, or a domain id whose node set is every node row with that domain_id
+ * (by domain_id alone, as the drain budget).  Let N_k be that node set.  Row k is the answer of the set-form
+ * composition lwse_resident_drain_whatif(N_k) -> unpin -> lwse_resident_place_whatif for D = N_k:
+ *   - the restarted groups are those of lwse_resident_drain_whatif(N_k): restart bits clear in the baseline
+ *     group results (the most recently submitted sweep), set after;
+ *   - U_k, the unpinned requests, are the resident request rows r with leader_node != LWSE_NONE whose
+ *     leader_node is in N_k or whose `group` field names a group row below the resident group count that the
+ *     drain restarts; the query gives them leader_node = LWSE_NONE;
+ *   - the placement is the what-if round (lwse_resident_place_whatif) over the resident node rows with
+ *     LWSE_NODE_SCHEDULABLE cleared on N_k, the resident occupancy counters, the resident request rows with
+ *     U_k unpinned and the resident n_namespaces, diffed against the rows of the most recently submitted tick
+ *     with LWSE_TICK_PLACE.  Occupancy does not move, so the answer is conservative: the pods of a restarted
+ *     group on nodes that are not drained still count against those nodes.
+ *
+ * Locality.  Per key the call solves only the namespaces the key can change, and every other row keeps its
+ * baseline row (DESIGN.md §3.5, "Drain placement"): a namespace v is solved for key k when (a) it holds a row
+ * of U_k, or (b) it has a row that is not pinned and is PLACED in a drained domain d and either k is a
+ * domain, or k is a node n with dom_free[d] - free[n] < size or n the row's chosen node.
+ *
+ * Readiness and errors: LWSE_ERR_NOT_READY when lwse_resident_drain_whatif or lwse_resident_place_whatif
+ * would answer it, or when the resident request table has no namespace; LWSE_ERR_INVALID_ARG for a NULL
+ * `out` or another scope; LWSE_ERR_UNSUPPORTED on an engine with a peer exchange, when the resident request
+ * count reaches 2^24, and where the namespace form does not fit the domains (the set-form composition then
+ * remains the answer); LWSE_ERR_OOM rather than a wrong row when a sized table refuses an entry.
+ * Isolation: as the drain what-if (the engine mutex, the what-if stream behind an event on the engine's
+ * stream, scratch of its own that only grows; no tick, graph, arena, change list, table, output row,
+ * occupancy counter, node index or tick info is touched).  `out` holds the rows in host memory (64 B each). */
+typedef struct lwse_drain_place_cost {
+  uint32_t groups_restarted;  /* the drain cost's groups_restarted for the key                           */
+  uint32_t unpinned;          /* |U_k|                                                                   */
+  uint32_t stranded;          /* rows of U_k that are not PLACED after                                   */
+  uint32_t bumped;            /* rows outside U_k that are PLACED before and not after                   */
+  uint32_t n_changed;         /* the lwse_place_whatif counters of the composed query                    */
+  uint32_t n_lost;
+  uint32_t n_moved;
+  uint32_t n_gained;
+  uint32_t n_placed;
+  uint32_t n_unschedulable;
+  uint32_t n_conflict;
+  uint32_t namespaces_solved; /* namespaces the call solved for this key                                 */
+  uint32_t reserved[4];
+} lwse_drain_place_cost;
+LWSE_API int lwse_resident_drain_place_cost(lwse_engine* e, uint32_t scope, lwse_drain_place_cost* out);
+
 /* ------------------------------------------------------------------------- */
 /* Peer exchange: the multi-GPU placement step without a collective library  */
 /* ------------------------------------------------------------------------- */

@@ -256,4 +256,20 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
+// The drain placement (lwse_resident_drain_place_cost): one row's contribution, baseline o and what-if v, to
+// words 2..10 of its key's lwse_drain_place_cost row (the three totals as deltas).
+constexpr uint32_t kDrainCounts = 9;  // stranded, bumped, changed, lost, moved, gained, PLACED, UNSCHED., CONFLICT
+__device__ __forceinline__ void drain_place_count(uint32_t* c, const uint4 o, const uint4 v, bool unpinned) {
+  const bool was = (o.z & LWSE_PLACE_PLACED) != 0u, is = (v.z & LWSE_PLACE_PLACED) != 0u;
+  c[0] += (unpinned && !is) ? 1u : 0u;
+  c[1] += (!unpinned && was && !is) ? 1u : 0u;
+  c[2] += (v.x != o.x || v.y != o.y || v.z != o.z || v.w != o.w) ? 1u : 0u;
+  c[3] += (was && !is) ? 1u : 0u;
+  c[4] += (was && is && o.x != v.x) ? 1u : 0u;
+  c[5] += (!was && is) ? 1u : 0u;
+  c[6] += (uint32_t)is - (uint32_t)was;
+  c[7] += ((v.z & LWSE_PLACE_UNSCHEDULABLE) ? 1u : 0u) - ((o.z & LWSE_PLACE_UNSCHEDULABLE) ? 1u : 0u);
+  c[8] += ((v.z & LWSE_PLACE_CONFLICT) ? 1u : 0u) - ((o.z & LWSE_PLACE_CONFLICT) ? 1u : 0u);
+}
+
 }  // namespace lwse

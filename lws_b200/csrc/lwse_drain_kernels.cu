@@ -416,9 +416,9 @@ struct DrainBudgetCostArgs {
   lwse_drain_budget_cost* cost;  // n_keys rows
   unsigned long long* keys;      // the table: LWS row << 32 | key, kEmptyKey when free
   uint4* vals;                   // {groups restarted, ready groups restarted, of those with index < replicas, 0}
-  uint32_t* counts;              // [0..1] pairs (u64), [2] refused inserts
+  uint32_t* counts;              // [0..1] pairs (u64), [2] refused inserts; pair mode: [8] pairs written
   uint64_t n_pods;
-  uint32_t n_lws, n_groups, n_nodes, n_domains, table_mask;
+  uint32_t n_lws, n_groups, n_nodes, n_domains, table_mask;  // pair mode: keys = the pair list, table_mask its capacity
 };
 
 constexpr unsigned long long kEmptyKey = ~0ull;
@@ -461,7 +461,9 @@ __device__ __forceinline__ void table_add(const DrainBudgetCostArgs& a, unsigned
   atomicAdd(a.counts + 2, 1u);  // full: the call fails
 }
 
-template <bool kInsert>
+// kPairs: every fresh (group, key) pair of every group, member or not, as key << 32 | group into keys[0 ..
+// table_mask) (the drain placement's restarts; the struct stays as the other instances read it).
+template <bool kInsert, bool kPairs = false>
 __global__ void __launch_bounds__(kCostThreads) drain_budget_walk_kernel(const DrainBudgetCostArgs a) {
   __shared__ uint32_t s_list[kCostThreads / 32][kCostList];
   constexpr uint32_t kFull = 0xFFFFFFFFu;
@@ -474,7 +476,7 @@ __global__ void __launch_bounds__(kCostThreads) drain_budget_walk_kernel(const D
     const uint4* row = reinterpret_cast<const uint4*>(a.groups + g);
     const uint4 ca = ldg_stream(row + 0), cb = ldg_stream(row + 1), cc = ldg_stream(row + 2), cd = ldg_stream(row + 3);
     const uint32_t leader_node = cc.y, pod_base = cc.z, pod_count = cc.w, lws_index = cd.x;
-    if (!kInsert && lane == 0) {
+    if (!kInsert && !kPairs && lane == 0) {
       const uint32_t lk = key_of_node(a, leader_node);
       if (lk != LWSE_NONE) atomicAdd(&a.cost[lk].leaders, 1u);
     }
@@ -527,7 +529,10 @@ __global__ void __launch_bounds__(kCostThreads) drain_budget_walk_kernel(const D
         }
       }
       if (!fresh) continue;
-      if (kInsert) {
+      if (kPairs) {
+        const uint32_t at = atomicAdd(a.counts + 8, 1u);
+        if (at < a.table_mask) a.keys[at] = (unsigned long long)key << 32 | g;
+      } else if (kInsert) {
         table_add(a, (unsigned long long)lws_index << 32 | key, ready, ready_nb);
       } else {
         lwse_drain_budget_cost* c = a.cost + key;
@@ -538,7 +543,7 @@ __global__ void __launch_bounds__(kCostThreads) drain_budget_walk_kernel(const D
       }
     }
   }
-  if (!kInsert) {
+  if (!kInsert && !kPairs) {
     pairs = warp_sum_u64(pairs);
     if (lane == 0 && pairs) atomicAdd(reinterpret_cast<unsigned long long*>(a.counts), pairs);
   }
@@ -596,6 +601,18 @@ int launch_drain_budget_cost(const DrainBudgetCostLaunch* p, int pass, int sm_co
       drain_budget_walk_kernel<true><<<walk_grid, kCostThreads, 0, s>>>(a);
       return launched_or_fail(1, cuda_err);
   }
+}
+
+int launch_drain_restart_pairs(const DrainBudgetCostLaunch* p, unsigned long long* pairs, uint32_t capacity, int sm_count,
+                               cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  if (p->n_groups == 0) return 0;
+  const DrainBudgetCostArgs a{p->lws, p->lws_out, p->groups, p->pod_state, p->pod_ident, p->baseline,
+                              p->by_domain ? p->nodes : nullptr, nullptr, pairs, nullptr, p->counts,
+                              p->n_pods, p->n_lws, p->n_groups, p->n_nodes, p->n_domains, capacity};
+  drain_budget_walk_kernel<false, true>
+      <<<grid_for(p->n_groups, kCostThreads / 32, (uint32_t)sm_count * 8u), kCostThreads, 0, s>>>(a);
+  return launched_or_fail(1, cuda_err);
 }
 
 // --------------------------------------------------------------------------

@@ -232,6 +232,12 @@ struct lwse_engine {
   // drain budget (lwse_resident_drain_budget*): the domain mask, the touched rows, the key rows, the (LWS, key)
   // table and its counters
   DevBuf dr_domains, dr_brows, dr_bcost, dr_table, dr_bwords;
+  // drain placement (lwse_resident_drain_place_cost): the drain budget's key rows and walk counters, the counters,
+  // the free slots per domain, the group -> request and key -> U_k indexes, the restart pairs, U_k's rows, the row
+  // positions, the item table and list, the key rows, the all-namespaces mask, the round scratch, the solve's
+  // per-CTA slices
+  DevBuf dp_cost, dp_words, dp_domfree, dp_gidx, dp_uidx, dp_pairs, dp_urows, dp_pos, dp_items, dp_rows, dp_touched, dp_round,
+      dp_slices;
   // DS drain (lwse_resident_ds_drain*): lost[L] and the after copy of lws_out, the before / after sweep outputs, the
   // touched DS rows, the reverse link index (count | first | cursor) and its entries, the key rows, the (DS, key) table
   DevBuf dd_lost, dd_lws_after, dd_out[2], dd_role_out[2], dd_revrole_out[2], dd_rows, dd_index, dd_entries, dd_cost, dd_table;
@@ -463,6 +469,8 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->wf_node_ix, &e->wf_touched, &e->wf_round, &e->wf_list,
                       &e->dr_state, &e->dr_groups, &e->dr_out, &e->dr_scan, &e->dr_mask, &e->dr_list, &e->dr_cost,
                       &e->dr_domains, &e->dr_brows, &e->dr_bcost, &e->dr_table, &e->dr_bwords,
+                      &e->dp_cost, &e->dp_words, &e->dp_domfree, &e->dp_gidx, &e->dp_uidx, &e->dp_pairs, &e->dp_urows, &e->dp_pos,
+                      &e->dp_items, &e->dp_rows, &e->dp_touched, &e->dp_round, &e->dp_slices,
                       &e->dd_lost, &e->dd_lws_after, &e->dd_out[0], &e->dd_out[1], &e->dd_role_out[0], &e->dd_role_out[1],
                       &e->dd_revrole_out[0], &e->dd_revrole_out[1], &e->dd_rows, &e->dd_index, &e->dd_entries, &e->dd_cost,
                       &e->dd_table, &e->rw_rows, &e->rw_lws, &e->rw_off, &e->rw_sums, &e->rw_groups, &e->rw_src,
@@ -2770,6 +2778,181 @@ LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lws
   LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 16, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   if (words[2]) return LWSE_ERR_OOM;  // an insert the table refused: no answer rather than a wrong one
+  return LWSE_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Drain placement
+// ---------------------------------------------------------------------------
+// Three host synchronisations, each sizing what follows: the restart pairs (the drain budget's pass 0 counts
+// them per key), then U_k and the rule-(b) candidates, then the answer.  Everything reads the resident tables,
+// the baseline group results and placement rows in place (nothing writes them while the call holds the mutex).
+LWSE_API int lwse_resident_drain_place_cost(lwse_engine* e, uint32_t scope, lwse_drain_place_cost* out) {
+  if (!e) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->r_loaded || e->n_nodes == 0 || !e->r_groups_swept) return LWSE_ERR_NOT_READY;  // (the drain what-if's rule)
+  if (!e->r_place_loaded || !e->r_place_current || e->n_domains == 0) return LWSE_ERR_NOT_READY;  // (the place what-if's)
+  if (e->rn_namespaces == 0) return LWSE_ERR_NOT_READY;
+  if (!out || (scope != LWSE_DRAIN_NODES && scope != LWSE_DRAIN_DOMAINS)) return LWSE_ERR_INVALID_ARG;
+  if (e->xch_world > 0 || e->rn_reqs >= (1u << 24) || !lwse::place_ns_supported(e->n_nodes, e->n_domains))
+    return LWSE_ERR_UNSUPPORTED;
+  const bool by_domain = scope == LWSE_DRAIN_DOMAINS;
+  const uint32_t nn = e->n_nodes, nd = e->n_domains, nr = e->rn_reqs, ng = e->rn_groups, n_ns = e->rn_namespaces;
+  const uint32_t nk = by_domain ? nd : nn;
+  uint32_t max_ns = 1;  // the largest namespace: the solve's per-CTA slices
+  {
+    std::vector<uint32_t> per(n_ns, 0);
+    for (uint32_t r = 0; r < nr; r++)
+      if (e->r_req_ns[r] < n_ns) max_ns = std::max(max_ns, ++per[e->r_req_ns[r]]);
+  }
+  const size_t round_bytes = lwse::place_ns_scratch_bytes(nn, nd, nr, n_ns);
+  DeviceGuard guard(e->device);
+  LWSE_CUDA(e, e->dp_cost.reserve((size_t)nk * sizeof(lwse_drain_budget_cost) + 16));
+  LWSE_CUDA(e, e->dp_words.reserve(128));
+  LWSE_CUDA(e, e->wf_words.reserve(256));  // (the counters, and |U| at word 32)
+  LWSE_CUDA(e, e->dp_domfree.reserve((size_t)nd * 4 + 16));
+  LWSE_CUDA(e, e->dp_gidx.reserve(((size_t)ng * 3 + 2 + nr) * 4 + 16));
+  LWSE_CUDA(e, e->dp_uidx.reserve(((size_t)nk * 3 + 2) * 4 + 16));
+  LWSE_CUDA(e, e->dp_pos.reserve((size_t)nr * 4 + 16));
+  LWSE_CUDA(e, e->dp_rows.reserve((size_t)nk * sizeof(lwse_drain_place_cost) + 16));
+  LWSE_CUDA(e, e->dp_touched.reserve((size_t)n_ns + 16));
+  LWSE_CUDA(e, e->dp_round.reserve(round_bytes));
+  const bool own_index = e->node_index_stale;  // (as the place what-if: a resident index behind the node rows is not read)
+  if (own_index) {
+    LWSE_CUDA(e, e->wf_dom_first.reserve(((size_t)nd + 1) * 4 + 16));
+    LWSE_CUDA(e, e->wf_node_order.reserve(((size_t)(nn + 255u) / 256u + 1u) * 1024u + 16));
+    LWSE_CUDA(e, e->wf_node_pos.reserve((size_t)nn * 4 + 16));
+    LWSE_CUDA(e, e->wf_node_ix.reserve(lwse::node_index_scratch_bytes(nd)));
+  }
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* d_words = (uint32_t*)e->dp_words.p;  // [0..15] this call's counters, [16..31] the walk's
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_cost.p, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
+  LWSE_CUDA(e, cudaMemsetAsync(d_words, 0, 128, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_gidx.p, 0, (size_t)ng * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_uidx.p, 0, (size_t)nk * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_pos.p, 0xFF, (size_t)nr * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_touched.p, 1, n_ns, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_round.p, 0, round_bytes, s));  // (the index counts start at zero)
+  int cuda_err = 0;
+  const uint32_t* dom_first = (const uint32_t*)e->dom_first.p;
+  const uint32_t* node_order = (const uint32_t*)e->node_order.p;
+  if (own_index) {
+    const size_t ix_bytes = lwse::node_index_scratch_bytes(nd);
+    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_ix.p, 0, ix_bytes, s));
+    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_order.p, 0, ((size_t)(nn + 255u) / 256u + 1u) * 1024u, s));
+    const int launched = lwse::launch_node_index((const lwse_node_rec*)e->nodes.p, nn, nd, (uint32_t*)e->wf_dom_first.p,
+                                                 (uint32_t*)e->wf_node_order.p, (uint32_t*)e->wf_node_pos.p, e->wf_node_ix.p,
+                                                 e->sm_count, s, false, &cuda_err);
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    dom_first = (const uint32_t*)e->wf_dom_first.p;
+    node_order = (const uint32_t*)e->wf_node_order.p;
+  }
+  {
+    const int launched = lwse::launch_place_whatif_index((const lwse_place_req*)e->r_preq.p, nr, n_ns, (const uint8_t*)e->dp_touched.p,
+                                                         nn, nd, e->dp_round.p, e->sm_count, s, &cuda_err);
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  }
+  // the restarted groups per key: the drain budget's pass 0 (key rows, the walk)
+  lwse::DrainBudgetCostLaunch bp{};
+  bp.lws = (const lwse_lws_rec*)e->r_lws.p;
+  bp.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
+  bp.groups = (const lwse_group_rec*)e->r_groups.p;
+  bp.pod_state = (const uint8_t*)e->r_pst.p;
+  bp.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
+  bp.baseline = (const lwse_group_out*)e->r_group_out.p;
+  bp.nodes = (const lwse_node_rec*)e->nodes.p;
+  bp.occupancy = (const uint32_t*)e->r_occ.p;
+  bp.cost = (lwse_drain_budget_cost*)e->dp_cost.p;
+  bp.counts = d_words + 16;
+  bp.n_pods = e->rn_pods;
+  bp.n_lws = e->rn_lws;
+  bp.n_groups = ng;
+  bp.n_nodes = nn;
+  bp.n_domains = nd;
+  bp.n_keys = nk;
+  bp.by_domain = by_domain;
+  int launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  lwse::DrainPlaceLaunch p{};
+  p.nodes = (const lwse_node_rec*)e->nodes.p;
+  p.occupancy = (const uint32_t*)e->r_occ.p;
+  p.dom_first = dom_first;
+  p.node_order = node_order;
+  p.dom_free = (uint32_t*)e->dp_domfree.p;
+  p.reqs = (const lwse_place_req*)e->r_preq.p;
+  p.base = (const lwse_place_out*)e->r_pout.p;
+  p.cost = (const lwse_drain_budget_cost*)e->dp_cost.p;
+  p.n_nodes = nn;
+  p.n_domains = nd;
+  p.n_reqs = nr;
+  p.n_namespaces = n_ns;
+  p.n_groups = ng;
+  p.n_keys = nk;
+  p.by_domain = by_domain;
+  p.g_count = (uint32_t*)e->dp_gidx.p;
+  p.g_first = p.g_count + ng;
+  p.g_cursor = p.g_first + ng + 1;
+  p.u_count = (uint32_t*)e->dp_uidx.p;
+  p.u_first = p.u_count + nk;
+  p.u_cursor = p.u_first + nk + 1;
+  p.pos = (uint32_t*)e->dp_pos.p;
+  p.rows = (lwse_drain_place_cost*)e->dp_rows.p;
+  p.counts = d_words;
+  p.round = e->dp_round.p;
+  p.round_bytes = round_bytes;
+  p.g_reqs = p.g_cursor + ng;  // (the pinned rows, at most nr)
+  launched = lwse::launch_drain_place(&p, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 32, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint32_t n_pairs = words[6];
+  // the restart pairs, then U_k counted and scanned
+  LWSE_CUDA(e, e->dp_pairs.reserve((size_t)n_pairs * 8 + 16));
+  launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dp_pairs.p, n_pairs, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  p.pairs = (const unsigned long long*)e->dp_pairs.p;
+  p.n_pairs = n_pairs;
+  launched = lwse::launch_drain_place(&p, 1, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 128, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 32, p.u_first + nk, 4, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  if (words[16 + 8] != n_pairs) return LWSE_ERR_OOM;  // (the walk found another pair count: no answer rather than a wrong one)
+  const uint32_t n_unp = words[32];
+  const uint64_t item_cap = (uint64_t)n_unp + words[3];
+  if (item_cap > (1ull << 30)) return LWSE_ERR_OOM;  // (the table index is 32-bit)
+  uint64_t slots = 256;
+  while (slots < 2 * item_cap) slots <<= 1;
+  // the solve's slices: results, unpinned list and marks per resident CTA, sized from the largest namespace
+  uint64_t grid = (uint64_t)e->sm_count * 2u;
+  if (grid > item_cap) grid = item_cap ? item_cap : 1;
+  while (grid > 1 && grid * max_ns * (sizeof(lwse_place_out) + 5) > (1ull << 30)) grid >>= 1;
+  const size_t slice_out = align256((size_t)grid * max_ns * sizeof(lwse_place_out));
+  const size_t slice_unp = align256((size_t)grid * max_ns * 4);
+  LWSE_CUDA(e, e->dp_slices.reserve(slice_out + slice_unp + (size_t)grid * max_ns + 16));
+  LWSE_CUDA(e, e->dp_items.reserve((size_t)slots * 8 + (size_t)item_cap * 8 + 16));
+  LWSE_CUDA(e, e->dp_urows.reserve((size_t)n_unp * 4 + 16));
+  p.u_rows = (uint32_t*)e->dp_urows.p;
+  p.n_unpinned = n_unp;
+  p.item_keys = (unsigned long long*)e->dp_items.p;
+  p.item_mask = (uint32_t)(slots - 1);
+  p.items = reinterpret_cast<uint2*>(p.item_keys + slots);
+  p.item_capacity = (uint32_t)item_cap;
+  LWSE_CUDA(e, cudaMemsetAsync(p.item_keys, 0xFF, (size_t)slots * 8, s));
+  p.s_out = (lwse_place_out*)e->dp_slices.p;
+  p.s_unpinned = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(e->dp_slices.p) + slice_out);
+  p.s_marks = static_cast<uint8_t*>(e->dp_slices.p) + slice_out + slice_unp;
+  p.slice_rows = max_ns;
+  p.grid = (uint32_t)grid;
+  launched = lwse::launch_drain_place(&p, 2, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(out, p.rows, (size_t)nk * sizeof(lwse_drain_place_cost), cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 64, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  if (words[5]) return LWSE_ERR_OOM;  // an item the table refused
   return LWSE_OK;
 }
 

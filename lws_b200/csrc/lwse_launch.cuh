@@ -331,6 +331,57 @@ struct DsDrainCostLaunch {
 };
 int launch_ds_drain_cost(const DsDrainCostLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
 
+// ---- lwse_drain_place_kernels.cu (and the drain instance of the namespace kernel) ----
+// lwse_resident_drain_place_cost.  counts (device, 16 words, zeroed by the caller): [0] PLACED [1] UNSCHEDULABLE
+// [2] CONFLICT baseline rows, [3] rule-(b) candidates, [4] items, [5] refused item inserts, [6] restart pairs.
+struct DrainPlaceLaunch {
+  const lwse_node_rec* nodes;
+  const uint32_t* occupancy;
+  const uint32_t* dom_first;           // the node index every placement form reads
+  const uint32_t* node_order;
+  uint32_t* dom_free;                  // [n_domains] free slots per domain (pass 0 writes them)
+  const lwse_place_req* reqs;
+  const lwse_place_out* base;          // the baseline rows
+  const lwse_drain_budget_cost* cost;  // the drain budget's pass 0 rows: groups_restarted per key
+  uint32_t n_nodes, n_domains, n_reqs, n_namespaces, n_groups, n_keys;
+  bool by_domain;
+  const unsigned long long* pairs;     // restart pairs key << 32 | group
+  uint32_t n_pairs;
+  uint32_t* g_count;                   // [n_groups] pinned request rows per group (zero between calls)
+  uint32_t* g_first;                   // [n_groups + 1]
+  uint32_t* g_cursor;                  // [n_groups]
+  uint32_t* g_reqs;                    // [n_reqs]
+  uint32_t* u_count;                   // [n_keys] |U_k| (zero between calls)
+  uint32_t* u_first;                   // [n_keys + 1]
+  uint32_t* u_cursor;                  // [n_keys]
+  uint32_t* u_rows;                    // [n_unpinned]
+  uint32_t n_unpinned;                 // u_first[n_keys], once pass 1 is done
+  uint32_t* pos;                       // [n_reqs] request row -> position in the namespace index
+  unsigned long long* item_keys;       // the (key, namespace) set: key << 32 | namespace, all-ones when free
+  uint32_t item_mask;
+  uint2* items;
+  uint32_t item_capacity;
+  lwse_drain_place_cost* rows;         // [n_keys]
+  uint32_t* counts;
+  // the solve
+  void* round;                         // namespace-form scratch (place_ns_scratch_bytes) holding the index of every namespace
+  size_t round_bytes;
+  lwse_place_out* s_out;               // [grid * slice_rows]
+  uint32_t* s_unpinned;                // [grid * slice_rows]
+  uint8_t* s_marks;                    // [grid * slice_rows]
+  uint32_t slice_rows, grid;
+};
+// Pass 0 (after the namespace index and the drain budget's pass 0): free slots per domain, the baseline totals, the group -> pinned
+// request index (count, scan, fill), U_k's leader rows counted, the rule-(b) candidates counted.
+// Pass 1 (pairs written): U_k's rows of restarted groups counted, then the U_k index scanned.
+// Pass 2 (u_rows, items sized): U_k filled, the key rows started, the items gathered (and the rows of U_k
+// outside every namespace counted), then the solve.
+int launch_drain_place(const DrainPlaceLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
+// The drain budget walk in pair mode: every restart pair key << 32 | group into pairs[p->counts[8]++] (below capacity).
+int launch_drain_restart_pairs(const DrainBudgetCostLaunch* p, unsigned long long* pairs, uint32_t capacity, int sm_count,
+                               cudaStream_t s, int* cuda_err);
+int launch_place_ns_drain(const DrainPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err);
+
 // ---- lwse_sha1_kernels.cu ----
 int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,
                 int sm_count, cudaStream_t s, int* cuda_err);

@@ -46,6 +46,7 @@
 #include <cuda.h>
 
 #include <cstdlib>
+#include <cstring>
 
 #include "lwse_device.cuh"
 #include "lwse_launch.cuh"
@@ -89,6 +90,26 @@ struct PlaceNsArgs {
   uint64_t xch_half_bytes;
   uint32_t xch_lagged;
 };
+
+// What the drain-placement instance of the namespace kernel reads besides PlaceNsArgs (lwse_resident_drain_place_cost).
+// That instance stages no word table, so the view travels in the bytes of its tensor-map parameter, and
+// PlaceNsArgs (with every other instance's code) stays as it is.  It runs over items (key, namespace) instead of
+// namespaces; out / unpinned / marks are per-CTA slices of slice_rows entries indexed by the position inside the
+// namespace, so that two CTAs may solve the same namespace for different keys at once.
+struct DrainNsView {
+  const uint2* items;            // {key, namespace}
+  const uint32_t* n_items;       // device count of insertions (capped by item_capacity)
+  uint32_t item_capacity;
+  const uint32_t* u_first;       // [n_keys + 1]: U_k = u_rows[u_first[k] .. u_first[k + 1])
+  const uint32_t* u_rows;
+  const uint32_t* pos;           // request row -> position in the namespace index (ns_rows), LWSE_NONE outside
+  uint8_t* marks;                // per CTA: 1 = the row at that position is in U_k
+  const lwse_place_out* base;    // the baseline rows
+  uint32_t* rows;                // the key rows (lwse_drain_place_cost, 16 words each)
+  uint32_t slice_rows;           // the largest namespace
+  uint32_t by_domain;
+};
+static_assert(sizeof(DrainNsView) <= sizeof(CUtensorMap), "the view travels in the tensor-map parameter");
 
 __device__ __forceinline__ uint32_t mix32n(uint32_t x) {
   x ^= x >> 16;
@@ -415,7 +436,12 @@ __device__ __forceinline__ void diff_row(const PlaceNsArgs& a, uint32_t r, const
 
 // kIndexed: the requests of a namespace are reached through the index (ns_rows); results, keys and the
 // unpinned list carry the request ROW either way.
-template <bool kScan, bool kIndexed>
+// kDrain (two-level, indexed): the drain-placement instance.  A persistent grid over DrainNsView::items; per item
+// the CTA lowers the staged capacity of the drained domain (a domain key: to 0; a node key: by the node's free
+// slots, and level 2 skips the node's word), reads the rows of U_k as unpinned, keeps every result and the
+// overflow state in its own slice (indexed by position, not row), diffs the namespace's rows against the
+// baseline and adds the counts to the key's row.  The rows keep their keys (priority, ROW).
+template <bool kScan, bool kIndexed, bool kDrain = false>
 __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
     place_ns_kernel(const PlaceNsArgs a, const __grid_constant__ CUtensorMap words_map) {
   extern __shared__ uint8_t s_dyn[];
@@ -440,6 +466,10 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
   NsReq* s_req = reinterpret_cast<NsReq*>(reinterpret_cast<uint8_t*>(s_slot) + (kScan ? 0u : free_bytes));
   unsigned long long* s_mbar = reinterpret_cast<unsigned long long*>(s_req + kNsCache);
   __shared__ uint32_t s_n_unp, s_n_cand, s_unsettled[3];
+  // kDrain: the view travels in the tensor-map parameter's bytes (launch_place_ns_drain).  That instance must never
+  // stage a word table (it would read the view as a tensor map): the two-level form stages none.
+  static_assert(!(kDrain && kScan), "the drain instance is two-level: its tensor-map parameter holds the view");
+  const DrainNsView* const drain = reinterpret_cast<const DrainNsView*>(&words_map);
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5, n_warps = blockDim.x >> 5;
   const uint32_t* words = table_bytes ? s_words : a.g_words;
   const uint32_t* order = table_bytes ? s_order : a.node_order;
@@ -474,8 +504,21 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
     bulk_load(s_first, a.dom_first, first_bytes, s_mbar);
   }
   bool staged = false;
+  uint32_t n_iter = 0, slice = 0;  // (kDrain; the other instances bound the loop by the parameter itself)
+  if constexpr (kDrain) {
+    n_iter = min(__ldcg(drain->n_items), drain->item_capacity);  // (an item the set refused is not in the list)
+    slice = blockIdx.x * drain->slice_rows;
+    mbar_wait(s_mbar);  // the overlays below write the staged capacities
+    staged = true;
+  }
 
-  for (uint32_t ns = blockIdx.x; ns < a.n_namespaces; ns += gridDim.x) {
+  for (uint32_t it = blockIdx.x; it < (kDrain ? n_iter : a.n_namespaces); it += gridDim.x) {
+    uint32_t ns = it, key = LWSE_NONE;
+    if constexpr (kDrain) {
+      const uint2 w = __ldcg(drain->items + it);
+      key = w.x;
+      ns = w.y;
+    }
     const uint32_t first = __ldcg(a.ns_first + ns), last = __ldcg(a.ns_first + ns + 1u);
     if (tid == 0) {
       s_n_unp = 0u;
@@ -485,6 +528,45 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
     for (uint32_t d = tid; d < a.n_domains; d += blockDim.x) s_hold[d] = ~0ull;
     __syncthreads();
     if (first >= last) continue;  // CTA-uniform
+    // where results and the unpinned list go: the row (by position in this CTA's slice for kDrain)
+    lwse_place_out* const obase = kDrain ? a.out + slice : a.out;
+    const uint32_t ubase = kDrain ? slice : first;
+    uint32_t skip_node = LWSE_NONE, od = LWSE_NONE, of = 0;  // kDrain: the drained node / domain, its staged capacity
+    if constexpr (kDrain) {
+      const DrainNsView& dv = *drain;
+      for (uint32_t p = tid; p < last - first; p += blockDim.x) dv.marks[slice + p] = 0u;
+      __syncthreads();
+      for (uint32_t j = __ldcg(dv.u_first + key) + tid, end = __ldcg(dv.u_first + key + 1u); j < end; j += blockDim.x) {
+        const uint32_t p = __ldcg(dv.pos + __ldcg(dv.u_rows + j));
+        if (p >= first && p < last) dv.marks[slice + p - first] = 1u;  // (LWSE_NONE: no namespace)
+      }
+      uint32_t lowered = 0;
+      if (dv.by_domain) {
+        od = key < a.n_domains ? key : LWSE_NONE;
+      } else if (key < a.n_nodes) {
+        const uint4 nr = ldg_keep(reinterpret_cast<const uint4*>(a.nodes + key));
+        const uint32_t fl = nr.w >> 16;
+        if ((fl & LWSE_NODE_SCHEDULABLE) && (fl & LWSE_NODE_HAS_TOPOLOGY) && nr.z < a.n_domains) {
+          const uint32_t cap = nr.w & 0xFFFFu, occ = occupancy_sum(a, a.occupancy, key);
+          lowered = cap > occ ? cap - occ : 0u;
+          od = nr.z;
+          skip_node = key;
+        }
+      }
+      if (od != LWSE_NONE) {
+        of = s_free[od];
+        __syncthreads();  // every thread has read the staged value before thread 0 lowers it
+        if (tid == 0) s_free[od] = dv.by_domain ? 0u : of - lowered;
+      }
+      __syncthreads();
+    }
+    auto req_hi = [&](uint32_t r, uint32_t p) -> uint4 {  // the request's second half, U_k unpinned for kDrain
+      uint4 hi = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r) + 1);
+      if constexpr (kDrain) {
+        if (__ldcg(drain->marks + slice + (p - first))) hi.w = LWSE_NONE;
+      }
+      return hi;
+    };
 
     // ---- phase 1: pinned claims, the list of live unpinned requests ----
     // the first kNsKeep requests of a thread stay in registers until their result is written
@@ -501,25 +583,26 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
         const uint32_t r = row_of(p);
         if constexpr (kIndexed) k_row[j] = r;
         k_lo[j] = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r));
-        k_hi[j] = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r) + 1);
+        k_hi[j] = req_hi(r, p);
       }
     }
-    auto claim = [&](uint32_t r, const uint4 lo, const uint4 hi) -> uint32_t {
+    // x: where the request's result and list entry go — its row, or (kDrain) its position in the namespace
+    auto claim = [&](uint32_t r, uint32_t x, const uint4 lo, const uint4 hi) -> uint32_t {
       const uint32_t leader = hi.w;
       uint32_t d = LWSE_NONE;
       if (leader == LWSE_NONE) {
         const bool dead = (int32_t)hi.z < 1;
         const uint4 row = make_uint4(LWSE_NONE, LWSE_NONE, dead ? LWSE_PLACE_UNSCHEDULABLE : 0u, 0u);
-        *reinterpret_cast<uint4*>(a.out + r) = row;
+        *reinterpret_cast<uint4*>(obase + x) = row;
         if (dead) {
           diff_row(a, r, row);
         } else {
           const uint32_t k = atomicAdd(&s_n_unp, 1u);
-          a.unpinned[first + k] = r;
+          a.unpinned[ubase + k] = x;
           if (k < kNsCache) {
             NsReq q;
             q.key = ns_place_key(u64_of(lo.x, lo.y), r, false);
-            q.r = r;
+            q.r = x;
             q.key_lo = lo.z;
             q.key_hi = lo.w;
             q.size = hi.z;
@@ -537,42 +620,48 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
       }
       return d;
     };
-    auto result = [&](uint32_t r, const uint4 lo, const uint4 hi, uint32_t d) {
+    auto result = [&](uint32_t r, uint32_t x, const uint4 lo, const uint4 hi, uint32_t d) {
       if (hi.w == LWSE_NONE) return;
       uint32_t flags = LWSE_PLACE_PINNED;
       if (d != LWSE_NONE) flags |= s_hold[d] == ns_place_key(u64_of(lo.x, lo.y), r, true) ? LWSE_PLACE_PLACED : LWSE_PLACE_CONFLICT;
       const uint4 row = make_uint4(d, hi.w, flags, 0u);
-      *reinterpret_cast<uint4*>(a.out + r) = row;
+      *reinterpret_cast<uint4*>(obase + x) = row;
       diff_row(a, r, row);
     };
 #pragma unroll
     for (uint32_t j = 0; j < kNsKeep; j++) {
       const uint32_t p = first + tid + j * blockDim.x;
-      if (p < last) k_dom[j] = claim(kIndexed ? k_row[j] : p, k_lo[j], k_hi[j]);
+      if (p < last) {
+        const uint32_t r = kIndexed ? k_row[j] : p;
+        k_dom[j] = claim(r, kDrain ? p - first : r, k_lo[j], k_hi[j]);
+      }
     }
     for (uint32_t p = first + tid + kNsKeep * blockDim.x; p < last; p += blockDim.x) {  // big namespaces: the rest, unkept
       const uint32_t r = row_of(p);
-      claim(r, ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r)), ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r) + 1));
+      claim(r, kDrain ? p - first : r, ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r)), req_hi(r, p));
     }
     __syncthreads();
     // results of the pinned requests: final from here on (pinned keys are below every unpinned key)
 #pragma unroll
     for (uint32_t j = 0; j < kNsKeep; j++) {
       const uint32_t p = first + tid + j * blockDim.x;
-      if (p < last) result(kIndexed ? k_row[j] : p, k_lo[j], k_hi[j], k_dom[j]);
+      if (p < last) {
+        const uint32_t r = kIndexed ? k_row[j] : p;
+        result(r, kDrain ? p - first : r, k_lo[j], k_hi[j], k_dom[j]);
+      }
     }
     for (uint32_t p = first + tid + kNsKeep * blockDim.x; p < last; p += blockDim.x) {
       const uint32_t r = row_of(p);
-      const uint4 lo = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r)), hi = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r) + 1);
+      const uint4 lo = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r)), hi = req_hi(r, p);
       uint32_t d = LWSE_NONE;
       if (hi.w != LWSE_NONE && hi.w < a.n_nodes) {
         const uint4 nr = ldg_keep(reinterpret_cast<const uint4*>(a.nodes + hi.w));
         if (((nr.w >> 16) & LWSE_NODE_HAS_TOPOLOGY) && nr.z < a.n_domains) d = nr.z;
       }
-      result(r, lo, hi, d);
+      result(r, kDrain ? p - first : r, lo, hi, d);
     }
     const uint32_t n_unp = s_n_unp;
-    if (n_unp == 0u) {
+    if (n_unp == 0u && !kDrain) {  // (kDrain: the diff below still runs; the rounds end at once)
       __syncthreads();
       continue;
     }
@@ -613,10 +702,11 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
         if (cached) {
           q = s_req[k];
         } else {  // overflow: the state lives in the result row (written by this warp only)
-          q.r = __ldcg(a.unpinned + first + k);
-          const uint4 o = __ldcg(reinterpret_cast<const uint4*>(a.out + q.r));
-          const uint4 lo = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + q.r)), hi = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + q.r) + 1);
-          q.key = ns_place_key(u64_of(lo.x, lo.y), q.r, false);
+          q.r = __ldcg(a.unpinned + ubase + k);
+          const uint32_t qrow = kDrain ? __ldcg(a.ns_rows + first + q.r) : q.r;
+          const uint4 o = __ldcg(reinterpret_cast<const uint4*>(obase + q.r));
+          const uint4 lo = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + qrow)), hi = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + qrow) + 1);
+          q.key = ns_place_key(u64_of(lo.x, lo.y), qrow, false);
           q.key_lo = lo.z;
           q.key_hi = lo.w;
           q.size = hi.z;
@@ -659,6 +749,9 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
               const uint32_t w = __ldcg(a.g_nodes2 + i);
               if ((w >> 28) == 0u) continue;
               const uint32_t n = w & 0x0FFFFFFFu;
+              if constexpr (kDrain) {
+                if (n == skip_node) continue;  // cordoned
+              }
               const uint32_t l = ((w >> 28) << 28) | (mix32n(key_hi ^ (n * 0x85EBCA77u)) >> 4);
               if (l > my_lo || (l == my_lo && n < my_n)) {
                 my_lo = l;
@@ -701,10 +794,10 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
         }
         if (lane == 0) {
           if (H == 0u || best_n == LWSE_NONE) {  // nothing feasible now, and the feasible set only shrinks
-            store_row(a.out + r, LWSE_NONE, LWSE_NONE, LWSE_PLACE_UNSCHEDULABLE, 0u);
+            store_row(obase + r, LWSE_NONE, LWSE_NONE, LWSE_PLACE_UNSCHEDULABLE, 0u);
             if (cached) s_req[k].dead = 1u;
           } else {
-            store_row(a.out + r, best_d, best_n, LWSE_PLACE_PLACED, H);
+            store_row(obase + r, best_d, best_n, LWSE_PLACE_PLACED, H);
             if (cached) s_req[k].cur = best_c;
             // A claim on an empty domain settles at once; any other outcome leaves somebody without
             // a domain who proposes again next round: count it.
@@ -728,6 +821,29 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
       }
     }
     __syncthreads();
+    if constexpr (kDrain) {  // the namespace's rows against the baseline, reduced in the CTA, one atomic per field
+      const DrainNsView& dv = *drain;
+      uint32_t c[kDrainCounts] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+      for (uint32_t p = first + tid; p < last; p += blockDim.x) {
+        const uint4 v = __ldcg(reinterpret_cast<const uint4*>(obase + (p - first)));
+        const uint4 o = __ldg(reinterpret_cast<const uint4*>(dv.base + row_of(p)));
+        drain_place_count(c, o, v, __ldcg(dv.marks + slice + (p - first)) != 0u);
+      }
+      uint32_t* const s_dcnt = reinterpret_cast<uint32_t*>(s_req);  // (the request cache is free after the rounds)
+      if (tid < kDrainCounts) s_dcnt[tid] = 0u;
+      __syncthreads();
+#pragma unroll
+      for (uint32_t f = 0; f < kDrainCounts; f++) {
+        const uint32_t sum = __reduce_add_sync(0xFFFFFFFFu, c[f]);
+        if (lane == 0 && sum) atomicAdd(&s_dcnt[f], sum);
+      }
+      __syncthreads();
+      uint32_t* krow = dv.rows + (size_t)key * 16u;
+      if (tid < kDrainCounts && s_dcnt[tid]) atomicAdd(krow + 2u + tid, s_dcnt[tid]);
+      if (tid == kDrainCounts) atomicAdd(krow + 11u, 1u);  // namespaces_solved
+      if (tid == 0 && od != LWSE_NONE) s_free[od] = of;
+      __syncthreads();
+    }
   }
   if (!staged) mbar_wait(s_mbar);  // never leave a bulk copy in flight behind a CTA that exits
 }
@@ -1021,6 +1137,90 @@ int launch_place_whatif_index(const lwse_place_req* d_reqs, uint32_t n_reqs, uin
     *cuda_err = (int)e;
     return -1;
   }
+  return 3;
+}
+
+// request row -> its position in the namespace index (rows of no namespace keep the caller's LWSE_NONE)
+__global__ void __launch_bounds__(256) drain_place_pos_kernel(const uint32_t* ns_first, const uint32_t* ns_rows,
+                                                              uint32_t n_namespaces, uint32_t* pos) {
+  const uint32_t n = __ldcg(ns_first + n_namespaces);
+  for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) pos[__ldcg(ns_rows + p)] = p;
+}
+
+// The drain-placement solve (lwse_resident_drain_place_cost): the capacities of the resident node index (the
+// condense kernel's part A alone: n_reqs = 0 leaves the request rows and the index alone), then the drain
+// instance over p->grid CTAs.  The round scratch holds the namespace index of every namespace
+// (launch_place_whatif_index with every namespace touched).
+int launch_place_ns_drain(const DrainPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  const NsLayout l = ns_layout(p->n_nodes, p->n_domains, p->n_reqs, p->n_namespaces);
+  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) {
+    *cuda_err = (int)cudaErrorInvalidValue;
+    return -1;
+  }
+  uint8_t* base = static_cast<uint8_t*>(p->round);
+  PlaceNsArgs a{};
+  a.nodes = p->nodes;
+  a.reqs = p->reqs;
+  a.occupancy = p->occupancy;
+  a.dom_first = p->dom_first;
+  a.node_order = p->node_order;
+  a.g_words = reinterpret_cast<uint32_t*>(base + l.words);
+  a.g_nodes2 = reinterpret_cast<uint32_t*>(base + l.nodes2);
+  a.g_dom_free = reinterpret_cast<uint32_t*>(base + l.dom_free);
+  a.ns_first = reinterpret_cast<uint32_t*>(base + l.ns_first);
+  a.ns_rows = reinterpret_cast<uint32_t*>(base + l.ns_rows);
+  a.ns_count = reinterpret_cast<uint32_t*>(base + l.ns_count);
+  a.ns_cursor = reinterpret_cast<uint32_t*>(base + l.ns_cursor);
+  a.counters = reinterpret_cast<uint32_t*>(base + l.counters) + 4u * 8u;  // a block no other call uses
+  a.n_nodes = p->n_nodes;
+  a.n_domains = p->n_domains;
+  a.n_namespaces = p->n_namespaces;
+  a.n_parts = 1u;
+  a.word_rows = l.word_rows;
+  {
+    uint64_t grid = ((uint64_t)p->n_domains * 32u + 255) / 256;
+    if (grid < 1) grid = 1;
+    if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
+    place_condense_kernel<<<(unsigned)grid, 256, 0, s>>>(a);  // (a.n_reqs = 0: capacities only)
+    grid = ((uint64_t)p->n_reqs + 255) / 256;
+    if (grid < 1) grid = 1;
+    if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
+    drain_place_pos_kernel<<<(unsigned)grid, 256, 0, s>>>(a.ns_first, a.ns_rows, p->n_namespaces, p->pos);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+  }
+  DrainNsView v{};
+  v.items = p->items;
+  v.n_items = p->counts + 4;
+  v.item_capacity = p->item_capacity;
+  v.u_first = p->u_first;
+  v.u_rows = p->u_rows;
+  v.pos = p->pos;
+  v.marks = p->s_marks;
+  v.base = p->base;
+  v.rows = reinterpret_cast<uint32_t*>(p->rows);
+  v.slice_rows = p->slice_rows;
+  v.by_domain = p->by_domain ? 1u : 0u;
+  // The drain instance stages no word table (two-level form), so its tensor-map parameter is free to carry the
+  // view by value; place_ns_kernel static_asserts that the instance is two-level.
+  CUtensorMap view;
+  memset(&view, 0, sizeof(view));
+  memcpy(&view, &v, sizeof(v));
+  a.n_reqs = p->n_reqs;
+  a.out = p->s_out;
+  a.unpinned = p->s_unpinned;
+  cudaError_t e = cudaSuccess;
+  const size_t smem = ns_smem_bytes(l.word_rows, p->n_domains, false, false);
+  static thread_local size_t attr_set = 0;
+  if (smem > attr_set) {
+    e = cudaFuncSetAttribute(place_ns_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    attr_set = smem;
+  }
+  place_ns_kernel<false, true, true><<<p->grid, kNsThreads, smem, s>>>(a, view);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
   return 3;
 }
 

@@ -48,6 +48,7 @@ SYMBOLS = {
     "lwse_resident_drain_cost": ([C.c_void_p, C.c_void_p], C.c_int),
     "lwse_resident_drain_budget": ([C.c_void_p, C.POINTER(R.DrainBudgetQuery)], C.c_int),
     "lwse_resident_drain_budget_cost": ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
+    "lwse_resident_drain_place_cost": ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_resident_ds_drain": ([C.c_void_p, C.POINTER(R.DsDrainQuery)], C.c_int),
     "lwse_resident_ds_drain_cost": ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_place_host": (
@@ -500,6 +501,16 @@ class Engine:
         n = self.n_nodes if scope == "nodes" else self.n_domains
         out = R.aligned_empty(max(n, 1), R.DRAIN_BUDGET_COST)
         self._check(lib().lwse_resident_drain_budget_cost(self._h, self._DRAIN_SCOPES[scope], R.ptr(out)))
+        return out[:n]
+
+    def resident_drain_place_cost(self, scope: str = "nodes") -> np.ndarray:
+        """lwse_resident_drain_place_cost: one ``records.DRAIN_PLACE_COST`` row per node (``scope="nodes"``) or per
+        domain (``"domains"``), row k holding what the three calls ``resident_drain_whatif`` →
+        ``IncrementalEncoder.drain_place_query`` → ``resident_place_whatif`` answer for that key alone: whether
+        the groups the drain restarts find a new exclusive domain — every key in one call."""
+        n = self.n_nodes if scope == "nodes" else self.n_domains
+        out = R.aligned_empty(max(n, 1), R.DRAIN_PLACE_COST)
+        self._check(lib().lwse_resident_drain_place_cost(self._h, self._DRAIN_SCOPES[scope], R.ptr(out)))
         return out[:n]
 
     def resident_ds_drain(self, nodes=None, domains=None, capacity=None, outputs=False):

@@ -599,6 +599,21 @@ class IncrementalEncoder:
         vals["leader_node"] = R.NONE
         return [self.whatif_cordon(node_names), (R.TABLE_PLACE_REQS, rows, vals)]
 
+    def drain_place_report(self, rows, scope: str = "nodes") -> list:
+        """A ``resident_drain_place_cost`` answer as dicts, one per key: ``node`` (scope ``"nodes"``) or
+        ``topology`` (``"domains"``) — the node's name or the topology value, None for a row nobody holds —
+        then the row's fields.  Nothing in the encoder changes."""
+        if scope == "nodes":
+            names = {row: name for name, row in self.node_index.items()}
+            field = "node"
+        elif scope == "domains":
+            names = {d: v for v, d in self._domain_ids.items()}
+            field = "topology"
+        else:
+            raise ValueError(f"unknown scope {scope!r}")
+        return [{field: names.get(k), **{f: int(r[f]) for f in R.DRAIN_PLACE_COST.names if f != "reserved"}}
+                for k, r in enumerate(rows)]
+
     # ------------------------------------------------------------------ results
     def tables(self):
         """(lws, groups, pod_state, pod_ident, reqs) trimmed to the rows in use (+ spare already laid out)."""

@@ -592,6 +592,15 @@ DRAIN_BUDGET_COST = np.dtype(DRAIN_COST.descr + [("lws_touched", "<u4"), ("lws_b
                                                  ("lws_loses_available", "<u4"), ("min_margin", "<i4")])
 assert DRAIN_BUDGET_COST.itemsize == 48
 
+# lwse_drain_place_cost: per node or per domain, whether the groups its drain restarts find a new domain
+DRAIN_PLACE_COST = np.dtype(
+    [("groups_restarted", "<u4"), ("unpinned", "<u4"), ("stranded", "<u4"), ("bumped", "<u4"), ("n_changed", "<u4"),
+     ("n_lost", "<u4"), ("n_moved", "<u4"), ("n_gained", "<u4"), ("n_placed", "<u4"), ("n_unschedulable", "<u4"),
+     ("n_conflict", "<u4"), ("namespaces_solved", "<u4"), ("reserved", "<u4", (4,))],
+    align=False,
+)
+assert DRAIN_PLACE_COST.itemsize == 64
+
 
 class DrainBudgetQuery(C.Structure):
     """lwse_drain_budget_query: the touched LWS rows of one drain set (node rows or domain ids in, the
