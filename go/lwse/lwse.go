@@ -211,6 +211,13 @@ func (e *Engine) DrainPlaceCost(scope uint32, out *C.lwse_drain_place_cost) erro
 	return e.check(C.lwse_resident_drain_place_cost(e.h, C.uint32_t(scope), out))
 }
 
+// DrainWaves packs distinct node rows (scope LWSE_DRAIN_NODES) or domain ids (LWSE_DRAIN_DOMAINS), in the order
+// given, first-fit into at most q.max_waves waves whose drain takes no LeaderWorkerSet below its floor.  A
+// maintenance controller drains wave 0, waits for recovery and calls again with the keys that remain.
+func (e *Engine) DrainWaves(q *C.lwse_drain_waves_query) error {
+	return e.check(C.lwse_resident_drain_waves(e.h, q))
+}
+
 // GroupKeys computes SHA-1 digests (20 bytes each) of n strings laid out CSR-style.
 func (e *Engine) GroupKeys(bytes *C.uint8_t, offsets *C.uint32_t, n uint32, digests *C.uint8_t) error {
 	return e.check(C.lwse_group_keys_host(e.h, bytes, offsets, C.uint32_t(n), digests))

@@ -1000,6 +1000,84 @@ typedef struct lwse_drain_budget_cost {
 } lwse_drain_budget_cost;
 LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lwse_drain_budget_cost* out);
 
+/* ---- drain waves --------------------------------------------------------------------------------
+ * "Which of these nodes (domains) can I drain together?"  A first-fit plan of a list of keys into waves whose
+ * set-form drain budget breaches no LeaderWorkerSet (DESIGN.md §3.5, "Drain waves").
+ *
+ * Definition.  ids[0..n_ids) are DISTINCT node rows (LWSE_DRAIN_NODES) or domain ids (LWSE_DRAIN_DOMAINS);
+ * scope, drain sets, EVALUATED, floor, ready_before, lost(L, D) and BREACHED are those of
+ * lwse_resident_drain_budget.  Waves W_0, W_1, ... start empty; the keys are taken in the caller's order and
+ * key k_i gets the first of:
+ *   1. LWSE_DRAINW_BREACHES_ALONE  the set form over {k_i} has n_breached > 0 (wave LWSE_NONE);
+ *   2. LWSE_DRAINW_PLANNED         wave w: the smallest index of an open wave such that the set form over
+ *                                  W_w ∪ {k_i} has n_breached == 0; with no such wave and fewer than max_waves
+ *                                  open, a new wave is opened for it;
+ *   3. LWSE_DRAINW_NO_WAVE         neither (wave LWSE_NONE).
+ * Every wave is judged against the same baseline (the most recently submitted sweep): the plan assumes that
+ * the groups one wave restarts are ready again before the next starts, so a controller drains wave 0, waits
+ * for recovery and calls again with the keys that remain.  The answer is the first-fit outcome of that
+ * sequential order, whatever the device interleaving; first-fit does not promise the fewest waves.
+ *
+ * Exact through the per-key restart pairs: draining a union of keys restarts the union of the groups each
+ * key restarts alone, so lost(L, W) is the number of distinct ready member groups of L among the pairs of W's
+ * keys, and adding k to W is admissible iff every evaluated L to which k adds new > 0 such groups has
+ * lost(L, W) + new <= ready_before - floor (in 64 bits).
+ *
+ * Readiness, isolation and errors: as lwse_resident_drain_budget, and LWSE_ERR_INVALID_ARG also for a
+ * duplicate or out-of-range id, max_waves of 0 or above LWSE_DRAIN_WAVES_MAX, a NULL ids / keys (n_ids > 0)
+ * or waves, or a nonzero reserved field; LWSE_ERR_UNSUPPORTED on an engine with a peer exchange (a plan is not
+ * a sum over ranks); LWSE_ERR_OOM rather than a wrong row when a sized scratch table refuses an entry.  A
+ * refused call writes no output.  n_ids = 0 is valid and opens no wave. */
+#define LWSE_DRAIN_WAVES_MAX 64u
+
+#define LWSE_DRAINW_PLANNED 0u
+#define LWSE_DRAINW_BREACHES_ALONE 1u
+#define LWSE_DRAINW_NO_WAVE 2u
+
+/* One key of the plan, in query order (32 B).  The alone columns equal row `id` of
+ * lwse_resident_drain_budget_cost for the same scope. */
+typedef struct lwse_drain_wave_key {
+  uint32_t id;                /* the node row or domain id                                               */
+  uint32_t wave;              /* its wave, or LWSE_NONE                                                  */
+  uint32_t status;            /* LWSE_DRAINW_*                                                           */
+  uint32_t groups_restarted;  /* the key alone                                                           */
+  uint32_t ready_restarted;
+  uint32_t lws_touched;
+  uint32_t lws_breached;
+  uint32_t reserved;
+} lwse_drain_wave_key;
+
+/* One opened wave (48 B): the set-form totals of lwse_resident_drain_budget over the wave's ids. */
+typedef struct lwse_drain_wave {
+  uint32_t n_keys;
+  uint32_t lws_touched;
+  uint32_t lws_loses_available;
+  uint32_t n_pods_evicted;
+  uint32_t n_leaders_evicted;
+  uint32_t n_groups_restarted;
+  uint32_t n_ready_restarted;
+  int32_t min_margin;         /* min over evaluated touched L of ready_after - floor; INT32_MAX for none */
+  uint64_t n_pods_recreated;
+  uint64_t reserved;
+} lwse_drain_wave;
+
+typedef struct lwse_drain_waves_query {
+  /* in */
+  const uint32_t* ids;        /* [n_ids] distinct node rows or domain ids (by scope), host memory        */
+  uint32_t n_ids;
+  uint32_t scope;             /* LWSE_DRAIN_NODES or LWSE_DRAIN_DOMAINS                                  */
+  uint32_t max_waves;         /* 1 .. LWSE_DRAIN_WAVES_MAX                                               */
+  uint32_t reserved;          /* 0                                                                       */
+  lwse_drain_wave_key* keys;  /* [n_ids] out                                                             */
+  lwse_drain_wave* waves;     /* [max_waves] out: rows 0 .. n_waves                                      */
+  /* out */
+  uint32_t n_waves;
+  uint32_t n_planned;
+  uint32_t n_breaches_alone;
+  uint32_t n_no_wave;
+} lwse_drain_waves_query;
+LWSE_API int lwse_resident_drain_waves(lwse_engine* e, lwse_drain_waves_query* q);
+
 /* ---- drain placement ----------------------------------------------------------------------------
  * "If I drain this node or this domain, do the groups it restarts find a new exclusive domain?" — for every
  * node (LWSE_DRAIN_NODES, n_nodes rows) or every domain (LWSE_DRAIN_DOMAINS, n_domains rows) in one call.

@@ -272,4 +272,47 @@ __device__ __forceinline__ void drain_place_count(uint32_t* c, const uint4 o, co
   c[8] += ((v.z & LWSE_PLACE_CONFLICT) ? 1u : 0u) - ((o.z & LWSE_PLACE_CONFLICT) ? 1u : 0u);
 }
 
+// What the budget of one LWS row needs from its row and its baseline result row.
+// (lwse_drain_kernels.cu and lwse_drain_wave_kernels.cu: the drain budget's definition in lwse.h.)
+struct LwsBudget {
+  uint32_t gbase, gcount;  // the group range; gcount = 0 when it lies outside the group table
+  int32_t replicas, floor, ready_before;
+  bool evaluated, available;
+};
+
+constexpr uint32_t kBudgetExcluded = LWSE_LOUT_BAD_TABLE | LWSE_LOUT_IRREGULAR | LWSE_LOUT_RUP_ERROR | LWSE_LOUT_STATUS_ERROR;
+
+__device__ __forceinline__ int32_t clamp_i32(int64_t v) {
+  return (int32_t)(v < INT32_MIN ? (int64_t)INT32_MIN : (v > INT32_MAX ? (int64_t)INT32_MAX : v));
+}
+
+// scaled_value (lwse_device.cuh) rounded down, kept in 64 bits as Go's int: the floor's mu must not wrap
+// when a percentage above 100 of a large replicas passes int32.  (The sweep keeps its int32(mu), :313.)
+__device__ __forceinline__ int64_t unavailable_i64(int32_t val, bool is_percent, int32_t total) {
+  if (!is_percent) return val;
+  const int64_t num = (int64_t)val * (int64_t)total;
+  const int64_t q = num / 100;
+  return (num - q * 100 != 0 && num < 0) ? q - 1 : q;
+}
+
+__device__ __forceinline__ LwsBudget budget_of(const lwse_lws_rec* lws, const lwse_lws_out* lws_out, uint32_t L,
+                                               uint32_t n_groups) {
+  const uint4* row = reinterpret_cast<const uint4*>(lws + L);
+  const uint4 r0 = ldg_cached(row + 0), r1 = ldg_cached(row + 1), r3 = ldg_cached(row + 3);
+  const uint4* orow = reinterpret_cast<const uint4*>(lws_out + L);
+  const uint4 o0 = __ldg(orow + 0), o1 = __ldg(orow + 1);
+  const uint32_t lflags = r0.w, oflags = o1.z;
+  LwsBudget b;
+  b.replicas = (int32_t)r1.x;
+  b.gbase = r3.z;
+  b.gcount = (uint64_t)r3.z + r3.w <= n_groups ? r3.w : 0u;
+  b.evaluated = !(oflags & kBudgetExcluded) && !(lflags & LWSE_LWS_INTSTR_INVALID);
+  b.available = ((oflags & LWSE_LOUT_COND_MASK) >> LWSE_LOUT_COND_SHIFT) == LWSE_COND_AVAILABLE;
+  b.ready_before = (int32_t)o0.w;
+  const int64_t mu = unavailable_i64((int32_t)r1.w, lflags & LWSE_LWS_UNAVAIL_IS_PERCENT, b.replicas);  // :302
+  const int64_t fl = (int64_t)b.replicas - mu;
+  b.floor = b.evaluated ? clamp_i32(fl < 0 ? 0 : fl) : 0;
+  return b;
+}
+
 }  // namespace lwse

@@ -238,6 +238,13 @@ struct lwse_engine {
   // per-CTA slices
   DevBuf dp_cost, dp_words, dp_domfree, dp_gidx, dp_uidx, dp_pairs, dp_urows, dp_pos, dp_items, dp_rows, dp_touched, dp_round,
       dp_slices;
+  // drain waves (lwse_resident_drain_waves): the drain budget's key rows, the counters, the ids, the key positions, the
+  // key buckets (count | first | cursor), the restart pairs, the pair records, the touched-row index (count | first |
+  // cursor), the dense rows, the lost counters, the group and row wave masks, the stamps, the answer; the ids going
+  // in and the answer coming back through dv_host
+  DevBuf dv_cost, dv_words, dv_ids, dv_pos, dv_kidx, dv_pairs, dv_recs, dv_lidx, dv_dense, dv_lost, dv_gwaves, dv_rwaves,
+      dv_stamps, dv_out;
+  PinBuf dv_host;
   // DS drain (lwse_resident_ds_drain*): lost[L] and the after copy of lws_out, the before / after sweep outputs, the
   // touched DS rows, the reverse link index (count | first | cursor) and its entries, the key rows, the (DS, key) table
   DevBuf dd_lost, dd_lws_after, dd_out[2], dd_role_out[2], dd_revrole_out[2], dd_rows, dd_index, dd_entries, dd_cost, dd_table;
@@ -476,13 +483,15 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->dd_table, &e->rw_rows, &e->rw_lws, &e->rw_off, &e->rw_sums, &e->rw_groups, &e->rw_src,
                       &e->rw_group_out, &e->rw_now, &e->rw_scan, &e->dw_props, &e->dw_qroles, &e->dw_count, &e->dw_off,
                       &e->dw_sums, &e->dw_ds, &e->dw_roles, &e->dw_revroles, &e->dw_links, &e->dw_now, &e->dw_role_out,
-                      &e->dw_revrole_out};
+                      &e->dw_revrole_out, &e->dv_cost, &e->dv_words, &e->dv_ids, &e->dv_pos, &e->dv_kidx, &e->dv_pairs,
+                      &e->dv_recs, &e->dv_lidx, &e->dv_dense, &e->dv_lost, &e->dv_gwaves, &e->dv_rwaves, &e->dv_stamps,
+                      &e->dv_out};
     if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
     if (e->lf_stream) cudaStreamSynchronize(e->lf_stream);
     if (e->wf_stream) cudaStreamSynchronize(e->wf_stream);
     for (DevBuf* b : bufs) b->release();
     PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc, &e->rd_pin, &e->rd_stage, &e->fc_words, &e->lf_words,
-                      &e->wf_stage, &e->wf_words, &e->dw_words};
+                      &e->wf_stage, &e->wf_words, &e->dw_words, &e->dv_host};
     for (PinBuf* b : pins) b->release();
     if (e->ev_place) cudaEventDestroy(e->ev_place);
     if (e->h_rounds) cudaFreeHost(e->h_rounds);
@@ -2778,6 +2787,159 @@ LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lws
   LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 16, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   if (words[2]) return LWSE_ERR_OOM;  // an insert the table refused: no answer rather than a wrong one
+  return LWSE_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Drain waves
+// ---------------------------------------------------------------------------
+// Three host synchronisations, each sizing what follows: the restart pairs of every key (the drain budget's pass 0
+// counts them per key), then the touched LWS rows (the lost counters are sized by them, not by n_lws), then the
+// answer, read back with one copy.  Everything reads the resident tables and the baseline results in place.
+LWSE_API int lwse_resident_drain_waves(lwse_engine* e, lwse_drain_waves_query* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!drain_budget_ready(e)) return LWSE_ERR_NOT_READY;
+  if (q->scope != LWSE_DRAIN_NODES && q->scope != LWSE_DRAIN_DOMAINS) return LWSE_ERR_INVALID_ARG;
+  if (q->reserved || q->max_waves == 0 || q->max_waves > LWSE_DRAIN_WAVES_MAX || !q->waves) return LWSE_ERR_INVALID_ARG;
+  if (q->n_ids && (!q->ids || !q->keys)) return LWSE_ERR_INVALID_ARG;
+  const bool by_domain = q->scope == LWSE_DRAIN_DOMAINS;
+  const uint32_t nn = e->n_nodes, nk = by_domain ? e->n_domains : nn, m = q->n_ids;
+  const uint32_t nl = e->rn_lws, ng = e->rn_groups;
+  LWSE_CUDA(e, e->wf_stage.reserve((size_t)nk + 16));
+  uint8_t* seen = static_cast<uint8_t*>(e->wf_stage.h);
+  memset(seen, 0, nk);
+  for (uint32_t i = 0; i < m; i++) {
+    const uint32_t id = q->ids[i];
+    if (id >= nk || seen[id]) return LWSE_ERR_INVALID_ARG;  // out of range, or a duplicate
+    seen[id] = 1;
+  }
+  if (e->xch_world > 0) return LWSE_ERR_UNSUPPORTED;  // (a plan is not a sum over ranks)
+  const uint32_t mw = q->max_waves;
+  const size_t keys_bytes = (size_t)m * sizeof(lwse_drain_wave_key);
+  const size_t out_bytes = 16 + keys_bytes + (size_t)mw * sizeof(lwse_drain_wave);
+  DeviceGuard guard(e->device);
+  LWSE_CUDA(e, e->dv_cost.reserve((size_t)nk * sizeof(lwse_drain_budget_cost) + 16));
+  LWSE_CUDA(e, e->dv_words.reserve(128));
+  LWSE_CUDA(e, e->wf_words.reserve(128));
+  LWSE_CUDA(e, e->dv_ids.reserve((size_t)m * 4 + 16));
+  LWSE_CUDA(e, e->dv_pos.reserve((size_t)nk * 4 + 16));
+  LWSE_CUDA(e, e->dv_kidx.reserve(((size_t)m * 3 + 2) * 4 + 16));
+  LWSE_CUDA(e, e->dv_lidx.reserve(((size_t)nl * 3 + 2) * 4 + 16));
+  LWSE_CUDA(e, e->dv_dense.reserve((size_t)nl * 16 + 16));
+  LWSE_CUDA(e, e->dv_gwaves.reserve((size_t)ng * 8 + 16));
+  LWSE_CUDA(e, e->dv_out.reserve(out_bytes));
+  LWSE_CUDA(e, e->dv_host.reserve(out_bytes > (size_t)m * 4 ? out_bytes : (size_t)m * 4));
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* d_words = (uint32_t*)e->dv_words.p;  // [0..15] the walk's counters, [16..19] this call's (u64)
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  if (m) {
+    memcpy(e->dv_host.h, q->ids, (size_t)m * 4);
+    LWSE_CUDA(e, cudaMemcpyAsync(e->dv_ids.p, e->dv_host.h, (size_t)m * 4, cudaMemcpyHostToDevice, s));
+  }
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_cost.p, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
+  LWSE_CUDA(e, cudaMemsetAsync(d_words, 0, 128, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_pos.p, 0xFF, (size_t)nk * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_kidx.p, 0, (size_t)m * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lidx.p, 0, (size_t)nl * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_gwaves.p, 0, (size_t)ng * 8, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_out.p, 0, out_bytes, s));
+  // the key rows and their restart pairs: the drain budget's pass 0
+  lwse::DrainBudgetCostLaunch bp{};
+  bp.lws = (const lwse_lws_rec*)e->r_lws.p;
+  bp.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
+  bp.groups = (const lwse_group_rec*)e->r_groups.p;
+  bp.pod_state = (const uint8_t*)e->r_pst.p;
+  bp.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
+  bp.baseline = (const lwse_group_out*)e->r_group_out.p;
+  bp.nodes = (const lwse_node_rec*)e->nodes.p;
+  bp.occupancy = (const uint32_t*)e->r_occ.p;
+  bp.cost = (lwse_drain_budget_cost*)e->dv_cost.p;
+  bp.counts = d_words;
+  bp.n_pods = e->rn_pods;
+  bp.n_lws = nl;
+  bp.n_groups = ng;
+  bp.n_nodes = nn;
+  bp.n_domains = e->n_domains;
+  bp.n_keys = nk;
+  bp.by_domain = by_domain;
+  int cuda_err = 0;
+  int launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  lwse::DrainWavesLaunch p{};
+  p.lws = bp.lws;
+  p.lws_out = bp.lws_out;
+  p.groups = bp.groups;
+  p.baseline = bp.baseline;
+  p.cost = bp.cost;
+  p.ids = (const uint32_t*)e->dv_ids.p;
+  p.pos_of = (uint32_t*)e->dv_pos.p;
+  p.count = (uint32_t*)e->dv_kidx.p;
+  p.first = p.count + m;
+  p.cursor = p.first + m + 1;
+  p.l_count = (uint32_t*)e->dv_lidx.p;
+  p.l_first = p.l_count + nl;
+  p.l_cursor = p.l_first + nl + 1;
+  p.dense = (uint4*)e->dv_dense.p;
+  p.g_waves = (unsigned long long*)e->dv_gwaves.p;
+  p.out = (uint8_t*)e->dv_out.p;
+  p.counts = reinterpret_cast<unsigned long long*>(d_words + 16);
+  p.n_lws = nl;
+  p.n_groups = ng;
+  p.n_keys = nk;
+  p.m = m;
+  p.max_waves = mw;
+  p.cols = (m < mw ? m : mw) + 1u;
+  launched = lwse::launch_drain_waves(&p, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_words + 16, 8, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  uint64_t n_pairs = 0;
+  memcpy(&n_pairs, words, 8);
+  // (every index is 32-bit, and the plan kernel's items are a key's pairs times the columns)
+  if (n_pairs > 0xFFFFFFFFull / (LWSE_DRAIN_WAVES_MAX + 1u)) return LWSE_ERR_OOM;
+  LWSE_CUDA(e, e->dv_pairs.reserve((size_t)n_pairs * 8 + 16));
+  LWSE_CUDA(e, e->dv_recs.reserve((size_t)n_pairs * 16 + 16));
+  launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dv_pairs.p, (uint32_t)n_pairs, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  p.pairs = (const unsigned long long*)e->dv_pairs.p;
+  p.n_pairs = (uint32_t)n_pairs;
+  p.recs = (uint4*)e->dv_recs.p;
+  launched = lwse::launch_drain_waves(&p, 1, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 64, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 16, d_words + 16, 16, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 20, p.l_first + nl, 4, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  // (the walk found another pair count, or a bucket refused a pair: no answer rather than a wrong one)
+  if (ng && words[8] != n_pairs) return LWSE_ERR_OOM;
+  if (words[18] || words[19]) return LWSE_ERR_OOM;
+  const uint32_t n_dense = words[20];
+  LWSE_CUDA(e, e->dv_lost.reserve((size_t)n_dense * p.cols * 4 + 16));
+  LWSE_CUDA(e, e->dv_rwaves.reserve((size_t)n_dense * 16 + 16));
+  LWSE_CUDA(e, e->dv_stamps.reserve((size_t)n_dense * 8 + 16));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lost.p, 0, (size_t)n_dense * p.cols * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_rwaves.p, 0, (size_t)n_dense * 16, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_stamps.p, 0, (size_t)n_dense * 8, s));
+  p.n_dense = n_dense;
+  p.lost = (uint32_t*)e->dv_lost.p;
+  p.row_waves = (unsigned long long*)e->dv_rwaves.p;
+  p.stamps = (uint32_t*)e->dv_stamps.p;
+  launched = lwse::launch_drain_waves(&p, 2, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(e->dv_host.h, p.out, out_bytes, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint8_t* h = static_cast<const uint8_t*>(e->dv_host.h);
+  uint32_t totals[4];
+  memcpy(totals, h, 16);
+  if (m) memcpy(q->keys, h + 16, keys_bytes);
+  memcpy(q->waves, h + 16 + keys_bytes, (size_t)totals[0] * sizeof(lwse_drain_wave));
+  q->n_waves = totals[0];
+  q->n_planned = totals[1];
+  q->n_breaches_alone = totals[2];
+  q->n_no_wave = totals[3];
   return LWSE_OK;
 }
 

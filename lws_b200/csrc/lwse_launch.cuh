@@ -382,6 +382,43 @@ int launch_drain_restart_pairs(const DrainBudgetCostLaunch* p, unsigned long lon
                                cudaStream_t s, int* cuda_err);
 int launch_place_ns_drain(const DrainPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err);
 
+// ---- lwse_drain_wave_kernels.cu ----
+// lwse_resident_drain_waves.  out: the query totals (16 B), m lwse_drain_wave_key rows, then max_waves
+// lwse_drain_wave rows (the opened ones written).  counts (device, u64, zeroed by the caller): [0] the restart pairs
+// of every key, [1] pairs the key buckets refused.
+struct DrainWavesLaunch {
+  const lwse_lws_rec* lws;
+  const lwse_lws_out* lws_out;
+  const lwse_group_rec* groups;
+  const lwse_group_out* baseline;
+  const lwse_drain_budget_cost* cost;  // the drain budget's pass 0 rows of every key
+  const uint32_t* ids;                 // [m] the query's keys
+  uint32_t* pos_of;                    // [n_keys] the position of a listed key; all-ones (set by the caller) otherwise
+  uint32_t* count;                     // [m] the key buckets: pairs per position (zero between calls)
+  uint32_t* first;                     // [m + 1]
+  uint32_t* cursor;                    // [m]
+  const unsigned long long* pairs;     // the pair walk's key << 32 | group
+  uint32_t n_pairs;
+  uint4* recs;                         // [first[m]] {group, owner, bits, pod_count} by position
+  uint32_t* l_count;                   // [n_lws] 1 for a touched LWS row (zero between calls)
+  uint32_t* l_first;                   // [n_lws + 1] its dense row
+  uint32_t* l_cursor;                  // [n_lws]
+  uint4* dense;                        // [n_lws] {ready_before, floor, flags, 0} by dense row
+  uint32_t n_dense;                    // l_first[n_lws], once pass 1 is done
+  uint32_t* lost;                      // [n_dense * cols] lost groups per (dense row, wave), zeroed by the caller
+  uint32_t cols;                       // min(max_waves, m) + 1: the waves and the key-alone column
+  unsigned long long* g_waves;         // [n_groups] the waves that hold the group, zeroed by the caller
+  unsigned long long* row_waves;       // [2 * n_dense] the waves touching the row / losing one of its groups below replicas
+  uint32_t* stamps;                    // [2 * n_dense] the last position that touched / breached the row alone, zeroed
+  uint8_t* out;
+  unsigned long long* counts;
+  uint32_t n_lws, n_groups, n_keys, m, max_waves;
+};
+// Pass 0 (after the drain budget's pass 0): positions, bucket sizes and the alone columns; the buckets scanned.
+// Pass 1 (pairs written): the buckets filled, the touched rows scanned, the dense rows.  Pass 2 (n_dense, lost and
+// the wave masks sized): the plan, then the wave rows' per-row columns and pods / leaders.
+int launch_drain_waves(const DrainWavesLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
+
 // ---- lwse_sha1_kernels.cu ----
 int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,
                 int sm_count, cudaStream_t s, int* cuda_err);

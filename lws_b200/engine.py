@@ -49,6 +49,7 @@ SYMBOLS = {
     "lwse_resident_drain_budget": ([C.c_void_p, C.POINTER(R.DrainBudgetQuery)], C.c_int),
     "lwse_resident_drain_budget_cost": ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_resident_drain_place_cost": ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
+    "lwse_resident_drain_waves": ([C.c_void_p, C.POINTER(R.DrainWavesQuery)], C.c_int),
     "lwse_resident_ds_drain": ([C.c_void_p, C.POINTER(R.DsDrainQuery)], C.c_int),
     "lwse_resident_ds_drain_cost": ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_place_host": (
@@ -502,6 +503,27 @@ class Engine:
         out = R.aligned_empty(max(n, 1), R.DRAIN_BUDGET_COST)
         self._check(lib().lwse_resident_drain_budget_cost(self._h, self._DRAIN_SCOPES[scope], R.ptr(out)))
         return out[:n]
+
+    def resident_drain_waves(self, nodes=None, domains=None, max_waves=R.DRAIN_WAVES_MAX):
+        """lwse_resident_drain_waves: the distinct node rows ``nodes`` — or domain ids ``domains`` — packed first-fit,
+        in the order given, into at most ``max_waves`` waves whose drain takes no LeaderWorkerSet below its
+        floor.  Give exactly one of the two.  → dict: ``keys`` (``records.DRAIN_WAVE_KEY``, in query order),
+        ``waves`` (``records.DRAIN_WAVE``, one per opened wave) and the totals of ``records.DRAIN_WAVES_TOTALS``."""
+        if (nodes is None) == (domains is None):
+            raise ValueError("give node rows or domain ids")
+        ids = np.ascontiguousarray(nodes if domains is None else domains, dtype=np.uint32)
+        keys = R.aligned_empty(max(len(ids), 1), R.DRAIN_WAVE_KEY)
+        waves = R.aligned_empty(max(int(max_waves), 1), R.DRAIN_WAVE)
+        q = R.DrainWavesQuery()
+        q.ids = R.ptr(ids) if len(ids) else None
+        q.n_ids = len(ids)
+        q.scope = R.DRAIN_NODES if domains is None else R.DRAIN_DOMAINS
+        q.max_waves = int(max_waves)
+        q.keys, q.waves = R.ptr(keys), R.ptr(waves)
+        self._check(lib().lwse_resident_drain_waves(self._h, C.byref(q)))
+        out = {"keys": keys[: len(ids)], "waves": waves[: q.n_waves]}
+        out.update({k: getattr(q, k) for k in R.DRAIN_WAVES_TOTALS})
+        return out
 
     def resident_drain_place_cost(self, scope: str = "nodes") -> np.ndarray:
         """lwse_resident_drain_place_cost: one ``records.DRAIN_PLACE_COST`` row per node (``scope="nodes"``) or per

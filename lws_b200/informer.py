@@ -614,6 +614,28 @@ class IncrementalEncoder:
         return [{field: names.get(k), **{f: int(r[f]) for f in R.DRAIN_PLACE_COST.names if f != "reserved"}}
                 for k, r in enumerate(rows)]
 
+    def drain_waves_report(self, result: dict, scope: str = "nodes") -> dict:
+        """A ``resident_drain_waves`` answer with names: ``waves``, one list per wave of the node names (scope
+        ``"nodes"``) or topology values (``"domains"``) in it, in query order, and ``unplanned``, the keys without a
+        wave as (name, status) with status ``"breaches_alone"`` or ``"no_wave"``.  A key nobody holds is named
+        None.  Nothing in the encoder changes."""
+        if scope == "nodes":
+            names = {row: name for name, row in self.node_index.items()}
+        elif scope == "domains":
+            names = {d: v for v, d in self._domain_ids.items()}
+        else:
+            raise ValueError(f"unknown scope {scope!r}")
+        status = {R.DRAINW_BREACHES_ALONE: "breaches_alone", R.DRAINW_NO_WAVE: "no_wave"}
+        waves = [[] for _ in range(len(result["waves"]))]
+        unplanned = []
+        for k in result["keys"]:
+            name = names.get(int(k["id"]))
+            if int(k["status"]) == R.DRAINW_PLANNED:
+                waves[int(k["wave"])].append(name)
+            else:
+                unplanned.append((name, status[int(k["status"])]))
+        return {"waves": waves, "unplanned": unplanned}
+
     # ------------------------------------------------------------------ results
     def tables(self):
         """(lws, groups, pod_state, pod_ident, reqs) trimmed to the rows in use (+ spare already laid out)."""

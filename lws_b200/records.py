@@ -629,6 +629,52 @@ class DrainBudgetQuery(C.Structure):
 DRAIN_BUDGET_TOTALS = ("n_touched", "n_breached", "n_loses_available", "n_already_below", "n_pods_evicted",
                        "n_leaders_evicted", "n_groups_restarted", "n_ready_restarted", "n_pods_recreated")
 
+# drain waves (lwse_resident_drain_waves): the wave cap and the status of a key
+DRAIN_WAVES_MAX = 64
+DRAINW_PLANNED = 0
+DRAINW_BREACHES_ALONE = 1
+DRAINW_NO_WAVE = 2
+
+# lwse_drain_wave_key: one key of the plan, in query order
+DRAIN_WAVE_KEY = np.dtype(
+    [("id", "<u4"), ("wave", "<u4"), ("status", "<u4"), ("groups_restarted", "<u4"), ("ready_restarted", "<u4"),
+     ("lws_touched", "<u4"), ("lws_breached", "<u4"), ("reserved", "<u4")],
+    align=False,
+)
+assert DRAIN_WAVE_KEY.itemsize == 32
+
+# lwse_drain_wave: one opened wave, the set-form totals over its ids
+DRAIN_WAVE = np.dtype(
+    [("n_keys", "<u4"), ("lws_touched", "<u4"), ("lws_loses_available", "<u4"), ("n_pods_evicted", "<u4"),
+     ("n_leaders_evicted", "<u4"), ("n_groups_restarted", "<u4"), ("n_ready_restarted", "<u4"), ("min_margin", "<i4"),
+     ("n_pods_recreated", "<u8"), ("reserved", "<u8")],
+    align=False,
+)
+assert DRAIN_WAVE.itemsize == 48
+
+
+class DrainWavesQuery(C.Structure):
+    """lwse_drain_waves_query: a first-fit plan of distinct node rows or domain ids into waves (the ids and the wave
+    cap in, the DRAIN_WAVE_KEY and DRAIN_WAVE rows and the DRAIN_WAVES_TOTALS out)."""
+
+    _fields_ = [
+        ("ids", C.c_void_p),
+        ("n_ids", C.c_uint32),
+        ("scope", C.c_uint32),
+        ("max_waves", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("keys", C.c_void_p),
+        ("waves", C.c_void_p),
+        ("n_waves", C.c_uint32),
+        ("n_planned", C.c_uint32),
+        ("n_breaches_alone", C.c_uint32),
+        ("n_no_wave", C.c_uint32),
+    ]
+
+
+# the totals of a drain waves query, as Engine.resident_drain_waves returns them
+DRAIN_WAVES_TOTALS = ("n_waves", "n_planned", "n_breaches_alone", "n_no_wave")
+
 
 # DS drain (lwse_resident_ds_drain*): the flags of a touched DS
 DSD_TOUCHED = 1 << 0
