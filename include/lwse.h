@@ -1618,6 +1618,114 @@ typedef struct lwse_ds_drain_cost {
 } lwse_ds_drain_cost;
 LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds_drain_cost* out);
 
+/* ---- DS drain waves ------------------------------------------------------------------------
+ * "Which of these nodes (domains) can I drain together and keep every inference service up?"  The first-fit plan
+ * of lwse_resident_drain_waves with a wave rule that also reads the DS verdicts of lwse_resident_ds_drain
+ * (DESIGN.md §3.5, "DS drain waves").  A child LeaderWorkerSet with replicas 1 and maxUnavailable 1 has floor 0:
+ * the LWS rule lets a wave take its only replica, and the DS that reads it stops serving.
+ *
+ * Definition.  ids, scope, max_waves, drain sets, EVALUATED, floor, ready_before and lost(L, D) are those of
+ * lwse_resident_drain_waves; TOUCHED, SERVICE_LOST, OLD_SERVICE_LOST and STALLS those of lwse_resident_ds_drain.
+ * A drain set D TRIGGERS
+ *   LWSE_DSW_LWS_FLOOR       when the set form lwse_resident_drain_budget over D has n_breached > 0;
+ *   LWSE_DSW_DS_SERVICE      when lwse_resident_ds_drain over D has n_service_lost > 0;
+ *   LWSE_DSW_DS_OLD_SERVICE  when it has n_old_service_lost > 0;
+ *   LWSE_DSW_DS_STALL        when it has n_stalled > 0.
+ * `constraints` (nonzero, known bits only) names the verdicts the plan keeps.  Keys are taken in the caller's
+ * order and key k_i gets the first of:
+ *   1. LWSE_DRAINW_BREACHES_ALONE  {k_i} triggers a verdict in constraints (wave LWSE_NONE);
+ *   2. LWSE_DRAINW_PLANNED         wave w: the smallest index of an open wave such that W_w ∪ {k_i} triggers none
+ *                                  of them; with no such wave and fewer than max_waves open, a new wave;
+ *   3. LWSE_DRAINW_NO_WAVE         neither (wave LWSE_NONE).
+ * Every wave is judged against the same baseline, as in lwse_resident_drain_waves.
+ *
+ * Exact through one cap per LWS row.  A revision-role row r that takes the LWS value of child L (the link rule of
+ * lwse_ds_link) has ready_before(r) = lws_out[L].ready_replicas and ready_after(r) = ready_before - lost(L, D), so
+ * every row linked to L moves together.  Each DS verdict is an OR over its rows, gated by the DS's flags in the
+ * before sweep (see lwse_resident_ds_drain_cost), and is monotone in D.  A gated row therefore bounds lost(L, D):
+ *   - a new-revision spec row of a DS with NEW_READY before (SERVICE), or a spec row of old revision v of a DS with
+ *     bit v of ready_revs before (OLD_SERVICE): lost(L, D) <= ready_before - 1;
+ *   - a new-revision spec row of a DS with STABLE before (STALL; only a DS mid-rollout is STABLE): lost(L, D) = 0.
+ * Removed roles, rows that fall back and rows of BAD_TABLE DS bound nothing.  With slack(L) the minimum of
+ * ready_before - floor (LWS_FLOOR in constraints and L EVALUATED), ready_before - 1 (L linked from a row whose
+ * verdict is in constraints and gated) and 0 (STALL, likewise), +inf otherwise, adding k to W is admissible iff
+ * every L to which k adds new > 0 ready member groups has lost(L, W) + new <= slack(L).  Unlike the LWS plan, the
+ * groups of L count whether or not L is EVALUATED whenever some row the DS sweep reads takes L's value: the DS
+ * verdicts read lost(L, ·) for such an L either way.  With no link patch since the DS load no row takes an LWS
+ * value and the DS constraints bind nothing.
+ *
+ * Readiness, isolation and errors: as lwse_resident_ds_drain (LWSE_ERR_NOT_READY without a ready drain budget and
+ * resident DS tables; the what-if stream behind the engine-stream and DS-stream events; scratch of its own that
+ * only grows), plus the refusals of lwse_resident_drain_waves: LWSE_ERR_INVALID_ARG for a duplicate or
+ * out-of-range id, a bad max_waves, NULL outputs, a nonzero reserved field or a zero or unknown `constraints`
+ * bit; LWSE_ERR_UNSUPPORTED with a peer exchange; LWSE_ERR_OOM when a sized scratch table refuses an entry.  A
+ * refused call writes no output.  n_ids = 0 is valid and opens no wave. */
+#define LWSE_DSW_LWS_FLOOR (1u << 0)
+#define LWSE_DSW_DS_SERVICE (1u << 1)
+#define LWSE_DSW_DS_OLD_SERVICE (1u << 2)
+#define LWSE_DSW_DS_STALL (1u << 3)
+#define LWSE_DSW_ALL (LWSE_DSW_LWS_FLOOR | LWSE_DSW_DS_SERVICE | LWSE_DSW_DS_OLD_SERVICE | LWSE_DSW_DS_STALL)
+
+/* One key of the plan, in query order (48 B).  The alone columns equal row `id` of
+ * lwse_resident_drain_budget_cost and of lwse_resident_ds_drain_cost for the same scope. */
+typedef struct lwse_ds_drain_wave_key {
+  uint32_t id;                  /* the node row or domain id                                             */
+  uint32_t wave;                /* its wave, or LWSE_NONE                                                */
+  uint32_t status;              /* LWSE_DRAINW_*                                                         */
+  uint32_t alone;               /* the LWSE_DSW_* bits {id} triggers, whatever constraints holds         */
+  uint32_t groups_restarted;    /* the key alone                                                         */
+  uint32_t ready_restarted;
+  uint32_t lws_touched;
+  uint32_t lws_breached;
+  uint32_t ds_touched;
+  uint32_t ds_service_lost;
+  uint32_t ds_old_service_lost;
+  uint32_t ds_stalled;
+} lwse_ds_drain_wave_key;
+
+/* One opened wave (80 B): the totals of lwse_resident_drain_budget and of lwse_resident_ds_drain over the wave's
+ * ids.  The counts of verdicts in constraints are 0; the others report what the wave does to a verdict the caller
+ * did not enforce. */
+typedef struct lwse_ds_drain_wave {
+  uint32_t n_keys;
+  uint32_t lws_touched;
+  uint32_t lws_breached;
+  uint32_t lws_loses_available;
+  uint32_t n_pods_evicted;
+  uint32_t n_leaders_evicted;
+  uint32_t n_groups_restarted;
+  uint32_t n_ready_restarted;
+  int32_t min_margin;           /* min over evaluated touched L of ready_after - floor; INT32_MAX for none */
+  uint32_t ds_touched;
+  uint32_t ds_service_lost;
+  uint32_t ds_old_service_lost;
+  uint32_t ds_stalled;
+  uint32_t rows_touched;
+  uint32_t rows_zeroed;
+  uint32_t reserved;
+  uint64_t n_pods_recreated;
+  uint64_t reserved2;
+} lwse_ds_drain_wave;
+
+typedef struct lwse_ds_drain_waves_query {
+  /* in */
+  const uint32_t* ids;           /* [n_ids] distinct node rows or domain ids (by scope), host memory       */
+  uint32_t n_ids;
+  uint32_t scope;                /* LWSE_DRAIN_NODES or LWSE_DRAIN_DOMAINS                                 */
+  uint32_t max_waves;            /* 1 .. LWSE_DRAIN_WAVES_MAX                                              */
+  uint32_t constraints;          /* LWSE_DSW_* (nonzero)                                                   */
+  uint32_t reserved;             /* 0                                                                      */
+  uint32_t reserved1;            /* 0                                                                      */
+  lwse_ds_drain_wave_key* keys;  /* [n_ids] out                                                            */
+  lwse_ds_drain_wave* waves;     /* [max_waves] out: rows 0 .. n_waves                                     */
+  /* out */
+  uint32_t n_waves;
+  uint32_t n_planned;
+  uint32_t n_breaches_alone;
+  uint32_t n_no_wave;
+} lwse_ds_drain_waves_query;
+LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_query* q);
+
 /* ------------------------------------------------------------------------- */
 /* Group / subgroup keys (SHA-1) and subgroup indices                        */
 /* ------------------------------------------------------------------------- */

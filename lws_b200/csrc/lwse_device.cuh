@@ -315,4 +315,17 @@ __device__ __forceinline__ LwsBudget budget_of(const lwse_lws_rec* lws, const lw
   return b;
 }
 
+// The LWS row whose ready count revision-role row `row` takes under the link rule (the DS tick's linked_ready),
+// or LWSE_NONE.  (lwse_ds_kernels.cu and lwse_ds_drain_wave_kernels.cu: the DS drain's definition in lwse.h.)
+__device__ __forceinline__ uint32_t ds_link_target(const lwse_ds_link* links, const lwse_lws_rec* lws,
+                                                   const lwse_lws_out* lws_out, uint32_t n_lws, uint32_t row, bool exists) {
+  if (!exists) return LWSE_NONE;
+  const uint4 l = ldg_stream(links + row);  // {uid lo, uid hi, lws_row, reserved}
+  if (l.z >= n_lws) return LWSE_NONE;       // (LWSE_NONE included)
+  const uint64_t uid = __ldg(reinterpret_cast<const unsigned long long*>(&lws[l.z].uid_hash));
+  if (uid != u64_of(l.x, l.y)) return LWSE_NONE;
+  constexpr uint32_t kNoUpdate = LWSE_LOUT_IRREGULAR | LWSE_LOUT_BAD_TABLE | LWSE_LOUT_RUP_ERROR | LWSE_LOUT_STATUS_ERROR;
+  return (__ldg(&lws_out[l.z].flags) & kNoUpdate) ? LWSE_NONE : l.z;
+}
+
 }  // namespace lwse

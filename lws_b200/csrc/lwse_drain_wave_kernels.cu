@@ -16,6 +16,8 @@
 //                              columns are taken back and the key's groups join the wave it took.
 //   drain_waves_finish_kernel  every dense row's waves into their lws_touched / lws_loses_available / min_margin,
 //                              and every planned key's pods and leaders into its wave.
+// The DS drain waves (lwse_resident_ds_drain_waves) run the fill, dense and plan bodies with kCapped: pairs of linked
+// rows are bound too, and each dense row carries the slack its DS caps and the caller's constraints give it.
 #include "lwse_device.cuh"
 #include "lwse_launch.cuh"
 
@@ -41,7 +43,9 @@ constexpr uint32_t kPairMember = 1u << 0;
 constexpr uint32_t kPairReady = 1u << 1;    // the group's baseline row has COND_READY
 constexpr uint32_t kPairReadyNb = 1u << 2;  // ready, and its index in the LWS row's range is below replicas
 constexpr uint32_t kPairBound = 1u << 3;    // ready, of a member group of an evaluated row: it counts against a floor
+                                            // (the DS plan: of an evaluated or a linked row)
 constexpr uint32_t kDenseEvaluated = 1u << 0, kDenseAvailable = 1u << 1;
+constexpr uint32_t kDenseCapped = 1u << 2;  // the DS plan: some constraint bounds the row, its slack in w
 
 // (pair, wave) items the plan kernel takes per pass: a key's pairs times the open waves plus one.
 constexpr uint32_t kPlanThreads = 512;
@@ -65,7 +69,10 @@ __global__ void __launch_bounds__(256) drain_waves_keys_kernel(const DrainWavesL
   if ((threadIdx.x & 31u) == 0 && pairs) atomicAdd(p.counts, pairs);
 }
 
-__global__ void __launch_bounds__(256) drain_waves_fill_kernel(const DrainWavesLaunch p) {
+// kCapped (the DS plan): a ready member pair is also bound when some revision-role row a DS sweep reads takes the
+// value of its LWS row (caps[L] has kCapLinked), evaluated or not.
+template <bool kCapped>
+__device__ __forceinline__ void drain_waves_fill(const DrainWavesLaunch& p, const uint32_t* caps) {
   for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < p.n_pairs; j += gridDim.x * blockDim.x) {
     const unsigned long long pr = __ldg(p.pairs + j);
     const uint32_t key = (uint32_t)(pr >> 32), g = (uint32_t)pr;
@@ -81,7 +88,11 @@ __global__ void __launch_bounds__(256) drain_waves_fill_kernel(const DrainWavesL
     if (member) {
       bits |= kPairMember;
       if (ready && (int64_t)index < (int64_t)(int32_t)l1.x) bits |= kPairReadyNb;
-      if (ready && budget_of(p.lws, p.lws_out, L, p.n_groups).evaluated) bits |= kPairBound;
+      if constexpr (kCapped) {
+        if (ready && ((__ldg(caps + L) & kCapLinked) || budget_of(p.lws, p.lws_out, L, p.n_groups).evaluated)) bits |= kPairBound;
+      } else {
+        if (ready && budget_of(p.lws, p.lws_out, L, p.n_groups).evaluated) bits |= kPairBound;
+      }
       p.l_count[L] = 1u;
     }
     const uint32_t at = atomicAdd(p.cursor + pos, 1u);
@@ -90,7 +101,13 @@ __global__ void __launch_bounds__(256) drain_waves_fill_kernel(const DrainWavesL
   }
 }
 
-__global__ void __launch_bounds__(256) drain_waves_dense_kernel(const DrainWavesLaunch p) {
+__global__ void __launch_bounds__(256) drain_waves_fill_kernel(const DrainWavesLaunch p) { drain_waves_fill<false>(p, nullptr); }
+
+// kCapped: the dense row's w holds the row's slack under `constraints` (lwse.h, "DS drain waves"), clamped to
+// int32, and kDenseCapped is set when some constraint bounds the row.  The clamp keeps every answer: a bound
+// counter is >= 1 where it is checked, and the minimum is at most ready_before - 1 or ready_before - floor.
+template <bool kCapped>
+__device__ __forceinline__ void drain_waves_dense(const DrainWavesLaunch& p, const uint32_t* caps, uint32_t constraints) {
   const uint32_t stride = gridDim.x * blockDim.x;
   const uint32_t n_listed = __ldcg(p.first + p.m);
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < p.n_lws || i < n_listed; i += stride) {
@@ -98,8 +115,19 @@ __global__ void __launch_bounds__(256) drain_waves_dense_kernel(const DrainWaves
       const uint32_t d = __ldcg(p.l_first + i);
       if (__ldcg(p.l_first + i + 1) != d) {
         const LwsBudget b = budget_of(p.lws, p.lws_out, i, p.n_groups);
-        p.dense[d] = make_uint4((uint32_t)b.ready_before, (uint32_t)b.floor,
-                                (b.evaluated ? kDenseEvaluated : 0u) | (b.available ? kDenseAvailable : 0u), 0u);
+        uint32_t flags = (b.evaluated ? kDenseEvaluated : 0u) | (b.available ? kDenseAvailable : 0u), slack = 0u;
+        if constexpr (kCapped) {
+          const uint32_t c = __ldg(caps + i) & constraints;
+          int64_t cap = INT64_MAX;
+          if ((constraints & LWSE_DSW_LWS_FLOOR) && b.evaluated) cap = (int64_t)b.ready_before - b.floor;
+          if (c & (LWSE_DSW_DS_SERVICE | LWSE_DSW_DS_OLD_SERVICE)) cap = min(cap, (int64_t)b.ready_before - 1);
+          if (c & LWSE_DSW_DS_STALL) cap = min(cap, (int64_t)0);
+          if (cap != INT64_MAX) {
+            flags |= kDenseCapped;
+            slack = (uint32_t)clamp_i32(cap);
+          }
+        }
+        p.dense[d] = make_uint4((uint32_t)b.ready_before, (uint32_t)b.floor, flags, slack);
       }
     }
     if (i < n_listed) {
@@ -109,9 +137,16 @@ __global__ void __launch_bounds__(256) drain_waves_dense_kernel(const DrainWaves
   }
 }
 
-__device__ __forceinline__ int64_t slack_of(const uint4 d) { return (int64_t)(int32_t)d.x - (int32_t)d.y; }
+__global__ void __launch_bounds__(256) drain_waves_dense_kernel(const DrainWavesLaunch p) { drain_waves_dense<false>(p, nullptr, 0u); }
 
-__global__ void __launch_bounds__(kPlanThreads, 1) drain_waves_plan_kernel(const DrainWavesLaunch p) {
+template <bool kCapped>
+__device__ __forceinline__ int64_t slack_of(const uint4 d) {
+  if constexpr (kCapped) return (d.z & kDenseCapped) ? (int64_t)(int32_t)d.w : INT64_MAX;
+  return (int64_t)(int32_t)d.x - (int32_t)d.y;
+}
+
+template <bool kCapped>
+__device__ __forceinline__ void drain_waves_plan(const DrainWavesLaunch& p) {
   __shared__ unsigned long long s_bad, s_recreated[LWSE_DRAIN_WAVES_MAX];
   __shared__ uint32_t s_groups[LWSE_DRAIN_WAVES_MAX], s_ready[LWSE_DRAIN_WAVES_MAX], s_keys[LWSE_DRAIN_WAVES_MAX];
   __shared__ uint32_t s_alone_bad, s_touched, s_breached, s_wave, s_open, s_status[3];
@@ -145,7 +180,7 @@ __global__ void __launch_bounds__(kPlanThreads, 1) drain_waves_plan_kernel(const
       const uint4 r = __ldg(p.recs + b + j / cols);
       const uint32_t w = j % cols;
       if (!(r.z & kPairBound) || !(w == n_open || !((__ldcg(p.g_waves + r.x) >> w) & 1ull))) continue;
-      if ((int64_t)__ldcg(p.lost + (size_t)r.y * p.cols + w) <= slack_of(__ldg(p.dense + r.y))) continue;
+      if ((int64_t)__ldcg(p.lost + (size_t)r.y * p.cols + w) <= slack_of<kCapped>(__ldg(p.dense + r.y))) continue;
       if (w < n_open) {
         atomicOr(&s_bad, 1ull << w);
       } else {
@@ -219,6 +254,8 @@ __global__ void __launch_bounds__(kPlanThreads, 1) drain_waves_plan_kernel(const
                                                   s_status[LWSE_DRAINW_NO_WAVE]);
 }
 
+__global__ void __launch_bounds__(kPlanThreads, 1) drain_waves_plan_kernel(const DrainWavesLaunch p) { drain_waves_plan<false>(p); }
+
 __global__ void __launch_bounds__(256) drain_waves_finish_kernel(const DrainWavesLaunch p) {
   lwse_drain_wave* waves = reinterpret_cast<lwse_drain_wave*>(p.out + 16 + (size_t)p.m * sizeof(lwse_drain_wave_key));
   const uint32_t stride = gridDim.x * blockDim.x;
@@ -246,6 +283,36 @@ __global__ void __launch_bounds__(256) drain_waves_finish_kernel(const DrainWave
       atomicAdd(&waves[w].n_leaders_evicted, __ldg(&c->leaders));
     }
   }
+}
+
+__global__ void __launch_bounds__(256) drain_waves_fill_capped_kernel(const DrainWavesLaunch p, const uint32_t* caps) {
+  drain_waves_fill<true>(p, caps);
+}
+
+__global__ void __launch_bounds__(256) drain_waves_dense_capped_kernel(const DrainWavesLaunch p, const uint32_t* caps,
+                                                                       uint32_t constraints) {
+  drain_waves_dense<true>(p, caps, constraints);
+}
+
+__global__ void __launch_bounds__(kPlanThreads, 1) drain_waves_plan_capped_kernel(const DrainWavesLaunch p) {
+  drain_waves_plan<true>(p);
+}
+
+int launch_drain_waves_capped(const DrainWavesLaunch* p, const uint32_t* caps, uint32_t constraints, int pass, int sm_count,
+                              cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  if (pass == 1) {
+    drain_waves_fill_capped_kernel<<<grid_for(p->n_pairs, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p, caps);
+    if (launched_or_fail(1, cuda_err) < 0) return -1;
+    if (launch_index_scan(p->l_count, p->l_first, p->l_cursor, p->n_lws, s, cuda_err) < 0) return -1;
+    const uint64_t n = p->n_lws > p->n_pairs ? p->n_lws : p->n_pairs;
+    drain_waves_dense_capped_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p, caps, constraints);
+    return launched_or_fail(3, cuda_err);
+  }
+  drain_waves_plan_capped_kernel<<<1, kPlanThreads, 0, s>>>(*p);
+  const uint32_t n = p->n_dense > p->m ? p->n_dense : p->m;
+  drain_waves_finish_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(*p);
+  return launched_or_fail(2, cuda_err);
 }
 
 int launch_drain_waves(const DrainWavesLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err) {

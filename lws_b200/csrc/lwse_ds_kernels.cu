@@ -749,13 +749,7 @@ static unsigned ds_grid(uint32_t n_ds, int sm_count) {
 
 // The LWS row whose ready count revision-role row `row` takes under the link rule (linked_ready), or LWSE_NONE.
 __device__ __forceinline__ uint32_t ds_drain_link_of(const DsDrainLink& lk, uint32_t row, bool exists) {
-  if (!exists) return LWSE_NONE;
-  const uint4 l = ldg_stream(lk.links + row);  // {uid lo, uid hi, lws_row, reserved}
-  if (l.z >= lk.n_lws) return LWSE_NONE;       // (LWSE_NONE included)
-  const uint64_t uid = __ldg(reinterpret_cast<const unsigned long long*>(&lk.lws[l.z].uid_hash));
-  if (uid != u64_of(l.x, l.y)) return LWSE_NONE;
-  constexpr uint32_t kNoUpdate = LWSE_LOUT_IRREGULAR | LWSE_LOUT_BAD_TABLE | LWSE_LOUT_RUP_ERROR | LWSE_LOUT_STATUS_ERROR;
-  return (__ldg(&lk.lws_out[l.z].flags) & kNoUpdate) ? LWSE_NONE : l.z;
+  return ds_link_target(lk.links, lk.lws, lk.lws_out, lk.n_lws, row, exists);
 }
 
 __device__ __forceinline__ bool u4_ne(const uint4 a, const uint4 b) { return a.x != b.x || a.y != b.y || a.z != b.z || a.w != b.w; }

@@ -245,6 +245,9 @@ struct lwse_engine {
   DevBuf dv_cost, dv_words, dv_ids, dv_pos, dv_kidx, dv_pairs, dv_recs, dv_lidx, dv_dense, dv_lost, dv_gwaves, dv_rwaves,
       dv_stamps, dv_out;
   PinBuf dv_host;
+  // DS drain waves (lwse_resident_ds_drain_waves): the per-LWS-row caps and the answer; the rest is the drain
+  // waves' and the DS drain's scratch
+  DevBuf dx_caps, dx_out;
   // DS drain (lwse_resident_ds_drain*): lost[L] and the after copy of lws_out, the before / after sweep outputs, the
   // touched DS rows, the reverse link index (count | first | cursor) and its entries, the key rows, the (DS, key) table
   DevBuf dd_lost, dd_lws_after, dd_out[2], dd_role_out[2], dd_revrole_out[2], dd_rows, dd_index, dd_entries, dd_cost, dd_table;
@@ -485,7 +488,7 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->dw_sums, &e->dw_ds, &e->dw_roles, &e->dw_revroles, &e->dw_links, &e->dw_now, &e->dw_role_out,
                       &e->dw_revrole_out, &e->dv_cost, &e->dv_words, &e->dv_ids, &e->dv_pos, &e->dv_kidx, &e->dv_pairs,
                       &e->dv_recs, &e->dv_lidx, &e->dv_dense, &e->dv_lost, &e->dv_gwaves, &e->dv_rwaves, &e->dv_stamps,
-                      &e->dv_out};
+                      &e->dv_out, &e->dx_caps, &e->dx_out};
     if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
     if (e->lf_stream) cudaStreamSynchronize(e->lf_stream);
     if (e->wf_stream) cudaStreamSynchronize(e->wf_stream);
@@ -3372,6 +3375,243 @@ LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds
   LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 64, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   if (words[10]) return LWSE_ERR_OOM;  // an insert the (DS, key) table refused: no answer rather than a wrong one
+  return LWSE_OK;
+}
+
+// ---------------------------------------------------------------------------
+// DS drain waves
+// ---------------------------------------------------------------------------
+// The DS drain's before sweep, the drain waves chain with the DS caps, and the per-key forms of the drain budget
+// and the DS drain (their key rows give the alone columns), sharing the drain budget's pass 0 and one (LWS, key)
+// table.  Three host synchronisations, each sizing what follows: the pairs and the reverse link index entries, then
+// the touched LWS rows and the (DS, key) pairs, then the answer.  Words of dv_words: [0..15] the budget walk's
+// counters, [16..19] the drain waves' (u64), [20..22] the DS per-key form's, [24..25] the index entries (u64).
+LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_query* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!ds_drain_ready(e)) return LWSE_ERR_NOT_READY;
+  if (q->scope != LWSE_DRAIN_NODES && q->scope != LWSE_DRAIN_DOMAINS) return LWSE_ERR_INVALID_ARG;
+  if (q->reserved || q->reserved1 || q->max_waves == 0 || q->max_waves > LWSE_DRAIN_WAVES_MAX || !q->waves)
+    return LWSE_ERR_INVALID_ARG;
+  if (q->constraints == 0 || (q->constraints & ~LWSE_DSW_ALL)) return LWSE_ERR_INVALID_ARG;
+  if (q->n_ids && (!q->ids || !q->keys)) return LWSE_ERR_INVALID_ARG;
+  const bool by_domain = q->scope == LWSE_DRAIN_DOMAINS;
+  const uint32_t nn = e->n_nodes, nk = by_domain ? e->n_domains : nn, m = q->n_ids;
+  const uint32_t nl = e->rn_lws, ng = e->rn_groups;
+  LWSE_CUDA(e, e->wf_stage.reserve((size_t)nk + 16));
+  uint8_t* seen = static_cast<uint8_t*>(e->wf_stage.h);
+  memset(seen, 0, nk);
+  for (uint32_t i = 0; i < m; i++) {
+    const uint32_t id = q->ids[i];
+    if (id >= nk || seen[id]) return LWSE_ERR_INVALID_ARG;  // out of range, or a duplicate
+    seen[id] = 1;
+  }
+  if (e->xch_world > 0) return LWSE_ERR_UNSUPPORTED;  // (a plan is not a sum over ranks)
+  const uint32_t mw = q->max_waves;
+  const size_t plan_bytes = 16 + (size_t)m * sizeof(lwse_drain_wave_key) + (size_t)mw * sizeof(lwse_drain_wave);
+  const size_t keys_bytes = (size_t)m * sizeof(lwse_ds_drain_wave_key);
+  const size_t out_bytes = 16 + keys_bytes + (size_t)mw * sizeof(lwse_ds_drain_wave);
+  const size_t host_bytes = out_bytes > (size_t)m * 4 ? out_bytes : (size_t)m * 4;
+  DeviceGuard guard(e->device);
+  if (const int rc = reserve_ds_drain_outputs(e, 1); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, e->dr_bcost.reserve((size_t)nk * sizeof(lwse_drain_budget_cost) + 16));
+  LWSE_CUDA(e, e->dd_cost.reserve((size_t)nk * sizeof(lwse_ds_drain_cost) + 16));
+  LWSE_CUDA(e, e->dd_index.reserve((size_t)(nl + 1) * 3 * 4 + 16));
+  LWSE_CUDA(e, e->dv_words.reserve(128));
+  LWSE_CUDA(e, e->wf_words.reserve(192));
+  LWSE_CUDA(e, e->dv_ids.reserve((size_t)m * 4 + 16));
+  LWSE_CUDA(e, e->dv_pos.reserve((size_t)nk * 4 + 16));
+  LWSE_CUDA(e, e->dv_kidx.reserve(((size_t)m * 3 + 2) * 4 + 16));
+  LWSE_CUDA(e, e->dv_lidx.reserve(((size_t)nl * 3 + 2) * 4 + 16));
+  LWSE_CUDA(e, e->dv_dense.reserve((size_t)nl * 16 + 16));
+  LWSE_CUDA(e, e->dv_gwaves.reserve((size_t)ng * 8 + 16));
+  LWSE_CUDA(e, e->dv_out.reserve(plan_bytes));
+  LWSE_CUDA(e, e->dx_caps.reserve((size_t)nl * 4 + 16));
+  LWSE_CUDA(e, e->dx_out.reserve(out_bytes));
+  LWSE_CUDA(e, e->dv_host.reserve(host_bytes));
+  if (const int rc = ds_drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* d_words = (uint32_t*)e->dv_words.p;
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  uint32_t* d_count = (uint32_t*)e->dd_index.p;  // the reverse link index (count | first | cursor)
+  uint32_t* d_first = d_count + (nl + 1);
+  uint32_t* d_cursor = d_first + (nl + 1);
+  if (m) {
+    memcpy(e->dv_host.h, q->ids, (size_t)m * 4);
+    LWSE_CUDA(e, cudaMemcpyAsync(e->dv_ids.p, e->dv_host.h, (size_t)m * 4, cudaMemcpyHostToDevice, s));
+  }
+  LWSE_CUDA(e, cudaMemsetAsync(e->dr_bcost.p, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dd_cost.p, 0, (size_t)nk * sizeof(lwse_ds_drain_cost), s));
+  LWSE_CUDA(e, cudaMemsetAsync(d_words, 0, 128, s));
+  LWSE_CUDA(e, cudaMemsetAsync(d_count, 0, (size_t)(nl + 1) * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_pos.p, 0xFF, (size_t)nk * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_kidx.p, 0, (size_t)m * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lidx.p, 0, (size_t)nl * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_gwaves.p, 0, (size_t)ng * 8, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_out.p, 0, plan_bytes, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dx_caps.p, 0, (size_t)nl * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dx_out.p, 0, out_bytes, s));
+  // the before sweep (its ds_out gates the verdicts), the reverse link index's counts, the caps
+  if (const int rc = enqueue_ds_drain_sweep(e, 0, (const lwse_lws_out*)e->r_lws_out.p); rc != LWSE_OK) return rc;
+  lwse::DsDrainWavesLaunch d{};
+  d.t = ds_drain_tables(e, 0);
+  d.lk = ds_drain_link(e);
+  d.caps = (uint32_t*)e->dx_caps.p;
+  d.ds_cost = (const lwse_ds_drain_cost*)e->dd_cost.p;
+  d.out = (uint8_t*)e->dx_out.p;
+  d.max_waves = mw;
+  int cuda_err = 0;
+  int launched = lwse::launch_ds_drain_links(&d.t, &d.lk, d_count, d_cursor, nullptr, 0, (unsigned long long*)(d_words + 24),
+                                             false, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  launched = lwse::launch_index_scan(d_count, d_first, d_cursor, nl, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  launched = lwse::launch_ds_drain_waves(&d, nullptr, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  // the key rows, the member-pair count and the pair count: the drain budget's pass 0, then the key positions
+  lwse::DrainBudgetCostLaunch bp{};
+  bp.lws = (const lwse_lws_rec*)e->r_lws.p;
+  bp.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
+  bp.groups = (const lwse_group_rec*)e->r_groups.p;
+  bp.pod_state = (const uint8_t*)e->r_pst.p;
+  bp.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
+  bp.baseline = (const lwse_group_out*)e->r_group_out.p;
+  bp.nodes = (const lwse_node_rec*)e->nodes.p;
+  bp.occupancy = (const uint32_t*)e->r_occ.p;
+  bp.cost = (lwse_drain_budget_cost*)e->dr_bcost.p;
+  bp.counts = d_words;
+  bp.n_pods = e->rn_pods;
+  bp.n_lws = nl;
+  bp.n_groups = ng;
+  bp.n_nodes = nn;
+  bp.n_domains = e->n_domains;
+  bp.n_keys = nk;
+  bp.by_domain = by_domain;
+  launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  lwse::DrainWavesLaunch p{};
+  p.lws = bp.lws;
+  p.lws_out = bp.lws_out;
+  p.groups = bp.groups;
+  p.baseline = bp.baseline;
+  p.cost = bp.cost;
+  p.ids = (const uint32_t*)e->dv_ids.p;
+  p.pos_of = (uint32_t*)e->dv_pos.p;
+  p.count = (uint32_t*)e->dv_kidx.p;
+  p.first = p.count + m;
+  p.cursor = p.first + m + 1;
+  p.l_count = (uint32_t*)e->dv_lidx.p;
+  p.l_first = p.l_count + nl;
+  p.l_cursor = p.l_first + nl + 1;
+  p.dense = (uint4*)e->dv_dense.p;
+  p.g_waves = (unsigned long long*)e->dv_gwaves.p;
+  p.out = (uint8_t*)e->dv_out.p;
+  p.counts = reinterpret_cast<unsigned long long*>(d_words + 16);
+  p.n_lws = nl;
+  p.n_groups = ng;
+  p.n_keys = nk;
+  p.m = m;
+  p.max_waves = mw;
+  p.cols = (m < mw ? m : mw) + 1u;
+  launched = lwse::launch_drain_waves(&p, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 128, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  uint64_t member_pairs = 0, n_pairs = 0, n_entries = 0;
+  memcpy(&member_pairs, words, 8);
+  memcpy(&n_pairs, words + 16, 8);
+  memcpy(&n_entries, words + 24, 8);
+  // (every index is 32-bit, and the plan kernel's items are a key's pairs times the columns)
+  if (n_pairs > 0xFFFFFFFFull / (LWSE_DRAIN_WAVES_MAX + 1u)) return LWSE_ERR_OOM;
+  if (member_pairs > (1ull << 30) || n_entries > (1ull << 30)) return LWSE_ERR_OOM;
+  LWSE_CUDA(e, e->dv_pairs.reserve((size_t)n_pairs * 8 + 16));
+  LWSE_CUDA(e, e->dv_recs.reserve((size_t)n_pairs * 16 + 16));
+  LWSE_CUDA(e, e->dd_entries.reserve((size_t)n_entries * sizeof(uint4) + 16));
+  uint64_t slots = 256;
+  while (slots < 2 * member_pairs) slots <<= 1;
+  if (member_pairs) LWSE_CUDA(e, e->dr_table.reserve((size_t)slots * (sizeof(unsigned long long) + sizeof(uint4))));
+  launched = lwse::launch_ds_drain_links(&d.t, &d.lk, d_count, d_cursor, (uint4*)e->dd_entries.p, (uint32_t)n_entries, nullptr,
+                                         true, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dv_pairs.p, (uint32_t)n_pairs, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  p.pairs = (const unsigned long long*)e->dv_pairs.p;
+  p.n_pairs = (uint32_t)n_pairs;
+  p.recs = (uint4*)e->dv_recs.p;
+  launched = lwse::launch_drain_waves_capped(&p, d.caps, q->constraints, 1, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  // the per-key forms: the (LWS, key) table with the budget columns, then the (row, key) pair count
+  lwse::DsDrainCostLaunch c{};
+  c.first = d_first;
+  c.before = d.t.ds_out;
+  c.cost = (lwse_ds_drain_cost*)e->dd_cost.p;
+  c.counts = d_words + 20;
+  c.entries = (const uint4*)e->dd_entries.p;
+  if (member_pairs) {
+    bp.keys = (unsigned long long*)e->dr_table.p;
+    bp.vals = reinterpret_cast<uint4*>(bp.keys + slots);
+    bp.table_mask = (uint32_t)(slots - 1);
+    LWSE_CUDA(e, cudaMemsetAsync(bp.keys, 0xFF, (size_t)slots * sizeof(unsigned long long), s));
+    LWSE_CUDA(e, cudaMemsetAsync(bp.vals, 0, (size_t)slots * sizeof(uint4), s));
+    launched = lwse::launch_drain_budget_cost(&bp, 1, e->sm_count, s, &cuda_err);
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    c.lws_keys = bp.keys;
+    c.lws_vals = bp.vals;
+    c.lws_mask = bp.table_mask;
+    launched = lwse::launch_ds_drain_cost(&c, 0, e->sm_count, s, &cuda_err);
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  }
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 128, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 32, p.l_first + nl, 4, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  // (the walk found another pair count, or a bucket or the (LWS, key) table refused a pair: no answer rather than
+  // a wrong one)
+  if (ng && words[8] != n_pairs) return LWSE_ERR_OOM;
+  if (words[18] || words[19] || words[2]) return LWSE_ERR_OOM;
+  const uint32_t n_dense = words[32];
+  uint64_t ds_pairs = 0;
+  memcpy(&ds_pairs, words + 20, 8);
+  if (ds_pairs) {
+    if (ds_pairs > (1ull << 30)) return LWSE_ERR_OOM;
+    uint64_t ds_slots = 256;
+    while (ds_slots < 2 * ds_pairs) ds_slots <<= 1;
+    LWSE_CUDA(e, e->dd_table.reserve((size_t)ds_slots * (sizeof(unsigned long long) + sizeof(uint2))));
+    c.keys = (unsigned long long*)e->dd_table.p;
+    c.vals = reinterpret_cast<uint2*>(c.keys + ds_slots);
+    c.table_mask = (uint32_t)(ds_slots - 1);
+    LWSE_CUDA(e, cudaMemsetAsync(c.keys, 0xFF, (size_t)ds_slots * sizeof(unsigned long long), s));
+    LWSE_CUDA(e, cudaMemsetAsync(c.vals, 0, (size_t)ds_slots * sizeof(uint2), s));
+    launched = lwse::launch_ds_drain_cost(&c, 1, e->sm_count, s, &cuda_err);
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  }
+  LWSE_CUDA(e, e->dv_lost.reserve((size_t)n_dense * p.cols * 4 + 16));
+  LWSE_CUDA(e, e->dv_rwaves.reserve((size_t)n_dense * 16 + 16));
+  LWSE_CUDA(e, e->dv_stamps.reserve((size_t)n_dense * 8 + 16));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lost.p, 0, (size_t)n_dense * p.cols * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_rwaves.p, 0, (size_t)n_dense * 16, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_stamps.p, 0, (size_t)n_dense * 8, s));
+  p.n_dense = n_dense;
+  p.lost = (uint32_t*)e->dv_lost.p;
+  p.row_waves = (unsigned long long*)e->dv_rwaves.p;
+  p.stamps = (uint32_t*)e->dv_stamps.p;
+  launched = lwse::launch_drain_waves_capped(&p, d.caps, q->constraints, 2, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  launched = lwse::launch_ds_drain_waves(&d, &p, 1, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(e->dv_host.h, d.out, out_bytes, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_words + 20, 12, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  if (words[2]) return LWSE_ERR_OOM;  // an insert the (DS, key) table refused
+  const uint8_t* h = static_cast<const uint8_t*>(e->dv_host.h);
+  uint32_t totals[4];
+  memcpy(totals, h, 16);
+  if (m) memcpy(q->keys, h + 16, keys_bytes);
+  memcpy(q->waves, h + 16 + keys_bytes, (size_t)totals[0] * sizeof(lwse_ds_drain_wave));
+  q->n_waves = totals[0];
+  q->n_planned = totals[1];
+  q->n_breaches_alone = totals[2];
+  q->n_no_wave = totals[3];
   return LWSE_OK;
 }
 

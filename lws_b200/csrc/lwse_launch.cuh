@@ -418,6 +418,30 @@ struct DrainWavesLaunch {
 // Pass 1 (pairs written): the buckets filled, the touched rows scanned, the dense rows.  Pass 2 (n_dense, lost and
 // the wave masks sized): the plan, then the wave rows' per-row columns and pods / leaders.
 int launch_drain_waves(const DrainWavesLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
+// lwse_resident_ds_drain_waves: passes 1 and 2 of launch_drain_waves with the DS caps.  caps[n_lws] (device) holds
+// per LWS row kCapLinked and the LWSE_DSW_DS_* bits of the gated rows linked to it (ds_drain_waves_caps).  Pass 1
+// binds the ready member pairs of evaluated or linked rows and writes each dense row's slack under `constraints`;
+// pass 2 runs the plan against those slacks, then the wave rows' per-row columns.
+constexpr uint32_t kCapLinked = 1u << 4;
+int launch_drain_waves_capped(const DrainWavesLaunch* p, const uint32_t* caps, uint32_t constraints, int pass, int sm_count,
+                              cudaStream_t s, int* cuda_err);
+
+// ---- lwse_ds_drain_wave_kernels.cu ----
+// lwse_resident_ds_drain_waves, around the drain waves chain.  Pass 0 (after the before sweep into t's outputs):
+// caps[L] |= the bits of every row the sweep reads that takes L's value (caps zeroed by the caller).  Pass 1 (after
+// launch_drain_waves_capped pass 2 and the DS per-key form): the answer in `out` — the query totals (16 B), m
+// lwse_ds_drain_wave_key rows, max_waves lwse_ds_drain_wave rows (zeroed by the caller) — from the plan's rows in
+// w.out, the key rows of both per-key forms, each dense row's lost groups per wave and each DS's linked rows.
+struct DsDrainWavesLaunch {
+  lwse_ds_tables t;                   // the resident DS tables, ds_out = the before sweep
+  DsDrainLink lk;
+  uint32_t* caps;                     // [n_lws]
+  const lwse_ds_drain_cost* ds_cost;  // the DS per-key form's rows of every key
+  uint8_t* out;
+  uint32_t max_waves;
+};
+int launch_ds_drain_waves(const DsDrainWavesLaunch* d, const DrainWavesLaunch* w, int pass, int sm_count, cudaStream_t s,
+                          int* cuda_err);
 
 // ---- lwse_sha1_kernels.cu ----
 int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,

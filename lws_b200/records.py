@@ -728,6 +728,63 @@ class DsDrainQuery(C.Structure):
 DS_DRAIN_TOTALS = ("n_touched", "n_service_lost", "n_old_service_lost", "n_stalled", "n_changed", "rows_touched",
                    "rows_zeroed", "rows_linked")
 
+# DS drain waves (lwse_resident_ds_drain_waves): the verdicts a plan keeps (`constraints`) and a key triggers alone
+DSW_LWS_FLOOR = 1 << 0
+DSW_DS_SERVICE = 1 << 1
+DSW_DS_OLD_SERVICE = 1 << 2
+DSW_DS_STALL = 1 << 3
+DSW_ALL = DSW_LWS_FLOOR | DSW_DS_SERVICE | DSW_DS_OLD_SERVICE | DSW_DS_STALL
+DSW_NAMES = {DSW_LWS_FLOOR: "lws_floor", DSW_DS_SERVICE: "ds_service", DSW_DS_OLD_SERVICE: "ds_old_service",
+             DSW_DS_STALL: "ds_stall"}
+
+# lwse_ds_drain_wave_key: one key of the plan, in query order
+DS_DRAIN_WAVE_KEY = np.dtype(
+    [("id", "<u4"), ("wave", "<u4"), ("status", "<u4"), ("alone", "<u4"), ("groups_restarted", "<u4"),
+     ("ready_restarted", "<u4"), ("lws_touched", "<u4"), ("lws_breached", "<u4"), ("ds_touched", "<u4"),
+     ("ds_service_lost", "<u4"), ("ds_old_service_lost", "<u4"), ("ds_stalled", "<u4")],
+    align=False,
+)
+assert DS_DRAIN_WAVE_KEY.itemsize == 48
+
+# lwse_ds_drain_wave: one opened wave, the set-form totals of the drain budget and the DS drain over its ids
+DS_DRAIN_WAVE = np.dtype(
+    [("n_keys", "<u4"), ("lws_touched", "<u4"), ("lws_breached", "<u4"), ("lws_loses_available", "<u4"),
+     ("n_pods_evicted", "<u4"), ("n_leaders_evicted", "<u4"), ("n_groups_restarted", "<u4"),
+     ("n_ready_restarted", "<u4"), ("min_margin", "<i4"), ("ds_touched", "<u4"), ("ds_service_lost", "<u4"),
+     ("ds_old_service_lost", "<u4"), ("ds_stalled", "<u4"), ("rows_touched", "<u4"), ("rows_zeroed", "<u4"),
+     ("reserved", "<u4"), ("n_pods_recreated", "<u8"), ("reserved2", "<u8")],
+    align=False,
+)
+assert DS_DRAIN_WAVE.itemsize == 80
+
+
+class DsDrainWavesQuery(C.Structure):
+    """lwse_ds_drain_waves_query: a first-fit plan of distinct node rows or domain ids into waves that keep the
+    verdicts named in ``constraints`` (the ids, the cap and the DSW_* mask in, the DS_DRAIN_WAVE_KEY and
+    DS_DRAIN_WAVE rows and the DS_DRAIN_WAVES_TOTALS out)."""
+
+    _fields_ = [
+        ("ids", C.c_void_p),
+        ("n_ids", C.c_uint32),
+        ("scope", C.c_uint32),
+        ("max_waves", C.c_uint32),
+        ("constraints", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("reserved1", C.c_uint32),
+        ("keys", C.c_void_p),
+        ("waves", C.c_void_p),
+        ("n_waves", C.c_uint32),
+        ("n_planned", C.c_uint32),
+        ("n_breaches_alone", C.c_uint32),
+        ("n_no_wave", C.c_uint32),
+    ]
+
+
+assert C.sizeof(DsDrainWavesQuery) == 64
+
+# the totals of a DS drain waves query, as Engine.resident_ds_drain_waves returns them
+DS_DRAIN_WAVES_TOTALS = ("n_waves", "n_planned", "n_breaches_alone", "n_no_wave")
+
 
 class Config(C.Structure):
     _fields_ = [
