@@ -225,6 +225,13 @@ func (e *Engine) DsDrainWaves(q *C.lwse_ds_drain_waves_query) error {
 	return e.check(C.lwse_resident_ds_drain_waves(e.h, q))
 }
 
+// DrainPlaceWaves packs distinct node rows or domain ids, in the order given, first-fit into at most q.max_waves
+// waves whose drain triggers none of the verdicts in q.constraints (LWSE_DPW_*): no LeaderWorkerSet below its
+// floor, no unpinned request left without a new exclusive domain, and (opt-in) no other request losing its domain.
+func (e *Engine) DrainPlaceWaves(q *C.lwse_drain_place_waves_query) error {
+	return e.check(C.lwse_resident_drain_place_waves(e.h, q))
+}
+
 // GroupKeys computes SHA-1 digests (20 bytes each) of n strings laid out CSR-style.
 func (e *Engine) GroupKeys(bytes *C.uint8_t, offsets *C.uint32_t, n uint32, digests *C.uint8_t) error {
 	return e.check(C.lwse_group_keys_host(e.h, bytes, offsets, C.uint32_t(n), digests))

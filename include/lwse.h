@@ -1126,6 +1126,116 @@ typedef struct lwse_drain_place_cost {
 } lwse_drain_place_cost;
 LWSE_API int lwse_resident_drain_place_cost(lwse_engine* e, uint32_t scope, lwse_drain_place_cost* out);
 
+/* ---- drain placement waves ----------------------------------------------------------------------
+ * "Which of these nodes (domains) can I drain together so that every group the drain restarts finds a new
+ * exclusive domain?"  The first-fit plan of lwse_resident_drain_waves with a wave rule that also reads the
+ * set-form drain placement (DESIGN.md §3.5, "Drain placement waves").
+ *
+ * Definition.  ids, scope, max_waves, drain sets, EVALUATED, floor and lost(L, D) are those of
+ * lwse_resident_drain_waves.  For a drain set S with node set N_S (the union of its keys' node sets) the
+ * placement verdicts come from the set-form composition that lwse_resident_drain_place_cost states for one
+ * key, applied to N_S: the groups lwse_resident_drain_whatif(N_S) restarts; U_S, the pinned request rows whose
+ * leader is on N_S or whose `group` field names a restarted group; the placement what-if round with N_S
+ * cordoned and U_S unpinned, diffed against the baseline placement rows.  Occupancy does not move, so the
+ * answer is conservative, exactly as the per-key call is.  S TRIGGERS
+ *   LWSE_DPW_LWS_FLOOR  when the set form lwse_resident_drain_budget over S has n_breached > 0;
+ *   LWSE_DPW_STRANDED   when some row of U_S is not PLACED after;
+ *   LWSE_DPW_BUMPED     when some row outside U_S is PLACED before and not after.
+ * `constraints` (nonzero, known bits only) names the verdicts the plan keeps.  Keys are taken in the caller's
+ * order and key k_i gets the first of:
+ *   1. LWSE_DRAINW_BREACHES_ALONE  {k_i} triggers a verdict in constraints (wave LWSE_NONE);
+ *   2. LWSE_DRAINW_PLANNED         wave w: the smallest index of an open wave such that W_w ∪ {k_i} triggers none
+ *                                  of them; with no such wave and fewer than max_waves open, a new wave;
+ *   3. LWSE_DRAINW_NO_WAVE         neither (wave LWSE_NONE).
+ * Every wave is judged against the same baseline: the most recently submitted sweep and placement tick.
+ *
+ * The placement verdicts are NOT monotone in the set: draining more can unpin a pinned holder and free its
+ * domain for a request another key stranded.  So a key that triggers alone is BREACHES_ALONE by definition even
+ * when some wave would accept it, and the answer is the literal sequential first-fit, never a shortcut through
+ * monotonicity.  Every returned wave's final key set was itself a probe (the probe of its last key), so every
+ * wave is verified as a set: its row's placement counts are that probe's.
+ *
+ * Locality.  Per probe S = W ∪ {k} the call solves only the namespaces (a) holding a row of U_S, or (b) with a
+ * baseline row that is not pinned and is PLACED in a domain d that S touches where S holds d as a domain key, or
+ * the row's chosen node is in N_S, or dom_free[d] - sum of free[n] over the usable n in N_S ∩ d < size.  Every
+ * other row keeps its baseline row.
+ *
+ * Readiness, isolation and errors: LWSE_ERR_NOT_READY when lwse_resident_drain_waves or
+ * lwse_resident_drain_place_cost would answer it; LWSE_ERR_INVALID_ARG for a duplicate or out-of-range id, a
+ * bad max_waves, NULL outputs, a nonzero reserved field, or a zero or unknown `constraints` bit;
+ * LWSE_ERR_UNSUPPORTED with a peer exchange, at 2^24 resident requests or where the namespace form does not fit
+ * the domains; LWSE_ERR_OOM when a sized scratch table refuses an entry.  A refused call writes no output.
+ * Isolation as the other drain queries (the engine mutex, the what-if stream behind the snapshot event, scratch
+ * that only grows, nothing of the tick touched).  n_ids = 0 is valid and opens no wave. */
+#define LWSE_DPW_LWS_FLOOR (1u << 0)
+#define LWSE_DPW_STRANDED (1u << 1)
+#define LWSE_DPW_BUMPED (1u << 2)
+#define LWSE_DPW_ALL (LWSE_DPW_LWS_FLOOR | LWSE_DPW_STRANDED | LWSE_DPW_BUMPED)
+
+/* One key of the plan, in query order (48 B).  The floor alone columns equal row `id` of
+ * lwse_resident_drain_budget_cost, the placement alone columns row `id` of lwse_resident_drain_place_cost. */
+typedef struct lwse_drain_place_wave_key {
+  uint32_t id;                /* the node row or domain id                                               */
+  uint32_t wave;              /* its wave, or LWSE_NONE                                                  */
+  uint32_t status;            /* LWSE_DRAINW_*                                                           */
+  uint32_t alone;             /* the LWSE_DPW_* bits {id} triggers, whatever constraints holds           */
+  uint32_t groups_restarted;  /* the key alone                                                           */
+  uint32_t ready_restarted;
+  uint32_t lws_touched;
+  uint32_t lws_breached;
+  uint32_t unpinned;          /* |U_k|                                                                   */
+  uint32_t stranded;
+  uint32_t bumped;
+  uint32_t reserved;
+} lwse_drain_place_wave_key;
+
+/* One opened wave (96 B): the totals of lwse_resident_drain_budget and of the set-form drain placement over the
+ * wave's ids.  The counts of verdicts in constraints are 0; the others report what the wave does to a verdict
+ * the caller did not enforce. */
+typedef struct lwse_drain_place_wave {
+  uint32_t n_keys;
+  uint32_t lws_touched;
+  uint32_t lws_loses_available;
+  uint32_t n_pods_evicted;
+  uint32_t n_leaders_evicted;
+  uint32_t n_groups_restarted;
+  uint32_t n_ready_restarted;
+  int32_t min_margin;         /* min over evaluated touched L of ready_after - floor; INT32_MAX for none */
+  uint64_t n_pods_recreated;
+  uint32_t lws_breached;
+  uint32_t unpinned;          /* |U_S|                                                                   */
+  uint32_t stranded;
+  uint32_t bumped;
+  uint32_t n_changed;         /* the lwse_place_whatif counters of the set-form composition              */
+  uint32_t n_lost;
+  uint32_t n_moved;
+  uint32_t n_gained;
+  uint32_t n_placed;
+  uint32_t n_unschedulable;
+  uint32_t n_conflict;
+  uint32_t namespaces_solved; /* namespaces the wave's final probe solved                                */
+  uint32_t reserved[2];
+} lwse_drain_place_wave;
+
+typedef struct lwse_drain_place_waves_query {
+  /* in */
+  const uint32_t* ids;              /* [n_ids] distinct node rows or domain ids (by scope), host memory    */
+  uint32_t n_ids;
+  uint32_t scope;                   /* LWSE_DRAIN_NODES or LWSE_DRAIN_DOMAINS                              */
+  uint32_t max_waves;               /* 1 .. LWSE_DRAIN_WAVES_MAX                                           */
+  uint32_t constraints;             /* LWSE_DPW_* (nonzero)                                                */
+  uint32_t reserved;                /* 0                                                                   */
+  uint32_t reserved1;               /* 0                                                                   */
+  lwse_drain_place_wave_key* keys;  /* [n_ids] out                                                         */
+  lwse_drain_place_wave* waves;     /* [max_waves] out: rows 0 .. n_waves                                  */
+  /* out */
+  uint32_t n_waves;
+  uint32_t n_planned;
+  uint32_t n_breaches_alone;
+  uint32_t n_no_wave;
+} lwse_drain_place_waves_query;
+LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_waves_query* q);
+
 /* ------------------------------------------------------------------------- */
 /* Peer exchange: the multi-GPU placement step without a collective library  */
 /* ------------------------------------------------------------------------- */

@@ -315,6 +315,13 @@ int launch_drain_waves_capped(const DrainWavesLaunch* p, const uint32_t* caps, u
   return launched_or_fail(2, cuda_err);
 }
 
+int launch_drain_waves_finish(const DrainWavesLaunch* p, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  const uint32_t n = p->n_dense > p->m ? p->n_dense : p->m;
+  drain_waves_finish_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(*p);
+  return launched_or_fail(1, cuda_err);
+}
+
 int launch_drain_waves(const DrainWavesLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err) {
   *cuda_err = 0;
   switch (pass) {

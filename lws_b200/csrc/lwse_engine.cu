@@ -248,6 +248,10 @@ struct lwse_engine {
   // DS drain waves (lwse_resident_ds_drain_waves): the per-LWS-row caps and the answer; the rest is the drain
   // waves' and the DS drain's scratch
   DevBuf dx_caps, dx_out;
+  // drain placement waves (lwse_resident_drain_place_waves): the step state, the wave state (U, key and namespace
+  // masks, drained slots, per-wave counts), the column state, the items, the rule-(b) domain index, the alone bits,
+  // the answer; the rest is the drain waves' and the drain placement's scratch
+  DevBuf dq_state, dq_uwave, dq_kwave, dq_nswave, dq_drained, dq_small, dq_colns, dq_items, dq_dix, dq_out;
   // DS drain (lwse_resident_ds_drain*): lost[L] and the after copy of lws_out, the before / after sweep outputs, the
   // touched DS rows, the reverse link index (count | first | cursor) and its entries, the key rows, the (DS, key) table
   DevBuf dd_lost, dd_lws_after, dd_out[2], dd_role_out[2], dd_revrole_out[2], dd_rows, dd_index, dd_entries, dd_cost, dd_table;
@@ -3118,6 +3122,352 @@ LWSE_API int lwse_resident_drain_place_cost(lwse_engine* e, uint32_t scope, lwse
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 64, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   if (words[5]) return LWSE_ERR_OOM;  // an item the table refused
+  return LWSE_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Drain placement waves
+// ---------------------------------------------------------------------------
+// Setup: the drain waves chain up to its dense rows, then the drain placement's three passes (its per-key solve
+// gives every key's alone row), then the rule-(b) domain index.  Then one captured step per key, replayed m times
+// with the cursor in device memory (no host synchronisation per key), the finish, and one copy back.
+LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_waves_query* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!drain_budget_ready(e)) return LWSE_ERR_NOT_READY;
+  if (!e->r_place_loaded || !e->r_place_current || e->n_domains == 0 || e->rn_namespaces == 0) return LWSE_ERR_NOT_READY;
+  if (q->scope != LWSE_DRAIN_NODES && q->scope != LWSE_DRAIN_DOMAINS) return LWSE_ERR_INVALID_ARG;
+  if (q->reserved || q->reserved1 || q->max_waves == 0 || q->max_waves > LWSE_DRAIN_WAVES_MAX || !q->waves) return LWSE_ERR_INVALID_ARG;
+  if (q->constraints == 0 || (q->constraints & ~LWSE_DPW_ALL)) return LWSE_ERR_INVALID_ARG;
+  if (q->n_ids && (!q->ids || !q->keys)) return LWSE_ERR_INVALID_ARG;
+  const bool by_domain = q->scope == LWSE_DRAIN_DOMAINS;
+  const uint32_t nn = e->n_nodes, nd = e->n_domains, nk = by_domain ? nd : nn, m = q->n_ids;
+  const uint32_t nl = e->rn_lws, ng = e->rn_groups, nr = e->rn_reqs, n_ns = e->rn_namespaces;
+  LWSE_CUDA(e, e->wf_stage.reserve((size_t)nk + 16));
+  uint8_t* seen = static_cast<uint8_t*>(e->wf_stage.h);
+  memset(seen, 0, nk);
+  for (uint32_t i = 0; i < m; i++) {
+    const uint32_t id = q->ids[i];
+    if (id >= nk || seen[id]) return LWSE_ERR_INVALID_ARG;
+    seen[id] = 1;
+  }
+  if (e->xch_world > 0 || nr >= (1u << 24) || !lwse::place_ns_supported(nn, nd)) return LWSE_ERR_UNSUPPORTED;
+  const uint32_t mw = q->max_waves;
+  uint32_t max_ns = 1;
+  {
+    std::vector<uint32_t> per(n_ns, 0);
+    for (uint32_t r = 0; r < nr; r++)
+      if (e->r_req_ns[r] < n_ns) max_ns = std::max(max_ns, ++per[e->r_req_ns[r]]);
+  }
+  const size_t wkeys_bytes = (size_t)m * sizeof(lwse_drain_wave_key);
+  const size_t wout_bytes = 16 + wkeys_bytes + (size_t)mw * sizeof(lwse_drain_wave);
+  const size_t keys_bytes = (size_t)m * sizeof(lwse_drain_place_wave_key);
+  const size_t out_bytes = 16 + keys_bytes + (size_t)mw * sizeof(lwse_drain_place_wave);
+  const size_t round_bytes = lwse::place_ns_scratch_bytes(nn, nd, nr, n_ns);
+  DeviceGuard guard(e->device);
+  // the drain waves' scratch
+  LWSE_CUDA(e, e->dv_cost.reserve((size_t)nk * sizeof(lwse_drain_budget_cost) + 16));
+  LWSE_CUDA(e, e->dv_words.reserve(128));
+  LWSE_CUDA(e, e->wf_words.reserve(256));
+  LWSE_CUDA(e, e->dv_ids.reserve((size_t)m * 4 + 16));
+  LWSE_CUDA(e, e->dv_pos.reserve((size_t)nk * 4 + 16));
+  LWSE_CUDA(e, e->dv_kidx.reserve(((size_t)m * 3 + 2) * 4 + 16));
+  LWSE_CUDA(e, e->dv_lidx.reserve(((size_t)nl * 3 + 2) * 4 + 16));
+  LWSE_CUDA(e, e->dv_dense.reserve((size_t)nl * 16 + 16));
+  LWSE_CUDA(e, e->dv_gwaves.reserve((size_t)ng * 8 + 16));
+  LWSE_CUDA(e, e->dv_out.reserve(wout_bytes));
+  LWSE_CUDA(e, e->dv_host.reserve(std::max(out_bytes, (size_t)m * 4)));
+  // the drain placement's scratch
+  LWSE_CUDA(e, e->dp_cost.reserve((size_t)nk * sizeof(lwse_drain_budget_cost) + 16));
+  LWSE_CUDA(e, e->dp_words.reserve(128));
+  LWSE_CUDA(e, e->dp_domfree.reserve((size_t)nd * 4 + 16));
+  LWSE_CUDA(e, e->dp_gidx.reserve(((size_t)ng * 3 + 2 + nr) * 4 + 16));
+  LWSE_CUDA(e, e->dp_uidx.reserve(((size_t)nk * 3 + 2) * 4 + 16));
+  LWSE_CUDA(e, e->dp_pos.reserve((size_t)nr * 4 + 16));
+  LWSE_CUDA(e, e->dp_rows.reserve((size_t)nk * sizeof(lwse_drain_place_cost) + 16));
+  LWSE_CUDA(e, e->dp_touched.reserve((size_t)n_ns + 16));
+  LWSE_CUDA(e, e->dp_round.reserve(round_bytes));
+  // this call's
+  const size_t small_bytes = (size_t)LWSE_DRAIN_WAVES_MAX * 16 * 4 * 3 + (size_t)LWSE_DRAIN_WAVES_MAX * 4 + (size_t)m * 4;
+  LWSE_CUDA(e, e->dq_state.reserve(sizeof(lwse::DpwState) + 16));
+  LWSE_CUDA(e, e->dq_uwave.reserve((size_t)nr * 8 + 16));
+  LWSE_CUDA(e, e->dq_kwave.reserve((size_t)nk * 8 + 16));
+  LWSE_CUDA(e, e->dq_nswave.reserve((size_t)n_ns * 8 + 16));
+  LWSE_CUDA(e, e->dq_drained.reserve((size_t)LWSE_DRAIN_WAVES_MAX * nd * 4 + 16));
+  LWSE_CUDA(e, e->dq_small.reserve(small_bytes + 16));
+  LWSE_CUDA(e, e->dq_colns.reserve((size_t)LWSE_DRAIN_WAVES_MAX * n_ns * 4 + 16));
+  LWSE_CUDA(e, e->dq_items.reserve((size_t)LWSE_DRAIN_WAVES_MAX * n_ns * 8 + 16));
+  LWSE_CUDA(e, e->dq_dix.reserve(((size_t)nd * 3 + 2 + nr) * 4 + 16));
+  LWSE_CUDA(e, e->dq_out.reserve(out_bytes));
+  const bool own_index = e->node_index_stale;
+  if (own_index) {
+    LWSE_CUDA(e, e->wf_dom_first.reserve(((size_t)nd + 1) * 4 + 16));
+    LWSE_CUDA(e, e->wf_node_order.reserve(((size_t)(nn + 255u) / 256u + 1u) * 1024u + 16));
+    LWSE_CUDA(e, e->wf_node_pos.reserve((size_t)nn * 4 + 16));
+    LWSE_CUDA(e, e->wf_node_ix.reserve(lwse::node_index_scratch_bytes(nd)));
+  }
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  int cuda_err = 0;
+  // ---- the drain waves chain up to its dense rows (lwse_resident_drain_waves) ----
+  uint32_t* v_words = (uint32_t*)e->dv_words.p;
+  if (m) {
+    memcpy(e->dv_host.h, q->ids, (size_t)m * 4);
+    LWSE_CUDA(e, cudaMemcpyAsync(e->dv_ids.p, e->dv_host.h, (size_t)m * 4, cudaMemcpyHostToDevice, s));
+  }
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_cost.p, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
+  LWSE_CUDA(e, cudaMemsetAsync(v_words, 0, 128, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_pos.p, 0xFF, (size_t)nk * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_kidx.p, 0, (size_t)m * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lidx.p, 0, (size_t)nl * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_gwaves.p, 0, (size_t)ng * 8, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_out.p, 0, wout_bytes, s));
+  lwse::DrainBudgetCostLaunch bp{};
+  bp.lws = (const lwse_lws_rec*)e->r_lws.p;
+  bp.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
+  bp.groups = (const lwse_group_rec*)e->r_groups.p;
+  bp.pod_state = (const uint8_t*)e->r_pst.p;
+  bp.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
+  bp.baseline = (const lwse_group_out*)e->r_group_out.p;
+  bp.nodes = (const lwse_node_rec*)e->nodes.p;
+  bp.occupancy = (const uint32_t*)e->r_occ.p;
+  bp.cost = (lwse_drain_budget_cost*)e->dv_cost.p;
+  bp.counts = v_words;
+  bp.n_pods = e->rn_pods;
+  bp.n_lws = nl;
+  bp.n_groups = ng;
+  bp.n_nodes = nn;
+  bp.n_domains = nd;
+  bp.n_keys = nk;
+  bp.by_domain = by_domain;
+  int launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  lwse::DrainPlaceWavesLaunch d{};
+  lwse::DrainWavesLaunch& w = d.w;
+  w.lws = bp.lws;
+  w.lws_out = bp.lws_out;
+  w.groups = bp.groups;
+  w.baseline = bp.baseline;
+  w.cost = bp.cost;
+  w.ids = (const uint32_t*)e->dv_ids.p;
+  w.pos_of = (uint32_t*)e->dv_pos.p;
+  w.count = (uint32_t*)e->dv_kidx.p;
+  w.first = w.count + m;
+  w.cursor = w.first + m + 1;
+  w.l_count = (uint32_t*)e->dv_lidx.p;
+  w.l_first = w.l_count + nl;
+  w.l_cursor = w.l_first + nl + 1;
+  w.dense = (uint4*)e->dv_dense.p;
+  w.g_waves = (unsigned long long*)e->dv_gwaves.p;
+  w.out = (uint8_t*)e->dv_out.p;
+  w.counts = reinterpret_cast<unsigned long long*>(v_words + 16);
+  w.n_lws = nl;
+  w.n_groups = ng;
+  w.n_keys = nk;
+  w.m = m;
+  w.max_waves = mw;
+  w.cols = (m < mw ? m : mw) + 1u;
+  launched = lwse::launch_drain_waves(&w, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  // ---- the drain placement's pass 0 (lwse_resident_drain_place_cost) ----
+  uint32_t* p_words = (uint32_t*)e->dp_words.p;
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_cost.p, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
+  LWSE_CUDA(e, cudaMemsetAsync(p_words, 0, 128, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_gidx.p, 0, (size_t)ng * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_uidx.p, 0, (size_t)nk * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_pos.p, 0xFF, (size_t)nr * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_touched.p, 1, n_ns, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_round.p, 0, round_bytes, s));
+  const uint32_t* dom_first = (const uint32_t*)e->dom_first.p;
+  const uint32_t* node_order = (const uint32_t*)e->node_order.p;
+  if (own_index) {
+    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_ix.p, 0, lwse::node_index_scratch_bytes(nd), s));
+    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_order.p, 0, ((size_t)(nn + 255u) / 256u + 1u) * 1024u, s));
+    launched = lwse::launch_node_index((const lwse_node_rec*)e->nodes.p, nn, nd, (uint32_t*)e->wf_dom_first.p,
+                                       (uint32_t*)e->wf_node_order.p, (uint32_t*)e->wf_node_pos.p, e->wf_node_ix.p, e->sm_count, s,
+                                       false, &cuda_err);
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    dom_first = (const uint32_t*)e->wf_dom_first.p;
+    node_order = (const uint32_t*)e->wf_node_order.p;
+  }
+  launched = lwse::launch_place_whatif_index((const lwse_place_req*)e->r_preq.p, nr, n_ns, (const uint8_t*)e->dp_touched.p, nn, nd,
+                                             e->dp_round.p, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  lwse::DrainBudgetCostLaunch pb = bp;
+  pb.cost = (lwse_drain_budget_cost*)e->dp_cost.p;
+  pb.counts = p_words + 16;
+  launched = lwse::launch_drain_budget_cost(&pb, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  lwse::DrainPlaceLaunch& p = d.p;
+  p.nodes = (const lwse_node_rec*)e->nodes.p;
+  p.occupancy = (const uint32_t*)e->r_occ.p;
+  p.dom_first = dom_first;
+  p.node_order = node_order;
+  p.dom_free = (uint32_t*)e->dp_domfree.p;
+  p.reqs = (const lwse_place_req*)e->r_preq.p;
+  p.base = (const lwse_place_out*)e->r_pout.p;
+  p.cost = (const lwse_drain_budget_cost*)e->dp_cost.p;
+  p.n_nodes = nn;
+  p.n_domains = nd;
+  p.n_reqs = nr;
+  p.n_namespaces = n_ns;
+  p.n_groups = ng;
+  p.n_keys = nk;
+  p.by_domain = by_domain;
+  p.g_count = (uint32_t*)e->dp_gidx.p;
+  p.g_first = p.g_count + ng;
+  p.g_cursor = p.g_first + ng + 1;
+  p.g_reqs = p.g_cursor + ng;
+  p.u_count = (uint32_t*)e->dp_uidx.p;
+  p.u_first = p.u_count + nk;
+  p.u_cursor = p.u_first + nk + 1;
+  p.pos = (uint32_t*)e->dp_pos.p;
+  p.rows = (lwse_drain_place_cost*)e->dp_rows.p;
+  p.counts = p_words;
+  p.round = e->dp_round.p;
+  p.round_bytes = round_bytes;
+  launched = lwse::launch_drain_place(&p, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  // first synchronisation: the pair totals of both chains (the same walk)
+  LWSE_CUDA(e, cudaMemcpyAsync(words, v_words + 16, 8, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 2, p_words, 32, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  uint64_t n_pairs = 0;
+  memcpy(&n_pairs, words, 8);
+  const uint32_t all_pairs = words[2 + 6];
+  if (n_pairs > 0xFFFFFFFFull / (LWSE_DRAIN_WAVES_MAX + 1u)) return LWSE_ERR_OOM;
+  LWSE_CUDA(e, e->dv_pairs.reserve((size_t)n_pairs * 8 + 16));
+  LWSE_CUDA(e, e->dv_recs.reserve((size_t)n_pairs * 16 + 16));
+  LWSE_CUDA(e, e->dp_pairs.reserve((size_t)all_pairs * 8 + 16));
+  launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dv_pairs.p, (uint32_t)n_pairs, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  w.pairs = (const unsigned long long*)e->dv_pairs.p;
+  w.n_pairs = (uint32_t)n_pairs;
+  w.recs = (uint4*)e->dv_recs.p;
+  launched = lwse::launch_drain_waves(&w, 1, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  launched = lwse::launch_drain_restart_pairs(&pb, (unsigned long long*)e->dp_pairs.p, all_pairs, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  p.pairs = (const unsigned long long*)e->dp_pairs.p;
+  p.n_pairs = all_pairs;
+  launched = lwse::launch_drain_place(&p, 1, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  // second synchronisation: the touched rows, |U| and the rule-(b) count
+  LWSE_CUDA(e, cudaMemcpyAsync(words, v_words, 64, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 16, v_words + 16, 16, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 20, w.l_first + nl, 4, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 32, p_words, 128, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 64, p.u_first + nk, 4, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  if (ng && words[8] != n_pairs) return LWSE_ERR_OOM;
+  if (words[18] || words[19]) return LWSE_ERR_OOM;
+  if (words[32 + 16 + 8] != all_pairs) return LWSE_ERR_OOM;
+  const uint32_t n_dense = words[20];
+  LWSE_CUDA(e, e->dv_lost.reserve((size_t)n_dense * w.cols * 4 + 16));
+  LWSE_CUDA(e, e->dv_rwaves.reserve((size_t)n_dense * 16 + 16));
+  LWSE_CUDA(e, e->dv_stamps.reserve((size_t)n_dense * 8 + 16));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lost.p, 0, (size_t)n_dense * w.cols * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_rwaves.p, 0, (size_t)n_dense * 16, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_stamps.p, 0, (size_t)n_dense * 8, s));
+  w.n_dense = n_dense;
+  w.lost = (uint32_t*)e->dv_lost.p;
+  w.row_waves = (unsigned long long*)e->dv_rwaves.p;
+  w.stamps = (uint32_t*)e->dv_stamps.p;
+  // the drain placement's pass 2: U_k, positions, capacities and every key's alone row
+  const uint32_t n_unp = words[64];
+  const uint64_t item_cap = (uint64_t)n_unp + words[32 + 3];
+  if (item_cap > (1ull << 30)) return LWSE_ERR_OOM;
+  uint64_t slots = 256;
+  while (slots < 2 * item_cap) slots <<= 1;
+  uint64_t grid = (uint64_t)e->sm_count * 2u;
+  while (grid > 1 && grid * max_ns * (sizeof(lwse_place_out) + 5) > (1ull << 30)) grid >>= 1;
+  const size_t slice_out = align256((size_t)grid * max_ns * sizeof(lwse_place_out));
+  const size_t slice_unp = align256((size_t)grid * max_ns * 4);
+  LWSE_CUDA(e, e->dp_slices.reserve(slice_out + slice_unp + (size_t)grid * max_ns + 16));
+  LWSE_CUDA(e, e->dp_items.reserve((size_t)slots * 8 + (size_t)item_cap * 8 + 16));
+  LWSE_CUDA(e, e->dp_urows.reserve((size_t)n_unp * 4 + 16));
+  p.u_rows = (uint32_t*)e->dp_urows.p;
+  p.n_unpinned = n_unp;
+  p.item_keys = (unsigned long long*)e->dp_items.p;
+  p.item_mask = (uint32_t)(slots - 1);
+  p.items = reinterpret_cast<uint2*>(p.item_keys + slots);
+  p.item_capacity = (uint32_t)item_cap;
+  LWSE_CUDA(e, cudaMemsetAsync(p.item_keys, 0xFF, (size_t)slots * 8, s));
+  p.s_out = (lwse_place_out*)e->dp_slices.p;
+  p.s_unpinned = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(e->dp_slices.p) + slice_out);
+  p.s_marks = static_cast<uint8_t*>(e->dp_slices.p) + slice_out + slice_unp;
+  p.slice_rows = max_ns;
+  p.grid = (uint32_t)grid;
+  launched = lwse::launch_drain_place(&p, 2, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  // ---- this call's state, the domain index, the steps ----
+  uint8_t* small = static_cast<uint8_t*>(e->dq_small.p);
+  LWSE_CUDA(e, cudaMemsetAsync(e->dq_state.p, 0, sizeof(lwse::DpwState), s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dq_uwave.p, 0, (size_t)nr * 8, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dq_kwave.p, 0, (size_t)nk * 8, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dq_nswave.p, 0, (size_t)n_ns * 8, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dq_drained.p, 0, (size_t)LWSE_DRAIN_WAVES_MAX * nd * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(small, 0, small_bytes, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dq_colns.p, 0, (size_t)LWSE_DRAIN_WAVES_MAX * n_ns * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dq_dix.p, 0, (size_t)nd * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dq_out.p, 0, out_bytes, s));
+  d.st = (lwse::DpwState*)e->dq_state.p;
+  d.constraints = q->constraints;
+  d.max_waves = mw;
+  d.u_wave = (unsigned long long*)e->dq_uwave.p;
+  d.key_wave = (unsigned long long*)e->dq_kwave.p;
+  d.ns_wave = (unsigned long long*)e->dq_nswave.p;
+  d.drained = (uint32_t*)e->dq_drained.p;
+  d.wnons = reinterpret_cast<uint32_t*>(small);
+  d.wplace = d.wnons + LWSE_DRAIN_WAVES_MAX * 16;
+  d.col_rows = d.wplace + LWSE_DRAIN_WAVES_MAX * 16;
+  d.wbreach = d.col_rows + LWSE_DRAIN_WAVES_MAX * 16;
+  d.kalone = d.wbreach + LWSE_DRAIN_WAVES_MAX;
+  d.col_ns = (uint32_t*)e->dq_colns.p;
+  d.items = (uint2*)e->dq_items.p;
+  d.item_capacity = LWSE_DRAIN_WAVES_MAX * n_ns;
+  d.dix_count = (uint32_t*)e->dq_dix.p;
+  d.dix_first = d.dix_count + nd;
+  d.dix_cursor = d.dix_first + nd + 1;
+  d.dix_rows = d.dix_cursor + nd;
+  d.out = (uint8_t*)e->dq_out.p;
+  launched = lwse::launch_drain_place_waves(&d, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (m) {
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    LWSE_CUDA(e, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    launched = lwse::launch_drain_place_waves(&d, 1, e->sm_count, s, &cuda_err);
+    const cudaError_t ce = cudaStreamEndCapture(s, &graph);
+    if (launched < 0 || ce != cudaSuccess) {
+      if (graph) cudaGraphDestroy(graph);
+      return fail_cuda(e, launched < 0 ? (cudaError_t)cuda_err : ce);
+    }
+    cudaError_t ge = cudaGraphInstantiate(&exec, graph, 0);
+    cudaGraphDestroy(graph);
+    for (uint32_t i = 0; ge == cudaSuccess && i < m; i++) ge = cudaGraphLaunch(exec, s);
+    if (exec) cudaGraphExecDestroy(exec);
+    if (ge != cudaSuccess) return fail_cuda(e, ge);
+    e->launches += (uint64_t)launched * m;
+  }
+  launched = lwse::launch_drain_place_waves(&d, 2, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(e->dv_host.h, d.out, out_bytes, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words, p_words, 64, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 16, &d.st->refused, 4, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  if (words[5] || words[16]) return LWSE_ERR_OOM;  // an item a table refused
+  const uint8_t* h = static_cast<const uint8_t*>(e->dv_host.h);
+  uint32_t totals[4];
+  memcpy(totals, h, 16);
+  if (m) memcpy(q->keys, h + 16, keys_bytes);
+  memcpy(q->waves, h + 16 + keys_bytes, (size_t)totals[0] * sizeof(lwse_drain_place_wave));
+  q->n_waves = totals[0];
+  q->n_planned = totals[1];
+  q->n_breaches_alone = totals[2];
+  q->n_no_wave = totals[3];
   return LWSE_OK;
 }
 

@@ -426,6 +426,45 @@ constexpr uint32_t kCapLinked = 1u << 4;
 int launch_drain_waves_capped(const DrainWavesLaunch* p, const uint32_t* caps, uint32_t constraints, int pass, int sm_count,
                               cudaStream_t s, int* cuda_err);
 
+// The drain waves finish alone (the wave rows' per-row columns and pods / leaders), after a plan written elsewhere.
+int launch_drain_waves_finish(const DrainWavesLaunch* p, int sm_count, cudaStream_t s, int* cuda_err);
+
+// ---- lwse_drain_place_wave_kernels.cu (and the set-overlay instance of the namespace kernel) ----
+// lwse_resident_drain_place_waves.  The step state lives in device memory so that one captured step replays for
+// every key: the key and its position, the open waves, the step's items and refusals, the floor verdicts of the
+// columns, the status counts.
+struct DpwState {
+  uint32_t key, i, n_open, n_items, refused, alone_bad, touched, breached;
+  unsigned long long bad;  // the open waves whose floor the key breaks
+  uint32_t status[4];
+};
+struct DrainPlaceWavesLaunch {
+  DrainWavesLaunch w;              // the floor plan (the drain waves chain up to its dense rows)
+  DrainPlaceLaunch p;              // the drain placement after its passes: U_k, positions, dom_free, the alone rows
+  DpwState* st;
+  uint32_t constraints, max_waves;
+  unsigned long long* u_wave;      // [n_reqs] bit w: the row is in U of wave w
+  unsigned long long* key_wave;    // [n_keys] bit w: the node (domain) is in wave w
+  unsigned long long* ns_wave;     // [n_namespaces] bit w: the namespace is solved for wave w
+  uint32_t* drained;               // [64 * n_domains] node scope: the free slots wave w drains from domain d
+  uint32_t* wnons;                 // [64 * 16] per wave: [1] |U_W|, [2..10] its rows of no namespace counted
+  uint32_t* wplace;                // [64 * 16] per wave: its last probe's counts (lwse_drain_place_cost words)
+  uint32_t* col_rows;              // [64 * 16] the step's column rows (lwse_drain_place_cost words)
+  uint32_t* col_ns;                // [64 * n_namespaces] the step's (column, namespace) flags
+  uint2* items;                    // {column, namespace}
+  uint32_t item_capacity;
+  uint32_t* dix_count;             // [n_domains] the rule-(b) rows by baseline domain (count | first | cursor)
+  uint32_t* dix_first;
+  uint32_t* dix_cursor;
+  uint32_t* dix_rows;              // [n_reqs]
+  uint32_t* kalone;                // [m] the LWSE_DPW_* bits each key triggers alone
+  uint32_t* wbreach;               // [64] lws_breached per wave
+  uint8_t* out;                    // the answer: totals (16 B), m key rows, max_waves wave rows
+};
+// Pass 0: the domain index and the first columns.  Pass 1: one step.  Pass 2: the finish.
+int launch_drain_place_waves(const DrainPlaceWavesLaunch* d, int pass, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_place_ns_drain_set(const DrainPlaceWavesLaunch* d, int sm_count, cudaStream_t s, int* cuda_err);
+
 // ---- lwse_ds_drain_wave_kernels.cu ----
 // lwse_resident_ds_drain_waves, around the drain waves chain.  Pass 0 (after the before sweep into t's outputs):
 // caps[L] |= the bits of every row the sweep reads that takes L's value (caps zeroed by the caller).  Pass 1 (after

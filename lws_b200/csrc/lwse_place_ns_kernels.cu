@@ -111,6 +111,18 @@ struct DrainNsView {
 };
 static_assert(sizeof(DrainNsView) <= sizeof(CUtensorMap), "the view travels in the tensor-map parameter");
 
+// The set-overlay instance (lwse_resident_drain_place_waves): DrainNsView with items {column, namespace} of the
+// current probe W_c ∪ {k}, `rows` the column rows and U_k read through u_first / u_rows at the key in state[0]; the
+// wave state says what W_c already drains.
+struct SetNsView {
+  DrainNsView d;
+  const uint32_t* state;                // [0] the key k of the current step
+  const unsigned long long* u_wave;     // [n_reqs] bit c: the row is in U of wave c
+  const unsigned long long* key_wave;   // [n_nodes] (node scope) or [n_domains] (domain scope) bit c: in wave c
+  const uint32_t* drained;              // node scope: [64 * n_domains] free slots wave c drains from domain d
+};
+static_assert(sizeof(SetNsView) <= sizeof(CUtensorMap), "the view travels in the tensor-map parameter");
+
 __device__ __forceinline__ uint32_t mix32n(uint32_t x) {
   x ^= x >> 16;
   x *= 0x85EBCA6Bu;
@@ -441,7 +453,11 @@ __device__ __forceinline__ void diff_row(const PlaceNsArgs& a, uint32_t r, const
 // slots, and level 2 skips the node's word), reads the rows of U_k as unpinned, keeps every result and the
 // overflow state in its own slice (indexed by position, not row), diffs the namespace's rows against the
 // baseline and adds the counts to the key's row.  The rows keep their keys (priority, ROW).
-template <bool kScan, bool kIndexed, bool kDrain = false>
+// kSet (with kDrain): the set-overlay instance.  Item {c, ns} solves ns for the probe W_c ∪ {k}: the staged
+// capacities are rebuilt from the resident ones minus what the column drains (every domain of W_c and k zeroed, or
+// every domain lowered by the free slots of its drained nodes), level 2 skips every drained node, and U_{W_c} ∪ U_k
+// read as unpinned; the namespace's diff goes to column c's row.
+template <bool kScan, bool kIndexed, bool kDrain = false, bool kSet = false>
 __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
     place_ns_kernel(const PlaceNsArgs a, const __grid_constant__ CUtensorMap words_map) {
   extern __shared__ uint8_t s_dyn[];
@@ -470,6 +486,8 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
   // stage a word table (it would read the view as a tensor map): the two-level form stages none.
   static_assert(!(kDrain && kScan), "the drain instance is two-level: its tensor-map parameter holds the view");
   const DrainNsView* const drain = reinterpret_cast<const DrainNsView*>(&words_map);
+  const SetNsView* const set = reinterpret_cast<const SetNsView*>(&words_map);
+  static_assert(!kSet || kDrain, "the set instance is a drain instance");
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5, n_warps = blockDim.x >> 5;
   const uint32_t* words = table_bytes ? s_words : a.g_words;
   const uint32_t* order = table_bytes ? s_order : a.node_order;
@@ -532,7 +550,42 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
     lwse_place_out* const obase = kDrain ? a.out + slice : a.out;
     const uint32_t ubase = kDrain ? slice : first;
     uint32_t skip_node = LWSE_NONE, od = LWSE_NONE, of = 0;  // kDrain: the drained node / domain, its staged capacity
-    if constexpr (kDrain) {
+    unsigned long long skip_bit = 0ull;                      // kSet: the column's bit in key_wave
+    if constexpr (kSet) {
+      const DrainNsView& dv = set->d;
+      const uint32_t k = __ldcg(set->state), c = key;
+      skip_bit = 1ull << c;
+      for (uint32_t p = tid; p < last - first; p += blockDim.x)
+        dv.marks[slice + p] = (__ldcg(set->u_wave + __ldcg(a.ns_rows + first + p)) & skip_bit) ? 1u : 0u;
+      __syncthreads();
+      for (uint32_t j = __ldcg(dv.u_first + k) + tid, end = __ldcg(dv.u_first + k + 1u); j < end; j += blockDim.x) {
+        const uint32_t p = __ldcg(dv.pos + __ldcg(dv.u_rows + j));
+        if (p >= first && p < last) dv.marks[slice + p - first] = 1u;
+      }
+      uint32_t kd = LWSE_NONE, kf = 0;
+      if (dv.by_domain) {
+        kd = k < a.n_domains ? k : LWSE_NONE;
+      } else if (k < a.n_nodes) {
+        skip_node = k;
+        const uint4 nr = ldg_keep(reinterpret_cast<const uint4*>(a.nodes + k));
+        const uint32_t fl = nr.w >> 16;
+        if ((fl & LWSE_NODE_SCHEDULABLE) && (fl & LWSE_NODE_HAS_TOPOLOGY) && nr.z < a.n_domains) {
+          const uint32_t cap = nr.w & 0xFFFFu, occ = occupancy_sum(a, a.occupancy, k);
+          kf = cap > occ ? cap - occ : 0u;
+          kd = nr.z;
+        }
+      }
+      for (uint32_t d = tid; d < a.n_domains; d += blockDim.x) {
+        uint32_t f = __ldcg(a.g_dom_free + d);
+        if (dv.by_domain) {
+          if (d == kd || (__ldcg(set->key_wave + d) & skip_bit)) f = 0u;
+        } else {
+          f -= __ldcg(set->drained + (size_t)c * a.n_domains + d) + (d == kd ? kf : 0u);
+        }
+        s_free[d] = f;
+      }
+      __syncthreads();
+    } else if constexpr (kDrain) {
       const DrainNsView& dv = *drain;
       for (uint32_t p = tid; p < last - first; p += blockDim.x) dv.marks[slice + p] = 0u;
       __syncthreads();
@@ -749,7 +802,9 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
               const uint32_t w = __ldcg(a.g_nodes2 + i);
               if ((w >> 28) == 0u) continue;
               const uint32_t n = w & 0x0FFFFFFFu;
-              if constexpr (kDrain) {
+              if constexpr (kSet) {
+                if (n == skip_node || (!set->d.by_domain && (__ldcg(set->key_wave + n) & skip_bit))) continue;  // cordoned
+              } else if constexpr (kDrain) {
                 if (n == skip_node) continue;  // cordoned
               }
               const uint32_t l = ((w >> 28) << 28) | (mix32n(key_hi ^ (n * 0x85EBCA77u)) >> 4);
@@ -1222,6 +1277,71 @@ int launch_place_ns_drain(const DrainPlaceLaunch* p, int sm_count, cudaStream_t 
   e = cudaGetLastError();
   if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
   return 3;
+}
+
+// The set-overlay solve of one drain placement waves step: the capacities and positions are those the drain
+// placement's solve left (launch_place_ns_drain ran at setup); a persistent grid over the step's items.
+int launch_place_ns_drain_set(const DrainPlaceWavesLaunch* d, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  const DrainPlaceLaunch* p = &d->p;
+  const NsLayout l = ns_layout(p->n_nodes, p->n_domains, p->n_reqs, p->n_namespaces);
+  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) {
+    *cuda_err = (int)cudaErrorInvalidValue;
+    return -1;
+  }
+  uint8_t* base = static_cast<uint8_t*>(p->round);
+  PlaceNsArgs a{};
+  a.nodes = p->nodes;
+  a.reqs = p->reqs;
+  a.occupancy = p->occupancy;
+  a.dom_first = p->dom_first;
+  a.node_order = p->node_order;
+  a.g_words = reinterpret_cast<uint32_t*>(base + l.words);
+  a.g_nodes2 = reinterpret_cast<uint32_t*>(base + l.nodes2);
+  a.g_dom_free = reinterpret_cast<uint32_t*>(base + l.dom_free);
+  a.ns_first = reinterpret_cast<uint32_t*>(base + l.ns_first);
+  a.ns_rows = reinterpret_cast<uint32_t*>(base + l.ns_rows);
+  a.ns_count = reinterpret_cast<uint32_t*>(base + l.ns_count);
+  a.ns_cursor = reinterpret_cast<uint32_t*>(base + l.ns_cursor);
+  a.counters = reinterpret_cast<uint32_t*>(base + l.counters) + 4u * 8u;
+  a.n_nodes = p->n_nodes;
+  a.n_domains = p->n_domains;
+  a.n_namespaces = p->n_namespaces;
+  a.n_parts = 1u;
+  a.word_rows = l.word_rows;
+  a.n_reqs = p->n_reqs;
+  a.out = p->s_out;
+  a.unpinned = p->s_unpinned;
+  SetNsView v{};
+  v.d.items = d->items;
+  v.d.n_items = &d->st->n_items;
+  v.d.item_capacity = d->item_capacity;
+  v.d.u_first = p->u_first;
+  v.d.u_rows = p->u_rows;
+  v.d.pos = p->pos;
+  v.d.marks = p->s_marks;
+  v.d.base = p->base;
+  v.d.rows = d->col_rows;
+  v.d.slice_rows = p->slice_rows;
+  v.d.by_domain = p->by_domain ? 1u : 0u;
+  v.state = &d->st->key;
+  v.u_wave = d->u_wave;
+  v.key_wave = d->key_wave;
+  v.drained = d->drained;
+  CUtensorMap view;
+  memset(&view, 0, sizeof(view));
+  memcpy(&view, &v, sizeof(v));
+  const size_t smem = ns_smem_bytes(l.word_rows, p->n_domains, false, false);
+  static thread_local size_t attr_set = 0;
+  if (smem > attr_set) {
+    const cudaError_t e = cudaFuncSetAttribute(place_ns_kernel<false, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    attr_set = smem;
+  }
+  place_ns_kernel<false, true, true, true><<<p->grid, kNsThreads, smem, s>>>(a, view);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+  return 1;
 }
 
 int launch_index_scan(uint32_t* d_count, uint32_t* d_first, uint32_t* d_cursor, uint32_t n, cudaStream_t s, int* cuda_err) {

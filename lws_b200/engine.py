@@ -53,6 +53,7 @@ SYMBOLS = {
     "lwse_resident_ds_drain": ([C.c_void_p, C.POINTER(R.DsDrainQuery)], C.c_int),
     "lwse_resident_ds_drain_cost": ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_resident_ds_drain_waves": ([C.c_void_p, C.POINTER(R.DsDrainWavesQuery)], C.c_int),
+    "lwse_resident_drain_place_waves": ([C.c_void_p, C.POINTER(R.DrainPlaceWavesQuery)], C.c_int),
     "lwse_place_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
         C.c_int,
@@ -599,6 +600,32 @@ class Engine:
         self._check(lib().lwse_resident_ds_drain_waves(self._h, C.byref(q)))
         out = {"keys": keys[: len(ids)], "waves": waves[: q.n_waves]}
         out.update({k: getattr(q, k) for k in R.DS_DRAIN_WAVES_TOTALS})
+        return out
+
+    def resident_drain_place_waves(self, nodes=None, domains=None, max_waves=R.DRAIN_WAVES_MAX,
+                                   constraints=R.DPW_LWS_FLOOR | R.DPW_STRANDED):
+        """lwse_resident_drain_place_waves: the distinct node rows ``nodes`` — or domain ids ``domains`` — packed
+        first-fit, in the order given, into at most ``max_waves`` waves whose drain triggers none of the verdicts in
+        ``constraints`` (``records.DPW_*``).  The default keeps every LeaderWorkerSet at its floor and finds every
+        request the wave unpins a new exclusive domain; ``DPW_BUMPED`` (no other request loses its domain) is
+        opt-in.  Give exactly one of the two.  → dict: ``keys`` (``records.DRAIN_PLACE_WAVE_KEY``, in query order),
+        ``waves`` (``records.DRAIN_PLACE_WAVE``, one per opened wave) and the totals of
+        ``records.DRAIN_WAVES_TOTALS``."""
+        if (nodes is None) == (domains is None):
+            raise ValueError("give node rows or domain ids")
+        ids = np.ascontiguousarray(nodes if domains is None else domains, dtype=np.uint32)
+        keys = R.aligned_empty(max(len(ids), 1), R.DRAIN_PLACE_WAVE_KEY)
+        waves = R.aligned_empty(max(int(max_waves), 1), R.DRAIN_PLACE_WAVE)
+        q = R.DrainPlaceWavesQuery()
+        q.ids = R.ptr(ids) if len(ids) else None
+        q.n_ids = len(ids)
+        q.scope = R.DRAIN_NODES if domains is None else R.DRAIN_DOMAINS
+        q.max_waves = int(max_waves)
+        q.constraints = int(constraints)
+        q.keys, q.waves = R.ptr(keys), R.ptr(waves)
+        self._check(lib().lwse_resident_drain_place_waves(self._h, C.byref(q)))
+        out = {"keys": keys[: len(ids)], "waves": waves[: q.n_waves]}
+        out.update({k: getattr(q, k) for k in R.DRAIN_WAVES_TOTALS})
         return out
 
     def resident_patch(self, which: int, rows, values):

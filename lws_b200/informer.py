@@ -647,6 +647,17 @@ class IncrementalEncoder:
         base["unplanned"] = [(name, st, a) for (name, st), a in zip(base["unplanned"], alone)]
         return base
 
+    def drain_place_waves_report(self, result: dict, scope: str = "nodes") -> dict:
+        """A ``resident_drain_place_waves`` answer with names, as ``drain_waves_report``: ``waves``, one list per
+        wave of the node names or topology values in it, and ``unplanned``, the keys without a wave as (name,
+        status, alone) with ``alone`` the names (``records.DPW_NAMES``) of the verdicts the key triggers by itself.
+        Nothing in the encoder changes."""
+        base = self.drain_waves_report(result, scope)
+        alone = [[n for bit, n in R.DPW_NAMES.items() if int(k["alone"]) & bit]
+                 for k in result["keys"] if int(k["status"]) != R.DRAINW_PLANNED]
+        base["unplanned"] = [(name, st, a) for (name, st), a in zip(base["unplanned"], alone)]
+        return base
+
     # ------------------------------------------------------------------ results
     def tables(self):
         """(lws, groups, pod_state, pod_ident, reqs) trimmed to the rows in use (+ spare already laid out)."""

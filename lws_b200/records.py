@@ -785,6 +785,44 @@ assert C.sizeof(DsDrainWavesQuery) == 64
 # the totals of a DS drain waves query, as Engine.resident_ds_drain_waves returns them
 DS_DRAIN_WAVES_TOTALS = ("n_waves", "n_planned", "n_breaches_alone", "n_no_wave")
 
+# drain placement waves (lwse_resident_drain_place_waves): the verdicts a plan keeps and a key triggers alone
+DPW_LWS_FLOOR = 1 << 0
+DPW_STRANDED = 1 << 1
+DPW_BUMPED = 1 << 2
+DPW_ALL = DPW_LWS_FLOOR | DPW_STRANDED | DPW_BUMPED
+DPW_NAMES = {DPW_LWS_FLOOR: "lws_floor", DPW_STRANDED: "stranded", DPW_BUMPED: "bumped"}
+
+# lwse_drain_place_wave_key: one key of the plan, in query order
+DRAIN_PLACE_WAVE_KEY = np.dtype(
+    [("id", "<u4"), ("wave", "<u4"), ("status", "<u4"), ("alone", "<u4"), ("groups_restarted", "<u4"),
+     ("ready_restarted", "<u4"), ("lws_touched", "<u4"), ("lws_breached", "<u4"), ("unpinned", "<u4"),
+     ("stranded", "<u4"), ("bumped", "<u4"), ("reserved", "<u4")],
+    align=False,
+)
+assert DRAIN_PLACE_WAVE_KEY.itemsize == 48
+
+# lwse_drain_place_wave: one opened wave, the set-form totals of the drain budget and the drain placement
+DRAIN_PLACE_WAVE = np.dtype(
+    [("n_keys", "<u4"), ("lws_touched", "<u4"), ("lws_loses_available", "<u4"), ("n_pods_evicted", "<u4"),
+     ("n_leaders_evicted", "<u4"), ("n_groups_restarted", "<u4"), ("n_ready_restarted", "<u4"), ("min_margin", "<i4"),
+     ("n_pods_recreated", "<u8"), ("lws_breached", "<u4"), ("unpinned", "<u4"), ("stranded", "<u4"), ("bumped", "<u4"),
+     ("n_changed", "<u4"), ("n_lost", "<u4"), ("n_moved", "<u4"), ("n_gained", "<u4"), ("n_placed", "<u4"),
+     ("n_unschedulable", "<u4"), ("n_conflict", "<u4"), ("namespaces_solved", "<u4"), ("reserved", "<u4", (2,))],
+    align=False,
+)
+assert DRAIN_PLACE_WAVE.itemsize == 96
+
+
+class DrainPlaceWavesQuery(C.Structure):
+    """lwse_drain_place_waves_query: a first-fit plan of distinct node rows or domain ids into waves whose
+    restarted groups find a new exclusive domain (the ids, the cap and the DPW_* mask in, the DRAIN_PLACE_WAVE_KEY
+    and DRAIN_PLACE_WAVE rows and the DRAIN_WAVES_TOTALS out)."""
+
+    _fields_ = DsDrainWavesQuery._fields_
+
+
+assert C.sizeof(DrainPlaceWavesQuery) == 64
+
 
 class Config(C.Structure):
     _fields_ = [
