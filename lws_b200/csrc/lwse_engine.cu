@@ -2263,6 +2263,60 @@ static bool whatif_timing() {
   return on;
 }
 
+// Every what-if runs on wf_stream behind an event on the engine's stream (the most recently submitted tick, both
+// branches joined), reading the resident tables and the baseline results in place: nothing writes them while
+// the call holds the mutex, and the call synchronizes its stream before it returns.
+static int drain_begin_locked(lwse_engine* e) {
+  if (!e->wf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->wf_stream, cudaStreamNonBlocking));
+  if (!e->ev_wf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_wf, cudaEventDisableTiming));
+  LWSE_CUDA(e, cudaEventRecord(e->ev_wf, e->stream));
+  LWSE_CUDA(e, cudaStreamWaitEvent(e->wf_stream, e->ev_wf, 0));
+  e->wf_timed = false;
+  if (whatif_timing()) {
+    if (!e->ev_wf_t0) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t0));
+    if (!e->ev_wf_t1) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t1));
+    LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t0, e->wf_stream));
+  }
+  return LWSE_OK;
+}
+
+static int drain_end_locked(lwse_engine* e) {
+  if (whatif_timing()) {
+    LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t1, e->wf_stream));
+    e->wf_timed = true;
+  }
+  return LWSE_OK;
+}
+
+// The scratch of a private node index (wf_node_*), reserved before the snapshot: a reserve may reallocate.
+static int reserve_node_index(lwse_engine* e) {
+  LWSE_CUDA(e, e->wf_dom_first.reserve(((size_t)e->n_domains + 1) * 4 + 16));
+  LWSE_CUDA(e, e->wf_node_order.reserve(((size_t)(e->n_nodes + 255u) / 256u + 1u) * 1024u + 16));
+  LWSE_CUDA(e, e->wf_node_pos.reserve((size_t)e->n_nodes * 4 + 16));
+  LWSE_CUDA(e, e->wf_node_ix.reserve(lwse::node_index_scratch_bytes(e->n_domains)));
+  return LWSE_OK;
+}
+
+// A node index over `nodes` in the wf_node_* scratch, on s, for a what-if whose node rows the resident index
+// does not describe; the index pointers are set to it (node_pos may be null).
+static int own_node_index(lwse_engine* e, const lwse_node_rec* nodes, cudaStream_t s, const uint32_t** dom_first,
+                          const uint32_t** node_order, const uint32_t** node_pos) {
+  // The build wants its per-domain counts at zero.  A build leaves them so but not its cursors, and their
+  // places move with n_domains (counts at [0, n), cursors at [n, 2n)): cleared before every build, as
+  // lwse_upload_nodes clears the resident ones.  The padding of the order rows stays zero.
+  LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_ix.p, 0, lwse::node_index_scratch_bytes(e->n_domains), s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_order.p, 0, ((size_t)(e->n_nodes + 255u) / 256u + 1u) * 1024u, s));
+  int cuda_err = 0;
+  const int launched = lwse::launch_node_index(nodes, e->n_nodes, e->n_domains, (uint32_t*)e->wf_dom_first.p,
+                                               (uint32_t*)e->wf_node_order.p, (uint32_t*)e->wf_node_pos.p, e->wf_node_ix.p,
+                                               e->sm_count, s, false, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  *dom_first = (const uint32_t*)e->wf_dom_first.p;
+  *node_order = (const uint32_t*)e->wf_node_order.p;
+  if (node_pos) *node_pos = (const uint32_t*)e->wf_node_pos.p;
+  return LWSE_OK;
+}
+
 // Patched copies of the node and request rows in what-if scratch, the round over them on wf_stream
 // (only the touched namespaces in the namespace form), then one diff kernel against the baseline rows
 // (r_pout, read in place: nothing writes them while the call holds the mutex).  The resident node
@@ -2319,9 +2373,6 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
   for (uint8_t t : touched) n_touched += t;
 
   DeviceGuard guard(e->device);
-  if (!e->wf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->wf_stream, cudaStreamNonBlocking));
-  if (!e->ev_wf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_wf, cudaEventDisableTiming));
-  cudaStream_t s = e->wf_stream;
   // staging (the previous call synchronized its stream: the buffer is free)
   LWSE_CUDA(e, e->wf_stage.reserve(stage_need));
   LWSE_CUDA(e, e->wf_words.reserve(64));
@@ -2342,19 +2393,8 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
   const uint32_t list_cap = q->capacity < rn ? q->capacity : rn;  // (at most rn rows can differ)
   LWSE_CUDA(e, e->wf_list.reserve(64 + 16 + (size_t)list_cap * (4 + 2 * sizeof(lwse_place_out))));
   if (node_rows) LWSE_CUDA(e, e->wf_nodes.reserve(b_nodes + 16));
-  if (node_rebuild) {
-    const size_t order_padded = ((size_t)(e->n_nodes + 255u) / 256u + 1u) * 1024u;
-    const size_t ix_bytes = lwse::node_index_scratch_bytes(e->n_domains);
-    LWSE_CUDA(e, e->wf_dom_first.reserve(((size_t)e->n_domains + 1) * 4 + 16));
-    LWSE_CUDA(e, e->wf_node_order.reserve(order_padded + 16));
-    LWSE_CUDA(e, e->wf_node_pos.reserve((size_t)e->n_nodes * 4 + 16));
-    LWSE_CUDA(e, e->wf_node_ix.reserve(ix_bytes));
-    // The build wants its per-domain counts at zero.  A build leaves them so but not its cursors, and their
-    // places move with n_domains (counts at [0, n), cursors at [n, 2n)): cleared before every build, as
-    // lwse_upload_nodes clears the resident ones.  The padding of the order rows stays zero.
-    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_ix.p, 0, ix_bytes, s));
-    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_order.p, 0, order_padded, s));
-  }
+  if (node_rebuild)
+    if (const int rc = reserve_node_index(e); rc != LWSE_OK) return rc;
   size_t round_bytes = 0;
   bool round_fresh = false;
   if (ns_form) {
@@ -2370,16 +2410,8 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
     e->wf_geometry[0] = e->wf_geometry[1] = e->wf_geometry[2] = e->wf_geometry[3] = 0;  // (the general form re-initialises it)
   }
 
-  // the snapshot: behind everything on the engine's stream, both branches of every tick submitted so far joined
-  LWSE_CUDA(e, cudaEventRecord(e->ev_wf, e->stream));
-  LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_wf, 0));
-  const bool timing = whatif_timing();
-  e->wf_timed = false;
-  if (timing) {
-    if (!e->ev_wf_t0) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t0));
-    if (!e->ev_wf_t1) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t1));
-    LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t0, s));
-  }
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
   lwse_node_rec* d_nodes = (lwse_node_rec*)e->nodes.p;
   lwse_place_req* d_reqs = (lwse_place_req*)e->wf_reqs.p;
   lwse_place_out* d_out = (lwse_place_out*)e->wf_out.p;
@@ -2428,15 +2460,8 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
   const uint32_t* dom_first = (const uint32_t*)e->dom_first.p;
   const uint32_t* node_order = (const uint32_t*)e->node_order.p;
   const uint32_t* node_pos = (const uint32_t*)e->node_pos.p;
-  if (node_rebuild) {
-    const int launched = lwse::launch_node_index(d_nodes, e->n_nodes, e->n_domains, (uint32_t*)e->wf_dom_first.p,
-                                                 (uint32_t*)e->wf_node_order.p, (uint32_t*)e->wf_node_pos.p, e->wf_node_ix.p,
-                                                 e->sm_count, s, false, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-    dom_first = (const uint32_t*)e->wf_dom_first.p;
-    node_order = (const uint32_t*)e->wf_node_order.p;
-    node_pos = (const uint32_t*)e->wf_node_pos.p;
-  }
+  if (node_rebuild)
+    if (const int rc = own_node_index(e, d_nodes, s, &dom_first, &node_order, &node_pos); rc != LWSE_OK) return rc;
   if (ns_form) {
     if (round_fresh) LWSE_CUDA(e, cudaMemsetAsync(e->wf_round.p, 0, round_bytes, s));  // (index counts and counters start at zero)
     int launched = lwse::launch_place_whatif_index(d_reqs, n_total, n_ns, (const uint8_t*)e->wf_touched.p, e->n_nodes, e->n_domains,
@@ -2466,10 +2491,7 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
                                                         d_after, list_cap, d_counts, e->sm_count, s, &cuda_err);
     if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
-  if (timing) {
-    LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t1, s));
-    e->wf_timed = true;
-  }
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_counts, 32, cudaMemcpyDeviceToHost, s));
   if (q->n_extra)
@@ -2498,27 +2520,48 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
 // ---------------------------------------------------------------------------
 // Drain what-if and drain cost
 // ---------------------------------------------------------------------------
-// Both on wf_stream behind an event on the engine's stream (the most recently submitted tick, both branches
-// joined), reading the resident tables and the baseline group results in place: nothing writes them while
-// the call holds the mutex, and the call synchronizes its stream before it returns.
-static int drain_begin_locked(lwse_engine* e) {
-  if (!e->wf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->wf_stream, cudaStreamNonBlocking));
-  if (!e->ev_wf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_wf, cudaEventDisableTiming));
-  LWSE_CUDA(e, cudaEventRecord(e->ev_wf, e->stream));
-  LWSE_CUDA(e, cudaStreamWaitEvent(e->wf_stream, e->ev_wf, 0));
-  e->wf_timed = false;
-  if (whatif_timing()) {
-    if (!e->ev_wf_t0) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t0));
-    if (!e->ev_wf_t1) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t1));
-    LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t0, e->wf_stream));
-  }
-  return LWSE_OK;
+// The restart walk over the resident tables (the drain budget's passes and the pair walk), its key rows in `cost`
+// and its counters at `counts`.
+static lwse::DrainBudgetCostLaunch restart_walk(const lwse_engine* e, bool by_domain, lwse_drain_budget_cost* cost,
+                                                uint32_t* counts) {
+  lwse::DrainBudgetCostLaunch p{};
+  p.lws = (const lwse_lws_rec*)e->r_lws.p;
+  p.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
+  p.groups = (const lwse_group_rec*)e->r_groups.p;
+  p.pod_state = (const uint8_t*)e->r_pst.p;
+  p.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
+  p.baseline = (const lwse_group_out*)e->r_group_out.p;
+  p.nodes = (const lwse_node_rec*)e->nodes.p;
+  p.occupancy = (const uint32_t*)e->r_occ.p;
+  p.cost = cost;
+  p.counts = counts;
+  p.n_pods = e->rn_pods;
+  p.n_lws = e->rn_lws;
+  p.n_groups = e->rn_groups;
+  p.n_nodes = e->n_nodes;
+  p.n_domains = e->n_domains;
+  p.n_keys = by_domain ? e->n_domains : e->n_nodes;
+  p.by_domain = by_domain;
+  return p;
 }
 
-static int drain_end_locked(lwse_engine* e) {
-  if (whatif_timing()) {
-    LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t1, e->wf_stream));
-    e->wf_timed = true;
+// The slots of a linear-probing table for `pairs` entries: a power of two at least twice their count, so a probe
+// always finds a free slot, and at least 256.
+static uint64_t table_slots(uint64_t pairs) {
+  uint64_t slots = 256;
+  while (slots < 2 * pairs) slots <<= 1;
+  return slots;
+}
+
+// The query's m keys are distinct and below nk (marked in wf_stage's host side: before the snapshot, so nothing
+// in flight reads it).
+static int check_key_ids(lwse_engine* e, const uint32_t* ids, uint32_t m, uint32_t nk) {
+  LWSE_CUDA(e, e->wf_stage.reserve((size_t)nk + 16));
+  uint8_t* seen = static_cast<uint8_t*>(e->wf_stage.h);
+  memset(seen, 0, nk);
+  for (uint32_t i = 0; i < m; i++) {
+    if (ids[i] >= nk || seen[ids[i]]) return LWSE_ERR_INVALID_ARG;  // out of range, or a duplicate
+    seen[ids[i]] = 1;
   }
   return LWSE_OK;
 }
@@ -2748,24 +2791,7 @@ LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lws
   LWSE_CUDA(e, e->wf_words.reserve(64));
   if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
   cudaStream_t s = e->wf_stream;
-  lwse::DrainBudgetCostLaunch p{};
-  p.lws = (const lwse_lws_rec*)e->r_lws.p;
-  p.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
-  p.groups = (const lwse_group_rec*)e->r_groups.p;
-  p.pod_state = (const uint8_t*)e->r_pst.p;
-  p.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
-  p.baseline = (const lwse_group_out*)e->r_group_out.p;
-  p.nodes = (const lwse_node_rec*)e->nodes.p;
-  p.occupancy = (const uint32_t*)e->r_occ.p;
-  p.cost = (lwse_drain_budget_cost*)e->dr_bcost.p;
-  p.counts = (uint32_t*)e->dr_bwords.p;
-  p.n_pods = e->rn_pods;
-  p.n_lws = e->rn_lws;
-  p.n_groups = e->rn_groups;
-  p.n_nodes = nn;
-  p.n_domains = e->n_domains;
-  p.n_keys = n_keys;
-  p.by_domain = by_domain;
+  lwse::DrainBudgetCostLaunch p = restart_walk(e, by_domain, (lwse_drain_budget_cost*)e->dr_bcost.p, (uint32_t*)e->dr_bwords.p);
   LWSE_CUDA(e, cudaMemsetAsync(p.cost, 0, cost_bytes, s));
   LWSE_CUDA(e, cudaMemsetAsync(p.counts, 0, 64, s));
   int cuda_err = 0;
@@ -2778,8 +2804,7 @@ LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lws
   memcpy(&pairs, words, 8);
   if (pairs) {
     if (pairs > (1ull << 30)) return LWSE_ERR_OOM;  // (the table index is 32-bit)
-    uint64_t slots = 256;
-    while (slots < 2 * pairs) slots <<= 1;
+    const uint64_t slots = table_slots(pairs);
     LWSE_CUDA(e, e->dr_table.reserve((size_t)slots * (sizeof(unsigned long long) + sizeof(uint4))));
     p.keys = (unsigned long long*)e->dr_table.p;
     p.vals = reinterpret_cast<uint4*>(p.keys + slots);
@@ -2800,6 +2825,134 @@ LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lws
 // ---------------------------------------------------------------------------
 // Drain waves
 // ---------------------------------------------------------------------------
+// The drain waves chain up to its dense rows, shared by lwse_resident_drain_waves, lwse_resident_ds_drain_waves and
+// lwse_resident_drain_place_waves.  Its steps enqueue on wf_stream and never synchronize.  The caller zeroes the
+// counter blocks the steps write (one block may hold other counters too), issues every read-back, and launches
+// passes 1 and 2, whose variant differs between the planners.
+
+// A waves answer: the totals (16 B), m key rows, then max_waves wave rows.  (Templates over the query and row
+// types, so with C++ linkage inside the API block.)
+extern "C++" {
+template <class Key, class Wave>
+static size_t waves_answer_bytes(uint32_t m, uint32_t max_waves) {
+  return 16 + (size_t)m * sizeof(Key) + (size_t)max_waves * sizeof(Wave);
+}
+
+// A waves answer, read back into dv_host by the caller's last synchronisation, copied out to the query.
+template <class Q>
+static void copy_waves_answer(const lwse_engine* e, Q* q) {
+  const uint8_t* h = static_cast<const uint8_t*>(e->dv_host.h);
+  const size_t keys_bytes = (size_t)q->n_ids * sizeof(*q->keys);
+  uint32_t totals[4];
+  memcpy(totals, h, 16);
+  if (q->n_ids) memcpy(q->keys, h + 16, keys_bytes);
+  memcpy(q->waves, h + 16 + keys_bytes, (size_t)totals[0] * sizeof(*q->waves));
+  q->n_waves = totals[0];
+  q->n_planned = totals[1];
+  q->n_breaches_alone = totals[2];
+  q->n_no_wave = totals[3];
+}
+}  // extern "C++"
+
+// The chain's scratch for m keys out of nk, and dv_host, which carries the keys in and the caller's answer of
+// answer_bytes out: reserved once at the larger size, before the snapshot.
+static int reserve_drain_waves(lwse_engine* e, uint32_t m, uint32_t nk, uint32_t max_waves, size_t answer_bytes) {
+  const uint32_t nl = e->rn_lws, ng = e->rn_groups;
+  LWSE_CUDA(e, e->dv_ids.reserve((size_t)m * 4 + 16));
+  LWSE_CUDA(e, e->dv_pos.reserve((size_t)nk * 4 + 16));
+  LWSE_CUDA(e, e->dv_kidx.reserve(((size_t)m * 3 + 2) * 4 + 16));
+  LWSE_CUDA(e, e->dv_lidx.reserve(((size_t)nl * 3 + 2) * 4 + 16));
+  LWSE_CUDA(e, e->dv_dense.reserve((size_t)nl * 16 + 16));
+  LWSE_CUDA(e, e->dv_gwaves.reserve((size_t)ng * 8 + 16));
+  LWSE_CUDA(e, e->dv_out.reserve(waves_answer_bytes<lwse_drain_wave_key, lwse_drain_wave>(m, max_waves)));
+  LWSE_CUDA(e, e->dv_host.reserve(std::max(answer_bytes, (size_t)m * 4)));
+  return LWSE_OK;
+}
+
+// The keys in through dv_host, the chain's scratch and the walk's key rows zeroed, the restart walk's pass 0 (`bp`),
+// then the chain's pass 0 into p, its counters at `counts`.
+static int enqueue_drain_waves_setup(lwse_engine* e, const lwse::DrainBudgetCostLaunch& bp, const uint32_t* ids, uint32_t m,
+                                     uint32_t max_waves, unsigned long long* counts, lwse::DrainWavesLaunch* p) {
+  const uint32_t nl = e->rn_lws, ng = e->rn_groups, nk = bp.n_keys;
+  cudaStream_t s = e->wf_stream;
+  if (m) {
+    memcpy(e->dv_host.h, ids, (size_t)m * 4);
+    LWSE_CUDA(e, cudaMemcpyAsync(e->dv_ids.p, e->dv_host.h, (size_t)m * 4, cudaMemcpyHostToDevice, s));
+  }
+  LWSE_CUDA(e, cudaMemsetAsync(bp.cost, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_pos.p, 0xFF, (size_t)nk * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_kidx.p, 0, (size_t)m * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lidx.p, 0, (size_t)nl * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_gwaves.p, 0, (size_t)ng * 8, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_out.p, 0, waves_answer_bytes<lwse_drain_wave_key, lwse_drain_wave>(m, max_waves), s));
+  int cuda_err = 0;
+  int launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  p->lws = bp.lws;
+  p->lws_out = bp.lws_out;
+  p->groups = bp.groups;
+  p->baseline = bp.baseline;
+  p->cost = bp.cost;
+  p->ids = (const uint32_t*)e->dv_ids.p;
+  p->pos_of = (uint32_t*)e->dv_pos.p;
+  p->count = (uint32_t*)e->dv_kidx.p;
+  p->first = p->count + m;
+  p->cursor = p->first + m + 1;
+  p->l_count = (uint32_t*)e->dv_lidx.p;
+  p->l_first = p->l_count + nl;
+  p->l_cursor = p->l_first + nl + 1;
+  p->dense = (uint4*)e->dv_dense.p;
+  p->g_waves = (unsigned long long*)e->dv_gwaves.p;
+  p->out = (uint8_t*)e->dv_out.p;
+  p->counts = counts;
+  p->n_lws = nl;
+  p->n_groups = ng;
+  p->n_keys = nk;
+  p->m = m;
+  p->max_waves = max_waves;
+  p->cols = (m < max_waves ? m : max_waves) + 1u;
+  launched = lwse::launch_drain_waves(p, 0, e->sm_count, s, &cuda_err);
+  return count_launch(e, launched, cuda_err);
+}
+
+// The buffers for n_pairs restart pairs, directly after the synchronisation that read the count.
+static int reserve_drain_waves_pairs(lwse_engine* e, uint64_t n_pairs) {
+  // (every index is 32-bit, and the plan kernel's items are a key's pairs times the columns)
+  if (n_pairs > 0xFFFFFFFFull / (LWSE_DRAIN_WAVES_MAX + 1u)) return LWSE_ERR_OOM;
+  LWSE_CUDA(e, e->dv_pairs.reserve((size_t)n_pairs * 8 + 16));
+  LWSE_CUDA(e, e->dv_recs.reserve((size_t)n_pairs * 16 + 16));
+  return LWSE_OK;
+}
+
+// The walk in pair mode into dv_pairs, and p's pairs set for its pass 1.
+static int enqueue_drain_waves_pairs(lwse_engine* e, const lwse::DrainBudgetCostLaunch& bp, uint32_t n_pairs,
+                                     lwse::DrainWavesLaunch* p) {
+  int cuda_err = 0;
+  const int launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dv_pairs.p, n_pairs, e->sm_count,
+                                                        e->wf_stream, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  p->pairs = (const unsigned long long*)e->dv_pairs.p;
+  p->n_pairs = n_pairs;
+  p->recs = (uint4*)e->dv_recs.p;
+  return LWSE_OK;
+}
+
+// The scratch of n_dense touched LWS rows, reserved, zeroed and set in p for its pass 2.
+static int enqueue_drain_waves_dense(lwse_engine* e, uint32_t n_dense, lwse::DrainWavesLaunch* p) {
+  cudaStream_t s = e->wf_stream;
+  LWSE_CUDA(e, e->dv_lost.reserve((size_t)n_dense * p->cols * 4 + 16));
+  LWSE_CUDA(e, e->dv_rwaves.reserve((size_t)n_dense * 16 + 16));
+  LWSE_CUDA(e, e->dv_stamps.reserve((size_t)n_dense * 8 + 16));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lost.p, 0, (size_t)n_dense * p->cols * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_rwaves.p, 0, (size_t)n_dense * 16, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dv_stamps.p, 0, (size_t)n_dense * 8, s));
+  p->n_dense = n_dense;
+  p->lost = (uint32_t*)e->dv_lost.p;
+  p->row_waves = (unsigned long long*)e->dv_rwaves.p;
+  p->stamps = (uint32_t*)e->dv_stamps.p;
+  return LWSE_OK;
+}
+
 // Three host synchronisations, each sizing what follows: the restart pairs of every key (the drain budget's pass 0
 // counts them per key), then the touched LWS rows (the lost counters are sized by them, not by n_lws), then the
 // answer, read back with one copy.  Everything reads the resident tables and the baseline results in place.
@@ -2811,109 +2964,35 @@ LWSE_API int lwse_resident_drain_waves(lwse_engine* e, lwse_drain_waves_query* q
   if (q->reserved || q->max_waves == 0 || q->max_waves > LWSE_DRAIN_WAVES_MAX || !q->waves) return LWSE_ERR_INVALID_ARG;
   if (q->n_ids && (!q->ids || !q->keys)) return LWSE_ERR_INVALID_ARG;
   const bool by_domain = q->scope == LWSE_DRAIN_DOMAINS;
-  const uint32_t nn = e->n_nodes, nk = by_domain ? e->n_domains : nn, m = q->n_ids;
+  const uint32_t nk = by_domain ? e->n_domains : e->n_nodes, m = q->n_ids;
   const uint32_t nl = e->rn_lws, ng = e->rn_groups;
-  LWSE_CUDA(e, e->wf_stage.reserve((size_t)nk + 16));
-  uint8_t* seen = static_cast<uint8_t*>(e->wf_stage.h);
-  memset(seen, 0, nk);
-  for (uint32_t i = 0; i < m; i++) {
-    const uint32_t id = q->ids[i];
-    if (id >= nk || seen[id]) return LWSE_ERR_INVALID_ARG;  // out of range, or a duplicate
-    seen[id] = 1;
-  }
+  if (const int rc = check_key_ids(e, q->ids, m, nk); rc != LWSE_OK) return rc;
   if (e->xch_world > 0) return LWSE_ERR_UNSUPPORTED;  // (a plan is not a sum over ranks)
-  const uint32_t mw = q->max_waves;
-  const size_t keys_bytes = (size_t)m * sizeof(lwse_drain_wave_key);
-  const size_t out_bytes = 16 + keys_bytes + (size_t)mw * sizeof(lwse_drain_wave);
+  const size_t out_bytes = waves_answer_bytes<lwse_drain_wave_key, lwse_drain_wave>(m, q->max_waves);
   DeviceGuard guard(e->device);
   LWSE_CUDA(e, e->dv_cost.reserve((size_t)nk * sizeof(lwse_drain_budget_cost) + 16));
   LWSE_CUDA(e, e->dv_words.reserve(128));
   LWSE_CUDA(e, e->wf_words.reserve(128));
-  LWSE_CUDA(e, e->dv_ids.reserve((size_t)m * 4 + 16));
-  LWSE_CUDA(e, e->dv_pos.reserve((size_t)nk * 4 + 16));
-  LWSE_CUDA(e, e->dv_kidx.reserve(((size_t)m * 3 + 2) * 4 + 16));
-  LWSE_CUDA(e, e->dv_lidx.reserve(((size_t)nl * 3 + 2) * 4 + 16));
-  LWSE_CUDA(e, e->dv_dense.reserve((size_t)nl * 16 + 16));
-  LWSE_CUDA(e, e->dv_gwaves.reserve((size_t)ng * 8 + 16));
-  LWSE_CUDA(e, e->dv_out.reserve(out_bytes));
-  LWSE_CUDA(e, e->dv_host.reserve(out_bytes > (size_t)m * 4 ? out_bytes : (size_t)m * 4));
+  if (const int rc = reserve_drain_waves(e, m, nk, q->max_waves, out_bytes); rc != LWSE_OK) return rc;
   if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
   cudaStream_t s = e->wf_stream;
-  uint32_t* d_words = (uint32_t*)e->dv_words.p;  // [0..15] the walk's counters, [16..19] this call's (u64)
+  uint32_t* d_words = (uint32_t*)e->dv_words.p;  // [0..15] the walk's counters, [16..19] the chain's (u64)
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
-  if (m) {
-    memcpy(e->dv_host.h, q->ids, (size_t)m * 4);
-    LWSE_CUDA(e, cudaMemcpyAsync(e->dv_ids.p, e->dv_host.h, (size_t)m * 4, cudaMemcpyHostToDevice, s));
-  }
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_cost.p, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
   LWSE_CUDA(e, cudaMemsetAsync(d_words, 0, 128, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_pos.p, 0xFF, (size_t)nk * 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_kidx.p, 0, (size_t)m * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lidx.p, 0, (size_t)nl * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_gwaves.p, 0, (size_t)ng * 8, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_out.p, 0, out_bytes, s));
   // the key rows and their restart pairs: the drain budget's pass 0
-  lwse::DrainBudgetCostLaunch bp{};
-  bp.lws = (const lwse_lws_rec*)e->r_lws.p;
-  bp.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
-  bp.groups = (const lwse_group_rec*)e->r_groups.p;
-  bp.pod_state = (const uint8_t*)e->r_pst.p;
-  bp.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
-  bp.baseline = (const lwse_group_out*)e->r_group_out.p;
-  bp.nodes = (const lwse_node_rec*)e->nodes.p;
-  bp.occupancy = (const uint32_t*)e->r_occ.p;
-  bp.cost = (lwse_drain_budget_cost*)e->dv_cost.p;
-  bp.counts = d_words;
-  bp.n_pods = e->rn_pods;
-  bp.n_lws = nl;
-  bp.n_groups = ng;
-  bp.n_nodes = nn;
-  bp.n_domains = e->n_domains;
-  bp.n_keys = nk;
-  bp.by_domain = by_domain;
-  int cuda_err = 0;
-  int launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  const lwse::DrainBudgetCostLaunch bp = restart_walk(e, by_domain, (lwse_drain_budget_cost*)e->dv_cost.p, d_words);
   lwse::DrainWavesLaunch p{};
-  p.lws = bp.lws;
-  p.lws_out = bp.lws_out;
-  p.groups = bp.groups;
-  p.baseline = bp.baseline;
-  p.cost = bp.cost;
-  p.ids = (const uint32_t*)e->dv_ids.p;
-  p.pos_of = (uint32_t*)e->dv_pos.p;
-  p.count = (uint32_t*)e->dv_kidx.p;
-  p.first = p.count + m;
-  p.cursor = p.first + m + 1;
-  p.l_count = (uint32_t*)e->dv_lidx.p;
-  p.l_first = p.l_count + nl;
-  p.l_cursor = p.l_first + nl + 1;
-  p.dense = (uint4*)e->dv_dense.p;
-  p.g_waves = (unsigned long long*)e->dv_gwaves.p;
-  p.out = (uint8_t*)e->dv_out.p;
-  p.counts = reinterpret_cast<unsigned long long*>(d_words + 16);
-  p.n_lws = nl;
-  p.n_groups = ng;
-  p.n_keys = nk;
-  p.m = m;
-  p.max_waves = mw;
-  p.cols = (m < mw ? m : mw) + 1u;
-  launched = lwse::launch_drain_waves(&p, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_drain_waves_setup(e, bp, q->ids, m, q->max_waves, (unsigned long long*)(d_words + 16), &p);
+      rc != LWSE_OK)
+    return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words + 16, 8, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   uint64_t n_pairs = 0;
   memcpy(&n_pairs, words, 8);
-  // (every index is 32-bit, and the plan kernel's items are a key's pairs times the columns)
-  if (n_pairs > 0xFFFFFFFFull / (LWSE_DRAIN_WAVES_MAX + 1u)) return LWSE_ERR_OOM;
-  LWSE_CUDA(e, e->dv_pairs.reserve((size_t)n_pairs * 8 + 16));
-  LWSE_CUDA(e, e->dv_recs.reserve((size_t)n_pairs * 16 + 16));
-  launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dv_pairs.p, (uint32_t)n_pairs, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  p.pairs = (const unsigned long long*)e->dv_pairs.p;
-  p.n_pairs = (uint32_t)n_pairs;
-  p.recs = (uint4*)e->dv_recs.p;
-  launched = lwse::launch_drain_waves(&p, 1, e->sm_count, s, &cuda_err);
+  if (const int rc = reserve_drain_waves_pairs(e, n_pairs); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_drain_waves_pairs(e, bp, (uint32_t)n_pairs, &p); rc != LWSE_OK) return rc;
+  int cuda_err = 0;
+  int launched = lwse::launch_drain_waves(&p, 1, e->sm_count, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 64, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words + 16, d_words + 16, 16, cudaMemcpyDeviceToHost, s));
@@ -2922,37 +3001,153 @@ LWSE_API int lwse_resident_drain_waves(lwse_engine* e, lwse_drain_waves_query* q
   // (the walk found another pair count, or a bucket refused a pair: no answer rather than a wrong one)
   if (ng && words[8] != n_pairs) return LWSE_ERR_OOM;
   if (words[18] || words[19]) return LWSE_ERR_OOM;
-  const uint32_t n_dense = words[20];
-  LWSE_CUDA(e, e->dv_lost.reserve((size_t)n_dense * p.cols * 4 + 16));
-  LWSE_CUDA(e, e->dv_rwaves.reserve((size_t)n_dense * 16 + 16));
-  LWSE_CUDA(e, e->dv_stamps.reserve((size_t)n_dense * 8 + 16));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lost.p, 0, (size_t)n_dense * p.cols * 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_rwaves.p, 0, (size_t)n_dense * 16, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_stamps.p, 0, (size_t)n_dense * 8, s));
-  p.n_dense = n_dense;
-  p.lost = (uint32_t*)e->dv_lost.p;
-  p.row_waves = (unsigned long long*)e->dv_rwaves.p;
-  p.stamps = (uint32_t*)e->dv_stamps.p;
+  if (const int rc = enqueue_drain_waves_dense(e, words[20], &p); rc != LWSE_OK) return rc;
   launched = lwse::launch_drain_waves(&p, 2, e->sm_count, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(e->dv_host.h, p.out, out_bytes, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
-  const uint8_t* h = static_cast<const uint8_t*>(e->dv_host.h);
-  uint32_t totals[4];
-  memcpy(totals, h, 16);
-  if (m) memcpy(q->keys, h + 16, keys_bytes);
-  memcpy(q->waves, h + 16 + keys_bytes, (size_t)totals[0] * sizeof(lwse_drain_wave));
-  q->n_waves = totals[0];
-  q->n_planned = totals[1];
-  q->n_breaches_alone = totals[2];
-  q->n_no_wave = totals[3];
+  copy_waves_answer(e, q);
   return LWSE_OK;
 }
 
 // ---------------------------------------------------------------------------
 // Drain placement
 // ---------------------------------------------------------------------------
+// The drain placement chain, shared by lwse_resident_drain_place_cost and lwse_resident_drain_place_waves.  Its
+// steps enqueue on wf_stream and never synchronize.  The caller zeroes dp_words ([0..15] the chain's counters,
+// [16..31] its restart walk's) and issues every read-back.
+
+// The largest namespace's request count: the rows of the solve's per-CTA slices.
+static uint32_t largest_namespace(const lwse_engine* e) {
+  const uint32_t n_ns = e->rn_namespaces;
+  uint32_t max_ns = 1;
+  std::vector<uint32_t> per(n_ns, 0);
+  for (uint32_t r = 0; r < e->rn_reqs; r++)
+    if (e->r_req_ns[r] < n_ns) max_ns = std::max(max_ns, ++per[e->r_req_ns[r]]);
+  return max_ns;
+}
+
+// The chain's scratch for nk keys, before the snapshot.
+static int reserve_drain_place(lwse_engine* e, uint32_t nk) {
+  const uint32_t nd = e->n_domains, nr = e->rn_reqs, ng = e->rn_groups, n_ns = e->rn_namespaces;
+  LWSE_CUDA(e, e->dp_cost.reserve((size_t)nk * sizeof(lwse_drain_budget_cost) + 16));
+  LWSE_CUDA(e, e->dp_words.reserve(128));
+  LWSE_CUDA(e, e->dp_domfree.reserve((size_t)nd * 4 + 16));
+  LWSE_CUDA(e, e->dp_gidx.reserve(((size_t)ng * 3 + 2 + nr) * 4 + 16));
+  LWSE_CUDA(e, e->dp_uidx.reserve(((size_t)nk * 3 + 2) * 4 + 16));
+  LWSE_CUDA(e, e->dp_pos.reserve((size_t)nr * 4 + 16));
+  LWSE_CUDA(e, e->dp_rows.reserve((size_t)nk * sizeof(lwse_drain_place_cost) + 16));
+  LWSE_CUDA(e, e->dp_touched.reserve((size_t)n_ns + 16));
+  LWSE_CUDA(e, e->dp_round.reserve(lwse::place_ns_scratch_bytes(e->n_nodes, nd, nr, n_ns)));
+  if (e->node_index_stale) return reserve_node_index(e);  // (as the place what-if: a stale resident index is not read)
+  return LWSE_OK;
+}
+
+// The chain's scratch and the walk's key rows zeroed, the node index, every namespace's request index, the restart
+// walk's pass 0 (`bp`, into dp_cost with its counters at dp_words + 16), then the chain's pass 0 into p.
+static int enqueue_drain_place_setup(lwse_engine* e, const lwse::DrainBudgetCostLaunch& bp, lwse::DrainPlaceLaunch* p) {
+  const uint32_t nn = e->n_nodes, nd = e->n_domains, nr = e->rn_reqs, ng = e->rn_groups, n_ns = e->rn_namespaces;
+  const uint32_t nk = bp.n_keys;
+  const size_t round_bytes = lwse::place_ns_scratch_bytes(nn, nd, nr, n_ns);
+  cudaStream_t s = e->wf_stream;
+  LWSE_CUDA(e, cudaMemsetAsync(bp.cost, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_gidx.p, 0, (size_t)ng * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_uidx.p, 0, (size_t)nk * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_pos.p, 0xFF, (size_t)nr * 4 + 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_touched.p, 1, n_ns, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->dp_round.p, 0, round_bytes, s));  // (the index counts start at zero)
+  const uint32_t* dom_first = (const uint32_t*)e->dom_first.p;
+  const uint32_t* node_order = (const uint32_t*)e->node_order.p;
+  if (e->node_index_stale)
+    if (const int rc = own_node_index(e, (const lwse_node_rec*)e->nodes.p, s, &dom_first, &node_order, nullptr); rc != LWSE_OK)
+      return rc;
+  int cuda_err = 0;
+  int launched = lwse::launch_place_whatif_index((const lwse_place_req*)e->r_preq.p, nr, n_ns, (const uint8_t*)e->dp_touched.p,
+                                                 nn, nd, e->dp_round.p, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  // the restarted groups per key: the drain budget's pass 0 (key rows, the walk)
+  launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  p->nodes = (const lwse_node_rec*)e->nodes.p;
+  p->occupancy = (const uint32_t*)e->r_occ.p;
+  p->dom_first = dom_first;
+  p->node_order = node_order;
+  p->dom_free = (uint32_t*)e->dp_domfree.p;
+  p->reqs = (const lwse_place_req*)e->r_preq.p;
+  p->base = (const lwse_place_out*)e->r_pout.p;
+  p->cost = bp.cost;
+  p->n_nodes = nn;
+  p->n_domains = nd;
+  p->n_reqs = nr;
+  p->n_namespaces = n_ns;
+  p->n_groups = ng;
+  p->n_keys = nk;
+  p->by_domain = bp.by_domain;
+  p->g_count = (uint32_t*)e->dp_gidx.p;
+  p->g_first = p->g_count + ng;
+  p->g_cursor = p->g_first + ng + 1;
+  p->g_reqs = p->g_cursor + ng;  // (the pinned rows, at most nr)
+  p->u_count = (uint32_t*)e->dp_uidx.p;
+  p->u_first = p->u_count + nk;
+  p->u_cursor = p->u_first + nk + 1;
+  p->pos = (uint32_t*)e->dp_pos.p;
+  p->rows = (lwse_drain_place_cost*)e->dp_rows.p;
+  p->counts = (uint32_t*)e->dp_words.p;
+  p->round = e->dp_round.p;
+  p->round_bytes = round_bytes;
+  launched = lwse::launch_drain_place(p, 0, e->sm_count, s, &cuda_err);
+  return count_launch(e, launched, cuda_err);
+}
+
+// The walk in pair mode into dp_pairs (reserved by the caller after the count's synchronisation), then the chain's
+// pass 1: U_k counted and scanned.
+static int enqueue_drain_place_pairs(lwse_engine* e, const lwse::DrainBudgetCostLaunch& bp, uint32_t n_pairs,
+                                     lwse::DrainPlaceLaunch* p) {
+  int cuda_err = 0;
+  int launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dp_pairs.p, n_pairs, e->sm_count, e->wf_stream,
+                                                  &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  p->pairs = (const unsigned long long*)e->dp_pairs.p;
+  p->n_pairs = n_pairs;
+  launched = lwse::launch_drain_place(p, 1, e->sm_count, e->wf_stream, &cuda_err);
+  return count_launch(e, launched, cuda_err);
+}
+
+// The chain's pass 2 for n_unp unpinned rows and n_rule_b rule-(b) candidates, after the synchronisation that read
+// them: U_k, positions, capacities and every key's alone row.  The solve's slices (results, unpinned list and marks
+// per resident CTA) are sized from the largest namespace.  clamp_grid first clamps the grid to the items; the waves
+// plan does not, since its p->grid also sizes the per-key namespace round of its steps.
+static int enqueue_drain_place_solve(lwse_engine* e, uint32_t max_ns, uint32_t n_unp, uint32_t n_rule_b, bool clamp_grid,
+                                     lwse::DrainPlaceLaunch* p) {
+  const uint64_t item_cap = (uint64_t)n_unp + n_rule_b;
+  if (item_cap > (1ull << 30)) return LWSE_ERR_OOM;  // (the table index is 32-bit)
+  const uint64_t slots = table_slots(item_cap);
+  uint64_t grid = (uint64_t)e->sm_count * 2u;
+  if (clamp_grid && grid > item_cap) grid = item_cap ? item_cap : 1;
+  while (grid > 1 && grid * max_ns * (sizeof(lwse_place_out) + 5) > (1ull << 30)) grid >>= 1;
+  const size_t slice_out = align256((size_t)grid * max_ns * sizeof(lwse_place_out));
+  const size_t slice_unp = align256((size_t)grid * max_ns * 4);
+  LWSE_CUDA(e, e->dp_slices.reserve(slice_out + slice_unp + (size_t)grid * max_ns + 16));
+  LWSE_CUDA(e, e->dp_items.reserve((size_t)slots * 8 + (size_t)item_cap * 8 + 16));
+  LWSE_CUDA(e, e->dp_urows.reserve((size_t)n_unp * 4 + 16));
+  p->u_rows = (uint32_t*)e->dp_urows.p;
+  p->n_unpinned = n_unp;
+  p->item_keys = (unsigned long long*)e->dp_items.p;
+  p->item_mask = (uint32_t)(slots - 1);
+  p->items = reinterpret_cast<uint2*>(p->item_keys + slots);
+  p->item_capacity = (uint32_t)item_cap;
+  LWSE_CUDA(e, cudaMemsetAsync(p->item_keys, 0xFF, (size_t)slots * 8, e->wf_stream));
+  p->s_out = (lwse_place_out*)e->dp_slices.p;
+  p->s_unpinned = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(e->dp_slices.p) + slice_out);
+  p->s_marks = static_cast<uint8_t*>(e->dp_slices.p) + slice_out + slice_unp;
+  p->slice_rows = max_ns;
+  p->grid = (uint32_t)grid;
+  int cuda_err = 0;
+  const int launched = lwse::launch_drain_place(p, 2, e->sm_count, e->wf_stream, &cuda_err);
+  return count_launch(e, launched, cuda_err);
+}
+
 // Three host synchronisations, each sizing what follows: the restart pairs (the drain budget's pass 0 counts
 // them per key), then U_k and the rule-(b) candidates, then the answer.  Everything reads the resident tables,
 // the baseline group results and placement rows in place (nothing writes them while the call holds the mutex).
@@ -2966,157 +3161,31 @@ LWSE_API int lwse_resident_drain_place_cost(lwse_engine* e, uint32_t scope, lwse
   if (e->xch_world > 0 || e->rn_reqs >= (1u << 24) || !lwse::place_ns_supported(e->n_nodes, e->n_domains))
     return LWSE_ERR_UNSUPPORTED;
   const bool by_domain = scope == LWSE_DRAIN_DOMAINS;
-  const uint32_t nn = e->n_nodes, nd = e->n_domains, nr = e->rn_reqs, ng = e->rn_groups, n_ns = e->rn_namespaces;
-  const uint32_t nk = by_domain ? nd : nn;
-  uint32_t max_ns = 1;  // the largest namespace: the solve's per-CTA slices
-  {
-    std::vector<uint32_t> per(n_ns, 0);
-    for (uint32_t r = 0; r < nr; r++)
-      if (e->r_req_ns[r] < n_ns) max_ns = std::max(max_ns, ++per[e->r_req_ns[r]]);
-  }
-  const size_t round_bytes = lwse::place_ns_scratch_bytes(nn, nd, nr, n_ns);
+  const uint32_t nk = by_domain ? e->n_domains : e->n_nodes;
+  const uint32_t max_ns = largest_namespace(e);
   DeviceGuard guard(e->device);
-  LWSE_CUDA(e, e->dp_cost.reserve((size_t)nk * sizeof(lwse_drain_budget_cost) + 16));
-  LWSE_CUDA(e, e->dp_words.reserve(128));
   LWSE_CUDA(e, e->wf_words.reserve(256));  // (the counters, and |U| at word 32)
-  LWSE_CUDA(e, e->dp_domfree.reserve((size_t)nd * 4 + 16));
-  LWSE_CUDA(e, e->dp_gidx.reserve(((size_t)ng * 3 + 2 + nr) * 4 + 16));
-  LWSE_CUDA(e, e->dp_uidx.reserve(((size_t)nk * 3 + 2) * 4 + 16));
-  LWSE_CUDA(e, e->dp_pos.reserve((size_t)nr * 4 + 16));
-  LWSE_CUDA(e, e->dp_rows.reserve((size_t)nk * sizeof(lwse_drain_place_cost) + 16));
-  LWSE_CUDA(e, e->dp_touched.reserve((size_t)n_ns + 16));
-  LWSE_CUDA(e, e->dp_round.reserve(round_bytes));
-  const bool own_index = e->node_index_stale;  // (as the place what-if: a resident index behind the node rows is not read)
-  if (own_index) {
-    LWSE_CUDA(e, e->wf_dom_first.reserve(((size_t)nd + 1) * 4 + 16));
-    LWSE_CUDA(e, e->wf_node_order.reserve(((size_t)(nn + 255u) / 256u + 1u) * 1024u + 16));
-    LWSE_CUDA(e, e->wf_node_pos.reserve((size_t)nn * 4 + 16));
-    LWSE_CUDA(e, e->wf_node_ix.reserve(lwse::node_index_scratch_bytes(nd)));
-  }
+  if (const int rc = reserve_drain_place(e, nk); rc != LWSE_OK) return rc;
   if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
   cudaStream_t s = e->wf_stream;
   uint32_t* d_words = (uint32_t*)e->dp_words.p;  // [0..15] this call's counters, [16..31] the walk's
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_cost.p, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
   LWSE_CUDA(e, cudaMemsetAsync(d_words, 0, 128, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_gidx.p, 0, (size_t)ng * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_uidx.p, 0, (size_t)nk * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_pos.p, 0xFF, (size_t)nr * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_touched.p, 1, n_ns, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_round.p, 0, round_bytes, s));  // (the index counts start at zero)
-  int cuda_err = 0;
-  const uint32_t* dom_first = (const uint32_t*)e->dom_first.p;
-  const uint32_t* node_order = (const uint32_t*)e->node_order.p;
-  if (own_index) {
-    const size_t ix_bytes = lwse::node_index_scratch_bytes(nd);
-    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_ix.p, 0, ix_bytes, s));
-    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_order.p, 0, ((size_t)(nn + 255u) / 256u + 1u) * 1024u, s));
-    const int launched = lwse::launch_node_index((const lwse_node_rec*)e->nodes.p, nn, nd, (uint32_t*)e->wf_dom_first.p,
-                                                 (uint32_t*)e->wf_node_order.p, (uint32_t*)e->wf_node_pos.p, e->wf_node_ix.p,
-                                                 e->sm_count, s, false, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-    dom_first = (const uint32_t*)e->wf_dom_first.p;
-    node_order = (const uint32_t*)e->wf_node_order.p;
-  }
-  {
-    const int launched = lwse::launch_place_whatif_index((const lwse_place_req*)e->r_preq.p, nr, n_ns, (const uint8_t*)e->dp_touched.p,
-                                                         nn, nd, e->dp_round.p, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  }
-  // the restarted groups per key: the drain budget's pass 0 (key rows, the walk)
-  lwse::DrainBudgetCostLaunch bp{};
-  bp.lws = (const lwse_lws_rec*)e->r_lws.p;
-  bp.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
-  bp.groups = (const lwse_group_rec*)e->r_groups.p;
-  bp.pod_state = (const uint8_t*)e->r_pst.p;
-  bp.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
-  bp.baseline = (const lwse_group_out*)e->r_group_out.p;
-  bp.nodes = (const lwse_node_rec*)e->nodes.p;
-  bp.occupancy = (const uint32_t*)e->r_occ.p;
-  bp.cost = (lwse_drain_budget_cost*)e->dp_cost.p;
-  bp.counts = d_words + 16;
-  bp.n_pods = e->rn_pods;
-  bp.n_lws = e->rn_lws;
-  bp.n_groups = ng;
-  bp.n_nodes = nn;
-  bp.n_domains = nd;
-  bp.n_keys = nk;
-  bp.by_domain = by_domain;
-  int launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  const lwse::DrainBudgetCostLaunch bp = restart_walk(e, by_domain, (lwse_drain_budget_cost*)e->dp_cost.p, d_words + 16);
   lwse::DrainPlaceLaunch p{};
-  p.nodes = (const lwse_node_rec*)e->nodes.p;
-  p.occupancy = (const uint32_t*)e->r_occ.p;
-  p.dom_first = dom_first;
-  p.node_order = node_order;
-  p.dom_free = (uint32_t*)e->dp_domfree.p;
-  p.reqs = (const lwse_place_req*)e->r_preq.p;
-  p.base = (const lwse_place_out*)e->r_pout.p;
-  p.cost = (const lwse_drain_budget_cost*)e->dp_cost.p;
-  p.n_nodes = nn;
-  p.n_domains = nd;
-  p.n_reqs = nr;
-  p.n_namespaces = n_ns;
-  p.n_groups = ng;
-  p.n_keys = nk;
-  p.by_domain = by_domain;
-  p.g_count = (uint32_t*)e->dp_gidx.p;
-  p.g_first = p.g_count + ng;
-  p.g_cursor = p.g_first + ng + 1;
-  p.u_count = (uint32_t*)e->dp_uidx.p;
-  p.u_first = p.u_count + nk;
-  p.u_cursor = p.u_first + nk + 1;
-  p.pos = (uint32_t*)e->dp_pos.p;
-  p.rows = (lwse_drain_place_cost*)e->dp_rows.p;
-  p.counts = d_words;
-  p.round = e->dp_round.p;
-  p.round_bytes = round_bytes;
-  p.g_reqs = p.g_cursor + ng;  // (the pinned rows, at most nr)
-  launched = lwse::launch_drain_place(&p, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_drain_place_setup(e, bp, &p); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 32, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   const uint32_t n_pairs = words[6];
   // the restart pairs, then U_k counted and scanned
   LWSE_CUDA(e, e->dp_pairs.reserve((size_t)n_pairs * 8 + 16));
-  launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dp_pairs.p, n_pairs, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  p.pairs = (const unsigned long long*)e->dp_pairs.p;
-  p.n_pairs = n_pairs;
-  launched = lwse::launch_drain_place(&p, 1, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_drain_place_pairs(e, bp, n_pairs, &p); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 128, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words + 32, p.u_first + nk, 4, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   if (words[16 + 8] != n_pairs) return LWSE_ERR_OOM;  // (the walk found another pair count: no answer rather than a wrong one)
-  const uint32_t n_unp = words[32];
-  const uint64_t item_cap = (uint64_t)n_unp + words[3];
-  if (item_cap > (1ull << 30)) return LWSE_ERR_OOM;  // (the table index is 32-bit)
-  uint64_t slots = 256;
-  while (slots < 2 * item_cap) slots <<= 1;
-  // the solve's slices: results, unpinned list and marks per resident CTA, sized from the largest namespace
-  uint64_t grid = (uint64_t)e->sm_count * 2u;
-  if (grid > item_cap) grid = item_cap ? item_cap : 1;
-  while (grid > 1 && grid * max_ns * (sizeof(lwse_place_out) + 5) > (1ull << 30)) grid >>= 1;
-  const size_t slice_out = align256((size_t)grid * max_ns * sizeof(lwse_place_out));
-  const size_t slice_unp = align256((size_t)grid * max_ns * 4);
-  LWSE_CUDA(e, e->dp_slices.reserve(slice_out + slice_unp + (size_t)grid * max_ns + 16));
-  LWSE_CUDA(e, e->dp_items.reserve((size_t)slots * 8 + (size_t)item_cap * 8 + 16));
-  LWSE_CUDA(e, e->dp_urows.reserve((size_t)n_unp * 4 + 16));
-  p.u_rows = (uint32_t*)e->dp_urows.p;
-  p.n_unpinned = n_unp;
-  p.item_keys = (unsigned long long*)e->dp_items.p;
-  p.item_mask = (uint32_t)(slots - 1);
-  p.items = reinterpret_cast<uint2*>(p.item_keys + slots);
-  p.item_capacity = (uint32_t)item_cap;
-  LWSE_CUDA(e, cudaMemsetAsync(p.item_keys, 0xFF, (size_t)slots * 8, s));
-  p.s_out = (lwse_place_out*)e->dp_slices.p;
-  p.s_unpinned = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(e->dp_slices.p) + slice_out);
-  p.s_marks = static_cast<uint8_t*>(e->dp_slices.p) + slice_out + slice_unp;
-  p.slice_rows = max_ns;
-  p.grid = (uint32_t)grid;
-  launched = lwse::launch_drain_place(&p, 2, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_drain_place_solve(e, max_ns, words[32], words[3], /*clamp_grid=*/true, &p); rc != LWSE_OK)
+    return rc;
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(out, p.rows, (size_t)nk * sizeof(lwse_drain_place_cost), cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 64, cudaMemcpyDeviceToHost, s));
@@ -3143,50 +3212,17 @@ LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_wa
   const bool by_domain = q->scope == LWSE_DRAIN_DOMAINS;
   const uint32_t nn = e->n_nodes, nd = e->n_domains, nk = by_domain ? nd : nn, m = q->n_ids;
   const uint32_t nl = e->rn_lws, ng = e->rn_groups, nr = e->rn_reqs, n_ns = e->rn_namespaces;
-  LWSE_CUDA(e, e->wf_stage.reserve((size_t)nk + 16));
-  uint8_t* seen = static_cast<uint8_t*>(e->wf_stage.h);
-  memset(seen, 0, nk);
-  for (uint32_t i = 0; i < m; i++) {
-    const uint32_t id = q->ids[i];
-    if (id >= nk || seen[id]) return LWSE_ERR_INVALID_ARG;
-    seen[id] = 1;
-  }
+  if (const int rc = check_key_ids(e, q->ids, m, nk); rc != LWSE_OK) return rc;
   if (e->xch_world > 0 || nr >= (1u << 24) || !lwse::place_ns_supported(nn, nd)) return LWSE_ERR_UNSUPPORTED;
   const uint32_t mw = q->max_waves;
-  uint32_t max_ns = 1;
-  {
-    std::vector<uint32_t> per(n_ns, 0);
-    for (uint32_t r = 0; r < nr; r++)
-      if (e->r_req_ns[r] < n_ns) max_ns = std::max(max_ns, ++per[e->r_req_ns[r]]);
-  }
-  const size_t wkeys_bytes = (size_t)m * sizeof(lwse_drain_wave_key);
-  const size_t wout_bytes = 16 + wkeys_bytes + (size_t)mw * sizeof(lwse_drain_wave);
-  const size_t keys_bytes = (size_t)m * sizeof(lwse_drain_place_wave_key);
-  const size_t out_bytes = 16 + keys_bytes + (size_t)mw * sizeof(lwse_drain_place_wave);
-  const size_t round_bytes = lwse::place_ns_scratch_bytes(nn, nd, nr, n_ns);
+  const uint32_t max_ns = largest_namespace(e);
+  const size_t out_bytes = waves_answer_bytes<lwse_drain_place_wave_key, lwse_drain_place_wave>(m, mw);
   DeviceGuard guard(e->device);
-  // the drain waves' scratch
   LWSE_CUDA(e, e->dv_cost.reserve((size_t)nk * sizeof(lwse_drain_budget_cost) + 16));
   LWSE_CUDA(e, e->dv_words.reserve(128));
   LWSE_CUDA(e, e->wf_words.reserve(256));
-  LWSE_CUDA(e, e->dv_ids.reserve((size_t)m * 4 + 16));
-  LWSE_CUDA(e, e->dv_pos.reserve((size_t)nk * 4 + 16));
-  LWSE_CUDA(e, e->dv_kidx.reserve(((size_t)m * 3 + 2) * 4 + 16));
-  LWSE_CUDA(e, e->dv_lidx.reserve(((size_t)nl * 3 + 2) * 4 + 16));
-  LWSE_CUDA(e, e->dv_dense.reserve((size_t)nl * 16 + 16));
-  LWSE_CUDA(e, e->dv_gwaves.reserve((size_t)ng * 8 + 16));
-  LWSE_CUDA(e, e->dv_out.reserve(wout_bytes));
-  LWSE_CUDA(e, e->dv_host.reserve(std::max(out_bytes, (size_t)m * 4)));
-  // the drain placement's scratch
-  LWSE_CUDA(e, e->dp_cost.reserve((size_t)nk * sizeof(lwse_drain_budget_cost) + 16));
-  LWSE_CUDA(e, e->dp_words.reserve(128));
-  LWSE_CUDA(e, e->dp_domfree.reserve((size_t)nd * 4 + 16));
-  LWSE_CUDA(e, e->dp_gidx.reserve(((size_t)ng * 3 + 2 + nr) * 4 + 16));
-  LWSE_CUDA(e, e->dp_uidx.reserve(((size_t)nk * 3 + 2) * 4 + 16));
-  LWSE_CUDA(e, e->dp_pos.reserve((size_t)nr * 4 + 16));
-  LWSE_CUDA(e, e->dp_rows.reserve((size_t)nk * sizeof(lwse_drain_place_cost) + 16));
-  LWSE_CUDA(e, e->dp_touched.reserve((size_t)n_ns + 16));
-  LWSE_CUDA(e, e->dp_round.reserve(round_bytes));
+  if (const int rc = reserve_drain_waves(e, m, nk, mw, out_bytes); rc != LWSE_OK) return rc;
+  if (const int rc = reserve_drain_place(e, nk); rc != LWSE_OK) return rc;
   // this call's
   const size_t small_bytes = (size_t)LWSE_DRAIN_WAVES_MAX * 16 * 4 * 3 + (size_t)LWSE_DRAIN_WAVES_MAX * 4 + (size_t)m * 4;
   LWSE_CUDA(e, e->dq_state.reserve(sizeof(lwse::DpwState) + 16));
@@ -3199,136 +3235,24 @@ LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_wa
   LWSE_CUDA(e, e->dq_items.reserve((size_t)LWSE_DRAIN_WAVES_MAX * n_ns * 8 + 16));
   LWSE_CUDA(e, e->dq_dix.reserve(((size_t)nd * 3 + 2 + nr) * 4 + 16));
   LWSE_CUDA(e, e->dq_out.reserve(out_bytes));
-  const bool own_index = e->node_index_stale;
-  if (own_index) {
-    LWSE_CUDA(e, e->wf_dom_first.reserve(((size_t)nd + 1) * 4 + 16));
-    LWSE_CUDA(e, e->wf_node_order.reserve(((size_t)(nn + 255u) / 256u + 1u) * 1024u + 16));
-    LWSE_CUDA(e, e->wf_node_pos.reserve((size_t)nn * 4 + 16));
-    LWSE_CUDA(e, e->wf_node_ix.reserve(lwse::node_index_scratch_bytes(nd)));
-  }
   if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
   cudaStream_t s = e->wf_stream;
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
   int cuda_err = 0;
-  // ---- the drain waves chain up to its dense rows (lwse_resident_drain_waves) ----
+  // ---- the drain waves chain up to its pass 0 (lwse_resident_drain_waves) ----
   uint32_t* v_words = (uint32_t*)e->dv_words.p;
-  if (m) {
-    memcpy(e->dv_host.h, q->ids, (size_t)m * 4);
-    LWSE_CUDA(e, cudaMemcpyAsync(e->dv_ids.p, e->dv_host.h, (size_t)m * 4, cudaMemcpyHostToDevice, s));
-  }
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_cost.p, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
   LWSE_CUDA(e, cudaMemsetAsync(v_words, 0, 128, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_pos.p, 0xFF, (size_t)nk * 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_kidx.p, 0, (size_t)m * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lidx.p, 0, (size_t)nl * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_gwaves.p, 0, (size_t)ng * 8, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_out.p, 0, wout_bytes, s));
-  lwse::DrainBudgetCostLaunch bp{};
-  bp.lws = (const lwse_lws_rec*)e->r_lws.p;
-  bp.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
-  bp.groups = (const lwse_group_rec*)e->r_groups.p;
-  bp.pod_state = (const uint8_t*)e->r_pst.p;
-  bp.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
-  bp.baseline = (const lwse_group_out*)e->r_group_out.p;
-  bp.nodes = (const lwse_node_rec*)e->nodes.p;
-  bp.occupancy = (const uint32_t*)e->r_occ.p;
-  bp.cost = (lwse_drain_budget_cost*)e->dv_cost.p;
-  bp.counts = v_words;
-  bp.n_pods = e->rn_pods;
-  bp.n_lws = nl;
-  bp.n_groups = ng;
-  bp.n_nodes = nn;
-  bp.n_domains = nd;
-  bp.n_keys = nk;
-  bp.by_domain = by_domain;
-  int launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  const lwse::DrainBudgetCostLaunch bp = restart_walk(e, by_domain, (lwse_drain_budget_cost*)e->dv_cost.p, v_words);
   lwse::DrainPlaceWavesLaunch d{};
   lwse::DrainWavesLaunch& w = d.w;
-  w.lws = bp.lws;
-  w.lws_out = bp.lws_out;
-  w.groups = bp.groups;
-  w.baseline = bp.baseline;
-  w.cost = bp.cost;
-  w.ids = (const uint32_t*)e->dv_ids.p;
-  w.pos_of = (uint32_t*)e->dv_pos.p;
-  w.count = (uint32_t*)e->dv_kidx.p;
-  w.first = w.count + m;
-  w.cursor = w.first + m + 1;
-  w.l_count = (uint32_t*)e->dv_lidx.p;
-  w.l_first = w.l_count + nl;
-  w.l_cursor = w.l_first + nl + 1;
-  w.dense = (uint4*)e->dv_dense.p;
-  w.g_waves = (unsigned long long*)e->dv_gwaves.p;
-  w.out = (uint8_t*)e->dv_out.p;
-  w.counts = reinterpret_cast<unsigned long long*>(v_words + 16);
-  w.n_lws = nl;
-  w.n_groups = ng;
-  w.n_keys = nk;
-  w.m = m;
-  w.max_waves = mw;
-  w.cols = (m < mw ? m : mw) + 1u;
-  launched = lwse::launch_drain_waves(&w, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_drain_waves_setup(e, bp, q->ids, m, mw, (unsigned long long*)(v_words + 16), &w); rc != LWSE_OK)
+    return rc;
   // ---- the drain placement's pass 0 (lwse_resident_drain_place_cost) ----
   uint32_t* p_words = (uint32_t*)e->dp_words.p;
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_cost.p, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
   LWSE_CUDA(e, cudaMemsetAsync(p_words, 0, 128, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_gidx.p, 0, (size_t)ng * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_uidx.p, 0, (size_t)nk * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_pos.p, 0xFF, (size_t)nr * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_touched.p, 1, n_ns, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dp_round.p, 0, round_bytes, s));
-  const uint32_t* dom_first = (const uint32_t*)e->dom_first.p;
-  const uint32_t* node_order = (const uint32_t*)e->node_order.p;
-  if (own_index) {
-    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_ix.p, 0, lwse::node_index_scratch_bytes(nd), s));
-    LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_order.p, 0, ((size_t)(nn + 255u) / 256u + 1u) * 1024u, s));
-    launched = lwse::launch_node_index((const lwse_node_rec*)e->nodes.p, nn, nd, (uint32_t*)e->wf_dom_first.p,
-                                       (uint32_t*)e->wf_node_order.p, (uint32_t*)e->wf_node_pos.p, e->wf_node_ix.p, e->sm_count, s,
-                                       false, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-    dom_first = (const uint32_t*)e->wf_dom_first.p;
-    node_order = (const uint32_t*)e->wf_node_order.p;
-  }
-  launched = lwse::launch_place_whatif_index((const lwse_place_req*)e->r_preq.p, nr, n_ns, (const uint8_t*)e->dp_touched.p, nn, nd,
-                                             e->dp_round.p, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  lwse::DrainBudgetCostLaunch pb = bp;
-  pb.cost = (lwse_drain_budget_cost*)e->dp_cost.p;
-  pb.counts = p_words + 16;
-  launched = lwse::launch_drain_budget_cost(&pb, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  const lwse::DrainBudgetCostLaunch pb = restart_walk(e, by_domain, (lwse_drain_budget_cost*)e->dp_cost.p, p_words + 16);
   lwse::DrainPlaceLaunch& p = d.p;
-  p.nodes = (const lwse_node_rec*)e->nodes.p;
-  p.occupancy = (const uint32_t*)e->r_occ.p;
-  p.dom_first = dom_first;
-  p.node_order = node_order;
-  p.dom_free = (uint32_t*)e->dp_domfree.p;
-  p.reqs = (const lwse_place_req*)e->r_preq.p;
-  p.base = (const lwse_place_out*)e->r_pout.p;
-  p.cost = (const lwse_drain_budget_cost*)e->dp_cost.p;
-  p.n_nodes = nn;
-  p.n_domains = nd;
-  p.n_reqs = nr;
-  p.n_namespaces = n_ns;
-  p.n_groups = ng;
-  p.n_keys = nk;
-  p.by_domain = by_domain;
-  p.g_count = (uint32_t*)e->dp_gidx.p;
-  p.g_first = p.g_count + ng;
-  p.g_cursor = p.g_first + ng + 1;
-  p.g_reqs = p.g_cursor + ng;
-  p.u_count = (uint32_t*)e->dp_uidx.p;
-  p.u_first = p.u_count + nk;
-  p.u_cursor = p.u_first + nk + 1;
-  p.pos = (uint32_t*)e->dp_pos.p;
-  p.rows = (lwse_drain_place_cost*)e->dp_rows.p;
-  p.counts = p_words;
-  p.round = e->dp_round.p;
-  p.round_bytes = round_bytes;
-  launched = lwse::launch_drain_place(&p, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_drain_place_setup(e, pb, &p); rc != LWSE_OK) return rc;
   // first synchronisation: the pair totals of both chains (the same walk)
   LWSE_CUDA(e, cudaMemcpyAsync(words, v_words + 16, 8, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words + 2, p_words, 32, cudaMemcpyDeviceToHost, s));
@@ -3336,23 +3260,12 @@ LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_wa
   uint64_t n_pairs = 0;
   memcpy(&n_pairs, words, 8);
   const uint32_t all_pairs = words[2 + 6];
-  if (n_pairs > 0xFFFFFFFFull / (LWSE_DRAIN_WAVES_MAX + 1u)) return LWSE_ERR_OOM;
-  LWSE_CUDA(e, e->dv_pairs.reserve((size_t)n_pairs * 8 + 16));
-  LWSE_CUDA(e, e->dv_recs.reserve((size_t)n_pairs * 16 + 16));
+  if (const int rc = reserve_drain_waves_pairs(e, n_pairs); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, e->dp_pairs.reserve((size_t)all_pairs * 8 + 16));
-  launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dv_pairs.p, (uint32_t)n_pairs, e->sm_count, s, &cuda_err);
+  if (const int rc = enqueue_drain_waves_pairs(e, bp, (uint32_t)n_pairs, &w); rc != LWSE_OK) return rc;
+  int launched = lwse::launch_drain_waves(&w, 1, e->sm_count, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  w.pairs = (const unsigned long long*)e->dv_pairs.p;
-  w.n_pairs = (uint32_t)n_pairs;
-  w.recs = (uint4*)e->dv_recs.p;
-  launched = lwse::launch_drain_waves(&w, 1, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  launched = lwse::launch_drain_restart_pairs(&pb, (unsigned long long*)e->dp_pairs.p, all_pairs, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  p.pairs = (const unsigned long long*)e->dp_pairs.p;
-  p.n_pairs = all_pairs;
-  launched = lwse::launch_drain_place(&p, 1, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_drain_place_pairs(e, pb, all_pairs, &p); rc != LWSE_OK) return rc;
   // second synchronisation: the touched rows, |U| and the rule-(b) count
   LWSE_CUDA(e, cudaMemcpyAsync(words, v_words, 64, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words + 16, v_words + 16, 16, cudaMemcpyDeviceToHost, s));
@@ -3363,44 +3276,10 @@ LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_wa
   if (ng && words[8] != n_pairs) return LWSE_ERR_OOM;
   if (words[18] || words[19]) return LWSE_ERR_OOM;
   if (words[32 + 16 + 8] != all_pairs) return LWSE_ERR_OOM;
-  const uint32_t n_dense = words[20];
-  LWSE_CUDA(e, e->dv_lost.reserve((size_t)n_dense * w.cols * 4 + 16));
-  LWSE_CUDA(e, e->dv_rwaves.reserve((size_t)n_dense * 16 + 16));
-  LWSE_CUDA(e, e->dv_stamps.reserve((size_t)n_dense * 8 + 16));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lost.p, 0, (size_t)n_dense * w.cols * 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_rwaves.p, 0, (size_t)n_dense * 16, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_stamps.p, 0, (size_t)n_dense * 8, s));
-  w.n_dense = n_dense;
-  w.lost = (uint32_t*)e->dv_lost.p;
-  w.row_waves = (unsigned long long*)e->dv_rwaves.p;
-  w.stamps = (uint32_t*)e->dv_stamps.p;
+  if (const int rc = enqueue_drain_waves_dense(e, words[20], &w); rc != LWSE_OK) return rc;
   // the drain placement's pass 2: U_k, positions, capacities and every key's alone row
-  const uint32_t n_unp = words[64];
-  const uint64_t item_cap = (uint64_t)n_unp + words[32 + 3];
-  if (item_cap > (1ull << 30)) return LWSE_ERR_OOM;
-  uint64_t slots = 256;
-  while (slots < 2 * item_cap) slots <<= 1;
-  uint64_t grid = (uint64_t)e->sm_count * 2u;
-  while (grid > 1 && grid * max_ns * (sizeof(lwse_place_out) + 5) > (1ull << 30)) grid >>= 1;
-  const size_t slice_out = align256((size_t)grid * max_ns * sizeof(lwse_place_out));
-  const size_t slice_unp = align256((size_t)grid * max_ns * 4);
-  LWSE_CUDA(e, e->dp_slices.reserve(slice_out + slice_unp + (size_t)grid * max_ns + 16));
-  LWSE_CUDA(e, e->dp_items.reserve((size_t)slots * 8 + (size_t)item_cap * 8 + 16));
-  LWSE_CUDA(e, e->dp_urows.reserve((size_t)n_unp * 4 + 16));
-  p.u_rows = (uint32_t*)e->dp_urows.p;
-  p.n_unpinned = n_unp;
-  p.item_keys = (unsigned long long*)e->dp_items.p;
-  p.item_mask = (uint32_t)(slots - 1);
-  p.items = reinterpret_cast<uint2*>(p.item_keys + slots);
-  p.item_capacity = (uint32_t)item_cap;
-  LWSE_CUDA(e, cudaMemsetAsync(p.item_keys, 0xFF, (size_t)slots * 8, s));
-  p.s_out = (lwse_place_out*)e->dp_slices.p;
-  p.s_unpinned = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(e->dp_slices.p) + slice_out);
-  p.s_marks = static_cast<uint8_t*>(e->dp_slices.p) + slice_out + slice_unp;
-  p.slice_rows = max_ns;
-  p.grid = (uint32_t)grid;
-  launched = lwse::launch_drain_place(&p, 2, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_drain_place_solve(e, max_ns, words[64], words[32 + 3], /*clamp_grid=*/false, &p); rc != LWSE_OK)
+    return rc;
   // ---- this call's state, the domain index, the steps ----
   uint8_t* small = static_cast<uint8_t*>(e->dq_small.p);
   LWSE_CUDA(e, cudaMemsetAsync(e->dq_state.p, 0, sizeof(lwse::DpwState), s));
@@ -3459,15 +3338,7 @@ LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_wa
   LWSE_CUDA(e, cudaMemcpyAsync(words + 16, &d.st->refused, 4, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   if (words[5] || words[16]) return LWSE_ERR_OOM;  // an item a table refused
-  const uint8_t* h = static_cast<const uint8_t*>(e->dv_host.h);
-  uint32_t totals[4];
-  memcpy(totals, h, 16);
-  if (m) memcpy(q->keys, h + 16, keys_bytes);
-  memcpy(q->waves, h + 16 + keys_bytes, (size_t)totals[0] * sizeof(lwse_drain_place_wave));
-  q->n_waves = totals[0];
-  q->n_planned = totals[1];
-  q->n_breaches_alone = totals[2];
-  q->n_no_wave = totals[3];
+  copy_waves_answer(e, q);
   return LWSE_OK;
 }
 
@@ -3642,24 +3513,7 @@ LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds
   launched = lwse::launch_index_scan(d_count, d_first, d_cursor, nl, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   // the drain budget's (LWS, key) table: vals.y = lost(L, key)
-  lwse::DrainBudgetCostLaunch p{};
-  p.lws = (const lwse_lws_rec*)e->r_lws.p;
-  p.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
-  p.groups = (const lwse_group_rec*)e->r_groups.p;
-  p.pod_state = (const uint8_t*)e->r_pst.p;
-  p.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
-  p.baseline = (const lwse_group_out*)e->r_group_out.p;
-  p.nodes = (const lwse_node_rec*)e->nodes.p;
-  p.occupancy = (const uint32_t*)e->r_occ.p;
-  p.cost = (lwse_drain_budget_cost*)e->dr_bcost.p;
-  p.counts = d_words;
-  p.n_pods = e->rn_pods;
-  p.n_lws = nl;
-  p.n_groups = e->rn_groups;
-  p.n_nodes = nn;
-  p.n_domains = e->n_domains;
-  p.n_keys = n_keys;
-  p.by_domain = by_domain;
+  lwse::DrainBudgetCostLaunch p = restart_walk(e, by_domain, (lwse_drain_budget_cost*)e->dr_bcost.p, d_words);
   lwse::DsDrainCostLaunch c{};
   c.first = d_first;
   c.before = t.ds_out;
@@ -3686,8 +3540,7 @@ LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds
                                          true, e->sm_count, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   if (pairs) {
-    uint64_t slots = 256;
-    while (slots < 2 * pairs) slots <<= 1;
+    const uint64_t slots = table_slots(pairs);
     LWSE_CUDA(e, e->dr_table.reserve((size_t)slots * (sizeof(unsigned long long) + sizeof(uint4))));
     p.keys = (unsigned long long*)e->dr_table.p;
     p.vals = reinterpret_cast<uint4*>(p.keys + slots);
@@ -3746,22 +3599,12 @@ LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_qu
   if (q->constraints == 0 || (q->constraints & ~LWSE_DSW_ALL)) return LWSE_ERR_INVALID_ARG;
   if (q->n_ids && (!q->ids || !q->keys)) return LWSE_ERR_INVALID_ARG;
   const bool by_domain = q->scope == LWSE_DRAIN_DOMAINS;
-  const uint32_t nn = e->n_nodes, nk = by_domain ? e->n_domains : nn, m = q->n_ids;
+  const uint32_t nk = by_domain ? e->n_domains : e->n_nodes, m = q->n_ids;
   const uint32_t nl = e->rn_lws, ng = e->rn_groups;
-  LWSE_CUDA(e, e->wf_stage.reserve((size_t)nk + 16));
-  uint8_t* seen = static_cast<uint8_t*>(e->wf_stage.h);
-  memset(seen, 0, nk);
-  for (uint32_t i = 0; i < m; i++) {
-    const uint32_t id = q->ids[i];
-    if (id >= nk || seen[id]) return LWSE_ERR_INVALID_ARG;  // out of range, or a duplicate
-    seen[id] = 1;
-  }
+  if (const int rc = check_key_ids(e, q->ids, m, nk); rc != LWSE_OK) return rc;
   if (e->xch_world > 0) return LWSE_ERR_UNSUPPORTED;  // (a plan is not a sum over ranks)
   const uint32_t mw = q->max_waves;
-  const size_t plan_bytes = 16 + (size_t)m * sizeof(lwse_drain_wave_key) + (size_t)mw * sizeof(lwse_drain_wave);
-  const size_t keys_bytes = (size_t)m * sizeof(lwse_ds_drain_wave_key);
-  const size_t out_bytes = 16 + keys_bytes + (size_t)mw * sizeof(lwse_ds_drain_wave);
-  const size_t host_bytes = out_bytes > (size_t)m * 4 ? out_bytes : (size_t)m * 4;
+  const size_t out_bytes = waves_answer_bytes<lwse_ds_drain_wave_key, lwse_ds_drain_wave>(m, mw);
   DeviceGuard guard(e->device);
   if (const int rc = reserve_ds_drain_outputs(e, 1); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, e->dr_bcost.reserve((size_t)nk * sizeof(lwse_drain_budget_cost) + 16));
@@ -3769,16 +3612,9 @@ LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_qu
   LWSE_CUDA(e, e->dd_index.reserve((size_t)(nl + 1) * 3 * 4 + 16));
   LWSE_CUDA(e, e->dv_words.reserve(128));
   LWSE_CUDA(e, e->wf_words.reserve(192));
-  LWSE_CUDA(e, e->dv_ids.reserve((size_t)m * 4 + 16));
-  LWSE_CUDA(e, e->dv_pos.reserve((size_t)nk * 4 + 16));
-  LWSE_CUDA(e, e->dv_kidx.reserve(((size_t)m * 3 + 2) * 4 + 16));
-  LWSE_CUDA(e, e->dv_lidx.reserve(((size_t)nl * 3 + 2) * 4 + 16));
-  LWSE_CUDA(e, e->dv_dense.reserve((size_t)nl * 16 + 16));
-  LWSE_CUDA(e, e->dv_gwaves.reserve((size_t)ng * 8 + 16));
-  LWSE_CUDA(e, e->dv_out.reserve(plan_bytes));
+  if (const int rc = reserve_drain_waves(e, m, nk, mw, out_bytes); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, e->dx_caps.reserve((size_t)nl * 4 + 16));
   LWSE_CUDA(e, e->dx_out.reserve(out_bytes));
-  LWSE_CUDA(e, e->dv_host.reserve(host_bytes));
   if (const int rc = ds_drain_begin_locked(e); rc != LWSE_OK) return rc;
   cudaStream_t s = e->wf_stream;
   uint32_t* d_words = (uint32_t*)e->dv_words.p;
@@ -3786,19 +3622,9 @@ LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_qu
   uint32_t* d_count = (uint32_t*)e->dd_index.p;  // the reverse link index (count | first | cursor)
   uint32_t* d_first = d_count + (nl + 1);
   uint32_t* d_cursor = d_first + (nl + 1);
-  if (m) {
-    memcpy(e->dv_host.h, q->ids, (size_t)m * 4);
-    LWSE_CUDA(e, cudaMemcpyAsync(e->dv_ids.p, e->dv_host.h, (size_t)m * 4, cudaMemcpyHostToDevice, s));
-  }
-  LWSE_CUDA(e, cudaMemsetAsync(e->dr_bcost.p, 0, (size_t)nk * sizeof(lwse_drain_budget_cost), s));
   LWSE_CUDA(e, cudaMemsetAsync(e->dd_cost.p, 0, (size_t)nk * sizeof(lwse_ds_drain_cost), s));
   LWSE_CUDA(e, cudaMemsetAsync(d_words, 0, 128, s));
   LWSE_CUDA(e, cudaMemsetAsync(d_count, 0, (size_t)(nl + 1) * 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_pos.p, 0xFF, (size_t)nk * 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_kidx.p, 0, (size_t)m * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lidx.p, 0, (size_t)nl * 4 + 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_gwaves.p, 0, (size_t)ng * 8, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_out.p, 0, plan_bytes, s));
   LWSE_CUDA(e, cudaMemsetAsync(e->dx_caps.p, 0, (size_t)nl * 4, s));
   LWSE_CUDA(e, cudaMemsetAsync(e->dx_out.p, 0, out_bytes, s));
   // the before sweep (its ds_out gates the verdicts), the reverse link index's counts, the caps
@@ -3819,75 +3645,25 @@ LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_qu
   launched = lwse::launch_ds_drain_waves(&d, nullptr, 0, e->sm_count, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   // the key rows, the member-pair count and the pair count: the drain budget's pass 0, then the key positions
-  lwse::DrainBudgetCostLaunch bp{};
-  bp.lws = (const lwse_lws_rec*)e->r_lws.p;
-  bp.lws_out = (const lwse_lws_out*)e->r_lws_out.p;
-  bp.groups = (const lwse_group_rec*)e->r_groups.p;
-  bp.pod_state = (const uint8_t*)e->r_pst.p;
-  bp.pod_ident = (const lwse_pod_ident*)e->r_pid.p;
-  bp.baseline = (const lwse_group_out*)e->r_group_out.p;
-  bp.nodes = (const lwse_node_rec*)e->nodes.p;
-  bp.occupancy = (const uint32_t*)e->r_occ.p;
-  bp.cost = (lwse_drain_budget_cost*)e->dr_bcost.p;
-  bp.counts = d_words;
-  bp.n_pods = e->rn_pods;
-  bp.n_lws = nl;
-  bp.n_groups = ng;
-  bp.n_nodes = nn;
-  bp.n_domains = e->n_domains;
-  bp.n_keys = nk;
-  bp.by_domain = by_domain;
-  launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  lwse::DrainBudgetCostLaunch bp = restart_walk(e, by_domain, (lwse_drain_budget_cost*)e->dr_bcost.p, d_words);
   lwse::DrainWavesLaunch p{};
-  p.lws = bp.lws;
-  p.lws_out = bp.lws_out;
-  p.groups = bp.groups;
-  p.baseline = bp.baseline;
-  p.cost = bp.cost;
-  p.ids = (const uint32_t*)e->dv_ids.p;
-  p.pos_of = (uint32_t*)e->dv_pos.p;
-  p.count = (uint32_t*)e->dv_kidx.p;
-  p.first = p.count + m;
-  p.cursor = p.first + m + 1;
-  p.l_count = (uint32_t*)e->dv_lidx.p;
-  p.l_first = p.l_count + nl;
-  p.l_cursor = p.l_first + nl + 1;
-  p.dense = (uint4*)e->dv_dense.p;
-  p.g_waves = (unsigned long long*)e->dv_gwaves.p;
-  p.out = (uint8_t*)e->dv_out.p;
-  p.counts = reinterpret_cast<unsigned long long*>(d_words + 16);
-  p.n_lws = nl;
-  p.n_groups = ng;
-  p.n_keys = nk;
-  p.m = m;
-  p.max_waves = mw;
-  p.cols = (m < mw ? m : mw) + 1u;
-  launched = lwse::launch_drain_waves(&p, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = enqueue_drain_waves_setup(e, bp, q->ids, m, mw, (unsigned long long*)(d_words + 16), &p); rc != LWSE_OK)
+    return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 128, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   uint64_t member_pairs = 0, n_pairs = 0, n_entries = 0;
   memcpy(&member_pairs, words, 8);
   memcpy(&n_pairs, words + 16, 8);
   memcpy(&n_entries, words + 24, 8);
-  // (every index is 32-bit, and the plan kernel's items are a key's pairs times the columns)
-  if (n_pairs > 0xFFFFFFFFull / (LWSE_DRAIN_WAVES_MAX + 1u)) return LWSE_ERR_OOM;
   if (member_pairs > (1ull << 30) || n_entries > (1ull << 30)) return LWSE_ERR_OOM;
-  LWSE_CUDA(e, e->dv_pairs.reserve((size_t)n_pairs * 8 + 16));
-  LWSE_CUDA(e, e->dv_recs.reserve((size_t)n_pairs * 16 + 16));
+  if (const int rc = reserve_drain_waves_pairs(e, n_pairs); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, e->dd_entries.reserve((size_t)n_entries * sizeof(uint4) + 16));
-  uint64_t slots = 256;
-  while (slots < 2 * member_pairs) slots <<= 1;
+  const uint64_t slots = table_slots(member_pairs);
   if (member_pairs) LWSE_CUDA(e, e->dr_table.reserve((size_t)slots * (sizeof(unsigned long long) + sizeof(uint4))));
   launched = lwse::launch_ds_drain_links(&d.t, &d.lk, d_count, d_cursor, (uint4*)e->dd_entries.p, (uint32_t)n_entries, nullptr,
                                          true, e->sm_count, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dv_pairs.p, (uint32_t)n_pairs, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  p.pairs = (const unsigned long long*)e->dv_pairs.p;
-  p.n_pairs = (uint32_t)n_pairs;
-  p.recs = (uint4*)e->dv_recs.p;
+  if (const int rc = enqueue_drain_waves_pairs(e, bp, (uint32_t)n_pairs, &p); rc != LWSE_OK) return rc;
   launched = lwse::launch_drain_waves_capped(&p, d.caps, q->constraints, 1, e->sm_count, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   // the per-key forms: the (LWS, key) table with the budget columns, then the (row, key) pair count
@@ -3923,8 +3699,7 @@ LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_qu
   memcpy(&ds_pairs, words + 20, 8);
   if (ds_pairs) {
     if (ds_pairs > (1ull << 30)) return LWSE_ERR_OOM;
-    uint64_t ds_slots = 256;
-    while (ds_slots < 2 * ds_pairs) ds_slots <<= 1;
+    const uint64_t ds_slots = table_slots(ds_pairs);
     LWSE_CUDA(e, e->dd_table.reserve((size_t)ds_slots * (sizeof(unsigned long long) + sizeof(uint2))));
     c.keys = (unsigned long long*)e->dd_table.p;
     c.vals = reinterpret_cast<uint2*>(c.keys + ds_slots);
@@ -3934,16 +3709,7 @@ LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_qu
     launched = lwse::launch_ds_drain_cost(&c, 1, e->sm_count, s, &cuda_err);
     if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
-  LWSE_CUDA(e, e->dv_lost.reserve((size_t)n_dense * p.cols * 4 + 16));
-  LWSE_CUDA(e, e->dv_rwaves.reserve((size_t)n_dense * 16 + 16));
-  LWSE_CUDA(e, e->dv_stamps.reserve((size_t)n_dense * 8 + 16));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_lost.p, 0, (size_t)n_dense * p.cols * 4, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_rwaves.p, 0, (size_t)n_dense * 16, s));
-  LWSE_CUDA(e, cudaMemsetAsync(e->dv_stamps.p, 0, (size_t)n_dense * 8, s));
-  p.n_dense = n_dense;
-  p.lost = (uint32_t*)e->dv_lost.p;
-  p.row_waves = (unsigned long long*)e->dv_rwaves.p;
-  p.stamps = (uint32_t*)e->dv_stamps.p;
+  if (const int rc = enqueue_drain_waves_dense(e, n_dense, &p); rc != LWSE_OK) return rc;
   launched = lwse::launch_drain_waves_capped(&p, d.caps, q->constraints, 2, e->sm_count, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   launched = lwse::launch_ds_drain_waves(&d, &p, 1, e->sm_count, s, &cuda_err);
@@ -3953,15 +3719,7 @@ LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_qu
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words + 20, 12, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   if (words[2]) return LWSE_ERR_OOM;  // an insert the (DS, key) table refused
-  const uint8_t* h = static_cast<const uint8_t*>(e->dv_host.h);
-  uint32_t totals[4];
-  memcpy(totals, h, 16);
-  if (m) memcpy(q->keys, h + 16, keys_bytes);
-  memcpy(q->waves, h + 16 + keys_bytes, (size_t)totals[0] * sizeof(lwse_ds_drain_wave));
-  q->n_waves = totals[0];
-  q->n_planned = totals[1];
-  q->n_breaches_alone = totals[2];
-  q->n_no_wave = totals[3];
+  copy_waves_answer(e, q);
   return LWSE_OK;
 }
 

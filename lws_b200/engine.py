@@ -474,22 +474,48 @@ class Engine:
 
     _DRAIN_SCOPES = {"nodes": R.DRAIN_NODES, "domains": R.DRAIN_DOMAINS}
 
+    @staticmethod
+    def _drain_ids(nodes, domains):
+        """A drain set given as exactly one of node rows or domain ids → (ids as uint32, its ``records.DRAIN_*``
+        scope)."""
+        if (nodes is None) == (domains is None):
+            raise ValueError("give node rows or domain ids")
+        ids = np.ascontiguousarray(nodes if domains is None else domains, dtype=np.uint32)
+        return ids, R.DRAIN_NODES if domains is None else R.DRAIN_DOMAINS
+
+    def _drain_waves(self, call, query, key_dtype, wave_dtype, totals, nodes, domains, max_waves, constraints=None):
+        """One waves plan: a ``query`` filled and passed to ``call`` → dict: the key rows, the opened wave rows and
+        the fields ``totals`` names."""
+        ids, scope = self._drain_ids(nodes, domains)
+        keys = R.aligned_empty(max(len(ids), 1), key_dtype)
+        waves = R.aligned_empty(max(int(max_waves), 1), wave_dtype)
+        q = query()
+        q.ids = R.ptr(ids) if len(ids) else None
+        q.n_ids = len(ids)
+        q.scope = scope
+        q.max_waves = int(max_waves)
+        if constraints is not None:
+            q.constraints = int(constraints)
+        q.keys, q.waves = R.ptr(keys), R.ptr(waves)
+        self._check(call(self._h, C.byref(q)))
+        out = {"keys": keys[: len(ids)], "waves": waves[: q.n_waves]}
+        out.update({k: getattr(q, k) for k in totals})
+        return out
+
     def resident_drain_budget(self, nodes=None, domains=None, capacity=None):
         """lwse_resident_drain_budget: the LeaderWorkerSet rows a drain of the node rows ``nodes`` — or of every
         node in the domain ids ``domains`` — touches, each with its availability floor, ready count before
         and after, and ``records.DRAINB_*`` flags.  Give exactly one of the two.  ``capacity`` None lists every
         touched row.  → dict: ``rows`` (``records.DRAIN_BUDGET``) and the totals of
         ``records.DRAIN_BUDGET_TOTALS``."""
-        if (nodes is None) == (domains is None):
-            raise ValueError("give node rows or domain ids")
-        ids = np.ascontiguousarray(nodes if domains is None else domains, dtype=np.uint32)
+        ids, scope = self._drain_ids(nodes, domains)
         n_res = getattr(self, "_resident_shape", (0, 0))[0]
         cap = n_res if capacity is None else int(capacity)
         rows = R.aligned_empty(max(cap, 1), R.DRAIN_BUDGET)
         q = R.DrainBudgetQuery()
         q.ids = R.ptr(ids) if len(ids) else None
         q.n_ids = len(ids)
-        q.scope = R.DRAIN_NODES if domains is None else R.DRAIN_DOMAINS
+        q.scope = scope
         q.capacity = cap
         q.rows = R.ptr(rows)
         self._check(lib().lwse_resident_drain_budget(self._h, C.byref(q)))
@@ -511,21 +537,8 @@ class Engine:
         in the order given, into at most ``max_waves`` waves whose drain takes no LeaderWorkerSet below its
         floor.  Give exactly one of the two.  → dict: ``keys`` (``records.DRAIN_WAVE_KEY``, in query order),
         ``waves`` (``records.DRAIN_WAVE``, one per opened wave) and the totals of ``records.DRAIN_WAVES_TOTALS``."""
-        if (nodes is None) == (domains is None):
-            raise ValueError("give node rows or domain ids")
-        ids = np.ascontiguousarray(nodes if domains is None else domains, dtype=np.uint32)
-        keys = R.aligned_empty(max(len(ids), 1), R.DRAIN_WAVE_KEY)
-        waves = R.aligned_empty(max(int(max_waves), 1), R.DRAIN_WAVE)
-        q = R.DrainWavesQuery()
-        q.ids = R.ptr(ids) if len(ids) else None
-        q.n_ids = len(ids)
-        q.scope = R.DRAIN_NODES if domains is None else R.DRAIN_DOMAINS
-        q.max_waves = int(max_waves)
-        q.keys, q.waves = R.ptr(keys), R.ptr(waves)
-        self._check(lib().lwse_resident_drain_waves(self._h, C.byref(q)))
-        out = {"keys": keys[: len(ids)], "waves": waves[: q.n_waves]}
-        out.update({k: getattr(q, k) for k in R.DRAIN_WAVES_TOTALS})
-        return out
+        return self._drain_waves(lib().lwse_resident_drain_waves, R.DrainWavesQuery, R.DRAIN_WAVE_KEY, R.DRAIN_WAVE,
+                                 R.DRAIN_WAVES_TOTALS, nodes, domains, max_waves)
 
     def resident_drain_place_cost(self, scope: str = "nodes") -> np.ndarray:
         """lwse_resident_drain_place_cost: one ``records.DRAIN_PLACE_COST`` row per node (``scope="nodes"``) or per
@@ -544,16 +557,14 @@ class Engine:
         two.  ``capacity`` None lists every touched DS; ``outputs`` also returns the after sweep's full
         ``role_out`` / ``revrole_out``.  → dict: ``rows`` (``records.DS_DRAIN``) and the totals of
         ``records.DS_DRAIN_TOTALS``."""
-        if (nodes is None) == (domains is None):
-            raise ValueError("give node rows or domain ids")
-        ids = np.ascontiguousarray(nodes if domains is None else domains, dtype=np.uint32)
+        ids, scope = self._drain_ids(nodes, domains)
         n_ds, n_roles, n_rr = getattr(self, "_ds_shape", (0, 0, 0))
         cap = n_ds if capacity is None else int(capacity)
         rows = R.aligned_empty(max(cap, 1), R.DS_DRAIN)
         q = R.DsDrainQuery()
         q.ids = R.ptr(ids) if len(ids) else None
         q.n_ids = len(ids)
-        q.scope = R.DRAIN_NODES if domains is None else R.DRAIN_DOMAINS
+        q.scope = scope
         q.capacity = cap
         q.rows = R.ptr(rows)
         role_out = revrole_out = None
@@ -585,22 +596,8 @@ class Engine:
         DisaggregatedSet serving; ``DSW_DS_STALL`` is opt-in, since it forbids any ready loss under a rolling DS.
         Give exactly one of the two.  → dict: ``keys`` (``records.DS_DRAIN_WAVE_KEY``, in query order), ``waves``
         (``records.DS_DRAIN_WAVE``, one per opened wave) and the totals of ``records.DS_DRAIN_WAVES_TOTALS``."""
-        if (nodes is None) == (domains is None):
-            raise ValueError("give node rows or domain ids")
-        ids = np.ascontiguousarray(nodes if domains is None else domains, dtype=np.uint32)
-        keys = R.aligned_empty(max(len(ids), 1), R.DS_DRAIN_WAVE_KEY)
-        waves = R.aligned_empty(max(int(max_waves), 1), R.DS_DRAIN_WAVE)
-        q = R.DsDrainWavesQuery()
-        q.ids = R.ptr(ids) if len(ids) else None
-        q.n_ids = len(ids)
-        q.scope = R.DRAIN_NODES if domains is None else R.DRAIN_DOMAINS
-        q.max_waves = int(max_waves)
-        q.constraints = int(constraints)
-        q.keys, q.waves = R.ptr(keys), R.ptr(waves)
-        self._check(lib().lwse_resident_ds_drain_waves(self._h, C.byref(q)))
-        out = {"keys": keys[: len(ids)], "waves": waves[: q.n_waves]}
-        out.update({k: getattr(q, k) for k in R.DS_DRAIN_WAVES_TOTALS})
-        return out
+        return self._drain_waves(lib().lwse_resident_ds_drain_waves, R.DsDrainWavesQuery, R.DS_DRAIN_WAVE_KEY,
+                                 R.DS_DRAIN_WAVE, R.DS_DRAIN_WAVES_TOTALS, nodes, domains, max_waves, constraints)
 
     def resident_drain_place_waves(self, nodes=None, domains=None, max_waves=R.DRAIN_WAVES_MAX,
                                    constraints=R.DPW_LWS_FLOOR | R.DPW_STRANDED):
@@ -611,22 +608,8 @@ class Engine:
         opt-in.  Give exactly one of the two.  → dict: ``keys`` (``records.DRAIN_PLACE_WAVE_KEY``, in query order),
         ``waves`` (``records.DRAIN_PLACE_WAVE``, one per opened wave) and the totals of
         ``records.DRAIN_WAVES_TOTALS``."""
-        if (nodes is None) == (domains is None):
-            raise ValueError("give node rows or domain ids")
-        ids = np.ascontiguousarray(nodes if domains is None else domains, dtype=np.uint32)
-        keys = R.aligned_empty(max(len(ids), 1), R.DRAIN_PLACE_WAVE_KEY)
-        waves = R.aligned_empty(max(int(max_waves), 1), R.DRAIN_PLACE_WAVE)
-        q = R.DrainPlaceWavesQuery()
-        q.ids = R.ptr(ids) if len(ids) else None
-        q.n_ids = len(ids)
-        q.scope = R.DRAIN_NODES if domains is None else R.DRAIN_DOMAINS
-        q.max_waves = int(max_waves)
-        q.constraints = int(constraints)
-        q.keys, q.waves = R.ptr(keys), R.ptr(waves)
-        self._check(lib().lwse_resident_drain_place_waves(self._h, C.byref(q)))
-        out = {"keys": keys[: len(ids)], "waves": waves[: q.n_waves]}
-        out.update({k: getattr(q, k) for k in R.DRAIN_WAVES_TOTALS})
-        return out
+        return self._drain_waves(lib().lwse_resident_drain_place_waves, R.DrainPlaceWavesQuery, R.DRAIN_PLACE_WAVE_KEY,
+                                 R.DRAIN_PLACE_WAVE, R.DRAIN_WAVES_TOTALS, nodes, domains, max_waves, constraints)
 
     def resident_patch(self, which: int, rows, values):
         """Overwrite rows of a resident table (rows: uint32 indices, values: packed rows)."""
