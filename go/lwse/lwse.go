@@ -211,6 +211,14 @@ func (e *Engine) DrainPlaceCost(scope uint32, out *C.lwse_drain_place_cost) erro
 	return e.check(C.lwse_resident_drain_place_cost(e.h, C.uint32_t(scope), out))
 }
 
+// RolloutPlace answers "do the groups this rollout adds find an exclusive domain?" for a list of resident
+// LeaderWorkerSets, or of proposed edits (q.recs), in one call: per entry the forecast's peak, the groups up to it
+// that need a request (surge), those left without a domain (stranded) and the other requests that lose theirs.
+// An admission webhook or a rollout controller checks an edit with it before pushing it.
+func (e *Engine) RolloutPlace(q *C.lwse_rollout_place_query) error {
+	return e.check(C.lwse_resident_rollout_place(e.h, q))
+}
+
 // DrainWaves packs distinct node rows (scope LWSE_DRAIN_NODES) or domain ids (LWSE_DRAIN_DOMAINS), in the order
 // given, first-fit into at most q.max_waves waves whose drain takes no LeaderWorkerSet below its floor.  A
 // maintenance controller drains wave 0, waits for recovery and calls again with the keys that remain.

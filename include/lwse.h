@@ -1236,6 +1236,84 @@ typedef struct lwse_drain_place_waves_query {
 } lwse_drain_place_waves_query;
 LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_waves_query* q);
 
+/* ---- rollout placement --------------------------------------------------------------------------
+ * "Do the groups this rollout adds find an exclusive domain?" — for a list of LeaderWorkerSets, resident rows or
+ * proposed edits, in one call.  The forecasts (lwse_resident_forecast, lwse_resident_rollout_whatif) assume every
+ * group the leader StatefulSet holds becomes ready; an exclusive group that finds no free domain in its namespace
+ * stays Pending instead (DESIGN.md §3.5, "Rollout placement").
+ *
+ * Definition.  Entry i names a resident LWS row L_i, a namespace id ns_i < the resident n_namespaces and, when
+ * `recs` is given, a proposal P_i (an lwse_lws_rec with the contract of lwse_resident_rollout_whatif); without
+ * `recs` P_i is the resident row L_i.  Each entry is answered on its own, as if its rollout were the only change;
+ * several entries may name the same row.
+ *   1. F_i is lwse_resident_rollout_whatif's forecast row for (L_i, P_i) — with P_i = L_i, lwse_resident_forecast's
+ *      row of L_i — and peak = F_i.peak_sts_replicas.
+ *   2. E_i holds, ascending, every group index g in [0, peak) with g >= group_count of L_i, or whose group row
+ *      group_base + g lacks LWSE_GRP_POD_PRESENT: the groups encode_place_requests gives a request once their
+ *      leader pods exist.  Row j of E_i is the request {priority, group_key} = the encoder's mix of
+ *      (P_i.uid_hash, g), group = group_base + g, ns = ns_i, size = P_i.size, leader_node = LWSE_NONE.
+ *   3. The answer is lwse_resident_place_whatif with no segments, extra = E_i (extra row j has row index and key
+ *      rn_reqs + j) and the resident n_namespaces.  It solves ns_i alone (every other row keeps its baseline row):
+ *      one namespace per entry, none when E_i is empty.
+ *   4. An entry is not solved, and gets a flag, when L_i lacks LWSE_LWS_EXCLUSIVE_TOPOLOGY (NOT_EXCLUSIVE), when
+ *      F_i has LWSE_LWSF_BAD_TABLE or LWSE_LWSF_NOT_FORECAST (NOT_FORECAST), or when P_i changes `size` or the
+ *      exclusive bit of L_i (NOT_MODELLED: the rolled groups would need new domains).  An UNFINISHED forecast is
+ *      solved with the peak of the cycles it replayed.  fc_flags and peak are F_i's for every entry.
+ *
+ * Readiness, isolation and errors: LWSE_ERR_NOT_READY wherever lwse_resident_forecast, lwse_resident_rollout_whatif
+ * or lwse_resident_place_whatif would return it; LWSE_ERR_INVALID_ARG for a NULL query or array (with n > 0),
+ * misaligned recs, a row >= n_lws or ns_i >= the resident n_namespaces; LWSE_ERR_UNSUPPORTED, writing nothing, on
+ * an engine with a peer exchange, when rn_reqs + max |E_i| reaches 2^24 (row keys are 24-bit), where the namespace
+ * form does not fit the domains, and when the proposals' slots reach the forecast's limit; LWSE_ERR_OOM rather
+ * than a wrong row when sized scratch refuses an entry.  The call holds the engine mutex and runs on the what-if
+ * stream behind one event on the engine's stream: the forecast snapshot and the placement baseline both come from
+ * the most recently submitted tick, in flight or not.  It touches no tick graph, arena, change list, table, output
+ * row, occupancy counter, node index or tick info; its scratch only grows.  n == 0 is a valid empty answer.
+ * A refused call writes neither the rows, the extra rows nor the totals. */
+typedef struct lwse_rollout_place { /* 64 B */
+  uint32_t flags;            /* LWSE_RPL_*                                                              */
+  uint32_t fc_flags;         /* F_i.flags                                                               */
+  int32_t peak;              /* F_i.peak_sts_replicas                                                   */
+  uint32_t surge;            /* |E_i| (0 for an entry that is not solved)                               */
+  uint32_t placed;           /* rows of E_i PLACED after                                                */
+  uint32_t stranded;         /* rows of E_i not PLACED after                                            */
+  uint32_t own_lost;         /* resident rows whose `group` lies in L_i's range, PLACED before, not after */
+  uint32_t bumped;           /* other resident rows PLACED before and not after                         */
+  uint32_t n_changed;        /* the lwse_place_whatif counters of the composed query                    */
+  uint32_t n_lost;
+  uint32_t n_moved;
+  uint32_t n_gained;
+  uint32_t n_placed;
+  uint32_t n_unschedulable;
+  uint32_t n_conflict;
+  uint32_t namespaces_solved; /* 0 or 1                                                                 */
+} lwse_rollout_place;
+
+#define LWSE_RPL_SOLVED (1u << 0)        /* answered: the counters hold the composed query's              */
+#define LWSE_RPL_NOT_EXCLUSIVE (1u << 1) /* L_i lacks LWSE_LWS_EXCLUSIVE_TOPOLOGY                          */
+#define LWSE_RPL_NOT_FORECAST (1u << 2)  /* F_i has LWSE_LWSF_BAD_TABLE or LWSE_LWSF_NOT_FORECAST          */
+#define LWSE_RPL_NOT_MODELLED (1u << 3)  /* P_i changes size or the exclusive bit                          */
+#define LWSE_RPL_STRANDS (1u << 4)       /* stranded > 0                                                   */
+#define LWSE_RPL_BUMPS (1u << 5)         /* bumped > 0                                                     */
+
+typedef struct lwse_rollout_place_query {
+  const uint32_t* rows;      /* [n] resident LWS rows                                                   */
+  const uint32_t* ns;        /* [n] namespace ids                                                       */
+  const lwse_lws_rec* recs;  /* [n] proposals, 16-byte aligned, or NULL: the resident rows              */
+  uint32_t n;
+  uint32_t reserved;         /* 0                                                                       */
+  lwse_rollout_place* out;   /* [n] out, host memory                                                    */
+  lwse_place_req* extra;     /* [extra_capacity] out, host memory, or NULL: the rows of every E_i, entry
+                                after entry in query order (the first extra_capacity of n_surge rows)   */
+  uint64_t extra_capacity;
+  /* out */
+  uint32_t n_solved;         /* entries with LWSE_RPL_SOLVED                                            */
+  uint32_t n_strands;        /* entries with LWSE_RPL_STRANDS                                           */
+  uint64_t n_surge;          /* sum of surge                                                            */
+  uint64_t n_stranded;       /* sum of stranded                                                         */
+} lwse_rollout_place_query;
+LWSE_API int lwse_resident_rollout_place(lwse_engine* e, lwse_rollout_place_query* q);
+
 /* ------------------------------------------------------------------------- */
 /* Peer exchange: the multi-GPU placement step without a collective library  */
 /* ------------------------------------------------------------------------- */

@@ -238,6 +238,10 @@ struct lwse_engine {
   // per-CTA slices
   DevBuf dp_cost, dp_words, dp_domfree, dp_gidx, dp_uidx, dp_pairs, dp_urows, dp_pos, dp_items, dp_rows, dp_touched, dp_round,
       dp_slices;
+  // rollout placement (lwse_resident_rollout_place): the entries' rows and namespaces, the answer rows, the entries'
+  // {first extra row, |E_i|, group range}, the |E_i| index (count | first | cursor), the items, the counters, the
+  // extra rows, the all-namespaces mask, the round scratch, the solve's per-CTA slices
+  DevBuf rp_in, rp_rows, rp_ent, rp_idx, rp_items, rp_words, rp_extra, rp_touched, rp_round, rp_slices;
   // drain waves (lwse_resident_drain_waves): the drain budget's key rows, the counters, the ids, the key positions, the
   // key buckets (count | first | cursor), the restart pairs, the pair records, the touched-row index (count | first |
   // cursor), the dense rows, the lost counters, the group and row wave masks, the stamps, the answer; the ids going
@@ -485,6 +489,8 @@ LWSE_API void lwse_destroy(lwse_engine* e) {
                       &e->dr_domains, &e->dr_brows, &e->dr_bcost, &e->dr_table, &e->dr_bwords,
                       &e->dp_cost, &e->dp_words, &e->dp_domfree, &e->dp_gidx, &e->dp_uidx, &e->dp_pairs, &e->dp_urows, &e->dp_pos,
                       &e->dp_items, &e->dp_rows, &e->dp_touched, &e->dp_round, &e->dp_slices,
+                      &e->rp_in, &e->rp_rows, &e->rp_ent, &e->rp_idx, &e->rp_items, &e->rp_words, &e->rp_extra,
+                      &e->rp_touched, &e->rp_round, &e->rp_slices,
                       &e->dd_lost, &e->dd_lws_after, &e->dd_out[0], &e->dd_out[1], &e->dd_role_out[0], &e->dd_role_out[1],
                       &e->dd_revrole_out[0], &e->dd_revrole_out[1], &e->dd_rows, &e->dd_index, &e->dd_entries, &e->dd_cost,
                       &e->dd_table, &e->rw_rows, &e->rw_lws, &e->rw_off, &e->rw_sums, &e->rw_groups, &e->rw_src,
@@ -4201,7 +4207,8 @@ LWSE_API int lwse_resident_ds_rollout_whatif(lwse_engine* e, lwse_ds_rollout_wha
 }
 
 // ---- rolling-update forecast of the LeaderWorkerSets ----
-// The forecast of device rows h.lws / h.group_out (sizes in h) on stream s into the host outputs `out`.
+// The forecast of device rows h.lws / h.group_out (sizes in h) on stream s into the host outputs `out`
+// (out->lws null: the rows stay in lf_fc on the device only).
 // Everything it writes on the device is its own scratch; returns once `out` is filled.  The slot layout
 // comes first (it sizes the private flag bytes), then the summary pass and the scan; the trajectory
 // buffer is sized by the rows that fit (not by step_capacity), so scratch only grows when a forecast
@@ -4234,7 +4241,7 @@ static int lws_forecast_locked(lwse_engine* e, lwse::LwsForecastHost& h, lwse_lw
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   const size_t b_fc = (size_t)h.n_lws * sizeof(lwse_lws_forecast);
   LWSE_CUDA(e, cudaMemcpyAsync(words, e->lf_totals.p, 32, cudaMemcpyDeviceToHost, s));
-  if (b_fc) LWSE_CUDA(e, cudaMemcpyAsync(out->lws, e->lf_fc.p, b_fc, cudaMemcpyDeviceToHost, s));
+  if (b_fc && out->lws) LWSE_CUDA(e, cudaMemcpyAsync(out->lws, e->lf_fc.p, b_fc, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   // the objects whose rows fit come first in row order: the written rows are [0, n_steps_written)
   if (words[3]) return fail_cuda(e, cudaErrorAssert);  // a bounds check refused an access (an engine defect)
@@ -4284,6 +4291,22 @@ LWSE_API int lwse_lws_forecast_host(lwse_engine* e, const lwse_lws_rec* lws, uin
   return lws_forecast_locked(e, h, out, s);
 }
 
+// The resident forecast's snapshot: the resident LWS rows and group results copied on stream s into the forecast's
+// own buffers, and the forecast's input over them in *h.
+static int forecast_snapshot(lwse_engine* e, cudaStream_t s, lwse::LwsForecastHost* h) {
+  const size_t b_lws = (size_t)e->rn_lws * sizeof(lwse_lws_rec), b_go = (size_t)e->rn_groups * sizeof(lwse_group_out);
+  LWSE_CUDA(e, e->lf_lws.reserve(b_lws + 16));
+  LWSE_CUDA(e, e->lf_group_out.reserve(b_go + 16));
+  if (b_lws) LWSE_CUDA(e, cudaMemcpyAsync(e->lf_lws.p, e->r_lws.p, b_lws, cudaMemcpyDeviceToDevice, s));
+  if (b_go) LWSE_CUDA(e, cudaMemcpyAsync(e->lf_group_out.p, e->r_group_out.p, b_go, cudaMemcpyDeviceToDevice, s));
+  *h = lwse::LwsForecastHost{};
+  h->lws = (const lwse_lws_rec*)e->lf_lws.p;
+  h->n_lws = e->rn_lws;
+  h->group_out = (const lwse_group_out*)e->lf_group_out.p;
+  h->n_groups = e->rn_groups;
+  return LWSE_OK;
+}
+
 // Snapshot on the engine's stream, replay on lf_stream: the ticks in flight keep running, and none of
 // their buffers is written.
 LWSE_API int lwse_resident_forecast(lwse_engine* e, lwse_lws_forecast_out* out) {
@@ -4295,54 +4318,35 @@ LWSE_API int lwse_resident_forecast(lwse_engine* e, lwse_lws_forecast_out* out) 
   int rc = lws_forecast_stream(e);
   if (rc != LWSE_OK) return rc;
   if (!e->ev_lf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_lf, cudaEventDisableTiming));
-  const size_t b_lws = (size_t)e->rn_lws * sizeof(lwse_lws_rec), b_go = (size_t)e->rn_groups * sizeof(lwse_group_out);
-  LWSE_CUDA(e, e->lf_lws.reserve(b_lws + 16));
-  LWSE_CUDA(e, e->lf_group_out.reserve(b_go + 16));
-  if (b_lws) LWSE_CUDA(e, cudaMemcpyAsync(e->lf_lws.p, e->r_lws.p, b_lws, cudaMemcpyDeviceToDevice, e->stream));
-  if (b_go) LWSE_CUDA(e, cudaMemcpyAsync(e->lf_group_out.p, e->r_group_out.p, b_go, cudaMemcpyDeviceToDevice, e->stream));
+  lwse::LwsForecastHost h{};
+  if (const int src = forecast_snapshot(e, e->stream, &h); src != LWSE_OK) return src;
   LWSE_CUDA(e, cudaEventRecord(e->ev_lf, e->stream));
   LWSE_CUDA(e, cudaStreamWaitEvent(e->lf_stream, e->ev_lf, 0));
-  lwse::LwsForecastHost h{};
-  h.lws = (const lwse_lws_rec*)e->lf_lws.p;
-  h.n_lws = e->rn_lws;
-  h.group_out = (const lwse_group_out*)e->lf_group_out.p;
-  h.n_groups = e->rn_groups;
   return lws_forecast_locked(e, h, out, e->lf_stream);
 }
 
 // ---- rollout what-if ----
-// On lf_stream behind an event on the engine's stream; reads the resident rows, groups, pods and group
-// results in place (the mutex keeps the next tick out until the call returns).  The layout sizes the
-// gathered group table at one synchronisation; the gather, the sweep's group pass, the restore of the
-// foreign-owned rows and the LWS pass follow, then the forecast over the proposals' rows.  `now` is copied
-// out last, so that a refused forecast writes nothing.
-LWSE_API int lwse_resident_rollout_whatif(lwse_engine* e, lwse_rollout_whatif* q) {
-  if (!e || !q) return LWSE_ERR_INVALID_ARG;
-  std::lock_guard<std::mutex> lock(e->mu);
-  if (!e->r_loaded || !e->r_groups_swept) return LWSE_ERR_NOT_READY;
-  const uint32_t n = q->n;
-  if (n && (!q->rows || !q->recs || !q->now || !q->fc.lws)) return LWSE_ERR_INVALID_ARG;
-  if (!aligned16(q->recs)) return LWSE_ERR_INVALID_ARG;
-  for (uint32_t i = 0; i < n; i++)
-    if (q->rows[i] >= e->rn_lws) return LWSE_ERR_INVALID_ARG;
-  if (n == 0) {
-    q->fc.n_steps_written = 0;
-    q->fc.n_steps_needed = 0;
-    return LWSE_OK;
-  }
-  DeviceGuard guard(e->device);
-  if (const int rc = lws_forecast_stream(e); rc != LWSE_OK) return rc;
-  if (!e->ev_lf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_lf, cudaEventDisableTiming));
-  cudaStream_t s = e->lf_stream;
+// The chain's first scratch for n proposals, before the snapshot.
+static int reserve_rollout_whatif(lwse_engine* e, uint32_t n) {
   LWSE_CUDA(e, e->rw_rows.reserve((size_t)n * 4 + 16));
   LWSE_CUDA(e, e->rw_lws.reserve((size_t)n * sizeof(lwse_lws_rec) + 16));
   LWSE_CUDA(e, e->rw_off.reserve((size_t)n * 8 + 16));
   LWSE_CUDA(e, e->rw_sums.reserve(16 + (size_t)lwse::forecast_scan_words(n) * 8));  // [0] total, then the block sums
   LWSE_CUDA(e, e->lf_words.reserve(32));
-  LWSE_CUDA(e, cudaMemcpyAsync(e->rw_rows.p, q->rows, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-  LWSE_CUDA(e, cudaMemcpyAsync(e->rw_lws.p, q->recs, (size_t)n * sizeof(lwse_lws_rec), cudaMemcpyHostToDevice, s));
-  LWSE_CUDA(e, cudaEventRecord(e->ev_lf, e->stream));
-  LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_lf, 0));
+  return LWSE_OK;
+}
+
+static int upload_rollout_proposals(lwse_engine* e, const uint32_t* rows, const lwse_lws_rec* recs, uint32_t n, cudaStream_t s) {
+  LWSE_CUDA(e, cudaMemcpyAsync(e->rw_rows.p, rows, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(e->rw_lws.p, recs, (size_t)n * sizeof(lwse_lws_rec), cudaMemcpyHostToDevice, s));
+  return LWSE_OK;
+}
+
+// The chain on stream s over the n uploaded proposals: the layout sizes the gathered group table at one
+// synchronisation; the gather, the sweep's group pass, the restore of the foreign-owned rows and the LWS pass follow,
+// then the forecast over the proposals' rows into fc (its device rows stay in lf_fc).  The `now` rows are left in
+// rw_now.
+static int enqueue_rollout_whatif(lwse_engine* e, uint32_t n, cudaStream_t s, lwse_lws_forecast_out* fc) {
   unsigned long long* d_sums = (unsigned long long*)e->rw_sums.p;
   lwse::RolloutWhatifHost h{};
   h.lws = (const lwse_lws_rec*)e->r_lws.p;
@@ -4401,9 +4405,176 @@ LWSE_API int lwse_resident_rollout_whatif(lwse_engine* e, lwse_rollout_whatif* q
   f.n_lws = n;
   f.group_out = (const lwse_group_out*)e->rw_group_out.p;
   f.n_groups = ng;
-  if (const int rc = lws_forecast_locked(e, f, &q->fc, s); rc != LWSE_OK) return rc;
+  return lws_forecast_locked(e, f, fc, s);
+}
+
+// On lf_stream behind an event on the engine's stream; reads the resident rows, groups, pods and group
+// results in place (the mutex keeps the next tick out until the call returns).  `now` is copied out last, so
+// that a refused forecast writes nothing.
+LWSE_API int lwse_resident_rollout_whatif(lwse_engine* e, lwse_rollout_whatif* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->r_loaded || !e->r_groups_swept) return LWSE_ERR_NOT_READY;
+  const uint32_t n = q->n;
+  if (n && (!q->rows || !q->recs || !q->now || !q->fc.lws)) return LWSE_ERR_INVALID_ARG;
+  if (!aligned16(q->recs)) return LWSE_ERR_INVALID_ARG;
+  for (uint32_t i = 0; i < n; i++)
+    if (q->rows[i] >= e->rn_lws) return LWSE_ERR_INVALID_ARG;
+  if (n == 0) {
+    q->fc.n_steps_written = 0;
+    q->fc.n_steps_needed = 0;
+    return LWSE_OK;
+  }
+  DeviceGuard guard(e->device);
+  if (const int rc = lws_forecast_stream(e); rc != LWSE_OK) return rc;
+  if (!e->ev_lf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_lf, cudaEventDisableTiming));
+  cudaStream_t s = e->lf_stream;
+  if (const int rc = reserve_rollout_whatif(e, n); rc != LWSE_OK) return rc;
+  if (const int rc = upload_rollout_proposals(e, q->rows, q->recs, n, s); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaEventRecord(e->ev_lf, e->stream));
+  LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_lf, 0));
+  if (const int rc = enqueue_rollout_whatif(e, n, s, &q->fc); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(q->now, e->rw_now.p, (size_t)n * sizeof(lwse_lws_out), cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
+  return LWSE_OK;
+}
+
+// ---- rollout placement ----
+// On wf_stream behind one event on the engine's stream: the forecast (the resident forecast's snapshot, or the
+// rollout what-if's chain over the proposals), then the count kernel, read back at one synchronisation (max |E_i|
+// sizes the slices and decides the 24-bit refusal), then the scan, the extra rows, every namespace's request index,
+// the solve and the finish, read back at a second.  The rows are copied out last, so that a refused call writes
+// nothing.
+LWSE_API int lwse_resident_rollout_place(lwse_engine* e, lwse_rollout_place_query* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if (!e->r_loaded || !e->r_groups_swept) return LWSE_ERR_NOT_READY;  // (the forecast's rule)
+  if (!e->r_place_loaded || !e->r_place_current || e->n_nodes == 0 || e->n_domains == 0) return LWSE_ERR_NOT_READY;
+  const uint32_t n = q->n;
+  if (n && (!q->rows || !q->ns || !q->out)) return LWSE_ERR_INVALID_ARG;
+  if (!aligned16(q->recs) || (q->extra_capacity && !q->extra)) return LWSE_ERR_INVALID_ARG;
+  for (uint32_t i = 0; i < n; i++)
+    if (q->rows[i] >= e->rn_lws || q->ns[i] >= e->rn_namespaces) return LWSE_ERR_INVALID_ARG;
+  if (e->xch_world > 0 || e->rn_reqs >= (1u << 24) || !lwse::place_ns_supported(e->n_nodes, e->n_domains))
+    return LWSE_ERR_UNSUPPORTED;
+  if (n == 0) {
+    q->n_solved = q->n_strands = 0;
+    q->n_surge = q->n_stranded = 0;
+    return LWSE_OK;
+  }
+  const uint32_t nn = e->n_nodes, nd = e->n_domains, nr = e->rn_reqs, n_ns = e->rn_namespaces;
+  const bool proposals = q->recs != nullptr;
+  DeviceGuard guard(e->device);
+  // scratch sized by n and the resident tables, before the snapshot
+  LWSE_CUDA(e, e->wf_words.reserve(128));
+  LWSE_CUDA(e, e->rp_in.reserve((size_t)n * 8 + 16));
+  LWSE_CUDA(e, e->rp_rows.reserve((size_t)n * sizeof(lwse_rollout_place) + 16));
+  LWSE_CUDA(e, e->rp_ent.reserve((size_t)n * 16 + 16));
+  LWSE_CUDA(e, e->rp_idx.reserve(((size_t)n * 3 + 1) * 4 + 16));
+  LWSE_CUDA(e, e->rp_items.reserve((size_t)n * 8 + 16));
+  LWSE_CUDA(e, e->rp_words.reserve(128));
+  LWSE_CUDA(e, e->rp_touched.reserve((size_t)n_ns + 16));
+  const size_t round_bytes = lwse::place_ns_scratch_bytes(nn, nd, nr, n_ns);
+  LWSE_CUDA(e, e->rp_round.reserve(round_bytes));
+  if (e->node_index_stale)
+    if (const int rc = reserve_node_index(e); rc != LWSE_OK) return rc;
+  if (proposals)
+    if (const int rc = reserve_rollout_whatif(e, n); rc != LWSE_OK) return rc;
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* d_words = (uint32_t*)e->rp_words.p;
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  uint32_t* d_rows_in = (uint32_t*)e->rp_in.p;
+  LWSE_CUDA(e, cudaMemcpyAsync(d_rows_in, q->rows, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(d_rows_in + n, q->ns, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  LWSE_CUDA(e, cudaMemsetAsync(d_words, 0, 128, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->rp_idx.p, 0, (size_t)n * 4, s));  // (the |E_i| counts start at zero)
+  // the forecast rows F_i, on the device only (lf_fc): per entry (proposals) or per resident row
+  lwse_lws_forecast_out fc{};
+  if (proposals) {
+    if (const int rc = upload_rollout_proposals(e, q->rows, q->recs, n, s); rc != LWSE_OK) return rc;
+    if (const int rc = enqueue_rollout_whatif(e, n, s, &fc); rc != LWSE_OK) return rc;
+  } else {
+    lwse::LwsForecastHost h{};
+    if (const int rc = forecast_snapshot(e, s, &h); rc != LWSE_OK) return rc;
+    if (const int rc = lws_forecast_locked(e, h, &fc, s); rc != LWSE_OK) return rc;
+  }
+  lwse::RolloutPlaceLaunch p{};
+  p.lws = (const lwse_lws_rec*)e->r_lws.p;
+  p.groups = (const lwse_group_rec*)e->r_groups.p;
+  p.n_groups = e->rn_groups;
+  p.rows = d_rows_in;
+  p.ns = d_rows_in + n;
+  p.recs = proposals ? (const lwse_lws_rec*)e->rw_lws.p : nullptr;
+  p.fc = (const lwse_lws_forecast*)e->lf_fc.p;
+  p.fc_by_row = !proposals;
+  p.n = n;
+  p.rows_out = (uint32_t*)e->rp_rows.p;
+  p.ent = (uint4*)e->rp_ent.p;
+  p.e_count = (uint32_t*)e->rp_idx.p;
+  p.e_first = p.e_count + n;
+  p.e_cursor = p.e_first + n + 1;
+  p.items = (uint2*)e->rp_items.p;
+  p.counts = d_words;
+  int cuda_err = 0;
+  int launched = lwse::launch_rollout_place(&p, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 16, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint32_t n_items = words[0], max_extra = words[1];
+  const uint64_t n_extra = (uint64_t)words[2] | (uint64_t)words[3] << 32;
+  if ((uint64_t)nr + max_extra >= (1ull << 24)) return LWSE_ERR_UNSUPPORTED;  // (row keys are 24-bit)
+  if (n_extra >= (1ull << 32)) return LWSE_ERR_OOM;                          // (the scan's offsets are 32-bit)
+  // the solve's slices: the largest namespace plus the largest E_i per resident CTA
+  const uint64_t slice_rows = (uint64_t)largest_namespace(e) + max_extra;
+  uint64_t grid = n_items ? std::min<uint64_t>((uint64_t)e->sm_count * 2u, n_items) : 0;
+  while (grid > 1 && grid * slice_rows * (sizeof(lwse_place_out) + 4) > (1ull << 30)) grid >>= 1;
+  if (grid && grid * slice_rows * (sizeof(lwse_place_out) + 4) > (1ull << 31)) return LWSE_ERR_OOM;
+  const size_t slice_out = align256((size_t)grid * slice_rows * sizeof(lwse_place_out));
+  LWSE_CUDA(e, e->rp_extra.reserve((size_t)n_extra * sizeof(lwse_place_req) + 16));
+  LWSE_CUDA(e, e->rp_slices.reserve(slice_out + (size_t)grid * slice_rows * 4 + 16));
+  p.extra = (lwse_place_req*)e->rp_extra.p;
+  p.nodes = (const lwse_node_rec*)e->nodes.p;
+  p.occupancy = (const uint32_t*)e->r_occ.p;
+  p.dom_first = (const uint32_t*)e->dom_first.p;
+  p.node_order = (const uint32_t*)e->node_order.p;
+  p.reqs = (const lwse_place_req*)e->r_preq.p;
+  p.base = (const lwse_place_out*)e->r_pout.p;
+  p.n_nodes = nn;
+  p.n_domains = nd;
+  p.n_reqs = nr;
+  p.n_namespaces = n_ns;
+  p.round = e->rp_round.p;
+  p.round_bytes = round_bytes;
+  p.s_out = (lwse_place_out*)e->rp_slices.p;
+  p.s_unpinned = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(e->rp_slices.p) + slice_out);
+  p.slice_rows = (uint32_t)slice_rows;
+  p.grid = (uint32_t)grid;
+  // the baseline's totals (a diff of the baseline rows against themselves counts them), every namespace's index
+  launched = lwse::launch_place_whatif_diff(p.base, p.base, 0, nr, nullptr, nullptr, nullptr, 0, d_words + 16, e->sm_count, s,
+                                            &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (grid) {
+    LWSE_CUDA(e, cudaMemsetAsync(e->rp_touched.p, 1, n_ns, s));
+    LWSE_CUDA(e, cudaMemsetAsync(e->rp_round.p, 0, round_bytes, s));  // (the index counts start at zero)
+    if (e->node_index_stale)
+      if (const int rc = own_node_index(e, p.nodes, s, &p.dom_first, &p.node_order, nullptr); rc != LWSE_OK) return rc;
+    launched = lwse::launch_place_whatif_index(p.reqs, nr, n_ns, (const uint8_t*)e->rp_touched.p, nn, nd, e->rp_round.p,
+                                               e->sm_count, s, &cuda_err);
+    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  }
+  launched = lwse::launch_rollout_place(&p, 1, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 64, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(q->out, p.rows_out, (size_t)n * sizeof(lwse_rollout_place), cudaMemcpyDeviceToHost, s));
+  if (const uint64_t listed = std::min<uint64_t>(n_extra, q->extra_capacity))
+    LWSE_CUDA(e, cudaMemcpyAsync(q->extra, p.extra, (size_t)listed * sizeof(lwse_place_req), cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  q->n_solved = words[4];
+  q->n_strands = words[5];
+  q->n_surge = (uint64_t)words[6] | (uint64_t)words[7] << 32;
+  q->n_stranded = (uint64_t)words[8] | (uint64_t)words[9] << 32;
   return LWSE_OK;
 }
 

@@ -382,6 +382,48 @@ int launch_drain_restart_pairs(const DrainBudgetCostLaunch* p, unsigned long lon
                                cudaStream_t s, int* cuda_err);
 int launch_place_ns_drain(const DrainPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err);
 
+// ---- lwse_rollout_place_kernels.cu ----
+// Rollout placement (lwse_resident_rollout_place).  Entry i: resident row rows[i], namespace ns[i], proposal
+// recs[i] (null: the resident row), forecast row fc[fc_by_row ? rows[i] : i].
+struct RolloutPlaceLaunch {
+  const lwse_lws_rec* lws;        // the resident rows
+  const lwse_group_rec* groups;   // the resident group rows
+  uint32_t n_groups;
+  const uint32_t* rows;           // [n]
+  const uint32_t* ns;             // [n]
+  const lwse_lws_rec* recs;       // [n] or null
+  const lwse_lws_forecast* fc;
+  bool fc_by_row;
+  uint32_t n;
+  uint32_t* rows_out;             // [n] lwse_rollout_place, 16 words each
+  uint4* ent;                     // [n] {first extra row, |E_i|, group_base, group_count}
+  uint32_t* e_count;              // [n] |E_i| (zero between calls: the scan clears it)
+  uint32_t* e_first;              // [n + 1]
+  uint32_t* e_cursor;             // [n]
+  uint2* items;                   // [n] {entry, namespace}: answerable entries with E_i non-empty
+  uint32_t* counts;               // 32 words, zeroed by the caller: [0] items [1] max |E_i| [2..3] sum |E_i| (u64),
+                                  // [4..9] the finish's totals, [16..22] a place_whatif_diff block over the baseline
+                                  // alone (its PLACED / UNSCHEDULABLE / CONFLICT at [20..22])
+  lwse_place_req* extra;          // [sum |E_i|]
+  // the solve
+  const lwse_node_rec* nodes;
+  const uint32_t* occupancy;
+  const uint32_t* dom_first;
+  const uint32_t* node_order;
+  const lwse_place_req* reqs;     // the resident request rows
+  const lwse_place_out* base;     // the baseline rows
+  uint32_t n_nodes, n_domains, n_reqs, n_namespaces;
+  void* round;                    // namespace-form scratch holding the index of every namespace
+  size_t round_bytes;
+  lwse_place_out* s_out;          // [grid * slice_rows]
+  uint32_t* s_unpinned;           // [grid * slice_rows]
+  uint32_t slice_rows, grid;
+};
+// Pass 0: the count kernel (flags, |E_i|, the rows started, the items).  Pass 1 (after the host read max |E_i|):
+// the scan, the fill of the extra rows, the capacities and the solve, then the finish.
+int launch_rollout_place(const RolloutPlaceLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err);
+
 // ---- lwse_drain_wave_kernels.cu ----
 // lwse_resident_drain_waves.  out: the query totals (16 B), m lwse_drain_wave_key rows, then max_waves
 // lwse_drain_wave rows (the opened ones written).  counts (device, u64, zeroed by the caller): [0] the restart pairs

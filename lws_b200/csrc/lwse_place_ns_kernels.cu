@@ -123,6 +123,21 @@ struct SetNsView {
 };
 static_assert(sizeof(SetNsView) <= sizeof(CUtensorMap), "the view travels in the tensor-map parameter");
 
+// The rollout instance (lwse_resident_rollout_place): DrainNsView's items {entry, namespace}, slices, baseline and
+// rows (u_first, u_rows, pos, marks and by_domain unused); per entry its extra rows E_i after the namespace's
+// resident rows.
+struct RollNsView {
+  DrainNsView d;
+  const lwse_place_req* extra;  // every entry's E_i, entry i's at ent[i].x
+  const uint4* ent;             // [entries] {first extra row, |E_i|, group_base, group_count}
+  uint32_t n_resident;          // extra row j of an entry has row index (and key) n_resident + j
+};
+static_assert(sizeof(RollNsView) <= sizeof(CUtensorMap), "the view travels in the tensor-map parameter");
+
+// The rollout instance's counters, words 4..14 of the entry's lwse_rollout_place row: placed, stranded, own_lost,
+// bumped, then the what-if counters (the three totals as deltas against the baseline).
+constexpr uint32_t kRollCounts = 11;
+
 __device__ __forceinline__ uint32_t mix32n(uint32_t x) {
   x ^= x >> 16;
   x *= 0x85EBCA6Bu;
@@ -457,7 +472,10 @@ __device__ __forceinline__ void diff_row(const PlaceNsArgs& a, uint32_t r, const
 // capacities are rebuilt from the resident ones minus what the column drains (every domain of W_c and k zeroed, or
 // every domain lowered by the free slots of its drained nodes), level 2 skips every drained node, and U_{W_c} ∪ U_k
 // read as unpinned; the namespace's diff goes to column c's row.
-template <bool kScan, bool kIndexed, bool kDrain = false, bool kSet = false>
+// kRoll (with kDrain): the rollout instance.  Item {i, ns} solves ns with entry i's extra rows E_i: positions run over
+// the namespace's resident rows through the index, then over E_i's rows (row index n_resident + j); nothing is
+// lowered or unpinned; the namespace's diff goes to entry i's row.
+template <bool kScan, bool kIndexed, bool kDrain = false, bool kSet = false, bool kRoll = false>
 __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
     place_ns_kernel(const PlaceNsArgs a, const __grid_constant__ CUtensorMap words_map) {
   extern __shared__ uint8_t s_dyn[];
@@ -488,6 +506,8 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
   const DrainNsView* const drain = reinterpret_cast<const DrainNsView*>(&words_map);
   const SetNsView* const set = reinterpret_cast<const SetNsView*>(&words_map);
   static_assert(!kSet || kDrain, "the set instance is a drain instance");
+  const RollNsView* const roll = reinterpret_cast<const RollNsView*>(&words_map);
+  static_assert(!kRoll || (kDrain && !kSet), "the rollout instance is a drain instance of its own");
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5, n_warps = blockDim.x >> 5;
   const uint32_t* words = table_bytes ? s_words : a.g_words;
   const uint32_t* order = table_bytes ? s_order : a.node_order;
@@ -537,7 +557,9 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
       key = w.x;
       ns = w.y;
     }
-    const uint32_t first = __ldcg(a.ns_first + ns), last = __ldcg(a.ns_first + ns + 1u);
+    uint4 ent = make_uint4(0u, 0u, 0u, 0u);  // kRoll: the entry's {first extra row, |E_i|, group range}
+    if constexpr (kRoll) ent = __ldcg(roll->ent + key);
+    const uint32_t first = __ldcg(a.ns_first + ns), last_res = __ldcg(a.ns_first + ns + 1u), last = last_res + ent.y;
     if (tid == 0) {
       s_n_unp = 0u;
       s_n_cand = 0u;
@@ -585,7 +607,7 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
         s_free[d] = f;
       }
       __syncthreads();
-    } else if constexpr (kDrain) {
+    } else if constexpr (kDrain && !kRoll) {
       const DrainNsView& dv = *drain;
       for (uint32_t p = tid; p < last - first; p += blockDim.x) dv.marks[slice + p] = 0u;
       __syncthreads();
@@ -613,9 +635,15 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
       }
       __syncthreads();
     }
+    auto req_at = [&](uint32_t r, uint32_t p) -> const uint4* {  // the request row at position p (row r)
+      if constexpr (kRoll) {
+        if (p >= last_res) return reinterpret_cast<const uint4*>(roll->extra + ent.x + (p - last_res));
+      }
+      return reinterpret_cast<const uint4*>(a.reqs + r);
+    };
     auto req_hi = [&](uint32_t r, uint32_t p) -> uint4 {  // the request's second half, U_k unpinned for kDrain
-      uint4 hi = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r) + 1);
-      if constexpr (kDrain) {
+      uint4 hi = ldg_keep(req_at(r, p) + 1);
+      if constexpr (kDrain && !kRoll) {
         if (__ldcg(drain->marks + slice + (p - first))) hi.w = LWSE_NONE;
       }
       return hi;
@@ -626,6 +654,9 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
     uint4 k_lo[kNsKeep], k_hi[kNsKeep];
     uint32_t k_dom[kNsKeep], k_row[kNsKeep];
     auto row_of = [&](uint32_t p) -> uint32_t {  // position in the namespace's range -> request row
+      if constexpr (kRoll) {
+        if (p >= last_res) return roll->n_resident + (p - last_res);
+      }
       if constexpr (kIndexed) return __ldcg(a.ns_rows + p);
       return p;
     };
@@ -635,7 +666,7 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
       if (p < last) {
         const uint32_t r = row_of(p);
         if constexpr (kIndexed) k_row[j] = r;
-        k_lo[j] = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r));
+        k_lo[j] = ldg_keep(req_at(r, p));
         k_hi[j] = req_hi(r, p);
       }
     }
@@ -691,7 +722,7 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
     }
     for (uint32_t p = first + tid + kNsKeep * blockDim.x; p < last; p += blockDim.x) {  // big namespaces: the rest, unkept
       const uint32_t r = row_of(p);
-      claim(r, kDrain ? p - first : r, ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r)), req_hi(r, p));
+      claim(r, kDrain ? p - first : r, ldg_keep(req_at(r, p)), req_hi(r, p));
     }
     __syncthreads();
     // results of the pinned requests: final from here on (pinned keys are below every unpinned key)
@@ -705,7 +736,7 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
     }
     for (uint32_t p = first + tid + kNsKeep * blockDim.x; p < last; p += blockDim.x) {
       const uint32_t r = row_of(p);
-      const uint4 lo = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + r)), hi = req_hi(r, p);
+      const uint4 lo = ldg_keep(req_at(r, p)), hi = req_hi(r, p);
       uint32_t d = LWSE_NONE;
       if (hi.w != LWSE_NONE && hi.w < a.n_nodes) {
         const uint4 nr = ldg_keep(reinterpret_cast<const uint4*>(a.nodes + hi.w));
@@ -756,9 +787,10 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
           q = s_req[k];
         } else {  // overflow: the state lives in the result row (written by this warp only)
           q.r = __ldcg(a.unpinned + ubase + k);
-          const uint32_t qrow = kDrain ? __ldcg(a.ns_rows + first + q.r) : q.r;
+          const uint32_t qrow = kRoll ? row_of(first + q.r) : kDrain ? __ldcg(a.ns_rows + first + q.r) : q.r;
           const uint4 o = __ldcg(reinterpret_cast<const uint4*>(obase + q.r));
-          const uint4 lo = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + qrow)), hi = ldg_keep(reinterpret_cast<const uint4*>(a.reqs + qrow) + 1);
+          const uint4* const qreq = kRoll ? req_at(qrow, first + q.r) : reinterpret_cast<const uint4*>(a.reqs + qrow);
+          const uint4 lo = ldg_keep(qreq), hi = ldg_keep(qreq + 1);
           q.key = ns_place_key(u64_of(lo.x, lo.y), qrow, false);
           q.key_lo = lo.z;
           q.key_hi = lo.w;
@@ -876,7 +908,48 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
       }
     }
     __syncthreads();
-    if constexpr (kDrain) {  // the namespace's rows against the baseline, reduced in the CTA, one atomic per field
+    if constexpr (kRoll) {  // the namespace's rows against the baseline, E_i's rows, reduced in the CTA
+      const DrainNsView& dv = roll->d;
+      uint32_t c[kRollCounts] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+      for (uint32_t p = first + tid; p < last; p += blockDim.x) {
+        const uint4 v = __ldcg(reinterpret_cast<const uint4*>(obase + (p - first)));
+        const bool is = (v.z & LWSE_PLACE_PLACED) != 0u;
+        c[8] += is ? 1u : 0u;
+        c[9] += (v.z & LWSE_PLACE_UNSCHEDULABLE) ? 1u : 0u;
+        c[10] += (v.z & LWSE_PLACE_CONFLICT) ? 1u : 0u;
+        if (p >= last_res) {  // a row of E_i
+          c[0] += is ? 1u : 0u;
+          c[1] += is ? 0u : 1u;
+          continue;
+        }
+        const uint32_t r = row_of(p);
+        const uint4 o = __ldg(reinterpret_cast<const uint4*>(dv.base + r));
+        const bool was = (o.z & LWSE_PLACE_PLACED) != 0u;
+        const bool own = __ldg(&a.reqs[r].group) - ent.z < ent.w;
+        c[2] += (own && was && !is) ? 1u : 0u;
+        c[3] += (!own && was && !is) ? 1u : 0u;
+        c[4] += (v.x != o.x || v.y != o.y || v.z != o.z || v.w != o.w) ? 1u : 0u;
+        c[5] += (was && !is) ? 1u : 0u;
+        c[6] += (was && is && o.x != v.x) ? 1u : 0u;
+        c[7] += (!was && is) ? 1u : 0u;
+        c[8] -= was ? 1u : 0u;
+        c[9] -= (o.z & LWSE_PLACE_UNSCHEDULABLE) ? 1u : 0u;
+        c[10] -= (o.z & LWSE_PLACE_CONFLICT) ? 1u : 0u;
+      }
+      uint32_t* const s_rcnt = reinterpret_cast<uint32_t*>(s_req);  // (the request cache is free after the rounds)
+      if (tid < kRollCounts) s_rcnt[tid] = 0u;
+      __syncthreads();
+#pragma unroll
+      for (uint32_t f = 0; f < kRollCounts; f++) {
+        const uint32_t sum = __reduce_add_sync(0xFFFFFFFFu, c[f]);
+        if (lane == 0 && sum) atomicAdd(&s_rcnt[f], sum);
+      }
+      __syncthreads();
+      uint32_t* erow = dv.rows + (size_t)key * 16u;
+      if (tid < kRollCounts && s_rcnt[tid]) atomicAdd(erow + 4u + tid, s_rcnt[tid]);
+      if (tid == kRollCounts) atomicAdd(erow + 15u, 1u);  // namespaces_solved
+      __syncthreads();
+    } else if constexpr (kDrain) {  // the namespace's rows against the baseline, reduced in the CTA, one atomic per field
       const DrainNsView& dv = *drain;
       uint32_t c[kDrainCounts] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
       for (uint32_t p = first + tid; p < last; p += blockDim.x) {
@@ -1342,6 +1415,73 @@ int launch_place_ns_drain_set(const DrainPlaceWavesLaunch* d, int sm_count, cuda
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
   return 1;
+}
+
+// The rollout placement solve: the capacities of the node index (the condense kernel's part A alone), then the
+// rollout instance over p->grid CTAs.  The round scratch holds the namespace index of every namespace.
+int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  const NsLayout l = ns_layout(p->n_nodes, p->n_domains, p->n_reqs, p->n_namespaces);
+  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) {
+    *cuda_err = (int)cudaErrorInvalidValue;
+    return -1;
+  }
+  uint8_t* base = static_cast<uint8_t*>(p->round);
+  PlaceNsArgs a{};
+  a.nodes = p->nodes;
+  a.reqs = p->reqs;
+  a.occupancy = p->occupancy;
+  a.dom_first = p->dom_first;
+  a.node_order = p->node_order;
+  a.g_words = reinterpret_cast<uint32_t*>(base + l.words);
+  a.g_nodes2 = reinterpret_cast<uint32_t*>(base + l.nodes2);
+  a.g_dom_free = reinterpret_cast<uint32_t*>(base + l.dom_free);
+  a.ns_first = reinterpret_cast<uint32_t*>(base + l.ns_first);
+  a.ns_rows = reinterpret_cast<uint32_t*>(base + l.ns_rows);
+  a.ns_count = reinterpret_cast<uint32_t*>(base + l.ns_count);
+  a.ns_cursor = reinterpret_cast<uint32_t*>(base + l.ns_cursor);
+  a.counters = reinterpret_cast<uint32_t*>(base + l.counters) + 4u * 8u;  // a block no other call uses
+  a.n_nodes = p->n_nodes;
+  a.n_domains = p->n_domains;
+  a.n_namespaces = p->n_namespaces;
+  a.n_parts = 1u;
+  a.word_rows = l.word_rows;
+  {
+    uint64_t grid = ((uint64_t)p->n_domains * 32u + 255) / 256;
+    if (grid < 1) grid = 1;
+    if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
+    place_condense_kernel<<<(unsigned)grid, 256, 0, s>>>(a);  // (a.n_reqs = 0: capacities only)
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+  }
+  RollNsView v{};
+  v.d.items = p->items;
+  v.d.n_items = p->counts;
+  v.d.item_capacity = p->n;
+  v.d.base = p->base;
+  v.d.rows = p->rows_out;
+  v.d.slice_rows = p->slice_rows;
+  v.extra = p->extra;
+  v.ent = p->ent;
+  v.n_resident = p->n_reqs;
+  CUtensorMap view;
+  memset(&view, 0, sizeof(view));
+  memcpy(&view, &v, sizeof(v));
+  a.n_reqs = p->n_reqs;
+  a.out = p->s_out;
+  a.unpinned = p->s_unpinned;
+  const size_t smem = ns_smem_bytes(l.word_rows, p->n_domains, false, false);
+  static thread_local size_t attr_set = 0;
+  if (smem > attr_set) {
+    const cudaError_t e =
+        cudaFuncSetAttribute(place_ns_kernel<false, true, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    attr_set = smem;
+  }
+  place_ns_kernel<false, true, true, false, true><<<p->grid, kNsThreads, smem, s>>>(a, view);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+  return 2;
 }
 
 int launch_index_scan(uint32_t* d_count, uint32_t* d_first, uint32_t* d_cursor, uint32_t n, cudaStream_t s, int* cuda_err) {

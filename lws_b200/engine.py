@@ -54,6 +54,7 @@ SYMBOLS = {
     "lwse_resident_ds_drain_cost": ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int),
     "lwse_resident_ds_drain_waves": ([C.c_void_p, C.POINTER(R.DsDrainWavesQuery)], C.c_int),
     "lwse_resident_drain_place_waves": ([C.c_void_p, C.POINTER(R.DrainPlaceWavesQuery)], C.c_int),
+    "lwse_resident_rollout_place": ([C.c_void_p, C.POINTER(R.RolloutPlaceQuery)], C.c_int),
     "lwse_place_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
         C.c_int,
@@ -900,6 +901,42 @@ class Engine:
         out = self._lws_forecast(call, n, steps, step_capacity)
         out["now"] = now
         return out
+
+    def resident_rollout_place(self, rows, ns, recs=None, extra=False):
+        """lwse_resident_rollout_place: for each entry (resident LWS row ``rows[i]``, namespace id ``ns[i]`` and,
+        with ``recs``, a proposed LWS_REC as ``resident_rollout_whatif`` takes it), whether the groups its rollout
+        adds up to the forecast's peak find an exclusive domain — each entry answered on its own, as the
+        composition ``resident_forecast`` (or ``resident_rollout_whatif``) → extra request rows →
+        ``resident_place_whatif`` would (lwse.h, "rollout placement").  → dict: ``rows`` (``records.ROLLOUT_PLACE``,
+        one per entry), the query's ``lws_rows`` and ``ns``, the totals of ``records.ROLLOUT_PLACE_TOTALS`` and,
+        with ``extra``, ``extra``: every entry's extra request rows (PLACE_REQ), entry after entry in query order.  Changes nothing resident and waits
+        for no tick."""
+        rows = np.ascontiguousarray(rows, dtype=np.uint32)
+        ns = np.ascontiguousarray(ns, dtype=np.uint32)
+        assert len(ns) == len(rows)
+        n = len(rows)
+        if recs is not None:
+            recs = np.asarray(recs)
+            assert recs.dtype == R.LWS_REC and len(recs) == n
+            recs = _aligned16(recs)
+        out = R.aligned_empty(max(n, 1), R.ROLLOUT_PLACE)
+        q = R.RolloutPlaceQuery()
+        q.rows = R.ptr(rows) if n else None
+        q.ns = R.ptr(ns) if n else None
+        q.recs = R.ptr(recs) if (recs is not None and n) else None
+        q.n = n
+        q.out = R.ptr(out)
+        if extra:  # sized by a first call without them
+            probe = R.RolloutPlaceQuery.from_buffer_copy(q)
+            self._check(lib().lwse_resident_rollout_place(self._h, C.byref(probe)))
+            xs = R.aligned_empty(max(probe.n_surge, 1), R.PLACE_REQ)
+            q.extra, q.extra_capacity = R.ptr(xs), probe.n_surge
+        self._check(lib().lwse_resident_rollout_place(self._h, C.byref(q)))
+        res = {"rows": out[:n], "lws_rows": rows, "ns": ns}
+        res.update({k: getattr(q, k) for k in R.ROLLOUT_PLACE_TOTALS})
+        if extra:
+            res["extra"] = xs[: min(q.n_surge, probe.n_surge)]
+        return res
 
     # ------------------------------------------------------------- group keys
     def group_keys_host(self, strings) -> np.ndarray:

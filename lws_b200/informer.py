@@ -553,6 +553,39 @@ class IncrementalEncoder:
         rec["group_base"] = sl.group_base
         return sl.lws_row, rec[0]
 
+    def rollout_place_query(self, keys=None) -> tuple:
+        """The entries of ``Engine.resident_rollout_place`` for every resident exclusive object, or for the named
+        ``keys`` ((namespace, name); non-exclusive ones included, which the call flags) → (rows, ns), in key order.
+        Nothing in the encoder changes."""
+        if keys is None:
+            keys = [k for k, sl in self.slots.items()
+                    if int(self.lws["flags"][sl.lws_row]) & R.LWS_EXCLUSIVE_TOPOLOGY]
+        keys = sorted(keys)
+        rows = np.array([self.slots[k].lws_row for k in keys], dtype=np.uint32)
+        ns = np.array([self.ns_ids[k[0]] for k in keys], dtype=np.uint32)
+        return rows, ns
+
+    def rollout_place_proposal(self, item: encoder.LwsItem) -> tuple:
+        """``whatif_rollout``'s proposal plus the object's namespace id → (LWS row, LWS_REC row, ns), for
+        ``Engine.resident_rollout_place(rows, ns, recs)``.  KeyError for an object that is not resident."""
+        row, rec = self.whatif_rollout(item)
+        return row, rec, self.ns_ids[item.lws.namespace]
+
+    def rollout_place_report(self, result: dict) -> list:
+        """A ``resident_rollout_place`` answer as dicts, one per entry that strands or bumps, in query order:
+        ``namespace`` and ``name`` (None for a row no object holds), then the row's fields, its ``records.RPL_*``
+        flags named.  Nothing in the encoder changes."""
+        names = {sl.lws_row: k for k, sl in self.slots.items()}
+        out = []
+        for r, row in zip(np.asarray(result["lws_rows"]).tolist(), result["rows"]):
+            if not (int(row["flags"]) & (R.RPL_STRANDS | R.RPL_BUMPS)):
+                continue
+            ns, name = names.get(int(r), (None, None))
+            d = {"namespace": ns, "name": name, **{f: int(row[f]) for f in R.ROLLOUT_PLACE.names}}
+            d["flags"] = [v for b, v in R.RPL_NAMES.items() if int(row["flags"]) & b]
+            out.append(d)
+        return out
+
     def whatif_drain(self, node_names) -> np.ndarray:
         """The node rows of the named nodes, for ``Engine.resident_drain_whatif`` (sorted, each once)."""
         return np.array(sorted({self.node_index[n] for n in node_names}), dtype=np.uint32)

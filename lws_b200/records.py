@@ -824,6 +824,50 @@ class DrainPlaceWavesQuery(C.Structure):
 assert C.sizeof(DrainPlaceWavesQuery) == 64
 
 
+# lwse_rollout_place: per entry, whether the groups its rollout adds find an exclusive domain
+ROLLOUT_PLACE = np.dtype(
+    [("flags", "<u4"), ("fc_flags", "<u4"), ("peak", "<i4"), ("surge", "<u4"), ("placed", "<u4"), ("stranded", "<u4"),
+     ("own_lost", "<u4"), ("bumped", "<u4"), ("n_changed", "<u4"), ("n_lost", "<u4"), ("n_moved", "<u4"),
+     ("n_gained", "<u4"), ("n_placed", "<u4"), ("n_unschedulable", "<u4"), ("n_conflict", "<u4"),
+     ("namespaces_solved", "<u4")],
+    align=False,
+)
+assert ROLLOUT_PLACE.itemsize == 64
+
+RPL_SOLVED = 1 << 0
+RPL_NOT_EXCLUSIVE = 1 << 1
+RPL_NOT_FORECAST = 1 << 2
+RPL_NOT_MODELLED = 1 << 3
+RPL_STRANDS = 1 << 4
+RPL_BUMPS = 1 << 5
+RPL_NAMES = {RPL_SOLVED: "solved", RPL_NOT_EXCLUSIVE: "not_exclusive", RPL_NOT_FORECAST: "not_forecast",
+             RPL_NOT_MODELLED: "not_modelled", RPL_STRANDS: "strands", RPL_BUMPS: "bumps"}
+ROLLOUT_PLACE_TOTALS = ("n_solved", "n_strands", "n_surge", "n_stranded")
+
+
+class RolloutPlaceQuery(C.Structure):
+    """lwse_rollout_place_query: entries (LWS row, namespace id, optional proposed LWS_REC) in, one ROLLOUT_PLACE
+    row per entry, optionally every entry's extra PLACE_REQ rows, and the ROLLOUT_PLACE_TOTALS out."""
+
+    _fields_ = [
+        ("rows", C.c_void_p),
+        ("ns", C.c_void_p),
+        ("recs", C.c_void_p),
+        ("n", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("out", C.c_void_p),
+        ("extra", C.c_void_p),
+        ("extra_capacity", C.c_uint64),
+        ("n_solved", C.c_uint32),
+        ("n_strands", C.c_uint32),
+        ("n_surge", C.c_uint64),
+        ("n_stranded", C.c_uint64),
+    ]
+
+
+assert C.sizeof(RolloutPlaceQuery) == 80
+
+
 class Config(C.Structure):
     _fields_ = [
         ("abi_version", C.c_uint32),
