@@ -19,22 +19,36 @@
 
 namespace {
 
+// The CUDA objects all engines hold (allocations, streams, events, graph executables, peer mappings): the owners
+// below count each one they acquire and release (lwse_debug_cuda_objects).
+std::atomic<int64_t> g_cuda_objects{0};
+
 // A device buffer that only grows (sweeps reuse their staging memory).
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { release(); }
   cudaError_t reserve(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
+    release();
     size_t want = bytes + bytes / 8 + 256;
     cudaError_t e = cudaMalloc(&p, want);
-    if (e == cudaSuccess) cap = want;
+    if (e == cudaSuccess) {
+      cap = want;
+      ++g_cuda_objects;
+    } else {
+      p = nullptr;
+    }
     return e;
   }
   void release() {
-    if (p) cudaFree(p);
+    if (p) {
+      cudaFree(p);
+      --g_cuda_objects;
+    }
     p = nullptr;
     cap = 0;
   }
@@ -46,16 +60,19 @@ struct PinBuf {
   void* h = nullptr;
   void* d = nullptr;
   size_t cap = 0;
+  PinBuf() = default;
+  PinBuf(const PinBuf&) = delete;
+  PinBuf& operator=(const PinBuf&) = delete;
+  ~PinBuf() { release(); }
   cudaError_t reserve(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
-    if (h) cudaFreeHost(h);
-    h = d = nullptr;
-    cap = 0;
+    release();
     const size_t want = bytes + bytes / 8 + 4096;
     cudaError_t e = cudaHostAlloc(&h, want, cudaHostAllocMapped);
     if (e == cudaSuccess) e = cudaHostGetDevicePointer(&d, h, 0);
     if (e == cudaSuccess) {
       cap = want;
+      ++g_cuda_objects;
       memset(h, 0, want);  // sequence words and counters start at zero
     } else if (h) {
       cudaFreeHost(h);
@@ -64,7 +81,10 @@ struct PinBuf {
     return e;
   }
   void release() {
-    if (h) cudaFreeHost(h);
+    if (h) {
+      cudaFreeHost(h);
+      --g_cuda_objects;
+    }
     h = d = nullptr;
     cap = 0;
   }
@@ -75,6 +95,81 @@ struct PinBuf {
   template <typename T>
   T* dev_of(const T* host_ptr) const {
     return reinterpret_cast<T*>(static_cast<uint8_t*>(d) + (reinterpret_cast<const uint8_t*>(host_ptr) - static_cast<uint8_t*>(h)));
+  }
+};
+
+// A CUDA handle that destroys itself.  It converts to the raw handle, so it passes wherever one is taken.
+template <typename T, cudaError_t (*Destroy)(T)>
+struct Owned {
+  T h = nullptr;
+  Owned() = default;
+  Owned(const Owned&) = delete;
+  Owned& operator=(const Owned&) = delete;
+  ~Owned() { reset(); }
+  operator T() const { return h; }
+  void reset() {
+    if (h) {
+      Destroy(h);
+      --g_cuda_objects;
+    }
+    h = nullptr;
+  }
+
+ protected:
+  cudaError_t adopt(cudaError_t e) {  // the result of the call that created h
+    if (e == cudaSuccess)
+      ++g_cuda_objects;
+    else
+      h = nullptr;
+    return e;
+  }
+};
+
+struct Stream : Owned<cudaStream_t, cudaStreamDestroy> {
+  // `highest`: at the device's highest stream priority
+  cudaError_t ensure(unsigned flags, bool highest = false) {
+    if (h) return cudaSuccess;
+    if (!highest) return adopt(cudaStreamCreateWithFlags(&h, flags));
+    int least = 0, greatest = 0;
+    const cudaError_t e = cudaDeviceGetStreamPriorityRange(&least, &greatest);
+    return e != cudaSuccess ? e : adopt(cudaStreamCreateWithPriority(&h, flags, greatest));
+  }
+};
+
+struct Event : Owned<cudaEvent_t, cudaEventDestroy> {
+  cudaError_t ensure(unsigned flags) { return h ? cudaSuccess : adopt(cudaEventCreateWithFlags(&h, flags)); }
+};
+
+struct GraphExec : Owned<cudaGraphExec_t, cudaGraphExecDestroy> {
+  cudaError_t ensure(cudaGraph_t graph) { return h ? cudaSuccess : adopt(cudaGraphInstantiate(&h, graph, 0)); }
+};
+
+// The exchange buffers of the peers, by rank (lwse_exchange_connect).  The own rank's entry is the engine's own
+// buffer: it is not opened here and never closed.
+struct PeerMaps {
+  void* p[LWSE_MAX_RANKS] = {};
+  bool opened[LWSE_MAX_RANKS] = {};
+  PeerMaps() = default;
+  PeerMaps(const PeerMaps&) = delete;
+  PeerMaps& operator=(const PeerMaps&) = delete;
+  ~PeerMaps() { close(); }
+  cudaError_t open(uint32_t rank, const cudaIpcMemHandle_t& handle) {
+    const cudaError_t e = cudaIpcOpenMemHandle(&p[rank], handle, cudaIpcMemLazyEnablePeerAccess);
+    if (e == cudaSuccess) {
+      opened[rank] = true;
+      ++g_cuda_objects;
+    }
+    return e;
+  }
+  void close() {
+    for (uint32_t r = 0; r < LWSE_MAX_RANKS; r++) {
+      if (opened[r]) {
+        cudaIpcCloseMemHandle(p[r]);
+        --g_cuda_objects;
+      }
+      opened[r] = false;
+      p[r] = nullptr;
+    }
   }
 };
 
@@ -89,11 +184,11 @@ struct TickPlaceResult {
 struct lwse_engine {
   int device = 0;
   int sm_count = lwse::kSmCount;
-  cudaStream_t stream = nullptr;
-  cudaStream_t side_stream = nullptr;  // placement round of lwse_reconcile_device
-  cudaStream_t hist_stream = nullptr;  // copies the unpinned-request count of a round to the host, off the critical path
-  cudaEvent_t ev_hist = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  Stream stream;
+  Stream side_stream;                  // placement round of lwse_reconcile_device
+  Stream hist_stream;                  // copies the unpinned-request count of a round to the host, off the critical path
+  Event ev_hist;
+  Event ev_fork, ev_join;
   std::mutex mu;
   int last_cuda_error = 0;
   uint64_t launches = 0;
@@ -140,7 +235,7 @@ struct lwse_engine {
   size_t chg_bytes = 0;              // one slot of `chg`
   // a tick replayed as a CUDA graph (one cudaGraphLaunch instead of ~10 launches)
   struct TickGraph {
-    cudaGraphExec_t exec = nullptr;
+    GraphExec exec;
     uint32_t seen = 0;      // eager ticks with this key so far (the first one lets every buffer settle)
     uint32_t kernels = 0;   // kernel nodes (launch accounting)
     bool failed = false;    // capture or instantiation failed once: this key stays eager
@@ -149,19 +244,19 @@ struct lwse_engine {
   std::unordered_map<uint32_t, TickGraph> tick_graphs;
   PinBuf tdesc;                      // 2 slots x kScatterDescBytes: the scatter's segment descriptors of the tick of that parity
   DevBuf tdesc_dev;                  // device copy (the copy node at the root of a tick graph fills it)
-  cudaStream_t copy_stream = nullptr;  // the patch copy of a replayed tick: overlaps the previous tick's kernels
-  cudaEvent_t ev_dma = nullptr;
-  cudaStream_t pub_stream = nullptr;   // the publish kernels: tick k+1 starts while tick k's changed rows travel to the host
-  cudaEvent_t ev_done = nullptr;       // behind the last kernel of a tick on the engine's stream (both branches joined)
-  cudaEvent_t ev_mid = nullptr;        // (graph capture) between the condense and the namespace kernel
+  Stream copy_stream;                  // the patch copy of a replayed tick: overlaps the previous tick's kernels
+  Event ev_dma;
+  Stream pub_stream;                   // the publish kernels: tick k+1 starts while tick k's changed rows travel to the host
+  Event ev_done;                       // behind the last kernel of a tick on the engine's stream (both branches joined)
+  Event ev_mid;                        // (graph capture) between the condense and the namespace kernel
   int use_graph = 1;                 // LWSE_TICK_GRAPH: 0 never, 1 when a tick is in flight (default), 2 always
   uint64_t graph_ticks = 0;
-  cudaEvent_t ev_pub = nullptr;      // behind the previous tick's publish kernel: the next tick's side stream starts there
-  uint32_t* h_counts = nullptr;      // pinned, 2 words
+  Event ev_pub;                      // behind the previous tick's publish kernel: the next tick's side stream starts there
+  PinBuf h_counts;                   // 2 words
   DevBuf h_counts_dev;               // event-pod count of the host entry point's sweep
   uint32_t place_calls = 0;          // selects the scratch half
   uint32_t place_geometry[4] = {0, 0, 0, 0};  // (n_reqs, n_namespaces, nodes, domains) the scratch was laid out for
-  cudaEvent_t ev_place = nullptr;    // end of the last placement call: the next one (any stream) orders behind it
+  Event ev_place;                    // end of the last placement call: the next one (any stream) orders behind it
   bool place_pending = false;
   DevBuf place_ns_scratch;           // namespace-parallel form (grouped request tables)
   uint32_t place_ns_calls = 0;
@@ -178,7 +273,7 @@ struct lwse_engine {
   const uint32_t* place_unpinned = nullptr;  // device: its unpinned-request count
   DevBuf ds, ds_roles, ds_revroles, ds_out, ds_role_out, ds_revrole_out;
   // resident DS tables (lwse_ds_resident_*): their own stream, never ordered with the LWS ticks
-  cudaStream_t ds_stream = nullptr;
+  Stream ds_stream;
   DevBuf rd_ds, rd_roles, rd_revroles;
   DevBuf rd_out[2], rd_role_out[2], rd_revrole_out[2];  // output sets, alternating by tick parity
   DevBuf rd_marks, rd_ones;          // DS rows the tick's scatter patched / a column of ones the scatter copies there
@@ -192,7 +287,7 @@ struct lwse_engine {
   bool rd_loaded = false, rd_all = false;
   DevBuf rd_links;                   // LWSE_TABLE_DS_LINKS: revision-role row → resident LWS row
   bool rd_linked = false;            // a link patch arrived since the DS load: ticks run the linked sweep
-  cudaEvent_t ev_ds_link = nullptr;  // the engine's stream at the start of a linked DS tick
+  Event ev_ds_link;                  // the engine's stream at the start of a linked DS tick
   lwse_ds_tick_info last_ds_info{};  // lwse_ds_resident_tick_info
   // rollout forecast (lwse_ds_forecast_*): a private copy of the revision-role rows, the replay's sweep
   // outputs, the forecast rows and the trajectory; never the DS tick's buffers
@@ -204,8 +299,8 @@ struct lwse_engine {
                                      // patches of LWS, group and pod rows
   // rolling-update forecast (lwse_lws_forecast_*): a snapshot of the LWS rows and group results, the private
   // flag slots, the forecast rows and the trajectory, on a stream of its own; never a tick's buffers
-  cudaStream_t lf_stream = nullptr;
-  cudaEvent_t ev_lf = nullptr;       // the engine's stream where a resident forecast takes its snapshot
+  Stream lf_stream;
+  Event ev_lf;                       // the engine's stream where a resident forecast takes its snapshot
   DevBuf lf_lws, lf_group_out, lf_slot_off, lf_slots, lf_fc, lf_steps, lf_totals;
   PinBuf lf_words;                   // the three totals, copied back
   // rollout what-if (lwse_resident_rollout_whatif): on lf_stream, the proposals' rows and their resident rows, the
@@ -217,9 +312,9 @@ struct lwse_engine {
                                      // since any patch of those rows made without a round
   // placement what-if (lwse_resident_place_whatif): patched copies of the node and request rows, the what-if
   // round's rows, its own node index and round scratch, on a stream of its own; never a tick's buffers
-  cudaStream_t wf_stream = nullptr;
-  cudaEvent_t ev_wf = nullptr;       // the engine's stream where a what-if takes its snapshot
-  cudaEvent_t ev_wf_t0 = nullptr, ev_wf_t1 = nullptr;  // (LWSE_WHATIF_TIMING=1) around the last what-if's device work
+  Stream wf_stream;
+  Event ev_wf;                       // the engine's stream where a what-if takes its snapshot
+  Event ev_wf_t0, ev_wf_t1;          // (LWSE_WHATIF_TIMING=1) around the last what-if's device work
   bool wf_timed = false;
   DevBuf wf_nodes, wf_reqs, wf_out, wf_dom_first, wf_node_order, wf_node_pos, wf_node_ix, wf_touched, wf_round, wf_list;
   PinBuf wf_stage;                   // the call's segments, extra rows and namespace mask (the scatter reads them here)
@@ -259,7 +354,7 @@ struct lwse_engine {
   // DS drain (lwse_resident_ds_drain*): lost[L] and the after copy of lws_out, the before / after sweep outputs, the
   // touched DS rows, the reverse link index (count | first | cursor) and its entries, the key rows, the (DS, key) table
   DevBuf dd_lost, dd_lws_after, dd_out[2], dd_role_out[2], dd_revrole_out[2], dd_rows, dd_index, dd_entries, dd_cost, dd_table;
-  cudaEvent_t ev_dd = nullptr;       // the DS stream where a DS drain starts
+  Event ev_dd;                       // the DS stream where a DS drain starts
   // DS rollout what-if (lwse_resident_ds_rollout_whatif): on the what-if stream, the proposals and the query's role
   // rows, the layout's counts, offsets and block sums, the proposed DS, role, revision-role and link rows, and the
   // linked sweep's outputs; the forecast that follows uses the fc_* scratch above
@@ -268,10 +363,10 @@ struct lwse_engine {
   PinBuf dw_words;                   // the layout's total, copied back
   uint32_t r_sweep_flags = 0;        // LWSE_SWEEP_GANG of the most recently submitted sweep (r_group_out's flags)
   DevBuf sha_bytes, sha_offsets, sha_digests, sha_ints;
-  uint32_t* h_rounds = nullptr;  // pinned
+  PinBuf h_rounds;
   // peer exchange of the multi-GPU placement step (lwse_exchange_*)
   DevBuf xch, xch_peers_dev;
-  void* xch_peer[LWSE_MAX_RANKS] = {};
+  PeerMaps xch_peer;
   uint32_t xch_world = 0, xch_rank = 0, xch_reqs_per_part = 0;
   uint64_t xch_stride = 0, xch_reqs_off = 0, xch_half = 0, xch_flags_off = 0, xch_step = 0;
   bool xch_connected = false;
@@ -304,11 +399,7 @@ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) ==
 
 // Tick graphs freeze device pointers and sizes in their kernel nodes: whatever reallocates or
 // resizes a resident buffer drops them (the next ticks re-capture).
-void invalidate_tick_graphs(lwse_engine* e) {
-  for (auto& kv : e->tick_graphs)
-    if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-  e->tick_graphs.clear();
-}
+void invalidate_tick_graphs(lwse_engine* e) { e->tick_graphs.clear(); }
 
 struct DeviceGuard {
   int prev = -1;
@@ -377,15 +468,6 @@ LWSE_API uint32_t lwse_shard_of(uint64_t uid_hash, uint32_t n_shards) {
   return (uint32_t)(x % n_shards);
 }
 
-// The placement round of a tick is short and latency-bound; at the highest priority its CTAs
-// take the first SM slots the sweep kernels free instead of queueing behind their blocks.
-static cudaError_t create_side_stream(cudaStream_t* s) {
-  int least = 0, greatest = 0;
-  cudaError_t e = cudaDeviceGetStreamPriorityRange(&least, &greatest);
-  if (e != cudaSuccess) return e;
-  return cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, greatest);
-}
-
 LWSE_API int lwse_create(const lwse_config* cfg, lwse_engine** out) {
   if (!cfg || !out) return LWSE_ERR_INVALID_ARG;
   *out = nullptr;
@@ -409,41 +491,24 @@ LWSE_API int lwse_create(const lwse_config* cfg, lwse_engine** out) {
     return LWSE_ERR_NO_DEVICE;
   }
   e->sm_count = prop.multiProcessorCount;
-  if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      create_side_stream(&e->side_stream) != cudaSuccess ||
-      cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&e->ev_pub, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&e->ev_dma, cudaEventDisableTiming) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&e->pub_stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreateWithFlags(&e->ev_done, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&e->ev_mid, cudaEventDisableTiming) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&e->hist_stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreateWithFlags(&e->ev_hist, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&e->ev_place, cudaEventDisableTiming) != cudaSuccess ||
-      cudaMallocHost(reinterpret_cast<void**>(&e->h_rounds), 64) != cudaSuccess ||
-      cudaMallocHost(reinterpret_cast<void**>(&e->h_counts), 64) != cudaSuccess) {
+  // The placement round of a tick (side stream) is short and latency-bound; at the highest priority its CTAs
+  // take the first SM slots the sweep kernels free instead of queueing behind their blocks.
+  if (e->stream.ensure(cudaStreamNonBlocking) != cudaSuccess ||
+      e->side_stream.ensure(cudaStreamNonBlocking, /*highest=*/true) != cudaSuccess ||
+      e->ev_fork.ensure(cudaEventDisableTiming) != cudaSuccess || e->ev_join.ensure(cudaEventDisableTiming) != cudaSuccess ||
+      e->ev_pub.ensure(cudaEventDisableTiming) != cudaSuccess || e->ev_dma.ensure(cudaEventDisableTiming) != cudaSuccess ||
+      e->copy_stream.ensure(cudaStreamNonBlocking) != cudaSuccess || e->pub_stream.ensure(cudaStreamNonBlocking) != cudaSuccess ||
+      e->ev_done.ensure(cudaEventDisableTiming) != cudaSuccess || e->ev_mid.ensure(cudaEventDisableTiming) != cudaSuccess ||
+      e->hist_stream.ensure(cudaStreamNonBlocking) != cudaSuccess || e->ev_hist.ensure(cudaEventDisableTiming) != cudaSuccess ||
+      e->ev_place.ensure(cudaEventDisableTiming) != cudaSuccess || e->h_rounds.reserve(64) != cudaSuccess ||
+      e->h_counts.reserve(64) != cudaSuccess) {
     (void)cudaGetLastError();
-    if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-    if (e->ev_join) cudaEventDestroy(e->ev_join);
-    if (e->ev_pub) cudaEventDestroy(e->ev_pub);
-    if (e->ev_dma) cudaEventDestroy(e->ev_dma);
-    if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-    if (e->ev_done) cudaEventDestroy(e->ev_done);
-    if (e->ev_mid) cudaEventDestroy(e->ev_mid);
-    if (e->pub_stream) cudaStreamDestroy(e->pub_stream);
-    if (e->ev_hist) cudaEventDestroy(e->ev_hist);
-    if (e->ev_place) cudaEventDestroy(e->ev_place);
-    if (e->hist_stream) cudaStreamDestroy(e->hist_stream);
-    if (e->side_stream) cudaStreamDestroy(e->side_stream);
-    if (e->stream) cudaStreamDestroy(e->stream);
     delete e;
     return LWSE_ERR_CUDA;
   }
   if (e->h_counts_dev.reserve(64) != cudaSuccess) {
     (void)cudaGetLastError();
-    lwse_destroy(e);
+    delete e;
     return LWSE_ERR_OOM;
   }
   {
@@ -454,83 +519,15 @@ LWSE_API int lwse_create(const lwse_config* cfg, lwse_engine** out) {
   return LWSE_OK;
 }
 
+// The members free themselves when the engine is deleted, with its device current.
 LWSE_API void lwse_destroy(lwse_engine* e) {
   if (!e) return;
-  {
-    DeviceGuard guard(e->device);
-    cudaStreamSynchronize(e->stream);
-    cudaStreamSynchronize(e->side_stream);
-    cudaStreamSynchronize(e->hist_stream);  // its copies target h_rounds, freed below
-    if (e->copy_stream) cudaStreamSynchronize(e->copy_stream);
-    if (e->pub_stream) cudaStreamSynchronize(e->pub_stream);
-    for (auto& kv : e->tick_graphs)
-      if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
-    e->tick_graphs.clear();
-    for (uint32_t p = 0; p < e->xch_world; p++)
-      if (e->xch_connected && p != e->xch_rank && e->xch_peer[p]) cudaIpcCloseMemHandle(e->xch_peer[p]);
-    e->xch.release();
-    e->xch_peers_dev.release();
-    DevBuf* bufs[] = {&e->nodes,      &e->dom_first, &e->node_order, &e->node_pos, &e->node_ix, &e->lws,  &e->groups,     &e->pod_state,   &e->pod_ident,
-                      &e->scan_scratch, &e->lws_out,
-                      &e->group_out,  &e->occupancy,   &e->place_reqs, &e->place_out,   &e->place_occ,
-                      &e->place_scratch, &e->ds,       &e->ds_roles,   &e->ds_revroles, &e->ds_out,
-                      &e->ds_role_out, &e->ds_revrole_out, &e->sha_bytes, &e->sha_offsets, &e->sha_digests, &e->sha_ints,
-                      &e->r_lws, &e->r_groups, &e->r_pst, &e->r_pid, &e->r_lws_out, &e->r_group_out, &e->r_scan,
-                      &e->r_counts, &e->r_occ, &e->r_preq, &e->r_pout, &e->r_pout_prev, &e->h_counts_dev, &e->place_ns_scratch,
-                      &e->arena_mirror, &e->stage_mirror, &e->chg_dev, &e->tdesc_dev,
-                      &e->rd_ds, &e->rd_roles, &e->rd_revroles, &e->rd_out[0], &e->rd_out[1], &e->rd_role_out[0],
-                      &e->rd_role_out[1], &e->rd_revrole_out[0], &e->rd_revrole_out[1], &e->rd_marks, &e->rd_ones,
-                      &e->rd_counters, &e->rd_stage_dev, &e->rd_links, &e->fc_rows, &e->fc_ds_out, &e->fc_role_out,
-                      &e->fc_revrole_out, &e->fc_ds, &e->fc_roles, &e->fc_steps, &e->fc_totals,
-                      &e->lf_lws, &e->lf_group_out, &e->lf_slot_off, &e->lf_slots, &e->lf_fc, &e->lf_steps, &e->lf_totals,
-                      &e->wf_nodes, &e->wf_reqs, &e->wf_out, &e->wf_dom_first, &e->wf_node_order, &e->wf_node_pos,
-                      &e->wf_node_ix, &e->wf_touched, &e->wf_round, &e->wf_list,
-                      &e->dr_state, &e->dr_groups, &e->dr_out, &e->dr_scan, &e->dr_mask, &e->dr_list, &e->dr_cost,
-                      &e->dr_domains, &e->dr_brows, &e->dr_bcost, &e->dr_table, &e->dr_bwords,
-                      &e->dp_cost, &e->dp_words, &e->dp_domfree, &e->dp_gidx, &e->dp_uidx, &e->dp_pairs, &e->dp_urows, &e->dp_pos,
-                      &e->dp_items, &e->dp_rows, &e->dp_touched, &e->dp_round, &e->dp_slices,
-                      &e->rp_in, &e->rp_rows, &e->rp_ent, &e->rp_idx, &e->rp_items, &e->rp_words, &e->rp_extra,
-                      &e->rp_touched, &e->rp_round, &e->rp_slices,
-                      &e->dd_lost, &e->dd_lws_after, &e->dd_out[0], &e->dd_out[1], &e->dd_role_out[0], &e->dd_role_out[1],
-                      &e->dd_revrole_out[0], &e->dd_revrole_out[1], &e->dd_rows, &e->dd_index, &e->dd_entries, &e->dd_cost,
-                      &e->dd_table, &e->rw_rows, &e->rw_lws, &e->rw_off, &e->rw_sums, &e->rw_groups, &e->rw_src,
-                      &e->rw_group_out, &e->rw_now, &e->rw_scan, &e->dw_props, &e->dw_qroles, &e->dw_count, &e->dw_off,
-                      &e->dw_sums, &e->dw_ds, &e->dw_roles, &e->dw_revroles, &e->dw_links, &e->dw_now, &e->dw_role_out,
-                      &e->dw_revrole_out, &e->dv_cost, &e->dv_words, &e->dv_ids, &e->dv_pos, &e->dv_kidx, &e->dv_pairs,
-                      &e->dv_recs, &e->dv_lidx, &e->dv_dense, &e->dv_lost, &e->dv_gwaves, &e->dv_rwaves, &e->dv_stamps,
-                      &e->dv_out, &e->dx_caps, &e->dx_out};
-    if (e->ds_stream) cudaStreamSynchronize(e->ds_stream);
-    if (e->lf_stream) cudaStreamSynchronize(e->lf_stream);
-    if (e->wf_stream) cudaStreamSynchronize(e->wf_stream);
-    for (DevBuf* b : bufs) b->release();
-    PinBuf* pins[] = {&e->arena, &e->stage, &e->chg, &e->tickw, &e->tdesc, &e->rd_pin, &e->rd_stage, &e->fc_words, &e->lf_words,
-                      &e->wf_stage, &e->wf_words, &e->dw_words, &e->dv_host};
-    for (PinBuf* b : pins) b->release();
-    if (e->ev_place) cudaEventDestroy(e->ev_place);
-    if (e->h_rounds) cudaFreeHost(e->h_rounds);
-    if (e->h_counts) cudaFreeHost(e->h_counts);
-    cudaEventDestroy(e->ev_hist);
-    cudaStreamDestroy(e->hist_stream);
-    cudaEventDestroy(e->ev_fork);
-    cudaEventDestroy(e->ev_join);
-    if (e->ev_pub) cudaEventDestroy(e->ev_pub);
-    if (e->ev_dma) cudaEventDestroy(e->ev_dma);
-    if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-    if (e->ev_done) cudaEventDestroy(e->ev_done);
-    if (e->ev_mid) cudaEventDestroy(e->ev_mid);
-    if (e->pub_stream) cudaStreamDestroy(e->pub_stream);
-    if (e->ds_stream) cudaStreamDestroy(e->ds_stream);
-    if (e->ev_ds_link) cudaEventDestroy(e->ev_ds_link);
-    if (e->lf_stream) cudaStreamDestroy(e->lf_stream);
-    if (e->ev_lf) cudaEventDestroy(e->ev_lf);
-    if (e->wf_stream) cudaStreamDestroy(e->wf_stream);
-    if (e->ev_wf) cudaEventDestroy(e->ev_wf);
-    if (e->ev_wf_t0) cudaEventDestroy(e->ev_wf_t0);
-    if (e->ev_wf_t1) cudaEventDestroy(e->ev_wf_t1);
-    if (e->ev_dd) cudaEventDestroy(e->ev_dd);
-    cudaStreamDestroy(e->side_stream);
-    cudaStreamDestroy(e->stream);
-  }
+  DeviceGuard guard(e->device);
+  // work in flight writes buffers that are about to be freed (a device synchronize would also wait for other engines)
+  const cudaStream_t streams[] = {e->stream,     e->side_stream, e->hist_stream, e->copy_stream,
+                                  e->pub_stream, e->ds_stream,   e->lf_stream,   e->wf_stream};
+  for (cudaStream_t s : streams)
+    if (s) cudaStreamSynchronize(s);
   delete e;
 }
 
@@ -730,11 +727,11 @@ static int sweep_host_locked(lwse_engine* e, const lwse_lws_tables* h, const std
   if (want_occ)
     LWSE_CUDA(e, cudaMemcpyAsync(h->node_occupancy, e->occupancy.p, (size_t)e->n_nodes * 4,
                                  cudaMemcpyDeviceToHost, s));
-  if (counted) LWSE_CUDA(e, cudaMemcpyAsync(e->h_counts, e->h_counts_dev.p, 4, cudaMemcpyDeviceToHost, s));
+  if (counted) LWSE_CUDA(e, cudaMemcpyAsync(e->h_counts.h, e->h_counts_dev.p, 4, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   if (counted) {
     e->ident_hint_pods = h->n_pods;
-    e->ident_hint_events = e->h_counts[0];
+    e->ident_hint_events = *static_cast<const uint32_t*>(e->h_counts.h);
   }
   return LWSE_OK;
 }
@@ -1186,10 +1183,11 @@ static int place_grouped_locked(lwse_engine* e, const lwse_place_req* d_reqs, ui
     e->place_pending = true;
   }
   if (rounds_out) {
-    LWSE_CUDA(e, cudaMemcpyAsync(e->h_rounds + 4, counters, 16, cudaMemcpyDeviceToHost, s));
+    uint32_t* const h_rounds = static_cast<uint32_t*>(e->h_rounds.h);
+    LWSE_CUDA(e, cudaMemcpyAsync(h_rounds + 4, counters, 16, cudaMemcpyDeviceToHost, s));
     LWSE_CUDA(e, cudaStreamSynchronize(s));
-    *rounds_out = e->h_rounds[4];
-    if (scans_out) *scans_out = e->h_rounds[7];
+    *rounds_out = h_rounds[4];
+    if (scans_out) *scans_out = h_rounds[7];
   }
   return LWSE_OK;
 }
@@ -1214,7 +1212,8 @@ static int place_locked(lwse_engine* e, const lwse_place_req* d_reqs, uint32_t n
   // the two scratch halves are laid out for one geometry; any change re-initialises them
   const uint32_t geometry[4] = {n_reqs, n_namespaces, e->n_nodes, e->n_domains};
   const bool fresh = before != e->place_scratch.p || memcmp(geometry, e->place_geometry, sizeof(geometry)) != 0;
-  if (fresh) e->h_rounds[2] = 0xFFFFFFFFu;  // no history for this geometry
+  uint32_t* const h_rounds = static_cast<uint32_t*>(e->h_rounds.h);
+  if (fresh) h_rounds[2] = 0xFFFFFFFFu;  // no history for this geometry
   memcpy(e->place_geometry, geometry, sizeof(geometry));
   // placement calls of one engine share the scratch (a call resets the half the next one uses):
   // whatever streams they run on, each orders behind the previous one
@@ -1230,13 +1229,13 @@ static int place_locked(lwse_engine* e, const lwse_place_req* d_reqs, uint32_t n
                                     (const uint32_t*)e->node_order.p, (const uint32_t*)e->node_pos.p, e->n_nodes,
                                     e->n_domains, d_reqs,
                                     n_reqs, d_occupancy, n_namespaces, d_out, e->place_scratch.p,
-                                    scratch, rounds_out ? e->h_rounds : nullptr, e->sm_count, s, &cuda_err,
+                                    scratch, rounds_out ? h_rounds : nullptr, e->sm_count, s, &cuda_err,
                                     e->place_calls++, fresh, n_parts, reqs_per_part, part_stride_bytes,
-                                    e->h_rounds + 2, &e->place_counters, &e->place_unpinned, after_push);
+                                    h_rounds + 2, &e->place_counters, &e->place_unpinned, after_push);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   e->place_rounds_ptr = e->place_counters + 3;
   e->place_scans_ptr = nullptr;
-  if (rounds_out) *rounds_out = e->h_rounds[0];
+  if (rounds_out) *rounds_out = h_rounds[0];
   if (eager) {
     LWSE_CUDA(e, cudaEventRecord(e->ev_place, s));
     e->place_pending = true;
@@ -1245,7 +1244,7 @@ static int place_locked(lwse_engine* e, const lwse_place_req* d_reqs, uint32_t n
   // the round's unpinned-request count, copied on a third stream so that nothing waits for it
   if (n_reqs > 1024u && e->place_unpinned && eager) {
     LWSE_CUDA(e, cudaStreamWaitEvent(e->hist_stream, e->ev_place, 0));
-    LWSE_CUDA(e, cudaMemcpyAsync(e->h_rounds + 2, e->place_unpinned, 4, cudaMemcpyDeviceToHost, e->hist_stream));
+    LWSE_CUDA(e, cudaMemcpyAsync(h_rounds + 2, e->place_unpinned, 4, cudaMemcpyDeviceToHost, e->hist_stream));
   }
   return LWSE_OK;
 }
@@ -1371,16 +1370,22 @@ LWSE_API int lwse_exchange_connect(lwse_engine* e, const void* handles) {
   std::lock_guard<std::mutex> lock(e->mu);
   if (!e->xch_world || e->xch_connected) return LWSE_ERR_NOT_READY;
   DeviceGuard guard(e->device);
-  for (uint32_t p = 0; p < e->xch_world; p++) {
+  cudaError_t err = cudaSuccess;
+  for (uint32_t p = 0; err == cudaSuccess && p < e->xch_world; p++) {
     if (p == e->xch_rank) {
-      e->xch_peer[p] = e->xch.p;
+      e->xch_peer.p[p] = e->xch.p;
       continue;
     }
     cudaIpcMemHandle_t h;
     memcpy(&h, static_cast<const uint8_t*>(handles) + (size_t)p * LWSE_IPC_HANDLE_BYTES, sizeof(h));
-    LWSE_CUDA(e, cudaIpcOpenMemHandle(&e->xch_peer[p], h, cudaIpcMemLazyEnablePeerAccess));
+    err = e->xch_peer.open(p, h);
   }
-  LWSE_CUDA(e, cudaMemcpy(e->xch_peers_dev.p, e->xch_peer, sizeof(void*) * e->xch_world, cudaMemcpyHostToDevice));
+  if (err == cudaSuccess)
+    err = cudaMemcpy(e->xch_peers_dev.p, e->xch_peer.p, sizeof(void*) * e->xch_world, cudaMemcpyHostToDevice);
+  if (err != cudaSuccess) {
+    e->xch_peer.close();  // a retry starts from no mappings
+    return fail_cuda(e, err);
+  }
   e->xch_connected = true;
   return LWSE_OK;
 }
@@ -1529,6 +1534,10 @@ extern "C" __attribute__((visibility("default"))) int lwse_debug_resident_read(l
   return LWSE_OK;
 }
 
+// Test aid (not part of lwse.h): the CUDA objects all engines of the process hold (allocations, streams, events,
+// graph executables, peer mappings).  Tests check that a closed engine gave back all of its own.
+extern "C" __attribute__((visibility("default"))) int64_t lwse_debug_cuda_objects(void) { return g_cuda_objects.load(); }
+
 // Tuning aid (not part of lwse.h): phase timestamps of the most recent placement kernel.
 extern "C" __attribute__((visibility("default"))) int lwse_debug_place_trace(lwse_engine* e, uint64_t* out16) {
   if (!e || !out16 || !e->place_scratch.p || e->place_calls == 0) return LWSE_ERR_NOT_READY;
@@ -1609,7 +1618,7 @@ LWSE_API int lwse_reconcile_host(lwse_engine* e, const lwse_lws_tables* h, const
                                  (lwse_place_out*)e->place_out.p, nullptr, ps, 1, n_reqs, 0, false, form);
     if (prc != LWSE_OK) return prc;
     if (promised && e->place_scans_ptr != nullptr) {  // (the namespace kernels ran: their counter block)
-      LWSE_CUDA(e, cudaMemcpyAsync(e->h_rounds + 8, e->place_rounds_ptr + 2, 4, cudaMemcpyDeviceToHost, ps));
+      LWSE_CUDA(e, cudaMemcpyAsync(static_cast<uint32_t*>(e->h_rounds.h) + 8, e->place_rounds_ptr + 2, 4, cudaMemcpyDeviceToHost, ps));
       check_order = true;
     }
     LWSE_CUDA(e, cudaMemcpyAsync(place_out, e->place_out.p, (size_t)n_reqs * sizeof(lwse_place_out), cudaMemcpyDeviceToHost, ps));
@@ -1619,7 +1628,7 @@ LWSE_API int lwse_reconcile_host(lwse_engine* e, const lwse_lws_tables* h, const
   if (n_reqs) {
     const cudaError_t pe = cudaStreamSynchronize(e->side_stream);
     if (rc_sweep == LWSE_OK && pe != cudaSuccess) return fail_cuda(e, pe);
-    if (rc_sweep == LWSE_OK && check_order && e->h_rounds[8] != 0u) return LWSE_ERR_BAD_TABLE;
+    if (rc_sweep == LWSE_OK && check_order && static_cast<const uint32_t*>(e->h_rounds.h)[8] != 0u) return LWSE_ERR_BAD_TABLE;
   }
   return rc_sweep;
 }
@@ -1943,7 +1952,7 @@ static int capture_tick_graph(lwse_engine* e, const TickPlan& p, lwse_engine::Ti
     cudaGraph_t graph = nullptr;
     const cudaError_t ee = cudaStreamEndCapture(s, &graph);
     if (ee != cudaSuccess || graph == nullptr) cap(ee != cudaSuccess ? ee : cudaErrorUnknown);
-    if (crc == LWSE_OK) cap(cudaGraphInstantiate(&tg.exec, graph, 0));
+    if (crc == LWSE_OK) cap(tg.exec.ensure(graph));
     if (graph) cudaGraphDestroy(graph);
   } else {
     crc = LWSE_ERR_CUDA;
@@ -1952,8 +1961,7 @@ static int capture_tick_graph(lwse_engine* e, const TickPlan& p, lwse_engine::Ti
   e->launches = launches_before;
   if (crc != LWSE_OK || !tg.exec) {
     (void)cudaGetLastError();
-    if (tg.exec) cudaGraphExecDestroy(tg.exec);
-    tg.exec = nullptr;
+    tg.exec.reset();
     tg.failed = true;
     e->node_index_stale = e->node_index_stale || p.node_rebuild;  // (the eager run builds it)
   } else {
@@ -2273,14 +2281,14 @@ static bool whatif_timing() {
 // branches joined), reading the resident tables and the baseline results in place: nothing writes them while
 // the call holds the mutex, and the call synchronizes its stream before it returns.
 static int drain_begin_locked(lwse_engine* e) {
-  if (!e->wf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->wf_stream, cudaStreamNonBlocking));
-  if (!e->ev_wf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_wf, cudaEventDisableTiming));
+  LWSE_CUDA(e, e->wf_stream.ensure(cudaStreamNonBlocking));
+  LWSE_CUDA(e, e->ev_wf.ensure(cudaEventDisableTiming));
   LWSE_CUDA(e, cudaEventRecord(e->ev_wf, e->stream));
   LWSE_CUDA(e, cudaStreamWaitEvent(e->wf_stream, e->ev_wf, 0));
   e->wf_timed = false;
   if (whatif_timing()) {
-    if (!e->ev_wf_t0) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t0));
-    if (!e->ev_wf_t1) LWSE_CUDA(e, cudaEventCreate(&e->ev_wf_t1));
+    LWSE_CUDA(e, e->ev_wf_t0.ensure(cudaEventDefault));
+    LWSE_CUDA(e, e->ev_wf_t1.ensure(cudaEventDefault));
     LWSE_CUDA(e, cudaEventRecord(e->ev_wf_t0, e->wf_stream));
   }
   return LWSE_OK;
@@ -3321,7 +3329,7 @@ LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_wa
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   if (m) {
     cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
+    GraphExec exec;
     LWSE_CUDA(e, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
     launched = lwse::launch_drain_place_waves(&d, 1, e->sm_count, s, &cuda_err);
     const cudaError_t ce = cudaStreamEndCapture(s, &graph);
@@ -3329,10 +3337,9 @@ LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_wa
       if (graph) cudaGraphDestroy(graph);
       return fail_cuda(e, launched < 0 ? (cudaError_t)cuda_err : ce);
     }
-    cudaError_t ge = cudaGraphInstantiate(&exec, graph, 0);
+    cudaError_t ge = exec.ensure(graph);
     cudaGraphDestroy(graph);
     for (uint32_t i = 0; ge == cudaSuccess && i < m; i++) ge = cudaGraphLaunch(exec, s);
-    if (exec) cudaGraphExecDestroy(exec);
     if (ge != cudaSuccess) return fail_cuda(e, ge);
     e->launches += (uint64_t)launched * m;
   }
@@ -3356,8 +3363,8 @@ static bool ds_drain_ready(const lwse_engine* e) { return drain_budget_ready(e) 
 // drain_begin_locked, with the what-if stream also behind the DS stream (the last DS tick or load: nothing is
 // in flight there while the mutex is held, but the call does not depend on that).
 static int ds_drain_begin_locked(lwse_engine* e) {
-  if (!e->wf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->wf_stream, cudaStreamNonBlocking));
-  if (!e->ev_dd) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_dd, cudaEventDisableTiming));
+  LWSE_CUDA(e, e->wf_stream.ensure(cudaStreamNonBlocking));
+  LWSE_CUDA(e, e->ev_dd.ensure(cudaEventDisableTiming));
   LWSE_CUDA(e, cudaEventRecord(e->ev_dd, e->ds_stream));
   LWSE_CUDA(e, cudaStreamWaitEvent(e->wf_stream, e->ev_dd, 0));
   return drain_begin_locked(e);
@@ -3801,7 +3808,7 @@ LWSE_API int lwse_ds_resident_load(lwse_engine* e, const lwse_ds_tables* h) {
   if ((h->n_ds && !h->ds) || (h->n_roles && !h->roles) || (h->n_revroles && !h->revroles)) return LWSE_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(e->mu);
   DeviceGuard guard(e->device);
-  if (!e->ds_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->ds_stream, cudaStreamNonBlocking));
+  LWSE_CUDA(e, e->ds_stream.ensure(cudaStreamNonBlocking));
   cudaStream_t s = e->ds_stream;
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   e->rd_loaded = false;  // (until every copy below succeeded)
@@ -3959,7 +3966,7 @@ LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, u
       // waits for everything enqueued there now (the most recently submitted LWS tick, in flight or
       // not) and nothing else — no drain, no dropped results.  The engine mutex is held until this call
       // has its results, so no later LWS tick can overwrite those rows while the DS kernel reads them.
-      if (!e->ev_ds_link) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_ds_link, cudaEventDisableTiming));
+      LWSE_CUDA(e, e->ev_ds_link.ensure(cudaEventDisableTiming));
       LWSE_CUDA(e, cudaEventRecord(e->ev_ds_link, e->stream));
       LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_ds_link, 0));
     }
@@ -4132,7 +4139,7 @@ LWSE_API int lwse_resident_ds_rollout_whatif(lwse_engine* e, lwse_ds_rollout_wha
     return LWSE_OK;
   }
   DeviceGuard guard(e->device);
-  if (!e->wf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->wf_stream, cudaStreamNonBlocking));
+  LWSE_CUDA(e, e->wf_stream.ensure(cudaStreamNonBlocking));
   cudaStream_t s = e->wf_stream;
   const size_t nr = (size_t)n * LWSE_DS_MAX_ROLES;
   LWSE_CUDA(e, e->dw_props.reserve((size_t)n * sizeof(lwse_ds_proposal) + 16));
@@ -4265,7 +4272,7 @@ static int lws_forecast_locked(lwse_engine* e, lwse::LwsForecastHost& h, lwse_lw
 }
 
 static int lws_forecast_stream(lwse_engine* e) {
-  if (!e->lf_stream) LWSE_CUDA(e, cudaStreamCreateWithFlags(&e->lf_stream, cudaStreamNonBlocking));
+  LWSE_CUDA(e, e->lf_stream.ensure(cudaStreamNonBlocking));
   return LWSE_OK;
 }
 
@@ -4317,7 +4324,7 @@ LWSE_API int lwse_resident_forecast(lwse_engine* e, lwse_lws_forecast_out* out) 
   DeviceGuard guard(e->device);
   int rc = lws_forecast_stream(e);
   if (rc != LWSE_OK) return rc;
-  if (!e->ev_lf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_lf, cudaEventDisableTiming));
+  LWSE_CUDA(e, e->ev_lf.ensure(cudaEventDisableTiming));
   lwse::LwsForecastHost h{};
   if (const int src = forecast_snapshot(e, e->stream, &h); src != LWSE_OK) return src;
   LWSE_CUDA(e, cudaEventRecord(e->ev_lf, e->stream));
@@ -4427,7 +4434,7 @@ LWSE_API int lwse_resident_rollout_whatif(lwse_engine* e, lwse_rollout_whatif* q
   }
   DeviceGuard guard(e->device);
   if (const int rc = lws_forecast_stream(e); rc != LWSE_OK) return rc;
-  if (!e->ev_lf) LWSE_CUDA(e, cudaEventCreateWithFlags(&e->ev_lf, cudaEventDisableTiming));
+  LWSE_CUDA(e, e->ev_lf.ensure(cudaEventDisableTiming));
   cudaStream_t s = e->lf_stream;
   if (const int rc = reserve_rollout_whatif(e, n); rc != LWSE_OK) return rc;
   if (const int rc = upload_rollout_proposals(e, q->rows, q->recs, n, s); rc != LWSE_OK) return rc;
