@@ -219,6 +219,14 @@ func (e *Engine) RolloutPlace(q *C.lwse_rollout_place_query) error {
 	return e.check(C.lwse_resident_rollout_place(e.h, q))
 }
 
+// RolloutPlaceWaves packs distinct resident LeaderWorkerSets, or proposed edits of them (q.recs), first-fit in the
+// order given into at most q.max_waves waves whose rollouts, pushed together, give every group they add an
+// exclusive domain (LWSE_RPW_STRANDED) and, with LWSE_RPW_BUMPED, take none from a placed group.  A fleet-wide
+// template bump pushes wave 0, waits for its rollouts to finish and calls again with the objects that remain.
+func (e *Engine) RolloutPlaceWaves(q *C.lwse_rollout_place_waves_query) error {
+	return e.check(C.lwse_resident_rollout_place_waves(e.h, q))
+}
+
 // DrainWaves packs distinct node rows (scope LWSE_DRAIN_NODES) or domain ids (LWSE_DRAIN_DOMAINS), in the order
 // given, first-fit into at most q.max_waves waves whose drain takes no LeaderWorkerSet below its floor.  A
 // maintenance controller drains wave 0, waits for recovery and calls again with the keys that remain.

@@ -1314,6 +1314,96 @@ typedef struct lwse_rollout_place_query {
 } lwse_rollout_place_query;
 LWSE_API int lwse_resident_rollout_place(lwse_engine* e, lwse_rollout_place_query* q);
 
+/* ---- rollout placement waves --------------------------------------------------------------------
+ * "Which of these rollouts can I push together so that the groups they add all find an exclusive domain?"  The
+ * first-fit plan of the drain waves over the entries of lwse_resident_rollout_place, with the rollouts of one wave
+ * solved together (DESIGN.md §3.5, "Rollout placement waves").
+ *
+ * Definition.  rows, ns and recs are the entries of lwse_resident_rollout_place, with the same contract, except
+ * that the rows must be distinct.  E_i is that call's extra rows of entry i.  For a set S of entries the set form is
+ * lwse_resident_place_whatif with no segments, the resident n_namespaces and extra = E_{i1} || E_{i2} || ... over
+ * S in query order, diffed against the baseline.  A resident row is S's own when its `group` lies in the group
+ * range of an entry of S whose ns is the row's namespace.  S TRIGGERS
+ *   LWSE_RPW_STRANDED  when some extra row is not PLACED after;
+ *   LWSE_RPW_BUMPED    when some resident row PLACED before is not PLACED after (own_lost or bumped).
+ * `constraints` (nonzero, known bits only) names the verdicts the plan keeps.  Only entries that
+ * lwse_resident_rollout_place marks LWSE_RPL_SOLVED take part.  Keys are taken in query order and key k_i gets the
+ * first of:
+ *   3. LWSE_ROLLW_NOT_SOLVED       the entry is not SOLVED (wave LWSE_NONE);
+ *   1. LWSE_ROLLW_TRIGGERS_ALONE   {k_i} triggers a verdict in constraints (wave LWSE_NONE);
+ *   0. LWSE_ROLLW_PLANNED          wave w: the lowest open wave such that W_w ∪ {k_i} triggers none of them; with
+ *                                  no such wave and fewer than max_waves open, a new wave;
+ *   2. LWSE_ROLLW_NO_WAVE          neither (wave LWSE_NONE).
+ * Every wave is judged against the same baseline, the most recently submitted tick: the plan assumes that a
+ * wave's rollouts finish, and their surge groups go away, before the next wave starts.  The rollouts of one wave
+ * are modelled at their peaks at the same time, so the plan is conservative as lwse_resident_rollout_place is.
+ * The placement verdicts are not monotone in the set, so a key that triggers alone is TRIGGERS_ALONE even when
+ * some wave would take it; the answer is the literal first-fit.  The plan decomposes exactly by namespace: keys of
+ * different namespaces never wait for each other (DESIGN.md §3.5).
+ *
+ * Readiness, isolation and errors are lwse_resident_rollout_place's, and: LWSE_ERR_INVALID_ARG for a duplicate
+ * row, max_waves of 0 or above LWSE_DRAIN_WAVES_MAX, a zero or unknown `constraints` bit, a nonzero reserved field,
+ * a NULL keys (n > 0) or waves; LWSE_ERR_UNSUPPORTED also when rn_reqs + the sum of |E_i| over the SOLVED entries
+ * reaches 2^24 (checked before the plan).  A refused call writes no output.  n = 0 is valid and opens no wave. */
+#define LWSE_RPW_STRANDED (1u << 0)
+#define LWSE_RPW_BUMPED (1u << 1)
+#define LWSE_RPW_ALL (LWSE_RPW_STRANDED | LWSE_RPW_BUMPED)
+
+#define LWSE_ROLLW_PLANNED 0u        /* = LWSE_DRAINW_PLANNED */
+#define LWSE_ROLLW_TRIGGERS_ALONE 1u /* = LWSE_DRAINW_BREACHES_ALONE */
+#define LWSE_ROLLW_NO_WAVE 2u        /* = LWSE_DRAINW_NO_WAVE */
+#define LWSE_ROLLW_NOT_SOLVED 3u
+
+/* One key of the plan, in query order (16 B). */
+typedef struct lwse_rollout_wave_key {
+  uint32_t wave;              /* its wave, or LWSE_NONE                                                  */
+  uint32_t status;            /* LWSE_ROLLW_*                                                            */
+  uint32_t alone;             /* the LWSE_RPW_* bits {k_i} triggers, whatever constraints holds          */
+  uint32_t reserved;
+} lwse_rollout_wave_key;
+
+/* One opened wave (64 B): the totals of the set form over the wave's final key set.  The counts of verdicts in
+ * constraints are 0; the others report what the wave does to a verdict the caller did not enforce. */
+typedef struct lwse_rollout_wave {
+  uint32_t n_keys;
+  uint32_t surge;             /* extra rows: placed + stranded                                           */
+  uint32_t placed;
+  uint32_t stranded;
+  uint32_t own_lost;          /* the wave's own resident rows PLACED before and not after                */
+  uint32_t bumped;            /* other resident rows PLACED before and not after                         */
+  uint32_t n_changed;         /* the lwse_place_whatif counters of the set form                          */
+  uint32_t n_lost;
+  uint32_t n_moved;
+  uint32_t n_gained;
+  uint32_t n_placed;
+  uint32_t n_unschedulable;
+  uint32_t n_conflict;
+  uint32_t namespaces;        /* distinct namespaces among the wave's entries                            */
+  uint32_t reserved[2];
+} lwse_rollout_wave;
+
+typedef struct lwse_rollout_place_waves_query {
+  /* in */
+  const uint32_t* rows;             /* [n] distinct resident LWS rows                                      */
+  const uint32_t* ns;               /* [n] namespace ids                                                   */
+  const lwse_lws_rec* recs;         /* [n] proposals, 16-byte aligned, or NULL: the resident rows          */
+  uint32_t n;
+  uint32_t max_waves;               /* 1 .. LWSE_DRAIN_WAVES_MAX                                           */
+  uint32_t constraints;             /* LWSE_RPW_* (nonzero)                                                */
+  uint32_t reserved;                /* 0                                                                   */
+  lwse_rollout_wave_key* keys;      /* [n] out                                                             */
+  lwse_rollout_wave* waves;         /* [max_waves] out: rows 0 .. n_waves                                  */
+  lwse_rollout_place* alone_rows;   /* [n] out, or NULL: lwse_resident_rollout_place's rows for the query  */
+  /* out */
+  uint32_t n_waves;
+  uint32_t n_planned;
+  uint32_t n_triggers_alone;
+  uint32_t n_no_wave;
+  uint32_t n_not_solved;
+  uint32_t reserved1;
+} lwse_rollout_place_waves_query;
+LWSE_API int lwse_resident_rollout_place_waves(lwse_engine* e, lwse_rollout_place_waves_query* q);
+
 /* ------------------------------------------------------------------------- */
 /* Peer exchange: the multi-GPU placement step without a collective library  */
 /* ------------------------------------------------------------------------- */

@@ -337,6 +337,11 @@ struct lwse_engine {
   // {first extra row, |E_i|, group range}, the |E_i| index (count | first | cursor), the items, the counters, the
   // extra rows, the all-namespaces mask, the round scratch, the solve's per-CTA slices
   DevBuf rp_in, rp_rows, rp_ent, rp_idx, rp_items, rp_words, rp_extra, rp_touched, rp_round, rp_slices;
+  // rollout placement waves (lwse_resident_rollout_place_waves): the round state and wave totals, the per-namespace
+  // counts (K_ns | first | cursor | T_ns | p_ns), the per-key ranks, lists and active namespaces, the per-slot
+  // state, the column lists, the round's slices, the answer; the answer going back (host)
+  DevBuf rq_state, rq_ns, rq_keys, rq_slots, rq_col, rq_slices, rq_out;
+  PinBuf rq_host;
   // drain waves (lwse_resident_drain_waves): the drain budget's key rows, the counters, the ids, the key positions, the
   // key buckets (count | first | cursor), the restart pairs, the pair records, the touched-row index (count | first |
   // cursor), the dense rows, the lost counters, the group and row wave masks, the stamps, the answer; the ids going
@@ -4447,32 +4452,14 @@ LWSE_API int lwse_resident_rollout_whatif(lwse_engine* e, lwse_rollout_whatif* q
 }
 
 // ---- rollout placement ----
-// On wf_stream behind one event on the engine's stream: the forecast (the resident forecast's snapshot, or the
-// rollout what-if's chain over the proposals), then the count kernel, read back at one synchronisation (max |E_i|
-// sizes the slices and decides the 24-bit refusal), then the scan, the extra rows, every namespace's request index,
-// the solve and the finish, read back at a second.  The rows are copied out last, so that a refused call writes
-// nothing.
-LWSE_API int lwse_resident_rollout_place(lwse_engine* e, lwse_rollout_place_query* q) {
-  if (!e || !q) return LWSE_ERR_INVALID_ARG;
-  std::lock_guard<std::mutex> lock(e->mu);
-  if (!e->r_loaded || !e->r_groups_swept) return LWSE_ERR_NOT_READY;  // (the forecast's rule)
-  if (!e->r_place_loaded || !e->r_place_current || e->n_nodes == 0 || e->n_domains == 0) return LWSE_ERR_NOT_READY;
-  const uint32_t n = q->n;
-  if (n && (!q->rows || !q->ns || !q->out)) return LWSE_ERR_INVALID_ARG;
-  if (!aligned16(q->recs) || (q->extra_capacity && !q->extra)) return LWSE_ERR_INVALID_ARG;
-  for (uint32_t i = 0; i < n; i++)
-    if (q->rows[i] >= e->rn_lws || q->ns[i] >= e->rn_namespaces) return LWSE_ERR_INVALID_ARG;
-  if (e->xch_world > 0 || e->rn_reqs >= (1u << 24) || !lwse::place_ns_supported(e->n_nodes, e->n_domains))
-    return LWSE_ERR_UNSUPPORTED;
-  if (n == 0) {
-    q->n_solved = q->n_strands = 0;
-    q->n_surge = q->n_stranded = 0;
-    return LWSE_OK;
-  }
+// The chain's first part, on wf_stream behind one event on the engine's stream: the scratch sized by n and the
+// resident tables, the forecast (the resident forecast's snapshot, or the rollout what-if's chain over the
+// proposals), then the count kernel, read back at one synchronisation into words[0..3] (the items, max |E_i| and
+// sum |E_i|, which size the slices and decide the 24-bit refusal).
+static int rollout_place_count(lwse_engine* e, const uint32_t* rows, const uint32_t* ns, const lwse_lws_rec* recs, uint32_t n,
+                               lwse::RolloutPlaceLaunch* p) {
   const uint32_t nn = e->n_nodes, nd = e->n_domains, nr = e->rn_reqs, n_ns = e->rn_namespaces;
-  const bool proposals = q->recs != nullptr;
-  DeviceGuard guard(e->device);
-  // scratch sized by n and the resident tables, before the snapshot
+  const bool proposals = recs != nullptr;
   LWSE_CUDA(e, e->wf_words.reserve(128));
   LWSE_CUDA(e, e->rp_in.reserve((size_t)n * 8 + 16));
   LWSE_CUDA(e, e->rp_rows.reserve((size_t)n * sizeof(lwse_rollout_place) + 16));
@@ -4481,8 +4468,7 @@ LWSE_API int lwse_resident_rollout_place(lwse_engine* e, lwse_rollout_place_quer
   LWSE_CUDA(e, e->rp_items.reserve((size_t)n * 8 + 16));
   LWSE_CUDA(e, e->rp_words.reserve(128));
   LWSE_CUDA(e, e->rp_touched.reserve((size_t)n_ns + 16));
-  const size_t round_bytes = lwse::place_ns_scratch_bytes(nn, nd, nr, n_ns);
-  LWSE_CUDA(e, e->rp_round.reserve(round_bytes));
+  LWSE_CUDA(e, e->rp_round.reserve(lwse::place_ns_scratch_bytes(nn, nd, nr, n_ns)));
   if (e->node_index_stale)
     if (const int rc = reserve_node_index(e); rc != LWSE_OK) return rc;
   if (proposals)
@@ -4492,88 +4478,136 @@ LWSE_API int lwse_resident_rollout_place(lwse_engine* e, lwse_rollout_place_quer
   uint32_t* d_words = (uint32_t*)e->rp_words.p;
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
   uint32_t* d_rows_in = (uint32_t*)e->rp_in.p;
-  LWSE_CUDA(e, cudaMemcpyAsync(d_rows_in, q->rows, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-  LWSE_CUDA(e, cudaMemcpyAsync(d_rows_in + n, q->ns, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(d_rows_in, rows, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(d_rows_in + n, ns, (size_t)n * 4, cudaMemcpyHostToDevice, s));
   LWSE_CUDA(e, cudaMemsetAsync(d_words, 0, 128, s));
   LWSE_CUDA(e, cudaMemsetAsync(e->rp_idx.p, 0, (size_t)n * 4, s));  // (the |E_i| counts start at zero)
   // the forecast rows F_i, on the device only (lf_fc): per entry (proposals) or per resident row
   lwse_lws_forecast_out fc{};
   if (proposals) {
-    if (const int rc = upload_rollout_proposals(e, q->rows, q->recs, n, s); rc != LWSE_OK) return rc;
+    if (const int rc = upload_rollout_proposals(e, rows, recs, n, s); rc != LWSE_OK) return rc;
     if (const int rc = enqueue_rollout_whatif(e, n, s, &fc); rc != LWSE_OK) return rc;
   } else {
     lwse::LwsForecastHost h{};
     if (const int rc = forecast_snapshot(e, s, &h); rc != LWSE_OK) return rc;
     if (const int rc = lws_forecast_locked(e, h, &fc, s); rc != LWSE_OK) return rc;
   }
-  lwse::RolloutPlaceLaunch p{};
-  p.lws = (const lwse_lws_rec*)e->r_lws.p;
-  p.groups = (const lwse_group_rec*)e->r_groups.p;
-  p.n_groups = e->rn_groups;
-  p.rows = d_rows_in;
-  p.ns = d_rows_in + n;
-  p.recs = proposals ? (const lwse_lws_rec*)e->rw_lws.p : nullptr;
-  p.fc = (const lwse_lws_forecast*)e->lf_fc.p;
-  p.fc_by_row = !proposals;
-  p.n = n;
-  p.rows_out = (uint32_t*)e->rp_rows.p;
-  p.ent = (uint4*)e->rp_ent.p;
-  p.e_count = (uint32_t*)e->rp_idx.p;
-  p.e_first = p.e_count + n;
-  p.e_cursor = p.e_first + n + 1;
-  p.items = (uint2*)e->rp_items.p;
-  p.counts = d_words;
+  *p = lwse::RolloutPlaceLaunch{};
+  p->lws = (const lwse_lws_rec*)e->r_lws.p;
+  p->groups = (const lwse_group_rec*)e->r_groups.p;
+  p->n_groups = e->rn_groups;
+  p->rows = d_rows_in;
+  p->ns = d_rows_in + n;
+  p->recs = proposals ? (const lwse_lws_rec*)e->rw_lws.p : nullptr;
+  p->fc = (const lwse_lws_forecast*)e->lf_fc.p;
+  p->fc_by_row = !proposals;
+  p->n = n;
+  p->rows_out = (uint32_t*)e->rp_rows.p;
+  p->ent = (uint4*)e->rp_ent.p;
+  p->e_count = (uint32_t*)e->rp_idx.p;
+  p->e_first = p->e_count + n;
+  p->e_cursor = p->e_first + n + 1;
+  p->items = (uint2*)e->rp_items.p;
+  p->counts = d_words;
   int cuda_err = 0;
-  int launched = lwse::launch_rollout_place(&p, 0, e->sm_count, s, &cuda_err);
+  const int launched = lwse::launch_rollout_place(p, 0, e->sm_count, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 16, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
-  const uint32_t n_items = words[0], max_extra = words[1];
-  const uint64_t n_extra = (uint64_t)words[2] | (uint64_t)words[3] << 32;
-  if ((uint64_t)nr + max_extra >= (1ull << 24)) return LWSE_ERR_UNSUPPORTED;  // (row keys are 24-bit)
-  if (n_extra >= (1ull << 32)) return LWSE_ERR_OOM;                          // (the scan's offsets are 32-bit)
+  return LWSE_OK;
+}
+
+// The chain's second part, enqueued on wf_stream after the refusals: the slices, the extra rows, the baseline's
+// totals, every namespace's request index, the scan, the fill, the solve and the finish.
+static int rollout_place_solve(lwse_engine* e, uint32_t n_items, uint32_t max_extra, uint64_t n_extra,
+                               lwse::RolloutPlaceLaunch* p) {
+  const uint32_t nn = e->n_nodes, nd = e->n_domains, nr = e->rn_reqs, n_ns = e->rn_namespaces;
+  cudaStream_t s = e->wf_stream;
   // the solve's slices: the largest namespace plus the largest E_i per resident CTA
   const uint64_t slice_rows = (uint64_t)largest_namespace(e) + max_extra;
   uint64_t grid = n_items ? std::min<uint64_t>((uint64_t)e->sm_count * 2u, n_items) : 0;
   while (grid > 1 && grid * slice_rows * (sizeof(lwse_place_out) + 4) > (1ull << 30)) grid >>= 1;
   if (grid && grid * slice_rows * (sizeof(lwse_place_out) + 4) > (1ull << 31)) return LWSE_ERR_OOM;
   const size_t slice_out = align256((size_t)grid * slice_rows * sizeof(lwse_place_out));
+  const size_t round_bytes = lwse::place_ns_scratch_bytes(nn, nd, nr, n_ns);
   LWSE_CUDA(e, e->rp_extra.reserve((size_t)n_extra * sizeof(lwse_place_req) + 16));
   LWSE_CUDA(e, e->rp_slices.reserve(slice_out + (size_t)grid * slice_rows * 4 + 16));
-  p.extra = (lwse_place_req*)e->rp_extra.p;
-  p.nodes = (const lwse_node_rec*)e->nodes.p;
-  p.occupancy = (const uint32_t*)e->r_occ.p;
-  p.dom_first = (const uint32_t*)e->dom_first.p;
-  p.node_order = (const uint32_t*)e->node_order.p;
-  p.reqs = (const lwse_place_req*)e->r_preq.p;
-  p.base = (const lwse_place_out*)e->r_pout.p;
-  p.n_nodes = nn;
-  p.n_domains = nd;
-  p.n_reqs = nr;
-  p.n_namespaces = n_ns;
-  p.round = e->rp_round.p;
-  p.round_bytes = round_bytes;
-  p.s_out = (lwse_place_out*)e->rp_slices.p;
-  p.s_unpinned = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(e->rp_slices.p) + slice_out);
-  p.slice_rows = (uint32_t)slice_rows;
-  p.grid = (uint32_t)grid;
+  p->extra = (lwse_place_req*)e->rp_extra.p;
+  p->nodes = (const lwse_node_rec*)e->nodes.p;
+  p->occupancy = (const uint32_t*)e->r_occ.p;
+  p->dom_first = (const uint32_t*)e->dom_first.p;
+  p->node_order = (const uint32_t*)e->node_order.p;
+  p->reqs = (const lwse_place_req*)e->r_preq.p;
+  p->base = (const lwse_place_out*)e->r_pout.p;
+  p->n_nodes = nn;
+  p->n_domains = nd;
+  p->n_reqs = nr;
+  p->n_namespaces = n_ns;
+  p->round = e->rp_round.p;
+  p->round_bytes = round_bytes;
+  p->s_out = (lwse_place_out*)e->rp_slices.p;
+  p->s_unpinned = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(e->rp_slices.p) + slice_out);
+  p->slice_rows = (uint32_t)slice_rows;
+  p->grid = (uint32_t)grid;
   // the baseline's totals (a diff of the baseline rows against themselves counts them), every namespace's index
-  launched = lwse::launch_place_whatif_diff(p.base, p.base, 0, nr, nullptr, nullptr, nullptr, 0, d_words + 16, e->sm_count, s,
-                                            &cuda_err);
+  int cuda_err = 0;
+  int launched = lwse::launch_place_whatif_diff(p->base, p->base, 0, nr, nullptr, nullptr, nullptr, 0, p->counts + 16,
+                                                e->sm_count, s, &cuda_err);
   if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   if (grid) {
     LWSE_CUDA(e, cudaMemsetAsync(e->rp_touched.p, 1, n_ns, s));
     LWSE_CUDA(e, cudaMemsetAsync(e->rp_round.p, 0, round_bytes, s));  // (the index counts start at zero)
     if (e->node_index_stale)
-      if (const int rc = own_node_index(e, p.nodes, s, &p.dom_first, &p.node_order, nullptr); rc != LWSE_OK) return rc;
-    launched = lwse::launch_place_whatif_index(p.reqs, nr, n_ns, (const uint8_t*)e->rp_touched.p, nn, nd, e->rp_round.p,
+      if (const int rc = own_node_index(e, p->nodes, s, &p->dom_first, &p->node_order, nullptr); rc != LWSE_OK) return rc;
+    launched = lwse::launch_place_whatif_index(p->reqs, nr, n_ns, (const uint8_t*)e->rp_touched.p, nn, nd, e->rp_round.p,
                                                e->sm_count, s, &cuda_err);
     if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
   }
-  launched = lwse::launch_rollout_place(&p, 1, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  launched = lwse::launch_rollout_place(p, 1, e->sm_count, s, &cuda_err);
+  return count_launch(e, launched, cuda_err);
+}
+
+// The checks both rollout placement calls make before anything is enqueued.
+static int rollout_place_check(const lwse_engine* e, const uint32_t* rows, const uint32_t* ns, const lwse_lws_rec* recs,
+                               uint32_t n) {
+  if (!e->r_loaded || !e->r_groups_swept) return LWSE_ERR_NOT_READY;  // (the forecast's rule)
+  if (!e->r_place_loaded || !e->r_place_current || e->n_nodes == 0 || e->n_domains == 0) return LWSE_ERR_NOT_READY;
+  if (n && (!rows || !ns)) return LWSE_ERR_INVALID_ARG;
+  if (!aligned16(recs)) return LWSE_ERR_INVALID_ARG;
+  for (uint32_t i = 0; i < n; i++)
+    if (rows[i] >= e->rn_lws || ns[i] >= e->rn_namespaces) return LWSE_ERR_INVALID_ARG;
+  return LWSE_OK;
+}
+
+// The forecast and the count kernel, read back at one synchronisation (max |E_i| sizes the slices and decides the
+// 24-bit refusal), then the scan, the extra rows, every namespace's request index, the solve and the finish, read
+// back at a second.  The rows are copied out last, so that a refused call writes nothing.
+LWSE_API int lwse_resident_rollout_place(lwse_engine* e, lwse_rollout_place_query* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  const uint32_t n = q->n;
+  if (const int rc = rollout_place_check(e, q->rows, q->ns, q->recs, n); rc != LWSE_OK) return rc;
+  if ((n && !q->out) || (q->extra_capacity && !q->extra)) return LWSE_ERR_INVALID_ARG;
+  if (e->xch_world > 0 || e->rn_reqs >= (1u << 24) || !lwse::place_ns_supported(e->n_nodes, e->n_domains))
+    return LWSE_ERR_UNSUPPORTED;
+  if (n == 0) {
+    q->n_solved = q->n_strands = 0;
+    q->n_surge = q->n_stranded = 0;
+    return LWSE_OK;
+  }
+  const uint32_t nr = e->rn_reqs;
+  DeviceGuard guard(e->device);
+  lwse::RolloutPlaceLaunch p{};
+  if (const int rc = rollout_place_count(e, q->rows, q->ns, q->recs, n, &p); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  const uint32_t n_items = words[0], max_extra = words[1];
+  const uint64_t n_extra = (uint64_t)words[2] | (uint64_t)words[3] << 32;
+  if ((uint64_t)nr + max_extra >= (1ull << 24)) return LWSE_ERR_UNSUPPORTED;  // (row keys are 24-bit)
+  if (n_extra >= (1ull << 32)) return LWSE_ERR_OOM;                          // (the scan's offsets are 32-bit)
+  if (const int rc = rollout_place_solve(e, n_items, max_extra, n_extra, &p); rc != LWSE_OK) return rc;
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
-  LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 64, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 64, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(q->out, p.rows_out, (size_t)n * sizeof(lwse_rollout_place), cudaMemcpyDeviceToHost, s));
   if (const uint64_t listed = std::min<uint64_t>(n_extra, q->extra_capacity))
     LWSE_CUDA(e, cudaMemcpyAsync(q->extra, p.extra, (size_t)listed * sizeof(lwse_place_req), cudaMemcpyDeviceToHost, s));
@@ -4582,6 +4616,131 @@ LWSE_API int lwse_resident_rollout_place(lwse_engine* e, lwse_rollout_place_quer
   q->n_strands = words[5];
   q->n_surge = (uint64_t)words[6] | (uint64_t)words[7] << 32;
   q->n_stranded = (uint64_t)words[8] | (uint64_t)words[9] << 32;
+  return LWSE_OK;
+}
+
+// ---- rollout placement waves ----
+// Setup: the rollout placement's chain (its rows are the alone rows), then the key rows, the ranks and the
+// per-namespace key lists, read back at a third synchronisation (R, the largest T_ns and the active namespaces
+// size the lists and the slices).  Then one captured round, replayed R times with the round in device memory (no
+// host synchronisation per round), the finish, and one copy back.
+LWSE_API int lwse_resident_rollout_place_waves(lwse_engine* e, lwse_rollout_place_waves_query* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  const uint32_t n = q->n;
+  if (const int rc = rollout_place_check(e, q->rows, q->ns, q->recs, n); rc != LWSE_OK) return rc;
+  if ((n && !q->keys) || !q->waves || q->reserved) return LWSE_ERR_INVALID_ARG;
+  if (q->max_waves == 0 || q->max_waves > LWSE_DRAIN_WAVES_MAX) return LWSE_ERR_INVALID_ARG;
+  if (q->constraints == 0 || (q->constraints & ~LWSE_RPW_ALL)) return LWSE_ERR_INVALID_ARG;
+  {
+    std::vector<uint32_t> sorted(q->rows, q->rows + n);
+    std::sort(sorted.begin(), sorted.end());
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) return LWSE_ERR_INVALID_ARG;
+  }
+  if (e->xch_world > 0 || e->rn_reqs >= (1u << 24) || !lwse::place_ns_supported(e->n_nodes, e->n_domains))
+    return LWSE_ERR_UNSUPPORTED;
+  if (n == 0) {
+    q->n_waves = q->n_planned = q->n_triggers_alone = q->n_no_wave = q->n_not_solved = 0;
+    return LWSE_OK;
+  }
+  const uint32_t nr = e->rn_reqs, n_ns = e->rn_namespaces, mw = q->max_waves;
+  DeviceGuard guard(e->device);
+  lwse::RolloutPlaceWavesLaunch w{};
+  lwse::RolloutPlaceLaunch& p = w.p;
+  if (const int rc = rollout_place_count(e, q->rows, q->ns, q->recs, n, &p); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  const uint32_t n_items = words[0], max_extra = words[1];
+  const uint64_t n_extra = (uint64_t)words[2] | (uint64_t)words[3] << 32;
+  if ((uint64_t)nr + n_extra >= (1ull << 24)) return LWSE_ERR_UNSUPPORTED;  // (a wave's rows are numbered after nr)
+  if (const int rc = rollout_place_solve(e, n_items, max_extra, n_extra, &p); rc != LWSE_OK) return rc;
+  // the ranks and the per-namespace key lists
+  const size_t out_bytes = 32 + (size_t)n * sizeof(lwse_rollout_wave_key) + LWSE_DRAIN_WAVES_MAX * sizeof(lwse_rollout_wave);
+  LWSE_CUDA(e, e->rq_state.reserve(64 + LWSE_DRAIN_WAVES_MAX * 64 + 16));
+  LWSE_CUDA(e, e->rq_ns.reserve(((size_t)n_ns * 5 + 1) * 4 + 16));
+  LWSE_CUDA(e, e->rq_keys.reserve((size_t)n * 4 * 3 + 16));
+  LWSE_CUDA(e, e->rq_slots.reserve((size_t)n * (16 + 64 + 8 + 4 + 4 + 4 * 11) + 16));
+  LWSE_CUDA(e, e->rq_out.reserve(out_bytes + 16));
+  LWSE_CUDA(e, e->rq_host.reserve(out_bytes + 16));
+  uint32_t* st = (uint32_t*)e->rq_state.p;
+  LWSE_CUDA(e, cudaMemsetAsync(st, 0, 64 + LWSE_DRAIN_WAVES_MAX * 64, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->rq_ns.p, 0, ((size_t)n_ns * 5 + 1) * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(e->rq_out.p, 0, out_bytes, s));
+  w.constraints = q->constraints;
+  w.max_waves = mw;
+  w.st = st;
+  w.wtot = st + 16;
+  w.ns_count = (uint32_t*)e->rq_ns.p;
+  w.ns_first = w.ns_count + n_ns;
+  w.ns_cursor = w.ns_first + n_ns + 1;
+  w.ns_extra = w.ns_cursor + n_ns;
+  w.ns_open = w.ns_extra + n_ns;
+  w.rank = (uint32_t*)e->rq_keys.p;
+  w.ns_keys = w.rank + n;
+  w.act = w.ns_keys + n;
+  w.out = (uint8_t*)e->rq_out.p;
+  int cuda_err = 0;
+  int launched = lwse::launch_rollout_place_waves(&w, 0, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 16, st, 32, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint32_t R = words[16 + 2], max_t = words[16 + 3];
+  // the slots (at most one per key), the column lists and the round's slices: the largest namespace plus its
+  // largest column (T_ns) per resident CTA
+  w.wc = std::min(mw, std::max(R, 1u));
+  uint8_t* slots = (uint8_t*)e->rq_slots.p;
+  w.desc = (uint4*)slots;
+  w.res = (uint32_t*)(slots + (size_t)n * 16);
+  w.items = (uint2*)(w.res + (size_t)n * 16);
+  w.col_n = (uint32_t*)(w.items + n);
+  w.col_rows = w.col_n + n;
+  w.contrib = w.col_rows + n;
+  LWSE_CUDA(e, cudaMemsetAsync(w.col_n, 0, (size_t)n * 4 * 13, s));
+  LWSE_CUDA(e, e->rq_col.reserve((size_t)n * w.wc * 16 + 16));
+  w.col = (uint4*)e->rq_col.p;
+  const uint64_t slice_rows = (uint64_t)largest_namespace(e) + max_t;
+  uint64_t grid = max_t ? std::min<uint64_t>((uint64_t)e->sm_count * 2u, n) : 0;
+  while (grid > 1 && grid * slice_rows * (sizeof(lwse_place_out) + 4) > (1ull << 30)) grid >>= 1;
+  if (grid && grid * slice_rows * (sizeof(lwse_place_out) + 4) > (1ull << 31)) return LWSE_ERR_OOM;
+  const size_t slice_out = align256((size_t)grid * slice_rows * sizeof(lwse_place_out));
+  LWSE_CUDA(e, e->rq_slices.reserve(slice_out + (size_t)grid * slice_rows * 4 + 16));
+  w.s_out = (lwse_place_out*)e->rq_slices.p;
+  w.s_unpinned = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(e->rq_slices.p) + slice_out);
+  w.slice_rows = (uint32_t)slice_rows;
+  w.grid = (uint32_t)grid;
+  if (R) {
+    cudaGraph_t graph = nullptr;
+    GraphExec exec;
+    LWSE_CUDA(e, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    launched = lwse::launch_rollout_place_waves(&w, 1, e->sm_count, s, &cuda_err);
+    const cudaError_t ce = cudaStreamEndCapture(s, &graph);
+    if (launched < 0 || ce != cudaSuccess) {
+      if (graph) cudaGraphDestroy(graph);
+      return fail_cuda(e, launched < 0 ? (cudaError_t)cuda_err : ce);
+    }
+    cudaError_t ge = exec.ensure(graph);
+    cudaGraphDestroy(graph);
+    for (uint32_t r = 0; ge == cudaSuccess && r < R; r++) ge = cudaGraphLaunch(exec, s);
+    if (ge != cudaSuccess) return fail_cuda(e, ge);
+    e->launches += (uint64_t)launched * R;
+  }
+  launched = lwse::launch_rollout_place_waves(&w, 2, e->sm_count, s, &cuda_err);
+  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(e->rq_host.h, w.out, out_bytes, cudaMemcpyDeviceToHost, s));
+  if (q->alone_rows)
+    LWSE_CUDA(e, cudaMemcpyAsync(q->alone_rows, p.rows_out, (size_t)n * sizeof(lwse_rollout_place), cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint8_t* h = static_cast<const uint8_t*>(e->rq_host.h);
+  uint32_t tot[5];
+  memcpy(tot, h, sizeof(tot));
+  memcpy(q->keys, h + 32, (size_t)n * sizeof(lwse_rollout_wave_key));
+  memcpy(q->waves, h + 32 + (size_t)n * sizeof(lwse_rollout_wave_key), (size_t)tot[0] * sizeof(lwse_rollout_wave));
+  q->n_waves = tot[0];
+  q->n_planned = tot[1];
+  q->n_triggers_alone = tot[2];
+  q->n_no_wave = tot[3];
+  q->n_not_solved = tot[4];
   return LWSE_OK;
 }
 

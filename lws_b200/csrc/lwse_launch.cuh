@@ -424,6 +424,42 @@ struct RolloutPlaceLaunch {
 int launch_rollout_place(const RolloutPlaceLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
 int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err);
 
+// ---- lwse_rollout_place_wave_kernels.cu ----
+// Rollout placement waves (lwse_resident_rollout_place_waves), over the rollout placement's setup p (its rows are
+// the alone rows).  A key takes part when it is SOLVED and clean alone; the K_ns keys of a namespace take rounds
+// 0 .. K_ns - 1 in query order.  Slot s = ns_first[ns] + w holds column (ns, w): its list of entries (at
+// ns_first[ns] * wc + w * K_ns in col), its extra rows, its committed contribution and the probe row of the round.
+struct RolloutPlaceWavesLaunch {
+  RolloutPlaceLaunch p;
+  uint32_t constraints, max_waves;
+  uint32_t wc;                    // list stride: min(max_waves, R)
+  uint32_t* st;                   // 16 words, zeroed: [0] round [1] items [2] R [3] max T_ns [4] active namespaces
+  uint32_t* rank;                 // [n] the key's round, LWSE_NONE when it does not take part
+  uint32_t* ns_count;             // [n_ns] K_ns (the scan zeroes it)
+  uint32_t* ns_first;             // [n_ns + 1]
+  uint32_t* ns_cursor;            // [n_ns]
+  uint32_t* ns_extra;             // [n_ns] T_ns, the extra rows of the namespace's keys, zeroed
+  uint32_t* ns_open;              // [n_ns] p_ns, the waves the namespace's keys use, zeroed
+  uint32_t* ns_keys;              // [n] per namespace its keys in query order
+  uint32_t* act;                  // [n] the namespaces with a key
+  uint4* desc;                    // [n] per slot: {k, first list entry, list length, column rows}
+  uint4* col;                     // [n * wc] {E_j's first extra row, offset in the column, group_base, group_count}
+  uint32_t* col_n;                // [n] per slot: list length, zeroed
+  uint32_t* col_rows;             // [n] per slot: the column's extra rows, zeroed
+  uint32_t* contrib;              // [n * 11] per slot: the committed contribution, zeroed
+  uint32_t* res;                  // [n * 16] per slot: the round's probe row (words 4..15 as lwse_rollout_place's)
+  uint2* items;                   // [n] {slot, namespace}
+  uint32_t* wtot;                 // [64 * 16] per wave: n_keys, the 11 counters, namespaces; zeroed
+  uint8_t* out;                   // the answer: 8 words of totals, n lwse_rollout_wave_key, 64 lwse_rollout_wave
+  lwse_place_out* s_out;          // [grid * slice_rows]
+  uint32_t* s_unpinned;           // [grid * slice_rows]
+  uint32_t slice_rows, grid;      // (grid 0: no column holds an extra row; no solve)
+};
+// Pass 0 (after the setup's finish): the key rows, the ranks, the scan and the per-namespace key lists.  Pass 1
+// (captured, replayed R times): items, the wave instance of place_ns_kernel, commit.  Pass 2: the finish.
+int launch_rollout_place_waves(const RolloutPlaceWavesLaunch* w, int pass, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_place_ns_rollout_wave(const RolloutPlaceWavesLaunch* w, cudaStream_t s, int* cuda_err);
+
 // ---- lwse_drain_wave_kernels.cu ----
 // lwse_resident_drain_waves.  out: the query totals (16 B), m lwse_drain_wave_key rows, then max_waves
 // lwse_drain_wave rows (the opened ones written).  counts (device, u64, zeroed by the caller): [0] the restart pairs

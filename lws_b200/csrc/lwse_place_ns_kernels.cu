@@ -134,6 +134,15 @@ struct RollNsView {
 };
 static_assert(sizeof(RollNsView) <= sizeof(CUtensorMap), "the view travels in the tensor-map parameter");
 
+// The rollout wave instance (lwse_resident_rollout_place_waves): RollNsView with items {slot, namespace}; slot s
+// probes column (ns, w) with key k: the extra rows of the ns entries already in wave w, in query order, then E_k.
+struct RollWaveNsView {
+  RollNsView r;
+  const uint4* desc;  // [slots] {k, first list entry, list length, the column's extra rows}
+  const uint4* col;   // the column lists: {E_j's first extra row, its offset in the column, group_base, group_count}
+};
+static_assert(sizeof(RollWaveNsView) <= sizeof(CUtensorMap), "the view travels in the tensor-map parameter");
+
 // The rollout instance's counters, words 4..14 of the entry's lwse_rollout_place row: placed, stranded, own_lost,
 // bumped, then the what-if counters (the three totals as deltas against the baseline).
 constexpr uint32_t kRollCounts = 11;
@@ -475,7 +484,10 @@ __device__ __forceinline__ void diff_row(const PlaceNsArgs& a, uint32_t r, const
 // kRoll (with kDrain): the rollout instance.  Item {i, ns} solves ns with entry i's extra rows E_i: positions run over
 // the namespace's resident rows through the index, then over E_i's rows (row index n_resident + j); nothing is
 // lowered or unpinned; the namespace's diff goes to entry i's row.
-template <bool kScan, bool kIndexed, bool kDrain = false, bool kSet = false, bool kRoll = false>
+// kWave (with kRoll): the rollout wave instance.  Item {s, ns} solves ns with the column's extra rows then E_k
+// (RollWaveNsView); extra position q has row index n_resident + q; a resident row lost counts as own when its
+// group lies in the range of k or of a listed entry; the namespace's diff goes to slot s's row.
+template <bool kScan, bool kIndexed, bool kDrain = false, bool kSet = false, bool kRoll = false, bool kWave = false>
 __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
     place_ns_kernel(const PlaceNsArgs a, const __grid_constant__ CUtensorMap words_map) {
   extern __shared__ uint8_t s_dyn[];
@@ -508,6 +520,8 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
   static_assert(!kSet || kDrain, "the set instance is a drain instance");
   const RollNsView* const roll = reinterpret_cast<const RollNsView*>(&words_map);
   static_assert(!kRoll || (kDrain && !kSet), "the rollout instance is a drain instance of its own");
+  const RollWaveNsView* const rwave = reinterpret_cast<const RollWaveNsView*>(&words_map);
+  static_assert(!kWave || kRoll, "the rollout wave instance is a rollout instance");
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5, n_warps = blockDim.x >> 5;
   const uint32_t* words = table_bytes ? s_words : a.g_words;
   const uint32_t* order = table_bytes ? s_order : a.node_order;
@@ -558,7 +572,14 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
       ns = w.y;
     }
     uint4 ent = make_uint4(0u, 0u, 0u, 0u);  // kRoll: the entry's {first extra row, |E_i|, group range}
-    if constexpr (kRoll) ent = __ldcg(roll->ent + key);
+    uint4 wd = make_uint4(0u, 0u, 0u, 0u);   // kWave: the slot's {k, first list entry, list length, column rows}
+    if constexpr (kWave) {
+      wd = __ldcg(rwave->desc + key);
+      ent = __ldcg(roll->ent + wd.x);
+      ent.y += wd.w;  // the positions: the column's rows, then E_k's
+    } else if constexpr (kRoll) {
+      ent = __ldcg(roll->ent + key);
+    }
     const uint32_t first = __ldcg(a.ns_first + ns), last_res = __ldcg(a.ns_first + ns + 1u), last = last_res + ent.y;
     if (tid == 0) {
       s_n_unp = 0u;
@@ -636,6 +657,19 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
       __syncthreads();
     }
     auto req_at = [&](uint32_t r, uint32_t p) -> const uint4* {  // the request row at position p (row r)
+      if constexpr (kWave) {
+        if (p >= last_res) {
+          const uint32_t q = p - last_res;
+          if (q >= wd.w) return reinterpret_cast<const uint4*>(roll->extra + ent.x + (q - wd.w));
+          uint32_t lo = wd.y, hi = wd.y + wd.z;  // the listed entry holding q: the last offset <= q
+          while (hi - lo > 1u) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (__ldg(&rwave->col[mid].y) <= q) lo = mid; else hi = mid;
+          }
+          const uint4 c = __ldg(rwave->col + lo);
+          return reinterpret_cast<const uint4*>(roll->extra + c.x + (q - c.y));
+        }
+      }
       if constexpr (kRoll) {
         if (p >= last_res) return reinterpret_cast<const uint4*>(roll->extra + ent.x + (p - last_res));
       }
@@ -925,7 +959,14 @@ __global__ void __launch_bounds__(kScan ? kNsScanThreads : kNsThreads, 2)
         const uint32_t r = row_of(p);
         const uint4 o = __ldg(reinterpret_cast<const uint4*>(dv.base + r));
         const bool was = (o.z & LWSE_PLACE_PLACED) != 0u;
-        const bool own = __ldg(&a.reqs[r].group) - ent.z < ent.w;
+        const uint32_t grp = __ldg(&a.reqs[r].group);
+        bool own = grp - ent.z < ent.w;
+        if constexpr (kWave) {  // a lost row: the listed entries' ranges too
+          for (uint32_t j = wd.y; !own && was && !is && j < wd.y + wd.z; j++) {
+            const uint4 c = __ldg(rwave->col + j);
+            own = grp - c.z < c.w;
+          }
+        }
         c[2] += (own && was && !is) ? 1u : 0u;
         c[3] += (!own && was && !is) ? 1u : 0u;
         c[4] += (v.x != o.x || v.y != o.y || v.z != o.z || v.w != o.w) ? 1u : 0u;
@@ -1417,15 +1458,8 @@ int launch_place_ns_drain_set(const DrainPlaceWavesLaunch* d, int sm_count, cuda
   return 1;
 }
 
-// The rollout placement solve: the capacities of the node index (the condense kernel's part A alone), then the
-// rollout instance over p->grid CTAs.  The round scratch holds the namespace index of every namespace.
-int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
-  const NsLayout l = ns_layout(p->n_nodes, p->n_domains, p->n_reqs, p->n_namespaces);
-  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) {
-    *cuda_err = (int)cudaErrorInvalidValue;
-    return -1;
-  }
+// The rollout instances' arguments over the round scratch, which holds the namespace index of every namespace.
+static PlaceNsArgs rollout_ns_args(const RolloutPlaceLaunch* p, const NsLayout& l) {
   uint8_t* base = static_cast<uint8_t*>(p->round);
   PlaceNsArgs a{};
   a.nodes = p->nodes;
@@ -1446,14 +1480,10 @@ int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStrea
   a.n_namespaces = p->n_namespaces;
   a.n_parts = 1u;
   a.word_rows = l.word_rows;
-  {
-    uint64_t grid = ((uint64_t)p->n_domains * 32u + 255) / 256;
-    if (grid < 1) grid = 1;
-    if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
-    place_condense_kernel<<<(unsigned)grid, 256, 0, s>>>(a);  // (a.n_reqs = 0: capacities only)
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
-  }
+  return a;
+}
+
+static RollNsView rollout_ns_view(const RolloutPlaceLaunch* p) {
   RollNsView v{};
   v.d.items = p->items;
   v.d.n_items = p->counts;
@@ -1464,6 +1494,28 @@ int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStrea
   v.extra = p->extra;
   v.ent = p->ent;
   v.n_resident = p->n_reqs;
+  return v;
+}
+
+// The rollout placement solve: the capacities of the node index (the condense kernel's part A alone), then the
+// rollout instance over p->grid CTAs.  The round scratch holds the namespace index of every namespace.
+int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  const NsLayout l = ns_layout(p->n_nodes, p->n_domains, p->n_reqs, p->n_namespaces);
+  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) {
+    *cuda_err = (int)cudaErrorInvalidValue;
+    return -1;
+  }
+  PlaceNsArgs a = rollout_ns_args(p, l);
+  {
+    uint64_t grid = ((uint64_t)p->n_domains * 32u + 255) / 256;
+    if (grid < 1) grid = 1;
+    if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
+    place_condense_kernel<<<(unsigned)grid, 256, 0, s>>>(a);  // (a.n_reqs = 0: capacities only)
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+  }
+  const RollNsView v = rollout_ns_view(p);
   CUtensorMap view;
   memset(&view, 0, sizeof(view));
   memcpy(&view, &v, sizeof(v));
@@ -1482,6 +1534,45 @@ int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStrea
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
   return 2;
+}
+
+// One round's solve of the rollout waves: the wave instance over w->grid CTAs, on the capacities and the namespace
+// index the setup's rollout solve left in the round scratch.
+int launch_place_ns_rollout_wave(const RolloutPlaceWavesLaunch* w, cudaStream_t s, int* cuda_err) {
+  *cuda_err = 0;
+  const RolloutPlaceLaunch* p = &w->p;
+  const NsLayout l = ns_layout(p->n_nodes, p->n_domains, p->n_reqs, p->n_namespaces);
+  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) {
+    *cuda_err = (int)cudaErrorInvalidValue;
+    return -1;
+  }
+  PlaceNsArgs a = rollout_ns_args(p, l);
+  RollWaveNsView v{};
+  v.r = rollout_ns_view(p);
+  v.r.d.items = w->items;
+  v.r.d.n_items = w->st + 1;
+  v.r.d.rows = w->res;
+  v.r.d.slice_rows = w->slice_rows;
+  v.desc = w->desc;
+  v.col = w->col;
+  CUtensorMap view;
+  memset(&view, 0, sizeof(view));
+  memcpy(&view, &v, sizeof(v));
+  a.n_reqs = p->n_reqs;
+  a.out = w->s_out;
+  a.unpinned = w->s_unpinned;
+  const size_t smem = ns_smem_bytes(l.word_rows, p->n_domains, false, false);
+  static thread_local size_t attr_set = 0;
+  if (smem > attr_set) {
+    const cudaError_t e = cudaFuncSetAttribute(place_ns_kernel<false, true, true, false, true, true>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    attr_set = smem;
+  }
+  place_ns_kernel<false, true, true, false, true, true><<<w->grid, kNsThreads, smem, s>>>(a, view);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+  return 1;
 }
 
 int launch_index_scan(uint32_t* d_count, uint32_t* d_first, uint32_t* d_cursor, uint32_t n, cudaStream_t s, int* cuda_err) {

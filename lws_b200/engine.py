@@ -55,6 +55,7 @@ SYMBOLS = {
     "lwse_resident_ds_drain_waves": ([C.c_void_p, C.POINTER(R.DsDrainWavesQuery)], C.c_int),
     "lwse_resident_drain_place_waves": ([C.c_void_p, C.POINTER(R.DrainPlaceWavesQuery)], C.c_int),
     "lwse_resident_rollout_place": ([C.c_void_p, C.POINTER(R.RolloutPlaceQuery)], C.c_int),
+    "lwse_resident_rollout_place_waves": ([C.c_void_p, C.POINTER(R.RolloutPlaceWavesQuery)], C.c_int),
     "lwse_place_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
         C.c_int,
@@ -158,6 +159,27 @@ def _aligned16(a: np.ndarray) -> np.ndarray:
     b = R.aligned_empty(len(a), a.dtype)
     b[:] = a
     return b
+
+
+def rollout_waves_args(rows, ns, recs, max_waves, constraints):
+    """The arguments of ``Engine.resident_rollout_place_waves`` as the call takes them → (rows, ns, recs);
+    ValueError for a duplicate row, a cap outside 1 .. DRAIN_WAVES_MAX or a zero or unknown constraint bit."""
+    rows = np.ascontiguousarray(rows, dtype=np.uint32)
+    ns = np.ascontiguousarray(ns, dtype=np.uint32)
+    if len(ns) != len(rows):
+        raise ValueError("rows and ns differ in length")
+    if len(np.unique(rows)) != len(rows):
+        raise ValueError("rollout waves take each LWS row once")
+    if not 1 <= max_waves <= R.DRAIN_WAVES_MAX:
+        raise ValueError(f"max_waves must be in 1 .. {R.DRAIN_WAVES_MAX}")
+    if constraints == 0 or constraints & ~R.RPW_ALL:
+        raise ValueError("constraints must be a nonzero mask of RPW_* bits")
+    if recs is not None:
+        recs = np.asarray(recs)
+        if recs.dtype != R.LWS_REC or len(recs) != len(rows):
+            raise ValueError("recs must be one LWS_REC per entry")
+        recs = _aligned16(recs)
+    return rows, ns, recs
 
 
 class Engine:
@@ -936,6 +958,36 @@ class Engine:
         res.update({k: getattr(q, k) for k in R.ROLLOUT_PLACE_TOTALS})
         if extra:
             res["extra"] = xs[: min(q.n_surge, probe.n_surge)]
+        return res
+
+    def resident_rollout_place_waves(self, rows, ns, recs=None, max_waves=R.DRAIN_WAVES_MAX,
+                                     constraints=R.RPW_STRANDED, alone=False):
+        """lwse_resident_rollout_place_waves: the entries of ``resident_rollout_place`` (distinct ``rows``) packed
+        first-fit, in the order given, into at most ``max_waves`` waves whose rollouts, pushed together, trigger
+        none of the verdicts in ``constraints`` (``records.RPW_*``).  The default finds every group the wave's
+        rollouts add an exclusive domain; ``RPW_BUMPED`` (no resident group loses its domain) is opt-in.  → dict:
+        ``keys`` (``records.ROLLOUT_WAVE_KEY``, in query order), ``waves`` (``records.ROLLOUT_WAVE``, one per opened
+        wave), the query's ``lws_rows`` and ``ns``, the totals of ``records.ROLLOUT_WAVES_TOTALS`` and, with
+        ``alone``, ``alone_rows``: ``resident_rollout_place``'s rows for the same query.  Changes nothing resident
+        and waits for no tick."""
+        rows, ns, recs = rollout_waves_args(rows, ns, recs, max_waves, constraints)
+        n = len(rows)
+        keys = R.aligned_empty(max(n, 1), R.ROLLOUT_WAVE_KEY)
+        waves = R.aligned_empty(max_waves, R.ROLLOUT_WAVE)
+        q = R.RolloutPlaceWavesQuery()
+        q.rows = R.ptr(rows) if n else None
+        q.ns = R.ptr(ns) if n else None
+        q.recs = R.ptr(recs) if (recs is not None and n) else None
+        q.n, q.max_waves, q.constraints = n, max_waves, constraints
+        q.keys, q.waves = R.ptr(keys), R.ptr(waves)
+        if alone:
+            alone_rows = R.aligned_empty(max(n, 1), R.ROLLOUT_PLACE)
+            q.alone_rows = R.ptr(alone_rows)
+        self._check(lib().lwse_resident_rollout_place_waves(self._h, C.byref(q)))
+        res = {"keys": keys[:n], "waves": waves[: q.n_waves], "lws_rows": rows, "ns": ns}
+        res.update({k: getattr(q, k) for k in R.ROLLOUT_WAVES_TOTALS})
+        if alone:
+            res["alone_rows"] = alone_rows[:n]
         return res
 
     # ------------------------------------------------------------- group keys

@@ -586,6 +586,23 @@ class IncrementalEncoder:
             out.append(d)
         return out
 
+    def rollout_place_waves_report(self, result: dict) -> dict:
+        """A ``resident_rollout_place_waves`` answer by name → {"waves": per opened wave the (namespace, name) of its
+        objects in query order, "unplanned": one dict per key that is not planned, in query order, with
+        ``namespace``, ``name``, ``status`` (``records.ROLLW_NAMES``) and ``alone`` (``records.RPW_NAMES``)}.  The
+        entries come from ``rollout_place_query`` or ``rollout_place_proposal``.  Nothing in the encoder changes."""
+        names = {sl.lws_row: k for k, sl in self.slots.items()}
+        waves = [[] for _ in range(len(result["waves"]))]
+        unplanned = []
+        for r, k in zip(np.asarray(result["lws_rows"]).tolist(), result["keys"]):
+            key = names.get(int(r), (None, None))
+            if int(k["status"]) == R.ROLLW_PLANNED:
+                waves[int(k["wave"])].append(key)
+                continue
+            unplanned.append({"namespace": key[0], "name": key[1], "status": R.ROLLW_NAMES[int(k["status"])],
+                              "alone": [v for b, v in R.RPW_NAMES.items() if int(k["alone"]) & b]})
+        return {"waves": waves, "unplanned": unplanned}
+
     def whatif_drain(self, node_names) -> np.ndarray:
         """The node rows of the named nodes, for ``Engine.resident_drain_whatif`` (sorted, each once)."""
         return np.array(sorted({self.node_index[n] for n in node_names}), dtype=np.uint32)

@@ -868,6 +868,61 @@ class RolloutPlaceQuery(C.Structure):
 assert C.sizeof(RolloutPlaceQuery) == 80
 
 
+# rollout placement waves (lwse_resident_rollout_place_waves): the verdicts a wave keeps and the status of a key
+RPW_STRANDED = 1 << 0
+RPW_BUMPED = 1 << 1
+RPW_ALL = RPW_STRANDED | RPW_BUMPED
+RPW_NAMES = {RPW_STRANDED: "stranded", RPW_BUMPED: "bumped"}
+ROLLW_PLANNED = DRAINW_PLANNED
+ROLLW_TRIGGERS_ALONE = DRAINW_BREACHES_ALONE
+ROLLW_NO_WAVE = DRAINW_NO_WAVE
+ROLLW_NOT_SOLVED = 3
+ROLLW_NAMES = {ROLLW_PLANNED: "planned", ROLLW_TRIGGERS_ALONE: "triggers_alone", ROLLW_NO_WAVE: "no_wave",
+               ROLLW_NOT_SOLVED: "not_solved"}
+
+# lwse_rollout_wave_key: one key of the plan, in query order
+ROLLOUT_WAVE_KEY = np.dtype([("wave", "<u4"), ("status", "<u4"), ("alone", "<u4"), ("reserved", "<u4")], align=False)
+assert ROLLOUT_WAVE_KEY.itemsize == 16
+
+# lwse_rollout_wave: one opened wave, the set-form totals over its keys
+ROLLOUT_WAVE = np.dtype(
+    [("n_keys", "<u4"), ("surge", "<u4"), ("placed", "<u4"), ("stranded", "<u4"), ("own_lost", "<u4"), ("bumped", "<u4"),
+     ("n_changed", "<u4"), ("n_lost", "<u4"), ("n_moved", "<u4"), ("n_gained", "<u4"), ("n_placed", "<u4"),
+     ("n_unschedulable", "<u4"), ("n_conflict", "<u4"), ("namespaces", "<u4"), ("reserved", "<u4", (2,))],
+    align=False,
+)
+assert ROLLOUT_WAVE.itemsize == 64
+ROLLOUT_WAVES_TOTALS = ("n_waves", "n_planned", "n_triggers_alone", "n_no_wave", "n_not_solved")
+
+
+class RolloutPlaceWavesQuery(C.Structure):
+    """lwse_rollout_place_waves_query: the entries of RolloutPlaceQuery (distinct rows), the cap and the RPW_* mask
+    in; the ROLLOUT_WAVE_KEY and ROLLOUT_WAVE rows, optionally the ROLLOUT_PLACE alone rows, and the
+    ROLLOUT_WAVES_TOTALS out."""
+
+    _fields_ = [
+        ("rows", C.c_void_p),
+        ("ns", C.c_void_p),
+        ("recs", C.c_void_p),
+        ("n", C.c_uint32),
+        ("max_waves", C.c_uint32),
+        ("constraints", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("keys", C.c_void_p),
+        ("waves", C.c_void_p),
+        ("alone_rows", C.c_void_p),
+        ("n_waves", C.c_uint32),
+        ("n_planned", C.c_uint32),
+        ("n_triggers_alone", C.c_uint32),
+        ("n_no_wave", C.c_uint32),
+        ("n_not_solved", C.c_uint32),
+        ("reserved1", C.c_uint32),
+    ]
+
+
+assert C.sizeof(RolloutPlaceWavesQuery) == 88
+
+
 class Config(C.Structure):
     _fields_ = [
         ("abi_version", C.c_uint32),
