@@ -205,14 +205,14 @@ __global__ void __launch_bounds__(kForecastScanThreads) scan_apply_kernel(const 
   }
 }
 
+// Enqueues the scan's kernels (three, one when n is 0); the caller checks them with the launches around.
 template <class Op>
-inline cudaError_t launch_forecast_scan(const Op& op, uint32_t n, unsigned long long* sums, unsigned long long* total,
-                                        unsigned long long* acc, cudaStream_t s) {
+inline void launch_forecast_scan(const Op& op, uint32_t n, unsigned long long* sums, unsigned long long* total,
+                                 unsigned long long* acc, cudaStream_t s) {
   const uint32_t blocks = forecast_scan_words(n);
   if (blocks) scan_block_sums_kernel<Op><<<blocks, kForecastScanThreads, 0, s>>>(op, n, sums);
   scan_carry_kernel<Op><<<1, kForecastScanThreads, 0, s>>>(sums, blocks, total);
   if (blocks) scan_apply_kernel<Op><<<blocks, kForecastScanThreads, 0, s>>>(op, n, sums, acc);
-  return cudaGetLastError();
 }
 
 // The trajectory layout: step_base (a row count after the summary pass) becomes the exclusive prefix over
@@ -239,6 +239,13 @@ struct StepLayoutOp {
     return written;
   }
 };
+
+// A grid of one CTA per per_cta items, at least one CTA and at most cap.
+inline unsigned grid_for(uint64_t items, uint32_t per_cta, uint32_t cap) {
+  uint64_t grid = (items + per_cta - 1) / per_cta;
+  if (grid < 1) grid = 1;
+  return (unsigned)(grid < cap ? grid : cap);
+}
 
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,

@@ -37,21 +37,6 @@ __device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v)
   return v;
 }
 
-static int launched_or_fail(int kernels, int* cuda_err) {
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return kernels;
-}
-
-static unsigned grid_for(uint64_t items, uint32_t per_cta, uint32_t cap) {
-  uint64_t grid = (items + per_cta - 1) / per_cta;
-  if (grid < 1) grid = 1;
-  return (unsigned)(grid < cap ? grid : cap);
-}
-
 // --------------------------------------------------------------------------
 // drain what-if: mark, then diff
 // --------------------------------------------------------------------------
@@ -92,13 +77,11 @@ __global__ void __launch_bounds__(256) drain_mark_kernel(const DrainMarkArgs a) 
 }
 
 int launch_drain_mark(const uint8_t* d_mask, uint32_t n_nodes, const lwse_pod_ident* d_ident, uint8_t* d_state, uint64_t n_pods,
-                      lwse_group_rec* d_groups, uint32_t n_groups, uint32_t* d_counts, int sm_count, cudaStream_t s,
-                      int* cuda_err) {
-  *cuda_err = 0;
+                      lwse_group_rec* d_groups, uint32_t n_groups, uint32_t* d_counts, int sm_count, cudaStream_t s) {
   const DrainMarkArgs a{d_mask, d_ident, d_state, d_groups, d_counts, n_pods, n_groups, n_nodes};
   const uint64_t items = n_pods > n_groups ? n_pods : n_groups;
   drain_mark_kernel<<<grid_for(items, 256, (uint32_t)sm_count * 16u), 256, 0, s>>>(a);
-  return launched_or_fail(1, cuda_err);
+  return launch_result(1);
 }
 
 struct DrainDiffArgs {
@@ -151,11 +134,10 @@ __global__ void __launch_bounds__(256) drain_diff_kernel(const DrainDiffArgs a) 
 
 int launch_drain_diff(const lwse_group_out* d_before, const lwse_group_out* d_after, const lwse_group_rec* d_groups,
                       uint32_t n_groups, uint32_t* d_rows, lwse_group_out* d_outs_before, lwse_group_out* d_outs_after,
-                      uint32_t capacity, uint32_t* d_counts, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                      uint32_t capacity, uint32_t* d_counts, int sm_count, cudaStream_t s) {
   const DrainDiffArgs a{d_before, d_after, d_groups, d_rows, d_outs_before, d_outs_after, d_counts, capacity, n_groups};
   drain_diff_kernel<<<grid_for(n_groups, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(a);
-  return launched_or_fail(1, cuda_err);
+  return launch_result(1);
 }
 
 // --------------------------------------------------------------------------
@@ -253,12 +235,11 @@ __global__ void __launch_bounds__(kCostThreads) drain_cost_kernel(const DrainCos
 
 int launch_drain_cost(const lwse_lws_rec* d_lws, uint32_t n_lws, const lwse_group_rec* d_groups, uint32_t n_groups,
                       const uint8_t* d_state, const lwse_pod_ident* d_ident, uint64_t n_pods, const lwse_group_out* d_baseline,
-                      lwse_drain_cost* d_cost, uint32_t n_nodes, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                      lwse_drain_cost* d_cost, uint32_t n_nodes, int sm_count, cudaStream_t s) {
   if (n_groups == 0) return 0;
   const DrainCostArgs a{d_lws, d_groups, d_state, d_ident, d_baseline, d_cost, n_pods, n_lws, n_groups, n_nodes};
   drain_cost_kernel<<<grid_for(n_groups, kCostThreads / 32, (uint32_t)sm_count * 8u), kCostThreads, 0, s>>>(a);
-  return launched_or_fail(1, cuda_err);
+  return launch_result(1);
 }
 
 // --------------------------------------------------------------------------
@@ -280,11 +261,10 @@ __global__ void __launch_bounds__(256) drain_domain_mask_kernel(const DrainDomai
 }
 
 int launch_drain_domain_mask(const uint8_t* d_domains, uint32_t n_domains, const lwse_node_rec* d_nodes, uint32_t n_nodes,
-                             uint8_t* d_mask, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                             uint8_t* d_mask, int sm_count, cudaStream_t s) {
   const DrainDomainMaskArgs a{d_domains, d_nodes, d_mask, n_nodes, n_domains};
   drain_domain_mask_kernel<<<grid_for(n_nodes, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(a);
-  return launched_or_fail(1, cuda_err);
+  return launch_result(1);
 }
 
 // The set form: one warp per LWS row over its group range, the what-if rows against the baseline.
@@ -350,13 +330,11 @@ __global__ void __launch_bounds__(256) drain_budget_kernel(const DrainBudgetArgs
 
 int launch_drain_budget(const lwse_lws_rec* d_lws, const lwse_lws_out* d_lws_out, uint32_t n_lws, const lwse_group_rec* d_groups,
                         const lwse_group_out* d_before, const lwse_group_out* d_after, uint32_t n_groups,
-                        lwse_drain_budget* d_rows, uint32_t capacity, uint32_t* d_counts, int sm_count, cudaStream_t s,
-                        int* cuda_err) {
-  *cuda_err = 0;
+                        lwse_drain_budget* d_rows, uint32_t capacity, uint32_t* d_counts, int sm_count, cudaStream_t s) {
   if (n_lws == 0) return 0;
   const DrainBudgetArgs a{d_lws, d_lws_out, d_groups, d_before, d_after, d_rows, d_counts, capacity, n_lws, n_groups};
   drain_budget_kernel<<<grid_for(n_lws, 256 / 32, (uint32_t)sm_count * 8u), 256, 0, s>>>(a);
-  return launched_or_fail(1, cuda_err);
+  return launch_result(1);
 }
 
 // The per-key form.  The walk is drain_cost_kernel's with the restart node mapped to its key (the node, or
@@ -538,8 +516,7 @@ __global__ void __launch_bounds__(256) drain_budget_finish_kernel(const DrainBud
   }
 }
 
-int launch_drain_budget_cost(const DrainBudgetCostLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_drain_budget_cost(const DrainBudgetCostLaunch* p, int pass, int sm_count, cudaStream_t s) {
   const DrainBudgetCostArgs a{p->lws, p->lws_out, p->groups, p->pod_state, p->pod_ident, p->baseline,
                               p->by_domain ? p->nodes : nullptr, p->cost, p->keys, p->vals, p->counts,
                               p->n_pods, p->n_lws, p->n_groups, p->n_nodes, p->n_domains, p->table_mask};
@@ -549,28 +526,27 @@ int launch_drain_budget_cost(const DrainBudgetCostLaunch* p, int pass, int sm_co
       const uint32_t n = p->n_keys > p->n_nodes ? p->n_keys : p->n_nodes;
       drain_budget_keys_init_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(a, p->occupancy, p->n_keys);
       if (p->n_groups) drain_budget_walk_kernel<false><<<walk_grid, kCostThreads, 0, s>>>(a);
-      return launched_or_fail(p->n_groups ? 2 : 1, cuda_err);
+      return launch_result(p->n_groups ? 2 : 1);
     }
     case 1:
       drain_budget_walk_kernel<true><<<walk_grid, kCostThreads, 0, s>>>(a);
       drain_budget_finish_kernel<<<grid_for((uint64_t)p->table_mask + 1, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(a);
-      return launched_or_fail(2, cuda_err);
+      return launch_result(2);
     default:  // the table alone, for the DS drain's per-key form
       drain_budget_walk_kernel<true><<<walk_grid, kCostThreads, 0, s>>>(a);
-      return launched_or_fail(1, cuda_err);
+      return launch_result(1);
   }
 }
 
 int launch_drain_restart_pairs(const DrainBudgetCostLaunch* p, unsigned long long* pairs, uint32_t capacity, int sm_count,
-                               cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                               cudaStream_t s) {
   if (p->n_groups == 0) return 0;
   const DrainBudgetCostArgs a{p->lws, p->lws_out, p->groups, p->pod_state, p->pod_ident, p->baseline,
                               p->by_domain ? p->nodes : nullptr, nullptr, pairs, nullptr, p->counts,
                               p->n_pods, p->n_lws, p->n_groups, p->n_nodes, p->n_domains, capacity};
   drain_budget_walk_kernel<false, true>
       <<<grid_for(p->n_groups, kCostThreads / 32, (uint32_t)sm_count * 8u), kCostThreads, 0, s>>>(a);
-  return launched_or_fail(1, cuda_err);
+  return launch_result(1);
 }
 
 // --------------------------------------------------------------------------
@@ -621,12 +597,11 @@ __global__ void __launch_bounds__(256) ds_drain_lost_kernel(const DsDrainLostArg
 
 int launch_ds_drain_lost(const lwse_lws_rec* d_lws, const lwse_lws_out* d_lws_out, uint32_t n_lws, const lwse_group_rec* d_groups,
                          const lwse_group_out* d_before, const lwse_group_out* d_after, uint32_t n_groups, uint32_t* d_lost,
-                         lwse_lws_out* d_lws_after, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                         lwse_lws_out* d_lws_after, int sm_count, cudaStream_t s) {
   if (n_lws == 0) return 0;
   const DsDrainLostArgs a{d_lws, d_lws_out, d_groups, d_before, d_after, d_lost, d_lws_after, n_lws, n_groups};
   ds_drain_lost_kernel<<<grid_for(n_lws, 256 / 32, (uint32_t)sm_count * 8u), 256, 0, s>>>(a);
-  return launched_or_fail(1, cuda_err);
+  return launch_result(1);
 }
 
 constexpr uint32_t kDsdNewZeroed = 1u << 0;   // a spec row of the new revision falls below 1 ready
@@ -700,16 +675,15 @@ __global__ void __launch_bounds__(256) ds_drain_finish_kernel(const DsDrainCostL
   }
 }
 
-int launch_ds_drain_cost(const DsDrainCostLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_ds_drain_cost(const DsDrainCostLaunch* p, int pass, int sm_count, cudaStream_t s) {
   const unsigned lws_grid = grid_for((uint64_t)p->lws_mask + 1, 256, (uint32_t)sm_count * 8u);
   if (pass == 0) {
     ds_drain_pairs_kernel<<<lws_grid, 256, 0, s>>>(*p);
-    return launched_or_fail(1, cuda_err);
+    return launch_result(1);
   }
   ds_drain_insert_kernel<<<lws_grid, 256, 0, s>>>(*p);
   ds_drain_finish_kernel<<<grid_for((uint64_t)p->table_mask + 1, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p);
-  return launched_or_fail(2, cuda_err);
+  return launch_result(2);
 }
 
 }  // namespace lwse

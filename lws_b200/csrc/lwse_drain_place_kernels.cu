@@ -19,21 +19,6 @@
 
 namespace lwse {
 
-static int launched_or_fail(int kernels, int* cuda_err) {
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return kernels;
-}
-
-static unsigned grid_for(uint64_t items, uint32_t per_cta, uint32_t cap) {
-  uint64_t grid = (items + per_cta - 1) / per_cta;
-  if (grid < 1) grid = 1;
-  return (unsigned)(grid < cap ? grid : cap);
-}
-
 constexpr unsigned long long kFreeItem = ~0ull;
 
 // The key whose drain set holds node n: the node itself, or its domain (by domain_id alone); LWSE_NONE for none.
@@ -203,23 +188,21 @@ __global__ void __launch_bounds__(256) drain_place_items_kernel(const DrainPlace
   }
 }
 
-int launch_drain_place(const DrainPlaceLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_drain_place(const DrainPlaceLaunch* p, int pass, int sm_count, cudaStream_t s) {
   const unsigned req_grid = grid_for(p->n_reqs, 256, (uint32_t)sm_count * 8u);
   switch (pass) {
     case 0: {
       drain_place_dom_free_kernel<<<grid_for((uint64_t)p->n_domains * 32u, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p);
       drain_place_prep_kernel<<<req_grid, 256, 0, s>>>(*p);
-      int n = launched_or_fail(2, cuda_err);
-      if (n < 0) return n;
-      if (launch_index_scan(p->g_count, p->g_first, p->g_cursor, p->n_groups, s, cuda_err) < 0) return -1;
+      if (const int r = launch_result(2); r < 0) return r;
+      if (const int r = launch_index_scan(p->g_count, p->g_first, p->g_cursor, p->n_groups, s); r < 0) return r;
       drain_place_group_fill_kernel<<<req_grid, 256, 0, s>>>(*p);
-      return launched_or_fail(4, cuda_err);
+      return launch_result(4);
     }
     case 1: {
       drain_place_unpin_kernel<false><<<grid_for(p->n_pairs, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p);
-      if (launched_or_fail(1, cuda_err) < 0) return -1;
-      if (launch_index_scan(p->u_count, p->u_first, p->u_cursor, p->n_keys, s, cuda_err) < 0) return -1;
+      if (const int r = launch_result(1); r < 0) return r;
+      if (const int r = launch_index_scan(p->u_count, p->u_first, p->u_cursor, p->n_keys, s); r < 0) return r;
       return 2;
     }
     default: {
@@ -227,9 +210,9 @@ int launch_drain_place(const DrainPlaceLaunch* p, int pass, int sm_count, cudaSt
       drain_place_unpin_kernel<true><<<grid_for(n, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p);
       drain_place_rows_kernel<<<grid_for(p->n_keys, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(*p);
       drain_place_items_kernel<<<grid_for((uint64_t)(p->n_reqs > p->n_unpinned ? p->n_reqs : p->n_unpinned), 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p);
-      if (launched_or_fail(3, cuda_err) < 0) return -1;
-      const int solved = launch_place_ns_drain(p, sm_count, s, cuda_err);
-      return solved < 0 ? -1 : 3 + solved;
+      if (const int r = launch_result(3); r < 0) return r;
+      const int solved = launch_place_ns_drain(p, sm_count, s);
+      return solved < 0 ? solved : 3 + solved;
     }
   }
 }

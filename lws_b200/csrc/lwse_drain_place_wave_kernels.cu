@@ -22,21 +22,6 @@
 
 namespace lwse {
 
-static int launched_or_fail(int kernels, int* cuda_err) {
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return kernels;
-}
-
-static unsigned grid_for(uint64_t items, uint32_t per_cta, uint32_t cap) {
-  uint64_t grid = (items + per_cta - 1) / per_cta;
-  if (grid < 1) grid = 1;
-  return (unsigned)(grid < cap ? grid : cap);
-}
-
 // (the pair record bits and dense flags of lwse_drain_wave_kernels.cu)
 constexpr uint32_t kPairMember = 1u << 0;
 constexpr uint32_t kPairReady = 1u << 1;
@@ -371,33 +356,32 @@ __global__ void __launch_bounds__(256) dpw_finish_kernel(const DrainPlaceWavesLa
                                                   d.st->status[LWSE_DRAINW_NO_WAVE]);
 }
 
-int launch_drain_place_waves(const DrainPlaceWavesLaunch* d, int pass, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_drain_place_waves(const DrainPlaceWavesLaunch* d, int pass, int sm_count, cudaStream_t s) {
   switch (pass) {
     case 0: {  // the rule-(b) domain index and the first step's columns
       const unsigned g = grid_for(d->p.n_reqs, 256, (uint32_t)sm_count * 8u);
       dpw_domain_count_kernel<<<g, 256, 0, s>>>(*d);
-      if (launched_or_fail(1, cuda_err) < 0) return -1;
-      if (launch_index_scan(d->dix_count, d->dix_first, d->dix_cursor, d->p.n_domains, s, cuda_err) < 0) return -1;
+      if (const int r = launch_result(1); r < 0) return r;
+      if (const int r = launch_index_scan(d->dix_count, d->dix_first, d->dix_cursor, d->p.n_domains, s); r < 0) return r;
       dpw_domain_fill_kernel<<<g, 256, 0, s>>>(*d);
       dpw_init_kernel<<<1, 256, 0, s>>>(*d);
-      return launched_or_fail(4, cuda_err);
+      return launch_result(4);
     }
     case 1: {  // one step (captured into the step graph)
       dpw_floor_kernel<<<1, kStepThreads, 0, s>>>(*d);
       dpw_items_kernel<<<(unsigned)sm_count * 2u, 256, 0, s>>>(*d);
-      if (launched_or_fail(2, cuda_err) < 0) return -1;
-      const int solved = launch_place_ns_drain_set(d, sm_count, s, cuda_err);
-      if (solved < 0) return -1;
+      if (const int r = launch_result(2); r < 0) return r;
+      const int solved = launch_place_ns_drain_set(d, sm_count, s);
+      if (solved < 0) return solved;
       dpw_commit_kernel<<<1, kStepThreads, 0, s>>>(*d);
-      return launched_or_fail(3 + solved, cuda_err);
+      return launch_result(3 + solved);
     }
     default: {  // the finish
-      if (launch_drain_waves_finish(&d->w, sm_count, s, cuda_err) < 0) return -1;
+      if (const int r = launch_drain_waves_finish(&d->w, sm_count, s); r < 0) return r;
       dpw_breached_kernel<<<grid_for(d->w.n_dense, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(*d);
       const uint32_t n = d->w.m > LWSE_DRAIN_WAVES_MAX ? d->w.m : LWSE_DRAIN_WAVES_MAX;
       dpw_finish_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(*d);
-      return launched_or_fail(3, cuda_err);
+      return launch_result(3);
     }
   }
 }

@@ -23,21 +23,6 @@
 
 namespace lwse {
 
-static int launched_or_fail(int kernels, int* cuda_err) {
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return kernels;
-}
-
-static unsigned grid_for(uint64_t items, uint32_t per_cta, uint32_t cap) {
-  uint64_t grid = (items + per_cta - 1) / per_cta;
-  if (grid < 1) grid = 1;
-  return (unsigned)(grid < cap ? grid : cap);
-}
-
 // A pair record: {group, owner (the LWS row, then its dense row; LWSE_NONE: not a member), bits, pod_count}.
 constexpr uint32_t kPairMember = 1u << 0;
 constexpr uint32_t kPairReady = 1u << 1;    // the group's baseline row has COND_READY
@@ -299,52 +284,49 @@ __global__ void __launch_bounds__(kPlanThreads, 1) drain_waves_plan_capped_kerne
 }
 
 int launch_drain_waves_capped(const DrainWavesLaunch* p, const uint32_t* caps, uint32_t constraints, int pass, int sm_count,
-                              cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                              cudaStream_t s) {
   if (pass == 1) {
     drain_waves_fill_capped_kernel<<<grid_for(p->n_pairs, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p, caps);
-    if (launched_or_fail(1, cuda_err) < 0) return -1;
-    if (launch_index_scan(p->l_count, p->l_first, p->l_cursor, p->n_lws, s, cuda_err) < 0) return -1;
+    if (const int r = launch_result(1); r < 0) return r;
+    if (const int r = launch_index_scan(p->l_count, p->l_first, p->l_cursor, p->n_lws, s); r < 0) return r;
     const uint64_t n = p->n_lws > p->n_pairs ? p->n_lws : p->n_pairs;
     drain_waves_dense_capped_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p, caps, constraints);
-    return launched_or_fail(3, cuda_err);
+    return launch_result(3);
   }
   drain_waves_plan_capped_kernel<<<1, kPlanThreads, 0, s>>>(*p);
   const uint32_t n = p->n_dense > p->m ? p->n_dense : p->m;
   drain_waves_finish_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(*p);
-  return launched_or_fail(2, cuda_err);
+  return launch_result(2);
 }
 
-int launch_drain_waves_finish(const DrainWavesLaunch* p, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_drain_waves_finish(const DrainWavesLaunch* p, int sm_count, cudaStream_t s) {
   const uint32_t n = p->n_dense > p->m ? p->n_dense : p->m;
   drain_waves_finish_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(*p);
-  return launched_or_fail(1, cuda_err);
+  return launch_result(1);
 }
 
-int launch_drain_waves(const DrainWavesLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_drain_waves(const DrainWavesLaunch* p, int pass, int sm_count, cudaStream_t s) {
   switch (pass) {
     case 0: {
       const uint32_t n = p->m > p->n_keys ? p->m : p->n_keys;
       drain_waves_keys_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(*p);
-      if (launched_or_fail(1, cuda_err) < 0) return -1;
-      if (launch_index_scan(p->count, p->first, p->cursor, p->m, s, cuda_err) < 0) return -1;
+      if (const int r = launch_result(1); r < 0) return r;
+      if (const int r = launch_index_scan(p->count, p->first, p->cursor, p->m, s); r < 0) return r;
       return 2;
     }
     case 1: {
       drain_waves_fill_kernel<<<grid_for(p->n_pairs, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p);
-      if (launched_or_fail(1, cuda_err) < 0) return -1;
-      if (launch_index_scan(p->l_count, p->l_first, p->l_cursor, p->n_lws, s, cuda_err) < 0) return -1;
+      if (const int r = launch_result(1); r < 0) return r;
+      if (const int r = launch_index_scan(p->l_count, p->l_first, p->l_cursor, p->n_lws, s); r < 0) return r;
       const uint64_t n = p->n_lws > p->n_pairs ? p->n_lws : p->n_pairs;
       drain_waves_dense_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 8u), 256, 0, s>>>(*p);
-      return launched_or_fail(3, cuda_err);
+      return launch_result(3);
     }
     default: {
       drain_waves_plan_kernel<<<1, kPlanThreads, 0, s>>>(*p);
       const uint32_t n = p->n_dense > p->m ? p->n_dense : p->m;
       drain_waves_finish_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(*p);
-      return launched_or_fail(2, cuda_err);
+      return launch_result(2);
     }
   }
 }

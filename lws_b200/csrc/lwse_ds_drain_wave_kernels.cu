@@ -19,21 +19,6 @@
 
 namespace lwse {
 
-static int launched_or_fail(int kernels, int* cuda_err) {
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return kernels;
-}
-
-static unsigned grid_for(uint64_t items, uint32_t per_cta, uint32_t cap) {
-  uint64_t grid = (items + per_cta - 1) / per_cta;
-  if (grid < 1) grid = 1;
-  return (unsigned)(grid < cap ? grid : cap);
-}
-
 __global__ void __launch_bounds__(128) ds_drain_waves_caps_kernel(const DsDrainWavesLaunch d) {
   const lwse_ds_tables& t = d.t;
   for (uint32_t ds = blockIdx.x * blockDim.x + threadIdx.x; ds < t.n_ds; ds += gridDim.x * blockDim.x) {
@@ -169,19 +154,17 @@ __global__ void __launch_bounds__(256) ds_drain_waves_finish_kernel(const DsDrai
   }
 }
 
-int launch_ds_drain_waves(const DsDrainWavesLaunch* d, const DrainWavesLaunch* w, int pass, int sm_count, cudaStream_t s,
-                          int* cuda_err) {
-  *cuda_err = 0;
+int launch_ds_drain_waves(const DsDrainWavesLaunch* d, const DrainWavesLaunch* w, int pass, int sm_count, cudaStream_t s) {
   if (pass == 0) {
     if (d->t.n_ds == 0) return 0;
     ds_drain_waves_caps_kernel<<<grid_for(d->t.n_ds, 128, (uint32_t)sm_count * 16u), 128, 0, s>>>(*d);
-    return launched_or_fail(1, cuda_err);
+    return launch_result(1);
   }
   uint32_t n = d->t.n_ds > w->n_dense ? d->t.n_ds : w->n_dense;
   n = n > w->m ? n : w->m;
   n = n > d->max_waves ? n : d->max_waves;
   ds_drain_waves_finish_kernel<<<grid_for(n, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(*d, *w);
-  return launched_or_fail(1, cuda_err);
+  return launch_result(1);
 }
 
 }  // namespace lwse

@@ -672,9 +672,7 @@ __global__ void __launch_bounds__(128) ds_forecast_kernel(const lwse_ds_tables i
 
 // write_pass = false: the summary pass and the scan.  write_pass = true: the write pass into h->steps,
 // which holds the rows the scan counted as written.  Both on stream s.
-int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s,
-                       int* cuda_err) {
-  *cuda_err = 0;
+int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s) {
   if (t->n_ds == 0) return 0;
   const uint32_t want = (t->n_ds + 127u) / 128u;
   const uint32_t cap = (uint32_t)sm_count * 16u;
@@ -692,30 +690,18 @@ int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool wr
                          t->n_ds, h->totals + 2, h->totals + 0, h->totals + 1, s);
     launched = 4;
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return launched;
+  return launch_result(launched);
 }
 
-int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s) {
   if (t->n_ds == 0) return 0;
   const uint32_t want = (t->n_ds + 127u) / 128u;
   const uint32_t cap = (uint32_t)sm_count * 16u;
   ds_sweep_kernel<false><<<want < cap ? want : cap, 128, 0, s>>>(*t, DsTickArgs{});
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
-int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s) {
   if (t->n_ds == 0) return 0;
   const uint32_t want = (t->n_ds + 127u) / 128u;
   const uint32_t cap = (uint32_t)sm_count * 16u;
@@ -726,12 +712,7 @@ int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, c
     ds_sweep_kernel<true, true><<<want < cap ? want : cap, 128, 0, s>>>(*t, a);
   else
     ds_sweep_kernel<true><<<want < cap ? want : cap, 128, 0, s>>>(*t, a);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 // ---- DS drain (lwse_resident_ds_drain*): the definitions are in lwse.h ----
@@ -876,8 +857,7 @@ __global__ void __launch_bounds__(128) ds_drain_links_kernel(const lwse_ds_table
 }
 
 int launch_ds_drain_sweep(const lwse_ds_tables* t, const DsDrainLink* lk, const lwse_lws_out* ready_from, int sm_count,
-                          cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                          cudaStream_t s) {
   if (t->n_ds == 0) return 0;
   DsTickArgs a{};
   a.links = lk->links;
@@ -885,41 +865,24 @@ int launch_ds_drain_sweep(const lwse_ds_tables* t, const DsDrainLink* lk, const 
   a.lws_out = ready_from;
   a.n_lws = lk->n_lws;
   ds_sweep_kernel<false, true><<<ds_grid(t->n_ds, sm_count), 128, 0, s>>>(*t, a);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 int launch_ds_drain_diff(const lwse_ds_tables* t, const DsDrainLink* lk, const DsDrainDiffHost* h, int sm_count,
-                         cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                         cudaStream_t s) {
   if (t->n_ds == 0) return 0;
   ds_drain_diff_kernel<<<ds_grid(t->n_ds, sm_count), 128, 0, s>>>(*t, *lk, *h);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 int launch_ds_drain_links(const lwse_ds_tables* t, const DsDrainLink* lk, uint32_t* count, uint32_t* cursor, uint4* entries,
-                          uint32_t capacity, unsigned long long* total, bool fill, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                          uint32_t capacity, unsigned long long* total, bool fill, int sm_count, cudaStream_t s) {
   if (t->n_ds == 0) return 0;
   if (fill)
     ds_drain_links_kernel<true><<<ds_grid(t->n_ds, sm_count), 128, 0, s>>>(*t, *lk, count, cursor, entries, capacity, total);
   else
     ds_drain_links_kernel<false><<<ds_grid(t->n_ds, sm_count), 128, 0, s>>>(*t, *lk, count, cursor, entries, capacity, total);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 }  // namespace lwse

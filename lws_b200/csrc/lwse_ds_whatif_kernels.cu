@@ -82,33 +82,22 @@ __global__ void __launch_bounds__(256) ds_whatif_gather_kernel(const DsWhatifHos
 }
 
 int launch_ds_whatif_layout(const DsWhatifHost* h, unsigned long long* sums, unsigned long long* total, int sm_count,
-                            cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                            cudaStream_t s) {
   int launched = 0;
   if (h->n) {
     const uint32_t want = (h->n + 255u) / 256u, cap = (uint32_t)sm_count * 8u;
     ds_whatif_count_kernel<<<want < cap ? want : cap, 256, 0, s>>>(*h);
     launched = 1;
   }
-  const cudaError_t e = launch_forecast_scan(DsWhatifLayoutOp{h->count, h->off}, h->n, sums, total, nullptr, s);
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return launched + (h->n ? 3 : 1);
+  launch_forecast_scan(DsWhatifLayoutOp{h->count, h->off}, h->n, sums, total, nullptr, s);
+  return launch_result(launched + (h->n ? 3 : 1));
 }
 
-int launch_ds_whatif_gather(const DsWhatifHost* h, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_ds_whatif_gather(const DsWhatifHost* h, int sm_count, cudaStream_t s) {
   if (h->n == 0) return 0;
   const uint32_t want = (h->n + 7u) / 8u, cap = (uint32_t)sm_count * 8u;
   ds_whatif_gather_kernel<<<want < cap ? want : cap, 256, 0, s>>>(*h);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 }  // namespace lwse

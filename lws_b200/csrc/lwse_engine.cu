@@ -385,19 +385,23 @@ int fail_cuda(lwse_engine* e, cudaError_t err) {
   return err == cudaErrorMemoryAllocation ? LWSE_ERR_OOM : LWSE_ERR_CUDA;
 }
 
-// The result of a launcher (kernels launched, or -1 with its CUDA error): counts the kernels, or fails.
-int count_launch(lwse_engine* e, int launched, int cuda_err) {
-  if (launched >= 0) {
-    e->launches += (uint64_t)launched;
-    return LWSE_OK;
-  }
-  return fail_cuda(e, (cudaError_t)cuda_err);
+// The result of a launcher (the kernels it launched, or its CUDA error negated): counts the kernels, or fails.
+int count_launch(lwse_engine* e, int result) {
+  if (result < 0) return fail_cuda(e, (cudaError_t)-result);
+  e->launches += (uint64_t)result;
+  return LWSE_OK;
 }
 
 #define LWSE_CUDA(e, call)                                \
   do {                                                    \
     cudaError_t err__ = (call);                           \
     if (err__ != cudaSuccess) return fail_cuda(e, err__); \
+  } while (0)
+
+#define LWSE_LAUNCH(e, call)                              \
+  do {                                                    \
+    const int rc__ = count_launch(e, (call));             \
+    if (rc__ != LWSE_OK) return rc__;                     \
   } while (0)
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
@@ -558,11 +562,9 @@ static bool node_patch_moves_index(const lwse_node_rec& old, const lwse_node_rec
 static int build_node_index_locked(lwse_engine* e, cudaStream_t s, bool pdl, bool* built = nullptr) {
   if (built) *built = false;
   if (!e->node_index_stale) return LWSE_OK;
-  int cuda_err = 0;
-  const int launched = lwse::launch_node_index((const lwse_node_rec*)e->nodes.p, e->n_nodes, e->n_domains, (uint32_t*)e->dom_first.p,
-                                               (uint32_t*)e->node_order.p, (uint32_t*)e->node_pos.p, e->node_ix.p, e->sm_count, s,
-                                               pdl, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_node_index((const lwse_node_rec*)e->nodes.p, e->n_nodes, e->n_domains, (uint32_t*)e->dom_first.p,
+                                         (uint32_t*)e->node_order.p, (uint32_t*)e->node_pos.p, e->node_ix.p, e->sm_count, s,
+                                         pdl));
   e->node_index_stale = false;
   if (built) *built = true;
   return LWSE_OK;
@@ -607,10 +609,8 @@ LWSE_API int lwse_upload_nodes(lwse_engine* e, const lwse_node_rec* nodes, uint3
   }
   if (e->r_loaded && n_nodes) {  // the resident pods' occupancy, counted again for the new table
     LWSE_CUDA(e, e->r_occ.reserve((size_t)n_nodes * 4 + 16));
-    int cuda_err = 0;
-    int launched = lwse::launch_occupancy((const lwse_pod_ident*)e->r_pid.p, e->rn_pods, (uint32_t*)e->r_occ.p, n_nodes,
-                                          e->sm_count, e->stream, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_occupancy((const lwse_pod_ident*)e->r_pid.p, e->rn_pods, (uint32_t*)e->r_occ.p, n_nodes,
+                                          e->sm_count, e->stream));
   }
   LWSE_CUDA(e, cudaStreamSynchronize(e->stream));
   e->place_ns_geometry[0] = e->place_ns_geometry[1] = e->place_ns_geometry[2] = e->place_ns_geometry[3] = 0;
@@ -625,10 +625,8 @@ static int sweep_device_locked(lwse_engine* e, const lwse_lws_tables* t, cudaStr
   // the scan bitmaps live in engine-owned scratch; it only grows (a growth is a
   // cudaMalloc, so size it with one warm-up call before capturing a graph)
   LWSE_CUDA(e, e->scan_scratch.reserve(lwse::lws_sweep_scratch_bytes(t->n_pods, t->n_groups)));
-  int cuda_err = 0;
-  int launched = lwse::launch_lws_sweep(t, (const lwse_node_rec*)e->nodes.p, e->n_nodes,
-                                        e->scan_scratch.p, e->sm_count, s, &cuda_err, nullptr);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_lws_sweep(t, (const lwse_node_rec*)e->nodes.p, e->n_nodes,
+                                        e->scan_scratch.p, e->sm_count, s, nullptr));
   return LWSE_OK;
 }
 
@@ -677,7 +675,6 @@ static int sweep_host_locked(lwse_engine* e, const lwse_lws_tables* h, const std
   d.lws_out = (lwse_lws_out*)e->lws_out.p;
   d.group_out = (lwse_group_out*)e->group_out.p;
   d.node_occupancy = want_occ ? (uint32_t*)e->occupancy.p : nullptr;
-  int cuda_err = 0;
   bool counted = false, prefetching = false;
   if (b_pst) {
     // The identity column (16 B / pod, 16 of the 17 input bytes per pod) is only read for pods
@@ -701,9 +698,8 @@ static int sweep_host_locked(lwse_engine* e, const lwse_lws_tables* h, const std
     if (mapped && few && h->n_groups && !(h->flags & (LWSE_SWEEP_SKIP_POD_SCAN | LWSE_SWEEP_SKIP_GROUP_PASS))) {
       LWSE_CUDA(e, cudaEventRecord(e->ev_fork, s));
       LWSE_CUDA(e, cudaStreamWaitEvent(e->side_stream, e->ev_fork, 0));
-      int launched = lwse::launch_ident_prefetch((const uint8_t*)e->pod_state.p, h->n_pods, (const lwse_pod_ident*)mapped,
-                                                 (lwse_pod_ident*)e->pod_ident.p, e->sm_count, e->side_stream, &cuda_err);
-      if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+      LWSE_LAUNCH(e, lwse::launch_ident_prefetch((const uint8_t*)e->pod_state.p, h->n_pods, (const lwse_pod_ident*)mapped,
+                                                 (lwse_pod_ident*)e->pod_ident.p, e->sm_count, e->side_stream));
       LWSE_CUDA(e, cudaEventRecord(e->ev_join, e->side_stream));
       prefetching = true;
       e->ident_rows = ~0ull;  // the device copy holds the event pods' rows only
@@ -721,10 +717,9 @@ static int sweep_host_locked(lwse_engine* e, const lwse_lws_tables* h, const std
     if (arc != LWSE_OK) return arc;
   }
   if (prefetching) LWSE_CUDA(e, cudaStreamWaitEvent(s, e->ev_join, 0));
-  int launched = lwse::launch_lws_sweep(&d, (const lwse_node_rec*)e->nodes.p, e->n_nodes, e->scan_scratch.p, e->sm_count,
-                                        s, &cuda_err, nullptr, counted ? (uint32_t*)e->h_counts_dev.p : nullptr,
-                                        /*first_pdl=*/false);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_lws_sweep(&d, (const lwse_node_rec*)e->nodes.p, e->n_nodes, e->scan_scratch.p, e->sm_count,
+                                        s, nullptr, counted ? (uint32_t*)e->h_counts_dev.p : nullptr,
+                                        /*first_pdl=*/false));
 
   // group results first: they are complete while the LWS pass still runs
   if (b_go) LWSE_CUDA(e, cudaMemcpyAsync(h->group_out, e->group_out.p, b_go, cudaMemcpyDeviceToHost, s));
@@ -810,10 +805,8 @@ LWSE_API int lwse_resident_load(lwse_engine* e, const lwse_lws_tables* h) {
   if (b_lo) LWSE_CUDA(e, cudaMemsetAsync(e->r_lws_out.p, 0xFF, b_lo, s));
   if (b_go) LWSE_CUDA(e, cudaMemsetAsync(e->r_group_out.p, 0xFF, b_go, s));
   if (e->n_nodes) {  // scheduled pods per node; identity-row patches keep it current from here on
-    int cuda_err = 0;
-    int launched = lwse::launch_occupancy((const lwse_pod_ident*)e->r_pid.p, h->n_pods, (uint32_t*)e->r_occ.p, e->n_nodes,
-                                          e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_occupancy((const lwse_pod_ident*)e->r_pid.p, h->n_pods, (uint32_t*)e->r_occ.p, e->n_nodes,
+                                          e->sm_count, s));
   }
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   e->rn_lws = h->n_lws;
@@ -1079,15 +1072,12 @@ static int enqueue_scatter_copies(lwse_engine* e, const ScatterPlan& p, cudaStre
 }
 
 static int launch_scatter_plan(lwse_engine* e, const ScatterPlan& p, cudaStream_t s) {
-  int cuda_err = 0;
   if (p.n) {
-    int launched = lwse::launch_scatter(p.sc, p.n, e->n_nodes ? (uint32_t*)e->r_occ.p : nullptr, e->n_nodes, s, true, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_scatter(p.sc, p.n, e->n_nodes ? (uint32_t*)e->r_occ.p : nullptr, e->n_nodes, s, true));
   }
   if (p.recount && e->n_nodes) {
-    int launched = lwse::launch_occupancy((const lwse_pod_ident*)e->r_pid.p, e->rn_pods, (uint32_t*)e->r_occ.p, e->n_nodes,
-                                          e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_occupancy((const lwse_pod_ident*)e->r_pid.p, e->rn_pods, (uint32_t*)e->r_occ.p, e->n_nodes,
+                                          e->sm_count, s));
   }
   return LWSE_OK;
 }
@@ -1172,14 +1162,12 @@ static int place_grouped_locked(lwse_engine* e, const lwse_place_req* d_reqs, ui
     const int rc = build_node_index_locked(e, s, false, &built);
     if (rc != LWSE_OK) return rc;
   }
-  int cuda_err = 0;
   const uint32_t* counters = nullptr;
-  int launched = lwse::launch_place_ns((const lwse_node_rec*)e->nodes.p, (const uint32_t*)e->dom_first.p,
+  LWSE_LAUNCH(e, lwse::launch_place_ns((const lwse_node_rec*)e->nodes.p, (const uint32_t*)e->dom_first.p,
                                        (const uint32_t*)e->node_order.p, e->n_nodes, e->n_domains, d_reqs, n_reqs,
                                        d_occupancy, n_parts, part_stride_bytes, n_namespaces, d_out, e->place_ns_scratch.p,
-                                       scratch, fresh, e->place_ns_calls++, scan, e->sm_count, s, &cuda_err, &counters,
-                                       (first_pdl || built) && !fresh, changes, xch, index);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+                                       scratch, fresh, e->place_ns_calls++, scan, e->sm_count, s, &counters,
+                                       (first_pdl || built) && !fresh, changes, xch, index));
   e->r_ns_index_ok = index != lwse::kNsIndexNone;  // (a grouped call writes its own ns_first over the index's)
   e->place_rounds_ptr = counters;
   e->place_scans_ptr = counters + 3;
@@ -1229,15 +1217,13 @@ static int place_locked(lwse_engine* e, const lwse_place_req* d_reqs, uint32_t n
     const int rc = build_node_index_locked(e, s, false);
     if (rc != LWSE_OK) return rc;
   }
-  int cuda_err = 0;
-  int launched = lwse::launch_place((const lwse_node_rec*)e->nodes.p, (const uint32_t*)e->dom_first.p,
+  LWSE_LAUNCH(e, lwse::launch_place((const lwse_node_rec*)e->nodes.p, (const uint32_t*)e->dom_first.p,
                                     (const uint32_t*)e->node_order.p, (const uint32_t*)e->node_pos.p, e->n_nodes,
                                     e->n_domains, d_reqs,
                                     n_reqs, d_occupancy, n_namespaces, d_out, e->place_scratch.p,
-                                    scratch, rounds_out ? h_rounds : nullptr, e->sm_count, s, &cuda_err,
+                                    scratch, rounds_out ? h_rounds : nullptr, e->sm_count, s,
                                     e->place_calls++, fresh, n_parts, reqs_per_part, part_stride_bytes,
-                                    h_rounds + 2, &e->place_counters, &e->place_unpinned, after_push);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+                                    h_rounds + 2, &e->place_counters, &e->place_unpinned, after_push));
   e->place_rounds_ptr = e->place_counters + 3;
   e->place_scans_ptr = nullptr;
   if (rounds_out) *rounds_out = h_rounds[0];
@@ -1411,14 +1397,10 @@ LWSE_API int lwse_reconcile_exchanged_device(lwse_engine* e, const lwse_lws_tabl
   LWSE_CUDA(e, cudaEventRecord(e->ev_fork, s));
   LWSE_CUDA(e, cudaStreamWaitEvent(e->side_stream, e->ev_fork, 0));
   const uint64_t step = ++e->xch_step;
-  int cuda_err = 0;
-  int launched = lwse::launch_exchange_push(d_local_part, (uint8_t* const*)e->xch_peers_dev.p, e->xch.p, e->xch_stride,
-                                            e->xch_stride, e->xch_half, e->xch_flags_off, step, step, e->xch_world,
-                                            e->xch_rank, e->side_stream, &cuda_err, false);
-  if (launched < 0) {
-    rc = fail_cuda(e, (cudaError_t)cuda_err);
-  } else {
-    e->launches += (uint64_t)launched;
+  rc = count_launch(e, lwse::launch_exchange_push(d_local_part, (uint8_t* const*)e->xch_peers_dev.p, e->xch.p,
+                                                 e->xch_stride, e->xch_stride, e->xch_half, e->xch_flags_off, step,
+                                                 step, e->xch_world, e->xch_rank, e->side_stream, false));
+  if (rc == LWSE_OK) {
     const uint8_t* half = static_cast<const uint8_t*>(e->xch.p) + (step % 3ull) * e->xch_half;
     rc = place_locked(e, reinterpret_cast<const lwse_place_req*>(half + e->xch_reqs_off),
                       e->xch_world * e->xch_reqs_per_part, reinterpret_cast<const uint32_t*>(half), n_namespaces,
@@ -1448,12 +1430,10 @@ static int shared_occupancy_place_locked(lwse_engine* e, const lwse_place_req* d
   const bool eager = cudaStreamIsCapturing(ps, &capturing) == cudaSuccess && capturing == cudaStreamCaptureStatusNone;
   const uint64_t step = eager ? ++e->xch_step : 0ull;
   const uint64_t read_step = (lagged && step > 1) ? step - 1 : step;
-  int cuda_err = 0;
-  int launched = lwse::launch_exchange_push(d_local_occ, (uint8_t* const*)e->xch_peers_dev.p, e->xch.p,
+  LWSE_LAUNCH(e, lwse::launch_exchange_push(d_local_occ, (uint8_t* const*)e->xch_peers_dev.p, e->xch.p,
                                             e->xch_reqs_off,  // the occupancy block of a part: n_nodes counters, 16-byte padded
                                             e->xch_stride, e->xch_half, e->xch_flags_off, step, read_step, e->xch_world,
-                                            e->xch_rank, ps, &cuda_err, lagged);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+                                            e->xch_rank, ps, lagged));
   if (n_reqs == 0) return LWSE_OK;
   const lwse::PlaceNsExchange xch{reinterpret_cast<const unsigned long long*>(static_cast<const uint8_t*>(e->xch.p) + e->xch_flags_off +
                                                                               (uint64_t)e->xch_world * 8u + 16u),
@@ -1849,10 +1829,8 @@ static int enqueue_sweep(lwse_engine* e, const TickPlan& p, int first_mode) {
   cl.group_out = reinterpret_cast<lwse_group_out*>(b.chg_dev + e->chg_off[3]);
   cl.group_capacity = e->rn_groups;
   cl.counts = b.counts;
-  int cuda_err = 0;
-  const int launched = lwse::launch_lws_sweep(&d, (const lwse_node_rec*)e->nodes.p, e->n_nodes, e->r_scan.p, e->sm_count,
-                                              e->stream, &cuda_err, &cl, nullptr, first_mode);
-  return count_launch(e, launched, cuda_err);
+  return count_launch(e, lwse::launch_lws_sweep(&d, (const lwse_node_rec*)e->nodes.p, e->n_nodes, e->r_scan.p, e->sm_count,
+                                                e->stream, &cl, nullptr, first_mode));
 }
 
 // How the round's first kernels are launched.  Eagerly the first one follows a kernel on the side stream; in a
@@ -1885,10 +1863,8 @@ static int enqueue_place(lwse_engine* e, const TickPlan& p, const PlaceLaunch& h
   }
   if (rc != LWSE_OK) return rc;
   if (!diffed) {
-    int cuda_err = 0;
-    const int launched = lwse::launch_place_diff((const lwse_place_out*)e->r_pout.p, changes.prev, e->rn_reqs, changes.rows,
-                                                 changes.outs, changes.capacity, changes.count, ps, &cuda_err);
-    if (const int drc = count_launch(e, launched, cuda_err); drc != LWSE_OK) return drc;
+    LWSE_LAUNCH(e, lwse::launch_place_diff((const lwse_place_out*)e->r_pout.p, changes.prev, e->rn_reqs, changes.rows,
+                                           changes.outs, changes.capacity, changes.count, ps));
   }
   *res = TickPlaceResult{diffed, e->place_rounds_ptr};
   return LWSE_OK;
@@ -1911,11 +1887,9 @@ static int enqueue_publish(lwse_engine* e, const TickPlan& p, uint32_t seq, cons
   LWSE_CUDA(e, cudaEventRecord(e->ev_done, e->stream));
   LWSE_CUDA(e, cudaStreamWaitEvent(e->pub_stream, e->ev_done, 0));
   const uint32_t* rounds = p.do_place ? placed.rounds_ptr : nullptr;
-  int cuda_err = 0;
-  const int launched = lwse::launch_publish(pl, rounds, b.words, 4, seq, b.counts + 2, e->last_changed[0] + e->last_changed[1],
-                                            e->pub_stream, &cuda_err,
-                                            p.do_place && placed.place_ns ? const_cast<uint32_t*>(rounds) : nullptr, 8u, /*pdl=*/false);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_publish(pl, rounds, b.words, 4, seq, b.counts + 2, e->last_changed[0] + e->last_changed[1],
+                                      e->pub_stream, p.do_place && placed.place_ns ? const_cast<uint32_t*>(rounds) : nullptr, 8u,
+                                      /*pdl=*/false));
   LWSE_CUDA(e, cudaEventRecord(e->ev_pub, e->pub_stream));
   return LWSE_OK;
 }
@@ -1936,9 +1910,8 @@ static int capture_tick_graph(lwse_engine* e, const TickPlan& p, lwse_engine::Ti
   if (ce == cudaSuccess) {
     auto cap = [&](cudaError_t x) { if (crc == LWSE_OK && x != cudaSuccess) { ce = x; crc = LWSE_ERR_CUDA; } };
     if (p.has_patches) {  // the graph's first node: an ordinary launch
-      int err = 0;
-      const int launched = lwse::launch_scatter_desc(d_desc_of(e, p.slot), e->sm_count, s, /*pdl=*/false, &err);
-      if (launched < 0) cap((cudaError_t)err); else e->launches += (uint64_t)launched;
+      const int launched = lwse::launch_scatter_desc(d_desc_of(e, p.slot), e->sm_count, s, /*pdl=*/false);
+      if (launched < 0) cap((cudaError_t)-launched); else e->launches += (uint64_t)launched;
     }
     if (p.do_place) {  // the round forks behind the scatter (it reads the request rows and the occupancy counters)
       cap(cudaEventRecord(e->ev_fork, s));
@@ -2325,11 +2298,9 @@ static int own_node_index(lwse_engine* e, const lwse_node_rec* nodes, cudaStream
   // lwse_upload_nodes clears the resident ones.  The padding of the order rows stays zero.
   LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_ix.p, 0, lwse::node_index_scratch_bytes(e->n_domains), s));
   LWSE_CUDA(e, cudaMemsetAsync(e->wf_node_order.p, 0, ((size_t)(e->n_nodes + 255u) / 256u + 1u) * 1024u, s));
-  int cuda_err = 0;
-  const int launched = lwse::launch_node_index(nodes, e->n_nodes, e->n_domains, (uint32_t*)e->wf_dom_first.p,
-                                               (uint32_t*)e->wf_node_order.p, (uint32_t*)e->wf_node_pos.p, e->wf_node_ix.p,
-                                               e->sm_count, s, false, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_node_index(nodes, e->n_nodes, e->n_domains, (uint32_t*)e->wf_dom_first.p,
+                                         (uint32_t*)e->wf_node_order.p, (uint32_t*)e->wf_node_pos.p, e->wf_node_ix.p,
+                                         e->sm_count, s, false));
   *dom_first = (const uint32_t*)e->wf_dom_first.p;
   *node_order = (const uint32_t*)e->wf_node_order.p;
   if (node_pos) *node_pos = (const uint32_t*)e->wf_node_pos.p;
@@ -2471,10 +2442,8 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
     sc[n_sc++] = lwse::ScatterSegHost{table, is_nodes ? (uint64_t)e->n_nodes : (uint64_t)rn,
                                       reinterpret_cast<const uint32_t*>(st_d + rat), st_d + vat, g.n, rb, false};
   }
-  int cuda_err = 0;
   if (n_sc) {
-    const int launched = lwse::launch_scatter(sc, n_sc, nullptr, 0, s, false, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_scatter(sc, n_sc, nullptr, 0, s, false));
   }
   const uint32_t* dom_first = (const uint32_t*)e->dom_first.p;
   const uint32_t* node_order = (const uint32_t*)e->node_order.p;
@@ -2483,19 +2452,16 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
     if (const int rc = own_node_index(e, d_nodes, s, &dom_first, &node_order, &node_pos); rc != LWSE_OK) return rc;
   if (ns_form) {
     if (round_fresh) LWSE_CUDA(e, cudaMemsetAsync(e->wf_round.p, 0, round_bytes, s));  // (index counts and counters start at zero)
-    int launched = lwse::launch_place_whatif_index(d_reqs, n_total, n_ns, (const uint8_t*)e->wf_touched.p, e->n_nodes, e->n_domains,
-                                                   e->wf_round.p, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-    launched = lwse::launch_place_ns(d_nodes, dom_first, node_order, e->n_nodes, e->n_domains, d_reqs, n_total,
-                                     (const uint32_t*)e->r_occ.p, 1, 0, n_ns, d_out, e->wf_round.p, round_bytes, false,
-                                     e->wf_calls++, false, e->sm_count, s, &cuda_err, nullptr, false, nullptr, nullptr,
-                                     lwse::kNsIndexReuse);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_place_whatif_index(d_reqs, n_total, n_ns, (const uint8_t*)e->wf_touched.p, e->n_nodes, e->n_domains,
+                                                   e->wf_round.p, e->sm_count, s));
+    LWSE_LAUNCH(e, lwse::launch_place_ns(d_nodes, dom_first, node_order, e->n_nodes, e->n_domains, d_reqs, n_total,
+                                         (const uint32_t*)e->r_occ.p, 1, 0, n_ns, d_out, e->wf_round.p, round_bytes, false,
+                                         e->wf_calls++, false, e->sm_count, s, nullptr, false, nullptr, nullptr,
+                                         lwse::kNsIndexReuse));
   } else {
-    const int launched = lwse::launch_place(d_nodes, dom_first, node_order, node_pos, e->n_nodes, e->n_domains, d_reqs, n_total,
-                                            (const uint32_t*)e->r_occ.p, n_ns, d_out, e->wf_round.p, round_bytes, nullptr,
-                                            e->sm_count, s, &cuda_err, 0u, true, 1, n_total, 0, nullptr, nullptr, nullptr, false);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_place(d_nodes, dom_first, node_order, node_pos, e->n_nodes, e->n_domains, d_reqs, n_total,
+                                      (const uint32_t*)e->r_occ.p, n_ns, d_out, e->wf_round.p, round_bytes, nullptr,
+                                      e->sm_count, s, 0u, true, 1, n_total, 0, nullptr, nullptr, nullptr, false));
   }
   // the diff against the baseline, the counts
   // (layout: [counts: 16 words] [rows: list_cap] [before: list_cap] [after: list_cap], the 16-byte rows aligned)
@@ -2506,9 +2472,8 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
   lwse_place_out* d_after = d_before + list_cap;
   LWSE_CUDA(e, cudaMemsetAsync(d_counts, 0, 64, s));
   {
-    const int launched = lwse::launch_place_whatif_diff((const lwse_place_out*)e->r_pout.p, d_out, rn, n_total, d_rows, d_before,
-                                                        d_after, list_cap, d_counts, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_place_whatif_diff((const lwse_place_out*)e->r_pout.p, d_out, rn, n_total, d_rows, d_before,
+                                                  d_after, list_cap, d_counts, e->sm_count, s));
   }
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
@@ -2610,10 +2575,8 @@ static int enqueue_drain_sweep(lwse_engine* e, uint32_t* d_counts, uint32_t* d_r
   cudaStream_t s = e->wf_stream;
   if (np) LWSE_CUDA(e, cudaMemcpyAsync(e->dr_state.p, e->r_pst.p, (size_t)np, cudaMemcpyDeviceToDevice, s));
   if (ng) LWSE_CUDA(e, cudaMemcpyAsync(e->dr_groups.p, e->r_groups.p, (size_t)ng * sizeof(lwse_group_rec), cudaMemcpyDeviceToDevice, s));
-  int cuda_err = 0;
-  int launched = lwse::launch_drain_mark((const uint8_t*)e->dr_mask.p, nn, (const lwse_pod_ident*)e->r_pid.p, (uint8_t*)e->dr_state.p,
-                                         np, (lwse_group_rec*)e->dr_groups.p, ng, d_counts, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_mark((const uint8_t*)e->dr_mask.p, nn, (const lwse_pod_ident*)e->r_pid.p, (uint8_t*)e->dr_state.p,
+                                         np, (lwse_group_rec*)e->dr_groups.p, ng, d_counts, e->sm_count, s));
   lwse_lws_tables d{};
   d.lws = (const lwse_lws_rec*)e->r_lws.p;
   d.n_lws = e->rn_lws;
@@ -2624,13 +2587,11 @@ static int enqueue_drain_sweep(lwse_engine* e, uint32_t* d_counts, uint32_t* d_r
   d.n_pods = np;
   d.group_out = (lwse_group_out*)e->dr_out.p;
   d.flags = e->r_sweep_flags | LWSE_SWEEP_SKIP_LWS_PASS;
-  launched = lwse::launch_lws_sweep(&d, (const lwse_node_rec*)e->nodes.p, nn, e->dr_scan.p, e->sm_count, s, &cuda_err, nullptr,
-                                    nullptr, /*first_mode=*/0);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  launched = lwse::launch_drain_diff((const lwse_group_out*)e->r_group_out.p, (const lwse_group_out*)e->dr_out.p,
-                                     (const lwse_group_rec*)e->r_groups.p, ng, d_rows, d_before, d_after, list_cap, d_counts,
-                                     e->sm_count, s, &cuda_err);
-  return count_launch(e, launched, cuda_err);
+  LWSE_LAUNCH(e, lwse::launch_lws_sweep(&d, (const lwse_node_rec*)e->nodes.p, nn, e->dr_scan.p, e->sm_count, s, nullptr,
+                                        nullptr, /*first_mode=*/0));
+  return count_launch(e, lwse::launch_drain_diff((const lwse_group_out*)e->r_group_out.p, (const lwse_group_out*)e->dr_out.p,
+                                                 (const lwse_group_rec*)e->r_groups.p, ng, d_rows, d_before, d_after, list_cap, d_counts,
+                                                 e->sm_count, s));
 }
 
 LWSE_API int lwse_resident_drain_whatif(lwse_engine* e, lwse_drain_whatif* q) {
@@ -2697,12 +2658,9 @@ LWSE_API int lwse_resident_drain_cost(lwse_engine* e, lwse_drain_cost* out) {
   lwse_drain_cost* d_cost = (lwse_drain_cost*)e->dr_cost.p;
   LWSE_CUDA(e, cudaMemsetAsync(d_cost, 0, (size_t)nn * sizeof(lwse_drain_cost), s));
   LWSE_CUDA(e, cudaMemcpy2DAsync(d_cost, sizeof(lwse_drain_cost), e->r_occ.p, 4, 4, nn, cudaMemcpyDeviceToDevice, s));
-  int cuda_err = 0;
-  const int launched = lwse::launch_drain_cost((const lwse_lws_rec*)e->r_lws.p, e->rn_lws, (const lwse_group_rec*)e->r_groups.p,
-                                               e->rn_groups, (const uint8_t*)e->r_pst.p, (const lwse_pod_ident*)e->r_pid.p,
-                                               e->rn_pods, (const lwse_group_out*)e->r_group_out.p, d_cost, nn, e->sm_count, s,
-                                               &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_cost((const lwse_lws_rec*)e->r_lws.p, e->rn_lws, (const lwse_group_rec*)e->r_groups.p,
+                                         e->rn_groups, (const uint8_t*)e->r_pst.p, (const lwse_pod_ident*)e->r_pid.p,
+                                         e->rn_pods, (const lwse_group_out*)e->r_group_out.p, d_cost, nn, e->sm_count, s));
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(out, d_cost, (size_t)nn * sizeof(lwse_drain_cost), cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
@@ -2726,10 +2684,8 @@ static int enqueue_drain_set(lwse_engine* e, const uint8_t* mask, bool by_domain
     return LWSE_OK;
   }
   if (nd) LWSE_CUDA(e, cudaMemcpyAsync(e->dr_domains.p, mask, nd, cudaMemcpyHostToDevice, s));
-  int cuda_err = 0;
-  const int launched = lwse::launch_drain_domain_mask((const uint8_t*)e->dr_domains.p, nd, (const lwse_node_rec*)e->nodes.p, nn,
-                                                      (uint8_t*)e->dr_mask.p, e->sm_count, s, &cuda_err);
-  return count_launch(e, launched, cuda_err);
+  return count_launch(e, lwse::launch_drain_domain_mask((const uint8_t*)e->dr_domains.p, nd, (const lwse_node_rec*)e->nodes.p, nn,
+                                                        (uint8_t*)e->dr_mask.p, e->sm_count, s));
 }
 
 // The set form: the drain what-if's sweep over the node mask (the given node rows, or the nodes of the given
@@ -2763,12 +2719,10 @@ LWSE_API int lwse_resident_drain_budget(lwse_engine* e, lwse_drain_budget_query*
   if (const int rc = enqueue_drain_set(e, mask, by_domain); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemsetAsync(d_counts, 0, 64, s));
   if (const int rc = enqueue_drain_sweep(e, d_counts, nullptr, nullptr, nullptr, 0); rc != LWSE_OK) return rc;
-  int cuda_err = 0;
-  const int launched = lwse::launch_drain_budget((const lwse_lws_rec*)e->r_lws.p, (const lwse_lws_out*)e->r_lws_out.p, nl,
-                                                 (const lwse_group_rec*)e->r_groups.p, (const lwse_group_out*)e->r_group_out.p,
-                                                 (const lwse_group_out*)e->dr_out.p, e->rn_groups, d_rows, list_cap, d_counts,
-                                                 e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_budget((const lwse_lws_rec*)e->r_lws.p, (const lwse_lws_out*)e->r_lws_out.p, nl,
+                                           (const lwse_group_rec*)e->r_groups.p, (const lwse_group_out*)e->r_group_out.p,
+                                           (const lwse_group_out*)e->dr_out.p, e->rn_groups, d_rows, list_cap, d_counts,
+                                           e->sm_count, s));
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_counts, 64, cudaMemcpyDeviceToHost, s));
@@ -2813,9 +2767,7 @@ LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lws
   lwse::DrainBudgetCostLaunch p = restart_walk(e, by_domain, (lwse_drain_budget_cost*)e->dr_bcost.p, (uint32_t*)e->dr_bwords.p);
   LWSE_CUDA(e, cudaMemsetAsync(p.cost, 0, cost_bytes, s));
   LWSE_CUDA(e, cudaMemsetAsync(p.counts, 0, 64, s));
-  int cuda_err = 0;
-  int launched = lwse::launch_drain_budget_cost(&p, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_budget_cost(&p, 0, e->sm_count, s));
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
   LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 16, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
@@ -2830,8 +2782,7 @@ LWSE_API int lwse_resident_drain_budget_cost(lwse_engine* e, uint32_t scope, lws
     p.table_mask = (uint32_t)(slots - 1);
     LWSE_CUDA(e, cudaMemsetAsync(p.keys, 0xFF, (size_t)slots * sizeof(unsigned long long), s));
     LWSE_CUDA(e, cudaMemsetAsync(p.vals, 0, (size_t)slots * sizeof(uint4), s));
-    launched = lwse::launch_drain_budget_cost(&p, 1, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_drain_budget_cost(&p, 1, e->sm_count, s));
   }
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   if (n_keys) LWSE_CUDA(e, cudaMemcpyAsync(out, p.cost, cost_bytes, cudaMemcpyDeviceToHost, s));
@@ -2904,9 +2855,7 @@ static int enqueue_drain_waves_setup(lwse_engine* e, const lwse::DrainBudgetCost
   LWSE_CUDA(e, cudaMemsetAsync(e->dv_lidx.p, 0, (size_t)nl * 4 + 4, s));
   LWSE_CUDA(e, cudaMemsetAsync(e->dv_gwaves.p, 0, (size_t)ng * 8, s));
   LWSE_CUDA(e, cudaMemsetAsync(e->dv_out.p, 0, waves_answer_bytes<lwse_drain_wave_key, lwse_drain_wave>(m, max_waves), s));
-  int cuda_err = 0;
-  int launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s));
   p->lws = bp.lws;
   p->lws_out = bp.lws_out;
   p->groups = bp.groups;
@@ -2930,8 +2879,7 @@ static int enqueue_drain_waves_setup(lwse_engine* e, const lwse::DrainBudgetCost
   p->m = m;
   p->max_waves = max_waves;
   p->cols = (m < max_waves ? m : max_waves) + 1u;
-  launched = lwse::launch_drain_waves(p, 0, e->sm_count, s, &cuda_err);
-  return count_launch(e, launched, cuda_err);
+  return count_launch(e, lwse::launch_drain_waves(p, 0, e->sm_count, s));
 }
 
 // The buffers for n_pairs restart pairs, directly after the synchronisation that read the count.
@@ -2946,10 +2894,8 @@ static int reserve_drain_waves_pairs(lwse_engine* e, uint64_t n_pairs) {
 // The walk in pair mode into dv_pairs, and p's pairs set for its pass 1.
 static int enqueue_drain_waves_pairs(lwse_engine* e, const lwse::DrainBudgetCostLaunch& bp, uint32_t n_pairs,
                                      lwse::DrainWavesLaunch* p) {
-  int cuda_err = 0;
-  const int launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dv_pairs.p, n_pairs, e->sm_count,
-                                                        e->wf_stream, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dv_pairs.p, n_pairs, e->sm_count,
+                                                  e->wf_stream));
   p->pairs = (const unsigned long long*)e->dv_pairs.p;
   p->n_pairs = n_pairs;
   p->recs = (uint4*)e->dv_recs.p;
@@ -3010,9 +2956,7 @@ LWSE_API int lwse_resident_drain_waves(lwse_engine* e, lwse_drain_waves_query* q
   memcpy(&n_pairs, words, 8);
   if (const int rc = reserve_drain_waves_pairs(e, n_pairs); rc != LWSE_OK) return rc;
   if (const int rc = enqueue_drain_waves_pairs(e, bp, (uint32_t)n_pairs, &p); rc != LWSE_OK) return rc;
-  int cuda_err = 0;
-  int launched = lwse::launch_drain_waves(&p, 1, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_waves(&p, 1, e->sm_count, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 64, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words + 16, d_words + 16, 16, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words + 20, p.l_first + nl, 4, cudaMemcpyDeviceToHost, s));
@@ -3021,8 +2965,7 @@ LWSE_API int lwse_resident_drain_waves(lwse_engine* e, lwse_drain_waves_query* q
   if (ng && words[8] != n_pairs) return LWSE_ERR_OOM;
   if (words[18] || words[19]) return LWSE_ERR_OOM;
   if (const int rc = enqueue_drain_waves_dense(e, words[20], &p); rc != LWSE_OK) return rc;
-  launched = lwse::launch_drain_waves(&p, 2, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_waves(&p, 2, e->sm_count, s));
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(e->dv_host.h, p.out, out_bytes, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
@@ -3081,13 +3024,10 @@ static int enqueue_drain_place_setup(lwse_engine* e, const lwse::DrainBudgetCost
   if (e->node_index_stale)
     if (const int rc = own_node_index(e, (const lwse_node_rec*)e->nodes.p, s, &dom_first, &node_order, nullptr); rc != LWSE_OK)
       return rc;
-  int cuda_err = 0;
-  int launched = lwse::launch_place_whatif_index((const lwse_place_req*)e->r_preq.p, nr, n_ns, (const uint8_t*)e->dp_touched.p,
-                                                 nn, nd, e->dp_round.p, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_place_whatif_index((const lwse_place_req*)e->r_preq.p, nr, n_ns, (const uint8_t*)e->dp_touched.p,
+                                                 nn, nd, e->dp_round.p, e->sm_count, s));
   // the restarted groups per key: the drain budget's pass 0 (key rows, the walk)
-  launched = lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_budget_cost(&bp, 0, e->sm_count, s));
   p->nodes = (const lwse_node_rec*)e->nodes.p;
   p->occupancy = (const uint32_t*)e->r_occ.p;
   p->dom_first = dom_first;
@@ -3115,22 +3055,17 @@ static int enqueue_drain_place_setup(lwse_engine* e, const lwse::DrainBudgetCost
   p->counts = (uint32_t*)e->dp_words.p;
   p->round = e->dp_round.p;
   p->round_bytes = round_bytes;
-  launched = lwse::launch_drain_place(p, 0, e->sm_count, s, &cuda_err);
-  return count_launch(e, launched, cuda_err);
+  return count_launch(e, lwse::launch_drain_place(p, 0, e->sm_count, s));
 }
 
 // The walk in pair mode into dp_pairs (reserved by the caller after the count's synchronisation), then the chain's
 // pass 1: U_k counted and scanned.
 static int enqueue_drain_place_pairs(lwse_engine* e, const lwse::DrainBudgetCostLaunch& bp, uint32_t n_pairs,
                                      lwse::DrainPlaceLaunch* p) {
-  int cuda_err = 0;
-  int launched = lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dp_pairs.p, n_pairs, e->sm_count, e->wf_stream,
-                                                  &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_restart_pairs(&bp, (unsigned long long*)e->dp_pairs.p, n_pairs, e->sm_count, e->wf_stream));
   p->pairs = (const unsigned long long*)e->dp_pairs.p;
   p->n_pairs = n_pairs;
-  launched = lwse::launch_drain_place(p, 1, e->sm_count, e->wf_stream, &cuda_err);
-  return count_launch(e, launched, cuda_err);
+  return count_launch(e, lwse::launch_drain_place(p, 1, e->sm_count, e->wf_stream));
 }
 
 // The chain's pass 2 for n_unp unpinned rows and n_rule_b rule-(b) candidates, after the synchronisation that read
@@ -3162,9 +3097,7 @@ static int enqueue_drain_place_solve(lwse_engine* e, uint32_t max_ns, uint32_t n
   p->s_marks = static_cast<uint8_t*>(e->dp_slices.p) + slice_out + slice_unp;
   p->slice_rows = max_ns;
   p->grid = (uint32_t)grid;
-  int cuda_err = 0;
-  const int launched = lwse::launch_drain_place(p, 2, e->sm_count, e->wf_stream, &cuda_err);
-  return count_launch(e, launched, cuda_err);
+  return count_launch(e, lwse::launch_drain_place(p, 2, e->sm_count, e->wf_stream));
 }
 
 // Three host synchronisations, each sizing what follows: the restart pairs (the drain budget's pass 0 counts
@@ -3257,7 +3190,6 @@ LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_wa
   if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
   cudaStream_t s = e->wf_stream;
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
-  int cuda_err = 0;
   // ---- the drain waves chain up to its pass 0 (lwse_resident_drain_waves) ----
   uint32_t* v_words = (uint32_t*)e->dv_words.p;
   LWSE_CUDA(e, cudaMemsetAsync(v_words, 0, 128, s));
@@ -3282,8 +3214,7 @@ LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_wa
   if (const int rc = reserve_drain_waves_pairs(e, n_pairs); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, e->dp_pairs.reserve((size_t)all_pairs * 8 + 16));
   if (const int rc = enqueue_drain_waves_pairs(e, bp, (uint32_t)n_pairs, &w); rc != LWSE_OK) return rc;
-  int launched = lwse::launch_drain_waves(&w, 1, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_waves(&w, 1, e->sm_count, s));
   if (const int rc = enqueue_drain_place_pairs(e, pb, all_pairs, &p); rc != LWSE_OK) return rc;
   // second synchronisation: the touched rows, |U| and the rule-(b) count
   LWSE_CUDA(e, cudaMemcpyAsync(words, v_words, 64, cudaMemcpyDeviceToHost, s));
@@ -3330,17 +3261,16 @@ LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_wa
   d.dix_cursor = d.dix_first + nd + 1;
   d.dix_rows = d.dix_cursor + nd;
   d.out = (uint8_t*)e->dq_out.p;
-  launched = lwse::launch_drain_place_waves(&d, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_place_waves(&d, 0, e->sm_count, s));
   if (m) {
     cudaGraph_t graph = nullptr;
     GraphExec exec;
     LWSE_CUDA(e, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    launched = lwse::launch_drain_place_waves(&d, 1, e->sm_count, s, &cuda_err);
+    const int launched = lwse::launch_drain_place_waves(&d, 1, e->sm_count, s);
     const cudaError_t ce = cudaStreamEndCapture(s, &graph);
     if (launched < 0 || ce != cudaSuccess) {
       if (graph) cudaGraphDestroy(graph);
-      return fail_cuda(e, launched < 0 ? (cudaError_t)cuda_err : ce);
+      return fail_cuda(e, launched < 0 ? (cudaError_t)-launched : ce);
     }
     cudaError_t ge = exec.ensure(graph);
     cudaGraphDestroy(graph);
@@ -3348,8 +3278,7 @@ LWSE_API int lwse_resident_drain_place_waves(lwse_engine* e, lwse_drain_place_wa
     if (ge != cudaSuccess) return fail_cuda(e, ge);
     e->launches += (uint64_t)launched * m;
   }
-  launched = lwse::launch_drain_place_waves(&d, 2, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_place_waves(&d, 2, e->sm_count, s));
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(e->dv_host.h, d.out, out_bytes, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words, p_words, 64, cudaMemcpyDeviceToHost, s));
@@ -3413,9 +3342,7 @@ static int enqueue_ds_drain_sweep(lwse_engine* e, int k, const lwse_lws_out* rea
   LWSE_CUDA(e, cudaMemsetAsync(t.role_out, 0, (size_t)t.n_roles * sizeof(lwse_ds_role_out) + 16, s));
   LWSE_CUDA(e, cudaMemsetAsync(t.revrole_out, 0, (size_t)t.n_revroles * sizeof(lwse_ds_revrole_out) + 16, s));
   const lwse::DsDrainLink lk = ds_drain_link(e);
-  int cuda_err = 0;
-  const int launched = lwse::launch_ds_drain_sweep(&t, &lk, ready_from, e->sm_count, s, &cuda_err);
-  return count_launch(e, launched, cuda_err);
+  return count_launch(e, lwse::launch_ds_drain_sweep(&t, &lk, ready_from, e->sm_count, s));
 }
 
 // The set form: the drain budget's mark → sweep (what-if group rows), lost[L] and the after copy of lws_out,
@@ -3451,12 +3378,10 @@ LWSE_API int lwse_resident_ds_drain(lwse_engine* e, lwse_ds_drain_query* q) {
   if (const int rc = enqueue_drain_set(e, mask, by_domain); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemsetAsync(d_counts, 0, 128, s));
   if (const int rc = enqueue_drain_sweep(e, d_counts, nullptr, nullptr, nullptr, 0); rc != LWSE_OK) return rc;
-  int cuda_err = 0;
-  int launched = lwse::launch_ds_drain_lost((const lwse_lws_rec*)e->r_lws.p, (const lwse_lws_out*)e->r_lws_out.p, nl,
+  LWSE_LAUNCH(e, lwse::launch_ds_drain_lost((const lwse_lws_rec*)e->r_lws.p, (const lwse_lws_out*)e->r_lws_out.p, nl,
                                             (const lwse_group_rec*)e->r_groups.p, (const lwse_group_out*)e->r_group_out.p,
                                             (const lwse_group_out*)e->dr_out.p, e->rn_groups, (uint32_t*)e->dd_lost.p,
-                                            (lwse_lws_out*)e->dd_lws_after.p, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+                                            (lwse_lws_out*)e->dd_lws_after.p, e->sm_count, s));
   if (const int rc = enqueue_ds_drain_sweep(e, 0, (const lwse_lws_out*)e->r_lws_out.p); rc != LWSE_OK) return rc;
   if (const int rc = enqueue_ds_drain_sweep(e, 1, (const lwse_lws_out*)e->dd_lws_after.p); rc != LWSE_OK) return rc;
   const lwse_ds_tables after = ds_drain_tables(e, 1);
@@ -3464,8 +3389,7 @@ LWSE_API int lwse_resident_ds_drain(lwse_engine* e, lwse_ds_drain_query* q) {
   const lwse::DsDrainDiffHost h{(const lwse_ds_out*)e->dd_out[0].p, (const lwse_ds_role_out*)e->dd_role_out[0].p,
                                 (const lwse_ds_revrole_out*)e->dd_revrole_out[0].p, (const uint32_t*)e->dd_lost.p,
                                 (lwse_ds_drain*)e->dd_rows.p, list_cap, d_counts};
-  launched = lwse::launch_ds_drain_diff(&after, &lk, &h, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_ds_drain_diff(&after, &lk, &h, e->sm_count, s));
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_counts, 128, cudaMemcpyDeviceToHost, s));
@@ -3513,7 +3437,6 @@ LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds
   LWSE_CUDA(e, e->dd_index.reserve((size_t)(nl + 1) * 3 * 4 + 16));
   if (const int rc = ds_drain_begin_locked(e); rc != LWSE_OK) return rc;
   cudaStream_t s = e->wf_stream;
-  int cuda_err = 0;
   // the before sweep (its ds_out gates the verdicts) and the reverse link index
   if (const int rc = enqueue_ds_drain_sweep(e, 0, (const lwse_lws_out*)e->r_lws_out.p); rc != LWSE_OK) return rc;
   const lwse_ds_tables t = ds_drain_tables(e, 0);
@@ -3525,11 +3448,9 @@ LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds
                                                   // [10] refused; [12..13] reverse-index entries (all u64 but [2], [10])
   LWSE_CUDA(e, cudaMemsetAsync(d_words, 0, 64, s));
   LWSE_CUDA(e, cudaMemsetAsync(d_count, 0, (size_t)(nl + 1) * 4, s));
-  int launched = lwse::launch_ds_drain_links(&t, &lk, d_count, d_cursor, nullptr, 0, (unsigned long long*)(d_words + 12),
-                                             false, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  launched = lwse::launch_index_scan(d_count, d_first, d_cursor, nl, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_ds_drain_links(&t, &lk, d_count, d_cursor, nullptr, 0, (unsigned long long*)(d_words + 12),
+                                             false, e->sm_count, s));
+  LWSE_LAUNCH(e, lwse::launch_index_scan(d_count, d_first, d_cursor, nl, s));
   // the drain budget's (LWS, key) table: vals.y = lost(L, key)
   lwse::DrainBudgetCostLaunch p = restart_walk(e, by_domain, (lwse_drain_budget_cost*)e->dr_bcost.p, d_words);
   lwse::DsDrainCostLaunch c{};
@@ -3539,8 +3460,7 @@ LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds
   c.counts = p.counts + 8;
   LWSE_CUDA(e, cudaMemsetAsync(p.cost, 0, (size_t)n_keys * sizeof(lwse_drain_budget_cost), s));
   LWSE_CUDA(e, cudaMemsetAsync(c.cost, 0, cost_bytes, s));
-  launched = lwse::launch_drain_budget_cost(&p, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_budget_cost(&p, 0, e->sm_count, s));
   uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
   LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 64, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
@@ -3554,9 +3474,8 @@ LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds
   if (pairs > (1ull << 30)) return LWSE_ERR_OOM;      // (the table index is 32-bit)
   LWSE_CUDA(e, e->dd_entries.reserve((size_t)n_entries * sizeof(uint4) + 16));
   c.entries = (const uint4*)e->dd_entries.p;
-  launched = lwse::launch_ds_drain_links(&t, &lk, d_count, d_cursor, (uint4*)e->dd_entries.p, (uint32_t)n_entries, nullptr,
-                                         true, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_ds_drain_links(&t, &lk, d_count, d_cursor, (uint4*)e->dd_entries.p, (uint32_t)n_entries, nullptr,
+                                             true, e->sm_count, s));
   if (pairs) {
     const uint64_t slots = table_slots(pairs);
     LWSE_CUDA(e, e->dr_table.reserve((size_t)slots * (sizeof(unsigned long long) + sizeof(uint4))));
@@ -3565,13 +3484,11 @@ LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds
     p.table_mask = (uint32_t)(slots - 1);
     LWSE_CUDA(e, cudaMemsetAsync(p.keys, 0xFF, (size_t)slots * sizeof(unsigned long long), s));
     LWSE_CUDA(e, cudaMemsetAsync(p.vals, 0, (size_t)slots * sizeof(uint4), s));
-    launched = lwse::launch_drain_budget_cost(&p, 2, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_drain_budget_cost(&p, 2, e->sm_count, s));
     c.lws_keys = p.keys;
     c.lws_vals = p.vals;
     c.lws_mask = p.table_mask;
-    launched = lwse::launch_ds_drain_cost(&c, 0, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_ds_drain_cost(&c, 0, e->sm_count, s));
     LWSE_CUDA(e, cudaMemcpyAsync(words, p.counts, 64, cudaMemcpyDeviceToHost, s));
     LWSE_CUDA(e, cudaStreamSynchronize(s));
     if (words[2]) return LWSE_ERR_OOM;  // an insert the (LWS, key) table refused
@@ -3587,8 +3504,7 @@ LWSE_API int lwse_resident_ds_drain_cost(lwse_engine* e, uint32_t scope, lwse_ds
       c.table_mask = (uint32_t)(ds_slots - 1);
       LWSE_CUDA(e, cudaMemsetAsync(c.keys, 0xFF, (size_t)ds_slots * sizeof(unsigned long long), s));
       LWSE_CUDA(e, cudaMemsetAsync(c.vals, 0, (size_t)ds_slots * sizeof(uint2), s));
-      launched = lwse::launch_ds_drain_cost(&c, 1, e->sm_count, s, &cuda_err);
-      if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+      LWSE_LAUNCH(e, lwse::launch_ds_drain_cost(&c, 1, e->sm_count, s));
     }
   }
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
@@ -3654,14 +3570,10 @@ LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_qu
   d.ds_cost = (const lwse_ds_drain_cost*)e->dd_cost.p;
   d.out = (uint8_t*)e->dx_out.p;
   d.max_waves = mw;
-  int cuda_err = 0;
-  int launched = lwse::launch_ds_drain_links(&d.t, &d.lk, d_count, d_cursor, nullptr, 0, (unsigned long long*)(d_words + 24),
-                                             false, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  launched = lwse::launch_index_scan(d_count, d_first, d_cursor, nl, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  launched = lwse::launch_ds_drain_waves(&d, nullptr, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_ds_drain_links(&d.t, &d.lk, d_count, d_cursor, nullptr, 0, (unsigned long long*)(d_words + 24),
+                                             false, e->sm_count, s));
+  LWSE_LAUNCH(e, lwse::launch_index_scan(d_count, d_first, d_cursor, nl, s));
+  LWSE_LAUNCH(e, lwse::launch_ds_drain_waves(&d, nullptr, 0, e->sm_count, s));
   // the key rows, the member-pair count and the pair count: the drain budget's pass 0, then the key positions
   lwse::DrainBudgetCostLaunch bp = restart_walk(e, by_domain, (lwse_drain_budget_cost*)e->dr_bcost.p, d_words);
   lwse::DrainWavesLaunch p{};
@@ -3678,12 +3590,10 @@ LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_qu
   LWSE_CUDA(e, e->dd_entries.reserve((size_t)n_entries * sizeof(uint4) + 16));
   const uint64_t slots = table_slots(member_pairs);
   if (member_pairs) LWSE_CUDA(e, e->dr_table.reserve((size_t)slots * (sizeof(unsigned long long) + sizeof(uint4))));
-  launched = lwse::launch_ds_drain_links(&d.t, &d.lk, d_count, d_cursor, (uint4*)e->dd_entries.p, (uint32_t)n_entries, nullptr,
-                                         true, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_ds_drain_links(&d.t, &d.lk, d_count, d_cursor, (uint4*)e->dd_entries.p, (uint32_t)n_entries, nullptr,
+                                             true, e->sm_count, s));
   if (const int rc = enqueue_drain_waves_pairs(e, bp, (uint32_t)n_pairs, &p); rc != LWSE_OK) return rc;
-  launched = lwse::launch_drain_waves_capped(&p, d.caps, q->constraints, 1, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_waves_capped(&p, d.caps, q->constraints, 1, e->sm_count, s));
   // the per-key forms: the (LWS, key) table with the budget columns, then the (row, key) pair count
   lwse::DsDrainCostLaunch c{};
   c.first = d_first;
@@ -3697,13 +3607,11 @@ LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_qu
     bp.table_mask = (uint32_t)(slots - 1);
     LWSE_CUDA(e, cudaMemsetAsync(bp.keys, 0xFF, (size_t)slots * sizeof(unsigned long long), s));
     LWSE_CUDA(e, cudaMemsetAsync(bp.vals, 0, (size_t)slots * sizeof(uint4), s));
-    launched = lwse::launch_drain_budget_cost(&bp, 1, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_drain_budget_cost(&bp, 1, e->sm_count, s));
     c.lws_keys = bp.keys;
     c.lws_vals = bp.vals;
     c.lws_mask = bp.table_mask;
-    launched = lwse::launch_ds_drain_cost(&c, 0, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_ds_drain_cost(&c, 0, e->sm_count, s));
   }
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 128, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words + 32, p.l_first + nl, 4, cudaMemcpyDeviceToHost, s));
@@ -3724,14 +3632,11 @@ LWSE_API int lwse_resident_ds_drain_waves(lwse_engine* e, lwse_ds_drain_waves_qu
     c.table_mask = (uint32_t)(ds_slots - 1);
     LWSE_CUDA(e, cudaMemsetAsync(c.keys, 0xFF, (size_t)ds_slots * sizeof(unsigned long long), s));
     LWSE_CUDA(e, cudaMemsetAsync(c.vals, 0, (size_t)ds_slots * sizeof(uint2), s));
-    launched = lwse::launch_ds_drain_cost(&c, 1, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_ds_drain_cost(&c, 1, e->sm_count, s));
   }
   if (const int rc = enqueue_drain_waves_dense(e, n_dense, &p); rc != LWSE_OK) return rc;
-  launched = lwse::launch_drain_waves_capped(&p, d.caps, q->constraints, 2, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
-  launched = lwse::launch_ds_drain_waves(&d, &p, 1, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_drain_waves_capped(&p, d.caps, q->constraints, 2, e->sm_count, s));
+  LWSE_LAUNCH(e, lwse::launch_ds_drain_waves(&d, &p, 1, e->sm_count, s));
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(e->dv_host.h, d.out, out_bytes, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words + 20, 12, cudaMemcpyDeviceToHost, s));
@@ -3760,9 +3665,7 @@ LWSE_API int lwse_sweep_ds_device(lwse_engine* e, const lwse_ds_tables* t, void*
   std::lock_guard<std::mutex> lock(e->mu);
   DeviceGuard guard(e->device);
   cudaStream_t s = stream ? (cudaStream_t)stream : e->stream;
-  int cuda_err = 0;
-  int launched = lwse::launch_ds_sweep(t, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_ds_sweep(t, e->sm_count, s));
   return LWSE_OK;
 }
 
@@ -3793,9 +3696,7 @@ LWSE_API int lwse_sweep_ds_host(lwse_engine* e, const lwse_ds_tables* h) {
   d.ds_out = (lwse_ds_out*)e->ds_out.p;
   d.role_out = (lwse_ds_role_out*)e->ds_role_out.p;
   d.revrole_out = (lwse_ds_revrole_out*)e->ds_revrole_out.p;
-  int cuda_err = 0;
-  int launched = lwse::launch_ds_sweep(&d, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_ds_sweep(&d, e->sm_count, s));
   if (o_ds) LWSE_CUDA(e, cudaMemcpyAsync(h->ds_out, e->ds_out.p, o_ds, cudaMemcpyDeviceToHost, s));
   if (o_ro) LWSE_CUDA(e, cudaMemcpyAsync(h->role_out, e->ds_role_out.p, o_ro, cudaMemcpyDeviceToHost, s));
   if (o_rr) LWSE_CUDA(e, cudaMemcpyAsync(h->revrole_out, e->ds_revrole_out.p, o_rr, cudaMemcpyDeviceToHost, s));
@@ -3936,15 +3837,13 @@ LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, u
     sc[n_sc++] = lwse::ScatterSegHost{base, rows, d_rows, d_vals, g.n, rb, false};
     if (is_ds) sc[n_sc++] = lwse::ScatterSegHost{e->rd_marks.p, rows, d_rows, e->rd_ones.p, g.n, 1u, false};
   }
-  int cuda_err = 0;
   if (cursor) LWSE_CUDA(e, cudaMemcpyAsync(ds_dev, hs, cursor, cudaMemcpyHostToDevice, s));
   for (int k = 0; k < n_rc; k++) {
     LWSE_CUDA(e, cudaMemcpyAsync(rc[k].dst, rc[k].src, rc[k].bytes, cudaMemcpyDeviceToDevice, s));
     if (rc[k].ds_n) LWSE_CUDA(e, cudaMemsetAsync(static_cast<uint8_t*>(e->rd_marks.p) + rc[k].ds_first, 1, rc[k].ds_n, s));
   }
   for (int k = 0; k < n_sc; k += 8) {  // (one launch takes up to eight segments)
-    const int launched = lwse::launch_scatter(sc + k, n_sc - k < 8 ? n_sc - k : 8, nullptr, 0, s, false, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_scatter(sc + k, n_sc - k < 8 ? n_sc - k : 8, nullptr, 0, s, false));
   }
   for (uint32_t i = 0; i < n_segs; i++)
     if (segs[i].table == LWSE_TABLE_DS_LINKS && segs[i].n) e->rd_linked = true;
@@ -3985,8 +3884,7 @@ LWSE_API int lwse_ds_resident_tick(lwse_engine* e, const lwse_patch_seg* segs, u
                              (uint32_t*)e->rd_counters.p, reinterpret_cast<uint32_t*>(pin_d), seq, e->rd_all,
                              linked ? (const lwse_ds_link*)e->rd_links.p : nullptr, (const lwse_lws_rec*)e->r_lws.p,
                              (const lwse_lws_out*)e->r_lws_out.p, lws_results ? e->rn_lws : 0u};
-    const int launched = lwse::launch_ds_tick(&t, &a, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_ds_tick(&t, &a, e->sm_count, s));
     cudaError_t werr = cudaSuccess;
     if (!wait_word(hw + 1, seq, s, &werr)) {
       const cudaError_t a2 = cudaStreamSynchronize(s);
@@ -4046,9 +3944,7 @@ static int forecast_locked(lwse_engine* e, const lwse_ds_tables& d, lwse_ds_fore
                          (lwse_ds_role_out*)e->fc_role_out.p, (lwse_ds_revrole_out*)e->fc_revrole_out.p,
                          (lwse_ds_forecast*)e->fc_ds.p, (lwse_ds_forecast_role*)e->fc_roles.p,
                          nullptr, cap, out->steps != nullptr, (unsigned long long*)e->fc_totals.p};
-  int cuda_err = 0;
-  int launched = lwse::launch_ds_forecast(&d, &h, false, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_ds_forecast(&d, &h, false, e->sm_count, s));
   uint64_t* words = static_cast<uint64_t*>(e->fc_words.h);
   LWSE_CUDA(e, cudaMemcpyAsync(words, e->fc_totals.p, 16, cudaMemcpyDeviceToHost, s));
   if (b_fc) LWSE_CUDA(e, cudaMemcpyAsync(out->ds, e->fc_ds.p, b_fc, cudaMemcpyDeviceToHost, s));
@@ -4061,8 +3957,7 @@ static int forecast_locked(lwse_engine* e, const lwse_ds_tables& d, lwse_ds_fore
   if (written) {
     LWSE_CUDA(e, e->fc_steps.reserve((size_t)written * sizeof(lwse_ds_role_out) + 16));
     h.steps = (lwse_ds_role_out*)e->fc_steps.p;
-    launched = lwse::launch_ds_forecast(&d, &h, true, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_ds_forecast(&d, &h, true, e->sm_count, s));
     LWSE_CUDA(e, cudaMemcpyAsync(out->steps, e->fc_steps.p, (size_t)written * sizeof(lwse_ds_role_out),
                                  cudaMemcpyDeviceToHost, s));
     LWSE_CUDA(e, cudaStreamSynchronize(s));
@@ -4177,9 +4072,7 @@ LWSE_API int lwse_resident_ds_rollout_whatif(lwse_engine* e, lwse_ds_rollout_wha
   h.s_ds = (lwse_ds_rec*)e->dw_ds.p;
   h.s_roles = (lwse_ds_role_rec*)e->dw_roles.p;
   unsigned long long* d_sums = (unsigned long long*)e->dw_sums.p;
-  int cuda_err = 0;
-  int launched = lwse::launch_ds_whatif_layout(&h, d_sums + 2, d_sums, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_ds_whatif_layout(&h, d_sums + 2, d_sums, e->sm_count, s));
   uint64_t* words = static_cast<uint64_t*>(e->dw_words.h);
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_sums, 8, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
@@ -4189,8 +4082,7 @@ LWSE_API int lwse_resident_ds_rollout_whatif(lwse_engine* e, lwse_ds_rollout_wha
   LWSE_CUDA(e, e->dw_revrole_out.reserve((size_t)nrr * sizeof(lwse_ds_revrole_out) + 16));
   h.s_revroles = (lwse_ds_revrole_rec*)e->dw_revroles.p;
   h.s_links = (lwse_ds_link*)e->dw_links.p;
-  launched = lwse::launch_ds_whatif_gather(&h, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_ds_whatif_gather(&h, e->sm_count, s));
   // the DS tick's first decision over the proposed rows: the linked sweep under the tick's link state (linked only
   // after a link patch since the DS load; LWS results only while the LWS rows are loaded and swept)
   lwse_ds_tables t{};
@@ -4207,8 +4099,7 @@ LWSE_API int lwse_resident_ds_rollout_whatif(lwse_engine* e, lwse_ds_rollout_wha
   const bool lws_results = e->rd_linked && e->r_loaded && e->r_swept;
   const lwse::DsDrainLink lk{(const lwse_ds_link*)e->dw_links.p, (const lwse_lws_rec*)e->r_lws.p,
                              (const lwse_lws_out*)e->r_lws_out.p, lws_results ? e->rn_lws : 0u};
-  launched = lwse::launch_ds_drain_sweep(&t, &lk, lk.lws_out, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_ds_drain_sweep(&t, &lk, lk.lws_out, e->sm_count, s));
   if (const int rc = forecast_locked(e, t, &q->fc, s); rc != LWSE_OK) return rc;
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(q->now, t.ds_out, (size_t)n * sizeof(lwse_ds_out), cudaMemcpyDeviceToHost, s));
@@ -4237,9 +4128,7 @@ static int lws_forecast_locked(lwse_engine* e, lwse::LwsForecastHost& h, lwse_lw
   h.fc = (lwse_lws_forecast*)e->lf_fc.p;
   h.totals = (unsigned long long*)e->lf_totals.p;
   uint64_t* words = static_cast<uint64_t*>(e->lf_words.h);
-  int cuda_err = 0;
-  int launched = lwse::launch_lws_forecast_slots(&h, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_lws_forecast_slots(&h, e->sm_count, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words, e->lf_totals.p, 32, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   const uint64_t n_slots = h.n_lws ? words[2] : 0u;
@@ -4249,8 +4138,7 @@ static int lws_forecast_locked(lwse_engine* e, lwse::LwsForecastHost& h, lwse_lw
   h.n_slots = (uint32_t)n_slots;
   h.steps = nullptr;
   h.steps_rows = 0;
-  launched = lwse::launch_lws_forecast(&h, false, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_lws_forecast(&h, false, e->sm_count, s));
   const size_t b_fc = (size_t)h.n_lws * sizeof(lwse_lws_forecast);
   LWSE_CUDA(e, cudaMemcpyAsync(words, e->lf_totals.p, 32, cudaMemcpyDeviceToHost, s));
   if (b_fc && out->lws) LWSE_CUDA(e, cudaMemcpyAsync(out->lws, e->lf_fc.p, b_fc, cudaMemcpyDeviceToHost, s));
@@ -4263,8 +4151,7 @@ static int lws_forecast_locked(lwse_engine* e, lwse::LwsForecastHost& h, lwse_lw
     LWSE_CUDA(e, e->lf_steps.reserve((size_t)written * sizeof(lwse_lws_forecast_step) + 16));
     h.steps = (lwse_lws_forecast_step*)e->lf_steps.p;
     h.steps_rows = written;
-    launched = lwse::launch_lws_forecast(&h, true, e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_lws_forecast(&h, true, e->sm_count, s));
     LWSE_CUDA(e, cudaMemcpyAsync(words, e->lf_totals.p, 32, cudaMemcpyDeviceToHost, s));
     LWSE_CUDA(e, cudaMemcpyAsync(out->steps, e->lf_steps.p, (size_t)written * sizeof(lwse_lws_forecast_step),
                                  cudaMemcpyDeviceToHost, s));
@@ -4368,9 +4255,7 @@ static int enqueue_rollout_whatif(lwse_engine* e, uint32_t n, cudaStream_t s, lw
   h.n = n;
   h.off = (unsigned long long*)e->rw_off.p;
   h.s_lws = (lwse_lws_rec*)e->rw_lws.p;
-  int cuda_err = 0;
-  int launched = lwse::launch_rollout_whatif_layout(&h, d_sums + 2, d_sums, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_rollout_whatif_layout(&h, d_sums + 2, d_sums, s));
   uint64_t* words = static_cast<uint64_t*>(e->lf_words.h);
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_sums, 8, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
@@ -4385,8 +4270,7 @@ static int enqueue_rollout_whatif(lwse_engine* e, uint32_t n, cudaStream_t s, lw
   LWSE_CUDA(e, e->rw_scan.reserve(lwse::lws_sweep_scratch_bytes(np, ng)));
   h.s_groups = (lwse_group_rec*)e->rw_groups.p;
   h.s_src = (uint32_t*)e->rw_src.p;
-  launched = lwse::launch_rollout_whatif_gather(&h, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_rollout_whatif_gather(&h, e->sm_count, s));
   // the group pass over {proposal rows, gathered groups, resident pods}, no occupancy
   lwse_lws_tables d{};
   d.lws = (const lwse_lws_rec*)e->rw_lws.p;
@@ -4400,18 +4284,14 @@ static int enqueue_rollout_whatif(lwse_engine* e, uint32_t n, cudaStream_t s, lw
   d.group_out = (lwse_group_out*)e->rw_group_out.p;
   d.flags = e->r_sweep_flags | LWSE_SWEEP_SKIP_LWS_PASS;
   const lwse_node_rec* nodes = (const lwse_node_rec*)e->nodes.p;
-  launched = lwse::launch_lws_sweep(&d, nodes, e->n_nodes, e->rw_scan.p, e->sm_count, s, &cuda_err, nullptr, nullptr,
-                                    /*first_mode=*/0);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_lws_sweep(&d, nodes, e->n_nodes, e->rw_scan.p, e->sm_count, s, nullptr, nullptr,
+                                        /*first_mode=*/0));
   // the rows other objects own keep the resident sweep's result, where the forecast and the LWS pass read it
-  launched = lwse::launch_rollout_whatif_restore(h.s_src, (const lwse_group_out*)e->r_group_out.p, d.group_out,
-                                                 lwse::lws_sweep_flag_column(e->rw_scan.p, np), ng, e->sm_count, s,
-                                                 &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_rollout_whatif_restore(h.s_src, (const lwse_group_out*)e->r_group_out.p, d.group_out,
+                                                     lwse::lws_sweep_flag_column(e->rw_scan.p, np), ng, e->sm_count, s));
   d.flags = e->r_sweep_flags | LWSE_SWEEP_SKIP_GROUP_PASS | LWSE_SWEEP_SKIP_POD_SCAN;  // the LWS pass alone
-  launched = lwse::launch_lws_sweep(&d, nodes, e->n_nodes, e->rw_scan.p, e->sm_count, s, &cuda_err, nullptr, nullptr,
-                                    /*first_mode=*/0);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_lws_sweep(&d, nodes, e->n_nodes, e->rw_scan.p, e->sm_count, s, nullptr, nullptr,
+                                        /*first_mode=*/0));
   lwse::LwsForecastHost f{};
   f.lws = (const lwse_lws_rec*)e->rw_lws.p;
   f.n_lws = n;
@@ -4509,9 +4389,7 @@ static int rollout_place_count(lwse_engine* e, const uint32_t* rows, const uint3
   p->e_cursor = p->e_first + n + 1;
   p->items = (uint2*)e->rp_items.p;
   p->counts = d_words;
-  int cuda_err = 0;
-  const int launched = lwse::launch_rollout_place(p, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_rollout_place(p, 0, e->sm_count, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 16, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   return LWSE_OK;
@@ -4550,21 +4428,17 @@ static int rollout_place_solve(lwse_engine* e, uint32_t n_items, uint32_t max_ex
   p->slice_rows = (uint32_t)slice_rows;
   p->grid = (uint32_t)grid;
   // the baseline's totals (a diff of the baseline rows against themselves counts them), every namespace's index
-  int cuda_err = 0;
-  int launched = lwse::launch_place_whatif_diff(p->base, p->base, 0, nr, nullptr, nullptr, nullptr, 0, p->counts + 16,
-                                                e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_place_whatif_diff(p->base, p->base, 0, nr, nullptr, nullptr, nullptr, 0, p->counts + 16,
+                                                e->sm_count, s));
   if (grid) {
     LWSE_CUDA(e, cudaMemsetAsync(e->rp_touched.p, 1, n_ns, s));
     LWSE_CUDA(e, cudaMemsetAsync(e->rp_round.p, 0, round_bytes, s));  // (the index counts start at zero)
     if (e->node_index_stale)
       if (const int rc = own_node_index(e, p->nodes, s, &p->dom_first, &p->node_order, nullptr); rc != LWSE_OK) return rc;
-    launched = lwse::launch_place_whatif_index(p->reqs, nr, n_ns, (const uint8_t*)e->rp_touched.p, nn, nd, e->rp_round.p,
-                                               e->sm_count, s, &cuda_err);
-    if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+    LWSE_LAUNCH(e, lwse::launch_place_whatif_index(p->reqs, nr, n_ns, (const uint8_t*)e->rp_touched.p, nn, nd, e->rp_round.p,
+                                                   e->sm_count, s));
   }
-  launched = lwse::launch_rollout_place(p, 1, e->sm_count, s, &cuda_err);
-  return count_launch(e, launched, cuda_err);
+  return count_launch(e, lwse::launch_rollout_place(p, 1, e->sm_count, s));
 }
 
 // The checks both rollout placement calls make before anything is enqueued.
@@ -4679,9 +4553,7 @@ LWSE_API int lwse_resident_rollout_place_waves(lwse_engine* e, lwse_rollout_plac
   w.ns_keys = w.rank + n;
   w.act = w.ns_keys + n;
   w.out = (uint8_t*)e->rq_out.p;
-  int cuda_err = 0;
-  int launched = lwse::launch_rollout_place_waves(&w, 0, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_rollout_place_waves(&w, 0, e->sm_count, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words + 16, st, 32, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));
   const uint32_t R = words[16 + 2], max_t = words[16 + 3];
@@ -4712,11 +4584,11 @@ LWSE_API int lwse_resident_rollout_place_waves(lwse_engine* e, lwse_rollout_plac
     cudaGraph_t graph = nullptr;
     GraphExec exec;
     LWSE_CUDA(e, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    launched = lwse::launch_rollout_place_waves(&w, 1, e->sm_count, s, &cuda_err);
+    const int launched = lwse::launch_rollout_place_waves(&w, 1, e->sm_count, s);
     const cudaError_t ce = cudaStreamEndCapture(s, &graph);
     if (launched < 0 || ce != cudaSuccess) {
       if (graph) cudaGraphDestroy(graph);
-      return fail_cuda(e, launched < 0 ? (cudaError_t)cuda_err : ce);
+      return fail_cuda(e, launched < 0 ? (cudaError_t)-launched : ce);
     }
     cudaError_t ge = exec.ensure(graph);
     cudaGraphDestroy(graph);
@@ -4724,8 +4596,7 @@ LWSE_API int lwse_resident_rollout_place_waves(lwse_engine* e, lwse_rollout_plac
     if (ge != cudaSuccess) return fail_cuda(e, ge);
     e->launches += (uint64_t)launched * R;
   }
-  launched = lwse::launch_rollout_place_waves(&w, 2, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_rollout_place_waves(&w, 2, e->sm_count, s));
   if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
   LWSE_CUDA(e, cudaMemcpyAsync(e->rq_host.h, w.out, out_bytes, cudaMemcpyDeviceToHost, s));
   if (q->alone_rows)
@@ -4749,9 +4620,7 @@ LWSE_API int lwse_resident_rollout_place_waves(lwse_engine* e, lwse_rollout_plac
 // ---------------------------------------------------------------------------
 static int group_keys_locked(lwse_engine* e, const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n,
                              uint8_t* d_digests, cudaStream_t s) {
-  int cuda_err = 0;
-  int launched = lwse::launch_sha1(d_bytes, d_offsets, n, d_digests, e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_sha1(d_bytes, d_offsets, n, d_digests, e->sm_count, s));
   return LWSE_OK;
 }
 
@@ -4794,10 +4663,8 @@ LWSE_API int lwse_subgroup_keys_device(lwse_engine* e, const uint8_t* d_bytes, c
     return LWSE_ERR_INVALID_ARG;
   std::lock_guard<std::mutex> lock(e->mu);
   DeviceGuard guard(e->device);
-  int cuda_err = 0;
-  int launched = lwse::launch_subgroup_keys(d_bytes, d_offsets, n, d_pod_count, d_subgroup_size, d_worker_index, d_index_out,
-                                            d_digests, e->sm_count, stream ? (cudaStream_t)stream : e->stream, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+  LWSE_LAUNCH(e, lwse::launch_subgroup_keys(d_bytes, d_offsets, n, d_pod_count, d_subgroup_size, d_worker_index, d_index_out,
+                                            d_digests, e->sm_count, stream ? (cudaStream_t)stream : e->stream));
   return LWSE_OK;
 }
 
@@ -4823,11 +4690,9 @@ LWSE_API int lwse_subgroup_keys_host(lwse_engine* e, const uint8_t* bytes, const
   LWSE_CUDA(e, cudaMemcpyAsync(d_int, pod_count, b_int, cudaMemcpyHostToDevice, s));
   LWSE_CUDA(e, cudaMemcpyAsync(d_int + n, subgroup_size, b_int, cudaMemcpyHostToDevice, s));
   LWSE_CUDA(e, cudaMemcpyAsync(d_int + 2 * (size_t)n, worker_index, b_int, cudaMemcpyHostToDevice, s));
-  int cuda_err = 0;
-  int launched = lwse::launch_subgroup_keys((const uint8_t*)e->sha_bytes.p, (const uint32_t*)e->sha_offsets.p, n, d_int, d_int + n,
+  LWSE_LAUNCH(e, lwse::launch_subgroup_keys((const uint8_t*)e->sha_bytes.p, (const uint32_t*)e->sha_offsets.p, n, d_int, d_int + n,
                                             d_int + 2 * (size_t)n, d_int + 3 * (size_t)n, (uint8_t*)e->sha_digests.p,
-                                            e->sm_count, s, &cuda_err);
-  if (const int rc = count_launch(e, launched, cuda_err); rc != LWSE_OK) return rc;
+                                            e->sm_count, s));
   LWSE_CUDA(e, cudaMemcpyAsync(index_out, d_int + 3 * (size_t)n, b_int, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaMemcpyAsync(digests, e->sha_digests.p, (size_t)n * 20, cudaMemcpyDeviceToHost, s));
   LWSE_CUDA(e, cudaStreamSynchronize(s));

@@ -93,9 +93,8 @@ __global__ void __launch_bounds__(256) exchange_push_kernel(const ExchangeArgs a
 
 int launch_exchange_push(const void* d_local_part, uint8_t* const* d_peer_base, void* d_local_base,
                          uint64_t part_bytes, uint64_t part_stride, uint64_t half_bytes, uint64_t flags_offset,
-                         uint64_t step, uint64_t wait_step, uint32_t world, uint32_t rank, cudaStream_t s, int* cuda_err,
+                         uint64_t step, uint64_t wait_step, uint32_t world, uint32_t rank, cudaStream_t s,
                          bool lagged) {
-  *cuda_err = 0;
   ExchangeArgs a{};
   uint8_t* base = static_cast<uint8_t*>(d_local_base);
   a.local_part = static_cast<const uint4*>(d_local_part);
@@ -119,12 +118,7 @@ int launch_exchange_push(const void* d_local_part, uint8_t* const* d_peer_base, 
   if (grid > 32u) grid = 32u;
   if (grid < 1u) grid = 1u;
   exchange_push_kernel<<<grid, 256, 0, s>>>(a);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 }  // namespace lwse

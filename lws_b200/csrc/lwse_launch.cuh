@@ -4,7 +4,8 @@
 // kernel that reads it cannot disagree on its layout.
 //
 // A launcher enqueues its kernels on the stream it is given and returns the number of kernels it
-// launched (>= 0), or -1 with *cuda_err set.
+// launched (>= 0), or the CUDA error it met, negated (-(int)err).  A launcher that calls another
+// passes the callee's negative result through unchanged.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -14,6 +15,12 @@
 #include "../../include/lwse.h"
 
 namespace lwse {
+
+// A launcher returns the kernels it enqueued (>= 0), or the CUDA error it met, negated.
+inline int launch_result(int kernels) {
+  const cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? kernels : -(int)e;
+}
 
 // ---- lwse_lws_kernels.cu ----
 int pick_tile(uint64_t items, uint64_t owners);  // lanes per object of the LWS pass (and of the forecast)
@@ -28,7 +35,7 @@ struct SweepChangeLists {  // device (or mapped host) pointers; all null = off
   uint32_t* counts = nullptr;  // device: [0] lws, [1] groups; zeroed by the caller (a tick's publish kernel resets them)
 };
 int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uint32_t n_nodes,
-                     void* scratch, int sm_count, cudaStream_t s, int* cuda_err, const SweepChangeLists* cl,
+                     void* scratch, int sm_count, cudaStream_t s, const SweepChangeLists* cl,
                      uint32_t* d_event_count = nullptr, int first_mode = 1);
 size_t lws_sweep_scratch_bytes(uint64_t n_pods, uint32_t n_groups);
 // The sweep scratch's flag column: one byte per group row, the low five bits of its group_out.flags, which
@@ -45,7 +52,7 @@ struct PublishListHost {
   uint32_t out_bytes;
 };
 int launch_publish(const PublishListHost* lists, const uint32_t* d_extra, uint32_t* h_words, uint32_t seq_slot,
-                   uint32_t seq, uint32_t* d_ticket, uint32_t expected_rows, cudaStream_t s, int* cuda_err,
+                   uint32_t seq, uint32_t* d_ticket, uint32_t expected_rows, cudaStream_t s,
                    uint32_t* d_clear, uint32_t n_clear, bool pdl);
 
 struct ScatterSegHost {
@@ -58,29 +65,29 @@ struct ScatterSegHost {
   bool is_ident;
 };
 int launch_scatter(const ScatterSegHost* segs, int n_segs, uint32_t* d_occupancy, uint32_t n_nodes, cudaStream_t s,
-                   bool pdl, int* cuda_err);
+                   bool pdl);
 // Bytes of one scatter descriptor block of a graph tick (write_scatter_desc / launch_scatter_desc); the
 // kernel file asserts that its argument block fits.
 constexpr size_t kScatterDescBytes = 512;
 bool write_scatter_desc(void* h_desc, const ScatterSegHost* segs, int n_segs, uint32_t* d_occupancy, uint32_t n_nodes);
-int launch_scatter_desc(const void* d_desc, int sm_count, cudaStream_t s, bool pdl, int* cuda_err);
+int launch_scatter_desc(const void* d_desc, int sm_count, cudaStream_t s, bool pdl);
 int launch_ident_prefetch(const uint8_t* d_state, uint64_t n_pods, const lwse_pod_ident* mapped_host_ident,
-                          lwse_pod_ident* d_ident, int sm_count, cudaStream_t s, int* cuda_err);
+                          lwse_pod_ident* d_ident, int sm_count, cudaStream_t s);
 int launch_occupancy(const lwse_pod_ident* d_ident, uint64_t n_pods, uint32_t* d_occupancy, uint32_t n_nodes, int sm_count,
-                     cudaStream_t s, int* cuda_err);
+                     cudaStream_t s);
 
 // ---- lwse_place_kernels.cu ----
 int launch_place(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, const uint32_t* d_node_order,
                  const uint32_t* d_node_pos, uint32_t n_nodes, uint32_t n_domains,
                  const lwse_place_req* d_reqs, uint32_t n_reqs, const uint32_t* d_occupancy,
                  uint32_t n_namespaces, lwse_place_out* d_out, void* d_scratch, size_t scratch_bytes,
-                 uint32_t* h_rounds, int sm_count, cudaStream_t s, int* cuda_err, uint32_t call_index,
+                 uint32_t* h_rounds, int sm_count, cudaStream_t s, uint32_t call_index,
                  bool fresh, uint32_t n_parts, uint32_t reqs_per_part, uint64_t part_stride_bytes,
                  uint32_t* h_unpinned, const uint32_t** d_counters_out, const uint32_t** d_unpinned_out,
                  bool after_push);
 size_t place_scratch_bytes(uint32_t n_nodes, uint32_t n_domains, uint32_t n_reqs, uint32_t n_namespaces);
 int launch_place_diff(const lwse_place_out* d_cur, lwse_place_out* d_prev, uint32_t n, uint32_t* d_rows,
-                      lwse_place_out* d_outs, uint32_t capacity, uint32_t* d_count, cudaStream_t s, int* cuda_err);
+                      lwse_place_out* d_outs, uint32_t capacity, uint32_t* d_count, cudaStream_t s);
 
 // ---- lwse_place_ns_kernels.cu ----
 struct PlaceNsChanges {  // a tick's change list (device memory); prev == null: off
@@ -111,24 +118,24 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
                     uint32_t n_domains, const lwse_place_req* d_reqs, uint32_t n_reqs,
                     const uint32_t* d_occupancy, uint32_t n_parts, uint64_t part_stride_bytes, uint32_t n_namespaces,
                     lwse_place_out* d_out, void* d_scratch, size_t scratch_bytes, bool fresh, uint32_t call_index, bool scan,
-                    int sm_count, cudaStream_t s, int* cuda_err, const uint32_t** d_counters_out, bool first_pdl,
+                    int sm_count, cudaStream_t s, const uint32_t** d_counters_out, bool first_pdl,
                     const PlaceNsChanges* changes, const PlaceNsExchange* xch, PlaceNsIndex index);
 size_t place_ns_scratch_bytes(uint32_t n_nodes, uint32_t n_domains, uint32_t n_reqs, uint32_t n_namespaces);
 size_t node_index_scratch_bytes(uint32_t n_domains);
 // The index block's scan (one CTA): first[0..n] = the exclusive scan of count[0..n) and its total, cursor = first,
 // count back to zero.
-int launch_index_scan(uint32_t* d_count, uint32_t* d_first, uint32_t* d_cursor, uint32_t n, cudaStream_t s, int* cuda_err);
+int launch_index_scan(uint32_t* d_count, uint32_t* d_first, uint32_t* d_cursor, uint32_t n, cudaStream_t s);
 int launch_node_index(const lwse_node_rec* d_nodes, uint32_t n_nodes, uint32_t n_domains, uint32_t* d_dom_first,
                       uint32_t* d_node_order, uint32_t* d_node_pos, void* d_scratch, int sm_count, cudaStream_t s,
-                      bool pdl, int* cuda_err);
+                      bool pdl);
 int launch_place_whatif_index(const lwse_place_req* d_reqs, uint32_t n_reqs, uint32_t n_namespaces, const uint8_t* d_touched,
-                              uint32_t n_nodes, uint32_t n_domains, void* d_scratch, int sm_count, cudaStream_t s, int* cuda_err);
+                              uint32_t n_nodes, uint32_t n_domains, void* d_scratch, int sm_count, cudaStream_t s);
 int launch_place_whatif_diff(const lwse_place_out* d_before, const lwse_place_out* d_after, uint32_t n_resident, uint32_t n_total,
                              uint32_t* d_rows, lwse_place_out* d_outs_before, lwse_place_out* d_outs_after, uint32_t capacity,
-                             uint32_t* d_counts, int sm_count, cudaStream_t s, int* cuda_err);
+                             uint32_t* d_counts, int sm_count, cudaStream_t s);
 
 // ---- lwse_ds_kernels.cu ----
-int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_ds_sweep(const lwse_ds_tables* t, int sm_count, cudaStream_t s);
 
 struct DsTickHost {
   const lwse_ds_out* prev_ds_out;
@@ -148,7 +155,7 @@ struct DsTickHost {
   const lwse_lws_out* lws_out;
   uint32_t n_lws;
 };
-int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_ds_tick(const lwse_ds_tables* t, const DsTickHost* h, int sm_count, cudaStream_t s);
 
 struct DsForecastHost {
   lwse_ds_revrole_rec* rows;
@@ -162,8 +169,7 @@ struct DsForecastHost {
   bool want_steps;  // a trajectory is asked for: the scan marks what does not fit in step_capacity
   unsigned long long* totals;  // device, 2 words, zeroed by the caller
 };
-int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s,
-                       int* cuda_err);
+int launch_ds_forecast(const lwse_ds_tables* t, const DsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s);
 
 // DS drain (lwse_resident_ds_drain*): the link table and the baseline LWS rows it points into.
 struct DsDrainLink {
@@ -175,7 +181,7 @@ struct DsDrainLink {
 // A linked DS sweep of t into t's outputs, reading ready counts from `ready_from` (the baseline, or its copy
 // with the drain's lost groups taken off) through the link rule of `lk`.
 int launch_ds_drain_sweep(const lwse_ds_tables* t, const DsDrainLink* lk, const lwse_lws_out* ready_from, int sm_count,
-                          cudaStream_t s, int* cuda_err);
+                          cudaStream_t s);
 // The set form's diff: t's outputs (after) against `before`; touched DS appended to rows (up to capacity).
 // counts (device, zeroed by the caller): [16] touched (the append cursor) [17] service lost [18] old service
 // lost [19] stalled [20] changed [21] rows touched [22] rows zeroed [23] rows linked.
@@ -189,14 +195,14 @@ struct DsDrainDiffHost {
   uint32_t* counts;
 };
 int launch_ds_drain_diff(const lwse_ds_tables* t, const DsDrainLink* lk, const DsDrainDiffHost* h, int sm_count,
-                         cudaStream_t s, int* cuda_err);
+                         cudaStream_t s);
 // The reverse link index of the per-key form: LWS row → the revision-role rows that take its value, once per DS
 // whose ranges hold the row (DS ranges may overlap).  fill = false: count[L] += rows per L (count zeroed by the
 // caller) and *total (u64, zeroed by the caller) += all of them.  fill = true: every such row's entry
 // {DS row, slot (0xFF: the new revision) | 0x100 when a spec role, ready_before, 0} at cursor[L]++, written only
 // below capacity (entries holds capacity rows; the caller sizes it from *total).
 int launch_ds_drain_links(const lwse_ds_tables* t, const DsDrainLink* lk, uint32_t* count, uint32_t* cursor, uint4* entries,
-                          uint32_t capacity, unsigned long long* total, bool fill, int sm_count, cudaStream_t s, int* cuda_err);
+                          uint32_t capacity, unsigned long long* total, bool fill, int sm_count, cudaStream_t s);
 constexpr uint32_t kDsDrainNewSlot = 0xFFu;
 constexpr uint32_t kDsDrainSpec = 0x100u;
 
@@ -217,8 +223,8 @@ struct LwsForecastHost {
   unsigned long long* totals;    // device: [0] rows needed, [1] rows written, [2] slots, [3] refused accesses
                                  // (zeroed by the caller), then forecast_scan_words(n_lws) words for the scans
 };
-int launch_lws_forecast_slots(const LwsForecastHost* h, int sm_count, cudaStream_t s, int* cuda_err);
-int launch_lws_forecast(const LwsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_lws_forecast_slots(const LwsForecastHost* h, int sm_count, cudaStream_t s);
+int launch_lws_forecast(const LwsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s);
 
 // ---- lwse_rollout_whatif_kernels.cu ----
 struct RolloutWhatifHost {
@@ -235,11 +241,11 @@ struct RolloutWhatifHost {
 // The layout: off[i] = the exclusive prefix of the proposals' gathered rows, *total = their sum (u64).
 // sums: forecast_scan_words(n) words.
 int launch_rollout_whatif_layout(const RolloutWhatifHost* h, unsigned long long* sums, unsigned long long* total,
-                                 cudaStream_t s, int* cuda_err);
-int launch_rollout_whatif_gather(const RolloutWhatifHost* h, int sm_count, cudaStream_t s, int* cuda_err);
+                                 cudaStream_t s);
+int launch_rollout_whatif_gather(const RolloutWhatifHost* h, int sm_count, cudaStream_t s);
 // The foreign-owned rows' baseline results into d_out and the sweep's flag column (lws_sweep_flag_column).
 int launch_rollout_whatif_restore(const uint32_t* d_src, const lwse_group_out* d_baseline, lwse_group_out* d_out,
-                                  uint8_t* d_gflag8, uint32_t n_rows, int sm_count, cudaStream_t s, int* cuda_err);
+                                  uint8_t* d_gflag8, uint32_t n_rows, int sm_count, cudaStream_t s);
 
 // ---- lwse_ds_whatif_kernels.cu ----
 struct DsWhatifHost {
@@ -259,31 +265,29 @@ struct DsWhatifHost {
 // The layout: count[i], then off[i] = their exclusive prefix and *total = their sum (u64, < 2^32 for
 // n <= LWSE_DS_WHATIF_MAX_PROPOSALS).  sums: forecast_scan_words(n) words.
 int launch_ds_whatif_layout(const DsWhatifHost* h, unsigned long long* sums, unsigned long long* total, int sm_count,
-                            cudaStream_t s, int* cuda_err);
-int launch_ds_whatif_gather(const DsWhatifHost* h, int sm_count, cudaStream_t s, int* cuda_err);
+                            cudaStream_t s);
+int launch_ds_whatif_gather(const DsWhatifHost* h, int sm_count, cudaStream_t s);
 
 // ---- lwse_drain_kernels.cu ----
 // The drain what-if's counters (device, 16 words, zeroed by the caller): [0] changed rows [1] pods evicted
 // [2] leaders evicted [3] groups restarted [4] ready groups restarted [6..7] pods recreated (u64).
 int launch_drain_mark(const uint8_t* d_mask, uint32_t n_nodes, const lwse_pod_ident* d_ident, uint8_t* d_state, uint64_t n_pods,
-                      lwse_group_rec* d_groups, uint32_t n_groups, uint32_t* d_counts, int sm_count, cudaStream_t s,
-                      int* cuda_err);
+                      lwse_group_rec* d_groups, uint32_t n_groups, uint32_t* d_counts, int sm_count, cudaStream_t s);
 int launch_drain_diff(const lwse_group_out* d_before, const lwse_group_out* d_after, const lwse_group_rec* d_groups,
                       uint32_t n_groups, uint32_t* d_rows, lwse_group_out* d_outs_before, lwse_group_out* d_outs_after,
-                      uint32_t capacity, uint32_t* d_counts, int sm_count, cudaStream_t s, int* cuda_err);
+                      uint32_t capacity, uint32_t* d_counts, int sm_count, cudaStream_t s);
 // d_cost: n_nodes rows with `pods` filled in and every other field zero.
 int launch_drain_cost(const lwse_lws_rec* d_lws, uint32_t n_lws, const lwse_group_rec* d_groups, uint32_t n_groups,
                       const uint8_t* d_state, const lwse_pod_ident* d_ident, uint64_t n_pods, const lwse_group_out* d_baseline,
-                      lwse_drain_cost* d_cost, uint32_t n_nodes, int sm_count, cudaStream_t s, int* cuda_err);
+                      lwse_drain_cost* d_cost, uint32_t n_nodes, int sm_count, cudaStream_t s);
 // The node mask of a set of domains (d_domains: n_domains bytes, 1 = drained) into d_mask (n_nodes bytes).
 int launch_drain_domain_mask(const uint8_t* d_domains, uint32_t n_domains, const lwse_node_rec* d_nodes, uint32_t n_nodes,
-                             uint8_t* d_mask, int sm_count, cudaStream_t s, int* cuda_err);
+                             uint8_t* d_mask, int sm_count, cudaStream_t s);
 // The drain budget's set form over a what-if sweep (d_after) against the baseline: touched rows appended to
 // d_rows (up to capacity); counters [8] touched [9] breached [10] loses available [11] already below.
 int launch_drain_budget(const lwse_lws_rec* d_lws, const lwse_lws_out* d_lws_out, uint32_t n_lws, const lwse_group_rec* d_groups,
                         const lwse_group_out* d_before, const lwse_group_out* d_after, uint32_t n_groups,
-                        lwse_drain_budget* d_rows, uint32_t capacity, uint32_t* d_counts, int sm_count, cudaStream_t s,
-                        int* cuda_err);
+                        lwse_drain_budget* d_rows, uint32_t capacity, uint32_t* d_counts, int sm_count, cudaStream_t s);
 // The drain budget's per-key form.  Pass 0: the key rows (cost zeroed by the caller) get their pods and cost
 // totals, and counts[0..1] (u64, zeroed by the caller) the (group, key) pairs the table must hold.  Pass 1
 // (keys all-ones and vals zeroed by the caller, table_mask + 1 a power of two > the pairs): the (LWS, key)
@@ -306,12 +310,12 @@ struct DrainBudgetCostLaunch {
   bool by_domain;
 };
 // Pass 2: the (LWS, key) table alone (pass 1 without the budget columns).
-int launch_drain_budget_cost(const DrainBudgetCostLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_drain_budget_cost(const DrainBudgetCostLaunch* p, int pass, int sm_count, cudaStream_t s);
 // The DS drain's set form: lost[L] (the drain budget's lost groups of every LWS row, d_after a what-if sweep
 // against the baseline d_before) and d_lws_after, a copy of d_lws_out with ready_replicas - lost[L].
 int launch_ds_drain_lost(const lwse_lws_rec* d_lws, const lwse_lws_out* d_lws_out, uint32_t n_lws, const lwse_group_rec* d_groups,
                          const lwse_group_out* d_before, const lwse_group_out* d_after, uint32_t n_groups, uint32_t* d_lost,
-                         lwse_lws_out* d_lws_after, int sm_count, cudaStream_t s, int* cuda_err);
+                         lwse_lws_out* d_lws_after, int sm_count, cudaStream_t s);
 // The DS drain's per-key form over the drain budget's (LWS, key) table (vals.y = lost(L, key)) and the reverse
 // link index.  Pass 0: counts[0..1] (u64, zeroed by the caller) = the (row, key) pairs.  Pass 1 (keys all-ones
 // and vals zeroed by the caller, table_mask + 1 a power of two > the pairs): the (DS, key) table, the key rows'
@@ -329,7 +333,7 @@ struct DsDrainCostLaunch {
   uint32_t table_mask;
   uint32_t* counts;
 };
-int launch_ds_drain_cost(const DsDrainCostLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_ds_drain_cost(const DsDrainCostLaunch* p, int pass, int sm_count, cudaStream_t s);
 
 // ---- lwse_drain_place_kernels.cu (and the drain instance of the namespace kernel) ----
 // lwse_resident_drain_place_cost.  counts (device, 16 words, zeroed by the caller): [0] PLACED [1] UNSCHEDULABLE
@@ -376,11 +380,11 @@ struct DrainPlaceLaunch {
 // Pass 1 (pairs written): U_k's rows of restarted groups counted, then the U_k index scanned.
 // Pass 2 (u_rows, items sized): U_k filled, the key rows started, the items gathered (and the rows of U_k
 // outside every namespace counted), then the solve.
-int launch_drain_place(const DrainPlaceLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_drain_place(const DrainPlaceLaunch* p, int pass, int sm_count, cudaStream_t s);
 // The drain budget walk in pair mode: every restart pair key << 32 | group into pairs[p->counts[8]++] (below capacity).
 int launch_drain_restart_pairs(const DrainBudgetCostLaunch* p, unsigned long long* pairs, uint32_t capacity, int sm_count,
-                               cudaStream_t s, int* cuda_err);
-int launch_place_ns_drain(const DrainPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err);
+                               cudaStream_t s);
+int launch_place_ns_drain(const DrainPlaceLaunch* p, int sm_count, cudaStream_t s);
 
 // ---- lwse_rollout_place_kernels.cu ----
 // Rollout placement (lwse_resident_rollout_place).  Entry i: resident row rows[i], namespace ns[i], proposal
@@ -421,8 +425,8 @@ struct RolloutPlaceLaunch {
 };
 // Pass 0: the count kernel (flags, |E_i|, the rows started, the items).  Pass 1 (after the host read max |E_i|):
 // the scan, the fill of the extra rows, the capacities and the solve, then the finish.
-int launch_rollout_place(const RolloutPlaceLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
-int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_rollout_place(const RolloutPlaceLaunch* p, int pass, int sm_count, cudaStream_t s);
+int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStream_t s);
 
 // ---- lwse_rollout_place_wave_kernels.cu ----
 // Rollout placement waves (lwse_resident_rollout_place_waves), over the rollout placement's setup p (its rows are
@@ -457,8 +461,8 @@ struct RolloutPlaceWavesLaunch {
 };
 // Pass 0 (after the setup's finish): the key rows, the ranks, the scan and the per-namespace key lists.  Pass 1
 // (captured, replayed R times): items, the wave instance of place_ns_kernel, commit.  Pass 2: the finish.
-int launch_rollout_place_waves(const RolloutPlaceWavesLaunch* w, int pass, int sm_count, cudaStream_t s, int* cuda_err);
-int launch_place_ns_rollout_wave(const RolloutPlaceWavesLaunch* w, cudaStream_t s, int* cuda_err);
+int launch_rollout_place_waves(const RolloutPlaceWavesLaunch* w, int pass, int sm_count, cudaStream_t s);
+int launch_place_ns_rollout_wave(const RolloutPlaceWavesLaunch* w, cudaStream_t s);
 
 // ---- lwse_drain_wave_kernels.cu ----
 // lwse_resident_drain_waves.  out: the query totals (16 B), m lwse_drain_wave_key rows, then max_waves
@@ -495,17 +499,17 @@ struct DrainWavesLaunch {
 // Pass 0 (after the drain budget's pass 0): positions, bucket sizes and the alone columns; the buckets scanned.
 // Pass 1 (pairs written): the buckets filled, the touched rows scanned, the dense rows.  Pass 2 (n_dense, lost and
 // the wave masks sized): the plan, then the wave rows' per-row columns and pods / leaders.
-int launch_drain_waves(const DrainWavesLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_drain_waves(const DrainWavesLaunch* p, int pass, int sm_count, cudaStream_t s);
 // lwse_resident_ds_drain_waves: passes 1 and 2 of launch_drain_waves with the DS caps.  caps[n_lws] (device) holds
 // per LWS row kCapLinked and the LWSE_DSW_DS_* bits of the gated rows linked to it (ds_drain_waves_caps).  Pass 1
 // binds the ready member pairs of evaluated or linked rows and writes each dense row's slack under `constraints`;
 // pass 2 runs the plan against those slacks, then the wave rows' per-row columns.
 constexpr uint32_t kCapLinked = 1u << 4;
 int launch_drain_waves_capped(const DrainWavesLaunch* p, const uint32_t* caps, uint32_t constraints, int pass, int sm_count,
-                              cudaStream_t s, int* cuda_err);
+                              cudaStream_t s);
 
 // The drain waves finish alone (the wave rows' per-row columns and pods / leaders), after a plan written elsewhere.
-int launch_drain_waves_finish(const DrainWavesLaunch* p, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_drain_waves_finish(const DrainWavesLaunch* p, int sm_count, cudaStream_t s);
 
 // ---- lwse_drain_place_wave_kernels.cu (and the set-overlay instance of the namespace kernel) ----
 // lwse_resident_drain_place_waves.  The step state lives in device memory so that one captured step replays for
@@ -540,8 +544,8 @@ struct DrainPlaceWavesLaunch {
   uint8_t* out;                    // the answer: totals (16 B), m key rows, max_waves wave rows
 };
 // Pass 0: the domain index and the first columns.  Pass 1: one step.  Pass 2: the finish.
-int launch_drain_place_waves(const DrainPlaceWavesLaunch* d, int pass, int sm_count, cudaStream_t s, int* cuda_err);
-int launch_place_ns_drain_set(const DrainPlaceWavesLaunch* d, int sm_count, cudaStream_t s, int* cuda_err);
+int launch_drain_place_waves(const DrainPlaceWavesLaunch* d, int pass, int sm_count, cudaStream_t s);
+int launch_place_ns_drain_set(const DrainPlaceWavesLaunch* d, int sm_count, cudaStream_t s);
 
 // ---- lwse_ds_drain_wave_kernels.cu ----
 // lwse_resident_ds_drain_waves, around the drain waves chain.  Pass 0 (after the before sweep into t's outputs):
@@ -557,20 +561,19 @@ struct DsDrainWavesLaunch {
   uint8_t* out;
   uint32_t max_waves;
 };
-int launch_ds_drain_waves(const DsDrainWavesLaunch* d, const DrainWavesLaunch* w, int pass, int sm_count, cudaStream_t s,
-                          int* cuda_err);
+int launch_ds_drain_waves(const DsDrainWavesLaunch* d, const DrainWavesLaunch* w, int pass, int sm_count, cudaStream_t s);
 
 // ---- lwse_sha1_kernels.cu ----
 int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,
-                int sm_count, cudaStream_t s, int* cuda_err);
+                int sm_count, cudaStream_t s);
 int launch_subgroup_keys(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, const int32_t* d_pod_count,
                          const int32_t* d_subgroup_size, const int32_t* d_worker_index, int32_t* d_index_out,
-                         uint8_t* d_digests, int sm_count, cudaStream_t s, int* cuda_err);
+                         uint8_t* d_digests, int sm_count, cudaStream_t s);
 
 // ---- lwse_exchange_kernels.cu ----
 int launch_exchange_push(const void* d_local_part, uint8_t* const* d_peer_base, void* d_local_base,
                          uint64_t part_bytes, uint64_t part_stride, uint64_t half_bytes, uint64_t flags_offset,
-                         uint64_t step, uint64_t wait_step, uint32_t world, uint32_t rank, cudaStream_t s, int* cuda_err,
+                         uint64_t step, uint64_t wait_step, uint32_t world, uint32_t rank, cudaStream_t s,
                          bool lagged);
 
 }  // namespace lwse

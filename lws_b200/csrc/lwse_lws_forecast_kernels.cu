@@ -209,18 +209,13 @@ static LwsForecastArgs forecast_args(const LwsForecastHost* h) {
                          h->slots, h->n_slots, h->fc,      h->steps, h->steps_rows, h->totals + 3};
 }
 
-// The private slot layout: slot_off and totals[2].  Returns the kernels launched, or -1.
-int launch_lws_forecast_slots(const LwsForecastHost* h, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+// The private slot layout: slot_off and totals[2].
+int launch_lws_forecast_slots(const LwsForecastHost* h, int sm_count, cudaStream_t s) {
   if (h->n_lws == 0) return 0;
   const uint32_t want = (h->n_lws + 255u) / 256u, cap = (uint32_t)sm_count * 8u;
   lws_forecast_slots_kernel<<<want < cap ? want : cap, 256, 0, s>>>(forecast_args(h), h->slot_off);
-  const cudaError_t e = launch_forecast_scan(SlotLayoutOp{h->slot_off}, h->n_lws, h->totals + 4, h->totals + 2, nullptr, s);
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 4;
+  launch_forecast_scan(SlotLayoutOp{h->slot_off}, h->n_lws, h->totals + 4, h->totals + 2, nullptr, s);
+  return launch_result(4);
 }
 
 template <int W, bool kWrite>
@@ -244,8 +239,7 @@ static void launch_replay(const LwsForecastArgs& a, int sm_count, cudaStream_t s
 
 // write_pass = false: the summary pass and the scan.  write_pass = true: the write pass into h->steps,
 // which holds the rows the scan counted as written.  Both on stream s.
-int launch_lws_forecast(const LwsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_lws_forecast(const LwsForecastHost* h, bool write_pass, int sm_count, cudaStream_t s) {
   if (h->n_lws == 0) return 0;
   const LwsForecastArgs a = forecast_args(h);
   int launched;
@@ -258,12 +252,7 @@ int launch_lws_forecast(const LwsForecastHost* h, bool write_pass, int sm_count,
                          h->n_lws, h->totals + 4, h->totals + 0, h->totals + 1, s);
     launched = 4;
   }
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return launched;
+  return launch_result(launched);
 }
 
 }  // namespace lwse

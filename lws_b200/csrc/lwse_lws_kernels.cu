@@ -162,18 +162,12 @@ __global__ void __launch_bounds__(256) ident_prefetch_kernel(const uint8_t* __re
 }
 
 int launch_ident_prefetch(const uint8_t* d_state, uint64_t n_pods, const lwse_pod_ident* mapped_host_ident,
-                          lwse_pod_ident* d_ident, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                          lwse_pod_ident* d_ident, int sm_count, cudaStream_t s) {
   if (n_pods == 0) return 0;
   const uint64_t want = (n_pods + 4095u) / 4096u;
   const uint32_t cap = (uint32_t)sm_count * 8u;
   ident_prefetch_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, s>>>(d_state, n_pods, mapped_host_ident, d_ident);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 // --------------------------------------------------------------------------
@@ -768,13 +762,12 @@ uint8_t* lws_sweep_flag_column(void* scratch, uint64_t n_pods) {
   return reinterpret_cast<uint8_t*>(static_cast<uint32_t*>(scratch) + 2 * bitmap_words(n_pods));
 }
 
-// Returns the number of kernels launched (>=0) or -1 with *cuda_err set.
 // scratch: lws_sweep_scratch_bytes(n_pods, n_groups) bytes of device memory.
 // first_pdl: the sweep's first kernel may start before the previous kernel on the stream has
 // finished (it reads only input tables before its griddepcontrol.wait) — false when that previous
 // kernel WRITES the input tables (the patch scatter of a tick).
 int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uint32_t n_nodes,
-                     void* scratch, int sm_count, cudaStream_t s, int* cuda_err, const SweepChangeLists* cl,
+                     void* scratch, int sm_count, cudaStream_t s, const SweepChangeLists* cl,
                      uint32_t* d_event_count, int first_mode) {
   // first_mode — how the sweep's FIRST kernel is launched:
   //   0  an ordinary launch (its predecessor is a copy, a memset, an event: nothing to overlap with)
@@ -787,7 +780,6 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
   // group rows: no group pass) mode 2 launches it as an ordinary launch.
   const bool first_pdl = first_mode == 1;
   const bool behind_writer = first_mode == 2;
-  *cuda_err = 0;
   int launches = 0;
   cudaError_t e = cudaSuccess;
   const uint64_t words = bitmap_words(t->n_pods);
@@ -806,13 +798,12 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
   const bool fused = group_pass && avg_pods <= 256 && avg_pods >= 16 && !(t->flags & LWSE_SWEEP_SKIP_POD_SCAN);
   if (t->node_occupancy && n_nodes && !(t->flags & LWSE_SWEEP_SKIP_POD_SCAN)) {
     e = cudaMemsetAsync(t->node_occupancy, 0, (size_t)n_nodes * sizeof(uint32_t), s);
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
     if (t->n_pods) {
       const uint64_t want = (t->n_pods + 255) / 256;
       const uint32_t cap = (uint32_t)sm_count * 16u;
       pod_occupancy_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, s>>>(t->pod_ident, t->n_pods, t->node_occupancy, n_nodes);
-      e = cudaGetLastError();
-      if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+      if (const int r = launch_result(0); r < 0) return r;
       launches++;
     }
   }
@@ -825,7 +816,7 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
     const bool pdl = !t->node_occupancy && first_mode != 0;
     if (pdl && first_mode == 2) a.sweep_flags |= kSweepWaitAtTop;
     e = launch_pdl(group_fused_kernel, dim3(grid), dim3(kFusedThreads), 0, s, pdl, a);
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
     launches++;
   }
   if (!fused && t->n_pods && t->n_groups && !(t->flags & LWSE_SWEEP_SKIP_POD_SCAN)) {
@@ -836,7 +827,7 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
     const uint64_t want = (chunks + 7) / 8;
     const uint32_t grid = (uint32_t)(want < (1u << 20) ? want : (1u << 20));
     e = launch_pdl(pod_scan_kernel<kScanUnroll>, dim3(grid), dim3(256), 0, s, first_pdl && !t->node_occupancy && !d_event_count, a);
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
     launches++;
   }
   if (group_pass && !fused) {
@@ -850,7 +841,7 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
       case 2: e = launch_group<2>(a, sm_count, s, pdl); break;
       default: e = launch_group<1>(a, sm_count, s, pdl); break;
     }
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
     launches++;
   }
   if (t->n_lws && !(t->flags & LWSE_SWEEP_SKIP_LWS_PASS)) {
@@ -865,7 +856,7 @@ int launch_lws_sweep(const lwse_lws_tables* t, const lwse_node_rec* d_nodes, uin
       case 16: e = launch_lws<16>(a, sm_count, s, pdl); break;
       default: e = launch_lws<32>(a, sm_count, s, pdl); break;
     }
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
     launches++;
   }
   return launches;
@@ -966,9 +957,8 @@ __global__ void __launch_bounds__(kPublishThreads) publish_lists_kernel(const Pu
 
 // lists[0..2]: the three slots (host_words[k] receives the count of slot k).
 int launch_publish(const PublishListHost* lists, const uint32_t* d_extra, uint32_t* h_words, uint32_t seq_slot,
-                   uint32_t seq, uint32_t* d_ticket, uint32_t expected_rows, cudaStream_t s, int* cuda_err,
+                   uint32_t seq, uint32_t* d_ticket, uint32_t expected_rows, cudaStream_t s,
                    uint32_t* d_clear, uint32_t n_clear, bool pdl) {
-  *cuda_err = 0;
   PublishArgs a{};
   for (int k = 0; k < 3; k++)
     a.list[k] = PublishList{lists[k].src_rows, static_cast<const uint4*>(lists[k].src_outs), lists[k].dst_rows,
@@ -984,10 +974,7 @@ int launch_publish(const PublishListHost* lists, const uint32_t* d_extra, uint32
   unsigned grid = expected_rows / 8192u + 1u;
   if (grid > 32u) grid = 32u;
   const cudaError_t e = launch_pdl(publish_lists_kernel, dim3(grid), dim3(kPublishThreads), 0, s, pdl, a);
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
+  if (e != cudaSuccess) return -(int)e;
   return 1;
 }
 
@@ -1117,50 +1104,36 @@ bool write_scatter_desc(void* h_desc, const ScatterSegHost* segs, int n_segs, ui
   memcpy(h_desc, &a, sizeof(a));
   return true;
 }
-int launch_scatter_desc(const void* d_desc, int sm_count, cudaStream_t s, bool pdl, int* cuda_err) {
-  *cuda_err = 0;
+int launch_scatter_desc(const void* d_desc, int sm_count, cudaStream_t s, bool pdl) {
   const cudaError_t e = launch_pdl(scatter_rows_desc_kernel, dim3((unsigned)sm_count * 4u), dim3(256), 0, s, pdl,
                                    static_cast<const ScatterArgs*>(d_desc));
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
+  if (e != cudaSuccess) return -(int)e;
   return 1;
 }
 
 int launch_scatter(const ScatterSegHost* segs, int n_segs, uint32_t* d_occupancy, uint32_t n_nodes, cudaStream_t s,
-                   bool pdl, int* cuda_err) {
-  *cuda_err = 0;
+                   bool pdl) {
   ScatterArgs a{};
-  if (!fill_scatter_args(segs, n_segs, d_occupancy, n_nodes, &a)) {
-    *cuda_err = (int)cudaErrorInvalidValue;
-    return -1;
-  }
+  if (!fill_scatter_args(segs, n_segs, d_occupancy, n_nodes, &a)) return -(int)cudaErrorInvalidValue;
   if (a.n_segs == 0) return 0;
   const uint64_t work = a.total_work;
   uint64_t grid = (work + 255) / 256;
   if (grid > (uint64_t)kSmCount * 16u) grid = (uint64_t)kSmCount * 16u;
   const cudaError_t e = launch_pdl(scatter_rows_kernel, dim3((unsigned)grid), dim3(256), 0, s, pdl, a);
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
+  if (e != cudaSuccess) return -(int)e;
   return 1;
 }
 
 // Scheduled pods per node of a resident identity column (at load).
 int launch_occupancy(const lwse_pod_ident* d_ident, uint64_t n_pods, uint32_t* d_occupancy, uint32_t n_nodes, int sm_count,
-                     cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                     cudaStream_t s) {
   cudaError_t e = cudaMemsetAsync(d_occupancy, 0, (size_t)n_nodes * 4, s);
-  if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+  if (e != cudaSuccess) return -(int)e;
   if (n_pods == 0) return 0;
   const uint64_t want = (n_pods + 255) / 256;
   const uint32_t cap = (uint32_t)sm_count * 16u;
   pod_occupancy_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, s>>>(d_ident, n_pods, d_occupancy, n_nodes);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
-  return 1;
+  return launch_result(1);
 }
 
 }  // namespace lwse

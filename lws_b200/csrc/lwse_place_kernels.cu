@@ -437,15 +437,11 @@ int launch_place(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, cons
                  const uint32_t* d_node_pos, uint32_t n_nodes, uint32_t n_domains, const lwse_place_req* d_reqs,
                  uint32_t n_reqs, const uint32_t* d_occupancy, uint32_t n_namespaces, lwse_place_out* d_out,
                  void* d_scratch, size_t scratch_bytes, uint32_t* h_rounds, int sm_count, cudaStream_t s,
-                 int* cuda_err, uint32_t call_index, bool fresh, uint32_t n_parts, uint32_t reqs_per_part,
-                 uint64_t part_stride_bytes, uint32_t* h_unpinned, const uint32_t** d_counters_out,
-                 const uint32_t** d_unpinned_out, bool after_push) {
-  *cuda_err = 0;
+                 uint32_t call_index, bool fresh, uint32_t n_parts, uint32_t reqs_per_part, uint64_t part_stride_bytes,
+                 uint32_t* h_unpinned, const uint32_t** d_counters_out, const uint32_t** d_unpinned_out, bool after_push) {
   if (n_reqs > 0xFFFFFFu || n_domains >= (1u << 28) ||
-      scratch_bytes < place_scratch_bytes(n_nodes, n_domains, n_reqs, n_namespaces)) {
-    *cuda_err = (int)cudaErrorInvalidValue;
-    return -1;
-  }
+      scratch_bytes < place_scratch_bytes(n_nodes, n_domains, n_reqs, n_namespaces))
+    return -(int)cudaErrorInvalidValue;
   const size_t half = place_half_bytes(n_nodes, n_domains, n_reqs, n_namespaces);
   const size_t holder_bytes = align_up((size_t)n_namespaces * hold_stride_of(n_domains) * 8, 256);
   const size_t zero_bytes = 256 + align_up((size_t)n_domains * 4 + 16, 256);
@@ -458,10 +454,7 @@ int launch_place(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, cons
       e = cudaMemsetAsync(base + h * half, 0xFF, holder_bytes, s);
       if (e == cudaSuccess) e = cudaMemsetAsync(base + h * half + holder_bytes, 0, zero_bytes, s);
     }
-    if (e != cudaSuccess) {
-      *cuda_err = (int)e;
-      return -1;
-    }
+    if (e != cudaSuccess) return -(int)e;
   }
   PlaceArgs a{};
   a.nodes = d_nodes;
@@ -559,17 +552,11 @@ int launch_place(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, cons
     void* params[] = {&a};
     e = cudaLaunchCooperativeKernel((const void*)place_kernel<false>, dim3(ctas), dim3(kPlaceThreads), params, 0, s);
   }
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
+  if (e != cudaSuccess) return -(int)e;
   if (h_rounds) {
     e = cudaMemcpyAsync(h_rounds, a.counters + 3, sizeof(uint32_t), cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) {
-      *cuda_err = (int)e;
-      return -1;
-    }
+    if (e != cudaSuccess) return -(int)e;
   }
   return 1;
 }
@@ -609,17 +596,13 @@ __global__ void __launch_bounds__(256) place_diff_kernel(const PlaceDiffArgs a) 
 }
 
 int launch_place_diff(const lwse_place_out* d_cur, lwse_place_out* d_prev, uint32_t n, uint32_t* d_rows,
-                      lwse_place_out* d_outs, uint32_t capacity, uint32_t* d_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                      lwse_place_out* d_outs, uint32_t capacity, uint32_t* d_count, cudaStream_t s) {
   PlaceDiffArgs a{d_cur, d_prev, n, d_rows, d_outs, capacity, d_count};
   unsigned grid = (n + 255u) / 256u;
   if (grid < 1u) grid = 1u;
   if (grid > (unsigned)kSmCount * 4u) grid = (unsigned)kSmCount * 4u;
   const cudaError_t e = launch_pdl(place_diff_kernel, dim3(grid), dim3(256), 0, s, true, a);
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
+  if (e != cudaSuccess) return -(int)e;
   return 1;
 }
 

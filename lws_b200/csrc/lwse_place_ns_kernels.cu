@@ -396,11 +396,10 @@ __global__ void __launch_bounds__(256) node_index_fill_kernel(const NodeIndexArg
 size_t node_index_scratch_bytes(uint32_t n_domains) { return (size_t)n_domains * 8u + 16u; }
 
 // count -> scan -> fill on `s`.  `scratch` (node_index_scratch_bytes) must be zero before the first build;
-// every build leaves it zero again.  `pdl`: the predecessor on `s` is a kernel.  Returns kernels launched or -1.
+// every build leaves it zero again.  `pdl`: the predecessor on `s` is a kernel.
 int launch_node_index(const lwse_node_rec* d_nodes, uint32_t n_nodes, uint32_t n_domains, uint32_t* d_dom_first,
                       uint32_t* d_node_order, uint32_t* d_node_pos, void* d_scratch, int sm_count, cudaStream_t s,
-                      bool pdl, int* cuda_err) {
-  *cuda_err = 0;
+                      bool pdl) {
   NodeIndexArgs a{};
   a.nodes = d_nodes;
   a.dom_count = static_cast<uint32_t*>(d_scratch);
@@ -418,10 +417,7 @@ int launch_node_index(const lwse_node_rec* d_nodes, uint32_t n_nodes, uint32_t n
     e = launch_pdl(place_index_scan_kernel, dim3(1), dim3(kIndexScanThreads), 0, s, true,
                    IndexScanArgs{a.dom_count, a.dom_first, a.dom_cursor, n_domains});
   if (e == cudaSuccess) e = launch_pdl(node_index_fill_kernel, dim3((unsigned)grid), dim3(256), 0, s, true, a);
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
+  if (e != cudaSuccess) return -(int)e;
   return 3;
 }
 
@@ -1098,19 +1094,15 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
                     uint32_t n_domains, const lwse_place_req* d_reqs, uint32_t n_reqs,
                     const uint32_t* d_occupancy, uint32_t n_parts, uint64_t part_stride_bytes, uint32_t n_namespaces,
                     lwse_place_out* d_out, void* d_scratch, size_t scratch_bytes, bool fresh, uint32_t call_index, bool scan,
-                    int sm_count, cudaStream_t s, int* cuda_err, const uint32_t** d_counters_out, bool first_pdl,
+                    int sm_count, cudaStream_t s, const uint32_t** d_counters_out, bool first_pdl,
                     const PlaceNsChanges* changes, const PlaceNsExchange* xch, PlaceNsIndex index) {
-  *cuda_err = 0;
   const NsLayout l = ns_layout(n_nodes, n_domains, n_reqs, n_namespaces);
-  if (scratch_bytes < l.total || n_reqs > 0xFFFFFFu) {
-    *cuda_err = (int)cudaErrorInvalidValue;
-    return -1;
-  }
+  if (scratch_bytes < l.total || n_reqs > 0xFFFFFFu) return -(int)cudaErrorInvalidValue;
   uint8_t* base = static_cast<uint8_t*>(d_scratch);
   cudaError_t e = cudaSuccess;
   if (fresh) {
     e = cudaMemsetAsync(base, 0, l.total, s);
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
   }
   PlaceNsArgs a{};
   a.nodes = d_nodes;
@@ -1192,7 +1184,7 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
       e = launch_pdl(place_index_scan_kernel, dim3(1), dim3(kIndexScanThreads), 0, s, true,
                      IndexScanArgs{a.ns_count, a.ns_first, a.ns_cursor, n_namespaces});
     if (e == cudaSuccess) e = launch_pdl(place_index_fill_kernel, dim3((unsigned)grid), dim3(256), 0, s, true, a);
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
     pdl = true;
     launched += 3;
   }
@@ -1203,10 +1195,10 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
     if (grid < 1) grid = 1;
     if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
     e = launch_pdl(place_condense_kernel, dim3((unsigned)grid), dim3(256), 0, s, pdl, a);
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
     if (changes && changes->mid_event) {
       e = cudaEventRecord(static_cast<cudaEvent_t>(changes->mid_event), s);
-      if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+      if (e != cudaSuccess) return -(int)e;
     }
   }
   {
@@ -1219,11 +1211,11 @@ int launch_place_ns(const lwse_node_rec* d_nodes, const uint32_t* d_dom_first, c
     static thread_local size_t attr_set[4] = {0, 0, 0, 0};
     if (smem > attr_set[variant]) {
       e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+      if (e != cudaSuccess) return -(int)e;
       attr_set[variant] = smem;
     }
     e = launch_pdl(kern, dim3(grid), dim3(scan ? kNsScanThreads : kNsThreads), smem, s, true, a, map);
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
   }
   return launched;
 }
@@ -1274,10 +1266,9 @@ __global__ void __launch_bounds__(256) place_whatif_fill_kernel(const WhatIfInde
 }
 
 // The masked namespace index in the namespace-form scratch `d_scratch` (laid out as launch_place_ns
-// lays it out for the same geometry; ns_count zero before, and again after).  Returns kernels launched or -1.
+// lays it out for the same geometry; ns_count zero before, and again after).
 int launch_place_whatif_index(const lwse_place_req* d_reqs, uint32_t n_reqs, uint32_t n_namespaces, const uint8_t* d_touched,
-                              uint32_t n_nodes, uint32_t n_domains, void* d_scratch, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                              uint32_t n_nodes, uint32_t n_domains, void* d_scratch, int sm_count, cudaStream_t s) {
   const NsLayout l = ns_layout(n_nodes, n_domains, n_reqs, n_namespaces);
   uint8_t* base = static_cast<uint8_t*>(d_scratch);
   WhatIfIndexArgs a{};
@@ -1292,21 +1283,12 @@ int launch_place_whatif_index(const lwse_place_req* d_reqs, uint32_t n_reqs, uin
   if (grid < 1) grid = 1;
   if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
   place_whatif_count_kernel<<<(unsigned)grid, 256, 0, s>>>(a);
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) {
-    place_index_scan_kernel<<<1, kIndexScanThreads, 0, s>>>(
-        IndexScanArgs{a.ns_count, reinterpret_cast<uint32_t*>(base + l.ns_first), a.ns_cursor, n_namespaces});
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) {
-    place_whatif_fill_kernel<<<(unsigned)grid, 256, 0, s>>>(a);
-    e = cudaGetLastError();
-  }
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 3;
+  if (const int r = launch_result(0); r < 0) return r;
+  place_index_scan_kernel<<<1, kIndexScanThreads, 0, s>>>(
+      IndexScanArgs{a.ns_count, reinterpret_cast<uint32_t*>(base + l.ns_first), a.ns_cursor, n_namespaces});
+  if (const int r = launch_result(0); r < 0) return r;
+  place_whatif_fill_kernel<<<(unsigned)grid, 256, 0, s>>>(a);
+  return launch_result(3);
 }
 
 // request row -> its position in the namespace index (rows of no namespace keep the caller's LWSE_NONE)
@@ -1320,13 +1302,9 @@ __global__ void __launch_bounds__(256) drain_place_pos_kernel(const uint32_t* ns
 // condense kernel's part A alone: n_reqs = 0 leaves the request rows and the index alone), then the drain
 // instance over p->grid CTAs.  The round scratch holds the namespace index of every namespace
 // (launch_place_whatif_index with every namespace touched).
-int launch_place_ns_drain(const DrainPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_place_ns_drain(const DrainPlaceLaunch* p, int sm_count, cudaStream_t s) {
   const NsLayout l = ns_layout(p->n_nodes, p->n_domains, p->n_reqs, p->n_namespaces);
-  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) {
-    *cuda_err = (int)cudaErrorInvalidValue;
-    return -1;
-  }
+  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) return -(int)cudaErrorInvalidValue;
   uint8_t* base = static_cast<uint8_t*>(p->round);
   PlaceNsArgs a{};
   a.nodes = p->nodes;
@@ -1356,8 +1334,7 @@ int launch_place_ns_drain(const DrainPlaceLaunch* p, int sm_count, cudaStream_t 
     if (grid < 1) grid = 1;
     if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
     drain_place_pos_kernel<<<(unsigned)grid, 256, 0, s>>>(a.ns_first, a.ns_rows, p->n_namespaces, p->pos);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (const int r = launch_result(0); r < 0) return r;
   }
   DrainNsView v{};
   v.items = p->items;
@@ -1379,30 +1356,23 @@ int launch_place_ns_drain(const DrainPlaceLaunch* p, int sm_count, cudaStream_t 
   a.n_reqs = p->n_reqs;
   a.out = p->s_out;
   a.unpinned = p->s_unpinned;
-  cudaError_t e = cudaSuccess;
   const size_t smem = ns_smem_bytes(l.word_rows, p->n_domains, false, false);
   static thread_local size_t attr_set = 0;
   if (smem > attr_set) {
-    e = cudaFuncSetAttribute(place_ns_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    const cudaError_t e = cudaFuncSetAttribute(place_ns_kernel<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return -(int)e;
     attr_set = smem;
   }
   place_ns_kernel<false, true, true><<<p->grid, kNsThreads, smem, s>>>(a, view);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
-  return 3;
+  return launch_result(3);
 }
 
 // The set-overlay solve of one drain placement waves step: the capacities and positions are those the drain
 // placement's solve left (launch_place_ns_drain ran at setup); a persistent grid over the step's items.
-int launch_place_ns_drain_set(const DrainPlaceWavesLaunch* d, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_place_ns_drain_set(const DrainPlaceWavesLaunch* d, int sm_count, cudaStream_t s) {
   const DrainPlaceLaunch* p = &d->p;
   const NsLayout l = ns_layout(p->n_nodes, p->n_domains, p->n_reqs, p->n_namespaces);
-  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) {
-    *cuda_err = (int)cudaErrorInvalidValue;
-    return -1;
-  }
+  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) return -(int)cudaErrorInvalidValue;
   uint8_t* base = static_cast<uint8_t*>(p->round);
   PlaceNsArgs a{};
   a.nodes = p->nodes;
@@ -1449,13 +1419,11 @@ int launch_place_ns_drain_set(const DrainPlaceWavesLaunch* d, int sm_count, cuda
   static thread_local size_t attr_set = 0;
   if (smem > attr_set) {
     const cudaError_t e = cudaFuncSetAttribute(place_ns_kernel<false, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
     attr_set = smem;
   }
   place_ns_kernel<false, true, true, true><<<p->grid, kNsThreads, smem, s>>>(a, view);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
-  return 1;
+  return launch_result(1);
 }
 
 // The rollout instances' arguments over the round scratch, which holds the namespace index of every namespace.
@@ -1499,21 +1467,16 @@ static RollNsView rollout_ns_view(const RolloutPlaceLaunch* p) {
 
 // The rollout placement solve: the capacities of the node index (the condense kernel's part A alone), then the
 // rollout instance over p->grid CTAs.  The round scratch holds the namespace index of every namespace.
-int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStream_t s) {
   const NsLayout l = ns_layout(p->n_nodes, p->n_domains, p->n_reqs, p->n_namespaces);
-  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) {
-    *cuda_err = (int)cudaErrorInvalidValue;
-    return -1;
-  }
+  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) return -(int)cudaErrorInvalidValue;
   PlaceNsArgs a = rollout_ns_args(p, l);
   {
     uint64_t grid = ((uint64_t)p->n_domains * 32u + 255) / 256;
     if (grid < 1) grid = 1;
     if (grid > (uint64_t)sm_count * 8u) grid = (uint64_t)sm_count * 8u;
     place_condense_kernel<<<(unsigned)grid, 256, 0, s>>>(a);  // (a.n_reqs = 0: capacities only)
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (const int r = launch_result(0); r < 0) return r;
   }
   const RollNsView v = rollout_ns_view(p);
   CUtensorMap view;
@@ -1527,25 +1490,19 @@ int launch_place_ns_rollout(const RolloutPlaceLaunch* p, int sm_count, cudaStrea
   if (smem > attr_set) {
     const cudaError_t e =
         cudaFuncSetAttribute(place_ns_kernel<false, true, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
     attr_set = smem;
   }
   place_ns_kernel<false, true, true, false, true><<<p->grid, kNsThreads, smem, s>>>(a, view);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
-  return 2;
+  return launch_result(2);
 }
 
 // One round's solve of the rollout waves: the wave instance over w->grid CTAs, on the capacities and the namespace
 // index the setup's rollout solve left in the round scratch.
-int launch_place_ns_rollout_wave(const RolloutPlaceWavesLaunch* w, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_place_ns_rollout_wave(const RolloutPlaceWavesLaunch* w, cudaStream_t s) {
   const RolloutPlaceLaunch* p = &w->p;
   const NsLayout l = ns_layout(p->n_nodes, p->n_domains, p->n_reqs, p->n_namespaces);
-  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) {
-    *cuda_err = (int)cudaErrorInvalidValue;
-    return -1;
-  }
+  if (p->round_bytes < l.total || p->n_reqs > 0xFFFFFFu) return -(int)cudaErrorInvalidValue;
   PlaceNsArgs a = rollout_ns_args(p, l);
   RollWaveNsView v{};
   v.r = rollout_ns_view(p);
@@ -1566,24 +1523,16 @@ int launch_place_ns_rollout_wave(const RolloutPlaceWavesLaunch* w, cudaStream_t 
   if (smem > attr_set) {
     const cudaError_t e = cudaFuncSetAttribute(place_ns_kernel<false, true, true, false, true, true>,
                                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
+    if (e != cudaSuccess) return -(int)e;
     attr_set = smem;
   }
   place_ns_kernel<false, true, true, false, true, true><<<w->grid, kNsThreads, smem, s>>>(a, view);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) { *cuda_err = (int)e; return -1; }
-  return 1;
+  return launch_result(1);
 }
 
-int launch_index_scan(uint32_t* d_count, uint32_t* d_first, uint32_t* d_cursor, uint32_t n, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_index_scan(uint32_t* d_count, uint32_t* d_first, uint32_t* d_cursor, uint32_t n, cudaStream_t s) {
   place_index_scan_kernel<<<1, kIndexScanThreads, 0, s>>>(IndexScanArgs{d_count, d_first, d_cursor, n});
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 // The what-if's diff against the baseline and its counts.  counts: [0] changed rows [1] lost [2] moved
@@ -1641,19 +1590,13 @@ __global__ void __launch_bounds__(256) place_whatif_diff_kernel(const WhatIfDiff
 
 int launch_place_whatif_diff(const lwse_place_out* d_before, const lwse_place_out* d_after, uint32_t n_resident, uint32_t n_total,
                              uint32_t* d_rows, lwse_place_out* d_outs_before, lwse_place_out* d_outs_after, uint32_t capacity,
-                             uint32_t* d_counts, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                             uint32_t* d_counts, int sm_count, cudaStream_t s) {
   const WhatIfDiffArgs a{d_before, d_after, d_rows, d_outs_before, d_outs_after, d_counts, capacity, n_resident, n_total};
   uint64_t grid = ((uint64_t)n_total + 255) / 256;
   if (grid < 1) grid = 1;
   if (grid > (uint64_t)sm_count * 4u) grid = (uint64_t)sm_count * 4u;
   place_whatif_diff_kernel<<<(unsigned)grid, 256, 0, s>>>(a);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 }  // namespace lwse

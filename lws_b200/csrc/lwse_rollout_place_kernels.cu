@@ -132,32 +132,23 @@ __global__ void __launch_bounds__(256) rollout_place_finish_kernel(const Rollout
   }
 }
 
-int launch_rollout_place(const RolloutPlaceLaunch* p, int pass, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
-  auto fail = [&]() -> int {
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) *cuda_err = (int)e;
-    return e == cudaSuccess ? 0 : -1;
-  };
+int launch_rollout_place(const RolloutPlaceLaunch* p, int pass, int sm_count, cudaStream_t s) {
   if (pass == 0) {
     rollout_place_count_kernel<<<warp_grid(p->n, sm_count), 256, 0, s>>>(*p);
-    return fail() < 0 ? -1 : 1;
+    return launch_result(1);
   }
   int n = 0;
-  if (launch_index_scan(p->e_count, p->e_first, p->e_cursor, p->n, s, cuda_err) < 0) return -1;
+  if (const int r = launch_index_scan(p->e_count, p->e_first, p->e_cursor, p->n, s); r < 0) return r;
   rollout_place_fill_kernel<<<warp_grid(p->n, sm_count), 256, 0, s>>>(*p);
-  if (fail() < 0) return -1;
+  if (const int r = launch_result(0); r < 0) return r;
   n = 2;
   if (p->grid) {
-    const int solved = launch_place_ns_rollout(p, sm_count, s, cuda_err);
-    if (solved < 0) return -1;
+    const int solved = launch_place_ns_rollout(p, sm_count, s);
+    if (solved < 0) return solved;
     n += solved;
   }
-  uint64_t grid = ((uint64_t)p->n + 255) / 256;
-  if (grid < 1) grid = 1;
-  if (grid > (uint64_t)sm_count * 4u) grid = (uint64_t)sm_count * 4u;
-  rollout_place_finish_kernel<<<(unsigned)grid, 256, 0, s>>>(*p);
-  return fail() < 0 ? -1 : n + 1;
+  rollout_place_finish_kernel<<<grid_for(p->n, 256, (uint32_t)sm_count * 4u), 256, 0, s>>>(*p);
+  return launch_result(n + 1);
 }
 
 }  // namespace lwse

@@ -186,39 +186,28 @@ __global__ void __launch_bounds__(1024) rollout_waves_finish_kernel(const Rollou
   }
 }
 
-int launch_rollout_place_waves(const RolloutPlaceWavesLaunch* w, int pass, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
-  auto fail = [&]() -> int {
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) *cuda_err = (int)e;
-    return e == cudaSuccess ? 0 : -1;
-  };
-  auto grid_of = [&](uint64_t n) -> unsigned {
-    uint64_t g = (n + 255) / 256;
-    if (g < 1) g = 1;
-    if (g > (uint64_t)sm_count * 4u) g = (uint64_t)sm_count * 4u;
-    return (unsigned)g;
-  };
+int launch_rollout_place_waves(const RolloutPlaceWavesLaunch* w, int pass, int sm_count, cudaStream_t s) {
+  const unsigned grid = grid_for(w->p.n, 256, (uint32_t)sm_count * 4u);
   if (pass == 0) {
     rollout_waves_rank_kernel<<<1, 1024, 0, s>>>(*w);
-    if (fail() < 0) return -1;
-    if (launch_index_scan(w->ns_count, w->ns_first, w->ns_cursor, w->p.n_namespaces, s, cuda_err) < 0) return -1;
-    rollout_waves_fill_kernel<<<grid_of(w->p.n), 256, 0, s>>>(*w);
-    return fail() < 0 ? -1 : 3;
+    if (const int r = launch_result(0); r < 0) return r;
+    if (const int r = launch_index_scan(w->ns_count, w->ns_first, w->ns_cursor, w->p.n_namespaces, s); r < 0) return r;
+    rollout_waves_fill_kernel<<<grid, 256, 0, s>>>(*w);
+    return launch_result(3);
   }
   if (pass == 1) {
-    rollout_waves_items_kernel<<<grid_of(w->p.n), 256, 0, s>>>(*w);
-    if (fail() < 0) return -1;
+    rollout_waves_items_kernel<<<grid, 256, 0, s>>>(*w);
+    if (const int r = launch_result(0); r < 0) return r;
     int n = 1;
     if (w->grid) {
-      if (launch_place_ns_rollout_wave(w, s, cuda_err) < 0) return -1;
+      if (const int r = launch_place_ns_rollout_wave(w, s); r < 0) return r;
       n++;
     }
     rollout_waves_commit_kernel<<<1, 1024, 0, s>>>(*w);
-    return fail() < 0 ? -1 : n + 1;
+    return launch_result(n + 1);
   }
   rollout_waves_finish_kernel<<<1, 1024, 0, s>>>(*w);
-  return fail() < 0 ? -1 : 1;
+  return launch_result(1);
 }
 
 }  // namespace lwse

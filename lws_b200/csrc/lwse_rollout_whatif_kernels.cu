@@ -80,42 +80,24 @@ __global__ void __launch_bounds__(256) rollout_whatif_restore_kernel(const uint3
 }
 
 int launch_rollout_whatif_layout(const RolloutWhatifHost* h, unsigned long long* sums, unsigned long long* total,
-                                 cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
-  const cudaError_t e = launch_forecast_scan(WhatifLayoutOp{h->lws, h->rows, h->n_groups, h->off}, h->n, sums, total,
-                                             nullptr, s);
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return h->n ? 3 : 1;
+                                 cudaStream_t s) {
+  launch_forecast_scan(WhatifLayoutOp{h->lws, h->rows, h->n_groups, h->off}, h->n, sums, total, nullptr, s);
+  return launch_result(h->n ? 3 : 1);
 }
 
-int launch_rollout_whatif_gather(const RolloutWhatifHost* h, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+int launch_rollout_whatif_gather(const RolloutWhatifHost* h, int sm_count, cudaStream_t s) {
   if (h->n == 0) return 0;
   const uint32_t want = (h->n + 7u) / 8u, cap = (uint32_t)sm_count * 8u;
   rollout_whatif_gather_kernel<<<want < cap ? want : cap, 256, 0, s>>>(*h);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 int launch_rollout_whatif_restore(const uint32_t* d_src, const lwse_group_out* d_baseline, lwse_group_out* d_out,
-                                  uint8_t* d_gflag8, uint32_t n_rows, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+                                  uint8_t* d_gflag8, uint32_t n_rows, int sm_count, cudaStream_t s) {
   if (n_rows == 0) return 0;
   const uint32_t want = (n_rows + 255u) / 256u, cap = (uint32_t)sm_count * 8u;
   rollout_whatif_restore_kernel<<<want < cap ? want : cap, 256, 0, s>>>(d_src, d_baseline, d_out, d_gflag8, n_rows);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 }  // namespace lwse

@@ -179,8 +179,7 @@ __global__ void __launch_bounds__(kShaWarps * 32) sha1_kernel(const Sha1Args a) 
   }
 }
 
-static int launch_sha1_form(const Sha1Args& a, bool subgroup, int sm_count, cudaStream_t s, int* cuda_err) {
-  *cuda_err = 0;
+static int launch_sha1_form(const Sha1Args& a, bool subgroup, int sm_count, cudaStream_t s) {
   if (a.n == 0) return 0;
   const uint32_t want = (a.n + kShaWarps * 32u - 1u) / (kShaWarps * 32u);
   const uint32_t cap = (uint32_t)sm_count * 16u;
@@ -189,25 +188,20 @@ static int launch_sha1_form(const Sha1Args& a, bool subgroup, int sm_count, cuda
     sha1_kernel<true><<<grid, kShaWarps * 32, 0, s>>>(a);
   else
     sha1_kernel<false><<<grid, kShaWarps * 32, 0, s>>>(a);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    *cuda_err = (int)e;
-    return -1;
-  }
-  return 1;
+  return launch_result(1);
 }
 
 int launch_sha1(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, uint8_t* d_digests,
-                int sm_count, cudaStream_t s, int* cuda_err) {
+                int sm_count, cudaStream_t s) {
   Sha1Args a{d_bytes, d_offsets, n, d_digests, nullptr, nullptr, nullptr, nullptr};
-  return launch_sha1_form(a, false, sm_count, s, cuda_err);
+  return launch_sha1_form(a, false, sm_count, s);
 }
 
 int launch_subgroup_keys(const uint8_t* d_bytes, const uint32_t* d_offsets, uint32_t n, const int32_t* d_pod_count,
                          const int32_t* d_subgroup_size, const int32_t* d_worker_index, int32_t* d_index_out,
-                         uint8_t* d_digests, int sm_count, cudaStream_t s, int* cuda_err) {
+                         uint8_t* d_digests, int sm_count, cudaStream_t s) {
   Sha1Args a{d_bytes, d_offsets, n, d_digests, d_pod_count, d_subgroup_size, d_worker_index, d_index_out};
-  return launch_sha1_form(a, true, sm_count, s, cuda_err);
+  return launch_sha1_form(a, true, sm_count, s);
 }
 
 }  // namespace lwse
