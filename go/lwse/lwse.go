@@ -227,6 +227,15 @@ func (e *Engine) RolloutPlaceWaves(q *C.lwse_rollout_place_waves_query) error {
 	return e.check(C.lwse_resident_rollout_place_waves(e.h, q))
 }
 
+// ScaleHeadroom answers "how many replicas can this object go to right now?" for a list of settled exclusive
+// LeaderWorkerSets in one call: per entry the largest replicas (up to an optional ceiling, such as the HPA's
+// maxReplicas) at which every group the scale-up adds still finds an exclusive domain, and the counters of the
+// first replicas that does not.  An autoscaler clamps its desired replicas to max_replicas before it writes the
+// scale subresource, so that no group it adds stays Pending.
+func (e *Engine) ScaleHeadroom(q *C.lwse_scale_headroom_query) error {
+	return e.check(C.lwse_resident_scale_headroom(e.h, q))
+}
+
 // DrainWaves packs distinct node rows (scope LWSE_DRAIN_NODES) or domain ids (LWSE_DRAIN_DOMAINS), in the order
 // given, first-fit into at most q.max_waves waves whose drain takes no LeaderWorkerSet below its floor.  A
 // maintenance controller drains wave 0, waits for recovery and calls again with the keys that remain.

@@ -1404,6 +1404,91 @@ typedef struct lwse_rollout_place_waves_query {
 } lwse_rollout_place_waves_query;
 LWSE_API int lwse_resident_rollout_place_waves(lwse_engine* e, lwse_rollout_place_waves_query* q);
 
+/* ---- scale headroom -----------------------------------------------------------------------------
+ * "How many replicas can this object go to right now before a group it adds finds no exclusive domain?" — the
+ * capacity question of an autoscaler (the HPA behind the LeaderWorkerSet scale subresource), for a list of exclusive
+ * LeaderWorkerSets in one call (DESIGN.md §3.5, "Scale headroom").
+ *
+ * Definition.  Entry i names a resident LWS row L_i, a namespace id ns_i < the resident n_namespaces and, with
+ * `ceilings`, a ceiling c_i (negative: none).  Entries are answered each on its own, as lwse_resident_rollout_place
+ * answers them; rows may repeat.  r0 = L_i.replicas.
+ *   1. P_i(R) is L_i with replicas := R and every other field unchanged (a scale-only edit).
+ *   2. E_i(R) holds, ascending, every group index g in [0, R) with g >= group_count, or whose group row lacks
+ *      LWSE_GRP_POD_PRESENT; row j is built as lwse_resident_rollout_place builds its row j (the encoder's mix of
+ *      (uid_hash, g), row index and key rn_reqs + j).
+ *   3. R is clean when lwse_resident_place_whatif with no segments and extra = E_i(R), diffed against the baseline,
+ *      triggers none of `constraints`: LWSE_RPW_STRANDED (always required: some extra row is not PLACED after) and,
+ *      opt-in, LWSE_RPW_BUMPED (some resident row PLACED before is not PLACED after, own_lost or bumped).
+ *   4. An entry is answered (LWSE_SHR_SOLVED) only when L_i is settled: exclusive (else NOT_EXCLUSIVE); its resident
+ *      forecast row without BAD_TABLE / NOT_FORECAST (else NOT_FORECAST); and (else NOT_SETTLED) LWSE_LWS_STS_EXISTS
+ *      without LWSE_LWS_UPDATED, sts_replicas == replicas, sts_partition == 0, partition == 0, a forecast row
+ *      without ROLLING / UNFINISHED / HELD and with peak_sts_replicas == final_replicas == replicas.  On a settled
+ *      row a scale-only edit to R >= r0 is Case 3 of rollingUpdateParameters: the rollout what-if's forecast of
+ *      P_i(R) has peak R, so E_i(R) is lwse_resident_rollout_place's E for the proposal P_i(R).  (With a held
+ *      partition the surge of calculateLWSUnreadyReplicas can lift the StatefulSet above R; hence the partition
+ *      clauses.)
+ *   5. R_pig is the smallest R with |E_i(R)| = n_domains + 1: each placed extra row holds a distinct (ns_i, domain)
+ *      pair, so R_pig always strands.  C_i = min(c_i, R_pig - 1).  max_replicas is the largest R in [r0, C_i]
+ *      that is clean (r0 when c_i <= r0 and r0 is clean), or -1 with LWSE_SHR_BLOCKED when r0 itself triggers.
+ *   6. The clean R form an interval [r0, H] (DESIGN.md §3.5), so the device bisects (r0, C_i]: exact, in
+ *      ceil(log2(C_i + 1 - r0)) rounds, plus one for the entries whose bisection ends below R_pig without probing it.
+ * The row carries lwse_resident_rollout_place's counters at `probe`: H + 1, the first R that triggers (r0 when
+ * BLOCKED); with LWSE_SHR_AT_CEILING (max_replicas = c_i, or r0 for a ceiling <= r0) at H itself.  STRANDS / BUMPS
+ * are the verdicts of that probe, whatever `constraints` holds.  An entry that is not solved has max_replicas and
+ * probe -1 and zero counters.
+ *
+ * Readiness, isolation and errors are lwse_resident_rollout_place's (the mutex; the what-if stream behind one event on
+ * the engine's stream; a tick in flight is neither waited on nor touched), and: LWSE_ERR_INVALID_ARG for a
+ * `constraints` without LWSE_RPW_STRANDED or with an unknown bit, a nonzero reserved field, a NULL out (n > 0);
+ * LWSE_ERR_UNSUPPORTED on an engine with a peer exchange, when rn_reqs + max |E| reaches 2^24 and where the namespace
+ * form does not fit the domains.  A refused call writes nothing.  n = 0 is a valid empty answer. */
+typedef struct lwse_scale_headroom { /* 64 B */
+  uint32_t flags;            /* LWSE_SHR_*                                                              */
+  int32_t replicas;          /* r0                                                                      */
+  int32_t max_replicas;      /* H, or -1                                                                */
+  int32_t probe;             /* the R whose counters follow, or -1                                      */
+  uint32_t surge;            /* lwse_rollout_place's counters of P_i(probe): |E_i(probe)|               */
+  uint32_t placed;
+  uint32_t stranded;
+  uint32_t own_lost;
+  uint32_t bumped;
+  uint32_t n_changed;
+  uint32_t n_lost;
+  uint32_t n_moved;
+  uint32_t n_gained;
+  uint32_t n_placed;
+  uint32_t n_unschedulable;
+  uint32_t n_conflict;
+} lwse_scale_headroom;
+
+#define LWSE_SHR_SOLVED (1u << 0)        /* answered                                                      */
+#define LWSE_SHR_NOT_EXCLUSIVE (1u << 1) /* L_i lacks LWSE_LWS_EXCLUSIVE_TOPOLOGY                          */
+#define LWSE_SHR_NOT_FORECAST (1u << 2)  /* its forecast row has BAD_TABLE or NOT_FORECAST                 */
+#define LWSE_SHR_NOT_SETTLED (1u << 3)   /* a rollout, a scale or a partition is in progress or held       */
+#define LWSE_SHR_BLOCKED (1u << 4)       /* r0 itself triggers: max_replicas = -1                          */
+#define LWSE_SHR_AT_CEILING (1u << 5)    /* max_replicas is the ceiling (or r0 for a ceiling <= r0)        */
+#define LWSE_SHR_STRANDS (1u << 6)       /* the probe strands an extra row                                 */
+#define LWSE_SHR_BUMPS (1u << 7)         /* the probe takes a resident row's domain (own_lost or bumped)   */
+
+typedef struct lwse_scale_headroom_query {
+  const uint32_t* rows;         /* [n] resident LWS rows                                                */
+  const uint32_t* ns;           /* [n] namespace ids                                                    */
+  const int32_t* ceilings;      /* [n] c_i (negative: none), or NULL: none                              */
+  uint32_t n;
+  uint32_t constraints;         /* LWSE_RPW_STRANDED, optionally | LWSE_RPW_BUMPED                      */
+  uint32_t reserved;            /* 0                                                                    */
+  uint32_t reserved1;           /* 0                                                                    */
+  lwse_scale_headroom* out;     /* [n] out, host memory                                                 */
+  lwse_rollout_place* current;  /* [n] out, or NULL: lwse_resident_rollout_place's rows of the resident rows */
+  /* out */
+  uint32_t n_solved;            /* entries with LWSE_SHR_SOLVED                                         */
+  uint32_t n_blocked;
+  uint32_t n_at_ceiling;
+  uint32_t rounds;              /* bisection rounds the call ran (the final probe included)             */
+  uint64_t headroom;            /* sum of max_replicas - r0 over the SOLVED entries that are not BLOCKED */
+} lwse_scale_headroom_query;
+LWSE_API int lwse_resident_scale_headroom(lwse_engine* e, lwse_scale_headroom_query* q);
+
 /* ------------------------------------------------------------------------- */
 /* Peer exchange: the multi-GPU placement step without a collective library  */
 /* ------------------------------------------------------------------------- */

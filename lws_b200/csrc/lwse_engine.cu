@@ -342,6 +342,10 @@ struct lwse_engine {
   // state, the column lists, the round's slices, the answer; the answer going back (host)
   DevBuf rq_state, rq_ns, rq_keys, rq_slots, rq_col, rq_slices, rq_out;
   PinBuf rq_host;
+  // scale headroom (lwse_resident_scale_headroom): the ceilings, the bounds per entry, the current / clean /
+  // triggering rows, the answer (its totals first, the setup's words after the rows); the answer going back (host)
+  DevBuf sh_ceil, sh_state, sh_rows, sh_out;
+  PinBuf sh_host;
   // drain waves (lwse_resident_drain_waves): the drain budget's key rows, the counters, the ids, the key positions, the
   // key buckets (count | first | cursor), the restart pairs, the pair records, the touched-row index (count | first |
   // cursor), the dense rows, the lost counters, the group and row wave masks, the stamps, the answer; the ids going
@@ -4335,9 +4339,10 @@ LWSE_API int lwse_resident_rollout_whatif(lwse_engine* e, lwse_rollout_whatif* q
 // The chain's first part, on wf_stream behind one event on the engine's stream: the scratch sized by n and the
 // resident tables, the forecast (the resident forecast's snapshot, or the rollout what-if's chain over the
 // proposals), then the count kernel, read back at one synchronisation into words[0..3] (the items, max |E_i| and
-// sum |E_i|, which size the slices and decide the 24-bit refusal).
+// sum |E_i|, which size the slices and decide the 24-bit refusal).  Without read_back the copy is enqueued and the
+// caller synchronises, after work of its own.
 static int rollout_place_count(lwse_engine* e, const uint32_t* rows, const uint32_t* ns, const lwse_lws_rec* recs, uint32_t n,
-                               lwse::RolloutPlaceLaunch* p) {
+                               lwse::RolloutPlaceLaunch* p, bool read_back = true) {
   const uint32_t nn = e->n_nodes, nd = e->n_domains, nr = e->rn_reqs, n_ns = e->rn_namespaces;
   const bool proposals = recs != nullptr;
   LWSE_CUDA(e, e->wf_words.reserve(128));
@@ -4391,7 +4396,7 @@ static int rollout_place_count(lwse_engine* e, const uint32_t* rows, const uint3
   p->counts = d_words;
   LWSE_LAUNCH(e, lwse::launch_rollout_place(p, 0, e->sm_count, s));
   LWSE_CUDA(e, cudaMemcpyAsync(words, d_words, 16, cudaMemcpyDeviceToHost, s));
-  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  if (read_back) LWSE_CUDA(e, cudaStreamSynchronize(s));
   return LWSE_OK;
 }
 
@@ -4612,6 +4617,97 @@ LWSE_API int lwse_resident_rollout_place_waves(lwse_engine* e, lwse_rollout_plac
   q->n_triggers_alone = tot[2];
   q->n_no_wave = tot[3];
   q->n_not_solved = tot[4];
+  return LWSE_OK;
+}
+
+// ---- scale headroom ----
+// Setup: the rollout placement's count on the resident rows and the setup kernel, read back at one synchronisation
+// (the entries that search, the largest |E| and the per-round sum of |E| size the slices, the grid and the extra
+// rows; the probe at r0 would size none for a settled object with all its pods), then the rollout placement's
+// solve, whose rows are the probes at r0 (the current rows), copied aside.  Then one captured round, replayed with
+// the bounds in device memory (no host synchronisation per round), the finish, and one copy back.
+LWSE_API int lwse_resident_scale_headroom(lwse_engine* e, lwse_scale_headroom_query* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  const uint32_t n = q->n;
+  if (const int rc = rollout_place_check(e, q->rows, q->ns, nullptr, n); rc != LWSE_OK) return rc;
+  if ((n && !q->out) || q->reserved || q->reserved1) return LWSE_ERR_INVALID_ARG;
+  if (!(q->constraints & LWSE_RPW_STRANDED) || (q->constraints & ~LWSE_RPW_ALL)) return LWSE_ERR_INVALID_ARG;
+  if (e->xch_world > 0 || e->rn_reqs >= (1u << 24) || !lwse::place_ns_supported(e->n_nodes, e->n_domains))
+    return LWSE_ERR_UNSUPPORTED;
+  if (n == 0) {
+    q->n_solved = q->n_blocked = q->n_at_ceiling = q->rounds = 0;
+    q->headroom = 0;
+    return LWSE_OK;
+  }
+  const uint32_t nr = e->rn_reqs;
+  const size_t row_bytes = (size_t)n * 64, out_bytes = 32 + row_bytes;
+  DeviceGuard guard(e->device);
+  LWSE_CUDA(e, e->sh_ceil.reserve((size_t)n * 4 + 16));
+  LWSE_CUDA(e, e->sh_state.reserve((size_t)n * 16 + 16));
+  LWSE_CUDA(e, e->sh_rows.reserve(row_bytes * 3 + 16));
+  LWSE_CUDA(e, e->sh_out.reserve(out_bytes + 32 + 16));
+  LWSE_CUDA(e, e->sh_host.reserve(out_bytes + 16));
+  lwse::ScaleHeadroomLaunch h{};
+  lwse::RolloutPlaceLaunch& p = h.p;
+  if (const int rc = rollout_place_count(e, q->rows, q->ns, nullptr, n, &p, /*read_back=*/false); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  uint32_t* words = static_cast<uint32_t*>(e->wf_words.h);
+  h.constraints = q->constraints;
+  h.n_domains = e->n_domains;
+  h.st = (uint4*)e->sh_state.p;
+  h.cur = (const uint32_t*)e->sh_rows.p;
+  h.clean = (uint32_t*)e->sh_rows.p + (size_t)n * 16;
+  h.trig = h.clean + (size_t)n * 16;
+  h.out = (uint32_t*)e->sh_out.p;
+  h.words = h.out + out_bytes / 4;
+  if (q->ceilings) {
+    LWSE_CUDA(e, cudaMemcpyAsync(e->sh_ceil.p, q->ceilings, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    h.ceilings = (const int32_t*)e->sh_ceil.p;
+  }
+  LWSE_CUDA(e, cudaMemsetAsync(h.out, 0, out_bytes + 32, s));
+  LWSE_LAUNCH(e, lwse::launch_scale_headroom(&h, 0, e->sm_count, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(words + 16, h.words, 32, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  // the r0 probes (every SOLVED entry of the rollout placement) and the rounds' probes share the sizes
+  const uint32_t n_items = std::max(words[0], words[16]), max_extra = std::max(words[1], words[17]);
+  const uint64_t n_extra = std::max((uint64_t)words[2] | (uint64_t)words[3] << 32, (uint64_t)words[18] | (uint64_t)words[19] << 32);
+  const uint32_t rounds = words[20];
+  if ((uint64_t)nr + max_extra >= (1ull << 24)) return LWSE_ERR_UNSUPPORTED;  // (row keys are 24-bit)
+  if (n_extra >= (1ull << 32)) return LWSE_ERR_OOM;                          // (the scan's offsets are 32-bit)
+  if (const int rc = rollout_place_solve(e, n_items, max_extra, n_extra, &p); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(e->sh_rows.p, p.rows_out, row_bytes, cudaMemcpyDeviceToDevice, s));
+  LWSE_CUDA(e, cudaMemsetAsync(p.counts, 0, 4, s));  // (the rounds gather their own items)
+  if (rounds) {
+    cudaGraph_t graph = nullptr;
+    GraphExec exec;
+    LWSE_CUDA(e, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    const int launched = lwse::launch_scale_headroom(&h, 1, e->sm_count, s);
+    const cudaError_t ce = cudaStreamEndCapture(s, &graph);
+    if (launched < 0 || ce != cudaSuccess) {
+      if (graph) cudaGraphDestroy(graph);
+      return fail_cuda(e, launched < 0 ? (cudaError_t)-launched : ce);
+    }
+    cudaError_t ge = exec.ensure(graph);
+    cudaGraphDestroy(graph);
+    for (uint32_t r = 0; ge == cudaSuccess && r < rounds; r++) ge = cudaGraphLaunch(exec, s);
+    if (ge != cudaSuccess) return fail_cuda(e, ge);
+    e->launches += (uint64_t)launched * rounds;
+  }
+  LWSE_LAUNCH(e, lwse::launch_scale_headroom(&h, 2, e->sm_count, s));
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  LWSE_CUDA(e, cudaMemcpyAsync(e->sh_host.h, h.out, out_bytes, cudaMemcpyDeviceToHost, s));
+  if (q->current) LWSE_CUDA(e, cudaMemcpyAsync(q->current, h.cur, row_bytes, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint8_t* hb = static_cast<const uint8_t*>(e->sh_host.h);
+  uint32_t tot[6];
+  memcpy(tot, hb, sizeof(tot));
+  memcpy(q->out, hb + 32, row_bytes);
+  q->n_solved = tot[0];
+  q->n_blocked = tot[1];
+  q->n_at_ceiling = tot[2];
+  q->rounds = rounds;
+  q->headroom = (uint64_t)tot[4] | (uint64_t)tot[5] << 32;
   return LWSE_OK;
 }
 

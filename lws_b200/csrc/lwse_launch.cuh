@@ -464,6 +464,27 @@ struct RolloutPlaceWavesLaunch {
 int launch_rollout_place_waves(const RolloutPlaceWavesLaunch* w, int pass, int sm_count, cudaStream_t s);
 int launch_place_ns_rollout_wave(const RolloutPlaceWavesLaunch* w, cudaStream_t s);
 
+// ---- lwse_scale_headroom_kernels.cu ----
+// Scale headroom (lwse_resident_scale_headroom), over the rollout placement's chain p on the resident rows (no
+// proposals, fc by row).  Entry i bisects [lo, hi) = st[i].{x, y}; each round's probes are p's rows, solved by
+// launch_rollout_place pass 1 as it stands.
+struct ScaleHeadroomLaunch {
+  RolloutPlaceLaunch p;
+  const int32_t* ceilings;        // [n] c_i (negative: none), or null
+  uint32_t constraints;           // LWSE_RPW_*
+  uint32_t n_domains;             // R_pig's bound (p's solve fields are set only after the setup)
+  uint4* st;                      // [n] {lo, hi, the entry's bits, r0}
+  const uint32_t* cur;            // [n * 16] p's rows after the setup's solve: the probe at r0 of a settled entry
+  uint32_t* clean;                // [n * 16] the row of the highest clean probe above r0
+  uint32_t* trig;                 // [n * 16] the row of the lowest triggering probe
+  uint32_t* words;                // 8 words, zeroed: [0] entries that search [1] max |E| [2..3] sum |E| (u64) [4] rounds
+  uint32_t* out;                  // the answer: 8 words of totals (zeroed), then n lwse_scale_headroom
+};
+// Pass 0 (after rollout_place pass 0): the setup kernel.  Pass 1 (captured, replayed words[4] times, after the
+// setup's solve and the copy of its rows to cur): the round kernel, launch_rollout_place pass 1, the commit.
+// Pass 2: the finish.
+int launch_scale_headroom(const ScaleHeadroomLaunch* h, int pass, int sm_count, cudaStream_t s);
+
 // ---- lwse_drain_wave_kernels.cu ----
 // lwse_resident_drain_waves.  out: the query totals (16 B), m lwse_drain_wave_key rows, then max_waves
 // lwse_drain_wave rows (the opened ones written).  counts (device, u64, zeroed by the caller): [0] the restart pairs

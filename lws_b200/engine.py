@@ -56,6 +56,7 @@ SYMBOLS = {
     "lwse_resident_drain_place_waves": ([C.c_void_p, C.POINTER(R.DrainPlaceWavesQuery)], C.c_int),
     "lwse_resident_rollout_place": ([C.c_void_p, C.POINTER(R.RolloutPlaceQuery)], C.c_int),
     "lwse_resident_rollout_place_waves": ([C.c_void_p, C.POINTER(R.RolloutPlaceWavesQuery)], C.c_int),
+    "lwse_resident_scale_headroom": ([C.c_void_p, C.POINTER(R.ScaleHeadroomQuery)], C.c_int),
     "lwse_place_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
         C.c_int,
@@ -988,6 +989,40 @@ class Engine:
         res.update({k: getattr(q, k) for k in R.ROLLOUT_WAVES_TOTALS})
         if alone:
             res["alone_rows"] = alone_rows[:n]
+        return res
+
+    def resident_scale_headroom(self, rows, ns, ceilings=None, constraints=R.RPW_STRANDED, current=False):
+        """lwse_resident_scale_headroom: for each entry (resident LWS row ``rows[i]``, namespace id ``ns[i]`` and,
+        with ``ceilings``, a ceiling such as an HPA's maxReplicas, negative for none), the largest replicas the
+        object can scale to before a group it adds triggers a verdict of ``constraints`` (``records.RPW_*``,
+        ``RPW_STRANDED`` always included) — answered for settled exclusive objects (lwse.h, "scale headroom").
+        → dict: ``rows`` (``records.SCALE_HEADROOM``, one per entry), the query's ``lws_rows``, ``ns`` and
+        ``ceilings``, the totals of ``records.SCALE_HEADROOM_TOTALS`` and, with ``current``, ``current``:
+        ``resident_rollout_place``'s rows of the resident rows.  Changes nothing resident and waits for no tick."""
+        rows = np.ascontiguousarray(rows, dtype=np.uint32)
+        ns = np.ascontiguousarray(ns, dtype=np.uint32)
+        if len(ns) != len(rows):
+            raise ValueError("rows and ns differ in length")
+        n = len(rows)
+        if ceilings is not None:
+            ceilings = np.ascontiguousarray(ceilings, dtype=np.int32)
+            if len(ceilings) != n:
+                raise ValueError("ceilings must be one int32 per entry")
+        out = R.aligned_empty(max(n, 1), R.SCALE_HEADROOM)
+        q = R.ScaleHeadroomQuery()
+        q.rows = R.ptr(rows) if n else None
+        q.ns = R.ptr(ns) if n else None
+        q.ceilings = R.ptr(ceilings) if (ceilings is not None and n) else None
+        q.n, q.constraints = n, constraints
+        q.out = R.ptr(out)
+        if current:
+            cur = R.aligned_empty(max(n, 1), R.ROLLOUT_PLACE)
+            q.current = R.ptr(cur)
+        self._check(lib().lwse_resident_scale_headroom(self._h, C.byref(q)))
+        res = {"rows": out[:n], "lws_rows": rows, "ns": ns, "ceilings": ceilings}
+        res.update({k: getattr(q, k) for k in R.SCALE_HEADROOM_TOTALS})
+        if current:
+            res["current"] = cur[:n]
         return res
 
     # ------------------------------------------------------------- group keys

@@ -603,6 +603,42 @@ class IncrementalEncoder:
                               "alone": [v for b, v in R.RPW_NAMES.items() if int(k["alone"]) & b]})
         return {"waves": waves, "unplanned": unplanned}
 
+    def scale_headroom_query(self, keys=None, ceilings=None) -> tuple:
+        """The entries of ``Engine.resident_scale_headroom``: ``rollout_place_query``'s (rows, ns) and, per key,
+        its ceiling from ``ceilings`` ({(namespace, name): an HPA's maxReplicas}; -1 for a key not in it)
+        → (rows, ns, ceilings), in key order.  Nothing in the encoder changes."""
+        if keys is None:
+            keys = [k for k, sl in self.slots.items()
+                    if int(self.lws["flags"][sl.lws_row]) & R.LWS_EXCLUSIVE_TOPOLOGY]
+        keys = sorted(keys)
+        rows, ns = self.rollout_place_query(keys)
+        ceil = np.array([int((ceilings or {}).get(k, -1)) for k in keys], dtype=np.int32)
+        return rows, ns, ceil
+
+    def scale_headroom_report(self, result: dict) -> list:
+        """A ``resident_scale_headroom`` answer as dicts, one per entry in query order: ``namespace`` and ``name``
+        (None for a row no object holds), ``replicas``, ``max_replicas``, ``headroom`` (max_replicas - replicas,
+        None when not answered or blocked), ``limit`` ("ceiling", "strands", "bumps", or None when not answered)
+        and the row's ``records.SHR_*`` flags named.  Nothing in the encoder changes."""
+        names = {sl.lws_row: k for k, sl in self.slots.items()}
+        out = []
+        for r, row in zip(np.asarray(result["lws_rows"]).tolist(), result["rows"]):
+            f = int(row["flags"])
+            ns, name = names.get(int(r), (None, None))
+            limit = None
+            if f & R.SHR_AT_CEILING:
+                limit = "ceiling"
+            elif f & R.SHR_STRANDS:
+                limit = "strands"
+            elif f & R.SHR_BUMPS:
+                limit = "bumps"
+            ok = (f & R.SHR_SOLVED) and not (f & R.SHR_BLOCKED)
+            out.append({"namespace": ns, "name": name, "replicas": int(row["replicas"]),
+                        "max_replicas": int(row["max_replicas"]),
+                        "headroom": int(row["max_replicas"]) - int(row["replicas"]) if ok else None,
+                        "limit": limit, "flags": [v for b, v in R.SHR_NAMES.items() if f & b]})
+        return out
+
     def whatif_drain(self, node_names) -> np.ndarray:
         """The node rows of the named nodes, for ``Engine.resident_drain_whatif`` (sorted, each once)."""
         return np.array(sorted({self.node_index[n] for n in node_names}), dtype=np.uint32)

@@ -923,6 +923,56 @@ class RolloutPlaceWavesQuery(C.Structure):
 assert C.sizeof(RolloutPlaceWavesQuery) == 88
 
 
+# lwse_scale_headroom: per entry, how far the object can scale up before a group it adds finds no exclusive domain
+SCALE_HEADROOM = np.dtype(
+    [("flags", "<u4"), ("replicas", "<i4"), ("max_replicas", "<i4"), ("probe", "<i4"), ("surge", "<u4"),
+     ("placed", "<u4"), ("stranded", "<u4"), ("own_lost", "<u4"), ("bumped", "<u4"), ("n_changed", "<u4"),
+     ("n_lost", "<u4"), ("n_moved", "<u4"), ("n_gained", "<u4"), ("n_placed", "<u4"), ("n_unschedulable", "<u4"),
+     ("n_conflict", "<u4")],
+    align=False,
+)
+assert SCALE_HEADROOM.itemsize == 64
+
+SHR_SOLVED = 1 << 0
+SHR_NOT_EXCLUSIVE = 1 << 1
+SHR_NOT_FORECAST = 1 << 2
+SHR_NOT_SETTLED = 1 << 3
+SHR_BLOCKED = 1 << 4
+SHR_AT_CEILING = 1 << 5
+SHR_STRANDS = 1 << 6
+SHR_BUMPS = 1 << 7
+SHR_NAMES = {SHR_SOLVED: "solved", SHR_NOT_EXCLUSIVE: "not_exclusive", SHR_NOT_FORECAST: "not_forecast",
+             SHR_NOT_SETTLED: "not_settled", SHR_BLOCKED: "blocked", SHR_AT_CEILING: "at_ceiling",
+             SHR_STRANDS: "strands", SHR_BUMPS: "bumps"}
+SCALE_HEADROOM_TOTALS = ("n_solved", "n_blocked", "n_at_ceiling", "rounds", "headroom")
+
+
+class ScaleHeadroomQuery(C.Structure):
+    """lwse_scale_headroom_query: entries (LWS row, namespace id, optional ceiling) and the RPW_* mask in; one
+    SCALE_HEADROOM row per entry, optionally the ROLLOUT_PLACE rows of the resident rows, and the
+    SCALE_HEADROOM_TOTALS out."""
+
+    _fields_ = [
+        ("rows", C.c_void_p),
+        ("ns", C.c_void_p),
+        ("ceilings", C.c_void_p),
+        ("n", C.c_uint32),
+        ("constraints", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("reserved1", C.c_uint32),
+        ("out", C.c_void_p),
+        ("current", C.c_void_p),
+        ("n_solved", C.c_uint32),
+        ("n_blocked", C.c_uint32),
+        ("n_at_ceiling", C.c_uint32),
+        ("rounds", C.c_uint32),
+        ("headroom", C.c_uint64),
+    ]
+
+
+assert C.sizeof(ScaleHeadroomQuery) == 80
+
+
 class Config(C.Structure):
     _fields_ = [
         ("abi_version", C.c_uint32),
