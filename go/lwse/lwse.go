@@ -227,6 +227,15 @@ func (e *Engine) RolloutPlaceWaves(q *C.lwse_rollout_place_waves_query) error {
 	return e.check(C.lwse_resident_rollout_place_waves(e.h, q))
 }
 
+// PlaceExplain answers "why is this group not placed?" for rows of a placement round: per row, how many topology
+// domains are too small, have no usable node, are held ahead of it in its namespace (and by which row), or are
+// open, the domain it falls short in by the fewest slots, and whether cordoned nodes would make one fit.  The
+// round is the last tick's, or the what-if round of q's segments and extra rows.  A controller turns a row into
+// the Pending event of an exclusive group; an autoscaler or rollout planner explains the rows a query stranded.
+func (e *Engine) PlaceExplain(q *C.lwse_place_explain_query) error {
+	return e.check(C.lwse_resident_place_explain(e.h, q))
+}
+
 // ScaleHeadroom answers "how many replicas can this object go to right now?" for a list of settled exclusive
 // LeaderWorkerSets in one call: per entry the largest replicas (up to an optional ceiling, such as the HPA's
 // maxReplicas) at which every group the scale-up adds still finds an exclusive domain, and the counters of the

@@ -829,6 +829,121 @@ typedef struct lwse_place_whatif {
 } lwse_place_whatif;
 LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q);
 
+/* ---- placement explanation -------------------------------------------------------------------
+ * "Why is this group not placed?" — for each chosen row of a placement round, which domains fit it, which are
+ * held ahead of it in its namespace and by whom, and by how many free slots it falls short.  The answer
+ * describes the given round; it is not itself a what-if.
+ *
+ * The round.  Without segments, without extra rows and with n_namespaces 0 or the resident count, the round
+ * explained is the BASELINE: the rows of the most recently submitted tick with LWSE_TICK_PLACE (in flight or
+ * not), over the resident node rows, occupancy counters and request rows.  Otherwise it is the WHAT-IF round
+ * lwse_resident_place_whatif computes for the same segs, extra and n_namespaces (the same meaning and the same
+ * refusals; extra row i is row rn_reqs + i).  A what-if with none of them gives the baseline's rows, so the two
+ * agree where they meet.  Rollout placement is defined as such a what-if, so explaining an entry's E_i as extra
+ * rows explains exactly the rows that entry strands.
+ *
+ * The rows.  With `rows` non-NULL, the n_rows listed row indices into the round, in the given order (duplicates
+ * allowed); with `rows` NULL, every row of the round whose lwse_place_out flags share a bit with `mask`, in
+ * ascending row order.  The first `capacity` are written to `out`; n_explained counts them all, and the totals
+ * cover them all.
+ *
+ * Per domain d of the round (n_domains of the node table), over the round's node rows and the resident
+ * occupancy occ[n]:
+ *   dom_free[d]  the spec's Σ free[n] (DESIGN.md §7: schedulable, labelled nodes of d, max(0, capacity − occ));
+ *   usable[d]    the number of schedulable labelled nodes of d;
+ *   free_all[d]  Σ max(0, capacity − occ) over every node labelled into d, schedulable or not (uint32), i.e.
+ *                dom_free[d] with the cordons lifted.
+ * The holder of (ns, d) is the PLACED row of the round, pinned or not, whose namespace is ns and domain is d;
+ * its key is the spec's key (the low 24 bits are its row).  A round has at most one.
+ *
+ * Explained row r, with spec key k, namespace ns < n_namespaces and size s (compared as signed integers): each
+ * domain falls in exactly one class, tested in this order:
+ *   own           r is PLACED in d;
+ *   no_usable     usable[d] == 0;
+ *   too_small     dom_free[d] < s;
+ *   held_pinned   (d fits) held by a pinned row with key < k;
+ *   held_earlier  (d fits) held by an unpinned row with key < k;
+ *   held_later    (d fits) held by a row with key > k;
+ *   open          (d fits) not held.
+ * fit_uncordoned counts the no_usable and too_small domains with free_all[d] >= s.  Named domains (LWSE_NONE
+ * when the set is empty):
+ *   best_domain      the argmax of the spec's level-1 hash hi = mix(key_lo ^ d·φ) | 1 over own, held_later and
+ *                    open, ties to the lower d: the domain the serial order gives an unpinned r;
+ *   blocker_domain   the argmax of hi over held_pinned and held_earlier, ties to the lower d, and blocker_row its
+ *                    holder: the domain r would take if that holder were gone;
+ *   shortfall_domain the too_small domain with the smallest s − dom_free[d] (= shortfall), ties to the lower d:
+ *                    the free slots r lacks in the closest domain too small for it.
+ * Row flags (LWSE_PEX_*): CAPACITY, no domain fits (usable[d] > 0 and dom_free[d] >= s); EXCLUSIVE, some fit and
+ * every one is held ahead of r; CORDONED, fit_uncordoned > 0 (a domain would fit with its cordoned nodes
+ * counted — not that r would place: lwse_resident_place_whatif with uncordoning segments answers that);
+ * CONFLICT, r is pinned and its leader's domain is held by a smaller pinned key (blocker_domain / blocker_row
+ * are then that domain and its holder); NO_CLAIM, r is pinned and its leader's node is missing, unlabelled or
+ * out of range; BAD_SIZE, r is unpinned with s < 1.  CAPACITY, EXCLUSIVE and CORDONED describe the domains as
+ * an unpinned request of r's size and key would see them; a pinned row's domain comes from its leader.  A row
+ * with ns >= n_namespaces carries NO_NAMESPACE alone: no domain is classified and every count is 0.
+ *
+ * The certificate.  The spec serves unpinned requests in ascending key order (a serial dictatorship), so in any
+ * round an UNSCHEDULABLE unpinned row of size >= 1 has open + held_later == 0, and a PLACED unpinned row has
+ * best_domain == its domain_id and score == hi(best_domain).
+ *
+ * Readiness, errors and isolation: exactly lwse_resident_place_whatif's — LWSE_ERR_NOT_READY and
+ * LWSE_ERR_UNSUPPORTED as it returns them (a peer exchange; rn_reqs + n_extra >= 2^24), the same
+ * LWSE_ERR_INVALID_ARG for segments, extra rows and namespaces, and LWSE_ERR_INVALID_ARG for a listed row at or
+ * beyond the round's row count or a NULL buffer with a count > 0.  A refused call writes nothing.  The call
+ * holds the engine mutex, runs on the what-if stream behind an event on the engine's stream, uses the what-if's
+ * scratch for a what-if round and scratch of its own (which only grows) for the explanation, and touches
+ * nothing of a tick.  Where the what-if runs the general form, so does the explained round. */
+typedef struct lwse_place_explain_row {
+  uint32_t row;              /* row of the round                                                        */
+  uint32_t flags;            /* LWSE_PEX_*                                                              */
+  uint32_t place_flags;      /* the round's lwse_place_out flags of the row                             */
+  uint32_t n_own;            /* the classes above: they sum to n_domains (0 with LWSE_PEX_NO_NAMESPACE) */
+  uint32_t n_no_usable;
+  uint32_t n_too_small;
+  uint32_t n_held_pinned;
+  uint32_t n_held_earlier;
+  uint32_t n_held_later;
+  uint32_t n_open;
+  uint32_t n_fit_uncordoned;
+  uint32_t best_domain;
+  uint32_t blocker_domain;
+  uint32_t blocker_row;
+  uint32_t shortfall;        /* 0 when shortfall_domain is LWSE_NONE                                    */
+  uint32_t shortfall_domain;
+} lwse_place_explain_row;   /* 64 B */
+
+#define LWSE_PEX_CAPACITY (1u << 0)
+#define LWSE_PEX_EXCLUSIVE (1u << 1)
+#define LWSE_PEX_CORDONED (1u << 2)
+#define LWSE_PEX_CONFLICT (1u << 3)
+#define LWSE_PEX_NO_CLAIM (1u << 4)
+#define LWSE_PEX_NO_NAMESPACE (1u << 5)
+#define LWSE_PEX_BAD_SIZE (1u << 6)
+
+typedef struct lwse_place_explain_query {
+  /* in: the round (as lwse_place_whatif) */
+  const lwse_patch_seg* segs;
+  uint32_t n_segs;
+  uint32_t n_extra;
+  const lwse_place_req* extra;
+  uint32_t n_namespaces;
+  /* in: the rows */
+  uint32_t mask;                    /* with rows == NULL: LWSE_PLACE_* bits that select a row               */
+  const uint32_t* rows;             /* [n_rows] row indices into the round, host memory; NULL: by mask      */
+  uint32_t n_rows;
+  uint32_t capacity;                /* rows `out` holds                                                     */
+  lwse_place_explain_row* out;      /* [capacity], host memory                                              */
+  /* out */
+  uint32_t n_explained;             /* rows selected (beyond capacity counted, not written)                 */
+  uint32_t round_rows;              /* rows of the round (rn_reqs + n_extra)                                */
+  uint32_t n_domains;
+  uint32_t whatif;                  /* 1: the what-if round was explained, 0: the baseline                   */
+  uint32_t form;                    /* the what-if's form (LWSE_TICK_FORM_*), 0 for the baseline             */
+  uint32_t n_flag[7];               /* rows carrying LWSE_PEX_* bit i                                        */
+  uint64_t n_class[8];              /* sums over the rows of n_own .. n_fit_uncordoned                       */
+} lwse_place_explain_query;
+LWSE_API int lwse_resident_place_explain(lwse_engine* e, lwse_place_explain_query* q);
+
 /* ---- drain what-if ------------------------------------------------------------------------------
  * "If I drain these nodes, which LeaderWorkerSet groups restart?" — answered on the resident tables
  * without changing them.  With RecreateGroupOnPodRestart / RecreateGroupAfterStart, evicting one pod of

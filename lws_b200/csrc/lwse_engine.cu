@@ -346,6 +346,11 @@ struct lwse_engine {
   // triggering rows, the answer (its totals first, the setup's words after the rows); the answer going back (host)
   DevBuf sh_ceil, sh_state, sh_rows, sh_out;
   PinBuf sh_host;
+  // placement explanation (lwse_resident_place_explain): on the what-if stream, the selected rows (their count, the
+  // mask form's chunk index, the list), the per-domain stats, the namespace marks, the holder table, the totals and
+  // rows; the caller's rows going in and the answer's words coming back through px_host
+  DevBuf px_sel, px_dom, px_mark, px_table, px_out;
+  PinBuf px_host;
   // drain waves (lwse_resident_drain_waves): the drain budget's key rows, the counters, the ids, the key positions, the
   // key buckets (count | first | cursor), the restart pairs, the pair records, the touched-row index (count | first |
   // cursor), the dense rows, the lost counters, the group and row wave masks, the stamps, the answer; the ids going
@@ -2311,37 +2316,51 @@ static int own_node_index(lwse_engine* e, const lwse_node_rec* nodes, cudaStream
   return LWSE_OK;
 }
 
-// Patched copies of the node and request rows in what-if scratch, the round over them on wf_stream
-// (only the touched namespaces in the namespace form), then one diff kernel against the baseline rows
-// (r_pout, read in place: nothing writes them while the call holds the mutex).  The resident node
-// index is read in place unless the node patches need another one.
-LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
-  if (!e || !q) return LWSE_ERR_INVALID_ARG;
-  std::lock_guard<std::mutex> lock(e->mu);
+// A what-if round (lwse_resident_place_whatif, lwse_resident_place_explain) in three steps: place_whatif_check
+// (readiness, arguments, the touched namespaces and the node-index decision, over the host mirror), then
+// place_whatif_reserve (its scratch: a reserve may reallocate, so before the snapshot), then, behind the snapshot
+// event, place_whatif_enqueue (patched copies of the node and request rows in what-if scratch, the round over them
+// on wf_stream, only the touched namespaces in the namespace form).  The resident node index is read in place
+// unless the node patches need another one.
+struct WhatifRound {
+  const lwse_patch_seg* segs = nullptr;
+  uint32_t n_segs = 0;
+  const lwse_place_req* extra = nullptr;
+  uint32_t n_extra = 0;
+  uint32_t n_ns = 0, rn = 0, n_total = 0, n_touched = 0;
+  bool ns_form = false, node_rows = false, node_rebuild = false, round_fresh = false;
+  size_t stage_need = 0, round_bytes = 0;
+  std::vector<uint8_t> touched;
+  // the round's tables, once enqueued
+  const lwse_node_rec* nodes = nullptr;
+  const lwse_place_req* reqs = nullptr;
+  lwse_place_out* out = nullptr;
+};
+
+// `bad_buffers`: the caller's own buffers are missing (refused as INVALID_ARG, after readiness).
+static int place_whatif_check(lwse_engine* e, const lwse_patch_seg* segs, uint32_t n_segs, const lwse_place_req* extra,
+                              uint32_t n_extra, uint32_t n_namespaces, bool bad_buffers, WhatifRound* w) {
   if (!e->r_loaded || !e->r_place_loaded || !e->r_place_current || e->n_nodes == 0 || e->n_domains == 0)
     return LWSE_ERR_NOT_READY;
   if (e->xch_world > 0) return LWSE_ERR_UNSUPPORTED;
-  if ((q->n_segs && !q->segs) || q->n_segs > LWSE_TICK_MAX_SEGS || (q->n_extra && (!q->extra || !q->extra_out)) ||
-      (q->capacity && (!q->rows || !q->before || !q->after)))
-    return LWSE_ERR_INVALID_ARG;
-  const uint32_t n_ns = q->n_namespaces ? q->n_namespaces : e->rn_namespaces;
+  if ((n_segs && !segs) || n_segs > LWSE_TICK_MAX_SEGS || (n_extra && !extra) || bad_buffers) return LWSE_ERR_INVALID_ARG;
+  const uint32_t n_ns = n_namespaces ? n_namespaces : e->rn_namespaces;
   if (n_ns == 0) return LWSE_ERR_INVALID_ARG;
   const uint32_t rn = e->rn_reqs;
-  if ((uint64_t)rn + q->n_extra >= (1ull << 24)) return LWSE_ERR_UNSUPPORTED;
-  const uint32_t n_total = rn + q->n_extra;
-  for (uint32_t i = 0; i < q->n_segs; i++)
-    if (q->segs[i].n && q->segs[i].table != LWSE_TABLE_NODES && q->segs[i].table != LWSE_TABLE_PLACE_REQS)
+  if ((uint64_t)rn + n_extra >= (1ull << 24)) return LWSE_ERR_UNSUPPORTED;
+  for (uint32_t i = 0; i < n_segs; i++)
+    if (segs[i].n && segs[i].table != LWSE_TABLE_NODES && segs[i].table != LWSE_TABLE_PLACE_REQS)
       return LWSE_ERR_INVALID_ARG;
   SegSummary ss;
-  if (const int crc = summarize_segments(e, q->segs, q->n_segs, &ss); crc != LWSE_OK) return crc;
+  if (const int crc = summarize_segments(e, segs, n_segs, &ss); crc != LWSE_OK) return crc;
   // the node-index decision is the tick's, over the mirror, which stays as it is; then the touched namespaces
   const bool node_rows = (ss.tables & (1u << LWSE_TABLE_NODES)) != 0;
   bool node_rebuild = ss.node_moves;
   std::vector<uint8_t> touched(n_ns, 0);
   for (uint32_t v = e->rn_namespaces; v < n_ns; v++) touched[v] = 1;  // (their resident rows were UNSCHEDULABLE)
-  size_t stage_need = align256((size_t)n_ns) + align256((size_t)q->n_extra * sizeof(lwse_place_req));
-  for (uint32_t i = 0; i < q->n_segs; i++) {
-    const lwse_patch_seg& g = q->segs[i];
+  size_t stage_need = align256((size_t)n_ns) + align256((size_t)n_extra * sizeof(lwse_place_req));
+  for (uint32_t i = 0; i < n_segs; i++) {
+    const lwse_patch_seg& g = segs[i];
     if (g.n == 0) continue;
     const bool range = (g.flags & LWSE_PATCH_RANGE) != 0;
     const uint32_t rb = g.table == LWSE_TABLE_NODES ? (uint32_t)sizeof(lwse_node_rec) : (uint32_t)sizeof(lwse_place_req);
@@ -2357,19 +2376,59 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
       }
     }
   }
-  for (uint32_t i = 0; i < q->n_extra; i++)
-    if (q->extra[i].ns < n_ns) touched[q->extra[i].ns] = 1;
+  for (uint32_t i = 0; i < n_extra; i++)
+    if (extra[i].ns < n_ns) touched[extra[i].ns] = 1;
   if (node_rows) std::fill(touched.begin(), touched.end(), (uint8_t)1);  // (capacities or domains moved under every namespace)
   // (a resident index behind the resident rows — node patches, and no round since because the request table is
   // empty — is not read either: the what-if builds its own)
   if (e->node_index_stale) node_rebuild = true;
   uint32_t n_touched = 0;
   for (uint8_t t : touched) n_touched += t;
+  w->segs = segs;
+  w->n_segs = n_segs;
+  w->extra = extra;
+  w->n_extra = n_extra;
+  w->n_ns = n_ns;
+  w->rn = rn;
+  w->n_total = rn + n_extra;
+  w->n_touched = n_touched;
+  w->node_rows = node_rows;
+  w->node_rebuild = node_rebuild;
+  w->stage_need = stage_need;
+  w->touched = std::move(touched);
+  return LWSE_OK;
+}
 
-  DeviceGuard guard(e->device);
+static int place_whatif_reserve(lwse_engine* e, WhatifRound* w) {
   // staging (the previous call synchronized its stream: the buffer is free)
-  LWSE_CUDA(e, e->wf_stage.reserve(stage_need));
+  LWSE_CUDA(e, e->wf_stage.reserve(w->stage_need));
   LWSE_CUDA(e, e->wf_words.reserve(64));
+  w->ns_form = lwse::place_ns_supported(e->n_nodes, e->n_domains);
+  LWSE_CUDA(e, e->wf_reqs.reserve((size_t)w->n_total * sizeof(lwse_place_req) + 16));
+  LWSE_CUDA(e, e->wf_out.reserve((size_t)w->n_total * sizeof(lwse_place_out) + 16));
+  LWSE_CUDA(e, e->wf_touched.reserve((size_t)w->n_ns + 16));
+  if (w->node_rows) LWSE_CUDA(e, e->wf_nodes.reserve((size_t)e->n_nodes * sizeof(lwse_node_rec) + 16));
+  if (w->node_rebuild)
+    if (const int rc = reserve_node_index(e); rc != LWSE_OK) return rc;
+  if (w->ns_form) {
+    w->round_bytes = lwse::place_ns_scratch_bytes(e->n_nodes, e->n_domains, w->n_total, w->n_ns);
+    const void* before = e->wf_round.p;
+    LWSE_CUDA(e, e->wf_round.reserve(w->round_bytes));
+    // wf_geometry names the layout the scratch holds zeroed counts for: a new buffer holds none until
+    // place_whatif_enqueue has cleared it, so a call that fails in between leaves the next one fresh
+    if (before != e->wf_round.p) memset(e->wf_geometry, 0, sizeof(e->wf_geometry));
+    const uint32_t geometry[4] = {w->n_total, w->n_ns, e->n_nodes, e->n_domains};
+    w->round_fresh = memcmp(geometry, e->wf_geometry, sizeof(geometry)) != 0;
+  } else {
+    w->round_bytes = lwse::place_scratch_bytes(e->n_nodes, e->n_domains, w->n_total, w->n_ns);
+    LWSE_CUDA(e, e->wf_round.reserve(w->round_bytes));
+    e->wf_geometry[0] = e->wf_geometry[1] = e->wf_geometry[2] = e->wf_geometry[3] = 0;  // (the general form re-initialises it)
+  }
+  return LWSE_OK;
+}
+
+// On wf_stream, behind drain_begin_locked.
+static int place_whatif_enqueue(lwse_engine* e, WhatifRound* w) {
   uint8_t* st_h = static_cast<uint8_t*>(e->wf_stage.h);
   size_t cursor = 0;
   auto stage = [&](const void* src, size_t bytes) -> size_t {
@@ -2378,38 +2437,13 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
     cursor += align256(bytes);
     return at;
   };
-  const bool ns_form = lwse::place_ns_supported(e->n_nodes, e->n_domains);
-  const size_t b_nodes = (size_t)e->n_nodes * sizeof(lwse_node_rec);
-  const size_t b_out = (size_t)n_total * sizeof(lwse_place_out);
-  LWSE_CUDA(e, e->wf_reqs.reserve((size_t)n_total * sizeof(lwse_place_req) + 16));
-  LWSE_CUDA(e, e->wf_out.reserve(b_out + 16));
-  LWSE_CUDA(e, e->wf_touched.reserve((size_t)n_ns + 16));
-  const uint32_t list_cap = q->capacity < rn ? q->capacity : rn;  // (at most rn rows can differ)
-  LWSE_CUDA(e, e->wf_list.reserve(64 + 16 + (size_t)list_cap * (4 + 2 * sizeof(lwse_place_out))));
-  if (node_rows) LWSE_CUDA(e, e->wf_nodes.reserve(b_nodes + 16));
-  if (node_rebuild)
-    if (const int rc = reserve_node_index(e); rc != LWSE_OK) return rc;
-  size_t round_bytes = 0;
-  bool round_fresh = false;
-  if (ns_form) {
-    round_bytes = lwse::place_ns_scratch_bytes(e->n_nodes, e->n_domains, n_total, n_ns);
-    const void* before = e->wf_round.p;
-    LWSE_CUDA(e, e->wf_round.reserve(round_bytes));
-    const uint32_t geometry[4] = {n_total, n_ns, e->n_nodes, e->n_domains};
-    round_fresh = before != e->wf_round.p || memcmp(geometry, e->wf_geometry, sizeof(geometry)) != 0;
-    memcpy(e->wf_geometry, geometry, sizeof(geometry));
-  } else {
-    round_bytes = lwse::place_scratch_bytes(e->n_nodes, e->n_domains, n_total, n_ns);
-    LWSE_CUDA(e, e->wf_round.reserve(round_bytes));
-    e->wf_geometry[0] = e->wf_geometry[1] = e->wf_geometry[2] = e->wf_geometry[3] = 0;  // (the general form re-initialises it)
-  }
-
-  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
   cudaStream_t s = e->wf_stream;
+  const uint32_t rn = w->rn, n_total = w->n_total, n_ns = w->n_ns;
+  const size_t b_nodes = (size_t)e->n_nodes * sizeof(lwse_node_rec);
   lwse_node_rec* d_nodes = (lwse_node_rec*)e->nodes.p;
   lwse_place_req* d_reqs = (lwse_place_req*)e->wf_reqs.p;
   lwse_place_out* d_out = (lwse_place_out*)e->wf_out.p;
-  if (node_rows) {
+  if (w->node_rows) {
     LWSE_CUDA(e, cudaMemcpyAsync(e->wf_nodes.p, e->nodes.p, b_nodes, cudaMemcpyDeviceToDevice, s));
     d_nodes = (lwse_node_rec*)e->wf_nodes.p;
   }
@@ -2417,20 +2451,20 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
     LWSE_CUDA(e, cudaMemcpyAsync(d_reqs, e->r_preq.p, (size_t)rn * sizeof(lwse_place_req), cudaMemcpyDeviceToDevice, s));
     LWSE_CUDA(e, cudaMemcpyAsync(d_out, e->r_pout.p, (size_t)rn * sizeof(lwse_place_out), cudaMemcpyDeviceToDevice, s));
   }
-  if (q->n_extra) {
-    const size_t at = stage(q->extra, (size_t)q->n_extra * sizeof(lwse_place_req));
-    LWSE_CUDA(e, cudaMemcpyAsync(d_reqs + rn, st_h + at, (size_t)q->n_extra * sizeof(lwse_place_req), cudaMemcpyHostToDevice, s));
-    LWSE_CUDA(e, cudaMemsetAsync(d_out + rn, 0, (size_t)q->n_extra * sizeof(lwse_place_out), s));
+  if (w->n_extra) {
+    const size_t at = stage(w->extra, (size_t)w->n_extra * sizeof(lwse_place_req));
+    LWSE_CUDA(e, cudaMemcpyAsync(d_reqs + rn, st_h + at, (size_t)w->n_extra * sizeof(lwse_place_req), cudaMemcpyHostToDevice, s));
+    LWSE_CUDA(e, cudaMemsetAsync(d_out + rn, 0, (size_t)w->n_extra * sizeof(lwse_place_out), s));
   }
   {
-    const size_t at = stage(touched.data(), n_ns);
+    const size_t at = stage(w->touched.data(), n_ns);
     LWSE_CUDA(e, cudaMemcpyAsync(e->wf_touched.p, st_h + at, n_ns, cudaMemcpyHostToDevice, s));
   }
   // the segments, into the copies: ranges by DMA first, then one scatter of the rest (as a tick applies them)
   lwse::ScatterSegHost sc[LWSE_TICK_MAX_SEGS];
   int n_sc = 0;
-  for (uint32_t i = 0; i < q->n_segs; i++) {
-    const lwse_patch_seg& g = q->segs[i];
+  for (uint32_t i = 0; i < w->n_segs; i++) {
+    const lwse_patch_seg& g = w->segs[i];
     if (g.n == 0) continue;
     const bool is_nodes = g.table == LWSE_TABLE_NODES;
     const uint32_t rb = is_nodes ? (uint32_t)sizeof(lwse_node_rec) : (uint32_t)sizeof(lwse_place_req);
@@ -2452,21 +2486,52 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
   const uint32_t* dom_first = (const uint32_t*)e->dom_first.p;
   const uint32_t* node_order = (const uint32_t*)e->node_order.p;
   const uint32_t* node_pos = (const uint32_t*)e->node_pos.p;
-  if (node_rebuild)
+  if (w->node_rebuild)
     if (const int rc = own_node_index(e, d_nodes, s, &dom_first, &node_order, &node_pos); rc != LWSE_OK) return rc;
-  if (ns_form) {
-    if (round_fresh) LWSE_CUDA(e, cudaMemsetAsync(e->wf_round.p, 0, round_bytes, s));  // (index counts and counters start at zero)
+  if (w->ns_form) {
+    if (w->round_fresh) {  // (index counts and counters start at zero)
+      LWSE_CUDA(e, cudaMemsetAsync(e->wf_round.p, 0, w->round_bytes, s));
+      const uint32_t geometry[4] = {n_total, n_ns, e->n_nodes, e->n_domains};
+      memcpy(e->wf_geometry, geometry, sizeof(geometry));
+    }
     LWSE_LAUNCH(e, lwse::launch_place_whatif_index(d_reqs, n_total, n_ns, (const uint8_t*)e->wf_touched.p, e->n_nodes, e->n_domains,
                                                    e->wf_round.p, e->sm_count, s));
     LWSE_LAUNCH(e, lwse::launch_place_ns(d_nodes, dom_first, node_order, e->n_nodes, e->n_domains, d_reqs, n_total,
-                                         (const uint32_t*)e->r_occ.p, 1, 0, n_ns, d_out, e->wf_round.p, round_bytes, false,
+                                         (const uint32_t*)e->r_occ.p, 1, 0, n_ns, d_out, e->wf_round.p, w->round_bytes, false,
                                          e->wf_calls++, false, e->sm_count, s, nullptr, false, nullptr, nullptr,
                                          lwse::kNsIndexReuse));
   } else {
     LWSE_LAUNCH(e, lwse::launch_place(d_nodes, dom_first, node_order, node_pos, e->n_nodes, e->n_domains, d_reqs, n_total,
-                                      (const uint32_t*)e->r_occ.p, n_ns, d_out, e->wf_round.p, round_bytes, nullptr,
+                                      (const uint32_t*)e->r_occ.p, n_ns, d_out, e->wf_round.p, w->round_bytes, nullptr,
                                       e->sm_count, s, 0u, true, 1, n_total, 0, nullptr, nullptr, nullptr, false));
   }
+  w->nodes = d_nodes;
+  w->reqs = d_reqs;
+  w->out = d_out;
+  return LWSE_OK;
+}
+
+// The what-if round, then one diff kernel against the baseline rows (r_pout, read in place: nothing writes them
+// while the call holds the mutex).
+LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  WhatifRound w;
+  const bool bad_buffers = (q->n_extra && !q->extra_out) || (q->capacity && (!q->rows || !q->before || !q->after));
+  if (const int rc = place_whatif_check(e, q->segs, q->n_segs, q->extra, q->n_extra, q->n_namespaces, bad_buffers, &w);
+      rc != LWSE_OK)
+    return rc;
+  const uint32_t rn = w.rn, n_total = w.n_total;
+
+  DeviceGuard guard(e->device);
+  const uint32_t list_cap = q->capacity < rn ? q->capacity : rn;  // (at most rn rows can differ)
+  LWSE_CUDA(e, e->wf_list.reserve(64 + 16 + (size_t)list_cap * (4 + 2 * sizeof(lwse_place_out))));
+  if (const int rc = place_whatif_reserve(e, &w); rc != LWSE_OK) return rc;
+
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  if (const int rc = place_whatif_enqueue(e, &w); rc != LWSE_OK) return rc;
+  lwse_place_out* d_out = w.out;
   // the diff against the baseline, the counts
   // (layout: [counts: 16 words] [rows: list_cap] [before: list_cap] [after: list_cap], the 16-byte rows aligned)
   uint32_t* d_counts = (uint32_t*)e->wf_list.p;
@@ -2500,8 +2565,115 @@ LWSE_API int lwse_resident_place_whatif(lwse_engine* e, lwse_place_whatif* q) {
   q->n_placed = words[4];
   q->n_unschedulable = words[5];
   q->n_conflict = words[6];
-  q->namespaces_solved = ns_form ? n_touched : 0u;
-  q->form = ns_form ? LWSE_TICK_FORM_NAMESPACE : LWSE_TICK_FORM_GENERAL;
+  q->namespaces_solved = w.ns_form ? w.n_touched : 0u;
+  q->form = w.ns_form ? LWSE_TICK_FORM_NAMESPACE : LWSE_TICK_FORM_GENERAL;
+  return LWSE_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Placement explanation
+// ---------------------------------------------------------------------------
+// The round is the baseline (r_pout over the resident node and request rows, read in place) or the what-if's (the
+// what-if's check, reserve and enqueue steps); launch_place_explain runs over it on wf_stream, behind the same
+// snapshot event, with scratch of its own (px_*).
+static uint64_t table_slots(uint64_t pairs);
+LWSE_API int lwse_resident_place_explain(lwse_engine* e, lwse_place_explain_query* q) {
+  if (!e || !q) return LWSE_ERR_INVALID_ARG;
+  std::lock_guard<std::mutex> lock(e->mu);
+  WhatifRound w;
+  const bool bad_buffers = (q->n_rows && !q->rows) || (q->capacity && !q->out);
+  if (const int rc = place_whatif_check(e, q->segs, q->n_segs, q->extra, q->n_extra, q->n_namespaces, bad_buffers, &w);
+      rc != LWSE_OK)
+    return rc;
+  const bool whatif = q->n_segs || q->n_extra || w.n_ns != e->rn_namespaces;
+  const bool by_mask = q->rows == nullptr;
+  const uint32_t n_total = w.n_total, nd = e->n_domains;
+  if (!by_mask)
+    for (uint32_t i = 0; i < q->n_rows; i++)
+      if (q->rows[i] >= n_total) return LWSE_ERR_INVALID_ARG;
+  const uint32_t n_listed = by_mask ? n_total : q->n_rows;
+  const uint32_t out_cap = q->capacity < n_listed ? q->capacity : n_listed;
+  const uint32_t n_chunks = by_mask ? (n_total + 255u) / 256u : 0u;
+  const uint64_t slots = table_slots(n_total);
+
+  DeviceGuard guard(e->device);
+  if (whatif)
+    if (const int rc = place_whatif_reserve(e, &w); rc != LWSE_OK) return rc;
+  // px_sel: [the listed count, 3 words of padding] [chunk count | first | cursor] [the list]
+  const size_t sel_words = 4 + (size_t)3 * n_chunks + 1 + n_listed;
+  LWSE_CUDA(e, e->px_sel.reserve(sel_words * 4 + 16));
+  LWSE_CUDA(e, e->px_dom.reserve((size_t)3 * nd * 4 + 16));
+  LWSE_CUDA(e, e->px_mark.reserve((size_t)w.n_ns + 16));
+  LWSE_CUDA(e, e->px_table.reserve((size_t)slots * 16));
+  LWSE_CUDA(e, e->px_out.reserve(128 + (size_t)out_cap * sizeof(lwse_place_explain_row)));
+  LWSE_CUDA(e, e->px_host.reserve(256 + (by_mask ? 0 : (size_t)n_listed * 4)));
+
+  if (const int rc = drain_begin_locked(e); rc != LWSE_OK) return rc;
+  cudaStream_t s = e->wf_stream;
+  lwse::PlaceExplainLaunch p{};
+  if (whatif) {
+    if (const int rc = place_whatif_enqueue(e, &w); rc != LWSE_OK) return rc;
+    p.nodes = w.nodes;
+    p.reqs = w.reqs;
+    p.res = w.out;
+  } else {
+    p.nodes = (const lwse_node_rec*)e->nodes.p;
+    p.reqs = (const lwse_place_req*)e->r_preq.p;
+    p.res = (const lwse_place_out*)e->r_pout.p;
+  }
+  uint32_t* sel = (uint32_t*)e->px_sel.p;
+  uint32_t* h_words = static_cast<uint32_t*>(e->px_host.h);
+  p.occupancy = (const uint32_t*)e->r_occ.p;
+  p.n_nodes = e->n_nodes;
+  p.n_domains = nd;
+  p.n_rows = n_total;
+  p.n_namespaces = w.n_ns;
+  p.by_mask = by_mask;
+  p.mask = q->mask;
+  p.chunk_count = sel + 4;
+  p.chunk_first = p.chunk_count + n_chunks;
+  p.chunk_cursor = p.chunk_first + n_chunks + 1;
+  p.list = p.chunk_cursor + n_chunks;
+  p.n_list = by_mask ? p.chunk_first + n_chunks : sel;
+  p.n_listed = n_listed;
+  p.dom = (uint32_t*)e->px_dom.p;
+  p.ns_mark = (uint8_t*)e->px_mark.p;
+  p.tkeys = (unsigned long long*)e->px_table.p;
+  p.tvals = p.tkeys + slots;
+  p.table_mask = (uint32_t)(slots - 1);
+  p.totals = (unsigned long long*)e->px_out.p;
+  p.out = reinterpret_cast<lwse_place_explain_row*>(static_cast<uint8_t*>(e->px_out.p) + 128);
+  p.capacity = out_cap;
+  if (!by_mask) {  // the caller's rows, behind their count (px_host: the previous call synchronized its stream)
+    h_words[0] = n_listed;
+    if (n_listed) memcpy(h_words + 64, q->rows, (size_t)n_listed * 4);
+    LWSE_CUDA(e, cudaMemcpyAsync(sel, h_words, 4, cudaMemcpyHostToDevice, s));
+    if (n_listed) LWSE_CUDA(e, cudaMemcpyAsync(p.list, h_words + 64, (size_t)n_listed * 4, cudaMemcpyHostToDevice, s));
+  }
+  LWSE_CUDA(e, cudaMemsetAsync(p.dom, 0, (size_t)3 * nd * 4, s));
+  LWSE_CUDA(e, cudaMemsetAsync(p.ns_mark, 0, w.n_ns, s));
+  LWSE_CUDA(e, cudaMemsetAsync(p.tkeys, 0xFF, (size_t)slots * 16, s));
+  LWSE_CUDA(e, cudaMemsetAsync(p.totals, 0, 128, s));
+  LWSE_LAUNCH(e, lwse::launch_place_explain(&p, e->sm_count, s));
+  if (const int rc = drain_end_locked(e); rc != LWSE_OK) return rc;
+  // read back: the totals and the listed count, then the rows
+  unsigned long long* h_totals = reinterpret_cast<unsigned long long*>(h_words);
+  LWSE_CUDA(e, cudaMemcpyAsync(h_totals, p.totals, 128, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaMemcpyAsync(h_words + 32, p.n_list, 4, cudaMemcpyDeviceToHost, s));
+  LWSE_CUDA(e, cudaStreamSynchronize(s));
+  const uint32_t n_explained = h_words[32];
+  const uint32_t listed = n_explained < out_cap ? n_explained : out_cap;
+  if (listed) {
+    LWSE_CUDA(e, cudaMemcpyAsync(q->out, p.out, (size_t)listed * sizeof(lwse_place_explain_row), cudaMemcpyDeviceToHost, s));
+    LWSE_CUDA(e, cudaStreamSynchronize(s));
+  }
+  q->n_explained = n_explained;
+  q->round_rows = n_total;
+  q->n_domains = nd;
+  q->whatif = whatif ? 1u : 0u;
+  q->form = whatif ? (w.ns_form ? LWSE_TICK_FORM_NAMESPACE : LWSE_TICK_FORM_GENERAL) : 0u;
+  for (uint32_t b = 0; b < 7; b++) q->n_flag[b] = (uint32_t)h_totals[8 + b];
+  for (uint32_t j = 0; j < 8; j++) q->n_class[j] = h_totals[j];
   return LWSE_OK;
 }
 

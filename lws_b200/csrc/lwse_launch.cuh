@@ -485,6 +485,35 @@ struct ScaleHeadroomLaunch {
 // Pass 2: the finish.
 int launch_scale_headroom(const ScaleHeadroomLaunch* h, int pass, int sm_count, cudaStream_t s);
 
+// ---- lwse_place_explain_kernels.cu ----
+// lwse_resident_place_explain over one round: its node, request and result rows (the baseline's in place, or a
+// what-if round's scratch) and the resident occupancy.
+struct PlaceExplainLaunch {
+  const lwse_node_rec* nodes;        // [n_nodes]
+  const uint32_t* occupancy;         // [n_nodes] or null
+  const lwse_place_req* reqs;        // [n_rows]
+  const lwse_place_out* res;         // [n_rows]
+  uint32_t n_nodes, n_domains, n_rows, n_namespaces;
+  bool by_mask;                      // select the rows whose result flags share a bit with `mask` into `list`
+  uint32_t mask;
+  uint32_t* chunk_count;             // by mask: [n_chunks] (256 rows each), then the scan's first [n_chunks + 1]
+  uint32_t* chunk_first;             //   and cursor [n_chunks]
+  uint32_t* chunk_cursor;
+  uint32_t* list;                    // the listed rows: filled by mask, or the caller's (uploaded)
+  const uint32_t* n_list;            // device word: the rows listed (by mask: chunk_first[n_chunks])
+  uint32_t n_listed;                 // their bound, for the grids (by mask: n_rows)
+  uint32_t* dom;                     // [3 * n_domains] dom_free | usable | free_all, zeroed by the caller
+  uint8_t* ns_mark;                  // [n_namespaces] namespaces of the listed rows, zeroed by the caller
+  unsigned long long* tkeys;         // [table_mask + 1] the holder table: ns << 32 | d, all-ones when free ...
+  unsigned long long* tvals;         // ... and the holder's spec key (all-ones before)
+  uint32_t table_mask;
+  lwse_place_explain_row* out;       // [capacity]
+  uint32_t capacity;
+  unsigned long long* totals;        // 16 words, zeroed by the caller: [0..7] the class sums, [8..14] the flag counts
+};
+// The stats, the selection (count, scan, fill by mask; mark by list), the holder table, the explanation.
+int launch_place_explain(const PlaceExplainLaunch* p, int sm_count, cudaStream_t s);
+
 // ---- lwse_drain_wave_kernels.cu ----
 // lwse_resident_drain_waves.  out: the query totals (16 B), m lwse_drain_wave_key rows, then max_waves
 // lwse_drain_wave rows (the opened ones written).  counts (device, u64, zeroed by the caller): [0] the restart pairs

@@ -57,6 +57,7 @@ SYMBOLS = {
     "lwse_resident_rollout_place": ([C.c_void_p, C.POINTER(R.RolloutPlaceQuery)], C.c_int),
     "lwse_resident_rollout_place_waves": ([C.c_void_p, C.POINTER(R.RolloutPlaceWavesQuery)], C.c_int),
     "lwse_resident_scale_headroom": ([C.c_void_p, C.POINTER(R.ScaleHeadroomQuery)], C.c_int),
+    "lwse_resident_place_explain": ([C.c_void_p, C.POINTER(R.PlaceExplainQuery)], C.c_int),
     "lwse_place_host": (
         [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)],
         C.c_int,
@@ -466,6 +467,41 @@ class Engine:
                "form": self.TICK_FORMS[q.form]}
         out.update({k: getattr(q, k) for k in R.PLACE_WHATIF})
         return out
+
+    def resident_place_explain(self, rows=None, mask=R.PLACE_UNSCHEDULABLE | R.PLACE_CONFLICT, segs=(), extra=None,
+                               n_namespaces=0, capacity=None):
+        """lwse_resident_place_explain: why rows of a placement round have their verdicts.  The round is the
+        baseline (the last tick's rows) without ``segs``, ``extra`` and a new ``n_namespaces``, else the what-if
+        round ``resident_place_whatif`` computes for them.  ``rows`` lists row indices into the round; None takes
+        every row whose result flags share a bit with ``mask`` (``records.PLACE_*``), ascending.  ``capacity`` None
+        returns every explained row.  → dict: ``rows`` (``records.PLACE_EXPLAIN``), ``n_explained``,
+        ``round_rows``, ``n_domains``, ``whatif``, ``form``, ``classes`` ({class: sum over the rows}) and ``flags``
+        ({``records.PEX_NAMES`` name: rows carrying it}).  Changes nothing resident and waits for no tick."""
+        tick = self.make_tick(segs)
+        extra = R.aligned_empty(0, R.PLACE_REQ) if extra is None else _aligned16(np.asarray(extra, dtype=R.PLACE_REQ))
+        listed = None if rows is None else np.ascontiguousarray(rows, dtype=np.uint32)
+        buf = None if listed is None else (listed if len(listed) else np.zeros(1, np.uint32))  # (non-NULL: a list)
+        bound = (getattr(self, "_n_place", 0) + len(extra)) if listed is None else len(listed)
+        cap = bound if capacity is None else int(capacity)
+        out = R.aligned_empty(max(cap, 1), R.PLACE_EXPLAIN)
+        q = R.PlaceExplainQuery()
+        q.segs = C.cast(tick.segs, C.c_void_p) if len(segs) else None
+        q.n_segs = len(segs)
+        q.extra = R.ptr(extra) if len(extra) else None
+        q.n_extra = len(extra)
+        q.n_namespaces = int(n_namespaces)
+        q.mask = int(mask)
+        q.rows = R.ptr(buf)
+        q.n_rows = 0 if listed is None else len(listed)
+        q.capacity = cap
+        q.out = R.ptr(out)
+        self._check(lib().lwse_resident_place_explain(self._h, C.byref(q)))
+        res = {"rows": out[: min(q.n_explained, cap)], "n_explained": q.n_explained, "round_rows": q.round_rows,
+               "n_domains": q.n_domains, "whatif": bool(q.whatif),
+               "form": self.TICK_FORMS[q.form] if q.whatif else None}
+        res["classes"] = {k: int(q.n_class[j]) for j, k in enumerate(R.PLACE_EXPLAIN_CLASSES)}
+        res["flags"] = {name: int(q.n_flag[b.bit_length() - 1]) for b, name in R.PEX_NAMES.items()}
+        return res
 
     def resident_drain_whatif(self, nodes, capacity=None):
         """lwse_resident_drain_whatif: the group rows of a sweep of the resident tables with every pod scheduled

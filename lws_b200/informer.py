@@ -639,6 +639,63 @@ class IncrementalEncoder:
                         "limit": limit, "flags": [v for b, v in R.SHR_NAMES.items() if f & b]})
         return out
 
+    def place_explain_report(self, result: dict, extra_groups=None) -> list:
+        """A ``resident_place_explain`` answer as dicts, one per row in answer order: ``namespace``, ``name`` and
+        ``group`` (the group index; None for a row no object holds), ``row``, the ``records.PEX_*`` flags named,
+        and ``message``, one line in the scheduler's style, e.g. ``0/625 domains available: 402 too small, 3
+        without a usable node (12 of these would fit with cordoned nodes), 220 held ahead in the namespace (180
+        pinned); 2 slots short in rack-17; would take rack-4, held by ns/lws-a group 3`` (the cordoned count covers
+        the too-small and the usable-less domains together).  A request row below the encoder's used request rows
+        is its group's row (others name no object); extra row i (the last ``len(extra_groups)`` rows of the round)
+        is ``extra_groups[i]``, a (namespace, name, group index) — for ``whatif_scale(key, r)``'s rows,
+        ``[(*key, int(g)) for g in rows["group"]]``.  Domain ids are named by their topology values.  Nothing in the
+        encoder changes."""
+        names = {d: v for v, d in self._domain_ids.items()}
+        n_res = int(result["round_rows"]) - len(extra_groups or ())
+
+        def who(row):
+            row = int(row)
+            if row >= n_res:
+                return tuple(extra_groups[row - n_res])
+            return self.object_of_group_row(int(self.reqs["group"][row])) if row < self.r_end else None
+
+        def dom(d):
+            return names.get(int(d), f"domain {int(d)}")
+
+        def holder(row):
+            h = who(row)
+            return f"{h[0]}/{h[1]} group {h[2]}" if h else f"row {int(row)}"
+
+        out = []
+        for e in result["rows"]:
+            f = int(e["flags"])
+            key = who(e["row"])
+            if f & R.PEX_NO_NAMESPACE:
+                msg = "no such namespace"
+            else:
+                avail = int(e["n_own"]) + int(e["n_open"]) + int(e["n_held_later"])
+                ahead = int(e["n_held_pinned"]) + int(e["n_held_earlier"])
+                parts = [f"{int(e['n_too_small'])} too small",
+                         f"{int(e['n_no_usable'])} without a usable node ({int(e['n_fit_uncordoned'])} of these would fit "
+                         "with cordoned nodes)",
+                         f"{ahead} held ahead in the namespace ({int(e['n_held_pinned'])} pinned)"]
+                msg = f"{avail}/{int(result['n_domains'])} domains available: " + ", ".join(parts)
+                if int(e["shortfall_domain"]) != R.NONE:
+                    n = int(e["shortfall"])
+                    msg += f"; {n} slot{'s' if n != 1 else ''} short in {dom(e['shortfall_domain'])}"
+                if f & R.PEX_CONFLICT:
+                    msg += f"; leader's domain {dom(e['blocker_domain'])} is held by {holder(e['blocker_row'])}"
+                elif int(e["blocker_domain"]) != R.NONE:
+                    msg += f"; would take {dom(e['blocker_domain'])}, held by {holder(e['blocker_row'])}"
+                if f & R.PEX_NO_CLAIM:
+                    msg += "; the leader's node has no topology domain"
+                if f & R.PEX_BAD_SIZE:
+                    msg += "; size below 1"
+            out.append({"namespace": key[0] if key else None, "name": key[1] if key else None,
+                        "group": key[2] if key else None, "row": int(e["row"]),
+                        "flags": [v for b, v in R.PEX_NAMES.items() if f & b], "message": msg})
+        return out
+
     def whatif_drain(self, node_names) -> np.ndarray:
         """The node rows of the named nodes, for ``Engine.resident_drain_whatif`` (sorted, each once)."""
         return np.array(sorted({self.node_index[n] for n in node_names}), dtype=np.uint32)

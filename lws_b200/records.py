@@ -973,6 +973,58 @@ class ScaleHeadroomQuery(C.Structure):
 assert C.sizeof(ScaleHeadroomQuery) == 80
 
 
+# lwse_place_explain_row: why a row of a placement round has its verdict (per-domain classes and named domains)
+PLACE_EXPLAIN = np.dtype(
+    [("row", "<u4"), ("flags", "<u4"), ("place_flags", "<u4"), ("n_own", "<u4"), ("n_no_usable", "<u4"),
+     ("n_too_small", "<u4"), ("n_held_pinned", "<u4"), ("n_held_earlier", "<u4"), ("n_held_later", "<u4"),
+     ("n_open", "<u4"), ("n_fit_uncordoned", "<u4"), ("best_domain", "<u4"), ("blocker_domain", "<u4"),
+     ("blocker_row", "<u4"), ("shortfall", "<u4"), ("shortfall_domain", "<u4")],
+    align=False,
+)
+assert PLACE_EXPLAIN.itemsize == 64
+# the class counts of a row, in the order of the query's n_class totals
+PLACE_EXPLAIN_CLASSES = ("n_own", "n_no_usable", "n_too_small", "n_held_pinned", "n_held_earlier", "n_held_later",
+                         "n_open", "n_fit_uncordoned")
+
+PEX_CAPACITY = 1 << 0
+PEX_EXCLUSIVE = 1 << 1
+PEX_CORDONED = 1 << 2
+PEX_CONFLICT = 1 << 3
+PEX_NO_CLAIM = 1 << 4
+PEX_NO_NAMESPACE = 1 << 5
+PEX_BAD_SIZE = 1 << 6
+PEX_NAMES = {PEX_CAPACITY: "capacity", PEX_EXCLUSIVE: "exclusive", PEX_CORDONED: "cordoned", PEX_CONFLICT: "conflict",
+             PEX_NO_CLAIM: "no_claim", PEX_NO_NAMESPACE: "no_namespace", PEX_BAD_SIZE: "bad_size"}
+
+
+class PlaceExplainQuery(C.Structure):
+    """lwse_place_explain_query: the round (segments, extra rows, namespaces as PlaceWhatIf) and the rows (a list,
+    or a PLACE_* mask) in; PLACE_EXPLAIN rows, the class sums and the PEX_* flag counts out."""
+
+    _fields_ = [
+        ("segs", C.c_void_p),
+        ("n_segs", C.c_uint32),
+        ("n_extra", C.c_uint32),
+        ("extra", C.c_void_p),
+        ("n_namespaces", C.c_uint32),
+        ("mask", C.c_uint32),
+        ("rows", C.c_void_p),
+        ("n_rows", C.c_uint32),
+        ("capacity", C.c_uint32),
+        ("out", C.c_void_p),
+        ("n_explained", C.c_uint32),
+        ("round_rows", C.c_uint32),
+        ("n_domains", C.c_uint32),
+        ("whatif", C.c_uint32),
+        ("form", C.c_uint32),
+        ("n_flag", C.c_uint32 * 7),
+        ("n_class", C.c_uint64 * 8),
+    ]
+
+
+assert C.sizeof(PlaceExplainQuery) == 168
+
+
 class Config(C.Structure):
     _fields_ = [
         ("abi_version", C.c_uint32),
